@@ -1,15 +1,17 @@
 #!/usr/bin/env python
-"""bench.py -- ADMM iterations/s of the B200 hot path on BASELINE.json's metric configs.
+"""bench.py -- ADMM iterations/s of the H100 hot path on BASELINE.json's metric configs.
 
-Default workload (config.workload) = BASELINE configs[2], the configuration the north-star target is quoted on:
-8 partitions x 1M rows x 10k features, 1 % nnz (100 stored values per row), lambda in {0.1, 1, 10} in ONE run,
-synthetic (SURVEY.md 8d: uniform distinct columns per row, N(0,1) values, seed 1000+p per partition).  The 8
-partitions are sharded over the N ranks (p % N): per-GPU work shrinks as N grows, scaling = "strong".
+Default workload (config.workload) = the shape of BASELINE configs[2], the configuration the north-star target is quoted on,
+with 4 partitions instead of 8: 4 partitions x 1M rows x 10k features, 1 % nnz (100 stored values per row), lambda in
+{0.1, 1, 10} in ONE run, synthetic (SURVEY.md 8d: uniform distinct columns per row, N(0,1) values, seed 1000+p per
+partition).  Each (partition, lambda) problem keeps ~3 GB of 10k-wide solver state (factor, inverses, Gram partials), so
+the 24 problems of 8 partitions do not fit one 80 GB H100; 12 do.  The partitions are sharded over the N ranks (p % N):
+per-GPU work shrinks as N grows, scaling = "strong".
 One "step" = one ADMM iteration = the x-update of every (partition, lambda) reducer + the consensus all-reduce +
 the z/u update (jobs/RegressionAdmmTrain.java:281-497; reducers = nblocks x #lambda, :355).  The timed region is
 a complete job of K iterations FROM THE COLD STATE z = u = 0 (Gram + Cholesky of every partition included), after
 W warm-up iterations of a throw-away job; inputs (0.8 GB CSR + 0.6 GB block-major list per partition, 400 MB per
-inverse Hessian) are far larger than the 126 MB L2, so nothing is flushed between iterations.
+inverse Hessian) are far larger than the 50 MB L2, so nothing is flushed between iterations.
 
     python bench.py --gpus N --steps K --warmup W            (N > 1: launched by torch.distributed.run)
     python bench.py --impl reference ...                      (CPU arm: the oracle port, rank 0 only)
@@ -20,6 +22,8 @@ Prints ONE JSON line (rank 0).  `value` = iterations/s with inputs resident in H
 the public API from pinned HOST buffers (upload + K iterations + model read-back in the timed region);
 `also.cfg2` = the same measurements for configs[1] (round 1's headline line), `parity` = the same kernels on a
 row-reduced copy of the workload against the CPU oracle in exact mode.
+
+    python bench.py ... --dump-outputs DIR                    (after the timed steps: what the timed job computed, as .npy)
 """
 import argparse
 import json
@@ -40,9 +44,9 @@ WORKLOADS = {
     # name: partitions, rows/partition, features, stored values per row (None = dense), lambdas
     "cfg2": dict(P=8, n=1_000_000, D=1000, nnz=None, lambdas=[1.0], scaling="strong",
                  desc="8 partitions x 1M x 1k dense, lambda=1 (BASELINE configs[1]); partitions sharded p%N over ranks"),
-    "cfg3": dict(P=8, n=1_000_000, D=10_000, nnz=100, lambdas=[0.1, 1.0, 10.0], scaling="strong",
-                 desc="8 partitions x 1M x 10k, 1% nnz (100/row), lambda in {0.1,1,10} in one run (BASELINE configs[2], the "
-                      "north-star target config); partitions sharded p%N over ranks"),
+    "cfg3": dict(P=4, n=1_000_000, D=10_000, nnz=100, lambdas=[0.1, 1.0, 10.0], scaling="strong",
+                 desc="4 partitions x 1M x 10k, 1% nnz (100/row), lambda in {0.1,1,10} in one run (BASELINE configs[2] with 4 "
+                      "of its 8 partitions, so that its solver state fits 80 GB); partitions sharded p%N over ranks"),
     "cfg4": dict(P=None, n=1_000_000, D=10_000, nnz=100, lambdas=[1.0], scaling="weak",
                  desc="8 partitions PER GPU x 1M x 10k, 1% nnz, lambda=1 (BASELINE configs[3] = 64 partitions on 8 GPUs; "
                       "P = 8*N at N GPUs, batched Gram + Cholesky)"),
@@ -66,7 +70,9 @@ def parse():
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-parity", action="store_true")
     ap.add_argument("--hessian-policy", type=int, default=0)
-    ap.add_argument("--keys", type=int, default=100_000, help="cfg5: number of NaiveTrain keys")
+    ap.add_argument("--keys", type=int, default=8192, help="cfg5: NaiveTrain keys per step (per rank)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write what the timed job computed (rank 0) to DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -94,7 +100,7 @@ def peaks():
             j = json.load(f)
         return dict(hbm=float(j["hbm_gbs"]), tf_burst=float(j["bf16_tflops"]), tf_sust=float(j["bf16_tflops_sustained"]), src="measured")
     except Exception:
-        return dict(hbm=6650.0, tf_burst=1590.0, tf_sust=1400.0, src="fallback")
+        return dict(hbm=3350.0, tf_burst=989.0, tf_sust=989.0, src="H100 SXM data sheet")
 
 
 # ------------------------------------------------------------------------------------------------ synthetic data
@@ -294,9 +300,19 @@ class Ctx:
     pass
 
 
-def run_admm_workload(cx, wl, K, W, want_e2e):
+def dump_outputs(d, arrays):
+    """Writes each array as d/<name>.npy (float32 or float64 as computed)."""
+    os.makedirs(d, exist_ok=True)
+    for name, a in arrays.items():
+        a = np.asarray(a)
+        assert a.dtype in (np.float32, np.float64), (name, a.dtype)
+        np.save(os.path.join(d, name + ".npy"), a)
+
+
+def run_admm_workload(cx, wl, K, W, want_e2e, dump_dir=""):
     """Resident-data leg (`value`) and host-buffer leg (`e2e`) of one ADMM workload on this rank's GPU.  Returns a dict on
-    rank 0 (None elsewhere)."""
+    rank 0 (None elsewhere).  dump_dir: rank 0 writes the consensus models z [L][D+1] (fp64) and its partitions' x (fp64) and
+    u (fp32), [partition][L][D+1], of the timed job."""
     import torch
     import torch.distributed as dist
     import mlease_b200 as mb
@@ -370,6 +386,9 @@ def run_admm_workload(cx, wl, K, W, want_e2e):
         dist.all_reduce(usum, op=dist.ReduceOp.SUM)
     launches = st1["kernel_launches"] - st0["kernel_launches"]
     last_maxdiff = st1["last_maxdiff"]
+    if dump_dir and rank == 0:
+        dump_outputs(dump_dir, {"z": z_final, "x": np.stack([[sess.x(p, l) for l in range(L)] for p in my_parts]),
+                                "u": np.stack([[sess.u(p, l) for l in range(L)] for p in my_parts])})
     sess.close(); del sess
     torch.cuda.empty_cache()
 
@@ -423,25 +442,13 @@ def run_admm_workload(cx, wl, K, W, want_e2e):
     gr_ms, gr_n = prof["ms"]["gram"], prof["launches"]["gram"]
     k1_total_bytes = prof["k1_bytes"]
     k1_gbs = (k1_total_bytes / 1e9) / (k1_ms / 1e3) if k1_ms > 0 else None
-    traffic, traffic_src = None, None   # DRAM bytes of one steady-state K1 launch from the committed ncu --set full capture (N=1)
-    try:
-        if world == 1 and wl["name"] in ("cfg2", "cfg3") and (P, n, D) == (WORKLOADS[wl["name"]]["P"], WORKLOADS[wl["name"]]["n"], WORKLOADS[wl["name"]]["D"]):
-            tj = json.load(open(os.path.join(ROOT, "profiles", "k1_traffic.json")))[wl["name"]]
-            # the captured launch served a known number of (partition, lambda) passes: its DRAM bytes per algorithmic byte, applied to
-            # this run's average launch (launches differ in how many problems are still running)
-            traffic = tj["traffic_over_algorithmic"] * (k1_total_bytes / max(k1_n, 1))
-            traffic_src = ("%s: %.3f GB of DRAM traffic for %.3f GB algorithmic in the captured launch, scaled to this run's average launch "
-                           "(a committed capture of this command, not measured by this run)"
-                           % (tj["source"], tj["traffic_bytes_per_launch"] / 1e9, tj["algorithmic_bytes_of_captured_launch"] / 1e9))
-    except Exception:
-        traffic = None
     fused = bool(st1.get("k1_fused"))
     shared_bytes = st1["k1_shared_bytes"] - st0["k1_shared_bytes"]
     roof = {"kernel": (("k1_csr_fused_kernel (score + reweight + gradient of ALL lambdas of a partition in one pass over its rows)" if fused
                         else "k1_csr_fx_kernel (fused score+reweight+gradient over the CSR rows)") if sparse else
                        "k1_dense_kernel (fused score+reweight+gradient, one pass over X)"), "bound": "hbm",
-            "achieved": k1_gbs, "peak": pk["hbm"], "unit": "GB/s", "frac": (k1_gbs / pk["hbm"]) if k1_gbs else None, "traffic": traffic,
-            "traffic_source": traffic_src, "peak_source": pk["src"] + " hbm_gbs (copy)", "launches": k1_n, "avg_launch_ms": k1_ms / max(k1_n, 1),
+            "achieved": k1_gbs, "peak": pk["hbm"], "unit": "GB/s", "frac": (k1_gbs / pk["hbm"]) if k1_gbs else None,
+            "peak_source": pk["src"] + " hbm_gbs (copy)", "launches": k1_n, "avg_launch_ms": k1_ms / max(k1_n, 1),
             "algorithmic_bytes_per_launch": k1_total_bytes / max(k1_n, 1),
             "algorithmic_bytes": ("(8*nnz + 17*n) per (partition, lambda) pass (SURVEY 8d); the lambdas of a partition share the rows through L2"
                                   if sparse else "n*(4*ldx + 9) per partition pass (SURVEY 8d)"),
@@ -454,10 +461,10 @@ def run_admm_workload(cx, wl, K, W, want_e2e):
         roof["shared_read"] = {"achieved": sg, "frac": (sg / pk["hbm"]) if sg else None, "bytes_per_launch": shared_bytes / max(k1_n, 1),
                                "bytes": "8*nnz + 9*n per partition pass + 8*n per lambda served"}
     gram_tf = (prof["gram_flops"] / 1e12) / (gr_ms / 1e3) if gr_ms > 0 else None
-    # CSR Gram: e4m3 operands (tcgen05 kind::f8f6f4).  MEASURED_PEAKS.json holds no fp8 number: the peak used is twice the measured
-    # sustained bf16 figure (the f8f6f4 MMA has twice the bf16 rate per SM); the bf16 peak is reported beside it.
+    # CSR Gram: e4m3 operands (wgmma .e4m3).  MEASURED_PEAKS.json holds no fp8 number: the peak used is twice the sustained bf16
+    # figure (the e4m3 wgmma has twice the bf16 rate per SM); the bf16 peak is reported beside it.
     g_peak = 2.0 * pk["tf_sust"] if sparse else pk["tf_sust"]
-    roof_gram = {"kernel": "gram_csr_tcgen05_kernel (e4m3 operands assembled from CSR, kind::f8f6f4)" if sparse else "gram_tcgen05_kernel (bf16, kind::f16)",
+    roof_gram = {"kernel": "gram_csr_wgmma_kernel (e4m3 operands assembled from CSR, wgmma m64n128k32)" if sparse else "gram_wgmma_kernel (bf16, wgmma m64n256k16)",
                  "bound": "tensor", "achieved": gram_tf, "peak": g_peak, "unit": "TFLOP/s", "frac": (gram_tf / g_peak) if gram_tf else None,
                  "frac_of_bf16_sustained": (gram_tf / pk["tf_sust"]) if gram_tf else None, "launches": gr_n,
                  "avg_launch_ms": gr_ms / max(gr_n, 1), "flops": "n*D'*(D'+1) per build actually run (lower triangle; cold-start builds shared across lambdas)",
@@ -477,7 +484,7 @@ def run_admm_workload(cx, wl, K, W, want_e2e):
 
 
 def parity_leg(cx, wl, iters=4):
-    """The same kernels (CSR K1, CSR Gram on tcgen05, wide Cholesky, shared cold-start factor) on a row-reduced copy of the
+    """The same kernels (CSR K1, CSR Gram on wgmma, wide Cholesky, shared cold-start factor) on a row-reduced copy of the
     workload -- same feature count, nnz/row and lambdas -- against the CPU oracle in exact mode at the same iteration count."""
     import torch
     import mlease_b200 as mb
@@ -509,15 +516,14 @@ def parity_leg(cx, wl, iters=4):
 
 
 def run_naive_workload(cx, K, W):
-    """BASELINE configs[4]: NaiveTrain per-key fits, `--keys` keys x 1000 rows x 256 dense features, lambda = 1.  Keys are
-    independent (replicas only): rank r fits keys r::N.  One "step" = one batch of 8192 keys generated on the device."""
+    """BASELINE configs[4]: NaiveTrain per-key fits, keys x 1000 rows x 256 dense features, lambda = 1.  Keys are independent
+    (replicas only): every rank fits its own batch.  One "step" = the fits of one batch of `--keys` keys generated on the
+    device (seed 1000 + rank); the K timed steps refit that batch."""
     import torch
     import torch.distributed as dist
     import mlease_b200 as mb
     args, world, rank, dev = cx.args, cx.world, cx.rank, cx.dev
-    nk, D, B = 1000, 256, 8192
-    keys_total = args.keys
-    my_keys = (keys_total + world - 1) // world
+    nk, D, B = 1000, 256, args.keys
     stream = torch.cuda.current_stream().cuda_stream
     g = torch.Generator(device=dev); g.manual_seed(1000 + rank)
     beta = torch.as_tensor((np.random.default_rng(999).normal(size=D) / np.sqrt(D)).astype(np.float32), device=dev)
@@ -526,7 +532,7 @@ def run_naive_workload(cx, K, W):
         X = torch.randn(nkeys * nk, D, generator=g, device=dev)
         y = (torch.rand(nkeys * nk, generator=g, device=dev) < torch.sigmoid(X @ beta - 1.0)).to(torch.int32)
         return X, y, np.arange(nkeys + 1, dtype=np.int64) * nk
-    X, y, krs = batch(min(B, my_keys))
+    X, y, krs = batch(B)
     for _ in range(max(W, 1)):
         mb.naive_train_dense(X, krs, y, 1.0, device=cx.local_rank, stream=stream)
     torch.cuda.synchronize()
@@ -534,13 +540,8 @@ def run_naive_workload(cx, K, W):
         dist.barrier()
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
-    done = 0
-    while done < my_keys:
-        kb = min(B, my_keys - done)
-        if kb != len(krs) - 1:
-            X, y, krs = batch(kb)
-        mb.naive_train_dense(X, krs, y, 1.0, device=cx.local_rank, stream=stream)
-        done += kb
+    for _ in range(K):
+        models, _skipped = mb.naive_train_dense(X, krs, y, 1.0, device=cx.local_rank, stream=stream)
     e1.record()
     torch.cuda.synchronize()
     tms = torch.tensor([e0.elapsed_time(e1)], dtype=torch.float64, device=dev)
@@ -548,9 +549,11 @@ def run_naive_workload(cx, K, W):
         dist.all_reduce(tms, op=dist.ReduceOp.MAX)
     if rank != 0:
         return None
+    if args.dump_outputs and K > 0:
+        dump_outputs(args.dump_outputs, {"models": np.asarray(models)})
     sec = float(tms.item()) / 1e3
-    return {"value": my_keys * world / sec, "unit": "per-key fits/s", "metric": "NaiveTrain per-key fits/sec", "seconds": sec,
-            "keys": my_keys * world, "rows_per_key": nk, "features": D, "scaling": "weak (replicas only)"}
+    return {"value": K * B * world / sec, "unit": "per-key fits/s", "metric": "NaiveTrain per-key fits/sec", "seconds": sec,
+            "keys": K * B * world, "rows_per_key": nk, "features": D, "scaling": "weak (replicas only)"}
 
 
 def main():
@@ -562,7 +565,7 @@ def main():
     K, W = args.steps, max(args.warmup, 0)
     if args.workload == "cfg5":
         wl = dict(name="cfg5", P=args.keys, n=1000, D=256, nnz=None, lambdas=[1.0], scaling="weak",
-                  desc="NaiveTrain per-key: %d keys x 1k rows x 256 dense features, lambda=1 (BASELINE configs[4])" % args.keys)
+                  desc="NaiveTrain per-key: %d keys per step x 1k rows x 256 dense features, lambda=1 (BASELINE configs[4])" % args.keys)
     else:
         wl = workload(args, args.workload, world)
     cfg = {"workload": wl["desc"], "name": wl["name"], "partitions": wl["P"], "rows_per_partition": wl["n"], "features": wl["D"],
@@ -614,7 +617,7 @@ def main():
             dist.destroy_process_group()
         return
 
-    res = run_admm_workload(cx, wl, K, W, not args.no_e2e)
+    res = run_admm_workload(cx, wl, K, W, not args.no_e2e, args.dump_outputs)
     also = {}
     for name in [a for a in args.also.split(",") if a and a != wl["name"] and a in WORKLOADS]:
         wl2 = workload(args, name, world)

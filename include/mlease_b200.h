@@ -1,5 +1,5 @@
 /*
- * mlease_b200.h -- C ABI of the B200-native ADMM logistic-regression hot path.
+ * mlease_b200.h -- C ABI of the H100-native ADMM logistic-regression hot path.
  *
  * Drop-in boundary for ONE path of linkedin/ml-ease: the body of
  * RegressionAdmmTrain.run() (jobs/RegressionAdmmTrain.java:278-501), the reducer it drives
@@ -179,7 +179,7 @@ typedef struct {
 int mlease_get_stats(mlease_session* s, mlease_stats* out);
 int mlease_world_get_stats(mlease_world* w, mlease_stats* out);   /* counters summed over the devices */
 /* Per-kernel device timing for roofline reporting (CUDA events on the session stream around every launch of
- * the Newton slot; categories: 0 = K1 fused pass, 1 = small kernels (reduce/decide, solve, poll), 2 = Gram (tcgen05),
+ * the Newton slot; categories: 0 = K1 fused pass, 1 = small kernels (reduce/decide, solve, poll), 2 = Gram (wgmma),
  * 3 = Cholesky).  enable: 1 on, 0 off, 2 on + reset accumulators, -1 read only.  Outputs (any may be NULL) are the
  * accumulators BEFORE this call's reset: ms4[4], count4[4], and the algorithmic work done by the session so far:
  * k1_bytes (SURVEY 8d: dense n*(4*ldx+9) per pass), k1_emit_bytes (bf16 operand writes), gram_flops (n*D'*(D'+1)). */
@@ -191,9 +191,9 @@ int mlease_profile(mlease_session* s, int32_t enable, double* ms4, int64_t* coun
  * LogisticRegressionL2.fun/grad/hessian (regression/liblinearfunc/LogisticRegressionL2.java:156-297)
  * evaluated on a resident partition at host vector w, prior mean m, prior precision q (=1/priorVar),
  * all of length num_features+1.  Any output may be NULL.  H is [Dt x Dt] row-major (full, symmetric).
- * tensor != 0 builds H with the tcgen05 Gram kernel (bf16 operands for dense partitions, e4m3 operands assembled from the rows
+ * tensor != 0 builds H with the wgmma Gram kernel (bf16 operands for dense partitions, e4m3 operands assembled from the rows
  * for CSR partitions with sorted unique rows), 0 with the fp32 SIMT debug kernel (dense bf16 operand only).
- * tensor == 2 returns in H the INVERSE the Newton direction is computed with (tcgen05 Gram + diag(q) -> fp64 blocked
+ * tensor == 2 returns in H the INVERSE the Newton direction is computed with (wgmma Gram + diag(q) -> fp64 blocked
  * Cholesky -> explicit inverse), so that tests can check H^-1 * H = I for every factorisation path.
  * ------------------------------------------------------------------------------------- */
 int mlease_objective(mlease_session* s, int32_t partition_id, const double* w, const double* m, const double* q,
@@ -256,7 +256,7 @@ int mlease_test_loglik(int32_t device, void* stream, int64_t nrows, const int32_
 
 /* Bench / profiling hooks (not part of the reference surface): time one fused K1 pass or one Gram build
  * on a resident partition with CUDA events on the session stream, `reps` launches, returns avg ms. */
-int mlease_time_kernel(mlease_session* s, int32_t partition_id, int32_t which /*1=K1,2=Gram tcgen05,3=cholesky*/,
+int mlease_time_kernel(mlease_session* s, int32_t partition_id, int32_t which /*1=K1,2=Gram wgmma,3=cholesky*/,
                        int32_t reps, int32_t emit_scaled, float* avg_ms);
 
 #ifdef __cplusplus

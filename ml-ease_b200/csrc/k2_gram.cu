@@ -1,19 +1,18 @@
 // k2_gram.cu -- K2: weighted Gram  G = Xt^T Xt  (Xt = diag(sqrt d) X in bf16, written by K1), the
 // data term of LogisticRegressionL2.hessian (llf/LogisticRegressionL2.java:258-297):
 //     H[m][n] = (m==n ? 1/priorVar[m] : 0) + sum_i D_ii x_im x_in ,  D_ii = w_i p_i (1-p_i).
-// It genuinely is a dense GEMM (K = rows, M = N = features), so it runs on the 5th-gen tensor
-// cores: TMA (tensor map, 128B swizzle) -> shared memory -> tcgen05.mma (bf16 x bf16 -> fp32 in
-// TMEM) -> tcgen05.ld epilogue.  Both operands are tiles of the SAME row-major matrix, i.e. they are
-// MN-major ("transposed") UMMA operands: no transpose pass over X is ever made.
+// It genuinely is a dense GEMM (K = rows, M = N = features), so it runs on the Hopper tensor
+// cores: TMA (tensor map, 128B swizzle) -> shared memory -> wgmma (bf16 x bf16 -> fp32 in
+// registers).  Both operands are tiles of the SAME row-major matrix, i.e. they are MN-major
+// ("transposed") wgmma operands: no transpose pass over X is ever made.
 //
 // Work decomposition: output tiles of 128 (M) x 256 (N) restricted to the lower block triangle,
-// split-K over row slices; each CTA owns one (tile, slice), accumulates it in TMEM (256 columns)
-// and stores the fp32 partial to Hpart[slice] (plain stores, deterministic).  chol_prep_kernel
+// split-K over row slices; each CTA owns one (tile, slice), accumulates it in registers and
+// stores the fp32 partial to Hpart[slice] (plain stores, deterministic).  chol_prep_kernel
 // (k3_cholesky.cu) sums the slices in fixed order and adds diag(q).
 //
-// Warp roles (192 threads): warp 0 = TMA producer (one elected lane), warp 1 = MMA issuer (one
-// elected lane) + TMEM allocator, warps 2-5 = epilogue (tcgen05.ld 32x32b, one TMEM lane quadrant
-// each: warp_id % 4).
+// Warpgroup roles (384 threads): warpgroup 0 = TMA producer (one lane), warpgroups 1-2 = consumers,
+// each issuing m64n256k16 wgmma for its 64 rows of the tile (128 fp32 accumulators a thread).
 //
 // A fp32 SIMT kernel computing the same partials from the same bf16 operand is kept ONLY as a
 // debug cross-check reachable through mlease_objective(tensor=0); the product path never uses it.
@@ -28,44 +27,46 @@
 namespace mlease {
 
 // ------------------------------------------------------------------------------------------
-// tcgen05 kernel
+// bf16 wgmma kernel
 // ------------------------------------------------------------------------------------------
-constexpr int GM = 128;          // tile rows  (UMMA M)
-constexpr int GN = 256;          // tile cols  (UMMA N)
+constexpr int GM = 128;          // tile rows
+constexpr int GN = 256;          // tile cols (wgmma N)
 constexpr int GK = 64;           // K (data rows) per pipeline stage
-constexpr int UK = 16;           // K per tcgen05.mma (bf16)
+constexpr int UK = 16;           // K per wgmma (bf16)
 constexpr int GSTAGES = 4;
 constexpr int G_A_BYTES = GK * GM * 2;   // 16 KB : 2 boxes of [64 k][64 feat]
 constexpr int G_B_BYTES = GK * GN * 2;   // 32 KB : 4 boxes
 constexpr int G_STAGE_BYTES = G_A_BYTES + G_B_BYTES;
 constexpr int G_BOX_BYTES = GK * 64 * 2; // 8 KB, one TMA box = 64 k-rows x 128 B
-constexpr int G_THREADS = 192;
+constexpr int G_THREADS = 384;
 constexpr size_t G_SMEM = (size_t)GSTAGES * G_STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
+// canonical MN-major SWIZZLE_128B layout (bf16) of a TMA box: ((64 elems,m),(8,k)) : ((1,LBO),(128B,SBO)), i.e.
+// SBO = 1024 B between 8-row K groups, LBO = one box (GK*128 B) between 64-element MN groups.
+constexpr uint32_t DESC_SW128 = 1, DESC_SW32 = 3;
 
-// UMMA shared-memory descriptor, MN-major operand, SWIZZLE_128B (cute::UMMA::SmemDescriptor layout):
-//   [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [61,64) layout=2 (SW128)
-// canonical MN-major SW128 layout (bf16): ((64 elems,m),(8,k)) : ((1,LBO),(128B,SBO)):
-//   SBO = 1024 B between 8-row K groups, LBO = GK*128 B between 64-element MN groups (one TMA box).
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// Instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 (1) @4, a/b_format BF16 (1) @7/@10,
-// a_major/b_major = MN (1) @15/@16, N>>3 @17, M>>4 @24.
-__device__ __forceinline__ uint32_t umma_idesc_bf16_mn(int M, int N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
+struct GramTile { short bi, bj; };   // 128-row block index, column block index (256 or 128 wide)
 
-struct GramTile { short bi, bj; };   // 128-row block index, 256-col block index
+// Stores a consumer warpgroup's m64nN accumulator into rows row0 .. row0+63 of the Dp x Dp partial.  wgmma D fragment: warp w
+// of the group holds rows 16w .. 16w+15; lane l holds rows 16w + l/4 and 16w + l/4 + 8, columns 8j + 2(l%4) + {0,1}, in
+// d[4j .. 4j+3].  Dp is a multiple of 128, so a column pair is either wholly inside or wholly outside.
+template <int N>
+__device__ __forceinline__ void store_acc(float* out, int Dp, int row0, int col0, const float (&d)[N / 2]) {
+  const int lane = threadIdx.x & 31, w = (threadIdx.x >> 5) & 3;
+  const int r = row0 + w * 16 + (lane >> 2);
+  if (r + 8 >= Dp) return;
+#pragma unroll
+  for (int j = 0; j < N / 8; j++) {
+    const int c = col0 + 8 * j + 2 * (lane & 3);
+    if (c < Dp) {
+      *reinterpret_cast<float2*>(out + (size_t)r * Dp + c) = make_float2(d[4 * j], d[4 * j + 1]);
+      *reinterpret_cast<float2*>(out + (size_t)(r + 8) * Dp + c) = make_float2(d[4 * j + 2], d[4 * j + 3]);
+    }
+  }
+}
 
 __global__ void __launch_bounds__(G_THREADS, 1)
-gram_tcgen05_kernel(const Problem* __restrict__ probs, const CUtensorMap* __restrict__ tmaps, const GramTile* __restrict__ tiles,
-                    int ntiles, int force, int share) {
+gram_wgmma_kernel(const Problem* __restrict__ probs, const CUtensorMap* __restrict__ tmaps, const GramTile* __restrict__ tiles,
+                  int ntiles, int force, int share) {
   // share = L > 1: the L problems of one partition are at the same iterate (cold start), so their Grams are identical;
   // only the first of each group is built and chol_prep_kernel reads it for the whole group
   if (share > 1 && blockIdx.z % share != 0) return;
@@ -87,28 +88,18 @@ gram_tcgen05_kernel(const Problem* __restrict__ probs, const CUtensorMap* __rest
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(g_smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)GSTAGES * G_STAGE_BYTES);
   uint64_t* empty_bar = full_bar + GSTAGES;
-  uint64_t* acc_bar = empty_bar + GSTAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_bar + 1);
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int lane = threadIdx.x & 31, wg = threadIdx.x >> 7;
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(tmap);
-    for (int s = 0; s < GSTAGES; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 1); }
-    mbar_init(acc_bar, 1);
+    for (int s = 0; s < GSTAGES; s++) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }   // 8 = the consumer warps
     fence_mbar_init();
   }
-  if (warp == 1) {
-    tmem_alloc(tmem_slot, GN);   // 256 columns x 128 lanes fp32
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    if (threadIdx.x == 0) {
       // ===== TMA producer =====
       for (int k = 0; k < nk; k++) {
         const int st = k % GSTAGES;
@@ -123,123 +114,77 @@ gram_tcgen05_kernel(const Problem* __restrict__ probs, const CUtensorMap* __rest
         for (int b = 0; b < GN / 64; b++) tma_load_2d(b_dst + b * G_BOX_BYTES, tmap, tile.bj * GN + b * 64, krow, &full_bar[st]);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer =====
-      const uint32_t idesc = umma_idesc_bf16_mn(GM, GN);
-      for (int k = 0; k < nk; k++) {
-        const int st = k % GSTAGES;
-        mbar_wait(&full_bar[st], (uint32_t)((k / GSTAGES) & 1));
-        tc_fence_after();
-        const uint32_t a_addr = smem_u32(smem + (size_t)st * G_STAGE_BYTES);
-        const uint32_t b_addr = a_addr + G_A_BYTES;
-#pragma unroll
-        for (int kk = 0; kk < GK / UK; kk++) {
-          // 16 k-rows = 2 swizzle atoms of 1024 B along K
-          const uint64_t da = umma_desc_mn_sw128(a_addr + kk * (UK * 128), G_BOX_BYTES, 1024);
-          const uint64_t db = umma_desc_mn_sw128(b_addr + kk * (UK * 128), G_BOX_BYTES, 1024);
-          umma_f16(tmem_base, da, db, idesc, (k | kk) != 0 ? 1u : 0u);
-        }
-        umma_commit(&empty_bar[st]);   // frees the smem stage when these MMAs retire
-      }
-      umma_commit(acc_bar);            // accumulator complete
-    }
   } else {
-    // ===== epilogue: warps 2..5 -> TMEM lane quadrant (warp % 4) =====
-    const int quad = warp & 3;
-    float* out = pb.Hpart + (size_t)slice * Dp * Dp;
-    const int row = tile.bi * GM + quad * 32 + lane;
-    if (nk > 0) {
-      mbar_wait(acc_bar, 0);
-      tc_fence_after();
-    }
-#pragma unroll 1
-    for (int c0 = 0; c0 < GN; c0 += 32) {
-      uint32_t r[32];
-      if (nk > 0) {
-        tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)c0, r);
-        tmem_ld_wait();
-      } else {
+    // ===== consumer warpgroup wg: the tile's rows (wg - 1) * 64 .. +63 = box wg - 1 of the A block =====
+    float acc[GN / 2];
 #pragma unroll
-        for (int j = 0; j < 32; j++) r[j] = 0u;
-      }
-      const int col = tile.bj * GN + c0;
-      if (row < Dp && col < Dp) {
-        float4* dst = reinterpret_cast<float4*>(out + (size_t)row * Dp + col);
+    for (int j = 0; j < GN / 2; j++) acc[j] = 0.f;
+    const uint32_t smem_base = smem_u32(smem);
+    for (int k = 0; k < nk; k++) {
+      const int st = k % GSTAGES;
+      mbar_wait(&full_bar[st], (uint32_t)((k / GSTAGES) & 1));
+      const uint32_t a_addr = smem_base + (uint32_t)(st * G_STAGE_BYTES + (wg - 1) * G_BOX_BYTES);
+      const uint32_t b_addr = smem_base + (uint32_t)(st * G_STAGE_BYTES + G_A_BYTES);
+      wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < 8; j++)
-          dst[j] = make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]), __uint_as_float(r[4 * j + 2]),
-                               __uint_as_float(r[4 * j + 3]));
-      }
+      for (int kk = 0; kk < GK / UK; kk++)   // 16 k-rows = 2 swizzle atoms of 1024 B along K
+        wgmma_bf16_m64n256k16_tt(acc, wgmma_desc(a_addr + kk * (UK * 128), G_BOX_BYTES, 1024, DESC_SW128),
+                                 wgmma_desc(b_addr + kk * (UK * 128), G_BOX_BYTES, 1024, DESC_SW128));
+      wgmma_commit();
+      wgmma_wait<1>();   // the previous stage's products have retired: hand its buffer back to the producer
+      if (k > 0 && lane == 0) mbar_arrive(&empty_bar[(k - 1) % GSTAGES]);
     }
-    tc_fence_before();
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, GN);
+    wgmma_wait<0>();
+    store_acc<GN>(pb.Hpart + (size_t)slice * Dp * Dp, Dp, tile.bi * GM + (wg - 1) * 64, tile.bj * GN, acc);
   }
 }
 
 // ------------------------------------------------------------------------------------------
-// Sparse variant: the same split-K tcgen05 Gram, but the operand tiles are ASSEMBLED IN SHARED MEMORY, as e4m3, from the
-// partition's block-major entry list (no dense Xt in HBM: at 1 % density that copy is 100x the input and makes the dense
-// kernel HBM-bound).  One K-step = one 32-row group; its entries for a 128-column block are one contiguous run of
-// (key, value), the key being the byte offset of the element inside the canonical MN-major SWIZZLE_128B operand block the
-// UMMA descriptors expect (sw128_off).  24 producer warps, one per operand block of a stage: load the run coalesced, scale
-// by sqrt(d_row) * 2^e, round to e4m3, store one byte at the key.  Positions outside the sparsity pattern are zero: the ring
-// is cleared once, and a producer re-clears exactly the entries it wrote when it gets its stage back.  Generic-proxy stores
-// are published to the tensor core's async proxy with fence.proxy.async before the mbarrier arrive.
-// Warp roles (29 warps): 0 = MMA issuer (leader CTA) + TMEM allocator, 1..24 = producers, 25..28 = epilogue.
-// Measured at 1M x 10k x 1 % (8 builds): bf16 operands 628 ms (1.27 PFLOP/s); e4m3 531 ms; unrolled issue loop 374 ms;
-// CTA pairs 353 ms; shared-space byte stores (the generic ones rebuilt the shared window base at every store) 337 ms =
-// 2.37 PFLOP/s.  What bounds it now is the MMA stream itself: with producers that ONLY hand stages over (no loads, no
-// stores) a build takes 40.0 ms instead of 44.7 (tools/time_gram.py), i.e. 2.5 PFLOP/s is what one tcgen05.mma.kind::f8f6f4
-// per K = 32 step delivers at the clocks a tensor-bound kernel sustains on this part (cuBLAS bf16 holds 1.43 PFLOP/s at a
-// median 1365 MHz, MEASURED_PEAKS.json).
+// Sparse variant: the same split-K Gram, but the operand tiles are ASSEMBLED IN SHARED MEMORY, as e4m3, from the partition's
+// block-major entry list (no dense Xt in HBM: at 1 % density that copy is 100x the input and makes the dense kernel
+// HBM-bound).  One K-step = one 32-row group = one m64n128k32 wgmma per consumer warpgroup; its entries for a 128-column block
+// are one contiguous run of (key, value), the key being the byte offset of the element inside the K-major SWIZZLE_32B operand
+// block the wgmma descriptors expect (kmaj_off; wgmma takes 8-bit operands K-major only).  Producer warps, one per operand
+// block of a stage: load the run coalesced, scale by sqrt(d_row) * 2^e, round to e4m3, store one byte at the key.  Positions
+// outside the sparsity pattern are zero: the ring is cleared once, and a producer re-clears exactly the entries it wrote when
+// it gets its stage back.  Generic-proxy stores are published to the tensor core's async proxy with fence.proxy.async before
+// the mbarrier arrive.
+// A CTA owns a 128 x 128 lower tile, two consumer warpgroups of 64 rows.  The tensor core keeps the running sum of an fp8
+// product at less than fp32 precision, so a consumer runs chains of S_CHAIN wgmma (K = 128 rows) into one set of 64
+// registers and adds each finished chain into a second, fp32, set; setmaxnreg moves the registers this takes from the
+// producer warpgroups to the consumers.
+// Warp roles (16 warps): 0..7 = consumers, 8..15 = producers (4 groups of an A-block and a B-block warp).
 // ------------------------------------------------------------------------------------------
 constexpr int SK = 32;                       // data rows (K) per stage
-constexpr int S_BOX_BYTES = SK * 128;        // 4 KB = one [32 k][128 cols] e4m3 operand block
-// NCTA = 1: a CTA owns a 128 x 256 tile: A block + two B blocks per stage (12 KB), 16 stages, 8 producer trios.
-// NCTA = 2: a CTA PAIR (cluster of 2, cta_group::2) owns a 256 x 256 tile: each CTA assembles ITS 128 rows of A and ITS 128 of the
-//           B tile's 256 columns (8 KB per stage), i.e. a third less producer work, shared-memory store traffic and operand read
-//           traffic per flop; 24 stages, 12 producer pairs.  K-step k lives in stage k % SST and belongs to producer group k % NGRP
-//           (SST = 2 NGRP: a group alternates between two stages, because the refill round trip is several MMA periods long).
-template <int NCTA> struct SCfg {
-  static constexpr int SPW = NCTA == 1 ? 3 : 2;        // producer warps per stage: one per operand block
-  static constexpr int NGRP = 24 / SPW;                // producer groups
-  static constexpr int SST = 2 * NGRP;                 // ring stages
-  static constexpr int STAGE_BYTES = SPW * S_BOX_BYTES;
-  static constexpr size_t SMEM = (size_t)SST * STAGE_BYTES + 1024 /*align*/ + 512 /*barriers*/;
-};
-constexpr int S_THREADS = (1 + 24 + 4) * 32;   // MMA warp, 24 producer warps, 4 epilogue warps
+constexpr int SN = 128;                      // tile cols
+constexpr int S_BOX_BYTES = SK * 128;        // 4 KB = one [128 cols][32 k] e4m3 operand block
+constexpr int SPW = 2;                       // producer warps per stage: one per operand block (A, B)
+constexpr int NGRP = 4;                      // producer groups: K-step k belongs to group k % NGRP
+constexpr int SST = 2 * NGRP;                // ring stages: K-step k lives in stage k % SST, so a group alternates between two
+                                             // stages (the refill round trip is several MMA periods long)
+constexpr int S_STAGE_BYTES = SPW * S_BOX_BYTES;
+constexpr int S_CONSUMER_WARPS = 8;
+constexpr int S_THREADS = (S_CONSUMER_WARPS + SPW * NGRP) * 32;   // 512: 128 registers a thread at launch
+constexpr int S_CHAIN = 4;                   // wgmma per fp32 promotion
+constexpr int S_REG_PRODUCER = 72, S_REG_CONSUMER = 184;          // 256 x 72 + 256 x 184 = 65536
+constexpr size_t S_SMEM = (size_t)SST * S_STAGE_BYTES + 1024 /*align*/ + 512 /*barriers*/;
 
-// byte offset of element (K-row k, column col < 128) inside one [32 k][128 cols] operand block of 1-byte elements: the canonical
-// MN-major SWIZZLE_128B layout has 128 B (= 128 e4m3 elements along MN) per K-row, 8 K-rows per 1024-B swizzle atom, and the
-// 16-byte chunk index XOR-ed with the row inside the atom
-__device__ __forceinline__ uint32_t sw128_off(int k, int col) {
-  return (uint32_t)(k * 128 + ((((col >> 4) ^ (k & 7)) << 4) | (col & 15)));
+// byte offset of element (K-row k < 32, column col < 128) inside one operand block of 1-byte elements in the canonical K-major
+// SWIZZLE_32B layout: 32 B (= the 32 K values) per column, 8 columns per 256-B swizzle atom, and the 16-byte chunk index
+// XOR-ed with bit 2 of the column (address bit 7)
+__device__ __forceinline__ uint32_t kmaj_off(int k, int col) {
+  return (uint32_t)(col * 32 + ((((k >> 4) ^ (col >> 2)) & 1) << 4) + (k & 15));
 }
-// Instruction descriptor for kind::f8f6f4: c_format F32 (1) @4, a/b_format E4M3 (0) @7/@10, a_major/b_major = MN (1) @15/@16
-// (valid for the 8-bit formats, cute/arch/mma_sm100_desc.hpp), N>>3 @17, M>>4 @24.
-__device__ __forceinline__ uint32_t umma_idesc_e4m3_mn(int M, int N) {
-  return (1u << 4) | (1u << 15) | (1u << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
+// the K-row (row inside the 32-row group) of a key
+__device__ __forceinline__ int kmaj_row(uint32_t key) { return (int)(((((key >> 4) ^ (key >> 7)) & 1) << 4) | (key & 15)); }
 
-template <int NCTA>
 __global__ void __launch_bounds__(S_THREADS, 1)
-gram_csr_tcgen05_kernel(const Problem* __restrict__ probs, const GramTile* __restrict__ tiles, int ntiles, int force, int bias_col, int share) {
-  using C = SCfg<NCTA>;
-  constexpr int SPW = C::SPW, NGRP = C::NGRP, SST = C::SST, STAGE_BYTES = C::STAGE_BYTES;
-  if (share > 1 && blockIdx.z % share != 0) return;   // see gram_tcgen05_kernel (both CTAs of a pair take the same exit)
+gram_csr_wgmma_kernel(const Problem* __restrict__ probs, const GramTile* __restrict__ tiles, int ntiles, int force, int bias_col, int share) {
+  if (share > 1 && blockIdx.z % share != 0) return;   // see gram_wgmma_kernel
   const Problem& pb = probs[blockIdx.z];
   Ctrl* ctrl = pb.ctrl;
   if (!force && (ctrl->done || !ctrl->need_hess)) return;
-  // NCTA = 2: the tile list holds (BI, bj) of 256 x 256 tiles; this CTA's rows are the 128-block 2 BI + rank
-  const uint32_t rank = NCTA == 2 ? cluster_ctarank() : 0u;
-  const GramTile tile_in = tiles[NCTA == 2 ? (blockIdx.x >> 1) : blockIdx.x];
-  const int tile_bi = NCTA == 2 ? tile_in.bi * 2 + (int)rank : tile_in.bi;
-  const int tile_bj = tile_in.bj;
+  const GramTile tile = tiles[blockIdx.x];
   const int slice = blockIdx.y, nslices = gridDim.y;
   const int Dp = pb.Dp;
   const long long n = pb.n;
@@ -251,71 +196,76 @@ gram_csr_tcgen05_kernel(const Problem* __restrict__ probs, const GramTile* __res
 
   extern __shared__ unsigned char g_smem_raw[];
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(g_smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)SST * STAGE_BYTES);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)SST * S_STAGE_BYTES);
   uint64_t* empty_bar = full_bar + SST;
-  uint64_t* acc_bar = empty_bar + SST;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_bar + 1);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   // clear the whole ring once
-  for (int e = threadIdx.x; e < SST * STAGE_BYTES / 16; e += S_THREADS) reinterpret_cast<uint4*>(smem)[e] = make_uint4(0u, 0u, 0u, 0u);
-  if (warp == 1 && lane == 0) {
-    // full: one arrival per producer warp of the stage, of BOTH CTAs for a pair (the barrier the MMA thread waits on is the leader's)
-    for (int s = 0; s < SST; s++) { mbar_init(&full_bar[s], SPW * NCTA); mbar_init(&empty_bar[s], 1); }
-    mbar_init(acc_bar, 1);
+  for (int e = threadIdx.x; e < SST * S_STAGE_BYTES / 16; e += S_THREADS) reinterpret_cast<uint4*>(smem)[e] = make_uint4(0u, 0u, 0u, 0u);
+  if (threadIdx.x == 0) {
+    // full: one arrival per producer warp of the stage; empty: one per consumer warp
+    for (int s = 0; s < SST; s++) { mbar_init(&full_bar[s], SPW); mbar_init(&empty_bar[s], S_CONSUMER_WARPS); }
     fence_mbar_init();
   }
-  if (warp == 0) {
-    if (NCTA == 2) { tmem_alloc2(tmem_slot, GN); tmem_relinquish2(); }
-    else { tmem_alloc(tmem_slot, GN); tmem_relinquish(); }
-  }
   fence_proxy_async_smem();   // the zero fill must be visible to the async proxy too
-  tc_fence_before();
-  if (NCTA == 2) cluster_sync_all(); else __syncthreads();   // the peer must see initialised barriers before its first remote arrive
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
 
-  if (warp == 0) {
-    if (lane == 0 && rank == 0) {
-      // ===== MMA issuer (the leader CTA's, for a pair) =====
-      // one tcgen05.mma.kind::f8f6f4 per stage: K = 32 = the stage's 32-row group (4 swizzle atoms, SBO = 1024 B apart);
-      // NCTA = 1: the B tile's second 128-column group sits LBO = 4 KB after the first; NCTA = 2: M = 256, each CTA holds one A
-      // block and one B block at the same offsets.  The loop over the ring is unrolled so that a stage's barrier addresses and
-      // descriptors are constants: at the e4m3 rate an MMA lasts ~130-220 clk, and the ~45 dependent single-thread instructions
-      // of a rolled iteration (address math, R2UR moves) were the bottleneck (ncu r02: tensor pipe 35 %).
-      const uint32_t idesc = umma_idesc_e4m3_mn(GM * NCTA, GN);
-      const uint32_t smem_base = smem_u32(smem);
-      const uint64_t da0 = umma_desc_mn_sw128(smem_base, S_BOX_BYTES, 1024);
-      const uint64_t db0 = umma_desc_mn_sw128(smem_base + S_BOX_BYTES, S_BOX_BYTES, 1024);
-      constexpr uint64_t DSTEP = (uint64_t)(STAGE_BYTES >> 4);   // the address field counts 16-byte units; the ring stays below its 14 bits
-      for (int k0 = 0; k0 < nk; k0 += SST) {
-        const uint32_t par = (uint32_t)((k0 / SST) & 1);
+  if (warp < S_CONSUMER_WARPS) {
+    // ===== consumer warpgroup wg: the tile's rows wg * 64 .. +63 = columns wg * 64 .. of the A block =====
+    setmaxnreg_inc<S_REG_CONSUMER>();
+    const int wg = warp >> 2;
+    float acc[SN / 2], chain[SN / 2];
 #pragma unroll
-        for (int st = 0; st < SST; st++) {
-          if (k0 + st < nk) {
-            if (NCTA == 2) mbar_wait_cluster(&full_bar[st], par); else mbar_wait(&full_bar[st], par);
-            tc_fence_after();
-            if (NCTA == 2) {
-              umma_f8_2cta(tmem_base, da0 + (uint64_t)st * DSTEP, db0 + (uint64_t)st * DSTEP, idesc, (k0 + st) != 0 ? 1u : 0u);
-              umma_commit_2cta(&empty_bar[st]);
-            } else {
-              umma_f8(tmem_base, da0 + (uint64_t)st * DSTEP, db0 + (uint64_t)st * DSTEP, idesc, (k0 + st) != 0 ? 1u : 0u);
-              umma_commit(&empty_bar[st]);
-            }
-          }
-        }
+    for (int j = 0; j < SN / 2; j++) acc[j] = 0.f;
+    const uint32_t smem_base = smem_u32(smem);
+    // stage k: wait for its operands, issue its product into the chain registers (accumulate = 0 starts a chain)
+    auto issue = [&](int k, uint32_t accumulate) {
+      const int st = k % SST;
+      mbar_wait(&full_bar[st], (uint32_t)((k / SST) & 1));
+      const uint32_t a_addr = smem_base + (uint32_t)(st * S_STAGE_BYTES + wg * 64 * SK);
+      const uint32_t b_addr = smem_base + (uint32_t)(st * S_STAGE_BYTES + S_BOX_BYTES);
+      wgmma_fence();
+      // K = 32 = the stage's 32-row group = one swizzle atom along K: LBO unused, SBO = 256 B between 8-column groups
+      wgmma_e4m3_m64n128k32(chain, wgmma_desc(a_addr, 16, 256, DESC_SW32), wgmma_desc(b_addr, 16, 256, DESC_SW32), accumulate);
+      wgmma_commit();
+    };
+    // stage k's product has retired: hand its buffer back to the producers
+    auto release = [&](int k) { if (lane == 0) mbar_arrive(&empty_bar[k % SST]); };
+    auto promote = [&]() {
+#pragma unroll
+      for (int j = 0; j < SN / 2; j++) acc[j] += chain[j];
+    };
+    // whole chains are straight-line code: a data-dependent branch between a wgmma and the next makes the compiler wait for
+    // every product in flight at the join
+    const int nfull = nk - nk % S_CHAIN;
+    for (int k0 = 0; k0 < nfull; k0 += S_CHAIN) {
+#pragma unroll
+      for (int c = 0; c < S_CHAIN; c++) {
+        issue(k0 + c, c != 0 ? 1u : 0u);
+        if (c > 0) { wgmma_wait<1>(); release(k0 + c - 1); }
       }
-      if (NCTA == 2) umma_commit_2cta(acc_bar); else umma_commit(acc_bar);
+      wgmma_wait<0>();
+      release(k0 + S_CHAIN - 1);
+      promote();
     }
-  } else if (warp <= 24) {
-    // ===== producers: SPW warps per stage, one per 128-column operand block (A block; the B tile's block(s) this CTA holds).
+    for (int k = nfull; k < nk; k++) {   // the last nk % S_CHAIN stages, a chain each
+      issue(k, 0u);
+      wgmma_wait<0>();
+      release(k);
+      promote();
+    }
+    store_acc<SN>(pb.Hpart + (size_t)slice * Dp * Dp, Dp, tile.bi * 128 + wg * 64, tile.bj * SN, acc);
+  } else {
+    // ===== producers: SPW warps per stage, one per 128-column operand block (the A block, the B block).
     // One K-step = one 32-row group, whose entries for a 128-column block are one contiguous run of the block-major list.
     // Offsets are fetched three uses ahead and the first 64 entries of a run two uses ahead, so the loads of a use are in flight
-    // during the whole previous uses.  Group t = (warp - 1) / SPW owns the K-steps k = t, t + NGRP, ...; K-step k lives in ring
-    // stage k % SST, so a group alternates between the stages t and t + NGRP.
-    const int grp = (warp - 1) / SPW, strm = (warp - 1) % SPW;
+    // during the whole previous uses.  Group t owns the K-steps k = t, t + NGRP, ...; K-step k lives in ring stage k % SST, so a
+    // group alternates between the stages t and t + NGRP.
+    setmaxnreg_dec<S_REG_PRODUCER>();
+    const int pw = warp - S_CONSUMER_WARPS;
+    const int grp = pw / SPW, strm = pw % SPW;
     const size_t strm_off = (size_t)strm * S_BOX_BYTES;
-    const int blk = strm == 0 ? tile_bi : (NCTA == 2 ? tile_bj * 2 + (int)rank : tile_bj * 2 + (strm - 1));
+    const int blk = strm == 0 ? tile.bi : tile.bj;
     const bool valid = blk < pb.nblk128;
     const long long ngroups = pb.bm_groups;
     const long long* __restrict__ my_offs = pb.bm_offs + (size_t)(valid ? blk : 0) * ngroups + (lane & 1);
@@ -324,11 +274,9 @@ gram_csr_tcgen05_kernel(const Problem* __restrict__ probs, const GramTile* __res
     const float* __restrict__ sdv = pb.sdvec;
     // the bias column (value 1 in every row, llf/LibLinearDataset.java:592-614) is not stored in the CSR rows
     const bool has_bias_col = valid && bias_col >= blk * 128 && bias_col < blk * 128 + 128;
-    const uint32_t bias_off = has_bias_col ? sw128_off(lane, bias_col - blk * 128) : 0u;
+    const uint32_t bias_off = has_bias_col ? kmaj_off(lane, bias_col - blk * 128) : 0u;
     constexpr uint32_t NOKEY = 0xFFFFFFFFu;
     const bool fetch = valid && lane < 2;
-    // the full barriers the MMA thread waits on are the leader's: a pair's producers arrive through the cluster address space
-    const uint32_t full0_remote = NCTA == 2 ? mapa_u32(&full_bar[0], 0) : 0u;
 
     // Pipeline registers: offsets three uses ahead (o_c), entries + sqrt(d) two uses ahead (set 2), one use ahead (set 1),
     // current (set 0); what the last TWO uses stored (p1 = previous use = the other stage, p2 = the use before = this stage).
@@ -362,7 +310,7 @@ gram_csr_tcgen05_kernel(const Problem* __restrict__ probs, const GramTile* __res
     bool p1row = false, p2row = false;
     for (int k = grp, use = 0; k < nk; k += NGRP, use++) {
       const int st = k % SST;
-      const uint32_t sbase = smem_base_u32 + (uint32_t)st * (uint32_t)STAGE_BYTES + (uint32_t)strm_off;   // shared-space address
+      const uint32_t sbase = smem_base_u32 + (uint32_t)st * (uint32_t)S_STAGE_BYTES + (uint32_t)strm_off;   // shared-space address
       // ---- un-write what the previous use of THIS STAGE (two uses ago) stored (same addresses, zero)
       const int fill = k / SST;   // how many times this stage has been filled before
       if (fill > 0) {
@@ -381,7 +329,7 @@ gram_csr_tcgen05_kernel(const Problem* __restrict__ probs, const GramTile* __res
       for (int q = 0; q < 2; q++) {
         const bool v = key0[q] != NOKEY;
         const uint32_t key = v ? key0[q] : 0u;
-        const float sdk = __shfl_sync(0xffffffffu, sd0, (key >> 7) & 31);
+        const float sdk = __shfl_sync(0xffffffffu, sd0, kmaj_row(key));
         if (v) sts_u8(sbase + key, to_e4m3(val0[q] * sdk));
       }
       for (uint32_t e0 = lo0 + 64; e0 < hi0; e0 += 32) {
@@ -389,18 +337,16 @@ gram_csr_tcgen05_kernel(const Problem* __restrict__ probs, const GramTile* __res
         const bool v = e < hi0;
         const uint32_t key = v ? (uint32_t)__ldg(keys + e) : 0u;
         const float val = v ? __ldg(bvals + e) : 0.f;
-        const float sdk = __shfl_sync(0xffffffffu, sd0, (key >> 7) & 31);
+        const float sdk = __shfl_sync(0xffffffffu, sd0, kmaj_row(key));
         if (v) sts_u8(sbase + key, to_e4m3(val * sdk));
       }
       const bool row_now = (ks0 + k) * SK + lane < n;
       if (row_now && has_bias_col) sts_u8(sbase + bias_off, to_e4m3(sd0));
       fence_proxy_async_smem();
       __syncwarp();
-      if (lane == 0) {
-        if (NCTA == 2) mbar_arrive_cluster(full0_remote + (uint32_t)st * 8u); else mbar_arrive(&full_bar[st]);
-      }
+      if (lane == 0) mbar_arrive(&full_bar[st]);
       // ---- issue the loads of the use after next.  AFTER the hand-over, not before this use's stores: the fence above compiles to
-      // MEMBAR.ALL.CTA, which waits for every load this thread still has in flight -- issued at the top of the use they would
+      // a memory barrier that waits for every load this thread still has in flight -- issued at the top of the use they would
       // make each hand-over wait out a DRAM round trip; issued here they have the whole next use to arrive.
       lo2 = __shfl_sync(0xffffffffu, o_c, 0); hi2 = __shfl_sync(0xffffffffu, o_c, 1);
       o_c = ld_offs(k + 3 * NGRP);
@@ -412,55 +358,12 @@ gram_csr_tcgen05_kernel(const Problem* __restrict__ probs, const GramTile* __res
       for (int q = 0; q < 2; q++) { p2key[q] = p1key[q]; p1key[q] = key0[q]; key0[q] = key1[q]; val0[q] = val1[q]; key1[q] = key2[q]; val1[q] = val2[q]; }
       sd0 = sd1; sd1 = sd2;
     }
-  } else {
-    // ===== epilogue: the last four warps -> TMEM lane quadrant (warp % 4); a pair's CTA holds its own 128 rows of the tile =====
-    const int quad = warp & 3;
-    float* out = pb.Hpart + (size_t)slice * Dp * Dp;
-    const int row = tile_bi * GM + quad * 32 + lane;
-    if (nk > 0) {
-      while (!mbar_try_wait(acc_bar, 0)) __nanosleep(512);   // the whole main loop long: do not spend issue slots on polling
-      tc_fence_after();
-    }
-#pragma unroll 1
-    for (int c0 = 0; c0 < GN; c0 += 32) {
-      uint32_t r[32];
-      if (nk > 0) {
-        tmem_ld_32x32b_x32(tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)c0, r);
-        tmem_ld_wait();
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; j++) r[j] = 0u;
-      }
-      const int col = tile_bj * GN + c0;
-      if (row < Dp && col < Dp) {
-        float4* dst = reinterpret_cast<float4*>(out + (size_t)row * Dp + col);
-#pragma unroll
-        for (int j = 0; j < 8; j++)
-          dst[j] = make_float4(__uint_as_float(r[4 * j]), __uint_as_float(r[4 * j + 1]), __uint_as_float(r[4 * j + 2]),
-                               __uint_as_float(r[4 * j + 3]));
-      }
-    }
-    tc_fence_before();
-  }
-  if (NCTA == 2) {
-    tc_fence_before();
-    cluster_sync_all();   // neither CTA may leave (or free its TMEM) while the pair's MMAs, commits or remote arrives can still touch it
-    if (warp == 0) {
-      tc_fence_after();
-      tmem_dealloc2(tmem_base, GN);
-    }
-  } else {
-    __syncthreads();
-    if (warp == 0) {
-      tc_fence_after();
-      tmem_dealloc(tmem_base, GN);
-    }
   }
 }
 
 // Block-major entry list for the CSR Gram.  For every 128-column block b and every 32-row group g the entries
 // (row in group, column in block, value) are stored contiguously at [offs[b*ngroups+g], offs[b*ngroups+g+1]); the key is
-// the byte offset of the element inside a swizzled [32 k][128 col] operand block (sw128_off), the value the stored float.
+// the byte offset of the element inside a swizzled [128 col][32 k] operand block (kmaj_off), the value the stored float.
 // Rows must be sorted by column (strictly increasing), which the upload checks.
 __global__ void __launch_bounds__(256) csr_bm_count_kernel(long long n, const long long* __restrict__ rowptr, const int* __restrict__ colidx,
                                                            int nblk, long long ngroups, long long* __restrict__ counts) {
@@ -502,7 +405,7 @@ __global__ void __launch_bounds__(256) csr_bm_fill_kernel(long long n, const lon
       }
       long long pos = offs[(size_t)b * ngroups + g] + (incl - c);
       for (long long e = s; e < j; e++, pos++) {
-        keys[pos] = (unsigned short)sw128_off(lane, colidx[e] - b * 128);
+        keys[pos] = (unsigned short)kmaj_off(lane, colidx[e] - b * 128);
         bvals[pos] = vals[e];
       }
     }
@@ -580,77 +483,53 @@ int gram_make_tensor_map(void* out_map_host /*CUtensorMap, 128 B*/, const void* 
   return r == CUDA_SUCCESS ? 0 : 2;
 }
 
-// Lower block-triangle tile list for a Dp x Dp output (Dp multiple of 128): 128 x 256 tiles (bi, bj), or, for the CTA-pair CSR
-// kernel, 256 x 256 tiles (BI, bj) whose two row blocks 2 BI and 2 BI + 1 belong to the two CTAs of the pair.
-int gram_tile_list(int Dp, short* bi_bj_pairs /*[2*max]*/, int max_tiles, int pair_tiles) {
+// Lower block-triangle tile list for a Dp x Dp output (Dp multiple of 128): 128 x 256 tiles (bi, bj) for the bf16 kernel, or
+// 128 x 128 tiles for the CSR kernel (csr_tiles != 0).
+int gram_tile_list(int Dp, short* bi_bj_pairs /*[2*max]*/, int max_tiles, int csr_tiles) {
   int n = 0;
-  const int rows = pair_tiles ? 2 * GM : GM;
-  const int nbi = (Dp + rows - 1) / rows, nbj = (Dp + GN - 1) / GN;
+  const int cols = csr_tiles ? SN : GN;
+  const int nbi = (Dp + GM - 1) / GM, nbj = (Dp + cols - 1) / cols;
   for (int bi = 0; bi < nbi; bi++)
     for (int bj = 0; bj < nbj; bj++)
-      if (bj * GN <= bi * rows + rows - 1) {
+      if (bj * cols <= bi * GM + GM - 1) {
         if (n >= max_tiles) return -1;
         bi_bj_pairs[2 * n] = (short)bi; bi_bj_pairs[2 * n + 1] = (short)bj; n++;
       }
   return n;
 }
 
-cudaError_t gram_launch_tcgen05(const Problem* d_probs, int nprob, const void* d_tmaps, const void* d_tiles, int ntiles,
-                                int nslices, int force, cudaStream_t st, int* launches, int share) {
-  {
-    // the attribute is per device: set it once for every device this process launches on
-    static bool configured[64] = {};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    if (dev < 0 || dev >= 64 || !configured[dev]) {
-      cudaError_t e = cudaFuncSetAttribute(gram_tcgen05_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G_SMEM);
-      if (e != cudaSuccess) return e;
-      if (dev >= 0 && dev < 64) configured[dev] = true;
-    }
-  }
-  gram_tcgen05_kernel<<<dim3(ntiles, nslices, nprob), G_THREADS, G_SMEM, st>>>(
-      d_probs, reinterpret_cast<const CUtensorMap*>(d_tmaps), reinterpret_cast<const GramTile*>(d_tiles), ntiles, force, share);
-  if (launches) *launches += 1;
-  return cudaGetLastError();
-}
-
-template <int NCTA>
-static cudaError_t gram_csr_configure() {
-  // the attribute is per device: set it once for every device this process launches on
-  static bool configured[64] = {};
+// the attribute is per device: set it once for every device this process launches on
+template <typename K>
+static cudaError_t set_smem_once(K kernel, size_t bytes, bool (&configured)[64]) {
   int dev = 0;
   cudaGetDevice(&dev);
   if (dev < 0 || dev >= 64 || !configured[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(gram_csr_tcgen05_kernel<NCTA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SCfg<NCTA>::SMEM);
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
     if (e != cudaSuccess) return e;
     if (dev >= 0 && dev < 64) configured[dev] = true;
   }
   return cudaSuccess;
 }
 
-// ncta = 2: d_tiles holds 256 x 256 pair tiles (gram_tile_list(..., 1)); the grid is a list of 2-CTA clusters along x.
-cudaError_t gram_launch_csr_tcgen05(const Problem* d_probs, int nprob, const void* d_tiles, int ntiles, int nslices, int force,
-                                    int bias_col, cudaStream_t st, int* launches, int share, int ncta) {
-  const GramTile* tl = reinterpret_cast<const GramTile*>(d_tiles);
-  if (ncta == 2) {
-    cudaError_t e = gram_csr_configure<2>();
-    if (e != cudaSuccess) return e;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(2 * ntiles, nslices, nprob);
-    cfg.blockDim = dim3(S_THREADS, 1, 1);
-    cfg.dynamicSmemBytes = SCfg<2>::SMEM;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    e = cudaLaunchKernelEx(&cfg, gram_csr_tcgen05_kernel<2>, d_probs, tl, ntiles, force, bias_col, share);
-    if (e != cudaSuccess) return e;
-  } else {
-    cudaError_t e = gram_csr_configure<1>();
-    if (e != cudaSuccess) return e;
-    gram_csr_tcgen05_kernel<1><<<dim3(ntiles, nslices, nprob), S_THREADS, SCfg<1>::SMEM, st>>>(d_probs, tl, ntiles, force, bias_col, share);
-  }
+cudaError_t gram_launch_wgmma(const Problem* d_probs, int nprob, const void* d_tmaps, const void* d_tiles, int ntiles,
+                              int nslices, int force, cudaStream_t st, int* launches, int share) {
+  static bool configured[64] = {};
+  cudaError_t e = set_smem_once(gram_wgmma_kernel, G_SMEM, configured);
+  if (e != cudaSuccess) return e;
+  gram_wgmma_kernel<<<dim3(ntiles, nslices, nprob), G_THREADS, G_SMEM, st>>>(
+      d_probs, reinterpret_cast<const CUtensorMap*>(d_tmaps), reinterpret_cast<const GramTile*>(d_tiles), ntiles, force, share);
+  if (launches) *launches += 1;
+  return cudaGetLastError();
+}
+
+// d_tiles holds the 128 x 128 tiles of gram_tile_list(..., 1)
+cudaError_t gram_launch_csr_wgmma(const Problem* d_probs, int nprob, const void* d_tiles, int ntiles, int nslices, int force,
+                                  int bias_col, cudaStream_t st, int* launches, int share) {
+  static bool configured[64] = {};
+  cudaError_t e = set_smem_once(gram_csr_wgmma_kernel, S_SMEM, configured);
+  if (e != cudaSuccess) return e;
+  gram_csr_wgmma_kernel<<<dim3(ntiles, nslices, nprob), S_THREADS, S_SMEM, st>>>(
+      d_probs, reinterpret_cast<const GramTile*>(d_tiles), ntiles, force, bias_col, share);
   if (launches) *launches += 1;
   return cudaGetLastError();
 }
@@ -661,7 +540,7 @@ cudaError_t csr_bm_offsets(long long n, const long long* rowptr, const int* coli
   const long long m = (long long)nblk * ngroups;
   cudaError_t e = cudaMemsetAsync(offs, 0, (size_t)(m + 1) * sizeof(long long), st);
   if (e != cudaSuccess) return e;
-  const int grid = (int)std::min<long long>((ngroups + 7) / 8, 148 * 32);
+  const int grid = (int)std::min<long long>((ngroups + 7) / 8, 132 * 32);
   csr_bm_count_kernel<<<std::max(grid, 1), 256, 0, st>>>(n, rowptr, colidx, nblk, ngroups, offs);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
   size_t tmp_bytes = 0;
@@ -675,7 +554,7 @@ cudaError_t csr_bm_offsets(long long n, const long long* rowptr, const int* coli
 
 cudaError_t csr_bm_fill(long long n, const long long* rowptr, const int* colidx, const float* vals, int nblk, long long ngroups,
                         const long long* offs, unsigned short* keys, float* bvals, cudaStream_t st) {
-  const int grid = (int)std::min<long long>((ngroups + 7) / 8, 148 * 32);
+  const int grid = (int)std::min<long long>((ngroups + 7) / 8, 132 * 32);
   csr_bm_fill_kernel<<<std::max(grid, 1), 256, 0, st>>>(n, rowptr, colidx, vals, nblk, ngroups, offs, keys, bvals);
   return cudaGetLastError();
 }

@@ -7,7 +7,7 @@
 //
 // fp64 on purpose: the Gram comes from bf16 tensor-core products, but the factorisation must not
 // break down when cond(H) approaches 1/eps_fp32; 3.3e8 flop at D'=1001 is latency- not
-// throughput-bound on B200's fp64 pipe.
+// throughput-bound on the fp64 pipe.
 #include <algorithm>
 #include <cstdlib>
 
@@ -21,7 +21,7 @@ constexpr int TB = 64;   // trailing-update tile
 // Hd (lower incl. diagonal) = sum_s Hpart[s] + diag(q); padded rows/cols (>= Dt) = identity.
 __global__ void chol_prep_kernel(const Problem* __restrict__ probs, int share) {
   const Problem& pb = probs[blockIdx.z];
-  // share = L > 1: the Gram partials of the group's first problem stand for the whole group (see gram_tcgen05_kernel)
+  // share = L > 1: the Gram partials of the group's first problem stand for the whole group (see gram_wgmma_kernel)
   const float* __restrict__ hpart = share > 1 ? probs[blockIdx.z - blockIdx.z % share].Hpart : pb.Hpart;
   Ctrl* c = pb.ctrl;
   if (c->done || !c->need_hess) return;
@@ -521,14 +521,14 @@ static cudaError_t dgemm_launch(const Problem* d_probs, int nprob, int mode, int
 // There Y = L^-1 is only ever read after rounding to bf16, and Y^T Y is SPD for ANY Y, so an inexact inverse cannot turn the
 // preconditioner indefinite (the factorisation itself -- pivots -- stays in fp64).  The two GEMMs of a merge,
 //   T = L21 * Y11 (mode 1)   and   Y21 = -Y22 * T (mode 2),
-// are half of the D'^3 flops of a 10k-wide factorisation and run at ~25 TFLOP/s on the fp64 pipe; here the fp64 operands
+// are half of the D'^3 flops of a 10k-wide factorisation and are bound by the fp64 pipe; here the fp64 operands
 // are rounded to tf32 on their way into shared memory (cvt.rna) and multiplied by mma.sync.m16n8k8 with fp32 accumulation:
 // operand rounding 2^-11, against 2^-8 of the bf16 storage the result ends up in.  128x128 tiles, K chunks of 16, the same
 // register-staged double buffer as dgemm_kernel; both operands are row-major (A[i][k], B[k][j]) as in dgemm_kernel<true,false>.
 // Shared-memory strides: A rows of 20 words (fragment loads (row g, k tg): bank 20 g + tg, all distinct), B rows of 136
 // words (fragment loads (k tg, col g): bank 8 tg + g, all distinct).
 // ------------------------------------------------------------------------------------------
-constexpr int MERGE_TF32_DEFAULT = 1;   // verified on a B200: GPU parity suite + bench with MLEASE_MERGE_TF32=1 (profiles/r02b_*)
+constexpr int MERGE_TF32_DEFAULT = 1;   // the GPU parity suite runs with it
 constexpr int TM = 128, TN = 128, TK = 16;
 constexpr int TA_LD = TK + 4, TB_LD = TN + 8;
 constexpr int TA_SZ = TM * TA_LD, TB_SZ = TK * TB_LD;   // 32-bit words per stage
@@ -697,7 +697,7 @@ static int wide_threshold() {
   static int t = -1;
   if (t < 0) {
     const char* e = getenv("MLEASE_WIDE_MIN");
-    t = e ? atoi(e) : 1000;   // measured on B200: D'=1001 (ldh 1024) rebuilds take 4.9 ms (8 problems) / 2.0 ms (1) wide vs 8.1 / 2.75 ms narrow
+    t = e ? atoi(e) : 1000;
   }
   return t;
 }

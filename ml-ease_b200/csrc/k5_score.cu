@@ -63,7 +63,7 @@ cudaError_t score_launch(int Dg, long long nrows, const long long* rowptr, const
                          cudaStream_t st) {
   if (nrows == 0) return cudaSuccess;
   long long blocks = (nrows + 7) / 8;
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   score_kernel<<<(int)blocks, 256, 0, st>>>(Dg, nrows, rowptr, colidx, vals, ldx, offset, d_model, intercept_term, binary_feature, pred);
   return cudaGetLastError();
 }

@@ -25,11 +25,11 @@ cudaError_t newton_solve(const Problem* d_probs, int nprob, int ldh, cudaStream_
 
 // K2 (k2_gram.cu)
 int gram_make_tensor_map(void* out_map_host, const void* xt, long long n, int Dp);
-int gram_tile_list(int Dp, short* bi_bj_pairs, int max_tiles, int pair_tiles = 0);
-cudaError_t gram_launch_tcgen05(const Problem* d_probs, int nprob, const void* d_tmaps, const void* d_tiles, int ntiles,
-                                int nslices, int force, cudaStream_t st, int* launches, int share = 0);
-cudaError_t gram_launch_csr_tcgen05(const Problem* d_probs, int nprob, const void* d_tiles, int ntiles, int nslices, int force,
-                                    int bias_col, cudaStream_t st, int* launches, int share = 0, int ncta = 1);
+int gram_tile_list(int Dp, short* bi_bj_pairs, int max_tiles, int csr_tiles = 0);
+cudaError_t gram_launch_wgmma(const Problem* d_probs, int nprob, const void* d_tmaps, const void* d_tiles, int ntiles,
+                              int nslices, int force, cudaStream_t st, int* launches, int share = 0);
+cudaError_t gram_launch_csr_wgmma(const Problem* d_probs, int nprob, const void* d_tiles, int ntiles, int nslices, int force,
+                                  int bias_col, cudaStream_t st, int* launches, int share = 0);
 cudaError_t csr_bm_offsets(long long n, const long long* rowptr, const int* colidx, int nblk, long long ngroups, long long* offs, cudaStream_t st);
 cudaError_t csr_bm_fill(long long n, const long long* rowptr, const int* colidx, const float* vals, int nblk, long long ngroups,
                         const long long* offs, unsigned short* keys, float* bvals, cudaStream_t st);

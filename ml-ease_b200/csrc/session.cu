@@ -143,7 +143,6 @@ struct Batch {
   bool csr = false;
   int has_bias = 1;
   int k1_grid = 1, gram_slices = 1, ntiles = 0;
-  int gram_ncta = 1;              // 2: the CSR Gram runs on CTA pairs (cta_group::2, 256 x 256 tiles); d_tiles then holds pair tiles
   int gram_from_csr = 0;          // every problem of the batch assembles its Gram tiles from CSR (no dense bf16 operand)
   int group_L = 1;                // problems b = g * group_L + l share the data of partition g (the lambdas of one partition)
   int k1_fused = 0;               // the fused multi-lambda CSR K1 runs (segment lists present): one launch, grid (sg_S, nprob / group_L)
@@ -255,8 +254,9 @@ int batch_alloc(Batch& B, int num_sms) {
     }
   }
   const int gpart_rows = B.k1_fused ? 1 : B.k1_grid;   // the fused kernel keeps its partials in gpart_f (fp32)
-  // Cost model for the rebuild policy (seconds, order of magnitude): one K1 pass streams the partition at ~5 TB/s; a rebuild
-  // is n*Dt^2 bf16 flop at ~1 PFLOP/s (tcgen05 Gram, lower triangle) plus ~Dt^3 fp64 flop at ~5 TFLOP/s (Cholesky + inverse).
+  // Cost model for the rebuild policy (seconds, order of magnitude only: the policy compares the two with a factor of 8): one K1
+  // pass streams the partition at ~5 TB/s; a rebuild is n*Dt^2 flop at ~1 PFLOP/s (tensor-core Gram, lower triangle) plus
+  // ~Dt^3 fp64 flop at ~5 TFLOP/s (Cholesky + inverse).
   {
     double bytes = 0;
     for (auto& p : B.h) bytes = std::max(bytes, B.csr ? 8.0 * (double)p.nnz_hint + 17.0 * (double)p.n : (double)p.n * 4.0 * ldx);
@@ -271,15 +271,14 @@ int batch_alloc(Batch& B, int num_sms) {
     if (const char* e = getenv("MLEASE_BFGS_M")) B.bfgs_m = std::max(1, std::min(BFGS_M, atoi(e)));   // tuning experiments only
   }
   // Gram decomposition
-  constexpr int MAX_TILES = 1 << 18;   // lower 128x256 tiles of Dp up to ~90k
+  constexpr int MAX_TILES = 1 << 18;   // lower 128x128 tiles of Dp up to ~90k
   std::vector<short> tiles(2 * (size_t)MAX_TILES);
-  B.gram_ncta = (B.gram_from_csr && !getenv("MLEASE_GRAM_1CTA")) ? 2 : 1;   // the variable exists for A/B measurements only
-  B.ntiles = gram_tile_list(B.Dp, tiles.data(), MAX_TILES, B.gram_ncta == 2);
+  B.ntiles = gram_tile_list(B.Dp, tiles.data(), MAX_TILES, B.gram_from_csr);
   if (B.ntiles <= 0) return fail(MLEASE_ERR_INVALID, "Gram tile list overflow");
   {
     const long long ksteps = (maxn + 63) / 64;
-    const long long base = (long long)B.ntiles * nprob;   // CTAs, or CTA pairs
-    const long long cap = std::max(1, num_sms / B.gram_ncta);
+    const long long base = (long long)B.ntiles * nprob;   // CTAs
+    const long long cap = std::max(1, num_sms);
     int best = 1;
     double best_eff = 0;
     for (int s = 1; s <= 16; s++) {
@@ -415,8 +414,8 @@ int batch_xupdate(Batch& B, cudaStream_t st, double xtol, int max_newton, int po
       const int share = (slot_idx == 0) ? share_first_gram : 0;
       if (share > 1)
         for (int b = 0; b < B.nprob; b++) if (b % share != 0) shared_flops += (double)B.h[b].n * (double)B.Dt * (double)(B.Dt + 1);
-      if (B.gram_from_csr) CK(gram_launch_csr_tcgen05(d_hess, n_hess, B.d_tiles, B.ntiles, B.gram_slices, 0, B.has_bias ? B.Dt - 1 : -1, st, &launches, share, B.gram_ncta));
-      else CK(gram_launch_tcgen05(d_hess, n_hess, B.d_tmaps, B.d_tiles, B.ntiles, B.gram_slices, 0, st, &launches, share));
+      if (B.gram_from_csr) CK(gram_launch_csr_wgmma(d_hess, n_hess, B.d_tiles, B.ntiles, B.gram_slices, 0, B.has_bias ? B.Dt - 1 : -1, st, &launches, share));
+      else CK(gram_launch_wgmma(d_hess, n_hess, B.d_tmaps, B.d_tiles, B.ntiles, B.gram_slices, 0, st, &launches, share));
       pf.end(st);
       pf.begin(3, st);
       const bool share_fact = share > 1 && share_first_factor;   // same rho too: same H, one factorisation per group
@@ -562,7 +561,7 @@ struct mlease_session {
   cudaStream_t copy_stream = nullptr;   // H2D of a CSR partition's arrays, overlapped with the previous partition's layout build
   cudaEvent_t copy_ev = nullptr;        // orders copy_stream after what the caller queued on `stream` (e.g. kernels that produce device inputs)
   int pending_csr = -1;                 // index into parts of the CSR partition whose checks and lists are not built yet
-  int num_sms = 148;
+  int num_sms = 132;
   std::vector<PartData> parts;
   std::vector<void*> owned;
   bool any_csr = false, any_dense = false;
@@ -788,7 +787,7 @@ int mlease_session_create(const mlease_admm_config* cfg, mlease_session** out) {
   CK(cudaSetDevice(cfg->device));
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, cfg->device));
-  if (prop.major != 10) return fail(MLEASE_ERR_CUDA, "this build targets sm_100a (B200) only; found sm_" + std::to_string(prop.major) + std::to_string(prop.minor));
+  if (prop.major != 9) return fail(MLEASE_ERR_CUDA, "this build targets sm_90a (H100) only; found sm_" + std::to_string(prop.major) + std::to_string(prop.minor));
   mlease_session* s = new mlease_session();
   s->cfg = *cfg;
   s->L = cfg->num_lambdas; s->P = cfg->num_blocks; s->Dg = cfg->num_features; s->Dt = s->Dg + 1;
@@ -1283,8 +1282,8 @@ int mlease_objective(mlease_session* s, int32_t pid, const double* w, const doub
   if (f) *f = c.f_t;
   if (H) {
     if (!tensor && B->gram_from_csr) return fail(MLEASE_ERR_INVALID, "the SIMT debug Gram needs the dense bf16 operand, which CSR partitions with sorted unique rows do not materialise");
-    if (tensor && B->gram_from_csr) CK(gram_launch_csr_tcgen05(B->d, 1, B->d_tiles, B->ntiles, B->gram_slices, 1, B->has_bias ? B->Dt - 1 : -1, s->stream, &launches, 0, B->gram_ncta));
-    else if (tensor) CK(gram_launch_tcgen05(B->d, 1, B->d_tmaps, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches));
+    if (tensor && B->gram_from_csr) CK(gram_launch_csr_wgmma(B->d, 1, B->d_tiles, B->ntiles, B->gram_slices, 1, B->has_bias ? B->Dt - 1 : -1, s->stream, &launches, 0));
+    else if (tensor) CK(gram_launch_wgmma(B->d, 1, B->d_tmaps, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches));
     else CK(gram_launch_simt(B->d, 1, B->Dp, 1, s->stream, &launches));
     if (tensor == 2) {
       // the inverse the Newton direction uses: split-K Gram partials + diag(q) -> fp64 Cholesky -> explicit inverse
@@ -1405,8 +1404,8 @@ int mlease_time_kernel(mlease_session* s, int32_t pid, int32_t which, int32_t re
   CK(batch_k1(*B, 1, s->stream, &launches));
   const int bias_col = B->has_bias ? B->Dt - 1 : -1;
   if (which == 3) {
-    if (B->gram_from_csr) CK(gram_launch_csr_tcgen05(B->d, 1, B->d_tiles, B->ntiles, B->gram_slices, 1, bias_col, s->stream, &launches, 0, B->gram_ncta));
-    else CK(gram_launch_tcgen05(B->d, 1, B->d_tmaps, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches));
+    if (B->gram_from_csr) CK(gram_launch_csr_wgmma(B->d, 1, B->d_tiles, B->ntiles, B->gram_slices, 1, bias_col, s->stream, &launches, 0));
+    else CK(gram_launch_wgmma(B->d, 1, B->d_tmaps, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches));
     Ctrl c; std::memset(&c, 0, sizeof(c)); c.need_hess = 1;
     CK(cudaMemcpyAsync(B->d_ctrl, &c, sizeof(Ctrl), cudaMemcpyHostToDevice, s->stream));
   }
@@ -1414,8 +1413,8 @@ int mlease_time_kernel(mlease_session* s, int32_t pid, int32_t which, int32_t re
   CK(cudaEventRecord(e0, s->stream));
   for (int r = 0; r < reps; r++) {
     if (which == 1) CK(batch_k1(*B, emit_scaled ? 1 : 0, s->stream, &launches));
-    else if (which == 2 && B->gram_from_csr) CK(gram_launch_csr_tcgen05(B->d, 1, B->d_tiles, B->ntiles, B->gram_slices, 1, bias_col, s->stream, &launches, 0, B->gram_ncta));
-    else if (which == 2) CK(gram_launch_tcgen05(B->d, 1, B->d_tmaps, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches));
+    else if (which == 2 && B->gram_from_csr) CK(gram_launch_csr_wgmma(B->d, 1, B->d_tiles, B->ntiles, B->gram_slices, 1, bias_col, s->stream, &launches, 0));
+    else if (which == 2) CK(gram_launch_wgmma(B->d, 1, B->d_tmaps, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches));
     else if (which == 3) CK(cholesky_launch(B->d, 1, B->ldh, s->stream, &launches));
     else return fail(MLEASE_ERR_INVALID, "which must be 1, 2 or 3");
   }
@@ -1530,7 +1529,7 @@ int mlease_naive_train(int32_t device, void* stream, int32_t K, int32_t Dg, cons
   cudaStream_t st = (cudaStream_t)stream;
   cudaDeviceProp prop;
   CK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) return fail(MLEASE_ERR_CUDA, "this build targets sm_100a (B200) only");
+  if (prop.major != 9) return fail(MLEASE_ERR_CUDA, "this build targets sm_90a (H100) only; found sm_" + std::to_string(prop.major) + std::to_string(prop.minor));
   const int Dt = Dg + 1, ldx = round_up(Dt, 4);
   // MLEASE_DEBUG: wall-clock of the host-side phases (allocation, ingest, solve, read-back)
   const bool dbg = getenv("MLEASE_DEBUG") != nullptr;

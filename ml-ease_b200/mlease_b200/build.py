@@ -1,4 +1,4 @@
-"""In-tree build of libmlease_b200.so (nvcc, sm_100a only).  `python -m mlease_b200.build`."""
+"""In-tree build of libmlease_b200.so (nvcc, sm_90a only).  `python -m mlease_b200.build`."""
 from __future__ import annotations
 
 import os
@@ -12,7 +12,7 @@ LIBDIR = os.path.join(ROOT, "lib")
 SO = os.path.join(LIBDIR, "libmlease_b200.so")
 SOURCES = ["session.cu", "k1_score_grad.cu", "k1_csr_fused.cu", "newton.cu", "k2_gram.cu", "k3_cholesky.cu", "k4_consensus.cu", "k5_score.cu", "k6_postvar.cu", "comm.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 
 
@@ -48,7 +48,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     if failed:
         raise RuntimeError("nvcc failed")
     if force or procs or _stale(SO, objs):
-        subprocess.check_call([NVCC, "-shared", "-o", SO] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-ldl"])
+        subprocess.check_call([NVCC, "-shared", "-o", SO] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-ldl"])
     build_host(force)
     return SO
 

@@ -11,7 +11,7 @@ for p in (ROOT, os.path.join(ROOT, "ml-ease_b200")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; select with -m gpu)")
 
 
 GOLDEN = os.path.join(ROOT, "tests", "golden")

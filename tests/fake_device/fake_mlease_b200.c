@@ -4,7 +4,7 @@
  * Its only purpose is to let RegressionAdmmTrain / RegressionTest / RegressionTestLoglik / RegressionNaiveTrain run end to end
  * without a GPU, so that their orchestration and file output can be compared between the plan-walker and the generic avro
  * paths and run under sanitizers.  It is not part of the product and is never linked into it: the product library refuses to
- * run without an sm_100 device (tests/test_abi.py). */
+ * run without an sm_90 device (tests/test_abi.py). */
 #include <math.h>
 #include <stdint.h>
 #include <stdlib.h>

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Regenerates tests/golden/*.npz.  Run HERE (container with /root/reference mounted):
+"""Regenerates tests/golden/*.npz from a checkout of the reference project:
 
-    python tests/golden/make_golden.py
+    python tests/golden/make_golden.py <reference checkout>
 
 1. sample_data.npz   -- the reference's only fixture, examples/sample-data.avro, decoded with
                         the minimal Avro object-container reader below (null codec, Pig-style
@@ -13,6 +13,8 @@
 3. oracle_frozen.npz -- frozen outputs of oracle/mlease_oracle.cpp (exact + faithful ADMM on the
                         fixture with 4 partitions, objective values, scores, loglik) so that any
                         later edit of the oracle that changes numbers is caught.
+sample_data_head.avro.gz (not written here) -- the first 12 blocks (157 records) of that fixture file,
+                        byte for byte, gzip-compressed: what the C++ avro readers are tested on.
 """
 import json
 import os
@@ -117,7 +119,7 @@ def read_avro(path):
 def main():
     from oracle import oracle as orc
 
-    schema, recs, nblocks = read_avro("/root/reference/examples/sample-data.avro")
+    schema, recs, nblocks = read_avro(os.path.join(sys.argv[1], "examples", "sample-data.avro"))
     names = sorted({f["name"] for r in recs for f in r["features"]}, key=lambda s: int(s))
     assert all(f["term"] in ("", None) for r in recs for f in r["features"])
     gid = {n: i for i, n in enumerate(names)}

@@ -49,10 +49,10 @@ def test_worst_case_bound_does_not_overflow_and_is_order_independent():
 
 def test_resolution_is_below_float32_rounding_of_the_contributions():
     rng = np.random.default_rng(1)
-    rows, wmax, vmax = 6757, 1.0, 5.0                                  # config 3: 1M rows over 148 CTAs, N(0,1) values
+    rows, wmax, vmax = 7576, 1.0, 5.0                                  # config 3: 1M rows over 132 CTAs, N(0,1) values
     e_hi, kbits = _scales(rows, wmax, vmax)
     assert kbits >= 16
-    n_hit = 70                                                          # ~1 % of the CTA's rows touch a given column
+    n_hit = 76                                                          # ~1 % of the CTA's rows touch a given column
     c = (rng.normal(size=n_hit) * 0.5).astype(np.float32)
     hi, lo = _accumulate(c, e_hi, kbits)
     exact = float(np.sum(c.astype(np.float64)))

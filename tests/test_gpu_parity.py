@@ -192,9 +192,9 @@ def _e4m3_round(a):
 @pytest.mark.parametrize("n,d,sparse", [(1000, 37, False), (2000, 100, False), (700, 300, False), (1000, 50, True), (3000, 700, True),
                                         (333, 255, True)])
 def test_gram_tcgen05_vs_oracle_hessian(mb, n, d, sparse):
-    """Dense partitions: the tcgen05 Gram against the fp64 Hessian and against the fp32 SIMT kernel on the same bf16 operand.
+    """Dense partitions: the wgmma Gram against the fp64 Hessian and against the fp32 SIMT kernel on the same bf16 operand.
     CSR partitions assemble their operand tiles from the CSR rows inside the Gram kernel (no dense copy exists, so no SIMT
-    run) as e4m3 with a power-of-two scale (kind::f8f6f4, twice the bf16 MMA rate; H only preconditions): the check is against
+    run) as e4m3 with a power-of-two scale (wgmma .e4m3, twice the bf16 MMA rate; H only preconditions): the check is against
     a numpy emulation of the e4m3-rounded scaled rows."""
     X, y, w, o = _mk(n, d, seed=3 * n + d, sparse=sparse)
     rng = np.random.default_rng(2)
@@ -229,8 +229,8 @@ def test_gram_tcgen05_vs_oracle_hessian(mb, n, d, sparse):
     e_tc = np.abs(H_tc - H_ref).max() / scale
     e_x = np.abs(H_tc - H_simt).max() / scale
     assert e_simt < 2e-2, ("simt vs oracle", e_simt)
-    assert e_tc < 2e-2, ("tcgen05 vs oracle", e_tc, e_simt, e_x)
-    assert e_x < 1e-3, ("tcgen05 vs simt", e_x)
+    assert e_tc < 2e-2, ("wgmma vs oracle", e_tc, e_simt, e_x)
+    assert e_x < 1e-3, ("wgmma vs simt", e_x)
 
 
 @pytest.mark.parametrize("n,d,sparse", [(1500, 100, False), (3000, 700, False), (2500, 1100, False), (4000, 2303, False), (5000, 2600, True)])

@@ -2,7 +2,7 @@
 //   (a) 1-D bulk TMA copies (cp.async.bulk, UBLKCP) into a shared-memory ring
 //   (b) plain ld.global.nc.v4 into registers
 //   (c) cp.async 16 B (LDGSTS) into a shared-memory ring
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o membw tools/membw.cu ; run on the B200.
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o membw tools/membw.cu ; run on the H100.
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -77,18 +77,18 @@ int main() {
     size_t smem = (size_t)S * tile + 64; if (smem * cps > 225 * 1024) continue;
     cudaFuncSetAttribute(k_bulk, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     char nm[96]; snprintf(nm, 96, "bulk tile=%dKB S=%d ctas/sm=%d", tile / 1024, S, cps);
-    time(nm, [&] { k_bulk<<<148 * cps, 256, smem>>>(x, nbytes, tile, S, out); });
+    time(nm, [&] { k_bulk<<<132 * cps, 256, smem>>>(x, nbytes, tile, S, out); });
   }
   for (int cps : {2, 4, 8}) {
     char nm[96];
-    snprintf(nm, 96, "ldg U=4 ctas/sm=%d", cps); time(nm, [&] { k_ldg<4><<<148 * cps, 256>>>((const float4*)x, nbytes / 16, out); });
-    snprintf(nm, 96, "ldg U=8 ctas/sm=%d", cps); time(nm, [&] { k_ldg<8><<<148 * cps, 256>>>((const float4*)x, nbytes / 16, out); });
-    snprintf(nm, 96, "ldg U=16 ctas/sm=%d", cps); time(nm, [&] { k_ldg<16><<<148 * cps, 256>>>((const float4*)x, nbytes / 16, out); });
+    snprintf(nm, 96, "ldg U=4 ctas/sm=%d", cps); time(nm, [&] { k_ldg<4><<<132 * cps, 256>>>((const float4*)x, nbytes / 16, out); });
+    snprintf(nm, 96, "ldg U=8 ctas/sm=%d", cps); time(nm, [&] { k_ldg<8><<<132 * cps, 256>>>((const float4*)x, nbytes / 16, out); });
+    snprintf(nm, 96, "ldg U=16 ctas/sm=%d", cps); time(nm, [&] { k_ldg<16><<<132 * cps, 256>>>((const float4*)x, nbytes / 16, out); });
   }
   for (int tile : {16384, 32768}) for (int cps : {1, 2}) {
     size_t smem = (size_t)3 * tile; cudaFuncSetAttribute(k_cpasync, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     char nm[96]; snprintf(nm, 96, "cp.async16 tile=%dKB S=3 ctas/sm=%d", tile / 1024, cps);
-    time(nm, [&] { k_cpasync<<<148 * cps, 256, smem>>>((const float4*)x, nbytes / 16, tile / 16, 3, out); });
+    time(nm, [&] { k_cpasync<<<132 * cps, 256, smem>>>((const float4*)x, nbytes / 16, tile / 16, 3, out); });
   }
   return 0;
 }

@@ -1,8 +1,7 @@
 #!/usr/bin/env python
 """WHICH=cholesky: times the factorisation + inverse of one 10k-wide system instead (ROWS=100000 keeps the data small).
-Times ONE CSR Gram build (1M x 10k x 1 %, the bench's partition 0) through mlease_time_kernel (MLEASE_GRAM_1CTA=1 selects the
-single-CTA variant).  Scratch tool for kernel work on a GPU box, not part of the product.  Round 2: 44.7 ms per build; 40.0 ms with producers
-that only hand stages over, i.e. the MMA stream itself (power-limited clocks) is 90 % of the time."""
+Times ONE CSR Gram build (1M x 10k x 1 %, the bench's partition 0) through mlease_time_kernel.  Scratch tool for kernel work on
+a GPU box, not part of the product."""
 import os, sys
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "ml-ease_b200"))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
