@@ -79,8 +79,11 @@ struct Problem {
   int csr_unique;          // every CSR row has strictly increasing column ids (parallel bf16 emit is exact)
   const long long* bm_offs;       // block-major entry list for the CSR Gram: run offsets [nblk128][bm_groups] (+1 total)
   const unsigned short* bm_keys;  // per entry: byte offset inside the swizzled [128 cols][32 rows] operand block
-  const float* bm_vals;           // per entry: the stored value
+  const float* bm_vals;           // per entry: the stored value (1 for the bias column, which the list holds explicitly)
   long long bm_groups;            // number of 32-row groups
+  long long bm_entries;           // entries of the list: nnz + n (one bias entry per row)
+  unsigned char* bm_e4m3;         // [bm_entries] this problem's Gram operand, e4m3(value * sqrt(d_row) * gram_scale), written by
+                                  // gram_csr_operand_kernel before every CSR Gram build (per problem: the list is shared, sdvec is not)
   float vmax, wmax;               // max |stored value| and max record weight of the partition (fixed-point scale of the CSR K1)
   int nblk128;             // number of 128-column blocks (Dp / 128)
   // fused multi-lambda CSR K1 (k1_csr_fused.cu): the partition's rows cut into sg_S segments of sg_rows rows; per segment the
@@ -173,6 +176,22 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) {
   }
+}
+// The same on a 32-bit shared-space address (see sts_u8): loops that hold barrier addresses in registers need no conversion.
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) { asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory"); }
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+  uint32_t ok;
+  do {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
+        "selp.u32 %0, 1, 0, p;\n"
+        "}\n"
+        : "=r"(ok)
+        : "r"(bar), "r"(parity)
+        : "memory");
+  } while (!ok);
 }
 
 // Byte store to a 32-bit shared-space address.  A pointer derived from the dynamic shared array by integer alignment loses its

@@ -143,16 +143,19 @@ gram_wgmma_kernel(const Problem* __restrict__ probs, const CUtensorMap* __restri
 // Sparse variant: the same split-K Gram, but the operand tiles are ASSEMBLED IN SHARED MEMORY, as e4m3, from the partition's
 // block-major entry list (no dense Xt in HBM: at 1 % density that copy is 100x the input and makes the dense kernel
 // HBM-bound).  One K-step = one 32-row group = one m64n128k32 wgmma per consumer warpgroup; its entries for a 128-column block
-// are one contiguous run of (key, value), the key being the byte offset of the element inside the K-major SWIZZLE_32B operand
-// block the wgmma descriptors expect (kmaj_off; wgmma takes 8-bit operands K-major only).  Producer warps, one per operand
-// block of a stage: load the run coalesced, scale by sqrt(d_row) * 2^e, round to e4m3, store one byte at the key.  Positions
-// outside the sparsity pattern are zero: the ring is cleared once, and a producer re-clears exactly the entries it wrote when
-// it gets its stage back.  Generic-proxy stores are published to the tensor core's async proxy with fence.proxy.async before
-// the mbarrier arrive.
+// are one contiguous run of (key, byte), the key being the byte offset of the element inside the K-major SWIZZLE_32B operand
+// block the wgmma descriptors expect (kmaj_off; wgmma takes 8-bit operands K-major only), the byte the finished e4m3 operand
+// element that gram_csr_operand_kernel wrote just before the build.  Producer warps, one per operand block of a stage: load
+// the run coalesced and store each byte at its key.  Positions outside the sparsity pattern are zero: the ring is cleared
+// once, and a producer re-clears exactly the entries it wrote when it gets its stage back.  Generic-proxy stores are
+// published to the tensor core's async proxy with fence.proxy.async before the mbarrier arrive.
 // A CTA owns a 128 x 128 lower tile, two consumer warpgroups of 64 rows.  The tensor core keeps the running sum of an fp8
 // product at less than fp32 precision, so a consumer runs chains of S_CHAIN wgmma (K = 128 rows) into one set of 64
 // registers and adds each finished chain into a second, fp32, set; setmaxnreg moves the registers this takes from the
 // producer warpgroups to the consumers.
+// The build is bound by instruction issue, not by the tensor pipe (one K-step is 128 tensor cycles of an SM for 8 consumer and
+// 2 producer warps): both loops are unrolled over the ring so that stage addresses, descriptors and barrier parities are
+// immediates or loop-carried registers, and the producers move ready-made bytes instead of scaling and rounding values.
 // Warp roles (16 warps): 0..7 = consumers, 8..15 = producers (4 groups of an A-block and a B-block warp).
 // ------------------------------------------------------------------------------------------
 constexpr int SK = 32;                       // data rows (K) per stage
@@ -166,6 +169,7 @@ constexpr int S_STAGE_BYTES = SPW * S_BOX_BYTES;
 constexpr int S_CONSUMER_WARPS = 8;
 constexpr int S_THREADS = (S_CONSUMER_WARPS + SPW * NGRP) * 32;   // 512: 128 registers a thread at launch
 constexpr int S_CHAIN = 4;                   // wgmma per fp32 promotion
+static_assert(SST == 2 * S_CHAIN, "the consumer loop runs two chains per pass over the ring");
 constexpr int S_REG_PRODUCER = 72, S_REG_CONSUMER = 184;          // 256 x 72 + 256 x 184 = 65536
 constexpr size_t S_SMEM = (size_t)SST * S_STAGE_BYTES + 1024 /*align*/ + 512 /*barriers*/;
 
@@ -179,7 +183,7 @@ __device__ __forceinline__ uint32_t kmaj_off(int k, int col) {
 __device__ __forceinline__ int kmaj_row(uint32_t key) { return (int)(((((key >> 4) ^ (key >> 7)) & 1) << 4) | (key & 15)); }
 
 __global__ void __launch_bounds__(S_THREADS, 1)
-gram_csr_wgmma_kernel(const Problem* __restrict__ probs, const GramTile* __restrict__ tiles, int ntiles, int force, int bias_col, int share) {
+gram_csr_wgmma_kernel(const Problem* __restrict__ probs, const GramTile* __restrict__ tiles, int ntiles, int force, int share) {
   if (share > 1 && blockIdx.z % share != 0) return;   // see gram_wgmma_kernel
   const Problem& pb = probs[blockIdx.z];
   Ctrl* ctrl = pb.ctrl;
@@ -187,8 +191,7 @@ gram_csr_wgmma_kernel(const Problem* __restrict__ probs, const GramTile* __restr
   const GramTile tile = tiles[blockIdx.x];
   const int slice = blockIdx.y, nslices = gridDim.y;
   const int Dp = pb.Dp;
-  const long long n = pb.n;
-  const long long ksteps_total = (n + SK - 1) / SK;
+  const long long ksteps_total = (pb.n + SK - 1) / SK;
   const long long per = (ksteps_total + nslices - 1) / nslices;
   const long long ks0 = slice * per;
   const long long ks1 = min(ksteps_total, ks0 + per);
@@ -198,6 +201,9 @@ gram_csr_wgmma_kernel(const Problem* __restrict__ probs, const GramTile* __restr
   unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(g_smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)SST * S_STAGE_BYTES);
   uint64_t* empty_bar = full_bar + SST;
+  // shared-space addresses: the ring, and the barriers of stage s at full_u32 + 8 s / empty_u32 + 8 s
+  const uint32_t smem_base = smem_u32(smem);
+  const uint32_t full_u32 = smem_base + (uint32_t)SST * S_STAGE_BYTES, empty_u32 = full_u32 + 8 * SST;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   // clear the whole ring once
@@ -217,41 +223,57 @@ gram_csr_wgmma_kernel(const Problem* __restrict__ probs, const GramTile* __restr
     float acc[SN / 2], chain[SN / 2];
 #pragma unroll
     for (int j = 0; j < SN / 2; j++) acc[j] = 0.f;
-    const uint32_t smem_base = smem_u32(smem);
-    // stage k: wait for its operands, issue its product into the chain registers (accumulate = 0 starts a chain)
-    auto issue = [&](int k, uint32_t accumulate) {
-      const int st = k % SST;
-      mbar_wait(&full_bar[st], (uint32_t)((k / SST) & 1));
-      const uint32_t a_addr = smem_base + (uint32_t)(st * S_STAGE_BYTES + wg * 64 * SK);
-      const uint32_t b_addr = smem_base + (uint32_t)(st * S_STAGE_BYTES + S_BOX_BYTES);
+    // Descriptors of stage 0 (K = 32 = the stage's 32-row group = one swizzle atom along K: LBO unused, SBO = 256 B between
+    // 8-column groups); stage st's differ by st * S_STAGE_BYTES / 16 in the start-address field, which cannot carry out of it
+    // (shared addresses are < 2^18).  Built once: left to itself the compiler re-derives every descriptor from the shared
+    // window base at every K-step.
+    const uint64_t desc_a0 = wgmma_desc(smem_base + (uint32_t)(wg * 64 * SK), 16, 256, DESC_SW32);
+    const uint64_t desc_b0 = wgmma_desc(smem_base + (uint32_t)S_BOX_BYTES, 16, 256, DESC_SW32);
+    const uint32_t desc_hi = (uint32_t)(desc_a0 >> 32);   // same SBO and layout for both operands
+    uint32_t a_lo = (uint32_t)desc_a0, b_lo = (uint32_t)desc_b0;
+    asm volatile("" : "+r"(a_lo), "+r"(b_lo));   // opaque: kept in registers, not recomputed
+    auto desc_a = [&](int st) { return ((uint64_t)desc_hi << 32) | (a_lo + (uint32_t)(st * S_STAGE_BYTES / 16)); };
+    auto desc_b = [&](int st) { return ((uint64_t)desc_hi << 32) | (b_lo + (uint32_t)(st * S_STAGE_BYTES / 16)); };
+    // stage st: wait for its operands (fill parity ph), issue its product into the chain registers (accumulate = 0 starts a chain)
+    auto issue = [&](int st, uint32_t ph, uint64_t a, uint64_t b, uint32_t accumulate) {
+      mbar_wait(full_u32 + 8 * st, ph);
       wgmma_fence();
-      // K = 32 = the stage's 32-row group = one swizzle atom along K: LBO unused, SBO = 256 B between 8-column groups
-      wgmma_e4m3_m64n128k32(chain, wgmma_desc(a_addr, 16, 256, DESC_SW32), wgmma_desc(b_addr, 16, 256, DESC_SW32), accumulate);
+      wgmma_e4m3_m64n128k32(chain, a, b, accumulate);
       wgmma_commit();
     };
-    // stage k's product has retired: hand its buffer back to the producers
-    auto release = [&](int k) { if (lane == 0) mbar_arrive(&empty_bar[k % SST]); };
+    // stage st's product has retired: hand its buffer back to the producers
+    auto release = [&](int st) { if (lane == 0) mbar_arrive(empty_u32 + 8 * st); };
     auto promote = [&]() {
 #pragma unroll
       for (int j = 0; j < SN / 2; j++) acc[j] += chain[j];
     };
-    // whole chains are straight-line code: a data-dependent branch between a wgmma and the next makes the compiler wait for
-    // every product in flight at the join
-    const int nfull = nk - nk % S_CHAIN;
-    for (int k0 = 0; k0 < nfull; k0 += S_CHAIN) {
+    // one whole chain in the stages s0 .. s0 + S_CHAIN - 1.  Straight-line code: a data-dependent branch between a wgmma and the
+    // next makes the compiler wait for every product in flight at the join
+    auto run_chain = [&](int s0, uint32_t ph) {
 #pragma unroll
       for (int c = 0; c < S_CHAIN; c++) {
-        issue(k0 + c, c != 0 ? 1u : 0u);
-        if (c > 0) { wgmma_wait<1>(); release(k0 + c - 1); }
+        issue(s0 + c, ph, desc_a(s0 + c), desc_b(s0 + c), c != 0 ? 1u : 0u);
+        if (c > 0) { wgmma_wait<1>(); release(s0 + c - 1); }
       }
       wgmma_wait<0>();
-      release(k0 + S_CHAIN - 1);
+      release(s0 + S_CHAIN - 1);
       promote();
+    };
+    // K-step k lives in stage k % SST and is that stage's fill k / SST: a pass over the ring is two chains at one parity
+    const int nring = nk - nk % SST, nfull = nk - nk % S_CHAIN;
+    uint32_t ph = 0;
+    int k = 0;
+    for (; k < nring; k += SST) {
+      run_chain(0, ph);
+      run_chain(S_CHAIN, ph);
+      ph ^= 1u;
     }
-    for (int k = nfull; k < nk; k++) {   // the last nk % S_CHAIN stages, a chain each
-      issue(k, 0u);
+    if (k < nfull) { run_chain(0, ph); k += S_CHAIN; }   // a last whole chain in stages 0 .. S_CHAIN - 1
+    for (; k < nk; k++) {   // the last nk % S_CHAIN stages, a chain each
+      const int st = k % SST;
+      issue(st, (uint32_t)(k / SST) & 1u, desc_a(st), desc_b(st), 0u);
       wgmma_wait<0>();
-      release(k);
+      release(st);
       promote();
     }
     store_acc<SN>(pb.Hpart + (size_t)slice * Dp * Dp, Dp, tile.bi * 128 + wg * 64, tile.bj * SN, acc);
@@ -260,103 +282,115 @@ gram_csr_wgmma_kernel(const Problem* __restrict__ probs, const GramTile* __restr
     // One K-step = one 32-row group, whose entries for a 128-column block are one contiguous run of the block-major list.
     // Offsets are fetched three uses ahead and the first 64 entries of a run two uses ahead, so the loads of a use are in flight
     // during the whole previous uses.  Group t owns the K-steps k = t, t + NGRP, ...; K-step k lives in ring stage k % SST, so a
-    // group alternates between the stages t and t + NGRP.
+    // group alternates between the stages t (stage 0 of the group) and t + NGRP (stage 1), and the loop handles one of each per
+    // pass: each stage keeps its own registers, and the run loaded after a hand-over is the stage's next one.
     setmaxnreg_dec<S_REG_PRODUCER>();
     const int pw = warp - S_CONSUMER_WARPS;
     const int grp = pw / SPW, strm = pw % SPW;
-    const size_t strm_off = (size_t)strm * S_BOX_BYTES;
     const int blk = strm == 0 ? tile.bi : tile.bj;
     const bool valid = blk < pb.nblk128;
-    const long long ngroups = pb.bm_groups;
-    const long long* __restrict__ my_offs = pb.bm_offs + (size_t)(valid ? blk : 0) * ngroups + (lane & 1);
+    const long long* __restrict__ my_offs = pb.bm_offs + (size_t)(valid ? blk : 0) * pb.bm_groups + ks0 + (lane & 1);
     const unsigned short* __restrict__ keys = pb.bm_keys;
-    const float* __restrict__ bvals = pb.bm_vals;
-    const float* __restrict__ sdv = pb.sdvec;
-    // the bias column (value 1 in every row, llf/LibLinearDataset.java:592-614) is not stored in the CSR rows
-    const bool has_bias_col = valid && bias_col >= blk * 128 && bias_col < blk * 128 + 128;
-    const uint32_t bias_off = has_bias_col ? kmaj_off(lane, bias_col - blk * 128) : 0u;
+    const unsigned char* __restrict__ bytes = pb.bm_e4m3;
     constexpr uint32_t NOKEY = 0xFFFFFFFFu;
     const bool fetch = valid && lane < 2;
+    // the list holds < 2^32 entries (checked at upload): entry numbers are 32-bit
+    auto ld_offs = [&](int k) -> uint32_t { return (fetch && k < nk) ? (uint32_t)__ldg(my_offs + k) : 0u; };
 
-    // Pipeline registers: offsets three uses ahead (o_c), entries + sqrt(d) two uses ahead (set 2), one use ahead (set 1),
-    // current (set 0); what the last TWO uses stored (p1 = previous use = the other stage, p2 = the use before = this stage).
-    auto ld_offs = [&](int k) -> uint32_t { return (fetch && k < nk) ? (uint32_t)__ldg(my_offs + ks0 + k) : 0u; };   // the list holds < 2^32 entries (checked at upload)
-    uint32_t lo0, hi0, lo1, hi1, lo2, hi2, p1lo = 0, p1hi = 0, p2lo = 0, p2hi = 0;
-    uint32_t key0[2], key1[2], key2[2], p1key[2] = {NOKEY, NOKEY}, p2key[2] = {NOKEY, NOKEY};
-    float val0[2], val1[2], val2[2], sd0, sd1, sd2;
-    auto ld_entries = [&](uint32_t lo, uint32_t hi, uint32_t* key, float* val) {
+    struct Run { uint32_t lo, hi, key[2], byte[2]; };   // a use's run [lo, hi) and its first 64 entries (lane, lane + 32)
+    struct Written { uint32_t lo, hi, key[2]; };        // the run a stage holds, to be cleared before its next fill
+    auto take_offs = [&](Run& r, uint32_t o) { r.lo = __shfl_sync(0xffffffffu, o, 0); r.hi = __shfl_sync(0xffffffffu, o, 1); };
+    auto ld_entries = [&](Run& r) {
 #pragma unroll
       for (int q = 0; q < 2; q++) {
-        const uint32_t e = lo + lane + 32 * q;
-        key[q] = e < hi ? (uint32_t)__ldg(keys + e) : NOKEY;
-        val[q] = e < hi ? __ldg(bvals + e) : 0.f;
+        const uint32_t e = r.lo + lane + 32 * q;
+        r.key[q] = e < r.hi ? (uint32_t)__ldg(keys + e) : NOKEY;
+        r.byte[q] = e < r.hi ? (uint32_t)__ldg(bytes + e) : 0u;
       }
     };
-    const float gscale = pb.gram_scale;   // power of two: keeps sqrt(d) x in e4m3's normal range; undone exactly by chol_prep
-    auto ld_sd = [&](int k) -> float {
-      const long long r = (ks0 + k) * SK + lane;
-      return (k < nk && r < n) ? sdv[r] * gscale : 0.f;   // sdvec is rewritten by K1 between builds: a plain load
-    };
-    auto to_e4m3 = [](float x) -> uint32_t { return (uint32_t)__nv_cvt_float_to_fp8(x, __NV_SATFINITE, __NV_E4M3); };
-    const uint32_t smem_base_u32 = smem_u32(smem);
-    {
-      const uint32_t oa = ld_offs(grp), ob = ld_offs(grp + NGRP);
-      lo0 = __shfl_sync(0xffffffffu, oa, 0); hi0 = __shfl_sync(0xffffffffu, oa, 1);
-      lo1 = __shfl_sync(0xffffffffu, ob, 0); hi1 = __shfl_sync(0xffffffffu, ob, 1);
-    }
+    Run r0, r1;
+    Written w0 = {0u, 0u, {NOKEY, NOKEY}}, w1 = {0u, 0u, {NOKEY, NOKEY}};
+    take_offs(r0, ld_offs(grp));
+    take_offs(r1, ld_offs(grp + NGRP));
     uint32_t o_c = ld_offs(grp + 2 * NGRP);
-    ld_entries(lo0, hi0, key0, val0); sd0 = ld_sd(grp);
-    ld_entries(lo1, hi1, key1, val1); sd1 = ld_sd(grp + NGRP);
-    bool p1row = false, p2row = false;
-    for (int k = grp, use = 0; k < nk; k += NGRP, use++) {
-      const int st = k % SST;
-      const uint32_t sbase = smem_base_u32 + (uint32_t)st * (uint32_t)S_STAGE_BYTES + (uint32_t)strm_off;   // shared-space address
-      // ---- un-write what the previous use of THIS STAGE (two uses ago) stored (same addresses, zero)
-      const int fill = k / SST;   // how many times this stage has been filled before
-      if (fill > 0) {
-        mbar_wait(&empty_bar[st], (uint32_t)((fill - 1) & 1));
+    ld_entries(r0);
+    ld_entries(r1);
+    const uint32_t sbase0 = smem_base + (uint32_t)(grp * S_STAGE_BYTES + strm * S_BOX_BYTES), sbase1 = sbase0 + NGRP * S_STAGE_BYTES;
+    const uint32_t full0 = full_u32 + 8 * grp, empty0 = empty_u32 + 8 * grp;
+    // one use: K-step k in the stage at sbase (barriers full / empty), r = its run, w = what the stage's previous fill stored
+    auto use = [&](int k, uint32_t sbase, uint32_t full, uint32_t empty, bool refill, uint32_t ph, Run& r, Written& w) {
+      // ---- un-write what the previous fill of this stage stored (same addresses, zero)
+      if (refill) {
+        mbar_wait(empty, ph);
 #pragma unroll
         for (int q = 0; q < 2; q++)
-          if (p2key[q] != NOKEY) sts_u8(sbase + p2key[q], 0u);
-        for (uint32_t e0 = p2lo + 64; e0 < p2hi; e0 += 32) {
+          if (w.key[q] != NOKEY) sts_u8(sbase + w.key[q], 0u);
+        for (uint32_t e0 = w.lo + 64; e0 < w.hi; e0 += 32) {
           const uint32_t e = e0 + lane;
-          if (e < p2hi) sts_u8(sbase + (uint32_t)__ldg(keys + e), 0u);
+          if (e < w.hi) sts_u8(sbase + (uint32_t)__ldg(keys + e), 0u);
         }
-        if (p2row && has_bias_col) sts_u8(sbase + bias_off, 0u);
       }
       // ---- write this use
 #pragma unroll
-      for (int q = 0; q < 2; q++) {
-        const bool v = key0[q] != NOKEY;
-        const uint32_t key = v ? key0[q] : 0u;
-        const float sdk = __shfl_sync(0xffffffffu, sd0, kmaj_row(key));
-        if (v) sts_u8(sbase + key, to_e4m3(val0[q] * sdk));
-      }
-      for (uint32_t e0 = lo0 + 64; e0 < hi0; e0 += 32) {
+      for (int q = 0; q < 2; q++)
+        if (r.key[q] != NOKEY) sts_u8(sbase + r.key[q], r.byte[q]);
+      for (uint32_t e0 = r.lo + 64; e0 < r.hi; e0 += 32) {
         const uint32_t e = e0 + lane;
-        const bool v = e < hi0;
-        const uint32_t key = v ? (uint32_t)__ldg(keys + e) : 0u;
-        const float val = v ? __ldg(bvals + e) : 0.f;
-        const float sdk = __shfl_sync(0xffffffffu, sd0, kmaj_row(key));
-        if (v) sts_u8(sbase + key, to_e4m3(val * sdk));
+        if (e < r.hi) sts_u8(sbase + (uint32_t)__ldg(keys + e), (uint32_t)__ldg(bytes + e));
       }
-      const bool row_now = (ks0 + k) * SK + lane < n;
-      if (row_now && has_bias_col) sts_u8(sbase + bias_off, to_e4m3(sd0));
       fence_proxy_async_smem();
       __syncwarp();
-      if (lane == 0) mbar_arrive(&full_bar[st]);
-      // ---- issue the loads of the use after next.  AFTER the hand-over, not before this use's stores: the fence above compiles to
-      // a memory barrier that waits for every load this thread still has in flight -- issued at the top of the use they would
-      // make each hand-over wait out a DRAM round trip; issued here they have the whole next use to arrive.
-      lo2 = __shfl_sync(0xffffffffu, o_c, 0); hi2 = __shfl_sync(0xffffffffu, o_c, 1);
+      if (lane == 0) mbar_arrive(full);
+      w.lo = r.lo; w.hi = r.hi; w.key[0] = r.key[0]; w.key[1] = r.key[1];
+      // ---- issue the loads of this stage's next use (K-step k + SST).  AFTER the hand-over, not before this use's stores: the
+      // fence above compiles to a memory barrier that waits for every load this thread still has in flight -- issued at the top
+      // of the use they would make each hand-over wait out a DRAM round trip; issued here they have the whole next use to arrive.
+      take_offs(r, o_c);
       o_c = ld_offs(k + 3 * NGRP);
-      ld_entries(lo2, hi2, key2, val2); sd2 = ld_sd(k + 2 * NGRP);
-      // ---- rotate
-      p2lo = p1lo; p2hi = p1hi; p2row = p1row; p1lo = lo0; p1hi = hi0; p1row = row_now;
-      lo0 = lo1; hi0 = hi1; lo1 = lo2; hi1 = hi2;
-#pragma unroll
-      for (int q = 0; q < 2; q++) { p2key[q] = p1key[q]; p1key[q] = key0[q]; key0[q] = key1[q]; val0[q] = val1[q]; key1[q] = key2[q]; val1[q] = val2[q]; }
-      sd0 = sd1; sd1 = sd2;
+      ld_entries(r);
+    };
+    // fill f >= 1 of a stage waits for the consumers' release of fill f - 1: empty-barrier phase parity (f - 1) & 1
+    uint32_t ph = 1u;
+    for (int k = grp; k < nk; k += SST) {
+      use(k, sbase0, full0, empty0, k >= SST, ph, r0, w0);
+      if (k + NGRP >= nk) break;
+      use(k + NGRP, sbase1, full0 + 8 * NGRP, empty0 + 8 * NGRP, k >= SST, ph, r1, w1);
+      ph ^= 1u;
+    }
+  }
+}
+
+// Gram operand of the CSR kernel, once per build: for every entry of the block-major list, the e4m3 byte
+// e4m3(value * (sqrt(d_row) * gram_scale)).  gram_scale is a power of two that keeps sqrt(d) x in e4m3's normal range (chol_prep
+// undoes it exactly).  sdvec is rewritten by K1 between builds, so this runs immediately before each build, gated like it.
+// One warp per 32-row group: lane l holds sqrt(d) of row 32 g + l, and the group's runs of every column block follow.
+__global__ void __launch_bounds__(256) gram_csr_operand_kernel(const Problem* __restrict__ probs, int force, int share) {
+  if (share > 1 && blockIdx.y % share != 0) return;   // see gram_wgmma_kernel
+  const Problem& pb = probs[blockIdx.y];
+  const Ctrl* ctrl = pb.ctrl;
+  if (!force && (ctrl->done || !ctrl->need_hess)) return;
+  const int lane = threadIdx.x & 31;
+  const long long n = pb.n, ngroups = pb.bm_groups;
+  const int nblk = pb.nblk128;
+  const long long* __restrict__ offs = pb.bm_offs;
+  const unsigned short* __restrict__ keys = pb.bm_keys;
+  const float* __restrict__ vals = pb.bm_vals;
+  unsigned char* __restrict__ out = pb.bm_e4m3;
+  const float gscale = pb.gram_scale;
+  const long long nw = ((long long)gridDim.x * blockDim.x) >> 5;
+  for (long long g = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; g < ngroups; g += nw) {
+    const long long r = g * SK + lane;
+    const float sd = r < n ? pb.sdvec[r] * gscale : 0.f;
+    for (int b = 0; b < nblk; b++) {
+      const uint32_t lo = (uint32_t)offs[(size_t)b * ngroups + g], hi = (uint32_t)offs[(size_t)b * ngroups + g + 1];
+      for (uint32_t e0 = lo; e0 < hi; e0 += 32) {
+        const uint32_t e = e0 + lane;
+        const bool v = e < hi;
+        const uint32_t key = v ? (uint32_t)keys[e] : 0u;
+        const float val = v ? vals[e] : 0.f;
+        const float sdk = __shfl_sync(0xffffffffu, sd, kmaj_row(key));
+        if (v) out[e] = (unsigned char)__nv_cvt_float_to_fp8(val * sdk, __NV_SATFINITE, __NV_E4M3);
+      }
     }
   }
 }
@@ -364,9 +398,15 @@ gram_csr_wgmma_kernel(const Problem* __restrict__ probs, const GramTile* __restr
 // Block-major entry list for the CSR Gram.  For every 128-column block b and every 32-row group g the entries
 // (row in group, column in block, value) are stored contiguously at [offs[b*ngroups+g], offs[b*ngroups+g+1]); the key is
 // the byte offset of the element inside a swizzled [128 col][32 k] operand block (kmaj_off), the value the stored float.
+// Every row also gets an entry of value 1 for the bias column bias_col (llf/LibLinearDataset.java:592-614), which the CSR
+// rows do not store; bias_col is larger than every stored column, so it is the row's last entry in its block.
 // Rows must be sorted by column (strictly increasing), which the upload checks.
+__device__ __forceinline__ bool bias_in_block(long long r, long long n, int bias_col, int b) {
+  return r < n && bias_col >= b * 128 && bias_col < b * 128 + 128;
+}
+
 __global__ void __launch_bounds__(256) csr_bm_count_kernel(long long n, const long long* __restrict__ rowptr, const int* __restrict__ colidx,
-                                                           int nblk, long long ngroups, long long* __restrict__ counts) {
+                                                           int bias_col, int nblk, long long ngroups, long long* __restrict__ counts) {
   const int lane = threadIdx.x & 31;
   const long long nw = ((long long)gridDim.x * blockDim.x) >> 5;
   for (long long g = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; g < ngroups; g += nw) {
@@ -376,7 +416,7 @@ __global__ void __launch_bounds__(256) csr_bm_count_kernel(long long n, const lo
     for (int b = 0; b < nblk; b++) {
       const long long s = j;
       while (j < j1 && colidx[j] < (b + 1) * 128) j++;
-      int c = (int)(j - s);
+      int c = (int)(j - s) + (bias_in_block(r, n, bias_col, b) ? 1 : 0);
       c = __reduce_add_sync(0xffffffffu, c);
       if (lane == 0) counts[(size_t)b * ngroups + g] = c;
     }
@@ -384,7 +424,7 @@ __global__ void __launch_bounds__(256) csr_bm_count_kernel(long long n, const lo
 }
 
 __global__ void __launch_bounds__(256) csr_bm_fill_kernel(long long n, const long long* __restrict__ rowptr, const int* __restrict__ colidx,
-                                                          const float* __restrict__ vals, int nblk, long long ngroups,
+                                                          const float* __restrict__ vals, int bias_col, int nblk, long long ngroups,
                                                           const long long* __restrict__ offs, unsigned short* __restrict__ keys,
                                                           float* __restrict__ bvals) {
   const int lane = threadIdx.x & 31;
@@ -396,7 +436,8 @@ __global__ void __launch_bounds__(256) csr_bm_fill_kernel(long long n, const lon
     for (int b = 0; b < nblk; b++) {
       const long long s = j;
       while (j < j1 && colidx[j] < (b + 1) * 128) j++;
-      const int c = (int)(j - s);
+      const bool bias = bias_in_block(r, n, bias_col, b);
+      const int c = (int)(j - s) + (bias ? 1 : 0);
       int incl = c;   // inclusive warp scan
 #pragma unroll
       for (int d = 1; d < 32; d <<= 1) {
@@ -407,6 +448,10 @@ __global__ void __launch_bounds__(256) csr_bm_fill_kernel(long long n, const lon
       for (long long e = s; e < j; e++, pos++) {
         keys[pos] = (unsigned short)kmaj_off(lane, colidx[e] - b * 128);
         bvals[pos] = vals[e];
+      }
+      if (bias) {
+        keys[pos] = (unsigned short)kmaj_off(lane, bias_col - b * 128);
+        bvals[pos] = 1.f;
       }
     }
   }
@@ -522,26 +567,29 @@ cudaError_t gram_launch_wgmma(const Problem* d_probs, int nprob, const void* d_t
   return cudaGetLastError();
 }
 
-// d_tiles holds the 128 x 128 tiles of gram_tile_list(..., 1)
+// One CSR Gram build: the operand pass, then the Gram, on the same stream and gated the same way.  d_tiles holds the
+// 128 x 128 tiles of gram_tile_list(..., 1)
 cudaError_t gram_launch_csr_wgmma(const Problem* d_probs, int nprob, const void* d_tiles, int ntiles, int nslices, int force,
-                                  int bias_col, cudaStream_t st, int* launches, int share) {
+                                  cudaStream_t st, int* launches, int share) {
   static bool configured[64] = {};
   cudaError_t e = set_smem_once(gram_csr_wgmma_kernel, S_SMEM, configured);
   if (e != cudaSuccess) return e;
+  gram_csr_operand_kernel<<<dim3(1024, nprob), 256, 0, st>>>(d_probs, force, share);   // ~8 warps an SM per problem
+  if ((e = cudaGetLastError()) != cudaSuccess) return e;
   gram_csr_wgmma_kernel<<<dim3(ntiles, nslices, nprob), S_THREADS, S_SMEM, st>>>(
-      d_probs, reinterpret_cast<const GramTile*>(d_tiles), ntiles, force, bias_col, share);
-  if (launches) *launches += 1;
+      d_probs, reinterpret_cast<const GramTile*>(d_tiles), ntiles, force, share);
+  if (launches) *launches += 2;
   return cudaGetLastError();
 }
 
 // counts -> exclusive offsets in place: offs has nblk*ngroups+1 entries (the last one = total entries)
-cudaError_t csr_bm_offsets(long long n, const long long* rowptr, const int* colidx, int nblk, long long ngroups, long long* offs,
-                           cudaStream_t st) {
+cudaError_t csr_bm_offsets(long long n, const long long* rowptr, const int* colidx, int bias_col, int nblk, long long ngroups,
+                           long long* offs, cudaStream_t st) {
   const long long m = (long long)nblk * ngroups;
   cudaError_t e = cudaMemsetAsync(offs, 0, (size_t)(m + 1) * sizeof(long long), st);
   if (e != cudaSuccess) return e;
   const int grid = (int)std::min<long long>((ngroups + 7) / 8, 132 * 32);
-  csr_bm_count_kernel<<<std::max(grid, 1), 256, 0, st>>>(n, rowptr, colidx, nblk, ngroups, offs);
+  csr_bm_count_kernel<<<std::max(grid, 1), 256, 0, st>>>(n, rowptr, colidx, bias_col, nblk, ngroups, offs);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
   size_t tmp_bytes = 0;
   if ((e = cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, offs, offs, (long long)(m + 1), st)) != cudaSuccess) return e;
@@ -552,10 +600,10 @@ cudaError_t csr_bm_offsets(long long n, const long long* rowptr, const int* coli
   return e != cudaSuccess ? e : e2;
 }
 
-cudaError_t csr_bm_fill(long long n, const long long* rowptr, const int* colidx, const float* vals, int nblk, long long ngroups,
-                        const long long* offs, unsigned short* keys, float* bvals, cudaStream_t st) {
+cudaError_t csr_bm_fill(long long n, const long long* rowptr, const int* colidx, const float* vals, int bias_col, int nblk,
+                        long long ngroups, const long long* offs, unsigned short* keys, float* bvals, cudaStream_t st) {
   const int grid = (int)std::min<long long>((ngroups + 7) / 8, 132 * 32);
-  csr_bm_fill_kernel<<<std::max(grid, 1), 256, 0, st>>>(n, rowptr, colidx, vals, nblk, ngroups, offs, keys, bvals);
+  csr_bm_fill_kernel<<<std::max(grid, 1), 256, 0, st>>>(n, rowptr, colidx, vals, bias_col, nblk, ngroups, offs, keys, bvals);
   return cudaGetLastError();
 }
 

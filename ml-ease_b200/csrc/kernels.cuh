@@ -29,9 +29,10 @@ int gram_tile_list(int Dp, short* bi_bj_pairs, int max_tiles, int csr_tiles = 0)
 cudaError_t gram_launch_wgmma(const Problem* d_probs, int nprob, const void* d_tmaps, const void* d_tiles, int ntiles,
                               int nslices, int force, cudaStream_t st, int* launches, int share = 0);
 cudaError_t gram_launch_csr_wgmma(const Problem* d_probs, int nprob, const void* d_tiles, int ntiles, int nslices, int force,
-                                  int bias_col, cudaStream_t st, int* launches, int share = 0);
-cudaError_t csr_bm_offsets(long long n, const long long* rowptr, const int* colidx, int nblk, long long ngroups, long long* offs, cudaStream_t st);
-cudaError_t csr_bm_fill(long long n, const long long* rowptr, const int* colidx, const float* vals, int nblk, long long ngroups,
+                                  cudaStream_t st, int* launches, int share = 0);
+cudaError_t csr_bm_offsets(long long n, const long long* rowptr, const int* colidx, int bias_col, int nblk, long long ngroups, long long* offs,
+                           cudaStream_t st);
+cudaError_t csr_bm_fill(long long n, const long long* rowptr, const int* colidx, const float* vals, int bias_col, int nblk, long long ngroups,
                         const long long* offs, unsigned short* keys, float* bvals, cudaStream_t st);
 cudaError_t gram_launch_simt(const Problem* d_probs, int nprob, int Dp, int force, cudaStream_t st, int* launches);
 

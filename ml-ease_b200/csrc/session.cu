@@ -130,6 +130,7 @@ struct PartData {
   unsigned short* bm_keys = nullptr;
   float* bm_vals = nullptr;
   long long bm_groups = 0;
+  long long bm_entries = 0;        // nnz + n: the list holds the bias column explicitly
   int nblk128 = 0;
   // segment lists of the fused multi-lambda CSR K1 (k1_csr_fused.cu), built at upload for rows with unique sorted columns
   int sg_S = 0, sg_rows = 0, sg_ngrp = 0;
@@ -322,7 +323,9 @@ int batch_alloc(Batch& B, int num_sms) {
   for (int b = 0; b < nprob; b++) {
     pool_off[b] = pool_bytes;
     const bool windows = B.gram_from_csr && k1_csr_window(ldx) > 0;   // then a second [n] vector (row residuals) follows sdvec
-    const size_t need = B.gram_from_csr ? (size_t)B.h[b].n * sizeof(float) * (windows ? 2 : 1) : (B.h[b].Xt ? 0 : (size_t)B.h[b].n * B.Dp * sizeof(__nv_bfloat16));
+    // CSR: sdvec (+ rvec), then the e4m3 operand bytes of the entry list
+    const size_t need = B.gram_from_csr ? (((size_t)B.h[b].n * sizeof(float) * (windows ? 2 : 1) + 255) & ~(size_t)255) + (size_t)B.h[b].bm_entries
+                                        : (B.h[b].Xt ? 0 : (size_t)B.h[b].n * B.Dp * sizeof(__nv_bfloat16));
     pool_bytes += (need + 255) & ~(size_t)255;
   }
   unsigned char* pool = nullptr;
@@ -357,6 +360,7 @@ int batch_alloc(Batch& B, int num_sms) {
     if (B.gram_from_csr) {
       p.sdvec = reinterpret_cast<float*>(pool + pool_off[b]);
       p.rvec = k1_csr_window(ldx) > 0 ? p.sdvec + p.n : nullptr;
+      p.bm_e4m3 = pool + pool_off[b] + (((size_t)p.n * sizeof(float) * (p.rvec ? 2 : 1) + 255) & ~(size_t)255);
       p.gram_from_csr = 1;
       std::memset(&maps[b], 0, sizeof(CUtensorMap));
     } else {
@@ -414,7 +418,7 @@ int batch_xupdate(Batch& B, cudaStream_t st, double xtol, int max_newton, int po
       const int share = (slot_idx == 0) ? share_first_gram : 0;
       if (share > 1)
         for (int b = 0; b < B.nprob; b++) if (b % share != 0) shared_flops += (double)B.h[b].n * (double)B.Dt * (double)(B.Dt + 1);
-      if (B.gram_from_csr) CK(gram_launch_csr_wgmma(d_hess, n_hess, B.d_tiles, B.ntiles, B.gram_slices, 0, B.has_bias ? B.Dt - 1 : -1, st, &launches, share));
+      if (B.gram_from_csr) CK(gram_launch_csr_wgmma(d_hess, n_hess, B.d_tiles, B.ntiles, B.gram_slices, 0, st, &launches, share));
       else CK(gram_launch_wgmma(d_hess, n_hess, B.d_tmaps, B.d_tiles, B.ntiles, B.gram_slices, 0, st, &launches, share));
       pf.end(st);
       pf.begin(3, st);
@@ -623,7 +627,7 @@ void fill_problem_data(Problem& p, const PartData& pd) {
   std::memset(&p, 0, sizeof(Problem));
   p.X = pd.X; p.n = pd.n; p.y = pd.y; p.w = pd.w; p.o = pd.o;
   p.rowptr = pd.rowptr; p.colidx = pd.colidx; p.vals = pd.vals; p.nnz_hint = pd.nnz; p.csr_unique = pd.csr_unique;
-  p.bm_offs = pd.bm_offs; p.bm_keys = pd.bm_keys; p.bm_vals = pd.bm_vals; p.bm_groups = pd.bm_groups;
+  p.bm_offs = pd.bm_offs; p.bm_keys = pd.bm_keys; p.bm_vals = pd.bm_vals; p.bm_groups = pd.bm_groups; p.bm_entries = pd.bm_entries;
   p.nblk128 = pd.nblk128; p.gram_from_csr = pd.bm_offs ? 1 : 0;
   p.vmax = pd.vmax; p.wmax = pd.wmax;
   p.sg_S = pd.sg_S; p.sg_rows = pd.sg_rows; p.sg_ngrp = pd.sg_ngrp; p.sg_perm = pd.sg_perm; p.sg_depth = pd.sg_depth; p.sg_goff = pd.sg_goff;
@@ -937,15 +941,18 @@ static int csr_build_layout(mlease_session* s, PartData& pd) {
   CK(cudaStreamSynchronize(s->stream));
   std::memcpy(&pd.vmax, s->h_flag, 4);
   pd.csr_unique = s->h_flag[1] ? 0 : 1;
-  if (pd.csr_unique && pd.nnz < (1LL << 32) - 64) {   // the Gram producers index the entry list with 32 bits
+  // the Gram producers index the entry list with 32 bits; the list holds one bias entry per row (session batches always have the
+  // intercept, column Dg)
+  if (pd.csr_unique && pd.nnz + nrows < (1LL << 32) - 64) {
     pd.nblk128 = round_up(s->ldx, 128) / 128;
     pd.bm_groups = (nrows + 31) / 32;
+    pd.bm_entries = pd.nnz + nrows;
     void *bo, *bk, *bv;
     if (int rc = sess_alloc(s, &bo, ((size_t)pd.nblk128 * pd.bm_groups + 1) * sizeof(long long))) return rc;
-    if (int rc = sess_alloc(s, &bk, (size_t)pd.nnz * sizeof(unsigned short))) return rc;
-    if (int rc = sess_alloc(s, &bv, (size_t)pd.nnz * sizeof(float))) return rc;
-    CK(csr_bm_offsets(nrows, pd.rowptr, pd.colidx, pd.nblk128, pd.bm_groups, (long long*)bo, s->stream));
-    CK(csr_bm_fill(nrows, pd.rowptr, pd.colidx, pd.vals, pd.nblk128, pd.bm_groups, (const long long*)bo, (unsigned short*)bk, (float*)bv, s->stream));
+    if (int rc = sess_alloc(s, &bk, (size_t)pd.bm_entries * sizeof(unsigned short))) return rc;
+    if (int rc = sess_alloc(s, &bv, (size_t)pd.bm_entries * sizeof(float))) return rc;
+    CK(csr_bm_offsets(nrows, pd.rowptr, pd.colidx, s->Dg, pd.nblk128, pd.bm_groups, (long long*)bo, s->stream));
+    CK(csr_bm_fill(nrows, pd.rowptr, pd.colidx, pd.vals, s->Dg, pd.nblk128, pd.bm_groups, (const long long*)bo, (unsigned short*)bk, (float*)bv, s->stream));
     pd.bm_offs = (long long*)bo; pd.bm_keys = (unsigned short*)bk; pd.bm_vals = (float*)bv;
     // segment lists of the fused multi-lambda K1
     int S = 0, rows = 0, LP = 0; size_t smem = 0;
@@ -1282,7 +1289,7 @@ int mlease_objective(mlease_session* s, int32_t pid, const double* w, const doub
   if (f) *f = c.f_t;
   if (H) {
     if (!tensor && B->gram_from_csr) return fail(MLEASE_ERR_INVALID, "the SIMT debug Gram needs the dense bf16 operand, which CSR partitions with sorted unique rows do not materialise");
-    if (tensor && B->gram_from_csr) CK(gram_launch_csr_wgmma(B->d, 1, B->d_tiles, B->ntiles, B->gram_slices, 1, B->has_bias ? B->Dt - 1 : -1, s->stream, &launches, 0));
+    if (tensor && B->gram_from_csr) CK(gram_launch_csr_wgmma(B->d, 1, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches, 0));
     else if (tensor) CK(gram_launch_wgmma(B->d, 1, B->d_tmaps, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches));
     else CK(gram_launch_simt(B->d, 1, B->Dp, 1, s->stream, &launches));
     if (tensor == 2) {
@@ -1402,9 +1409,8 @@ int mlease_time_kernel(mlease_session* s, int32_t pid, int32_t which, int32_t re
   CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1));
   // warm-up launch (also produces the scaled copy the Gram needs)
   CK(batch_k1(*B, 1, s->stream, &launches));
-  const int bias_col = B->has_bias ? B->Dt - 1 : -1;
   if (which == 3) {
-    if (B->gram_from_csr) CK(gram_launch_csr_wgmma(B->d, 1, B->d_tiles, B->ntiles, B->gram_slices, 1, bias_col, s->stream, &launches, 0));
+    if (B->gram_from_csr) CK(gram_launch_csr_wgmma(B->d, 1, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches, 0));
     else CK(gram_launch_wgmma(B->d, 1, B->d_tmaps, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches));
     Ctrl c; std::memset(&c, 0, sizeof(c)); c.need_hess = 1;
     CK(cudaMemcpyAsync(B->d_ctrl, &c, sizeof(Ctrl), cudaMemcpyHostToDevice, s->stream));
@@ -1413,7 +1419,7 @@ int mlease_time_kernel(mlease_session* s, int32_t pid, int32_t which, int32_t re
   CK(cudaEventRecord(e0, s->stream));
   for (int r = 0; r < reps; r++) {
     if (which == 1) CK(batch_k1(*B, emit_scaled ? 1 : 0, s->stream, &launches));
-    else if (which == 2 && B->gram_from_csr) CK(gram_launch_csr_wgmma(B->d, 1, B->d_tiles, B->ntiles, B->gram_slices, 1, bias_col, s->stream, &launches, 0));
+    else if (which == 2 && B->gram_from_csr) CK(gram_launch_csr_wgmma(B->d, 1, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches, 0));
     else if (which == 2) CK(gram_launch_wgmma(B->d, 1, B->d_tmaps, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches));
     else if (which == 3) CK(cholesky_launch(B->d, 1, B->ldh, s->stream, &launches));
     else return fail(MLEASE_ERR_INVALID, "which must be 1, 2 or 3");
