@@ -2,10 +2,16 @@
 seeded inputs.  Tolerances: objective/gradient 1e-5 relative (fp32 data path, fp64 reductions); Gram (bf16
 tensor-core operands) 2e-2 vs the fp64 Hessian and 1e-3 vs the fp32 SIMT kernel on the same bf16 operand;
 coefficients / z: 1e-5 relative (north star)."""
+import os
+import sys
+
 import numpy as np
 import pytest
 
 from oracle import oracle as orc
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from gram_reference import e4m3_round  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -173,22 +179,6 @@ def test_csr_feature_space_wider_than_one_gradient_window(mb, monkeypatch, fused
     assert np.abs(x - x_ref).max() <= 1e-5 * np.abs(x_ref).max(), (np.abs(x - x_ref).max() / np.abs(x_ref).max(), steps)
 
 
-def _bf16_round(a):
-    u = np.ascontiguousarray(a, np.float32).view(np.uint32).astype(np.uint64)
-    u = (u + 0x7FFF + ((u >> 16) & 1)) & 0xFFFF0000
-    return u.astype(np.uint32).view(np.float32)
-
-
-def _e4m3_round(a):
-    """Round-to-nearest-even onto the e4m3 grid (3 mantissa bits, exponents 2^-6 .. 2^8, subnormal step 2^-9, saturation at 448)."""
-    a = np.asarray(a, np.float64)
-    mag = np.minimum(np.abs(a), 448.0)
-    e = np.floor(np.log2(np.maximum(mag, 2.0 ** -20)))
-    e = np.clip(e, -6, 8)
-    step = 2.0 ** (e - 3)
-    return np.sign(a) * np.minimum(np.round(mag / step) * step, 448.0)    # np.round = half to even
-
-
 @pytest.mark.parametrize("n,d,sparse", [(1000, 37, False), (2000, 100, False), (700, 300, False), (1000, 50, True), (3000, 700, True),
                                         (333, 255, True)])
 def test_gram_tcgen05_vs_oracle_hessian(mb, n, d, sparse):
@@ -223,7 +213,7 @@ def test_gram_tcgen05_vs_oracle_hessian(mb, n, d, sparse):
         sd = np.sqrt(dd).astype(np.float32)
         amax = 0.5 * np.sqrt(np.float32(w.max())) * max(float(np.abs(v).max()), 1.0)
         g = 2.0 ** (np.frexp(np.float32(224.0) / np.float32(amax))[1] - 1)           # the library's power-of-two operand scale
-        Xt = _e4m3_round((Xb.astype(np.float32) * (sd * np.float32(g))[:, None]).astype(np.float32)) / g
+        Xt = e4m3_round((Xb.astype(np.float32) * (sd * np.float32(g))[:, None]).astype(np.float32)) / g
         H_simt = Xt.T @ Xt + prior
     e_simt = np.abs(H_simt - H_ref).max() / scale
     e_tc = np.abs(H_tc - H_ref).max() / scale

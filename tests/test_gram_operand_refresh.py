@@ -2,10 +2,16 @@
 is skipped, or that runs before K1 has rewritten sqrt(d), leaves the bytes of an earlier point: the Hessian is then stale, which
 only slows the solver's convergence and so escapes the parity tests.  These tests build two Hessians at different points in one
 session and check the second against an emulation at the second point."""
+import os
+import sys
+
 import numpy as np
 import pytest
 
 from oracle import oracle as orc
+
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from gram_reference import e4m3_round  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 
@@ -14,15 +20,6 @@ pytestmark = pytest.mark.gpu
 def mb():
     import mlease_b200
     return mlease_b200
-
-
-def _e4m3_round(a):
-    """Round-to-nearest-even onto the e4m3 grid (3 mantissa bits, exponents 2^-6 .. 2^8, subnormal step 2^-9, saturation at 448)."""
-    a = np.asarray(a, np.float64)
-    mag = np.minimum(np.abs(a), 448.0)
-    e = np.clip(np.floor(np.log2(np.maximum(mag, 2.0 ** -20))), -6, 8)
-    step = 2.0 ** (e - 3)
-    return np.sign(a) * np.minimum(np.round(mag / step) * step, 448.0)
 
 
 def _problem(n, d, seed):
@@ -45,7 +42,7 @@ def _expected(X, w, o, v, wv):
     sd = np.sqrt(dd).astype(np.float32)
     amax = 0.5 * np.sqrt(np.float32(w.max())) * max(float(np.abs(v).max()), 1.0)
     g = 2.0 ** (np.frexp(np.float32(224.0) / np.float32(amax))[1] - 1)   # the library's power-of-two operand scale
-    Xt = _e4m3_round((Xb.astype(np.float32) * (sd * np.float32(g))[:, None]).astype(np.float32)) / g
+    Xt = e4m3_round((Xb.astype(np.float32) * (sd * np.float32(g))[:, None]).astype(np.float32)) / g
     return Xt.T @ Xt
 
 
