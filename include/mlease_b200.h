@@ -66,7 +66,15 @@ typedef struct {
   /* solver knobs (no reference equivalent: the inner solve is exact Newton, not TRON) */
   double newton_xtol;          /* stop when |dir|_inf <= xtol*max(|beta|_inf,1e-2); 0 -> 2e-7 (float32 lattice of the data path) */
   int32_t max_newton;          /* max accepted Newton steps per x-update; 0 -> 50 */
-  int32_t hessian_policy;      /* 0 adaptive chord (refresh when contraction is poor), 1 every step */
+  int32_t hessian_policy;      /* Newton direction of the x-update.  0: Gram + Cholesky, adaptive chord (refactorise when the steps
+                                  contract poorly, L-BFGS pairs on the stale factor); 1: Gram + Cholesky at every step; 2: matrix-free
+                                  truncated Newton, preconditioned CG on Hessian-vector passes over the rows (CSR partitions with sorted
+                                  unique rows only, MLEASE_ERR_INVALID otherwise): no D'^2 state, O(D') per problem.  Automatic rule:
+                                  with 0 or 1, a CSR session whose Gram path would allocate more than the free device memory (~26 D'^2
+                                  bytes per (partition, lambda)) is built matrix-free instead of failing.  A matrix-free session never
+                                  forms H: with policy 2 (at any width) mlease_objective's H, mlease_posterior_variance(full = 1) and
+                                  the Gram / Cholesky timings of mlease_time_kernel return MLEASE_ERR_INVALID, and the CSR upload
+                                  builds no block-major Gram list. */
   void* stream;                /* cudaStream_t to run on (NULL = legacy default stream) */
 } mlease_admm_config;
 
@@ -179,8 +187,9 @@ typedef struct {
 int mlease_get_stats(mlease_session* s, mlease_stats* out);
 int mlease_world_get_stats(mlease_world* w, mlease_stats* out);   /* counters summed over the devices */
 /* Per-kernel device timing for roofline reporting (CUDA events on the session stream around every launch of
- * the Newton slot; categories: 0 = K1 fused pass, 1 = small kernels (reduce/decide, solve, poll), 2 = Gram (wgmma),
- * 3 = Cholesky).  enable: 1 on, 0 off, 2 on + reset accumulators, -1 read only.  Outputs (any may be NULL) are the
+ * the Newton slot; categories: 0 = K1 fused pass, 1 = small kernels (reduce/decide, solve, poll), 2 = Hessian: Gram builds
+ * (wgmma), or in a matrix-free session the diagonal pass + CG set-up and every Hv pass with its CG update, 3 = Cholesky).
+ * gram_flops counts the Gram builds actually run (none in a matrix-free session, whose mlease_stats.gram_builds stays 0).  enable: 1 on, 0 off, 2 on + reset accumulators, -1 read only.  Outputs (any may be NULL) are the
  * accumulators BEFORE this call's reset: ms4[4], count4[4], and the algorithmic work done by the session so far:
  * k1_bytes (SURVEY 8d: dense n*(4*ldx+9) per pass), k1_emit_bytes (bf16 operand writes), gram_flops (n*D'*(D'+1)). */
 int mlease_profile(mlease_session* s, int32_t enable, double* ms4, int64_t* count4, double* k1_bytes, double* k1_emit_bytes,
@@ -202,6 +211,10 @@ int mlease_objective(mlease_session* s, int32_t partition_id, const double* w, c
  * resident partition: exact Newton solve of the same objective.  x: in = init, out = minimiser. */
 int mlease_fit_partition(mlease_session* s, int32_t partition_id, double* x, const double* m, const double* q,
                          int32_t* newton_steps);
+/* LogisticRegressionL2.Hv (regression/liblinearfunc/LogisticRegressionL2.java:231-248) on a resident CSR partition with sorted
+ * unique rows: out = X^T D(w) X v + q .* v, D(w) = diag(weight_i p_i (1 - p_i)) at w, through the Hv mode of the CSR K1 kernels
+ * (the pass matrix-free sessions run for every CG step).  All vectors have num_features+1 entries (host memory). */
+int mlease_hessian_vector(mlease_session* s, int32_t partition_id, const double* w, const double* q, const double* v, double* out);
 
 /* Posterior variance of the model w of one resident partition under prior precision q (= 1/priorVar), the
  * computePosteriorVar / computeFullPostVar tail of LibLinear.train (regression/liblinearfunc/LibLinear.java:315-334) that
@@ -256,7 +269,7 @@ int mlease_test_loglik(int32_t device, void* stream, int64_t nrows, const int32_
 
 /* Bench / profiling hooks (not part of the reference surface): time one fused K1 pass or one Gram build
  * on a resident partition with CUDA events on the session stream, `reps` launches, returns avg ms. */
-int mlease_time_kernel(mlease_session* s, int32_t partition_id, int32_t which /*1=K1,2=Gram wgmma,3=cholesky*/,
+int mlease_time_kernel(mlease_session* s, int32_t partition_id, int32_t which /*1=K1,2=Gram wgmma,3=cholesky,4=Hv pass*/,
                        int32_t reps, int32_t emit_scaled, float* avg_ms);
 
 #ifdef __cplusplus

@@ -9,6 +9,7 @@ namespace mlease {
 
 constexpr int BFGS_M = 16;        // storage for secant pairs kept on top of the (possibly stale) explicit inverse Hessian
 constexpr int BFGS_M_DEFAULT = 6; // pairs actually used (Ctrl::bfgs_m)
+constexpr int CG_MAX_STEPS = 64;  // CG steps per matrix-free Newton direction (newton.cu, where the choice is explained)
 
 // ------------------------------------------------------------------------------------------
 // Per-problem control block, device resident.  A "problem" is one (local partition, lambda)
@@ -58,7 +59,18 @@ struct Ctrl {
   // factored inverse the direction kernels read: this problem's own Ysym after its own factorisation, the group leader's after a
   // shared cold-start factorisation (the lambdas of a partition then stream ONE copy of Y for all their directions)
   const void* ysym_use;
+  // matrix-free batches (hess_policy 2): preconditioned CG for the Newton direction (newton.cu cg_*_kernel)
+  int cg_active;     // this problem's CG runs: the Hv / diagonal K1 modes and the CG kernels work on it
+  int cg_iter;       // CG steps taken for the current direction
+  double cg_rz;      // r.z of the current CG step
+  double cg_g2;      // |g|_2^2 at the accepted point (forcing rule |r| <= eta |g|)
+  float hv_vinf;     // max |hv_vf[k]|, written with hv_vf: the fixed-point scale of the next Hv pass
 };
+
+// K1 modes: the gradient pass, and the two passes of the matrix-free solver over the same rows (fixed d = w p (1-p) of the last
+// gradient pass, read back from sdvec as sqrt(d)^2):  Hv:  column sums of t_i x_i with t_i = d_i (x_i . v) (v = hv_vf, fp32);
+// diagonal:  column sums of d_i x_ic^2 (the Jacobi preconditioner).
+enum { K1_GRAD = 0, K1_HV = 1, K1_DIAG = 2 };
 
 // One problem's device pointers.  Vectors have length ldv (= ldx, multiple of 4, >= Dt) and are
 // zero in [Dt, ldv).  The bias column is PHYSICAL: column Dt-1 of X is 1.0f for every row when the
@@ -142,6 +154,14 @@ struct Problem {
   int lambda_idx;
   int self_idx;            // index of this problem in its batch (tensor-map slot), valid also in compacted copies
   int part_local;
+  // Hessian-vector products (K1 modes K1_HV / K1_DIAG) and the matrix-free Newton-CG direction
+  float rowl1;             // max over rows of sum_j |x_ij| (stored values): bounds |x_i . v| for the fixed-point CSR scatter
+  float* hv_vf;            // [ldx] fp32 vector the Hv pass multiplies (aliases qf: the factored-inverse GEMV is not used then)
+  double* cg_r;            // [ldx] CG residual (matrix-free batches only, else NULL)
+  double* cg_p;            // [ldx] CG search direction
+  double* cg_z;            // [ldx] preconditioned residual
+  double* cg_Hp;           // [ldx] H p
+  double* cg_diag;         // [ldx] Jacobi preconditioner diag(H)
 };
 
 // ------------------------------------------------------------------------------------------

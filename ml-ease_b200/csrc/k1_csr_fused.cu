@@ -16,6 +16,9 @@
 // Per-segment partial gradients go to gpart_f[segment][column] (fp32, one writer per element); k1_partial_reduce_kernel adds
 // the segments in fp64 in segment order.  HBM traffic per partition pass: 8 B (CSR) + ~6.2 B (segment list) per stored value
 // + 9 B per row, for ALL lambdas together.
+// MODE K1_HV / K1_DIAG (matrix-free solver, common.cuh): phase A computes t_il = d_il (x_i . v_l) (v_l = hv_vf, interleaved like
+// beta) or t_il = d_il, with d_il = sqrt(d_il)^2 from sdvec of the last gradient pass; phase B is the same column sum of
+// x_ic t_il (x_ic^2 t_il for the diagonal).  The problems taking part are those with Ctrl::cg_active.
 #include <cub/cub.cuh>
 
 #include <algorithm>
@@ -36,7 +39,7 @@ __device__ __forceinline__ float vget(const float& v, int) { return v; }
 __device__ __forceinline__ float vget(const float2& v, int i) { return i == 0 ? v.x : v.y; }
 __device__ __forceinline__ float vget(const float4& v, int i) { return i == 0 ? v.x : i == 1 ? v.y : i == 2 ? v.z : v.w; }
 
-template <int LP>
+template <int LP, int MODE>
 __global__ void __launch_bounds__(K1F_THREADS, 1) k1_csr_fused_kernel(const Problem* __restrict__ probs, int L, int has_bias, int force_emit) {
   using V = typename VecOf<LP>::T;
   const int b0 = blockIdx.y * L;
@@ -47,7 +50,7 @@ __global__ void __launch_bounds__(K1F_THREADS, 1) k1_csr_fused_kernel(const Prob
     int a = 0, e = 0;
     for (int l = 0; l < L; l++) {
       Ctrl* c = probs[b0 + l].ctrl;
-      if (!c->done && !c->skip_eval) {   // skip_eval: the start-point gradient of this x-update is known without a pass (k4_consensus.cu)
+      if (MODE != K1_GRAD ? (c->cg_active != 0) : (!c->done && !c->skip_eval)) {   // skip_eval: the start-point gradient of this x-update is known without a pass (k4_consensus.cu)
         a |= 1 << l;
         if (force_emit >= 0 ? (force_emit != 0) : (c->emit != 0)) e |= 1 << l;
         if (seg == 0) c->k1_chunks = p0.sg_S;
@@ -67,7 +70,8 @@ __global__ void __launch_bounds__(K1F_THREADS, 1) k1_csr_fused_kernel(const Prob
     float* bs = reinterpret_cast<float*>(beta_s);
     for (int e = tid; e < ldx * LP; e += K1F_THREADS) {
       const int k = e / LP, l = e - k * LP;
-      bs[e] = (l < L && ((act >> l) & 1)) ? probs[b0 + l].beta_tf[k] : 0.f;
+      if constexpr (MODE == K1_GRAD) bs[e] = (l < L && ((act >> l) & 1)) ? probs[b0 + l].beta_tf[k] : 0.f;
+      else bs[e] = (MODE == K1_HV && l < L && ((act >> l) & 1)) ? probs[b0 + l].hv_vf[k] : 0.f;
     }
   }
   __syncthreads();
@@ -87,7 +91,7 @@ __global__ void __launch_bounds__(K1F_THREADS, 1) k1_csr_fused_kernel(const Prob
   const bool lam_on = lam_lane && lam_of < L && ((act >> lam_of) & 1);
   const bool lam_emit = lam_on && ((emit >> lam_of) & 1);
   const float bias_l = has_bias ? reinterpret_cast<const float*>(beta_s)[(size_t)(Dt - 1) * LP + lam_of] : 0.f;
-  float* __restrict__ sd_l = lam_emit ? probs[b0 + lam_of].sdvec : nullptr;
+  float* __restrict__ sd_l = (MODE != K1_GRAD ? lam_on : lam_emit) ? probs[b0 + lam_of].sdvec : nullptr;
   float* r_sf = reinterpret_cast<float*>(r_s);
   float loss = 0.f, rsum = 0.f;
   const long long rstep = 2LL * nw;
@@ -149,7 +153,18 @@ __global__ void __launch_bounds__(K1F_THREADS, 1) k1_csr_fused_kernel(const Prob
 #pragma unroll
       for (int m = K1F_HW / 2; m >= 1; m >>= 1) av += __shfl_xor_sync(0xffffffffu, av, m);
     }
-    if (lam_lane && has_row) {
+    if constexpr (MODE != K1_GRAD) {
+      if (lam_lane && has_row) {
+        float tv = 0.f;
+        if (lam_on) {
+          const float sd = sd_l[i];
+          tv = sd * sd;
+          if constexpr (MODE == K1_HV) tv *= av + bias_l;
+          rsum += tv;
+        }
+        r_sf[(size_t)(i - rb) * LP + lam_of] = tv;
+      }
+    } else if (lam_lane && has_row) {
       const float t = yy * (av + bias_l + oo);
       const float e = __expf(-fabsf(t));
       const float inv = __frcp_rn(1.f + e);
@@ -177,7 +192,7 @@ __global__ void __launch_bounds__(K1F_THREADS, 1) k1_csr_fused_kernel(const Prob
     double sa = 0.0, sb = 0.0;
     for (int wq = 0; wq < nw; wq++) { sa += (double)red[0][tid][wq]; sb += (double)red[1][tid][wq]; }
     const Problem& pl = probs[b0 + tid];
-    pl.fpart[seg] = sa;
+    if (MODE == K1_GRAD) pl.fpart[seg] = sa;
     if (has_bias) pl.gpart_f[(size_t)seg * ldx + Dt - 1] = (float)sb;
   }
   // ------------------------------------------------------------------ phase B: column sums from the segment list
@@ -205,8 +220,9 @@ __global__ void __launch_bounds__(K1F_THREADS, 1) k1_csr_fused_kernel(const Prob
 #pragma unroll
       for (int u = 0; u < UB; u++) {
         const V rr = r_s[rw[u]];
+        const float xv = MODE == K1_DIAG ? vv[u] * vv[u] : vv[u];
 #pragma unroll
-        for (int l = 0; l < LP; l++) acc[l] = fmaf(vv[u], vget(rr, l), acc[l]);
+        for (int l = 0; l < LP; l++) acc[l] = fmaf(xv, vget(rr, l), acc[l]);
       }
     }
     if (k < dep) {   // tail: predicated loads (padding value 0 * r_s[0])
@@ -221,8 +237,9 @@ __global__ void __launch_bounds__(K1F_THREADS, 1) k1_csr_fused_kernel(const Prob
 #pragma unroll
       for (int u = 0; u < UB; u++) {
         const V rr = r_s[rw[u]];
+        const float xv = MODE == K1_DIAG ? vv[u] * vv[u] : vv[u];
 #pragma unroll
-        for (int l = 0; l < LP; l++) acc[l] = fmaf(vv[u], vget(rr, l), acc[l]);
+        for (int l = 0; l < LP; l++) acc[l] = fmaf(xv, vget(rr, l), acc[l]);
       }
     }
     if (col >= 0) {
@@ -454,14 +471,17 @@ cudaError_t k1f_build(long long n, int Dg, long long nnz, const long long* rowpt
   return cudaSuccess;
 }
 
-cudaError_t k1f_launch(const Problem* d_probs, int ngroups, int L, int S, int LP, size_t smem, int has_bias, int force_emit, cudaStream_t st, int* launches) {
+cudaError_t k1f_launch(const Problem* d_probs, int ngroups, int L, int S, int LP, size_t smem, int has_bias, int force_emit, cudaStream_t st, int* launches,
+                       int mode) {
   cudaError_t e;
   const dim3 grid(S, ngroups);
-#define K1F_GO(LPV)                                                                                                        \
-  e = cudaFuncSetAttribute(k1_csr_fused_kernel<LPV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);                \
+#define K1F_GO(LPV, M)                                                                                                     \
+  e = cudaFuncSetAttribute(k1_csr_fused_kernel<LPV, M>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);             \
   if (e != cudaSuccess) return e;                                                                                            \
-  k1_csr_fused_kernel<LPV><<<grid, K1F_THREADS, smem, st>>>(d_probs, L, has_bias, force_emit);
-  if (LP == 1) { K1F_GO(1) } else if (LP == 2) { K1F_GO(2) } else { K1F_GO(4) }
+  k1_csr_fused_kernel<LPV, M><<<grid, K1F_THREADS, smem, st>>>(d_probs, L, has_bias, force_emit);
+#define K1F_GO_LP(M) if (LP == 1) { K1F_GO(1, M) } else if (LP == 2) { K1F_GO(2, M) } else { K1F_GO(4, M) }
+  if (mode == K1_HV) { K1F_GO_LP(K1_HV) } else if (mode == K1_DIAG) { K1F_GO_LP(K1_DIAG) } else { K1F_GO_LP(K1_GRAD) }
+#undef K1F_GO_LP
 #undef K1F_GO
   if (launches) *launches += 1;
   return cudaGetLastError();

@@ -13,6 +13,8 @@
 // so every element of X is read from HBM exactly once and from shared memory exactly once (into registers).
 // Per-CTA partial gradients are accumulated in fp64 registers and written to gpart; a fixed
 // order reduction (k1_reduce_decide in newton.cu) makes the result run-to-run deterministic.
+#include <algorithm>
+
 #include "kernels.cuh"
 
 namespace mlease {
@@ -69,13 +71,15 @@ __device__ __forceinline__ float k1_warp_rows_reduce(float (&p)[RT], int lane) {
 // (nprob_dyn = number of problems, <= 32, one-dimensional grid): the CTAs are dealt round-robin to the problems that are
 // still running, so a slot in which only some problems need a pass still uses every SM.  The chunk count a problem got is
 // published in Ctrl::k1_chunks for the reduction kernels; partial sums are combined in chunk order (deterministic).
+// In the Hv / diagonal modes the running problems are those whose CG runs (Ctrl::cg_active), so that the whole grid serves them.
 struct K1Map { int prob, chunk, nchunks; };
+template <int MODE = K1_GRAD>
 __device__ __forceinline__ K1Map k1_map(const Problem* __restrict__ probs, int nprob_dyn) {
   K1Map m;
   if (nprob_dyn == 0) { m.prob = blockIdx.y; m.chunk = blockIdx.x; m.nchunks = gridDim.x; return m; }
   __shared__ int s_act[34];
   if (threadIdx.x < 32) {
-    const bool a = (int)threadIdx.x < nprob_dyn && probs[threadIdx.x].ctrl->done == 0;
+    const bool a = (int)threadIdx.x < nprob_dyn && (MODE != K1_GRAD ? probs[threadIdx.x].ctrl->cg_active != 0 : probs[threadIdx.x].ctrl->done == 0);
     const unsigned mask = __ballot_sync(0xffffffffu, a);
     if (a) s_act[2 + __popc(mask & ((1u << threadIdx.x) - 1u))] = threadIdx.x;
     if (threadIdx.x == 0) s_act[0] = __popc(mask);
@@ -355,13 +359,23 @@ constexpr int K1_FX_THREADS = 768;   // 24 warps: 80 registers per thread, which
 // BSM: beta staged in shared memory (LDS gathers) / read through L1 from global memory.
 // WIN: the accumulators do not fit shared memory for all ldx columns (more than ~28k features): this launch accumulates the
 // columns [0, col_w) only and stores the row residuals r_i in rvec; k1_csr_fx_window_kernel adds the other column windows.
-template <bool BSM, bool WIN>
+// MODE K1_HV / K1_DIAG (common.cuh): the row weight is t_i = d_i (x_i . v + v_bias) / d_i instead of the residual, with the
+// fixed-point bound of k1_fx_mode_bound; problems take part when Ctrl::cg_active is set.
+// Fixed-point bound of the Hv / diagonal modes: |t_i| <= (w_i / 4) (rowl1 + 1) |v|_inf resp. w_i / 4, times max(|x|max, 1) per
+// contribution (max(|x|max^2, 1) for the diagonal).  |v|_inf is Ctrl::hv_vinf, written with hv_vf.
+template <int MODE>
+__device__ __forceinline__ float k1_fx_mode_bound(const Problem& pb, long long per) {
+  if constexpr (MODE == K1_HV) return (float)per * 0.25f * pb.wmax * (pb.rowl1 + 1.f) * pb.ctrl->hv_vinf * fmaxf(pb.vmax, 1.f);
+  return (float)per * 0.25f * pb.wmax * fmaxf(pb.vmax * pb.vmax, 1.f);
+}
+
+template <bool BSM, bool WIN, int MODE = K1_GRAD>
 __global__ void __launch_bounds__(K1_FX_THREADS, 1) k1_csr_fx_kernel(const Problem* __restrict__ probs, int has_bias, int force_emit, int nprob_dyn, int col_w) {
-  const K1Map km = k1_map(probs, nprob_dyn);
+  const K1Map km = k1_map<MODE>(probs, nprob_dyn);
   if (km.prob < 0) return;
   const Problem& pb = probs[km.prob];
   Ctrl* ctrl = pb.ctrl;
-  if (ctrl->done) return;
+  if (MODE != K1_GRAD ? !ctrl->cg_active : ctrl->done) return;
   if (km.chunk == 0 && threadIdx.x == 0) ctrl->k1_chunks = km.nchunks;
   const bool emit = force_emit >= 0 ? (force_emit != 0) : (ctrl->emit != 0);
   extern __shared__ __align__(16) float csr_sm[];
@@ -375,15 +389,15 @@ __global__ void __launch_bounds__(K1_FX_THREADS, 1) k1_csr_fx_kernel(const Probl
   float* b_s = csr_sm + 2 * (size_t)gs;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = blockDim.x >> 5;
   for (int k = tid; k < gs; k += blockDim.x) { g_hi[k] = 0; g_lo[k] = 0; }
+  const float* __restrict__ bg = MODE == K1_GRAD ? pb.beta_tf : pb.hv_vf;
   if (BSM)
-    for (int k = tid; k < ldx; k += blockDim.x) b_s[k] = pb.beta_tf[k];
+    for (int k = tid; k < ldx; k += blockDim.x) b_s[k] = bg[k];
   __syncthreads();
-  const float* __restrict__ bg = pb.beta_tf;
   const long long n = pb.n;
   const long long per = (n + km.nchunks - 1) / km.nchunks;
   const long long rb = (long long)km.chunk * per, re = min(n, rb + per);
   // fixed-point scales (powers of two: scaling is exact)
-  float bound = (float)per * pb.wmax * fmaxf(pb.vmax, has_bias ? 1.f : 0.f);
+  float bound = MODE != K1_GRAD ? k1_fx_mode_bound<MODE>(pb, per) : (float)per * pb.wmax * fmaxf(pb.vmax, has_bias ? 1.f : 0.f);
   if (!(bound > 0.f) || !(bound < 3.0e38f)) bound = 1.f;
   const int e_hi = 29 - (ilogbf(bound) + 1);
   int kbits = 30 - (64 - __clzll((unsigned long long)max(per, 1LL)));
@@ -431,22 +445,30 @@ __global__ void __launch_bounds__(K1_FX_THREADS, 1) k1_csr_fx_kernel(const Probl
 #pragma unroll
     for (int m = HW / 2; m >= 1; m >>= 1) a += __shfl_xor_sync(0xffffffffu, a, m);   // stays inside the half-warp
     a += bias_b;
-    const float t = yy * (a + oo);
-    const float e = __expf(-fabsf(t));
-    const float inv = __frcp_rn(1.f + e);
-    const float p = t >= 0.f ? inv : e * inv;
-    const float qq = t >= 0.f ? e * inv : inv;
-    if (sl == 0 && has_row) loss += (double)(ww * ((t >= 0.f ? 0.f : -t) - __logf(inv)));
-    const float rs = has_row ? -ww * yy * qq * s_hi : 0.f;     // contribution scale: c S = value * rs
+    float rs, rrow = 0.f, p = 0.f, qq = 0.f;
+    if constexpr (MODE != K1_GRAD) {
+      const float sd = has_row ? __ldg(pb.sdvec + i) : 0.f;
+      rrow = MODE == K1_HV ? sd * sd * a : sd * sd;
+      rs = rrow * s_hi;
+    } else {
+      const float t = yy * (a + oo);
+      const float e = __expf(-fabsf(t));
+      const float inv = __frcp_rn(1.f + e);
+      p = t >= 0.f ? inv : e * inv;
+      qq = t >= 0.f ? e * inv : inv;
+      if (sl == 0 && has_row) loss += (double)(ww * ((t >= 0.f ? 0.f : -t) - __logf(inv)));
+      rs = has_row ? -ww * yy * qq * s_hi : 0.f;     // contribution scale: c S = value * rs
+    }
 #pragma unroll
     for (int q = 0; q < NCH; q++) {
-      const float ts = v[q] * rs, h = rintf(ts);
+      const float ts = (MODE == K1_DIAG ? v[q] * v[q] : v[q]) * rs, h = rintf(ts);
       const int cc = (!WIN || c[q] < W) ? c[q] : dummy;
       atomicAdd(&g_hi[cc], (int)h);
       atomicAdd(&g_lo[cc], __float2int_rn((ts - h) * s_k));
     }
     for (int j = NCH * HW + sl; j < len; j += HW) {
-      const float ts = __ldg(vr + j) * rs, h = rintf(ts);
+      const float xj = __ldg(vr + j);
+      const float ts = (MODE == K1_DIAG ? xj * xj : xj) * rs, h = rintf(ts);
       int cc = __ldg(cr + j);
       if (WIN && cc >= W) cc = dummy;
       atomicAdd(&g_hi[cc], (int)h);
@@ -457,8 +479,8 @@ __global__ void __launch_bounds__(K1_FX_THREADS, 1) k1_csr_fx_kernel(const Probl
       atomicAdd(&g_hi[Dt - 1], (int)h);
       atomicAdd(&g_lo[Dt - 1], __float2int_rn((rs - h) * s_k));
     }
-    if (emit && sl == 0 && has_row) pb.sdvec[i] = sqrtf(ww * p * qq);   // the Gram kernel assembles the scaled rows itself
-    if (WIN && sl == 0 && has_row) pb.rvec[i] = -ww * yy * qq;           // residual for the other column windows
+    if (MODE == K1_GRAD && emit && sl == 0 && has_row) pb.sdvec[i] = sqrtf(ww * p * qq);   // the Gram kernel assembles the scaled rows itself
+    if (WIN && sl == 0 && has_row) pb.rvec[i] = MODE == K1_GRAD ? -ww * yy * qq : rrow;   // row weight for the other column windows
     i = in; j0 = j0n; len = lenn;
   }
   loss += __shfl_down_sync(0xffffffffu, loss, 16);   // lane 0 += lane 16
@@ -466,6 +488,7 @@ __global__ void __launch_bounds__(K1_FX_THREADS, 1) k1_csr_fx_kernel(const Probl
   double* gp = pb.gpart + (size_t)km.chunk * ldx;
   const double inv_hi = (double)ldexpf(1.f, -e_hi), inv_k = (double)ldexpf(1.f, -kbits);
   for (int k = tid; k < min(W, ldx); k += blockDim.x) gp[k] = ((double)g_hi[k] + (double)g_lo[k] * inv_k) * inv_hi;
+  if (MODE != K1_GRAD) return;
   __shared__ double red[32];
   if (lane == 0) red[warp] = loss;
   __syncthreads();
@@ -478,12 +501,13 @@ __global__ void __launch_bounds__(K1_FX_THREADS, 1) k1_csr_fx_kernel(const Probl
 
 // Columns [col_lo, col_lo + col_w) of the gradient for partitions too wide for one shared-memory window: same CTA -> rows
 // mapping and the same fixed-point scales as k1_csr_fx_kernel<.., true>, which ran first in this slot and left r_i in rvec.
+template <int MODE = K1_GRAD>
 __global__ void __launch_bounds__(K1_FX_THREADS, 1) k1_csr_fx_window_kernel(const Problem* __restrict__ probs, int has_bias, int nprob_dyn,
                                                                             int col_lo, int col_w) {
-  const K1Map km = k1_map(probs, nprob_dyn);
+  const K1Map km = k1_map<MODE>(probs, nprob_dyn);
   if (km.prob < 0) return;
   const Problem& pb = probs[km.prob];
-  if (pb.ctrl->done) return;
+  if (MODE != K1_GRAD ? !pb.ctrl->cg_active : pb.ctrl->done) return;
   extern __shared__ __align__(16) float csr_sm[];
   const int ldx = pb.ldx, Dt = pb.Dt;
   const int gs = col_w + 32;
@@ -495,7 +519,7 @@ __global__ void __launch_bounds__(K1_FX_THREADS, 1) k1_csr_fx_window_kernel(cons
   const long long n = pb.n;
   const long long per = (n + km.nchunks - 1) / km.nchunks;
   const long long rb = (long long)km.chunk * per, re = min(n, rb + per);
-  float bound = (float)per * pb.wmax * fmaxf(pb.vmax, has_bias ? 1.f : 0.f);
+  float bound = MODE != K1_GRAD ? k1_fx_mode_bound<MODE>(pb, per) : (float)per * pb.wmax * fmaxf(pb.vmax, has_bias ? 1.f : 0.f);
   if (!(bound > 0.f) || !(bound < 3.0e38f)) bound = 1.f;
   const int e_hi = 29 - (ilogbf(bound) + 1);
   int kbits = 30 - (64 - __clzll((unsigned long long)max(per, 1LL)));
@@ -512,7 +536,8 @@ __global__ void __launch_bounds__(K1_FX_THREADS, 1) k1_csr_fx_window_kernel(cons
     const float* __restrict__ vr = pb.vals + j0;
     const int* __restrict__ cr = pb.colidx + j0;
     for (int j = sl; j < len; j += 16) {
-      const float ts = __ldg(vr + j) * rs, h = rintf(ts);
+      const float xj = __ldg(vr + j);
+      const float ts = (MODE == K1_DIAG ? xj * xj : xj) * rs, h = rintf(ts);
       const int idx = __ldg(cr + j) - col_lo;
       const int cc = (unsigned)idx < (unsigned)col_w ? idx : dummy;
       const bool in = (unsigned)idx < (unsigned)col_w;
@@ -649,37 +674,48 @@ int k1_csr_window(int ldx) {
   return (int)((cap / 8 - 32) & ~(size_t)31);
 }
 
+// The CSR fixed-point K1 in mode MODE: one launch when the accumulators of every column fit shared memory, else the row pass with
+// columns [0, W) (it leaves the row weights in rvec) and one window launch per further W columns.
+template <int MODE>
+static cudaError_t k1_csr_fx_launch(const Problem* d_probs, dim3 grid_all, int ldx, int has_bias, int force_emit, cudaStream_t stream, int* launches,
+                                    int nprob_dyn) {
+  const size_t cap = 220 * 1024;
+  const size_t g_bytes = (size_t)2 * (ldx + 32) * 4;
+  cudaError_t e;
+  if (g_bytes <= cap) {
+    const bool bsm = g_bytes + (size_t)ldx * 4 <= cap;
+    const size_t smem = g_bytes + (bsm ? (size_t)ldx * 4 : 0);
+    e = bsm ? cudaFuncSetAttribute(k1_csr_fx_kernel<true, false, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
+            : cudaFuncSetAttribute(k1_csr_fx_kernel<false, false, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    if (bsm) k1_csr_fx_kernel<true, false, MODE><<<grid_all, K1_FX_THREADS, smem, stream>>>(d_probs, has_bias, force_emit, nprob_dyn, ldx);
+    else k1_csr_fx_kernel<false, false, MODE><<<grid_all, K1_FX_THREADS, smem, stream>>>(d_probs, has_bias, force_emit, nprob_dyn, ldx);
+    if (launches) *launches += 1;
+    return cudaGetLastError();
+  }
+  // wider than one shared-memory window: the first launch does the margins and columns [0, W), one more launch per window
+  const int W = k1_csr_window(ldx);
+  const size_t smem = (size_t)2 * (W + 32) * 4;
+  if ((e = cudaFuncSetAttribute(k1_csr_fx_kernel<false, true, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return e;
+  if ((e = cudaFuncSetAttribute(k1_csr_fx_window_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return e;
+  k1_csr_fx_kernel<false, true, MODE><<<grid_all, K1_FX_THREADS, smem, stream>>>(d_probs, has_bias, force_emit, nprob_dyn, W);
+  if (launches) *launches += 1;
+  for (int lo = W; lo < ldx; lo += W) {
+    k1_csr_fx_window_kernel<MODE><<<grid_all, K1_FX_THREADS, smem, stream>>>(d_probs, has_bias, nprob_dyn, lo, W);
+    if (launches) *launches += 1;
+  }
+  return cudaGetLastError();
+}
+
 cudaError_t k1_launch(const Problem* d_probs, int nprob, bool csr, int ldx, int has_bias, int ctas_per_problem,
-                      int force_emit, cudaStream_t stream, int* launches, int csr_fx, int nprob_dyn) {
+                      int force_emit, cudaStream_t stream, int* launches, int csr_fx, int nprob_dyn, int mode) {
   // dynamic mapping: ctas_per_problem is then the size of the whole one-dimensional grid
   const dim3 grid_all = nprob_dyn ? dim3(ctas_per_problem, 1) : dim3(ctas_per_problem, nprob);
+  if (mode != K1_GRAD && !(csr && csr_fx)) return cudaErrorInvalidValue;   // the Hv / diagonal modes exist for sorted unique CSR rows only
   if (csr && csr_fx) {
-    const size_t cap = 220 * 1024;
-    const size_t g_bytes = (size_t)2 * (ldx + 32) * 4;
-    cudaError_t e;
-    if (g_bytes <= cap) {
-      const bool bsm = g_bytes + (size_t)ldx * 4 <= cap;
-      const size_t smem = g_bytes + (bsm ? (size_t)ldx * 4 : 0);
-      e = bsm ? cudaFuncSetAttribute(k1_csr_fx_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)
-              : cudaFuncSetAttribute(k1_csr_fx_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-      if (e != cudaSuccess) return e;
-      if (bsm) k1_csr_fx_kernel<true, false><<<grid_all, K1_FX_THREADS, smem, stream>>>(d_probs, has_bias, force_emit, nprob_dyn, ldx);
-      else k1_csr_fx_kernel<false, false><<<grid_all, K1_FX_THREADS, smem, stream>>>(d_probs, has_bias, force_emit, nprob_dyn, ldx);
-      if (launches) *launches += 1;
-      return cudaGetLastError();
-    }
-    // wider than one shared-memory window: the first launch does the margins and columns [0, W), one more launch per window
-    const int W = k1_csr_window(ldx);
-    const size_t smem = (size_t)2 * (W + 32) * 4;
-    if ((e = cudaFuncSetAttribute(k1_csr_fx_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return e;
-    if ((e = cudaFuncSetAttribute(k1_csr_fx_window_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)) != cudaSuccess) return e;
-    k1_csr_fx_kernel<false, true><<<grid_all, K1_FX_THREADS, smem, stream>>>(d_probs, has_bias, force_emit, nprob_dyn, W);
-    if (launches) *launches += 1;
-    for (int lo = W; lo < ldx; lo += W) {
-      k1_csr_fx_window_kernel<<<grid_all, K1_FX_THREADS, smem, stream>>>(d_probs, has_bias, nprob_dyn, lo, W);
-      if (launches) *launches += 1;
-    }
-    return cudaGetLastError();
+    if (mode == K1_HV) return k1_csr_fx_launch<K1_HV>(d_probs, grid_all, ldx, has_bias, 0, stream, launches, nprob_dyn);
+    if (mode == K1_DIAG) return k1_csr_fx_launch<K1_DIAG>(d_probs, grid_all, ldx, has_bias, 0, stream, launches, nprob_dyn);
+    return k1_csr_fx_launch<K1_GRAD>(d_probs, grid_all, ldx, has_bias, force_emit, stream, launches, nprob_dyn);
   }
   if (csr) {
     const int beta_in_smem = (size_t)2 * ldx * 4 <= 200 * 1024 ? 1 : 0;
@@ -702,6 +738,24 @@ cudaError_t k1_launch(const Problem* d_probs, int nprob, bool csr, int ldx, int 
   if (p.G == 1) { K1_LAUNCH(1, 8) } else if (p.G == 2) { K1_LAUNCH(2, 8) } else { K1_LAUNCH(4, 4) }
 #undef K1_LAUNCH
   if (launches) *launches += 1;
+  return cudaGetLastError();
+}
+
+// max over rows of sum_j |v_ij|: warp per row; fp32 sums of non-negative terms, atomicMax on the bits (upload, once per partition)
+__global__ void csr_row_l1_kernel(long long n, const long long* __restrict__ rowptr, const float* __restrict__ vals, unsigned* __restrict__ out) {
+  const int lane = threadIdx.x & 31;
+  const long long nw = ((long long)gridDim.x * blockDim.x) >> 5;
+  float m = 0.f;
+  for (long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += nw) {
+    float a = 0.f;
+    for (long long j = rowptr[i] + lane; j < rowptr[i + 1]; j += 32) a += fabsf(vals[j]);
+    m = fmaxf(m, warp_sum(a));
+  }
+  if (lane == 0) atomicMax(out, __float_as_uint(m));
+}
+cudaError_t csr_row_l1_max(long long n, const long long* rowptr, const float* vals, unsigned* out, cudaStream_t st) {
+  if (n <= 0) return cudaSuccess;
+  csr_row_l1_kernel<<<(int)std::min<long long>((n + 7) / 8, 2048), 256, 0, st>>>(n, rowptr, vals, out);
   return cudaGetLastError();
 }
 

@@ -8,20 +8,33 @@ namespace mlease {
 bool k1_dense_plan(int ldx, int* R_out, int* S_out, int* G_out, size_t* smem_out, int* ctas_per_sm);
 int k1_csr_window(int ldx);
 cudaError_t k1_launch(const Problem* d_probs, int nprob, bool csr, int ldx, int has_bias, int ctas_per_problem,
-                      int force_emit, cudaStream_t stream, int* launches, int csr_fx = 0, int nprob_dyn = 0);
+                      int force_emit, cudaStream_t stream, int* launches, int csr_fx = 0, int nprob_dyn = 0, int mode = K1_GRAD);
 
 // fused multi-lambda CSR K1 (k1_csr_fused.cu)
 bool k1f_plan(long long n, int ldx, int L, int num_sms, int* S_out, int* rows_out, int* LP_out, size_t* smem_out);
 cudaError_t k1f_build(long long n, int Dg, long long nnz, const long long* rowptr, const int* colidx, const float* vals, int S, int sg_rows, int* ngrp_out,
                       int** perm_out, int** depth_out, long long** goff_out, unsigned short** row16_out, float** val_out, long long* total_out,
                       cudaStream_t st);
-cudaError_t k1f_launch(const Problem* d_probs, int ngroups, int L, int S, int LP, size_t smem, int has_bias, int force_emit, cudaStream_t st, int* launches);
+cudaError_t k1f_launch(const Problem* d_probs, int ngroups, int L, int S, int LP, size_t smem, int has_bias, int force_emit, cudaStream_t st, int* launches,
+                       int mode = K1_GRAD);
+// max over rows of sum_j |v_ij| (float bits, non-negative: order preserving) -> *out (k1_score_grad.cu)
+cudaError_t csr_row_l1_max(long long n, const long long* rowptr, const float* vals, unsigned* out, cudaStream_t st);
 
 // Newton state machine (newton.cu)
 cudaError_t newton_begin(const Problem* d_probs, int nprob, double xtol, int max_newton, int hess_policy,
                          int invalidate_hess, int rebuild_is_expensive, cudaStream_t st, int* launches, int bfgs_m = BFGS_M_DEFAULT, int self_scale = 0);
 cudaError_t k1_reduce_decide(const Problem* d_probs, int nprob, int Dt, cudaStream_t st, int* launches, int spec = 0);
 cudaError_t newton_solve(const Problem* d_probs, int nprob, int ldh, cudaStream_t st, int* launches, int group_L = 1);
+// matrix-free Newton-CG direction (newton.cu): begin (pick the problems that need a direction), the fixed-order reduction of the
+// Hv / diagonal partials (out 0: g_t, 1: cg_Hp, 2: cg_diag), init (after the diagonal pass), one CG step (after an Hv pass), and
+// the poll of the CG flags into *d_any (1 while a problem's CG still runs)
+cudaError_t cg_begin(const Problem* d_probs, int nprob, cudaStream_t st, int* launches);
+cudaError_t hv_reduce(const Problem* d_probs, int nprob, int Dt, int out, cudaStream_t st, int* launches);
+cudaError_t cg_init(const Problem* d_probs, int nprob, int Dt, cudaStream_t st, int* launches);
+cudaError_t cg_step(const Problem* d_probs, int nprob, int Dt, cudaStream_t st, int* launches);
+cudaError_t cg_poll(const Problem* d_probs, int nprob, int* d_any, cudaStream_t st, int* launches);
+// the direction bookkeeping of newton_solve alone (the direction is already in dir, no secant pairs)
+cudaError_t newton_finish(const Problem* d_probs, int nprob, int Dt, cudaStream_t st, int* launches);
 
 // K2 (k2_gram.cu)
 int gram_make_tensor_map(void* out_map_host, const void* xt, long long n, int Dp);

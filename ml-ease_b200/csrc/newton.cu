@@ -64,7 +64,9 @@ __global__ void newton_begin_kernel(const Problem* __restrict__ probs, double xt
     // Rebuild at the start point when there is no factor, when the policy says always, or when the previous
     // x-update's chord steps contracted slowly: a factor taken at a (nearly) converged point makes every later
     // x-update of the ADMM run a 2-3 pass affair, and costs about as much as 2.5 K1 passes.
-    c->emit = (hess_policy == 1 || !c->hess_valid || c->refresh_next) ? 1 : 0;
+    // (hess_policy 2, matrix-free: no Gram is ever built; the direction comes from the CG kernels below)
+    c->emit = (hess_policy != 2 && (hess_policy == 1 || !c->hess_valid || c->refresh_next)) ? 1 : 0;
+    c->cg_active = 0;
     c->refresh_next = 0;
     if (c->emit) c->skip_eval = 0;   // a rebuild at the start point needs K1's sqrt(d) there: regular first slot
     c->worst_ratio = 0.0;
@@ -183,6 +185,8 @@ __global__ void __launch_bounds__(1024) k1_reduce_decide_kernel(const Problem* _
         // policy for the NEXT accepted point: refresh when the chord step contracted poorly
         if (c->hess_policy == 1) {
           c->emit = 1;
+        } else if (c->hess_policy == 2) {
+          c->emit = 0;
         } else {
           // Wide systems (a rebuild costs more than ~8 passes) lean on the secant pairs instead of refactorising -- but not for
           // ever: a dozen steps on the same factor that still contract by less than 2x mean the factor was taken too far
@@ -206,7 +210,7 @@ __global__ void __launch_bounds__(1024) k1_reduce_decide_kernel(const Problem* _
     // A rebuild at this accepted point supersedes the secant pairs: drop them HERE (before the fused first L-BFGS loop
     // below runs), so that both loops of the recursion see the same, empty, pair set.
     if (action == 1 && c->need_hess) c->bfgs_count = 0;
-    if (action == 1 && have_dir && !c->need_hess && sy > 1e-10 * sqrt(ss * yy2) && sy > 0.0) {   // strictly convex => s.y > 0 up to rounding
+    if (action == 1 && have_dir && !c->need_hess && c->hess_policy != 2 && sy > 1e-10 * sqrt(ss * yy2) && sy > 0.0) {   // strictly convex => s.y > 0 up to rounding
       s_slot = c->bfgs_count % c->bfgs_m;
       pb.bfgs_rho[s_slot] = 1.0 / sy;
       c->bfgs_count++;
@@ -472,6 +476,177 @@ __global__ void __launch_bounds__(1024) newton_solve_kernel(const Problem* __res
     pb.beta_tf[k] = btf;
     if (fin) pb.beta[k] = bt;  // final tiny step taken in double, without another pass
   }
+}
+
+// ------------------------------------------------------------------------------------------
+// Matrix-free Newton direction (hess_policy 2): truncated Newton, the system H dir = g solved by Jacobi-preconditioned CG in fp64,
+// H touched only through Hv passes over the rows (K1_HV mode of the CSR K1 kernels) -- TRON's inner loop (bw/Tron.java:126-179)
+// without the trust region: the line search of k1_reduce_decide_kernel globalises the step as for the factored directions.
+//   slot:  K1 (d of the trial point into sdvec) -> decide -> cg_begin -> diagonal pass -> cg_init -> {Hv pass -> cg_step} x k
+//          -> newton_finish (the sign, the stop test and the next trial point of newton_solve_kernel, with no secant pairs)
+// Forcing rule |r|_2 <= CG_ETA |g|_2, TRON's eta = 0.1 (bw/Tron.java:138): each Newton step then removes ~90 % of the
+// gradient on top of the quadratic term, and the outer stop test (|dir|_inf <= xtol max(|beta|_inf, 1e-2)) is taken on a
+// direction that is itself accurate to 10 %, so the final point is accurate to xtol/10.  A tighter eta buys fewer Newton
+// steps (one K1 pass + one diagonal pass each) with more Hv passes per step; 0.1 keeps both small.  CG_MAX_STEPS caps the
+// work of one direction on an ill-conditioned system: CG iterates started at 0 are descent directions at every step, so a
+// capped direction is still a valid line-search direction (the outer Newton loop and its max_newton limit take over).
+constexpr double CG_ETA = 0.1;   // (CG_MAX_STEPS = 64: common.cuh, the host loop bounds its read-backs with it)
+
+__global__ void cg_begin_kernel(const Problem* __restrict__ probs, int nprob) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= nprob) return;
+  Ctrl* c = probs[b].ctrl;
+  c->cg_active = (!c->done && c->need_solve) ? 1 : 0;
+  c->cg_iter = 0;
+}
+
+// Fixed-order reduction of the Hv / diagonal partials (same order as k1_partial_reduce_kernel), data term only.
+template <int OUT>
+__global__ void __launch_bounds__(256) hv_partial_reduce_kernel(const Problem* __restrict__ probs) {
+  const Problem& pb = probs[blockIdx.y];
+  if (!pb.ctrl->cg_active) return;
+  __shared__ double sh[8][33];
+  const int c = threadIdx.x & 31, grp = threadIdx.x >> 5;
+  const int k = blockIdx.x * 32 + c;
+  const int nct = pb.ctrl->k1_chunks, ldx = pb.ldx;
+  double s = 0.0;
+  if (k < pb.Dt) {
+    if (pb.gpart_f) { for (int t = grp; t < nct; t += 8) s += (double)pb.gpart_f[(size_t)t * ldx + k]; }
+    else { for (int t = grp; t < nct; t += 8) s += pb.gpart[(size_t)t * ldx + k]; }
+  }
+  sh[grp][c] = s;
+  __syncthreads();
+  if (grp == 0 && k < pb.Dt) {
+    double a = 0.0;
+#pragma unroll
+    for (int g = 0; g < 8; g++) a += sh[g][c];
+    double* out = OUT == 0 ? pb.g_t : OUT == 1 ? pb.cg_Hp : pb.cg_diag;
+    out[k] = a;
+  }
+}
+
+// After the diagonal pass: M = diag(H) (data + prior), dir = 0, r = g, z = M^-1 r, p = z.
+__global__ void __launch_bounds__(1024) cg_init_kernel(const Problem* __restrict__ probs) {
+  const Problem& pb = probs[blockIdx.x];
+  Ctrl* c = pb.ctrl;
+  if (!c->cg_active) return;
+  __shared__ double sc[32];
+  const int NTD = blockDim.x, Dt = pb.Dt, ldx = pb.ldx;
+  double rz = 0.0, g2 = 0.0, vinf = 0.0;
+  for (int k = threadIdx.x; k < ldx; k += NTD) {
+    if (k < Dt) {
+      double m = pb.cg_diag[k] + pb.q[k];
+      if (!(m > 0.0)) m = 1.0;   // a column no row lists and no prior: any positive scale preconditions it
+      pb.cg_diag[k] = m;
+      const double r = pb.g_acc[k], z = r / m;
+      pb.cg_r[k] = r; pb.cg_z[k] = z; pb.cg_p[k] = z;
+      pb.hv_vf[k] = (float)z;
+      vinf = fmax(vinf, fabs((double)(float)z));
+      rz += r * z; g2 += r * r;
+    } else {
+      pb.hv_vf[k] = 0.f;
+    }
+    pb.dir[k] = 0.0;
+  }
+  rz = block_sum(rz, sc);
+  g2 = block_sum(g2, sc);
+  vinf = block_max(vinf, sc);
+  if (threadIdx.x == 0) { c->cg_rz = rz; c->cg_g2 = g2; c->hv_vinf = (float)vinf; }
+}
+
+// One CG step after the Hv pass of p (cg_Hp holds the data term X^T D X p).
+__global__ void __launch_bounds__(1024) cg_step_kernel(const Problem* __restrict__ probs) {
+  const Problem& pb = probs[blockIdx.x];
+  Ctrl* c = pb.ctrl;
+  if (!c->cg_active) return;
+  __shared__ double sc[32];
+  __shared__ int s_go;
+  const int NTD = blockDim.x, Dt = pb.Dt;
+  double php = 0.0;
+  for (int k = threadIdx.x; k < Dt; k += NTD) {
+    const double hp = pb.cg_Hp[k] + pb.q[k] * pb.cg_p[k];
+    pb.cg_Hp[k] = hp;
+    php += pb.cg_p[k] * hp;
+  }
+  php = block_sum(php, sc);
+  const double alpha = c->cg_rz / php;
+  double rr = 0.0;
+  if (php > 0.0) {
+    for (int k = threadIdx.x; k < Dt; k += NTD) {
+      pb.dir[k] += alpha * pb.cg_p[k];
+      const double r = pb.cg_r[k] - alpha * pb.cg_Hp[k];
+      pb.cg_r[k] = r;
+      rr += r * r;
+    }
+  }
+  rr = block_sum(rr, sc);
+  if (threadIdx.x == 0) {
+    int go = 0;
+    if (!(php > 0.0)) { c->fail = 1; c->done = 1; c->cg_active = 0; }   // non-positive curvature or NaN: "Model fitting error!"
+    else if (++c->cg_iter >= CG_MAX_STEPS || rr <= CG_ETA * CG_ETA * c->cg_g2) c->cg_active = 0;
+    else go = 1;
+    s_go = go;
+  }
+  __syncthreads();
+  if (!s_go) return;
+  double rz = 0.0;
+  for (int k = threadIdx.x; k < Dt; k += NTD) {
+    const double z = pb.cg_r[k] / pb.cg_diag[k];
+    pb.cg_z[k] = z;
+    rz += pb.cg_r[k] * z;
+  }
+  rz = block_sum(rz, sc);
+  const double beta = rz / c->cg_rz;
+  double vinf = 0.0;
+  for (int k = threadIdx.x; k < Dt; k += NTD) {
+    const double p = pb.cg_z[k] + beta * pb.cg_p[k];
+    pb.cg_p[k] = p;
+    pb.hv_vf[k] = (float)p;
+    vinf = fmax(vinf, fabs((double)(float)p));
+  }
+  vinf = block_max(vinf, sc);   // (its barriers also order every read of cg_rz above before the write below)
+  if (threadIdx.x == 0) { c->cg_rz = rz; c->hv_vinf = (float)vinf; }
+}
+
+__global__ void cg_poll_kernel(const Problem* __restrict__ probs, int nprob, int* __restrict__ any) {
+  int a = 0;
+  for (int b = threadIdx.x; b < nprob; b += blockDim.x) a |= probs[b].ctrl->cg_active;
+  a = __syncthreads_or(a);
+  if (threadIdx.x == 0) *any = a;
+}
+
+cudaError_t cg_begin(const Problem* d_probs, int nprob, cudaStream_t st, int* launches) {
+  cg_begin_kernel<<<(nprob + 255) / 256, 256, 0, st>>>(d_probs, nprob);
+  if (launches) *launches += 1;
+  return cudaGetLastError();
+}
+cudaError_t hv_reduce(const Problem* d_probs, int nprob, int Dt, int out, cudaStream_t st, int* launches) {
+  const dim3 grid((Dt + 31) / 32, nprob);
+  if (out == 0) hv_partial_reduce_kernel<0><<<grid, 256, 0, st>>>(d_probs);
+  else if (out == 1) hv_partial_reduce_kernel<1><<<grid, 256, 0, st>>>(d_probs);
+  else hv_partial_reduce_kernel<2><<<grid, 256, 0, st>>>(d_probs);
+  if (launches) *launches += 1;
+  return cudaGetLastError();
+}
+cudaError_t cg_init(const Problem* d_probs, int nprob, int Dt, cudaStream_t st, int* launches) {
+  cg_init_kernel<<<nprob, Dt > 2048 ? 1024 : NT, 0, st>>>(d_probs);
+  if (launches) *launches += 1;
+  return cudaGetLastError();
+}
+cudaError_t cg_step(const Problem* d_probs, int nprob, int Dt, cudaStream_t st, int* launches) {
+  cg_step_kernel<<<nprob, Dt > 2048 ? 1024 : NT, 0, st>>>(d_probs);
+  if (launches) *launches += 1;
+  return cudaGetLastError();
+}
+cudaError_t cg_poll(const Problem* d_probs, int nprob, int* d_any, cudaStream_t st, int* launches) {
+  cg_poll_kernel<<<1, 256, 0, st>>>(d_probs, nprob, d_any);
+  if (launches) *launches += 1;
+  return cudaGetLastError();
+}
+cudaError_t newton_finish(const Problem* d_probs, int nprob, int Dt, cudaStream_t st, int* launches) {
+  newton_solve_kernel<<<nprob, Dt > 2048 ? 1024 : NT, 0, st>>>(d_probs);
+  if (launches) *launches += 1;
+  return cudaGetLastError();
 }
 
 cudaError_t newton_begin(const Problem* d_probs, int nprob, double xtol, int max_newton, int hess_policy,

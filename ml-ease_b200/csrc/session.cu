@@ -126,6 +126,7 @@ struct PartData {
   long long nnz = 0;
   int csr_unique = 0;
   float vmax = 0.f, wmax = 1.f;
+  float rowl1 = 0.f;               // max over rows of sum_j |v_ij| (fixed-point bound of the Hv pass)
   long long* bm_offs = nullptr;    // block-major entry list for the CSR Gram (built at upload when rows are sorted & unique)
   unsigned short* bm_keys = nullptr;
   float* bm_vals = nullptr;
@@ -145,6 +146,9 @@ struct Batch {
   int has_bias = 1;
   int k1_grid = 1, gram_slices = 1, ntiles = 0;
   int gram_from_csr = 0;          // every problem of the batch assembles its Gram tiles from CSR (no dense bf16 operand)
+  int csr_fx = 0;                 // CSR rows sorted and unique: the deterministic K1 kernels (fixed point / segment lists) and their Hv
+                                  // modes run, sqrt(d) goes to sdvec.  The Gram path has it with its block-major lists; a matrix-free
+                                  // session (policy 2) builds no lists and has it from the rows alone
   int group_L = 1;                // problems b = g * group_L + l share the data of partition g (the lambdas of one partition)
   int k1_fused = 0;               // the fused multi-lambda CSR K1 runs (segment lists present): one launch, grid (sg_S, nprob / group_L)
   int k1f_LP = 1;                 // lambdas padded to 1 / 2 / 4 in the interleaved shared-memory vectors
@@ -153,6 +157,7 @@ struct Batch {
   int self_scale = 0;             // adapt a scalar multiplier of the stale inverse from the secant pairs (wide systems)
   int bfgs_m = BFGS_M_DEFAULT;    // secant pairs in use
   int rebuild_is_expensive = 0;   // cost model: Gram + Cholesky + inverse vs one K1 pass (set in batch_alloc)
+  int matfree = 0;                // Newton-CG directions from Hv passes: no Gram, factor or inverse is allocated (set in batch_alloc)
   std::vector<Problem> h;
   Problem* d = nullptr;
   Problem* d_compact = nullptr;   // large batches: Problem structs of the problems that may rebuild in the next slot
@@ -219,8 +224,20 @@ int dev_alloc(Batch& B, void** p, size_t bytes, bool zero = true) {
   return 0;
 }
 
+// Bytes the Gram path allocates for a batch beyond the O(D') solver state: split-K Gram partials (one slice at least), the fp64
+// factor, L^-1 and H^-1, the diagonal-block side buffers, the bf16 Y of wide systems and the e4m3 operands (~26 D'^2 per problem).
+static double gram_path_bytes(const Batch& B) {
+  const double Dp = round_up(B.ldx, 128), ldh = round_up(B.Dt, 32);
+  double per = Dp * Dp * 4.0 + 3.0 * ldh * ldh * 8.0 + 2.0 * ldh * 32 * 8.0 + (ldh > 2048 ? ldh * ldh * 2.0 : 0.0);
+  double bytes = per * B.nprob;
+  for (auto& p : B.h) bytes += (double)p.bm_entries;
+  return bytes;
+}
+
 // Allocate the per-problem solver state.  Data pointers (X, y, ...) and n must be filled in h[] first.
-int batch_alloc(Batch& B, int num_sms) {
+// hessian_policy 2 builds the batch matrix-free (Newton-CG on Hv passes, O(D') state per problem); with any other policy the batch
+// is built matrix-free when what the Gram path would allocate exceeds the free device memory (it could not run at all).
+int batch_alloc(Batch& B, int num_sms, int hessian_policy) {
   const int nprob = B.nprob, ldx = B.ldx;
   B.Dp = round_up(B.ldx, 128);
   B.ldh = round_up(B.Dt, 32);
@@ -243,9 +260,14 @@ int batch_alloc(Batch& B, int num_sms) {
   }
   B.gram_from_csr = B.csr ? 1 : 0;
   for (auto& p : B.h) if (!p.bm_offs) B.gram_from_csr = 0;
+  B.csr_fx = B.gram_from_csr;
+  if (hessian_policy == 2 && B.csr) {
+    B.csr_fx = 1;
+    for (auto& p : B.h) if (!p.csr_unique) B.csr_fx = 0;
+  }
   // fused multi-lambda CSR K1: every problem has segment lists, the groups are whole, and the shared-memory vectors fit
   B.k1_fused = 0;
-  if (B.csr && B.gram_from_csr && B.group_L >= 1 && B.group_L <= 4 && nprob % B.group_L == 0 && !getenv("MLEASE_NO_FUSED_K1")) {
+  if (B.csr && B.csr_fx && B.group_L >= 1 && B.group_L <= 4 && nprob % B.group_L == 0 && !getenv("MLEASE_NO_FUSED_K1")) {
     bool ok = true;
     for (auto& p : B.h) if (!p.sg_perm || p.sg_S != B.h[0].sg_S || p.sg_rows != B.h[0].sg_rows) ok = false;
     if (ok) {
@@ -255,6 +277,23 @@ int batch_alloc(Batch& B, int num_sms) {
     }
   }
   const int gpart_rows = B.k1_fused ? 1 : B.k1_grid;   // the fused kernel keeps its partials in gpart_f (fp32)
+  // Hv passes are modes of the deterministic CSR K1 kernels (sorted unique rows, fixed-point or segment-list accumulation)
+  if (hessian_policy == 2 && !B.csr)
+    return fail(MLEASE_ERR_INVALID, "hessian_policy 2 (matrix-free Newton-CG) needs CSR partitions; dense partitions (at most 4095 features) use the Gram path");
+  if (hessian_policy == 2 && !B.csr_fx)
+    return fail(MLEASE_ERR_INVALID, "hessian_policy 2 (matrix-free Newton-CG) needs CSR rows with strictly increasing column ids");
+  B.matfree = hessian_policy == 2 ? 1 : 0;
+  if (!B.matfree && B.csr && B.gram_from_csr) {
+    // the Gram path's bytes plus the O(D') state allocated with it (vectors, L-BFGS pairs, per-CTA partials, sqrt(d) per row) and
+    // a margin for the session's own vectors: a Gram path that would only just fit is not taken
+    double state = 0;
+    for (auto& p : B.h) state += 8.0 * (double)p.n;
+    state += (double)nprob * (8.0 * ((9 + 2 * BFGS_M + gpart_rows) * (double)ldx + B.k1_grid + 8) + 16.0 * ldx +
+                              (B.k1_fused ? 4.0 * B.k1_grid * ldx : 0.0));
+    size_t free_b = 0, total_b = 0;
+    CK(cudaMemGetInfo(&free_b, &total_b));
+    if (gram_path_bytes(B) + state + (256.0 * 1024 * 1024) > (double)free_b) B.matfree = 1;
+  }
   // Cost model for the rebuild policy (seconds, order of magnitude only: the policy compares the two with a factor of 8): one K1
   // pass streams the partition at ~5 TB/s; a rebuild is n*Dt^2 flop at ~1 PFLOP/s (tensor-core Gram, lower triangle) plus
   // ~Dt^3 fp64 flop at ~5 TFLOP/s (Cholesky + inverse).
@@ -265,7 +304,7 @@ int batch_alloc(Batch& B, int num_sms) {
     const double t_rebuild = (double)maxn * B.Dt * B.Dt / 1e15 + (double)B.Dt * B.Dt * B.Dt / 5e12 + 300e-6;
     // only wide systems qualify: small ones (NaiveTrain's per-key fits, cold-started every time) are launch-bound, not
     // flop-bound, and a mid-update rebuild saves them many lock-step slots
-    B.rebuild_is_expensive = (t_rebuild > 8.0 * t_pass && B.Dt > 2048) ? 1 : 0;
+    B.rebuild_is_expensive = (t_rebuild > 8.0 * t_pass && B.Dt > 2048 && !B.matfree) ? 1 : 0;
     B.self_scale = B.rebuild_is_expensive;
     if (const char* e = getenv("MLEASE_SELF_SCALE")) B.self_scale = atoi(e) ? 1 : 0;   // tuning experiments only
     B.bfgs_m = BFGS_M_DEFAULT;   // measured at 1M x 10k x 1 %: 12 / 16 pairs save 2-4 % of the K1 passes and cost 45-60 % more two-loop time
@@ -273,10 +312,10 @@ int batch_alloc(Batch& B, int num_sms) {
   }
   // Gram decomposition
   constexpr int MAX_TILES = 1 << 18;   // lower 128x128 tiles of Dp up to ~90k
-  std::vector<short> tiles(2 * (size_t)MAX_TILES);
-  B.ntiles = gram_tile_list(B.Dp, tiles.data(), MAX_TILES, B.gram_from_csr);
-  if (B.ntiles <= 0) return fail(MLEASE_ERR_INVALID, "Gram tile list overflow");
-  {
+  std::vector<short> tiles(B.matfree ? 2 : 2 * (size_t)MAX_TILES);
+  B.ntiles = B.matfree ? 0 : gram_tile_list(B.Dp, tiles.data(), MAX_TILES, B.gram_from_csr);
+  if (B.ntiles <= 0 && !B.matfree) return fail(MLEASE_ERR_INVALID, "Gram tile list overflow");
+  if (!B.matfree) {
     const long long ksteps = (maxn + 63) / 64;
     const long long base = (long long)B.ntiles * nprob;   // CTAs
     const long long cap = std::max(1, num_sms);
@@ -293,23 +332,26 @@ int batch_alloc(Batch& B, int num_sms) {
     while (best > 1 && (double)best * B.Dp * B.Dp * 4.0 * nprob > 1024.0 * 1024 * 1024) best--;
     B.gram_slices = best;
   }
-  const size_t nd = (size_t)nprob * ((9 + 2 * BFGS_M) * (size_t)ldx + 2 * BFGS_M + (size_t)gpart_rows * ldx + (size_t)B.k1_grid + 8);
+  // matrix-free: the CG vectors r, p, z, Hp and diag(H) per problem instead of the L-BFGS pairs (no secant pairs are kept there)
+  const size_t nd = (size_t)nprob * ((9 + (B.matfree ? 5 : 2 * BFGS_M)) * (size_t)ldx + 2 * BFGS_M + (size_t)gpart_rows * ldx + (size_t)B.k1_grid + 8);
   const size_t nf = (size_t)nprob * 4 * ldx;
-  double* dd; float* ff; float* hp; double* lc; double* ld; double* ldi; double* yi; double* hi;
+  double* dd; float* ff; float* hp = nullptr; double* lc = nullptr; double* ld = nullptr; double* ldi = nullptr; double* yi = nullptr; double* hi = nullptr;
   if (int rc = dev_alloc(B, (void**)&dd, nd * sizeof(double))) return rc;
   if (int rc = dev_alloc(B, (void**)&ff, nf * sizeof(float))) return rc;
   float* gpf = nullptr;
   if (B.k1_fused)
     if (int rc = dev_alloc(B, (void**)&gpf, (size_t)nprob * B.k1_grid * ldx * sizeof(float))) return rc;
-  if (int rc = dev_alloc(B, (void**)&hp, (size_t)nprob * B.gram_slices * B.Dp * B.Dp * sizeof(float))) return rc;
-  if (int rc = dev_alloc(B, (void**)&lc, (size_t)nprob * B.ldh * B.ldh * sizeof(double))) return rc;
-  if (int rc = dev_alloc(B, (void**)&ld, (size_t)nprob * B.ldh * 32 * sizeof(double))) return rc;
-  if (int rc = dev_alloc(B, (void**)&ldi, (size_t)nprob * B.ldh * 32 * sizeof(double))) return rc;
-  if (int rc = dev_alloc(B, (void**)&yi, (size_t)nprob * B.ldh * B.ldh * sizeof(double))) return rc;
-  if (int rc = dev_alloc(B, (void**)&hi, (size_t)nprob * B.ldh * B.ldh * sizeof(double))) return rc;
   __nv_bfloat16* hif = nullptr;
-  if (B.ldh > 2048)
-    if (int rc = dev_alloc(B, (void**)&hif, (size_t)nprob * B.ldh * B.ldh * sizeof(__nv_bfloat16))) return rc;
+  if (!B.matfree) {
+    if (int rc = dev_alloc(B, (void**)&hp, (size_t)nprob * B.gram_slices * B.Dp * B.Dp * sizeof(float))) return rc;
+    if (int rc = dev_alloc(B, (void**)&lc, (size_t)nprob * B.ldh * B.ldh * sizeof(double))) return rc;
+    if (int rc = dev_alloc(B, (void**)&ld, (size_t)nprob * B.ldh * 32 * sizeof(double))) return rc;
+    if (int rc = dev_alloc(B, (void**)&ldi, (size_t)nprob * B.ldh * 32 * sizeof(double))) return rc;
+    if (int rc = dev_alloc(B, (void**)&yi, (size_t)nprob * B.ldh * B.ldh * sizeof(double))) return rc;
+    if (int rc = dev_alloc(B, (void**)&hi, (size_t)nprob * B.ldh * B.ldh * sizeof(double))) return rc;
+    if (B.ldh > 2048)
+      if (int rc = dev_alloc(B, (void**)&hif, (size_t)nprob * B.ldh * B.ldh * sizeof(__nv_bfloat16))) return rc;
+  }
   if (int rc = dev_alloc(B, (void**)&B.d_ctrl, (size_t)nprob * sizeof(Ctrl))) return rc;
   if (int rc = dev_alloc(B, (void**)&B.d, (size_t)nprob * sizeof(Problem))) return rc;
   if (nprob > 64)
@@ -322,9 +364,9 @@ int batch_alloc(Batch& B, int num_sms) {
   size_t pool_bytes = 0;
   for (int b = 0; b < nprob; b++) {
     pool_off[b] = pool_bytes;
-    const bool windows = B.gram_from_csr && k1_csr_window(ldx) > 0;   // then a second [n] vector (row residuals) follows sdvec
-    // CSR: sdvec (+ rvec), then the e4m3 operand bytes of the entry list
-    const size_t need = B.gram_from_csr ? (((size_t)B.h[b].n * sizeof(float) * (windows ? 2 : 1) + 255) & ~(size_t)255) + (size_t)B.h[b].bm_entries
+    const bool windows = B.csr_fx && k1_csr_window(ldx) > 0;   // then a second [n] vector (row residuals) follows sdvec
+    // CSR: sdvec (+ rvec), then the e4m3 operand bytes of the entry list (none in a matrix-free batch)
+    const size_t need = B.csr_fx ? (((size_t)B.h[b].n * sizeof(float) * (windows ? 2 : 1) + 255) & ~(size_t)255) + (B.matfree ? 0 : (size_t)B.h[b].bm_entries)
                                         : (B.h[b].Xt ? 0 : (size_t)B.h[b].n * B.Dp * sizeof(__nv_bfloat16));
     pool_bytes += (need + 255) & ~(size_t)255;
   }
@@ -339,29 +381,32 @@ int batch_alloc(Batch& B, int num_sms) {
     p.beta = q; q += ldx; p.beta_t = q; q += ldx; p.m = q; q += ldx; p.q = q; q += ldx;
     p.g_t = q; q += ldx; p.g_acc = q; q += ldx; p.dir = q; q += ldx; p.x_d = q; q += ldx;
     p.qf = reinterpret_cast<float*>(q); p.tf = p.qf + ldx; q += ldx;   // one double-vector slot holds the two fp32 vectors of the triangular GEMVs
-    p.bfgs_S = q; q += (size_t)BFGS_M * ldx; p.bfgs_Y = q; q += (size_t)BFGS_M * ldx; p.bfgs_rho = q; q += BFGS_M; p.bfgs_alpha = q; q += BFGS_M;
+    if (!B.matfree) { p.bfgs_S = q; q += (size_t)BFGS_M * ldx; p.bfgs_Y = q; q += (size_t)BFGS_M * ldx; }
+    p.bfgs_rho = q; q += BFGS_M; p.bfgs_alpha = q; q += BFGS_M;
     p.gpart = q; q += (size_t)gpart_rows * ldx;
+    p.hv_vf = p.qf;
+    if (B.matfree) { p.cg_r = q; q += ldx; p.cg_p = q; q += ldx; p.cg_z = q; q += ldx; p.cg_Hp = q; q += ldx; p.cg_diag = q; q += ldx; }
     p.gpart_f = gpf ? gpf + (size_t)b * B.k1_grid * ldx : nullptr;
     p.fpart = q; q += B.k1_grid + 8;
     dd = q;
     float* f = ff;
     p.beta_tf = f; f += ldx; p.u_f = f; f += ldx; p.uplusx_f = f; f += ldx; p.x_f = f; f += ldx;
     ff = f;
-    p.Hpart = hp + (size_t)b * B.gram_slices * B.Dp * B.Dp;
-    p.Lc = lc + (size_t)b * B.ldh * B.ldh;
-    p.Ldiag = ld + (size_t)b * B.ldh * 32;
-    p.Ldinv = ldi + (size_t)b * B.ldh * 32;
-    p.Yinv = yi + (size_t)b * B.ldh * B.ldh;
-    p.Hinv = hi + (size_t)b * B.ldh * B.ldh;
+    p.Hpart = hp ? hp + (size_t)b * B.gram_slices * B.Dp * B.Dp : nullptr;
+    p.Lc = lc ? lc + (size_t)b * B.ldh * B.ldh : nullptr;
+    p.Ldiag = ld ? ld + (size_t)b * B.ldh * 32 : nullptr;
+    p.Ldinv = ldi ? ldi + (size_t)b * B.ldh * 32 : nullptr;
+    p.Yinv = yi ? yi + (size_t)b * B.ldh * B.ldh : nullptr;
+    p.Hinv = hi ? hi + (size_t)b * B.ldh * B.ldh : nullptr;
     p.Ysym = hif ? hif + (size_t)b * B.ldh * B.ldh : nullptr;
     p.ctrl = B.d_ctrl + b;
     // Gram operand state, carved out of ONE allocation for the whole batch (NaiveTrain batches hold thousands of problems:
     // one cudaMalloc / cudaFree each would cost more than the fits)
-    if (B.gram_from_csr) {
+    if (B.csr_fx) {
       p.sdvec = reinterpret_cast<float*>(pool + pool_off[b]);
       p.rvec = k1_csr_window(ldx) > 0 ? p.sdvec + p.n : nullptr;
-      p.bm_e4m3 = pool + pool_off[b] + (((size_t)p.n * sizeof(float) * (p.rvec ? 2 : 1) + 255) & ~(size_t)255);
-      p.gram_from_csr = 1;
+      p.bm_e4m3 = B.matfree ? nullptr : pool + pool_off[b] + (((size_t)p.n * sizeof(float) * (p.rvec ? 2 : 1) + 255) & ~(size_t)255);
+      p.gram_from_csr = B.gram_from_csr;
       std::memset(&maps[b], 0, sizeof(CUtensorMap));
     } else {
       p.gram_from_csr = 0;
@@ -375,11 +420,14 @@ int batch_alloc(Batch& B, int num_sms) {
   return 0;
 }
 
-// K1 of a slot: the fused multi-lambda CSR kernel when the batch has segment lists, the per-problem kernels otherwise
-cudaError_t batch_k1(Batch& B, int force_emit, cudaStream_t st, int* launches) {
+// K1 of a slot: the fused multi-lambda CSR kernel when the batch has segment lists, the per-problem kernels otherwise.
+// mode K1_HV / K1_DIAG: the Hessian-vector / Hessian-diagonal pass of the problems with Ctrl::cg_active (CSR batches whose rows
+// are sorted and unique only).
+cudaError_t batch_k1(Batch& B, int force_emit, cudaStream_t st, int* launches, int mode = K1_GRAD) {
+  if (mode != K1_GRAD && !(B.csr && B.csr_fx)) return cudaErrorInvalidValue;
   if (B.k1_fused)
-    return k1f_launch(B.d, B.nprob / B.group_L, B.group_L, B.h[0].sg_S, B.k1f_LP, B.k1f_smem, B.has_bias, force_emit, st, launches);
-  return k1_launch(B.d, B.nprob, B.csr, B.ldx, B.has_bias, B.k1_grid, force_emit, st, launches, B.gram_from_csr, B.k1_dyn);
+    return k1f_launch(B.d, B.nprob / B.group_L, B.group_L, B.h[0].sg_S, B.k1f_LP, B.k1f_smem, B.has_bias, force_emit, st, launches, mode);
+  return k1_launch(B.d, B.nprob, B.csr, B.ldx, B.has_bias, B.k1_grid, force_emit, st, launches, B.csr_fx, B.k1_dyn, mode);
 }
 
 // One x-update for every problem of the batch: beta (init), m, q must already be on the device.
@@ -388,6 +436,7 @@ int batch_xupdate(Batch& B, cudaStream_t st, double xtol, int max_newton, int po
   Profiler nop;
   Profiler& pf = prof ? *prof : nop;
   int launches = 0;
+  if (B.matfree) policy = 2;   // also when the batch was made matrix-free by the memory rule
   CK(newton_begin(B.d, B.nprob, xtol, max_newton, policy, invalidate, B.rebuild_is_expensive, st, &launches, B.bfgs_m, B.self_scale));
   // The first slot's flags are known on the host: every problem is running, and a rebuild is due iff the policy says
   // always, the factors were invalidated, or the mirrored control blocks say so (no factor yet / refresh requested).
@@ -396,7 +445,7 @@ int batch_xupdate(Batch& B, cudaStream_t st, double xtol, int max_newton, int po
   {
     bool emit0 = policy == 1 || invalidate || B.mirror.empty();
     for (auto& c : B.mirror) if (!c.hess_valid || c.refresh_next) emit0 = true;
-    if (emit0) flag |= 2;
+    if (emit0 && !B.matfree) flag |= 2;
   }
   B.mirror.resize(B.nprob);
   std::vector<Ctrl>& hc = B.mirror;
@@ -404,10 +453,36 @@ int batch_xupdate(Batch& B, cudaStream_t st, double xtol, int max_newton, int po
   const Problem* d_hess = B.d;   // problems the Gram / Cholesky grids run over (large batches: compacted by poll2_kernel)
   int n_hess = B.nprob;
   double shared_flops = 0;   // Gram builds that were not run because the group's first problem stood in for them
+  // Matrix-free direction of the problems that accepted a point this slot: diagonal pass, then CG steps in chunks of CG_CHUNK
+  // (Hv pass -> fixed-order reduction -> CG update each), one pinned read-back of the "any CG running" flag per chunk.
+  // Problems whose CG has finished return at once from every kernel of a chunk.
+  auto mf_direction = [&]() -> int {
+    constexpr int CG_CHUNK = 4;
+    pf.begin(2, st);
+    CK(cg_begin(B.d, B.nprob, st, &launches));
+    CK(batch_k1(B, 0, st, &launches, K1_DIAG));
+    CK(hv_reduce(B.d, B.nprob, B.Dt, 2, st, &launches));
+    CK(cg_init(B.d, B.nprob, B.Dt, st, &launches));
+    pf.end(st);
+    for (int steps = 0; steps < CG_MAX_STEPS; steps += CG_CHUNK) {
+      for (int j = 0; j < CG_CHUNK; j++) {
+        pf.begin(2, st);
+        CK(batch_k1(B, 0, st, &launches, K1_HV));
+        CK(hv_reduce(B.d, B.nprob, B.Dt, 1, st, &launches));
+        CK(cg_step(B.d, B.nprob, B.Dt, st, &launches));
+        pf.end(st);
+      }
+      CK(cg_poll(B.d, B.nprob, d_flag + 2, st, &launches));
+      CK(cudaMemcpyAsync(h_flag + 2, d_flag + 2, sizeof(int), cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
+      if (!h_flag[2]) break;
+    }
+    return 0;
+  };
   // One slot's launches.  with_hess: the Gram / Cholesky launches of a rebuild are included; spec: see k1_reduce_decide_kernel.
   auto enqueue_slot = [&](int slot_idx, bool with_hess, bool spec) -> int {
     pf.begin(0, st);
-    CK(batch_k1(B, -1, st, &launches));
+    CK(batch_k1(B, B.matfree ? 1 : -1, st, &launches));   // matrix-free: every pass leaves sqrt(d) of its point for the Hv passes
     pf.end(st);
     pf.begin(1, st);
     CK(k1_reduce_decide(B.d, B.nprob, B.Dt, st, &launches, spec ? 1 : 0));
@@ -438,8 +513,11 @@ int batch_xupdate(Batch& B, cudaStream_t st, double xtol, int max_newton, int po
       }
       pf.end(st);
     }
+    if (B.matfree)
+      if (int rc = mf_direction()) return rc;
     pf.begin(1, st);
-    CK(newton_solve(B.d, B.nprob, B.ldh, st, &launches, B.group_L));
+    if (B.matfree) CK(newton_finish(B.d, B.nprob, B.Dt, st, &launches));
+    else CK(newton_solve(B.d, B.nprob, B.ldh, st, &launches, B.group_L));
     if (!small) { poll2_kernel<<<1, 256, 0, st>>>(B.d, B.nprob, d_flag, B.d_compact); launches++; }
     pf.end(st);
     return 0;
@@ -629,7 +707,7 @@ void fill_problem_data(Problem& p, const PartData& pd) {
   p.rowptr = pd.rowptr; p.colidx = pd.colidx; p.vals = pd.vals; p.nnz_hint = pd.nnz; p.csr_unique = pd.csr_unique;
   p.bm_offs = pd.bm_offs; p.bm_keys = pd.bm_keys; p.bm_vals = pd.bm_vals; p.bm_groups = pd.bm_groups; p.bm_entries = pd.bm_entries;
   p.nblk128 = pd.nblk128; p.gram_from_csr = pd.bm_offs ? 1 : 0;
-  p.vmax = pd.vmax; p.wmax = pd.wmax;
+  p.vmax = pd.vmax; p.wmax = pd.wmax; p.rowl1 = pd.rowl1;
   p.sg_S = pd.sg_S; p.sg_rows = pd.sg_rows; p.sg_ngrp = pd.sg_ngrp; p.sg_perm = pd.sg_perm; p.sg_depth = pd.sg_depth; p.sg_goff = pd.sg_goff;
   p.sg_row16 = pd.sg_row16; p.sg_val = pd.sg_val;
   p.gram_scale = 1.f; p.gram_unscale = 1.f;
@@ -666,7 +744,7 @@ int finalize(mlease_session* s) {
       fill_problem_data(p, s->parts[pi]);
       p.lambda_idx = l; p.part_local = (int)pi;
     }
-  if (int rc = batch_alloc(*B, s->num_sms)) return rc;
+  if (int rc = batch_alloc(*B, s->num_sms, s->cfg.hessian_policy)) return rc;
   const size_t ldv = s->ldx;
   if (int rc = sess_alloc(s, (void**)&s->d_z, s->L * ldv * sizeof(double))) return rc;
   if (int rc = sess_alloc(s, (void**)&s->d_wz, s->L * ldv * sizeof(double))) return rc;
@@ -708,7 +786,7 @@ int ensure_scratch(mlease_session* s, int part_idx) {
   B->h.resize(1);
   fill_problem_data(B->h[0], s->parts[part_idx]);
   s->scratch_part = part_idx;
-  return batch_alloc(*B, s->num_sms);
+  return batch_alloc(*B, s->num_sms, s->cfg.hessian_policy);
 }
 
 double rho_eff_for_iter(mlease_session* s, int l, int iter) {
@@ -941,9 +1019,15 @@ static int csr_build_layout(mlease_session* s, PartData& pd) {
   CK(cudaStreamSynchronize(s->stream));
   std::memcpy(&pd.vmax, s->h_flag, 4);
   pd.csr_unique = s->h_flag[1] ? 0 : 1;
+  CK(cudaMemsetAsync(s->d_flag, 0, 4, s->stream));
+  CK(csr_row_l1_max(nrows, pd.rowptr, pd.vals, (unsigned*)s->d_flag, s->stream));
+  CK(cudaMemcpyAsync(s->h_flag, s->d_flag, 4, cudaMemcpyDeviceToHost, s->stream));
+  CK(cudaStreamSynchronize(s->stream));
+  std::memcpy(&pd.rowl1, s->h_flag, 4);
   // the Gram producers index the entry list with 32 bits; the list holds one bias entry per row (session batches always have the
   // intercept, column Dg)
-  if (pd.csr_unique && pd.nnz + nrows < (1LL << 32) - 64) {
+  // A matrix-free session (hessian_policy 2) builds no Gram, so it skips the block-major list (n D'/512 offsets + 6 B per entry)
+  if (pd.csr_unique && pd.nnz + nrows < (1LL << 32) - 64 && s->cfg.hessian_policy != 2) {
     pd.nblk128 = round_up(s->ldx, 128) / 128;
     pd.bm_groups = (nrows + 31) / 32;
     pd.bm_entries = pd.nnz + nrows;
@@ -954,6 +1038,8 @@ static int csr_build_layout(mlease_session* s, PartData& pd) {
     CK(csr_bm_offsets(nrows, pd.rowptr, pd.colidx, s->Dg, pd.nblk128, pd.bm_groups, (long long*)bo, s->stream));
     CK(csr_bm_fill(nrows, pd.rowptr, pd.colidx, pd.vals, s->Dg, pd.nblk128, pd.bm_groups, (const long long*)bo, (unsigned short*)bk, (float*)bv, s->stream));
     pd.bm_offs = (long long*)bo; pd.bm_keys = (unsigned short*)bk; pd.bm_vals = (float*)bv;
+  }
+  if (pd.csr_unique && pd.nnz + nrows < (1LL << 32) - 64) {
     // segment lists of the fused multi-lambda K1
     int S = 0, rows = 0, LP = 0; size_t smem = 0;
     if (!getenv("MLEASE_NO_FUSED_K1") && k1f_plan(nrows, s->ldx, s->L, s->num_sms, &S, &rows, &LP, &smem)) {
@@ -1288,6 +1374,7 @@ int mlease_objective(mlease_session* s, int32_t pid, const double* w, const doub
   CK(cudaStreamSynchronize(s->stream));
   if (f) *f = c.f_t;
   if (H) {
+    if (B->matfree) return fail(MLEASE_ERR_INVALID, "this session's problems are matrix-free (hessian_policy 2, or a Hessian too large for the device): use mlease_hessian_vector");
     if (!tensor && B->gram_from_csr) return fail(MLEASE_ERR_INVALID, "the SIMT debug Gram needs the dense bf16 operand, which CSR partitions with sorted unique rows do not materialise");
     if (tensor && B->gram_from_csr) CK(gram_launch_csr_wgmma(B->d, 1, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches, 0));
     else if (tensor) CK(gram_launch_wgmma(B->d, 1, B->d_tmaps, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches));
@@ -1353,6 +1440,7 @@ int mlease_posterior_variance(mlease_session* s, int32_t pid, const double* w, c
   if (int rc = ensure_scratch(s, pi)) return rc;
   Batch* B = s->scratch;
   const Problem& p = B->h[0];
+  if (full && B->matfree) return fail(MLEASE_ERR_INVALID, "the full posterior variance needs the Hessian matrix, which a matrix-free session does not form");
   if (full && B->csr && !s->parts[pi].csr_unique)
     return fail(MLEASE_ERR_INVALID, "the full Hessian needs rows with strictly increasing column ids (llf/LogisticRegressionL2.java:277)");
   std::vector<double> zero(s->Dt, 0.0);
@@ -1394,6 +1482,84 @@ int mlease_posterior_variance(mlease_session* s, int32_t pid, const double* w, c
   return 0;
 }
 
+int mlease_hessian_vector(mlease_session* s, int32_t pid, const double* w, const double* q, const double* v, double* out) {
+  if (!s || !w || !q || !v || !out) return fail(MLEASE_ERR_INVALID, "null argument");
+  CK(cudaSetDevice(s->cfg.device));
+  const int pi = find_part(s, pid);
+  if (pi < 0) return fail(MLEASE_ERR_INVALID, "partition not resident in this session");
+  if (int rc = ensure_scratch(s, pi)) return rc;
+  Batch* B = s->scratch;
+  if (!(B->csr && B->csr_fx)) return fail(MLEASE_ERR_INVALID, "Hessian-vector products need CSR rows with strictly increasing column ids");
+  std::vector<double> zero(s->Dt, 0.0);
+  if (int rc = scratch_set(s, w, zero.data(), q)) return rc;
+  const Problem& p = B->h[0];
+  int launches = 0;
+  // one gradient pass at w leaves sqrt(d) in sdvec; the Hv pass multiplies the fp32 copy of v (hv_vf) with X^T D X
+  CK(newton_begin(B->d, 1, 1e-8, 1, 1, 1, 0, s->stream, &launches));
+  CK(batch_k1(*B, 1, s->stream, &launches));
+  std::vector<float> vf(s->ldx, 0.f);
+  float vinf = 0.f;
+  for (int k = 0; k < s->Dt; k++) { vf[k] = (float)v[k]; vinf = std::max(vinf, std::fabs(vf[k])); }
+  CK(cudaMemcpyAsync(p.hv_vf, vf.data(), (size_t)s->ldx * sizeof(float), cudaMemcpyHostToDevice, s->stream));
+  CK(cudaMemcpyAsync(&B->d_ctrl->hv_vinf, &vinf, sizeof(float), cudaMemcpyHostToDevice, s->stream));
+  const int on = 1, off = 0;
+  CK(cudaMemcpyAsync(&B->d_ctrl->cg_active, &on, sizeof(int), cudaMemcpyHostToDevice, s->stream));
+  CK(batch_k1(*B, 0, s->stream, &launches, K1_HV));
+  CK(hv_reduce(B->d, 1, B->Dt, 0, s->stream, &launches));
+  CK(cudaMemcpyAsync(&B->d_ctrl->cg_active, &off, sizeof(int), cudaMemcpyHostToDevice, s->stream));
+  CK(cudaMemcpyAsync(out, p.g_t, (size_t)s->Dt * sizeof(double), cudaMemcpyDeviceToHost, s->stream));
+  CK(cudaStreamSynchronize(s->stream));   // (the stack values above are read by the copies before this returns)
+  for (int k = 0; k < s->Dt; k++) out[k] += q[k] * v[k];   // prior term s / priorVar (llf/LogisticRegressionL2.java:246)
+  s->cnt.launches += launches;
+  return 0;
+}
+
+// Test hook, not part of the C ABI (include/mlease_b200.h does not declare it): one Hv (mode 1) or Hessian-diagonal (mode 2) pass
+// over the session's ADMM batch -- every (partition, lambda) problem at its own point w[b] and vector v[b] (b = local partition * L
+// + lambda, Dt entries each), through the kernels a matrix-free x-update runs (fused multi-lambda or per-problem).  out[b] = the data
+// term X^T D X v resp. sum_i d_i x_ic^2, without the prior.  The batch's x-update state is consumed: begin() again before iterating.
+int mlease_internal_batch_hv(mlease_session* s, int32_t mode, const double* w, const double* v, double* out) {
+  if (!s || !w || !v || !out || (mode != K1_HV && mode != K1_DIAG)) return fail(MLEASE_ERR_INVALID, "bad argument");
+  if (!s->batch) return fail(MLEASE_ERR_STATE, "mlease_admm_begin was not called");
+  CK(cudaSetDevice(s->cfg.device));
+  Batch& B = *s->batch;
+  if (!(B.csr && B.csr_fx)) return fail(MLEASE_ERR_INVALID, "Hessian-vector passes need CSR rows with strictly increasing column ids");
+  const int nprob = B.nprob, ldx = s->ldx, Dt = s->Dt;
+  std::vector<Ctrl> c(nprob);
+  auto set_ctrl = [&](int skip_clear, int active) -> int {
+    CK(cudaMemcpy(c.data(), B.d_ctrl, (size_t)nprob * sizeof(Ctrl), cudaMemcpyDeviceToHost));
+    for (auto& x : c) { if (skip_clear) x.skip_eval = 0; x.cg_active = active; if (active < 0) { x.cg_active = 0; x.done = 1; } }
+    CK(cudaMemcpy(B.d_ctrl, c.data(), (size_t)nprob * sizeof(Ctrl), cudaMemcpyHostToDevice));
+    return 0;
+  };
+  std::vector<double> wb(ldx, 0.0);
+  for (int b = 0; b < nprob; b++) {
+    std::memcpy(wb.data(), w + (size_t)b * Dt, (size_t)Dt * sizeof(double));
+    CK(cudaMemcpy(B.h[b].beta, wb.data(), (size_t)ldx * sizeof(double), cudaMemcpyHostToDevice));
+  }
+  if (int rc = set_ctrl(1, 0)) return rc;
+  int launches = 0;
+  CK(newton_begin(B.d, nprob, 1e-8, 1, 2, 1, 0, s->stream, &launches));   // beta_t = float(w), every problem running
+  CK(batch_k1(B, 1, s->stream, &launches));                               // sqrt(d) at w
+  CK(cudaStreamSynchronize(s->stream));
+  if (int rc = set_ctrl(0, 1)) return rc;
+  std::vector<float> vf(ldx, 0.f);
+  for (int b = 0; b < nprob; b++) {
+    float vinf = 0.f;
+    for (int k = 0; k < Dt; k++) { vf[k] = (float)v[(size_t)b * Dt + k]; vinf = std::max(vinf, std::fabs(vf[k])); }
+    CK(cudaMemcpy(B.h[b].hv_vf, vf.data(), (size_t)ldx * sizeof(float), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(&B.d_ctrl[b].hv_vinf, &vinf, sizeof(float), cudaMemcpyHostToDevice));
+  }
+  CK(batch_k1(B, 0, s->stream, &launches, mode));
+  CK(hv_reduce(B.d, nprob, Dt, 0, s->stream, &launches));
+  CK(cudaStreamSynchronize(s->stream));
+  for (int b = 0; b < nprob; b++) CK(cudaMemcpy(out + (size_t)b * Dt, B.h[b].g_t, (size_t)Dt * sizeof(double), cudaMemcpyDeviceToHost));
+  if (int rc = set_ctrl(0, -1)) return rc;
+  B.mirror.clear();
+  s->cnt.launches += launches;
+  return 0;
+}
+
 int mlease_time_kernel(mlease_session* s, int32_t pid, int32_t which, int32_t reps, int32_t emit_scaled, float* avg_ms) {
   if (!s || !avg_ms || reps <= 0) return fail(MLEASE_ERR_INVALID, "bad argument");
   CK(cudaSetDevice(s->cfg.device));
@@ -1401,6 +1567,8 @@ int mlease_time_kernel(mlease_session* s, int32_t pid, int32_t which, int32_t re
   if (pi < 0) return fail(MLEASE_ERR_INVALID, "partition not resident in this session");
   if (int rc = ensure_scratch(s, pi)) return rc;
   Batch* B = s->scratch;
+  if ((which == 2 || which == 3) && B->matfree) return fail(MLEASE_ERR_INVALID, "a matrix-free session builds no Gram and no factor");
+  if (which == 4 && !(B->csr && B->csr_fx)) return fail(MLEASE_ERR_INVALID, "Hessian-vector passes need CSR rows with strictly increasing column ids");
   std::vector<double> zero(s->Dt, 0.0), one(s->Dt, 1.0);
   if (int rc = scratch_set(s, zero.data(), zero.data(), one.data())) return rc;
   int launches = 0;
@@ -1415,6 +1583,16 @@ int mlease_time_kernel(mlease_session* s, int32_t pid, int32_t which, int32_t re
     Ctrl c; std::memset(&c, 0, sizeof(c)); c.need_hess = 1;
     CK(cudaMemcpyAsync(B->d_ctrl, &c, sizeof(Ctrl), cudaMemcpyHostToDevice, s->stream));
   }
+  const int on = 1, off = 0;
+  if (which == 4) {   // Hv pass at beta = 0 (d from the warm-up pass) of v = 1
+    std::vector<float> vf(s->ldx, 0.f);
+    for (int k = 0; k < s->Dt; k++) vf[k] = 1.f;
+    CK(cudaMemcpyAsync(B->h[0].hv_vf, vf.data(), (size_t)s->ldx * sizeof(float), cudaMemcpyHostToDevice, s->stream));
+    const float vinf = 1.f;
+    CK(cudaMemcpyAsync(&B->d_ctrl->hv_vinf, &vinf, sizeof(float), cudaMemcpyHostToDevice, s->stream));
+    CK(cudaMemcpyAsync(&B->d_ctrl->cg_active, &on, sizeof(int), cudaMemcpyHostToDevice, s->stream));
+    CK(cudaStreamSynchronize(s->stream));
+  }
   CK(cudaStreamSynchronize(s->stream));
   CK(cudaEventRecord(e0, s->stream));
   for (int r = 0; r < reps; r++) {
@@ -1422,10 +1600,12 @@ int mlease_time_kernel(mlease_session* s, int32_t pid, int32_t which, int32_t re
     else if (which == 2 && B->gram_from_csr) CK(gram_launch_csr_wgmma(B->d, 1, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches, 0));
     else if (which == 2) CK(gram_launch_wgmma(B->d, 1, B->d_tmaps, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches));
     else if (which == 3) CK(cholesky_launch(B->d, 1, B->ldh, s->stream, &launches));
-    else return fail(MLEASE_ERR_INVALID, "which must be 1, 2 or 3");
+    else if (which == 4) { CK(batch_k1(*B, 0, s->stream, &launches, K1_HV)); CK(hv_reduce(B->d, 1, B->Dt, 0, s->stream, &launches)); }
+    else return fail(MLEASE_ERR_INVALID, "which must be 1, 2, 3 or 4");
   }
   CK(cudaEventRecord(e1, s->stream));
   CK(cudaEventSynchronize(e1));
+  if (which == 4) CK(cudaMemcpy(&B->d_ctrl->cg_active, &off, sizeof(int), cudaMemcpyHostToDevice));
   float ms = 0;
   CK(cudaEventElapsedTime(&ms, e0, e1));
   cudaEventDestroy(e0); cudaEventDestroy(e1);
@@ -1659,7 +1839,7 @@ int mlease_naive_train(int32_t device, void* stream, int32_t K, int32_t Dg, cons
         p.X = dX + (size_t)krs[k] * ldx;
       }
     }
-    if (int rc = batch_alloc(B, prop.multiProcessorCount)) return rc;
+    if (int rc = batch_alloc(B, prop.multiProcessorCount, 0)) return rc;
     lap("batch_alloc");
     double *dm, *dq, *dout; unsigned char* dmask = nullptr;
     if (int rc = t.get(&dm, (size_t)ldx)) return rc;

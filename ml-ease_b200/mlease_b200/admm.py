@@ -237,6 +237,14 @@ class AdmmSession:
         check(lib().mlease_fit_partition(self._h, partition_id, ptr(x), ptr(m), ptr(q), C.byref(steps)))
         return x, steps.value
 
+    def hessian_vector(self, partition_id, w, prior_precision, v):
+        """LogisticRegressionL2.Hv (llf/LogisticRegressionL2.java:231-248) at w with prior precision q: X^T D(w) X v + q * v,
+        computed by the Hv mode of the CSR K1 kernels (fp32 products, fp64 fixed-order reductions: bitwise repeatable)."""
+        w, q, v = (np.ascontiguousarray(a, np.float64) for a in (w, prior_precision, v))
+        out = np.zeros(self.Dt, np.float64)
+        check(lib().mlease_hessian_vector(self._h, int(partition_id), ptr(w), ptr(q), ptr(v), ptr(out)))
+        return out
+
     def posterior_variance(self, partition_id, w, prior_precision, full=False, want_cov=False):
         """LibLinear.train's computePosteriorVar tail (llf/LibLinear.java:315-334): diagonal (1 / hessianDiagonal) or full
         (diag of the inverse of the exact fp64 Hessian; want_cov also returns H^-1)."""
@@ -257,7 +265,7 @@ class AdmmSession:
 
     def time_kernel(self, partition_id, which, reps=5, emit_scaled=False):
         ms = C.c_float(0)
-        check(lib().mlease_time_kernel(self._h, partition_id, {"k1": 1, "gram": 2, "cholesky": 3}[which], reps, int(emit_scaled), C.byref(ms)))
+        check(lib().mlease_time_kernel(self._h, partition_id, {"k1": 1, "gram": 2, "cholesky": 3, "hv": 4}[which], reps, int(emit_scaled), C.byref(ms)))
         return ms.value
 
 
