@@ -71,6 +71,9 @@ struct Ctrl {
 // gradient pass, read back from sdvec as sqrt(d)^2):  Hv:  column sums of t_i x_i with t_i = d_i (x_i . v) (v = hv_vf, fp32);
 // diagonal:  column sums of d_i x_ic^2 (the Jacobi preconditioner).
 enum { K1_GRAD = 0, K1_HV = 1, K1_DIAG = 2 };
+// CSR Gram kernels (k2_gram.cu): e4m3 wgmma on operand blocks assembled in shared memory, or the exact sparse kernel that forms
+// only the nonzero products of each row.  batch_alloc picks one per batch from the data.
+enum { CSR_GRAM_WGMMA = 1, CSR_GRAM_SPARSE = 2 };
 
 // One problem's device pointers.  Vectors have length ldv (= ldx, multiple of 4, >= Dt) and are
 // zero in [Dt, ldv).  The bias column is PHYSICAL: column Dt-1 of X is 1.0f for every row when the
@@ -109,7 +112,9 @@ struct Problem {
   float* gpart_f;                   // [sg_S][ldx] per-segment partial gradients when the fused K1 runs (else NULL; gpart is used)
   float* sdvec;            // [n] sqrt(d_i) written by K1 when the Gram is assembled straight from CSR (no Xt)
   float* rvec;             // [n] row residuals r_i, only for CSR partitions wider than one K1 column window (else NULL)
-  int gram_from_csr;       // 1: gram_csr_wgmma_kernel builds the operand tiles in shared memory from the sparse rows
+  int gram_from_csr;       // 1: the Gram is built from the block-major entry list (no dense bf16 operand)
+  int csr_gram;            // which kernel builds it then: CSR_GRAM_WGMMA or CSR_GRAM_SPARSE (0 otherwise)
+  double gram_pairs;       // products of one sparse build, sum over rows of (k_i + 1)(k_i + 2) / 2 (host-side accounting only)
   float gram_scale;        // CSR Gram operands are e4m3: sqrt(d) x is multiplied by this power of two before rounding ...
   float gram_unscale;      // ... and the Gram sums by 1 / gram_scale^2 in chol_prep (1 for the bf16 dense-operand path)
   __nv_bfloat16* Xt;       // [n][Dp] bf16 = sqrt(d_i) * x_ij  (Gram operand), zero in [ldx, Dp)

@@ -14,6 +14,10 @@
 // Warpgroup roles (384 threads): warpgroup 0 = TMA producer (one lane), warpgroups 1-2 = consumers,
 // each issuing m64n256k16 wgmma for its 64 rows of the tile (128 fp32 accumulators a thread).
 //
+// CSR partitions have two kernels on the same e4m3 operand bytes: gram_csr_wgmma_kernel (operand blocks assembled in shared
+// memory, wgmma) and gram_csr_sparse_kernel (only the nonzero products of each row, exact int64 sums).  session.cu batch_alloc
+// picks one per batch from the data: the sparse one wins below about 3 % density at 10k features.
+//
 // A fp32 SIMT kernel computing the same partials from the same bf16 operand is kept ONLY as a
 // debug cross-check reachable through mlease_objective(tensor=0); the product path never uses it.
 #include <cuda.h>
@@ -395,6 +399,166 @@ __global__ void __launch_bounds__(256) gram_csr_operand_kernel(const Problem* __
   }
 }
 
+// ------------------------------------------------------------------------------------------
+// Sparse CSR Gram: the same partial from the same e4m3 operand bytes, but only the nonzero products of each row are formed.  At
+// 1 % density a 32-row x 128-column operand block holds ~1 % nonzeros, so the wgmma kernel above spends ~10^4 multiply-adds per
+// nonzero product; here each product is one integer multiply and (mostly) one native shared-memory atomic add.
+// Exact and deterministic: an e4m3 value is an integer number of units of 2^-9 (|v| <= 448 = 229376 units < 2^18), so a product
+// is an integer number of units of 2^-18 below 2^35.6, and the tile accumulates them as int64 (integer addition is associative:
+// the sum does not depend on the warp schedule).  A 64-bit shared atomic add is a compare-and-swap loop on sm_90a, so each cell
+// is a pair of 32-bit words: the product's low word goes in with a native ATOMS.ADD that returns the old word, and its high word
+// plus the carry out of the low add (old + lo < old) goes into the high word -- skipped when that is 0, which is the usual case
+// for |product| < 2^32 of either sign.  The pair holds the two's complement int64 sum exactly.  The epilogue rounds each cell
+// once to fp32.  The sum cannot overflow below
+// 2^27.4 rows (every row adds at most one product to a cell: rows have unique columns); gram_sparse_max_rows() states the limit
+// the batch rule applies.
+// One CTA per (128 x 128 lower tile (bi, bj), problem), one slice.  Each warp takes every SP_WARPS-th 32-row group; per group it
+// stages the bj run (row order: csr_bm_fill_kernel writes lane 0's entries, then lane 1's, ...) in shared memory with the start
+// and end of each row's entries, then every entry of the bi run multiplies the staged entries of its own row.  Diagonal tiles
+// use the pairs with c2 <= c1 only (the columns of a row's run increase) and mirror them in the epilogue.  Zero operand bytes
+// are skipped.  A bj run longer than SP_STAGE entries is staged in chunks, the bi run re-read for each.
+// ------------------------------------------------------------------------------------------
+constexpr int SP_THREADS = 1024;
+constexpr int SP_WARPS = SP_THREADS / 32;
+constexpr int SP_STAGE = 256;                                      // staged bj entries per warp and chunk
+constexpr size_t SP_ACC_BYTES = (size_t)SN * SN * 2 * sizeof(uint32_t);   // 128 KB: low words, then high words
+constexpr size_t SP_SMEM = SP_ACC_BYTES + (size_t)SP_WARPS * SP_STAGE * 4 + (size_t)SP_WARPS * 64 * 2;
+
+// e4m3 byte -> signed integer number of units of 2^-9 (subnormal m: m units; normal (e, m): (8 + m) << (e - 1)).  0x7F / 0xFF
+// (NaN) never occur: the operand pass converts with __NV_SATFINITE.
+__device__ __forceinline__ int e4m3_units(uint32_t b) {
+  const int e = (int)((b >> 3) & 15u), m = (int)(b & 7u);
+  const int mag = e ? (8 | m) << (e - 1) : m;
+  return (b & 0x80u) ? -mag : mag;
+}
+
+__global__ void __launch_bounds__(SP_THREADS, 1)
+gram_csr_sparse_kernel(const Problem* __restrict__ probs, const GramTile* __restrict__ tiles, int force, int share) {
+  if (share > 1 && blockIdx.z % share != 0) return;   // see gram_wgmma_kernel
+  const Problem& pb = probs[blockIdx.z];
+  Ctrl* ctrl = pb.ctrl;
+  if (!force && (ctrl->done || !ctrl->need_hess)) return;
+  const GramTile tile = tiles[blockIdx.x];
+  const int bi = tile.bi, bj = tile.bj;
+  const bool diag = bi == bj;
+  const int Dp = pb.Dp;
+  const long long ngroups = pb.bm_groups;
+
+  extern __shared__ __align__(16) unsigned char g_smem_raw[];
+  uint32_t* acc_lo = reinterpret_cast<uint32_t*>(g_smem_raw);   // [c1][c2]: low and high 32-bit words of an int64 sum
+  int* acc_hi = reinterpret_cast<int*>(g_smem_raw) + SN * SN;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  int* stage = reinterpret_cast<int*>(g_smem_raw + SP_ACC_BYTES) + warp * SP_STAGE;   // (units << 7) | c2
+  unsigned short* rs = reinterpret_cast<unsigned short*>(g_smem_raw + SP_ACC_BYTES + (size_t)SP_WARPS * SP_STAGE * 4) + warp * 64;
+  unsigned short* re = rs + 32;   // a row's staged entries: [rs[r], re[r])
+
+  for (int e = threadIdx.x; e < SN * SN; e += SP_THREADS) { acc_lo[e] = 0u; acc_hi[e] = 0; }
+  __syncthreads();
+
+  const bool valid = bi < pb.nblk128 && bj < pb.nblk128;
+  const long long* __restrict__ offs_i = pb.bm_offs + (size_t)bi * ngroups;
+  const long long* __restrict__ offs_j = pb.bm_offs + (size_t)bj * ngroups;
+  const unsigned short* __restrict__ keys = pb.bm_keys;
+  const unsigned char* __restrict__ bytes = pb.bm_e4m3;
+  const uint32_t lt = (1u << lane) - 1u;
+  // the list holds < 2^32 entries (checked at upload): entry numbers are 32-bit.  Lanes 0..3 fetch the run bounds of a group
+  // (bi lo, bi hi, bj lo, bj hi) two groups ahead, and the first 64 entries of both runs are loaded one group ahead: a warp has one
+  // group in flight, so without this every group would wait out two or three dependent global-memory round trips.
+  auto ld_bounds = [&](long long g) -> uint32_t {
+    if (!valid || g >= ngroups || lane >= 4) return 0u;
+    return (uint32_t)__ldg((lane < 2 ? offs_i : offs_j) + g + (lane & 1));
+  };
+  // an entry as (key << 8) | e4m3 byte; 0 past the end of its run (a zero byte: skipped like any zero operand)
+  auto ld_entry = [&](uint32_t e, uint32_t hi) -> uint32_t {
+    return e < hi ? ((uint32_t)__ldg(keys + e) << 8) | (uint32_t)__ldg(bytes + e) : 0u;
+  };
+  struct Group { uint32_t ilo, ihi, jlo, jhi, i[2], j[2]; };
+  auto take = [&](Group& q, uint32_t b) {
+    q.ilo = __shfl_sync(0xffffffffu, b, 0); q.ihi = __shfl_sync(0xffffffffu, b, 1);
+    q.jlo = __shfl_sync(0xffffffffu, b, 2); q.jhi = __shfl_sync(0xffffffffu, b, 3);
+#pragma unroll
+    for (int k = 0; k < 2; k++) { q.i[k] = ld_entry(q.ilo + lane + 32 * k, q.ihi); q.j[k] = ld_entry(q.jlo + lane + 32 * k, q.jhi); }
+  };
+  // entry base + lane of the run starting at lo (bound hi); base - lo is warp-uniform
+  auto entry = [&](uint32_t base, uint32_t lo, uint32_t hi, const uint32_t (&pre)[2]) -> uint32_t {
+    return base == lo ? pre[0] : base == lo + 32 ? pre[1] : ld_entry(base + lane, hi);
+  };
+  auto run = [&](const Group& q) {
+    if (q.ilo == q.ihi || q.jlo == q.jhi) return;
+    for (uint32_t c0 = q.jlo; c0 < q.jhi; c0 += SP_STAGE) {
+      const uint32_t c1 = min(q.jhi, c0 + SP_STAGE);   // >= jlo + 64 or = jhi: the prefetched entries lie in the first chunk
+      __syncwarp();   // the previous chunk's readers are done
+      rs[lane] = 0; re[lane] = 0;
+      __syncwarp();
+      // ---- stage the chunk's nonzero entries; a kept entry whose row differs from the previous kept one starts its row
+      int nst = 0, prev_row = -1;
+      for (uint32_t base = c0; base < c1; base += 32) {
+        const uint32_t x = entry(base, q.jlo, c1, q.j);
+        const int v = e4m3_units(x & 255u);
+        const uint32_t key = x >> 8;
+        const int r = kmaj_row(key);
+        const bool keep = v != 0;
+        const uint32_t m = __ballot_sync(0xffffffffu, keep);
+        const uint32_t below = m & lt;
+        const int up = __shfl_sync(0xffffffffu, r, below ? 31 - __clz(below) : 0);
+        const int pr = below ? up : prev_row;
+        const int s = nst + __popc(below);
+        if (keep) {
+          stage[s] = v * 128 + (int)(key >> 5);
+          if (r != pr) { rs[r] = (unsigned short)s; if (pr >= 0) re[pr] = (unsigned short)s; }
+        }
+        if (m) prev_row = __shfl_sync(0xffffffffu, r, 31 - __clz(m));
+        nst += __popc(m);
+      }
+      if (nst == 0) continue;
+      if (lane == 0) re[prev_row] = (unsigned short)nst;
+      __syncwarp();
+      // ---- every bi entry times the staged entries of its row
+      for (uint32_t base = q.ilo; base < q.ihi; base += 32) {
+        const uint32_t x = entry(base, q.ilo, q.ihi, q.i);
+        const int a = e4m3_units(x & 255u);
+        if (a == 0) continue;
+        const uint32_t key = x >> 8;
+        const int r = kmaj_row(key), col = (int)(key >> 5);
+        const int row = col * SN;
+        const int s1 = re[r];
+        for (int s = rs[r]; s < s1; s++) {
+          const int p = stage[s];
+          const int c2 = p & 127;
+          if (diag && c2 > col) break;
+          const long long prod = (long long)a * (long long)(p >> 7);
+          const uint32_t lo = (uint32_t)prod;
+          const uint32_t old = atomicAdd(acc_lo + row + c2, lo);
+          const int hi = (int)(prod >> 32) + (old + lo < old ? 1 : 0);
+          if (hi != 0) atomicAdd(acc_hi + row + c2, hi);
+        }
+      }
+    }
+  };
+  Group cur, nxt;
+  take(cur, ld_bounds(warp));
+  uint32_t nb = ld_bounds(warp + SP_WARPS);
+  for (long long g = warp; g < ngroups; g += SP_WARPS) {
+    take(nxt, nb);   // the next group's loads are in flight while this one runs
+    nb = ld_bounds(g + 2 * SP_WARPS);
+    run(cur);
+    cur = nxt;
+  }
+  __syncthreads();
+  // ---- one rounding per cell: units of 2^-18 -> fp32
+  float* out = pb.Hpart + (size_t)bi * SN * Dp + (size_t)bj * SN;
+  for (int e = threadIdx.x; e < SN * SN; e += SP_THREADS) {
+    const int c1 = e >> 7, c2 = e & 127;
+    const int idx = diag && c2 > c1 ? c2 * SN + c1 : e;
+    const long long v = (long long)(((unsigned long long)(uint32_t)acc_hi[idx] << 32) | acc_lo[idx]);
+    out[(size_t)c1 * Dp + c2] = __ll2float_rn(v) * 0x1p-18f;
+  }
+}
+
+// Largest partition (rows) the sparse kernel's int64 tile sums are safe for: every row adds at most one product of magnitude
+// <= 229376^2 < 2^35.62 units to a cell, and 2^27 * 2^35.62 < 2^63
+long long gram_sparse_max_rows() { return 1LL << 27; }
+
 // Block-major entry list for the CSR Gram.  For every 128-column block b and every 32-row group g the entries
 // (row in group, column in block, value) are stored contiguously at [offs[b*ngroups+g], offs[b*ngroups+g+1]); the key is
 // the byte offset of the element inside a swizzled [128 col][32 k] operand block (kmaj_off), the value the stored float.
@@ -529,17 +693,21 @@ int gram_make_tensor_map(void* out_map_host /*CUtensorMap, 128 B*/, const void* 
 }
 
 // Lower block-triangle tile list for a Dp x Dp output (Dp multiple of 128): 128 x 256 tiles (bi, bj) for the bf16 kernel, or
-// 128 x 128 tiles for the CSR kernel (csr_tiles != 0).
+// 128 x 128 tiles for the CSR kernels (csr_tiles != 0).  The tiles of one bi are consecutive, so CTAs resident at the same time
+// share the bi run of the entry list in L2; the sparse kernel (csr_tiles == 2) takes the bi in descending order, which puts the
+// tile of the intercept column (every row's last entry: the most contended cell) into the first wave.
 int gram_tile_list(int Dp, short* bi_bj_pairs /*[2*max]*/, int max_tiles, int csr_tiles) {
   int n = 0;
   const int cols = csr_tiles ? SN : GN;
   const int nbi = (Dp + GM - 1) / GM, nbj = (Dp + cols - 1) / cols;
-  for (int bi = 0; bi < nbi; bi++)
+  for (int k = 0; k < nbi; k++) {
+    const int bi = csr_tiles == 2 ? nbi - 1 - k : k;
     for (int bj = 0; bj < nbj; bj++)
       if (bj * cols <= bi * GM + GM - 1) {
         if (n >= max_tiles) return -1;
         bi_bj_pairs[2 * n] = (short)bi; bi_bj_pairs[2 * n + 1] = (short)bj; n++;
       }
+  }
   return n;
 }
 
@@ -578,6 +746,20 @@ cudaError_t gram_launch_csr_wgmma(const Problem* d_probs, int nprob, const void*
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
   gram_csr_wgmma_kernel<<<dim3(ntiles, nslices, nprob), S_THREADS, S_SMEM, st>>>(
       d_probs, reinterpret_cast<const GramTile*>(d_tiles), ntiles, force, share);
+  if (launches) *launches += 2;
+  return cudaGetLastError();
+}
+
+// One sparse CSR Gram build: the operand pass, then the sparse Gram into slice 0.  d_tiles holds the tiles of
+// gram_tile_list(..., 2)
+cudaError_t gram_launch_csr_sparse(const Problem* d_probs, int nprob, const void* d_tiles, int ntiles, int force, cudaStream_t st,
+                                   int* launches, int share) {
+  static bool configured[64] = {};
+  cudaError_t e = set_smem_once(gram_csr_sparse_kernel, SP_SMEM, configured);
+  if (e != cudaSuccess) return e;
+  gram_csr_operand_kernel<<<dim3(1024, nprob), 256, 0, st>>>(d_probs, force, share);
+  if ((e = cudaGetLastError()) != cudaSuccess) return e;
+  gram_csr_sparse_kernel<<<dim3(ntiles, 1, nprob), SP_THREADS, SP_SMEM, st>>>(d_probs, reinterpret_cast<const GramTile*>(d_tiles), force, share);
   if (launches) *launches += 2;
   return cudaGetLastError();
 }

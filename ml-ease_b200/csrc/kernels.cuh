@@ -43,6 +43,10 @@ cudaError_t gram_launch_wgmma(const Problem* d_probs, int nprob, const void* d_t
                               int nslices, int force, cudaStream_t st, int* launches, int share = 0);
 cudaError_t gram_launch_csr_wgmma(const Problem* d_probs, int nprob, const void* d_tiles, int ntiles, int nslices, int force,
                                   cudaStream_t st, int* launches, int share = 0);
+// the exact sparse CSR Gram (one slice; tiles of gram_tile_list(..., 2)) and the largest partition it accepts
+cudaError_t gram_launch_csr_sparse(const Problem* d_probs, int nprob, const void* d_tiles, int ntiles, int force, cudaStream_t st,
+                                   int* launches, int share = 0);
+long long gram_sparse_max_rows();
 cudaError_t csr_bm_offsets(long long n, const long long* rowptr, const int* colidx, int bias_col, int nblk, long long ngroups, long long* offs,
                            cudaStream_t st);
 cudaError_t csr_bm_fill(long long n, const long long* rowptr, const int* colidx, const float* vals, int bias_col, int nblk, long long ngroups,

@@ -77,6 +77,17 @@ __global__ void absmax_kernel(long long n, const float* __restrict__ a, unsigned
   m = warp_max(m);
   if ((threadIdx.x & 31) == 0) atomicMax(out, __float_as_uint(m));
 }
+// sum over rows of (k_i + 1)(k_i + 2) / 2 (k_i stored values plus the intercept): the products, lower triangle, of one sparse
+// CSR Gram build
+__global__ void csr_gram_pairs_kernel(long long n, const long long* __restrict__ rowptr, unsigned long long* __restrict__ out) {
+  unsigned long long s = 0;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const unsigned long long k = (unsigned long long)(rowptr[i + 1] - rowptr[i]);
+    s += (k + 1) * (k + 2) / 2;
+  }
+  for (int d = 16; d > 0; d >>= 1) s += __shfl_down_sync(0xffffffffu, s, d);
+  if ((threadIdx.x & 31) == 0) atomicAdd(out, s);
+}
 __global__ void check_csr_kernel(long long nnz, const int* colidx, float* vals, int Dg, int binary, int* bad) {
   for (long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x; j < nnz; j += (long long)gridDim.x * blockDim.x) {
     const int c = colidx[j];
@@ -133,6 +144,7 @@ struct PartData {
   long long bm_groups = 0;
   long long bm_entries = 0;        // nnz + n: the list holds the bias column explicitly
   int nblk128 = 0;
+  double gram_pairs = 0;           // products of one sparse Gram build: sum over rows of (k_i + 1)(k_i + 2) / 2
   // segment lists of the fused multi-lambda CSR K1 (k1_csr_fused.cu), built at upload for rows with unique sorted columns
   int sg_S = 0, sg_rows = 0, sg_ngrp = 0;
   int* sg_perm = nullptr; int* sg_depth = nullptr; long long* sg_goff = nullptr; unsigned short* sg_row16 = nullptr; float* sg_val = nullptr;
@@ -146,6 +158,7 @@ struct Batch {
   int has_bias = 1;
   int k1_grid = 1, gram_slices = 1, ntiles = 0;
   int gram_from_csr = 0;          // every problem of the batch assembles its Gram tiles from CSR (no dense bf16 operand)
+  int csr_gram = 0;               // the CSR Gram kernel of the batch (CSR_GRAM_WGMMA / CSR_GRAM_SPARSE, set in batch_alloc), else 0
   int csr_fx = 0;                 // CSR rows sorted and unique: the deterministic K1 kernels (fixed point / segment lists) and their Hv
                                   // modes run, sqrt(d) goes to sdvec.  The Gram path has it with its block-major lists; a matrix-free
                                   // session (policy 2) builds no lists and has it from the rows alone
@@ -179,7 +192,8 @@ struct Counters {
   int not_converged = 0, last_slots = 0;
   double k1_bytes = 0;     // algorithmic bytes of all K1 passes (SURVEY 8d): dense n*(4*ldx+9), CSR 8*nnz+8*n+9*n
   double k1_emit_bytes = 0;// extra bytes written by passes that emitted the scaled bf16 copy (n*Dp*2)
-  double gram_flops = 0;   // algorithmic flops of all Gram builds: n*Dt*(Dt+1) (lower triangle, 2 flop/MAC)
+  double gram_flops = 0;   // flops of all Gram builds as run: n*Dt*(Dt+1) (wgmma, lower triangle, 2 flop/MAC), or 2 per product
+                           // the sparse CSR kernel forms
   double k1_shared_bytes = 0;  // CSR: bytes of the K1 passes when the lambdas of a partition are counted as ONE read of its rows:
                                // per (partition, slot) with A active lambdas 8*nnz + 9*n + 8*n*A (rows once, r/d out per lambda)
 };
@@ -234,10 +248,29 @@ static double gram_path_bytes(const Batch& B) {
   return bytes;
 }
 
+// Cost of one CSR Gram build of a partition (seconds; only the comparison matters).  Both kernels read each 128-column block's
+// run of every 32-row group once per tile it belongs to (nblk + 1 tiles: `reads` entries in all).  wgmma: every 128 x 128 lower
+// tile times every 32-row group on the tensor pipe, plus the producers' run loads, which is what makes its rate fall at small n
+// and high density.  Sparse: per product (integer multiply + native shared atomic add), per (tile, group) visit (staging the
+// runs) and per entry read, with the whole device busy; a grid of fewer CTAs than SMs is that much slower.  Least-squares fits
+// of tools/time_gram.py on an H100 SXM at 700 W over 0.3 - 20 % density at 10k features (DESIGN.md section 4): within 15 % on
+// every shape, so near the crossover (~3 % at 10k features) the rule may pick a kernel up to ~15 % slower than the other.
+constexpr double GRAM_WGMMA_S_PER_MAC = 1.30e-15, GRAM_WGMMA_S_PER_READ = 4.26e-12;
+constexpr double GRAM_SPARSE_S_PER_PAIR = 2.69e-12, GRAM_SPARSE_S_PER_VISIT = 2.47e-10, GRAM_SPARSE_S_PER_READ = 1.36e-12;
+static double gram_cost(const Problem& p, int Dp, int kind, double ctas, int num_sms) {
+  const double nblk = Dp / 128, tiles = nblk * (nblk + 1) / 2, groups = (double)((p.n + 31) / 32);
+  const double reads = (nblk + 1) * (double)p.bm_entries;
+  if (kind == CSR_GRAM_WGMMA) return tiles * 128.0 * 128.0 * 32.0 * groups * GRAM_WGMMA_S_PER_MAC + reads * GRAM_WGMMA_S_PER_READ;
+  return (p.gram_pairs * GRAM_SPARSE_S_PER_PAIR + tiles * groups * GRAM_SPARSE_S_PER_VISIT + reads * GRAM_SPARSE_S_PER_READ) *
+         std::max(1.0, num_sms / std::max(1.0, ctas));
+}
+
 // Allocate the per-problem solver state.  Data pointers (X, y, ...) and n must be filled in h[] first.
 // hessian_policy 2 builds the batch matrix-free (Newton-CG on Hv passes, O(D') state per problem); with any other policy the batch
 // is built matrix-free when what the Gram path would allocate exceeds the free device memory (it could not run at all).
-int batch_alloc(Batch& B, int num_sms, int hessian_policy) {
+// CSR Gram batches pick their kernel from the data: the sparse kernel when its cost model is lower and every partition is within
+// its row limit (gram_sparse_max_rows), else the wgmma kernel.  csr_gram_force (a test hook's setting) overrides the choice.
+int batch_alloc(Batch& B, int num_sms, int hessian_policy, int csr_gram_force = 0) {
   const int nprob = B.nprob, ldx = B.ldx;
   B.Dp = round_up(B.ldx, 128);
   B.ldh = round_up(B.Dt, 32);
@@ -310,12 +343,27 @@ int batch_alloc(Batch& B, int num_sms, int hessian_policy) {
     B.bfgs_m = BFGS_M_DEFAULT;   // measured at 1M x 10k x 1 %: 12 / 16 pairs save 2-4 % of the K1 passes and cost 45-60 % more two-loop time
     if (const char* e = getenv("MLEASE_BFGS_M")) B.bfgs_m = std::max(1, std::min(BFGS_M, atoi(e)));   // tuning experiments only
   }
+  B.csr_gram = 0;
+  if (B.gram_from_csr && !B.matfree) {
+    double t_sparse = 0, t_wgmma = 0;
+    bool fits = true;
+    const double nblk = B.Dp / 128, ctas = nblk * (nblk + 1) / 2 * nprob;   // the sparse kernel's grid: one CTA per (tile, problem)
+    for (auto& p : B.h) {
+      t_sparse += gram_cost(p, B.Dp, CSR_GRAM_SPARSE, ctas, num_sms);
+      t_wgmma += gram_cost(p, B.Dp, CSR_GRAM_WGMMA, ctas, num_sms);
+      if (p.n > gram_sparse_max_rows()) fits = false;
+    }
+    B.csr_gram = (fits && t_sparse < t_wgmma) ? CSR_GRAM_SPARSE : CSR_GRAM_WGMMA;
+    if (csr_gram_force == CSR_GRAM_SPARSE && !fits)
+      return fail(MLEASE_ERR_INVALID, "the sparse CSR Gram's int64 sums hold at most 2^27 rows per partition");
+    if (csr_gram_force) B.csr_gram = csr_gram_force;
+  }
   // Gram decomposition
   constexpr int MAX_TILES = 1 << 18;   // lower 128x128 tiles of Dp up to ~90k
   std::vector<short> tiles(B.matfree ? 2 : 2 * (size_t)MAX_TILES);
-  B.ntiles = B.matfree ? 0 : gram_tile_list(B.Dp, tiles.data(), MAX_TILES, B.gram_from_csr);
+  B.ntiles = B.matfree ? 0 : gram_tile_list(B.Dp, tiles.data(), MAX_TILES, B.csr_gram == CSR_GRAM_SPARSE ? 2 : B.gram_from_csr);
   if (B.ntiles <= 0 && !B.matfree) return fail(MLEASE_ERR_INVALID, "Gram tile list overflow");
-  if (!B.matfree) {
+  if (!B.matfree && B.csr_gram != CSR_GRAM_SPARSE) {   // the sparse kernel has no split-K: one slice
     const long long ksteps = (maxn + 63) / 64;
     const long long base = (long long)B.ntiles * nprob;   // CTAs
     const long long cap = std::max(1, num_sms);
@@ -407,9 +455,11 @@ int batch_alloc(Batch& B, int num_sms, int hessian_policy) {
       p.rvec = k1_csr_window(ldx) > 0 ? p.sdvec + p.n : nullptr;
       p.bm_e4m3 = B.matfree ? nullptr : pool + pool_off[b] + (((size_t)p.n * sizeof(float) * (p.rvec ? 2 : 1) + 255) & ~(size_t)255);
       p.gram_from_csr = B.gram_from_csr;
+      p.csr_gram = B.csr_gram;
       std::memset(&maps[b], 0, sizeof(CUtensorMap));
     } else {
       p.gram_from_csr = 0;
+      p.csr_gram = 0;
       p.gram_scale = 1.f; p.gram_unscale = 1.f;   // bf16 dense-operand Gram: no operand scale
       if (!p.Xt) p.Xt = reinterpret_cast<__nv_bfloat16*>(pool + pool_off[b]);
       if (gram_make_tensor_map(&maps[b], p.Xt, p.n, B.Dp) != 0) return fail(MLEASE_ERR_CUDA, "cuTensorMapEncodeTiled failed");
@@ -418,6 +468,18 @@ int batch_alloc(Batch& B, int num_sms, int hessian_policy) {
   CK(cudaMemcpy(B.d_tmaps, maps.data(), (size_t)nprob * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
   CK(cudaMemcpy(B.d, B.h.data(), (size_t)nprob * sizeof(Problem), cudaMemcpyHostToDevice));
   return 0;
+}
+
+// One Gram build of the problems d_probs[0 .. n) with the batch's kernel (force / share: see gram_wgmma_kernel)
+cudaError_t batch_gram(const Batch& B, const Problem* d_probs, int n, int force, cudaStream_t st, int* launches, int share = 0) {
+  if (B.csr_gram == CSR_GRAM_SPARSE) return gram_launch_csr_sparse(d_probs, n, B.d_tiles, B.ntiles, force, st, launches, share);
+  if (B.gram_from_csr) return gram_launch_csr_wgmma(d_probs, n, B.d_tiles, B.ntiles, B.gram_slices, force, st, launches, share);
+  return gram_launch_wgmma(d_probs, n, B.d_tmaps, B.d_tiles, B.ntiles, B.gram_slices, force, st, launches, share);
+}
+
+// flops one Gram build of problem p runs: 2 per product the sparse kernel forms, n Dt (Dt + 1) (lower triangle) for the wgmma kernels
+static double gram_build_flops(const Batch& B, const Problem& p) {
+  return B.csr_gram == CSR_GRAM_SPARSE ? 2.0 * p.gram_pairs : (double)p.n * (double)B.Dt * (double)(B.Dt + 1);
 }
 
 // K1 of a slot: the fused multi-lambda CSR kernel when the batch has segment lists, the per-problem kernels otherwise.
@@ -492,9 +554,8 @@ int batch_xupdate(Batch& B, cudaStream_t st, double xtol, int max_newton, int po
       // cold start of a multi-lambda run: the L problems of a partition all sit at beta = 0, their Grams are the same
       const int share = (slot_idx == 0) ? share_first_gram : 0;
       if (share > 1)
-        for (int b = 0; b < B.nprob; b++) if (b % share != 0) shared_flops += (double)B.h[b].n * (double)B.Dt * (double)(B.Dt + 1);
-      if (B.gram_from_csr) CK(gram_launch_csr_wgmma(d_hess, n_hess, B.d_tiles, B.ntiles, B.gram_slices, 0, st, &launches, share));
-      else CK(gram_launch_wgmma(d_hess, n_hess, B.d_tmaps, B.d_tiles, B.ntiles, B.gram_slices, 0, st, &launches, share));
+        for (int b = 0; b < B.nprob; b++) if (b % share != 0) shared_flops += gram_build_flops(B, B.h[b]);
+      CK(batch_gram(B, d_hess, n_hess, 0, st, &launches, share));
       pf.end(st);
       pf.begin(3, st);
       const bool share_fact = share > 1 && share_first_factor;   // same rho too: same H, one factorisation per group
@@ -606,7 +667,7 @@ int batch_xupdate(Batch& B, cudaStream_t st, double xtol, int max_newton, int po
     const Problem& p = B.h[b];
     const double rowbytes = B.csr ? 17.0 : (4.0 * B.ldx + 9.0);
     cnt.k1_bytes += (double)c.evals * ((double)p.n * rowbytes + (B.csr ? 8.0 * (double)p.nnz_hint : 0.0));
-    cnt.gram_flops += (double)c.hess_builds * (double)p.n * (double)B.Dt * (double)(B.Dt + 1);
+    cnt.gram_flops += (double)c.hess_builds * gram_build_flops(B, p);
     cnt.k1_emit_bytes += (double)c.hess_builds * (double)p.n * (double)B.Dp * 2.0;
   }
   cnt.gram_flops -= shared_flops;
@@ -671,6 +732,7 @@ struct mlease_session {
   Profiler prof;
   double xtol = 1e-8;
   int max_newton = 50;
+  int csr_gram_force = 0;    // 0: batch_alloc picks the CSR Gram kernel; CSR_GRAM_WGMMA / CSR_GRAM_SPARSE (mlease_internal_set_csr_gram)
   ~mlease_session() {
     delete batch;
     delete scratch;
@@ -706,7 +768,7 @@ void fill_problem_data(Problem& p, const PartData& pd) {
   p.X = pd.X; p.n = pd.n; p.y = pd.y; p.w = pd.w; p.o = pd.o;
   p.rowptr = pd.rowptr; p.colidx = pd.colidx; p.vals = pd.vals; p.nnz_hint = pd.nnz; p.csr_unique = pd.csr_unique;
   p.bm_offs = pd.bm_offs; p.bm_keys = pd.bm_keys; p.bm_vals = pd.bm_vals; p.bm_groups = pd.bm_groups; p.bm_entries = pd.bm_entries;
-  p.nblk128 = pd.nblk128; p.gram_from_csr = pd.bm_offs ? 1 : 0;
+  p.nblk128 = pd.nblk128; p.gram_from_csr = pd.bm_offs ? 1 : 0; p.gram_pairs = pd.gram_pairs;
   p.vmax = pd.vmax; p.wmax = pd.wmax; p.rowl1 = pd.rowl1;
   p.sg_S = pd.sg_S; p.sg_rows = pd.sg_rows; p.sg_ngrp = pd.sg_ngrp; p.sg_perm = pd.sg_perm; p.sg_depth = pd.sg_depth; p.sg_goff = pd.sg_goff;
   p.sg_row16 = pd.sg_row16; p.sg_val = pd.sg_val;
@@ -744,7 +806,7 @@ int finalize(mlease_session* s) {
       fill_problem_data(p, s->parts[pi]);
       p.lambda_idx = l; p.part_local = (int)pi;
     }
-  if (int rc = batch_alloc(*B, s->num_sms, s->cfg.hessian_policy)) return rc;
+  if (int rc = batch_alloc(*B, s->num_sms, s->cfg.hessian_policy, s->csr_gram_force)) return rc;
   const size_t ldv = s->ldx;
   if (int rc = sess_alloc(s, (void**)&s->d_z, s->L * ldv * sizeof(double))) return rc;
   if (int rc = sess_alloc(s, (void**)&s->d_wz, s->L * ldv * sizeof(double))) return rc;
@@ -786,7 +848,7 @@ int ensure_scratch(mlease_session* s, int part_idx) {
   B->h.resize(1);
   fill_problem_data(B->h[0], s->parts[part_idx]);
   s->scratch_part = part_idx;
-  return batch_alloc(*B, s->num_sms, s->cfg.hessian_policy);
+  return batch_alloc(*B, s->num_sms, s->cfg.hessian_policy, s->csr_gram_force);
 }
 
 double rho_eff_for_iter(mlease_session* s, int l, int iter) {
@@ -1038,6 +1100,15 @@ static int csr_build_layout(mlease_session* s, PartData& pd) {
     CK(csr_bm_offsets(nrows, pd.rowptr, pd.colidx, s->Dg, pd.nblk128, pd.bm_groups, (long long*)bo, s->stream));
     CK(csr_bm_fill(nrows, pd.rowptr, pd.colidx, pd.vals, s->Dg, pd.nblk128, pd.bm_groups, (const long long*)bo, (unsigned short*)bk, (float*)bv, s->stream));
     pd.bm_offs = (long long*)bo; pd.bm_keys = (unsigned short*)bk; pd.bm_vals = (float*)bv;
+    // products of one sparse Gram build (the kernel choice of batch_alloc)
+    unsigned long long* d_pairs = reinterpret_cast<unsigned long long*>(s->d_flag);
+    CK(cudaMemsetAsync(d_pairs, 0, 8, s->stream));
+    csr_gram_pairs_kernel<<<(int)std::min<long long>((nrows + 255) / 256, 2048), 256, 0, s->stream>>>(nrows, pd.rowptr, d_pairs);
+    CK(cudaMemcpyAsync(s->h_flag, d_pairs, 8, cudaMemcpyDeviceToHost, s->stream));
+    CK(cudaStreamSynchronize(s->stream));
+    unsigned long long pairs = 0;
+    std::memcpy(&pairs, s->h_flag, 8);
+    pd.gram_pairs = (double)pairs;
   }
   if (pd.csr_unique && pd.nnz + nrows < (1LL << 32) - 64) {
     // segment lists of the fused multi-lambda K1
@@ -1376,8 +1447,7 @@ int mlease_objective(mlease_session* s, int32_t pid, const double* w, const doub
   if (H) {
     if (B->matfree) return fail(MLEASE_ERR_INVALID, "this session's problems are matrix-free (hessian_policy 2, or a Hessian too large for the device): use mlease_hessian_vector");
     if (!tensor && B->gram_from_csr) return fail(MLEASE_ERR_INVALID, "the SIMT debug Gram needs the dense bf16 operand, which CSR partitions with sorted unique rows do not materialise");
-    if (tensor && B->gram_from_csr) CK(gram_launch_csr_wgmma(B->d, 1, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches, 0));
-    else if (tensor) CK(gram_launch_wgmma(B->d, 1, B->d_tmaps, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches));
+    if (tensor) CK(batch_gram(*B, B->d, 1, 1, s->stream, &launches));
     else CK(gram_launch_simt(B->d, 1, B->Dp, 1, s->stream, &launches));
     if (tensor == 2) {
       // the inverse the Newton direction uses: split-K Gram partials + diag(q) -> fp64 Cholesky -> explicit inverse
@@ -1560,6 +1630,27 @@ int mlease_internal_batch_hv(mlease_session* s, int32_t mode, const double* w, c
   return 0;
 }
 
+// Test hooks, not part of the C ABI: the CSR Gram kernel of the batches allocated from now on -- 0 = picked from the data,
+// CSR_GRAM_WGMMA (1), CSR_GRAM_SPARSE (2).  Must be called before the ADMM batch exists; the one-problem scratch batch (objective,
+// timing) is rebuilt with the new setting on its next use.  The query returns the kind of the ADMM batch and of the scratch batch
+// (0: no such batch, or no CSR Gram).
+int mlease_internal_set_csr_gram(mlease_session* s, int32_t kind) {
+  if (!s || kind < 0 || kind > CSR_GRAM_SPARSE) return fail(MLEASE_ERR_INVALID, "bad argument");
+  if (s->batch) return fail(MLEASE_ERR_STATE, "the CSR Gram kernel is chosen when the ADMM batch is allocated: set it before");
+  s->csr_gram_force = kind;
+  delete s->scratch;
+  s->scratch = nullptr;
+  s->scratch_part = -1;
+  return 0;
+}
+
+int mlease_internal_csr_gram(mlease_session* s, int32_t* batch_kind, int32_t* scratch_kind) {
+  if (!s || !batch_kind || !scratch_kind) return fail(MLEASE_ERR_INVALID, "null argument");
+  *batch_kind = s->batch ? s->batch->csr_gram : 0;
+  *scratch_kind = s->scratch ? s->scratch->csr_gram : 0;
+  return 0;
+}
+
 int mlease_time_kernel(mlease_session* s, int32_t pid, int32_t which, int32_t reps, int32_t emit_scaled, float* avg_ms) {
   if (!s || !avg_ms || reps <= 0) return fail(MLEASE_ERR_INVALID, "bad argument");
   CK(cudaSetDevice(s->cfg.device));
@@ -1578,8 +1669,7 @@ int mlease_time_kernel(mlease_session* s, int32_t pid, int32_t which, int32_t re
   // warm-up launch (also produces the scaled copy the Gram needs)
   CK(batch_k1(*B, 1, s->stream, &launches));
   if (which == 3) {
-    if (B->gram_from_csr) CK(gram_launch_csr_wgmma(B->d, 1, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches, 0));
-    else CK(gram_launch_wgmma(B->d, 1, B->d_tmaps, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches));
+    CK(batch_gram(*B, B->d, 1, 1, s->stream, &launches));
     Ctrl c; std::memset(&c, 0, sizeof(c)); c.need_hess = 1;
     CK(cudaMemcpyAsync(B->d_ctrl, &c, sizeof(Ctrl), cudaMemcpyHostToDevice, s->stream));
   }
@@ -1597,8 +1687,7 @@ int mlease_time_kernel(mlease_session* s, int32_t pid, int32_t which, int32_t re
   CK(cudaEventRecord(e0, s->stream));
   for (int r = 0; r < reps; r++) {
     if (which == 1) CK(batch_k1(*B, emit_scaled ? 1 : 0, s->stream, &launches));
-    else if (which == 2 && B->gram_from_csr) CK(gram_launch_csr_wgmma(B->d, 1, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches, 0));
-    else if (which == 2) CK(gram_launch_wgmma(B->d, 1, B->d_tmaps, B->d_tiles, B->ntiles, B->gram_slices, 1, s->stream, &launches));
+    else if (which == 2) CK(batch_gram(*B, B->d, 1, 1, s->stream, &launches));
     else if (which == 3) CK(cholesky_launch(B->d, 1, B->ldh, s->stream, &launches));
     else if (which == 4) { CK(batch_k1(*B, 0, s->stream, &launches, K1_HV)); CK(hv_reduce(B->d, 1, B->Dt, 0, s->stream, &launches)); }
     else return fail(MLEASE_ERR_INVALID, "which must be 1, 2, 3 or 4");

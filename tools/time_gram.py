@@ -1,25 +1,106 @@
 #!/usr/bin/env python
-"""WHICH=cholesky: times the factorisation + inverse of one 10k-wide system instead (ROWS=100000 keeps the data small).
-Times ONE CSR Gram build (1M x 10k x 1 %, the bench's partition 0) through mlease_time_kernel.  Scratch tool for kernel work on
-a GPU box, not part of the product."""
-import os, sys
+"""Times one CSR Gram build with each kernel (e4m3 wgmma, exact sparse) on the same upload, at several densities at D = 10k plus
+the bench shape (1M x 10k x 1 %) and `bench.py --features 500` (1M x 500 x 20 %), through mlease_time_kernel; prints which kernel
+the automatic rule picks for each and a least-squares fit of the cost constants of batch_alloc's rule (csrc/session.cu).
+OUT=path also writes the table as JSON.  SHAPES=bench keeps the bench shape only.
+WHICH=cholesky: times the factorisation + inverse of one 10k-wide system instead (ROWS=100000 keeps the data small).
+Scratch tool for kernel work on a GPU box, not part of the product."""
+import ctypes as C
+import json
+import os
+import sys
+
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "ml-ease_b200"))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), ".."))
-import torch
-import mlease_b200 as mb
-import bench
+import numpy as np  # noqa: E402
+import torch  # noqa: E402
 
-n = int(os.environ.get("ROWS", 1000000)); D = 10000; nnz = 100
+import bench  # noqa: E402
+import mlease_b200 as mb  # noqa: E402
+from mlease_b200._native import check, lib  # noqa: E402
+
+WGMMA, SPARSE = 1, 2
 dev = torch.device("cuda:0")
-import numpy as np
-beta = (np.random.default_rng(7).normal(size=D) / np.sqrt(nnz)).astype(np.float32)
-rp, ci, vv, y = bench.gen_sparse(0, n, D, nnz, beta, dev)
-with mb.AdmmSession(1, D, [1.0], device=0) as s:
+REPS = int(os.environ.get("REPS", 3))
+
+
+def hooks():
+    L = lib()
+    L.mlease_internal_set_csr_gram.argtypes = [C.c_void_p, C.c_int32]
+    L.mlease_internal_set_csr_gram.restype = C.c_int
+    L.mlease_internal_csr_gram.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
+    L.mlease_internal_csr_gram.restype = C.c_int
+    return L
+
+
+def session(n, D, nnz):
+    beta = (np.random.default_rng(7).normal(size=D) / np.sqrt(nnz)).astype(np.float32)
+    rp, ci, vv, y = bench.gen_sparse(0, n, D, nnz, beta, dev, chunk=max(1000, min(250_000, 200_000_000 // D)))
+    s = mb.AdmmSession(1, D, [1.0], device=0)
     s.add_partition_csr(0, rp, ci, vv, y)
+    del rp, ci, vv, y
+    torch.cuda.empty_cache()
+    return s
+
+
+def time_gram(s, kind):
+    """ms per build with the kernel `kind` (0: the automatic choice), and the kind that ran"""
+    L = hooks()
+    check(L.mlease_internal_set_csr_gram(s._h, kind))
+    ms = s.time_kernel(0, "gram", reps=REPS)
+    b, sc = C.c_int32(), C.c_int32()
+    check(L.mlease_internal_csr_gram(s._h, C.byref(b), C.byref(sc)))
+    return ms, sc.value
+
+
+def main():
     if os.environ.get("WHICH", "gram") == "cholesky":
-        # factorisation + inverse of ONE 10k-wide system (MLEASE_MERGE_TF32=0 / 1: fp64 DMMA / TF32 merges of the inverse)
-        ms = s.time_kernel(0, "cholesky", reps=3)
-        print("cholesky+inverse ms per factorisation", ms, "MLEASE_MERGE_TF32", os.environ.get("MLEASE_MERGE_TF32", "default"))
-    else:
-        ms = s.time_kernel(0, "gram", reps=3)
-        print("gram ms per build", ms, "PFLOP/s", n * 10016.0 * 10017.0 / ms / 1e12)
+        n, D = int(os.environ.get("ROWS", 100000)), 10000
+        with session(n, D, 100) as s:
+            # factorisation + inverse of ONE 10k-wide system (MLEASE_MERGE_TF32=0 / 1: fp64 DMMA / TF32 merges of the inverse)
+            ms = s.time_kernel(0, "cholesky", reps=3)
+            print("cholesky+inverse ms per factorisation", ms, "MLEASE_MERGE_TF32", os.environ.get("MLEASE_MERGE_TF32", "default"))
+        return
+    # (rows, features, stored values per row): the row counts keep each upload near 10^8 stored values
+    shapes = [(1_000_000, 10_000, 100), (1_000_000, 500, 100), (1_000_000, 10_000, 30), (1_000_000, 10_000, 150),
+              (1_000_000, 10_000, 200), (300_000, 10_000, 300), (100_000, 10_000, 1000), (30_000, 10_000, 2000)]
+    if os.environ.get("SHAPES") == "bench":
+        shapes = shapes[:1]
+    print("device:", torch.cuda.get_device_name(0))
+    rows = []
+    for n, D, nnz in shapes:
+        with session(n, D, nnz) as s:
+            ms_w, _ = time_gram(s, WGMMA)
+            ms_s, _ = time_gram(s, SPARSE)
+            _, auto = time_gram(s, 0)
+        Dp = (D + 1 + 127) // 128 * 128   # ldx rounds D + 1 up to a multiple of 4; Dp to 128
+        nblk = Dp // 128
+        tiles, groups = nblk * (nblk + 1) // 2, (n + 31) // 32
+        r = dict(n=n, D=D, nnz=nnz, density=nnz / D, ms_wgmma=ms_w, ms_sparse=ms_s, auto="sparse" if auto == SPARSE else "wgmma",
+                 macs_wgmma=tiles * 128.0 * 128.0 * 32.0 * groups, pairs=n * (nnz + 1) * (nnz + 2) / 2.0,
+                 visits=float(tiles * groups), reads=(nblk + 1.0) * n * (nnz + 1))
+        rows.append(r)
+        print("n %8d D %6d nnz/row %5d (%5.2f %%): wgmma %9.3f ms  sparse %9.3f ms  auto %s" %
+              (n, D, nnz, 100.0 * nnz / D, ms_w, ms_s, r["auto"]), flush=True)
+    fit = {}
+    full = [r for r in rows if r["visits"] / ((r["n"] + 31) // 32) >= torch.cuda.get_device_properties(0).multi_processor_count]
+    if len(full) >= 3:
+        # the rule's models on the shapes that fill the device, relative least squares (every shape weighs the same):
+        #   sparse  s = s/pair * pairs + s/visit * (tile, group) visits + s/read * entries read (each block's run by nblk + 1 tiles)
+        #   wgmma   s = s/MAC * MACs + s/read * entries read (the producers' run loads)
+        for name, key, cols in (("sparse", "ms_sparse", ("pairs", "visits", "reads")), ("wgmma", "ms_wgmma", ("macs_wgmma", "reads"))):
+            A = np.array([[r[c] for c in cols] for r in full])
+            t = np.array([r[key] * 1e-3 for r in full])
+            c, *_ = np.linalg.lstsq(A / t[:, None], np.ones(len(full)), rcond=None)
+            fit[name] = dict(zip(cols, c))
+            print("%s fit (s per unit):" % name, {k: "%.3e" % v for k, v in fit[name].items()})
+            for r in full:
+                print("   %s model %9.3f ms  measured %9.3f ms  (%d x %d x %d)" %
+                      (name, 1e3 * sum(ci * r[k] for ci, k in zip(c, cols)), r[key], r["n"], r["D"], r["nnz"]))
+    if os.environ.get("OUT"):
+        with open(os.environ["OUT"], "w") as f:
+            json.dump(dict(device=torch.cuda.get_device_name(0), rows=rows, fit=fit), f, indent=1)
+
+
+if __name__ == "__main__":
+    main()
