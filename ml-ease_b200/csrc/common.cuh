@@ -7,8 +7,9 @@
 
 namespace mlease {
 
-constexpr int BFGS_M = 16;        // storage for secant pairs kept on top of the (possibly stale) explicit inverse Hessian
-constexpr int BFGS_M_DEFAULT = 6; // pairs actually used (Ctrl::bfgs_m)
+// Secant pairs kept on top of the (possibly stale) explicit inverse Hessian.  Measured at 1M x 10k x 1 %: 12 / 16 pairs save
+// 2-4 % of the K1 passes and cost 45-60 % more two-loop time.
+constexpr int BFGS_M = 6;
 constexpr int CG_MAX_STEPS = 64;  // CG steps per matrix-free Newton direction (newton.cu, where the choice is explained)
 
 // ------------------------------------------------------------------------------------------
@@ -30,9 +31,7 @@ struct Ctrl {
   int rejects;       // rejected trial points in this x-update
   int hess_builds;   // Gram+Cholesky rebuilds in this x-update
   int stall;         // consecutive poor contractions
-  int bfgs_count;    // secant pairs stored so far (ring of bfgs_m), reset when the Hessian is rebuilt
-  int bfgs_m;        // ring size in use (<= BFGS_M)
-  int self_scale;    // 1: adapt h0_scale from the secant pairs (set per x-update; wide systems)
+  int bfgs_count;    // secant pairs stored so far (ring of BFGS_M), reset when the Hessian is rebuilt
   double h0_scale;   // self-scaling factor applied to the explicit inverse inside the L-BFGS two-loop (wide systems only; 1 after a rebuild)
   int k1_chunks;     // number of per-CTA partials the last K1 pass wrote for this problem (gpart / fpart rows)
   int refresh_next;  // rebuild the Hessian at the first point of the NEXT x-update (chord steps contracted slowly)
@@ -54,6 +53,7 @@ struct Ctrl {
   int max_newton;
   int hess_policy;   // 0 adaptive chord, 1 every step
   int rebuild_is_expensive;  // a Gram+Cholesky rebuild costs more than ~8 passes over X: never rebuild mid-update, lean on L-BFGS
+                             // and adapt h0_scale from the secant pairs
   // cumulative counters (never reset by begin-of-iteration)
   long long tot_evals, tot_newton, tot_rejects, tot_hess;
   // factored inverse the direction kernels read: this problem's own Ysym after its own factorisation, the group leader's after a

@@ -596,9 +596,7 @@ __global__ void __launch_bounds__(1024) k1_csr_kernel(const Problem* __restrict_
     const float rr = -ww * yy * qq;
     for (long long j = j0 + lane; j < j1; j += 32) atomicAdd(&g_s[ci[j]], vv[j] * rr);
     if (has_bias && lane == 0) atomicAdd(&g_s[Dt - 1], rr);
-    if (emit && pb.gram_from_csr) {
-      if (lane == 0) pb.sdvec[i] = sqrtf(ww * p * qq);   // the Gram kernel assembles the scaled rows itself
-    } else if (emit) {
+    if (emit) {
       const float sd = sqrtf(ww * p * qq);
       __nv_bfloat16* xt = pb.Xt + (size_t)i * pb.Dp;
       if (uniq) {

@@ -22,7 +22,7 @@ cudaError_t csr_row_l1_max(long long n, const long long* rowptr, const float* va
 
 // Newton state machine (newton.cu)
 cudaError_t newton_begin(const Problem* d_probs, int nprob, double xtol, int max_newton, int hess_policy,
-                         int invalidate_hess, int rebuild_is_expensive, cudaStream_t st, int* launches, int bfgs_m = BFGS_M_DEFAULT, int self_scale = 0);
+                         int invalidate_hess, int rebuild_is_expensive, cudaStream_t st, int* launches);
 cudaError_t k1_reduce_decide(const Problem* d_probs, int nprob, int Dt, cudaStream_t st, int* launches, int spec = 0);
 cudaError_t newton_solve(const Problem* d_probs, int nprob, int ldh, cudaStream_t st, int* launches, int group_L = 1);
 // matrix-free Newton-CG direction (newton.cu): begin (pick the problems that need a direction), the fixed-order reduction of the

@@ -167,8 +167,6 @@ struct Batch {
   int k1f_LP = 1;                 // lambdas padded to 1 / 2 / 4 in the interleaved shared-memory vectors
   size_t k1f_smem = 0;
   int k1_dyn = 0;                 // > 0: K1 CTAs are dealt to the running problems at run time (value = nprob, <= 32); k1_grid = whole grid
-  int self_scale = 0;             // adapt a scalar multiplier of the stale inverse from the secant pairs (wide systems)
-  int bfgs_m = BFGS_M_DEFAULT;    // secant pairs in use
   int rebuild_is_expensive = 0;   // cost model: Gram + Cholesky + inverse vs one K1 pass (set in batch_alloc)
   int matfree = 0;                // Newton-CG directions from Hv passes: no Gram, factor or inverse is allocated (set in batch_alloc)
   std::vector<Problem> h;
@@ -242,7 +240,7 @@ int dev_alloc(Batch& B, void** p, size_t bytes, bool zero = true) {
 // factor, L^-1 and H^-1, the diagonal-block side buffers, the bf16 Y of wide systems and the e4m3 operands (~26 D'^2 per problem).
 static double gram_path_bytes(const Batch& B) {
   const double Dp = round_up(B.ldx, 128), ldh = round_up(B.Dt, 32);
-  double per = Dp * Dp * 4.0 + 3.0 * ldh * ldh * 8.0 + 2.0 * ldh * 32 * 8.0 + (ldh > 2048 ? ldh * ldh * 2.0 : 0.0);
+  double per = Dp * Dp * 4.0 + 3.0 * ldh * ldh * 8.0 + 2.0 * ldh * 32 * 8.0 + (cholesky_factored_direction((int)ldh) ? ldh * ldh * 2.0 : 0.0);
   double bytes = per * B.nprob;
   for (auto& p : B.h) bytes += (double)p.bm_entries;
   return bytes;
@@ -300,7 +298,7 @@ int batch_alloc(Batch& B, int num_sms, int hessian_policy, int csr_gram_force = 
   }
   // fused multi-lambda CSR K1: every problem has segment lists, the groups are whole, and the shared-memory vectors fit
   B.k1_fused = 0;
-  if (B.csr && B.csr_fx && B.group_L >= 1 && B.group_L <= 4 && nprob % B.group_L == 0 && !getenv("MLEASE_NO_FUSED_K1")) {
+  if (B.csr && B.csr_fx && B.group_L >= 1 && B.group_L <= 4 && nprob % B.group_L == 0) {
     bool ok = true;
     for (auto& p : B.h) if (!p.sg_perm || p.sg_S != B.h[0].sg_S || p.sg_rows != B.h[0].sg_rows) ok = false;
     if (ok) {
@@ -338,10 +336,6 @@ int batch_alloc(Batch& B, int num_sms, int hessian_policy, int csr_gram_force = 
     // only wide systems qualify: small ones (NaiveTrain's per-key fits, cold-started every time) are launch-bound, not
     // flop-bound, and a mid-update rebuild saves them many lock-step slots
     B.rebuild_is_expensive = (t_rebuild > 8.0 * t_pass && B.Dt > 2048 && !B.matfree) ? 1 : 0;
-    B.self_scale = B.rebuild_is_expensive;
-    if (const char* e = getenv("MLEASE_SELF_SCALE")) B.self_scale = atoi(e) ? 1 : 0;   // tuning experiments only
-    B.bfgs_m = BFGS_M_DEFAULT;   // measured at 1M x 10k x 1 %: 12 / 16 pairs save 2-4 % of the K1 passes and cost 45-60 % more two-loop time
-    if (const char* e = getenv("MLEASE_BFGS_M")) B.bfgs_m = std::max(1, std::min(BFGS_M, atoi(e)));   // tuning experiments only
   }
   B.csr_gram = 0;
   if (B.gram_from_csr && !B.matfree) {
@@ -397,7 +391,7 @@ int batch_alloc(Batch& B, int num_sms, int hessian_policy, int csr_gram_force = 
     if (int rc = dev_alloc(B, (void**)&ldi, (size_t)nprob * B.ldh * 32 * sizeof(double))) return rc;
     if (int rc = dev_alloc(B, (void**)&yi, (size_t)nprob * B.ldh * B.ldh * sizeof(double))) return rc;
     if (int rc = dev_alloc(B, (void**)&hi, (size_t)nprob * B.ldh * B.ldh * sizeof(double))) return rc;
-    if (B.ldh > 2048)
+    if (cholesky_factored_direction(B.ldh))
       if (int rc = dev_alloc(B, (void**)&hif, (size_t)nprob * B.ldh * B.ldh * sizeof(__nv_bfloat16))) return rc;
   }
   if (int rc = dev_alloc(B, (void**)&B.d_ctrl, (size_t)nprob * sizeof(Ctrl))) return rc;
@@ -413,9 +407,9 @@ int batch_alloc(Batch& B, int num_sms, int hessian_policy, int csr_gram_force = 
   for (int b = 0; b < nprob; b++) {
     pool_off[b] = pool_bytes;
     const bool windows = B.csr_fx && k1_csr_window(ldx) > 0;   // then a second [n] vector (row residuals) follows sdvec
-    // CSR: sdvec (+ rvec), then the e4m3 operand bytes of the entry list (none in a matrix-free batch)
+    // CSR: sdvec (+ rvec), then the e4m3 operand bytes of the entry list (none in a matrix-free batch); else the bf16 operand Xt
     const size_t need = B.csr_fx ? (((size_t)B.h[b].n * sizeof(float) * (windows ? 2 : 1) + 255) & ~(size_t)255) + (B.matfree ? 0 : (size_t)B.h[b].bm_entries)
-                                        : (B.h[b].Xt ? 0 : (size_t)B.h[b].n * B.Dp * sizeof(__nv_bfloat16));
+                                        : (size_t)B.h[b].n * B.Dp * sizeof(__nv_bfloat16);
     pool_bytes += (need + 255) & ~(size_t)255;
   }
   unsigned char* pool = nullptr;
@@ -461,7 +455,7 @@ int batch_alloc(Batch& B, int num_sms, int hessian_policy, int csr_gram_force = 
       p.gram_from_csr = 0;
       p.csr_gram = 0;
       p.gram_scale = 1.f; p.gram_unscale = 1.f;   // bf16 dense-operand Gram: no operand scale
-      if (!p.Xt) p.Xt = reinterpret_cast<__nv_bfloat16*>(pool + pool_off[b]);
+      p.Xt = reinterpret_cast<__nv_bfloat16*>(pool + pool_off[b]);
       if (gram_make_tensor_map(&maps[b], p.Xt, p.n, B.Dp) != 0) return fail(MLEASE_ERR_CUDA, "cuTensorMapEncodeTiled failed");
     }
   }
@@ -499,7 +493,7 @@ int batch_xupdate(Batch& B, cudaStream_t st, double xtol, int max_newton, int po
   Profiler& pf = prof ? *prof : nop;
   int launches = 0;
   if (B.matfree) policy = 2;   // also when the batch was made matrix-free by the memory rule
-  CK(newton_begin(B.d, B.nprob, xtol, max_newton, policy, invalidate, B.rebuild_is_expensive, st, &launches, B.bfgs_m, B.self_scale));
+  CK(newton_begin(B.d, B.nprob, xtol, max_newton, policy, invalidate, B.rebuild_is_expensive, st, &launches));
   // The first slot's flags are known on the host: every problem is running, and a rebuild is due iff the policy says
   // always, the factors were invalidated, or the mirrored control blocks say so (no factor yet / refresh requested).
   const bool small = B.nprob <= 64;   // small batches read the whole control array back each slot (one sync, no poll kernel)
@@ -593,7 +587,7 @@ int batch_xupdate(Batch& B, cudaStream_t st, double xtol, int max_newton, int po
       if (!B.h_ctrl[i]) CK(cudaMallocHost((void**)&B.h_ctrl[i], (size_t)B.nprob * sizeof(Ctrl)));
       if (!B.slot_ev[i]) CK(cudaEventCreateWithFlags(&B.slot_ev[i], cudaEventDisableTiming));
     }
-    const bool may_spec = policy == 0 && !getenv("MLEASE_NO_SLOT_PIPELINE");
+    const bool may_spec = policy == 0;
     auto flags_of = [&](const Ctrl* c, bool* all_valid) {
       int f = 0; bool v = true;
       for (int b = 0; b < B.nprob; b++) if (!c[b].done) { f |= 1; if (c[b].emit) f |= 2; if (!c[b].hess_valid) v = false; }
@@ -1113,7 +1107,7 @@ static int csr_build_layout(mlease_session* s, PartData& pd) {
   if (pd.csr_unique && pd.nnz + nrows < (1LL << 32) - 64) {
     // segment lists of the fused multi-lambda K1
     int S = 0, rows = 0, LP = 0; size_t smem = 0;
-    if (!getenv("MLEASE_NO_FUSED_K1") && k1f_plan(nrows, s->ldx, s->L, s->num_sms, &S, &rows, &LP, &smem)) {
+    if (k1f_plan(nrows, s->ldx, s->L, s->num_sms, &S, &rows, &LP, &smem)) {
       CK(k1f_build(nrows, s->Dg, pd.nnz, pd.rowptr, pd.colidx, pd.vals, S, rows, &pd.sg_ngrp, &pd.sg_perm, &pd.sg_depth, &pd.sg_goff, &pd.sg_row16,
                    &pd.sg_val, &pd.sg_total, s->stream));
       pd.sg_S = S; pd.sg_rows = rows;

@@ -38,15 +38,15 @@ def _sparse_parts(P, n, D, nnz, seed, binary=False):
     return parts, data, [p * n for p in range(P + 1)]
 
 
-# (rows, features, stored values per row, lambdas of the session, hessian_policy): mlease_hessian_vector runs on the session's
-# one-problem scratch batch -- the fused kernel with one lambda (default policy: a Gram-path scratch problem), the column windows,
-# and a width no Gram fits.  The multi-lambda and per-problem variants of the main batch: test_batch_hv_and_diagonal_match_oracle
+# (rows, features, stored values per row, lambdas of the session, hessian_policy, no segment lists): mlease_hessian_vector runs on
+# the session's one-problem scratch batch -- the fused kernel (default policy: a Gram-path scratch problem), the column windows
+# (two lambdas at 30 001 columns: the 2-wide interleaved beta of the fused kernel does not fit a CTA's shared memory, so the upload
+# builds no segment lists), and a width no Gram fits.  The multi-lambda and per-problem variants of the main batch:
+# test_batch_hv_and_diagonal_match_oracle
 @pytest.mark.parametrize("n,D,nnz,lambdas,policy,no_fused", [(4000, 300, 12, (0.1, 1.0, 10.0), 0, False),
-                                                             (3000, 30001, 60, (1.0,), 2, True),
+                                                             (3000, 30001, 60, (1.0, 2.0), 2, True),
                                                              (3000, 200001, 100, (1.0,), 2, False)])
-def test_hessian_vector_matches_oracle(mb, monkeypatch, n, D, nnz, lambdas, policy, no_fused):
-    if no_fused:   # no segment lists: the per-problem fixed-point kernels and their column windows run
-        monkeypatch.setenv("MLEASE_NO_FUSED_K1", "1")
+def test_hessian_vector_matches_oracle(mb, n, D, nnz, lambdas, policy, no_fused):
     parts, data, _ = _sparse_parts(1, n, D, nnz, seed=D)
     rng = np.random.default_rng(3)
     w = rng.normal(0, 0.3, D + 1); q = rng.uniform(0.5, 2.0, D + 1); v = rng.normal(size=D + 1)
@@ -57,6 +57,9 @@ def test_hessian_vector_matches_oracle(mb, monkeypatch, n, D, nnz, lambdas, poli
             s.add_partition_csr(0, *parts[0])
             outs.append(s.hessian_vector(0, w, q, v))
             outs.append(s.hessian_vector(0, w, q, v))
+            if no_fused:   # a policy-2 batch is cheap to allocate: it shows the partition has no segment lists
+                s.begin()
+                assert s.stats()["k1_fused"] == 0
     # the oracle leaves the entries of features no row lists at 0 (it drops them from the dataset): there Hv = q v exactly
     present = np.zeros(D + 1, bool); present[parts[0][1]] = True; present[D] = True
     err = np.abs(outs[0] - ref)[present].max() / np.abs(ref).max()
@@ -73,16 +76,15 @@ def _part_csr(part, D):
 
 # (partitions, rows, features, stored values per row, lambdas, no segment lists): the ADMM batch of a policy-2 session through the
 # kernels its CG runs -- fused multi-lambda with 4- and 2-wide interleaved vectors, the per-problem fixed-point kernel with its
-# accumulators and v in shared memory (5 lambdas: no fused kernel) under the dynamic CTA mapping, and the column windows
+# accumulators and v in shared memory (5 lambdas: no fused kernel) under the dynamic CTA mapping, and the column windows (2 lambdas
+# at 30 001 columns: no segment lists, see test_hessian_vector_matches_oracle)
 @pytest.mark.parametrize("P,n,D,nnz,L,no_fused", [(2, 3000, 300, 12, 3, False), (2, 3000, 300, 12, 2, False), (2, 3000, 300, 12, 5, False),
                                                   (2, 2000, 30001, 60, 2, True)])
-def test_batch_hv_and_diagonal_match_oracle(mb, monkeypatch, P, n, D, nnz, L, no_fused):
+def test_batch_hv_and_diagonal_match_oracle(mb, P, n, D, nnz, L, no_fused):
     """Every (partition, lambda) problem at its own point w and vector v: a wrong lambda's v or d, or a wrong diagonal, fails here (the
     ADMM parity cases could not see it: any SPD model leads the line search to the same minimiser)."""
     import ctypes as C
     from mlease_b200._native import lib, ptr, check
-    if no_fused:
-        monkeypatch.setenv("MLEASE_NO_FUSED_K1", "1")
     parts, _, _ = _sparse_parts(P, n, D, nnz, seed=D + L)
     rng = np.random.default_rng(L)
     nprob = P * L
@@ -95,6 +97,7 @@ def test_batch_hv_and_diagonal_match_oracle(mb, monkeypatch, P, n, D, nnz, L, no
         for p, part in enumerate(parts):
             s.add_partition_csr(p, *part)
         s.begin()
+        assert s.stats()["k1_fused"] == (0 if no_fused or L > 4 else 1)
         for mode, name in ((1, "Hv"), (2, "hessian_diag")):
             outs = []
             for rep in range(2):

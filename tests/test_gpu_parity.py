@@ -46,13 +46,6 @@ def mb():
     return mlease_b200
 
 
-@pytest.fixture
-def no_fused_k1(monkeypatch):
-    """Partitions uploaded while this is set get no segment lists: the per-problem CSR kernels (fixed-point shared-memory
-    accumulation, column windows) run instead of the fused multi-lambda kernel."""
-    monkeypatch.setenv("MLEASE_NO_FUSED_K1", "1")
-
-
 @pytest.mark.parametrize("n,d,sparse", [(1000, 37, False), (777, 100, False), (300, 1100, False), (500, 2500, False), (1000, 50, True),
                                         (4000, 3000, True), (50, 20, True), (20000, 700, True)])
 def test_k1_objective_and_gradient(mb, n, d, sparse):
@@ -85,18 +78,21 @@ def test_k1_objective_and_gradient(mb, n, d, sparse):
 
 
 @pytest.mark.parametrize("n,d", [(1000, 50), (4000, 3000)])
-def test_k1_per_problem_csr_kernels_without_segment_lists(mb, no_fused_k1, n, d):
+def test_k1_per_problem_csr_kernels_without_segment_lists(mb, n, d):
     """The pre-fusion CSR K1 (two-word fixed-point accumulation with native integer shared-memory atomics) stays the path for
-    partitions without segment lists (more than 4 lambdas, feature spaces too wide for the builder): same parity gate."""
+    partitions without segment lists (more than 4 lambdas, feature spaces too wide for the builder): same parity gate.  A session
+    of 5 lambdas uploads its partitions without them."""
     X, y, w, o = _mk(n, d, seed=n + d, sparse=True)
     rng = np.random.default_rng(1)
     wv = rng.normal(0, 0.3, d + 1); pm = rng.normal(0, 0.3, d + 1); pv = rng.uniform(0.2, 2.0, d + 1)
     rp, ci, v = _csr_of(X)
-    with _session(mb, d) as s:
+    with _session(mb, d, lambdas=(0.1, 0.3, 1.0, 3.0, 10.0)) as s:
         s.add_partition_csr(0, rp, ci, v, y, w, o)
         f, g, _ = s.objective(0, wv, pm, 1.0 / pv)
         f2, g2, _ = s.objective(0, wv, pm, 1.0 / pv)
         x, _ = s.fit_partition(0, np.zeros(d + 1), pm, 1.0 / pv)
+        s.begin()
+        assert s.stats()["k1_fused"] == 0
     data = orc.Csr(rp, ci, v, y, w, o, d)
     f_ref, g_ref = orc.objective("grad", data, wv, pm, pv)
     assert abs(f - f_ref) <= 1e-5 * abs(f_ref) and np.abs(g - g_ref).max() <= 1e-5 * np.abs(g_ref).max()
@@ -141,12 +137,13 @@ def test_csr_rows_with_repeated_and_unsorted_columns(mb):
 
 
 @pytest.mark.parametrize("fused", [False, True])
-def test_csr_feature_space_wider_than_one_gradient_window(mb, monkeypatch, fused):
+def test_csr_feature_space_wider_than_one_gradient_window(mb, fused):
     """30 001 columns: the per-CTA fixed-point gradient (8 bytes per column) no longer fits shared memory in one piece, so
     K1 runs one launch for the margins + the first 28 128 columns and one more per further column window; the Gram tile
-    list, the DMMA factorisation and the fp32 inverse copy are exercised at ldh = 30 016 as well."""
-    if not fused:
-        monkeypatch.setenv("MLEASE_NO_FUSED_K1", "1")   # the column-window kernels; with segment lists the fused kernel takes 30k columns in one launch
+    list, the DMMA factorisation and the fp32 inverse copy are exercised at ldh = 30 016 as well.  With one lambda the
+    partition gets segment lists and the fused kernel takes the 30k columns in one launch; with two, the 2-wide interleaved
+    beta (240 032 B) does not fit a CTA's shared memory, so there are no lists and the column-window kernels run."""
+    lambdas = (1.0,) if fused else (1.0, 2.0)
     n, D, nnz = 3000, 30000, 8
     r = np.random.default_rng(12)
     ci = np.stack([np.sort(r.choice(D, nnz, replace=False)) for _ in range(n)]).astype(np.int32)
@@ -166,11 +163,20 @@ def test_csr_feature_space_wider_than_one_gradient_window(mb, monkeypatch, fused
     # their coefficient is the prior mean, :374-383): evaluate at a point that agrees with that, so that fun/grad compare
     absent = np.ones(D + 1, bool); absent[ci.reshape(-1)] = False; absent[D] = False
     wv[absent] = pm[absent]
-    with _session(mb, D) as s:
+    with _session(mb, D, lambdas) as s:
         s.add_partition_csr(0, rp, ci.reshape(-1), v.reshape(-1), y, w, o)
         f, g, _ = s.objective(0, wv, pm, 1.0 / pv)
+        l0 = s.stats()["kernel_launches"]
         f2, g2, _ = s.objective(0, wv, pm, 1.0 / pv)
+        launches = s.stats()["kernel_launches"] - l0
         x, steps = s.fit_partition(0, np.zeros(D + 1), pm, 1.0 / pv)
+    if not fused:   # the same upload with one lambda: the column windows are one launch more than the fused kernel's one
+        with _session(mb, D) as s1:
+            s1.add_partition_csr(0, rp, ci.reshape(-1), v.reshape(-1), y, w, o)
+            s1.objective(0, wv, pm, 1.0 / pv)
+            l0 = s1.stats()["kernel_launches"]
+            s1.objective(0, wv, pm, 1.0 / pv)
+            assert launches == s1.stats()["kernel_launches"] - l0 + 1, launches
     f_ref, g_ref = orc.objective("grad", data, wv, pm, pv)
     assert abs(f - f_ref) <= 1e-5 * abs(f_ref), (f, f_ref)
     assert np.abs(g - g_ref).max() <= 1e-5 * np.abs(g_ref).max(), np.abs(g - g_ref).max() / np.abs(g_ref).max()

@@ -57,9 +57,9 @@ def main():
     if os.environ.get("WHICH", "gram") == "cholesky":
         n, D = int(os.environ.get("ROWS", 100000)), 10000
         with session(n, D, 100) as s:
-            # factorisation + inverse of ONE 10k-wide system (MLEASE_MERGE_TF32=0 / 1: fp64 DMMA / TF32 merges of the inverse)
+            # factorisation + inverse of ONE 10k-wide system (factored direction: TF32 merges of the inverse)
             ms = s.time_kernel(0, "cholesky", reps=3)
-            print("cholesky+inverse ms per factorisation", ms, "MLEASE_MERGE_TF32", os.environ.get("MLEASE_MERGE_TF32", "default"))
+            print("cholesky+inverse ms per factorisation", ms)
         return
     # (rows, features, stored values per row): the row counts keep each upload near 10^8 stored values
     shapes = [(1_000_000, 10_000, 100), (1_000_000, 500, 100), (1_000_000, 10_000, 30), (1_000_000, 10_000, 150),
