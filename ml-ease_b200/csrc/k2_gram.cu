@@ -412,17 +412,44 @@ __global__ void __launch_bounds__(256) gram_csr_operand_kernel(const Problem* __
 // once to fp32.  The sum cannot overflow below
 // 2^27.4 rows (every row adds at most one product to a cell: rows have unique columns); gram_sparse_max_rows() states the limit
 // the batch rule applies.
-// One CTA per (128 x 128 lower tile (bi, bj), problem), one slice.  Each warp takes every SP_WARPS-th 32-row group; per group it
-// stages the bj run (row order: csr_bm_fill_kernel writes lane 0's entries, then lane 1's, ...) in shared memory with the start
-// and end of each row's entries, then every entry of the bi run multiplies the staged entries of its own row.  Diagonal tiles
-// use the pairs with c2 <= c1 only (the columns of a row's run increase) and mirror them in the epilogue.  Zero operand bytes
-// are skipped.  A bj run longer than SP_STAGE entries is staged in chunks, the bi run re-read for each.
+// One CTA per (128 x 128 lower tile (bi, bj), problem), one slice.  A warp's unit of work is a span of consecutive 32-row groups:
+// SP_SPAN (256 rows), fewer on denser data (gram_sparse_span: the mean range of a span must fit 3/4 of a stage chunk, since each
+// further chunk re-reads the bi range); warp w takes the spans w, w + SP_WARPS, ...  The list is block-major with ascending
+// groups, so a block's entries for a span are one contiguous range [offs[b][g0], offs[b][g0 + span]), in row order (group, then
+// row in group: csr_bm_fill_kernel writes lane 0's entries, then lane 1's, ...), and an entry's row in the span is
+// 32 (group - g0) + kmaj_row(key), its group found by walking the span's warp-uniform group bounds as the entries go by.  Per
+// span the warp stages the bj range's nonzero entries in shared memory with each row's [start, end), then enumerates the
+// (bi entry, staged partner of its row) pairs in a flat index space: per 32 bi entries an inclusive warp scan of the partner
+// counts, then steps of 32 pairs, one per lane, each lane finding its owner entry from one OR-reduction of the owners' end
+// positions in the step (owners are compacted to a per-warp table first).  So lanes stay busy however the partners are spread
+// over the rows, and a row with 128 entries in both blocks (128^2 pairs) is as many full steps.  A bj range longer than SP_STAGE
+// entries is staged in chunks (boundaries may fall inside a row: each chunk pairs with its own part of the row), the bi range
+// re-read for each.
+// What bounds it (1M x 10k x 1 %, H100 at 400 W, 46.5 ms a build): the per-entry work, not the products.  Each batch of 32
+// entries is ~90 instructions to stage (load, decode, group, ballot, row table) and as many to scan on the bi side, for ~1.3
+// products per entry.  In a 52 ms form of the kernel (fixed 8-group spans, loads consumed as soon as issued), leaving out the pair
+// steps left 35 ms, and leaving out the whole bi side too left 18 ms.
+// Diagonal tiles keep the pairs with c2 <= c1 only (predicated) and mirror them in the epilogue.  Zero operand bytes (w = 0
+// rows, the end of a range) are skipped.
+// Same-cell contention: every row's intercept entry pairs with itself in the intercept's diagonal tile, so consecutive rows'
+// (intercept, intercept) products would be one step of 32 same-address atomics.  A lane sums that cell's products in an int64
+// register instead, and the warp adds its total once at the end (the sum is exact, so the order does not matter).  In the other
+// intercept tiles (bi = the intercept's block) the intercept row's products spread over the 128 cells of bj: at ~1 partner per
+// row, a step's 32 lanes meet ~4 same-cell pairs, no worse than a bank conflict, so those are left to the atomics.
 // ------------------------------------------------------------------------------------------
 constexpr int SP_THREADS = 1024;
 constexpr int SP_WARPS = SP_THREADS / 32;
-constexpr int SP_STAGE = 256;                                      // staged bj entries per warp and chunk
+constexpr int SP_SPAN = 8;                                         // 32-row groups per span
+constexpr int SP_ROWS = SP_SPAN * 32;                              // rows per span: the row table's length
+constexpr int SP_AHEAD = 1;                                        // batches of 32 entries loaded ahead of use (2: slower)
+constexpr int SP_STAGE = 448;                                      // staged bj entries per warp and chunk (< 2^16: u16 row table)
 constexpr size_t SP_ACC_BYTES = (size_t)SN * SN * 2 * sizeof(uint32_t);   // 128 KB: low words, then high words
-constexpr size_t SP_SMEM = SP_ACC_BYTES + (size_t)SP_WARPS * SP_STAGE * 4 + (size_t)SP_WARPS * 64 * 2;
+// per warp: the stage (int), the row table (u32: start | end << 16) and the owner table (int2), 3 KB
+constexpr size_t SP_WARP_BYTES = (size_t)SP_STAGE * 4 + (size_t)SP_ROWS * 4 + 32 * 8;
+constexpr size_t SP_SMEM = SP_ACC_BYTES + (size_t)SP_WARPS * SP_WARP_BYTES;
+static_assert(SP_SMEM <= 227 * 1024, "sparse Gram shared memory");
+static_assert(SP_STAGE % 16 == 0 && SP_SPAN + 1 <= 16, "layout of the stage and of the span bounds");
+static_assert(SP_SPAN == 8 && SP_STAGE == 448, "gram_sparse_span (kernels.cuh) assumes these");
 
 // e4m3 byte -> signed integer number of units of 2^-9 (subnormal m: m units; normal (e, m): (8 + m) << (e - 1)).  0x7F / 0xFF
 // (NaN) never occur: the operand pass converts with __NV_SATFINITE.
@@ -443,14 +470,20 @@ gram_csr_sparse_kernel(const Problem* __restrict__ probs, const GramTile* __rest
   const bool diag = bi == bj;
   const int Dp = pb.Dp;
   const long long ngroups = pb.bm_groups;
+  const int span = gram_sparse_span(pb.bm_entries, pb.nblk128, ngroups);   // groups per span, <= SP_SPAN
+  const long long nspans = (ngroups + span - 1) / span;
+  // the intercept's cell (column Dt - 1, the last entry of every row) when this is its diagonal tile, else -1 (matches no column)
+  const int hot = diag && (pb.Dt - 1) / SN == bi ? (pb.Dt - 1) % SN : -1;
 
   extern __shared__ __align__(16) unsigned char g_smem_raw[];
   uint32_t* acc_lo = reinterpret_cast<uint32_t*>(g_smem_raw);   // [c1][c2]: low and high 32-bit words of an int64 sum
   int* acc_hi = reinterpret_cast<int*>(g_smem_raw) + SN * SN;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  int* stage = reinterpret_cast<int*>(g_smem_raw + SP_ACC_BYTES) + warp * SP_STAGE;   // (units << 7) | c2
-  unsigned short* rs = reinterpret_cast<unsigned short*>(g_smem_raw + SP_ACC_BYTES + (size_t)SP_WARPS * SP_STAGE * 4) + warp * 64;
-  unsigned short* re = rs + 32;   // a row's staged entries: [rs[r], re[r])
+  unsigned char* wsm = g_smem_raw + SP_ACC_BYTES + (size_t)warp * SP_WARP_BYTES;
+  int* stage = reinterpret_cast<int*>(wsm);                                // (units << 7) | c2
+  uint32_t* rtab = reinterpret_cast<uint32_t*>(wsm + SP_STAGE * 4);        // a row's staged entries [start, end): start | end << 16
+  unsigned short* rtab16 = reinterpret_cast<unsigned short*>(rtab);        // start of row r at 2 r, end at 2 r + 1
+  int2* own = reinterpret_cast<int2*>(wsm + SP_STAGE * 4 + SP_ROWS * 4);  // owners of a batch: ((units << 7) | c1, start - first pair)
 
   for (int e = threadIdx.x; e < SN * SN; e += SP_THREADS) { acc_lo[e] = 0u; acc_hi[e] = 0; }
   __syncthreads();
@@ -461,42 +494,75 @@ gram_csr_sparse_kernel(const Problem* __restrict__ probs, const GramTile* __rest
   const unsigned short* __restrict__ keys = pb.bm_keys;
   const unsigned char* __restrict__ bytes = pb.bm_e4m3;
   const uint32_t lt = (1u << lane) - 1u;
-  // the list holds < 2^32 entries (checked at upload): entry numbers are 32-bit.  Lanes 0..3 fetch the run bounds of a group
-  // (bi lo, bi hi, bj lo, bj hi) two groups ahead, and the first 64 entries of both runs are loaded one group ahead: a warp has one
-  // group in flight, so without this every group would wait out two or three dependent global-memory round trips.
-  auto ld_bounds = [&](long long g) -> uint32_t {
-    if (!valid || g >= ngroups || lane >= 4) return 0u;
-    return (uint32_t)__ldg((lane < 2 ? offs_i : offs_j) + g + (lane & 1));
+  // a cell gets the product p (units of 2^-18, int64): the low word with a native atomic add that returns the old word, the high
+  // word plus the carry out of the low add when that is not 0
+  auto add_cell = [&](int cell, long long p) {
+    const uint32_t lo = (uint32_t)p;
+    const uint32_t old = atomicAdd(acc_lo + cell, lo);
+    const int hi = (int)(p >> 32) + (old + lo < old ? 1 : 0);
+    if (hi != 0) atomicAdd(acc_hi + cell, hi);
   };
-  // an entry as (key << 8) | e4m3 byte; 0 past the end of its run (a zero byte: skipped like any zero operand)
-  auto ld_entry = [&](uint32_t e, uint32_t hi) -> uint32_t {
-    return e < hi ? ((uint32_t)__ldg(keys + e) << 8) | (uint32_t)__ldg(bytes + e) : 0u;
+  // the list holds < 2^32 entries (checked at upload): entry numbers are 32-bit.  A span's group bounds, lane-distributed: lane k
+  // (k <= span) holds offs_i[g0 + k], lane 16 + k offs_j[g0 + k], clamped to the last group (a short last span's missing groups
+  // are empty).  Fetched two spans ahead, and the first SP_AHEAD batches of 32 entries of both ranges one span ahead: a warp has
+  // one span in flight.  Inside a range the entries are loaded SP_AHEAD batches ahead: most bj ranges are not in L2 (a wave's
+  // tiles read ~80 different bj blocks), so a batch's loads need the time of several batches' work to arrive.
+  auto ld_bounds = [&](long long s) -> uint32_t {
+    const int k = lane & 15;
+    if (!valid || s >= nspans || k > span) return 0u;
+    return (uint32_t)__ldg((lane < 16 ? offs_i : offs_j) + min(s * span + k, ngroups));
   };
-  struct Group { uint32_t ilo, ihi, jlo, jhi, i[2], j[2]; };
-  auto take = [&](Group& q, uint32_t b) {
-    q.ilo = __shfl_sync(0xffffffffu, b, 0); q.ihi = __shfl_sync(0xffffffffu, b, 1);
-    q.jlo = __shfl_sync(0xffffffffu, b, 2); q.jhi = __shfl_sync(0xffffffffu, b, 3);
+  // an entry's key and e4m3 byte, both 0 past the end of its range (a zero byte: skipped like any zero operand).  Kept as the two
+  // loaded registers until the entry is used: an instruction that combined them at the load would wait for the load right there
+  struct Entry { uint32_t key, byte; };
+  auto ld_entry = [&](uint32_t e, uint32_t hi) -> Entry {
+    Entry x = {0u, 0u};
+    if (e < hi) { x.key = __ldg(keys + e); x.byte = __ldg(bytes + e); }
+    return x;
+  };
+  struct Span { uint32_t b; Entry i[SP_AHEAD], j[SP_AHEAD]; };
+  auto take = [&](Span& q, uint32_t b) {
+    q.b = b;
+    const uint32_t ilo = __shfl_sync(0xffffffffu, b, 0), ihi = __shfl_sync(0xffffffffu, b, span);
+    const uint32_t jlo = __shfl_sync(0xffffffffu, b, 16), jhi = __shfl_sync(0xffffffffu, b, 16 + span);
 #pragma unroll
-    for (int k = 0; k < 2; k++) { q.i[k] = ld_entry(q.ilo + lane + 32 * k, q.ihi); q.j[k] = ld_entry(q.jlo + lane + 32 * k, q.jhi); }
+    for (int k = 0; k < SP_AHEAD; k++) { q.i[k] = ld_entry(ilo + lane + 32 * k, ihi); q.j[k] = ld_entry(jlo + lane + 32 * k, jhi); }
   };
-  // entry base + lane of the run starting at lo (bound hi); base - lo is warp-uniform
-  auto entry = [&](uint32_t base, uint32_t lo, uint32_t hi, const uint32_t (&pre)[2]) -> uint32_t {
-    return base == lo ? pre[0] : base == lo + 32 ? pre[1] : ld_entry(base + lane, hi);
+  // group of entry e of a range, from its bounds (lane 16 * side + k): k is the next bound not yet passed and nb its value, so the
+  // batch's first entry is in group k - 1; every bound below lim (the end of the batch) adds one to the entries at or past it
+  auto group_of = [&](uint32_t e, uint32_t lim, const Span& q, int side, int& k, uint32_t& nb) -> int {
+    int g = k - 1;
+    while (k < span && nb < lim) {
+      g += e >= nb ? 1 : 0;
+      k++;
+      nb = __shfl_sync(0xffffffffu, q.b, 16 * side + k);
+    }
+    return g;
   };
-  auto run = [&](const Group& q) {
-    if (q.ilo == q.ihi || q.jlo == q.jhi) return;
-    for (uint32_t c0 = q.jlo; c0 < q.jhi; c0 += SP_STAGE) {
-      const uint32_t c1 = min(q.jhi, c0 + SP_STAGE);   // >= jlo + 64 or = jhi: the prefetched entries lie in the first chunk
+  long long hot_sum = 0;   // this lane's products of the intercept's cell
+  auto run = [&](const Span& q) {
+    const uint32_t ilo = __shfl_sync(0xffffffffu, q.b, 0), ihi = __shfl_sync(0xffffffffu, q.b, span);
+    const uint32_t jlo = __shfl_sync(0xffffffffu, q.b, 16), jhi = __shfl_sync(0xffffffffu, q.b, 16 + span);
+    if (ilo == ihi || jlo == jhi) return;
+    int jk = 1;
+    uint32_t jnb = __shfl_sync(0xffffffffu, q.b, 17);
+    for (uint32_t c0 = jlo; c0 < jhi; c0 += SP_STAGE) {
+      const uint32_t c1 = min(jhi, c0 + SP_STAGE);   // >= jlo + 32 * SP_AHEAD or = jhi: the prefetched batches lie in the first chunk
       __syncwarp();   // the previous chunk's readers are done
-      rs[lane] = 0; re[lane] = 0;
+#pragma unroll
+      for (int k = 0; k < SP_ROWS / 128; k++) reinterpret_cast<uint4*>(rtab)[lane + 32 * k] = make_uint4(0u, 0u, 0u, 0u);
       __syncwarp();
       // ---- stage the chunk's nonzero entries; a kept entry whose row differs from the previous kept one starts its row
       int nst = 0, prev_row = -1;
+      Entry x[SP_AHEAD + 1];   // the batches base, base + 32, ...
+#pragma unroll
+      for (int k = 0; k < SP_AHEAD; k++) x[k] = c0 == jlo ? q.j[k] : ld_entry(c0 + 32 * k + lane, c1);
       for (uint32_t base = c0; base < c1; base += 32) {
-        const uint32_t x = entry(base, q.jlo, c1, q.j);
-        const int v = e4m3_units(x & 255u);
-        const uint32_t key = x >> 8;
-        const int r = kmaj_row(key);
+        x[SP_AHEAD] = ld_entry(base + 32 * SP_AHEAD + lane, c1);
+        const int g = group_of(base + lane, min(base + 32, c1), q, 1, jk, jnb);
+        const int v = e4m3_units(x[0].byte);
+        const uint32_t key = x[0].key;
+        const int r = 32 * g + kmaj_row(key);
         const bool keep = v != 0;
         const uint32_t m = __ballot_sync(0xffffffffu, keep);
         const uint32_t below = m & lt;
@@ -505,44 +571,76 @@ gram_csr_sparse_kernel(const Problem* __restrict__ probs, const GramTile* __rest
         const int s = nst + __popc(below);
         if (keep) {
           stage[s] = v * 128 + (int)(key >> 5);
-          if (r != pr) { rs[r] = (unsigned short)s; if (pr >= 0) re[pr] = (unsigned short)s; }
+          if (r != pr) { rtab16[2 * r] = (unsigned short)s; if (pr >= 0) rtab16[2 * pr + 1] = (unsigned short)s; }
         }
         if (m) prev_row = __shfl_sync(0xffffffffu, r, 31 - __clz(m));
         nst += __popc(m);
+#pragma unroll
+        for (int k = 0; k < SP_AHEAD; k++) x[k] = x[k + 1];
       }
       if (nst == 0) continue;
-      if (lane == 0) re[prev_row] = (unsigned short)nst;
+      if (lane == 0) rtab16[2 * prev_row + 1] = (unsigned short)nst;
       __syncwarp();
-      // ---- every bi entry times the staged entries of its row
-      for (uint32_t base = q.ilo; base < q.ihi; base += 32) {
-        const uint32_t x = entry(base, q.ilo, q.ihi, q.i);
-        const int a = e4m3_units(x & 255u);
-        if (a == 0) continue;
-        const uint32_t key = x >> 8;
-        const int r = kmaj_row(key), col = (int)(key >> 5);
-        const int row = col * SN;
-        const int s1 = re[r];
-        for (int s = rs[r]; s < s1; s++) {
-          const int p = stage[s];
-          const int c2 = p & 127;
-          if (diag && c2 > col) break;
-          const long long prod = (long long)a * (long long)(p >> 7);
-          const uint32_t lo = (uint32_t)prod;
-          const uint32_t old = atomicAdd(acc_lo + row + c2, lo);
-          const int hi = (int)(prod >> 32) + (old + lo < old ? 1 : 0);
-          if (hi != 0) atomicAdd(acc_hi + row + c2, hi);
+      // ---- the (bi entry, staged partner) pairs, 32 bi entries at a time
+      int ik = 1;
+      uint32_t inb = __shfl_sync(0xffffffffu, q.b, 1);
+#pragma unroll
+      for (int k = 0; k < SP_AHEAD; k++) x[k] = q.i[k];
+      for (uint32_t base = ilo; base < ihi; base += 32) {
+        x[SP_AHEAD] = ld_entry(base + 32 * SP_AHEAD + lane, ihi);
+        const int g = group_of(base + lane, min(base + 32, ihi), q, 0, ik, inb);
+        const int a = e4m3_units(x[0].byte);
+        const uint32_t key = x[0].key;
+        const uint32_t t = a != 0 ? rtab[32 * g + kmaj_row(key)] : 0u;
+        const int s0 = (int)(t & 0xFFFFu), cnt = (int)(t >> 16) - s0;
+        int incl = cnt;   // inclusive warp scan of the partner counts
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+          const int u = __shfl_up_sync(0xffffffffu, incl, d);
+          if (lane >= d) incl += u;
+        }
+        const int total = __shfl_sync(0xffffffffu, incl, 31);
+#pragma unroll
+        for (int k = 0; k < SP_AHEAD; k++) x[k] = x[k + 1];
+        if (total == 0) continue;
+        // owners (entries with partners) in lane order: pair p belongs to the owner of rank #{owners whose pairs end at or before p}
+        const uint32_t owners = __ballot_sync(0xffffffffu, cnt > 0);
+        __syncwarp();   // the previous batch's readers of own[] are done
+        if (cnt > 0) own[__popc(owners & lt)] = make_int2(a * 128 + (int)(key >> 5), s0 - (incl - cnt));
+        __syncwarp();
+        int before = 0;   // owners whose pairs end before this step
+        for (int p0 = 0; p0 < total; p0 += 32) {
+          const int end = incl - p0;
+          const uint32_t ends = __reduce_or_sync(0xffffffffu, cnt > 0 && end >= 0 && end < 32 ? 1u << end : 0u);
+          const int p = p0 + lane;
+          if (p < total) {
+            const int2 o = own[before + __popc(ends & (0xFFFFFFFFu >> (31 - lane)))];
+            const int pv = stage[p + o.y];
+            const int c1 = o.x & 127, c2 = pv & 127;
+            if (!diag || c2 <= c1) {
+              const long long prod = (long long)(o.x >> 7) * (long long)(pv >> 7);
+              if (c2 == hot && c1 == hot) hot_sum += prod;
+              else add_cell(c1 * SN + c2, prod);
+            }
+          }
+          before += __popc(ends);
         }
       }
     }
   };
-  Group cur, nxt;
+  Span cur, nxt;
   take(cur, ld_bounds(warp));
   uint32_t nb = ld_bounds(warp + SP_WARPS);
-  for (long long g = warp; g < ngroups; g += SP_WARPS) {
-    take(nxt, nb);   // the next group's loads are in flight while this one runs
-    nb = ld_bounds(g + 2 * SP_WARPS);
+  for (long long s = warp; s < nspans; s += SP_WARPS) {
+    take(nxt, nb);   // the next span's loads are in flight while this one runs
+    nb = ld_bounds(s + 2 * SP_WARPS);
     run(cur);
     cur = nxt;
+  }
+  if (hot >= 0) {
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) hot_sum += __shfl_down_sync(0xffffffffu, hot_sum, d);
+    if (lane == 0 && hot_sum != 0) add_cell(hot * SN + hot, hot_sum);
   }
   __syncthreads();
   // ---- one rounding per cell: units of 2^-18 -> fp32

@@ -249,17 +249,21 @@ static double gram_path_bytes(const Batch& B) {
 // Cost of one CSR Gram build of a partition (seconds; only the comparison matters).  Both kernels read each 128-column block's
 // run of every 32-row group once per tile it belongs to (nblk + 1 tiles: `reads` entries in all).  wgmma: every 128 x 128 lower
 // tile times every 32-row group on the tensor pipe, plus the producers' run loads, which is what makes its rate fall at small n
-// and high density.  Sparse: per product (integer multiply + native shared atomic add), per (tile, group) visit (staging the
-// runs) and per entry read, with the whole device busy; a grid of fewer CTAs than SMs is that much slower.  Least-squares fits
-// of tools/time_gram.py on an H100 SXM at 700 W over 0.3 - 20 % density at 10k features (DESIGN.md section 4): within 15 % on
-// every shape, so near the crossover (~3 % at 10k features) the rule may pick a kernel up to ~15 % slower than the other.
-constexpr double GRAM_WGMMA_S_PER_MAC = 1.30e-15, GRAM_WGMMA_S_PER_READ = 4.26e-12;
-constexpr double GRAM_SPARSE_S_PER_PAIR = 2.69e-12, GRAM_SPARSE_S_PER_VISIT = 2.47e-10, GRAM_SPARSE_S_PER_READ = 1.36e-12;
+// and high density.  Sparse: per product (integer multiply + native shared atomic add), per (tile, span) visit (gram_sparse_span
+// groups: fetching and walking the span's bounds) and per entry read (loading, decoding and staging or scanning it), with the
+// whole device busy; a grid of fewer CTAs than SMs is that much slower.  Relative least-squares fits of tools/time_gram.py on an
+// H100 80GB HBM3 at a 400 W power limit over 0.3 - 20 % density at 10k features (DESIGN.md section 4): the sparse model is within
+// 3.5 % and the wgmma model within 9.5 % of every measured shape, so near the crossover (~3 % at 10k features) the rule may pick
+// a kernel up to ~10 % slower than the other.
+constexpr double GRAM_WGMMA_S_PER_MAC = 1.317e-15, GRAM_WGMMA_S_PER_READ = 4.315e-12;
+constexpr double GRAM_SPARSE_S_PER_PAIR = 1.822e-12, GRAM_SPARSE_S_PER_VISIT = 4.652e-10, GRAM_SPARSE_S_PER_READ = 3.716e-12;
 static double gram_cost(const Problem& p, int Dp, int kind, double ctas, int num_sms) {
   const double nblk = Dp / 128, tiles = nblk * (nblk + 1) / 2, groups = (double)((p.n + 31) / 32);
+  const int span = gram_sparse_span(p.bm_entries, Dp / 128, (p.n + 31) / 32);
+  const double spans = (double)(((p.n + 31) / 32 + span - 1) / span);
   const double reads = (nblk + 1) * (double)p.bm_entries;
   if (kind == CSR_GRAM_WGMMA) return tiles * 128.0 * 128.0 * 32.0 * groups * GRAM_WGMMA_S_PER_MAC + reads * GRAM_WGMMA_S_PER_READ;
-  return (p.gram_pairs * GRAM_SPARSE_S_PER_PAIR + tiles * groups * GRAM_SPARSE_S_PER_VISIT + reads * GRAM_SPARSE_S_PER_READ) *
+  return (p.gram_pairs * GRAM_SPARSE_S_PER_PAIR + tiles * spans * GRAM_SPARSE_S_PER_VISIT + reads * GRAM_SPARSE_S_PER_READ) *
          std::max(1.0, num_sms / std::max(1.0, ctas));
 }
 
