@@ -267,6 +267,23 @@ int mlease_score(int32_t device, void* stream, int32_t num_features, int64_t nro
 int mlease_test_loglik(int32_t device, void* stream, int64_t nrows, const int32_t* response, const float* pred,
                        const float* weight, int64_t combiner_block, float* out_loglik, double* out_count);
 
+/* ItemModelTest (jobs/ItemModelTest.java:181-211): the rows of key k are [key_rowstart[k], key_rowstart[k+1]) of one CSR (rowptr
+ * [nrows+1] int64, colidx < num_features, any order, repeats add; vals; offset [nrows] or NULL); key_rowstart[0] = 0 and
+ * nrows = key_rowstart[num_keys].  Model m = l*num_keys + k is entries [model_ptr[m], model_ptr[m+1]) of model_col (strictly
+ * ascending within a model, checked; num_features = the intercept) and model_val (float).  An empty model is the reference's empty
+ * LinearModel: pred = float(offset).  binary_feature: every listed feature counts as 1.  pred [num_lambdas][nrows]; every pred is
+ * bitwise what mlease_score gives on its key's rows with its key's model widened to double.  All pointers host-or-device. */
+int mlease_score_keyed(int32_t device, void* stream, int32_t num_features, int32_t num_keys, const int64_t* key_rowstart,
+                       const int64_t* rowptr, const int32_t* colidx, const float* vals, const float* offset, int32_t num_lambdas,
+                       const int64_t* model_ptr, const int32_t* model_col, const float* model_val, int32_t binary_feature, float* pred);
+/* ItemModelTestLoglik (jobs/ItemModelTestLoglik.java:60-142): entry e = one (record, pred-map key) pair: entry_key[e] in
+ * [0, num_keys), entry_group[e] = combiner group (non-decreasing), the record's response (1, 0, -1) and weight (NULL = 1), pred[e].
+ * out_loglik / out_count [num_keys] (host): reducer float(sum of float combiner partials / sum of counts), partials added in group
+ * order; a key without entries gets count 0 and loglik NaN.  Deterministic. */
+int mlease_test_loglik_keyed(int32_t device, void* stream, int64_t nentries, const int32_t* entry_key, const int32_t* entry_group,
+                             const int32_t* response, const float* weight, const float* pred, int32_t num_keys,
+                             float* out_loglik, double* out_count);
+
 /* Bench / profiling hooks (not part of the reference surface): time one fused K1 pass or one Gram build
  * on a resident partition with CUDA events on the session stream, `reps` launches, returns avg ms. */
 int mlease_time_kernel(mlease_session* s, int32_t partition_id, int32_t which /*1=K1,2=Gram wgmma,3=cholesky,4=Hv pass*/,

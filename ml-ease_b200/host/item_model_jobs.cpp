@@ -1,0 +1,167 @@
+// item_model_jobs.cpp -- ItemModelTest (jobs/ItemModelTest.java:53-248) and ItemModelTestLoglik (jobs/ItemModelTestLoglik.java:40-142):
+// per-key scoring of RegressionNaiveTrain's "<lambda>#<key>" models and one test log-likelihood per key.  Reached through
+// mlease_job_run (register_job).
+#include <atomic>
+#include <cmath>
+
+#include "jobs_common.hpp"
+
+namespace mlease_jobs {
+namespace {
+
+// ============================================================================================ ItemModelTest
+// The records of one file as union-free bytes (transcode_plain), one string per record.  False when the schema or a record is
+// not plain; the generic encoder then writes the job's output.
+bool plain_records(const std::string& file, std::vector<std::string>& out) {
+  AvroFile af(file);
+  Plan plan;
+  try { plan = plan_build(*af.schema()); } catch (const std::exception&) { return false; }
+  {
+    const Plan* p = &plan;
+    while (p->type == Schema::Union) { const Plan* nx = nullptr; for (auto& k : p->kids) if (k.type != Schema::Null) { nx = &k; break; } if (!nx) return false; p = nx; }
+    if (p->type != Schema::Record) return false;
+  }
+  const size_t nb = af.num_blocks();
+  std::vector<std::vector<std::string>> parts(nb);
+  std::atomic<bool> plain{true};
+  parallel_blocks(nb, host_threads(), [&](size_t b) {
+    if (!plain.load()) return;
+    const std::string data = af.block_data(b);
+    const uint8_t* p = reinterpret_cast<const uint8_t*>(data.data());
+    const uint8_t* e = p + data.size();
+    try {
+      for (int64_t q = 0; q < af.block_records(b); q++) { std::string o; transcode_plain(plan, p, e, o); parts[b].push_back(std::move(o)); }
+    } catch (const NotPlain&) { plain.store(false); }
+  });
+  if (!plain.load()) return false;
+  for (auto& v : parts) for (auto& r : v) out.push_back(std::move(r));
+  return true;
+}
+
+// jobs/ItemModelTest.java:65-248.  Records are grouped by item key in Avro string order (unsigned bytes); inside a key they keep
+// input order (files in listing order, records in file order).  One mlease_score_keyed call scores every lambda.
+void run_item_model_test(const JobConfig& c) {
+  const std::string in = c.get("input.paths"), outBase = c.get("output.base.path"), itemKey = c.get("item.key");
+  const bool ignore_value = c.get_bool("binary.feature", false);
+  const std::vector<std::string> lams = c.get_list("lambda");
+  const int L = (int)lams.size();
+  const auto files = list_avro_files(in);
+  if (files.empty()) io_error("no input files under " + in);
+  Dictionary td; Rows rows;
+  for (auto& f : files) read_raw(f, td, rows, ignore_value, itemKey);
+  const size_t n = rows.n();
+  std::vector<size_t> order(n);
+  for (size_t i = 0; i < n; i++) order[i] = i;
+  std::stable_sort(order.begin(), order.end(), [&](size_t a, size_t b) { return rows.key[a] < rows.key[b]; });
+  std::vector<std::string> knames;
+  std::vector<int64_t> krs{0}, rp{0};
+  std::vector<int32_t> ci; std::vector<float> vv, oo;
+  for (size_t q = 0; q < n; q++) {
+    const size_t i = order[q];
+    if (q > 0 && rows.key[i] != rows.key[order[q - 1]]) krs.push_back((int64_t)q);
+    if (q == 0 || rows.key[i] != rows.key[order[q - 1]]) knames.push_back(rows.key[i]);
+    for (int64_t j = rows.rowptr[i]; j < rows.rowptr[i + 1]; j++) { ci.push_back(rows.colidx[j]); vv.push_back(rows.vals[j]); }
+    rp.push_back((int64_t)ci.size());
+    oo.push_back(rows.offset[i]);
+  }
+  if (n) krs.push_back((int64_t)n);
+  const int K = (int)knames.size();
+  // model "String.valueOf(float lambda)#itemKey" (:187); its features mapped to the test dictionary, the ones the test data never
+  // lists dropped (they cannot contribute), "(INTERCEPT)" to column Dg.  A key without a model gets the empty model (:189-197).
+  const int Dg = std::max<int>((int)td.names.size(), 1);
+  const auto models = read_linear_models(c.get("model.path"), true);
+  std::vector<int64_t> mp{0}; std::vector<int32_t> mc; std::vector<float> mv;
+  std::vector<std::pair<int32_t, float>> ent;
+  for (int l = 0; l < L; l++) {
+    const std::string prefix = java_float_to_string(std::stof(lams[l])) + "#";
+    for (int k = 0; k < K; k++) {
+      auto it = models.find(prefix + knames[k]);
+      if (it != models.end()) {
+        ent.clear();
+        for (auto& fv : it->second) {
+          if (fv.first == INTERCEPT) ent.emplace_back(Dg, (float)fv.second);
+          else if (const int id = td.find(fv.first); id >= 0) ent.emplace_back(id, (float)fv.second);
+        }
+        std::sort(ent.begin(), ent.end());
+        for (auto& e : ent) { mc.push_back(e.first); mv.push_back(e.second); }
+      }
+      mp.push_back((int64_t)mc.size());
+    }
+  }
+  std::vector<float> pred((size_t)L * n);
+  ck(mlease_score_keyed(c.get_int("gpu.device", 0), nullptr, Dg, K, krs.data(), rp.data(), ci.data(), vv.data(), oo.data(), L, mp.data(),
+                        mc.data(), mv.data(), ignore_value ? 1 : 0, pred.data()));
+  // output: every input field (unions removed) + pred, schema PerItemTestOutput (:214-248)
+  AvroReader first(files[0]);
+  for (size_t f = 1; f < files.size(); f++)
+    if (AvroReader(files[f]).schema_json() != first.schema_json()) io_error("input files of one ItemModelTest job must share one schema: " + files[f]);
+  const std::string schema = test_output_schema(first.schema(), "PerItemTestOutput", "com.linkedin.lab.regression.avro");
+  std::vector<std::string> plain;
+  bool fast = !host_generic_ingest();
+  for (size_t f = 0; fast && f < files.size(); f++) fast = plain_records(files[f], plain);
+  std::vector<Value> recs;
+  if (!fast) {
+    for (auto& f : files) { AvroReader rd(f); Value v; while (rd.next(v)) recs.push_back(v); }
+  }
+  for (int l = 0; l < L; l++) {
+    AvroWriter w(outBase + "/lambda-" + lams[l] + "/part-r-00000.avro", schema);
+    const float* pl = pred.data() + (size_t)l * n;
+    std::string rec;
+    for (size_t q = 0; q < n; q++) {
+      const size_t i = order[q];
+      if (fast) { rec = plain[i]; put_float(rec, pl[q]); w.append_encoded(rec.data(), rec.size(), 1); }
+      else { Value r = recs[i]; r.items.push_back(Value::of_float(pl[q])); w.append(r); }
+    }
+    w.close();
+  }
+}
+
+// ============================================================================================ ItemModelTestLoglik
+// jobs/ItemModelTestLoglik.java:60-142: one loglik per pred-map key.  One map task, hence one combiner group, per input file.
+void run_item_model_test_loglik(const JobConfig& c) {
+  const std::string in = c.get("input.paths"), out = c.get("output.path");
+  std::vector<std::string> ekey;
+  std::vector<int32_t> egroup, eresp;
+  std::vector<float> ew, ep;
+  int g = 0;
+  for (auto& f : list_avro_files(in)) {
+    AvroReader rd(f);
+    const Schema& s = rec_schema(rd.schema());
+    Value rec;
+    while (rd.next(rec)) {
+      const Value* r = field(rec, s, "response");
+      const Value* pm = field(rec, s, "pred");
+      if (!r || !pm) io_error("response/pred is null");
+      const int resp = (int)num_of(*r);
+      if (resp != 1 && resp != 0 && resp != -1) io_error("response should be 1,0 or -1!");   // :74-77
+      if (pm->type != Schema::Map) io_error("pred is not a map<string, float>");
+      const Value* w = field(rec, s, "weight");
+      const float wt = w ? (float)num_of(*w) : 1.0f;
+      for (auto& e : pm->items) { ekey.push_back(e.map_key); egroup.push_back(g); eresp.push_back(resp); ew.push_back(wt); ep.push_back((float)num_of(e)); }
+    }
+    g++;
+  }
+  std::map<std::string, int32_t> ids;   // key order of the reducer's output
+  for (auto& k : ekey) ids.emplace(k, 0);
+  int32_t K = 0;
+  for (auto& kv : ids) kv.second = K++;
+  std::vector<int32_t> eid(ekey.size());
+  for (size_t e = 0; e < ekey.size(); e++) eid[e] = ids[ekey[e]];
+  std::vector<float> ll(K); std::vector<double> cnt(K);
+  if (!eid.empty())
+    ck(mlease_test_loglik_keyed(c.get_int("gpu.device", 0), nullptr, (int64_t)eid.size(), eid.data(), egroup.data(), eresp.data(), ew.data(), ep.data(), K,
+                                ll.data(), cnt.data()));
+  AvroWriter w(out + "/part-r-00000.avro", SCHEMA_TEST_LOGLIK);
+  for (auto& kv : ids) {
+    Value r; r.type = Schema::Record;
+    r.items = {Value::of_string(kv.first), Value::of_float(ll[kv.second]), Value::of_double(cnt[kv.second])};
+    w.append(r);
+  }
+  w.close();
+}
+
+[[maybe_unused]] const bool registered = register_job("ItemModelTest", run_item_model_test) &&
+                                         register_job("ItemModelTestLoglik", run_item_model_test_loglik);
+
+}  // namespace
+}  // namespace mlease_jobs

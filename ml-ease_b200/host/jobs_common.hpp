@@ -1,0 +1,134 @@
+// jobs_common.hpp -- what the job translation units of the host layer share: the job config, the record containers, the
+// readers and writers of regression_jobs.cpp that other jobs reuse, and the registry through which jobs defined outside
+// regression_jobs.cpp are reached by mlease_job_run.
+#pragma once
+#include <algorithm>
+#include <fstream>
+#include <map>
+#include <stdexcept>
+#include <string>
+#include <unordered_map>
+#include <vector>
+
+#include "../../include/mlease_b200.h"
+#include "avro_io.hpp"
+#include "avro_walk.hpp"
+
+namespace mlease_jobs {
+using namespace mlease_host;
+
+struct JobError : std::runtime_error { using std::runtime_error::runtime_error; };
+[[noreturn]] void io_error(const std::string& m);
+void ck(int rc);   // non-zero status of the device library -> JobError with its message
+
+// ------------------------------------------------------------------------------------------ JobConfig
+struct JobConfig {
+  std::map<std::string, std::string> kv;
+  static std::string trim(const std::string& s) {
+    size_t a = s.find_first_not_of(" \t\r\n"), b = s.find_last_not_of(" \t\r\n");
+    return a == std::string::npos ? "" : s.substr(a, b - a + 1);
+  }
+  // java.util.Properties subset: key=value | key:value | key value, '#'/'!' comments, trailing '\' continuation
+  static JobConfig load(const std::string& file) {
+    std::ifstream f(file);
+    if (!f) io_error("cannot open job config " + file);
+    JobConfig c;
+    std::string line, acc;
+    while (std::getline(f, line)) {
+      std::string t = trim(line);
+      if (acc.empty() && (t.empty() || t[0] == '#' || t[0] == '!')) continue;
+      if (!t.empty() && t.back() == '\\') { acc += t.substr(0, t.size() - 1); continue; }
+      acc += t;
+      size_t p = acc.find_first_of("=: \t");
+      std::string k = p == std::string::npos ? acc : acc.substr(0, p);
+      std::string v = p == std::string::npos ? "" : acc.substr(p);
+      size_t q = v.find_first_not_of(" \t");
+      if (q != std::string::npos && (v[q] == '=' || v[q] == ':')) v = v.substr(q + 1);
+      c.kv[trim(k)] = trim(v);
+      acc.clear();
+    }
+    return c;
+  }
+  bool has(const std::string& k) const { return kv.count(k) > 0; }
+  std::string get(const std::string& k) const {
+    auto it = kv.find(k);
+    if (it == kv.end()) io_error("Key " + k + " is not in the job config");   // JobConfig.getString(key) on a missing key
+    return it->second;
+  }
+  std::string get(const std::string& k, const std::string& d) const { auto it = kv.find(k); return it == kv.end() ? d : it->second; }
+  int get_int(const std::string& k) const { return std::stoi(get(k)); }
+  int get_int(const std::string& k, int d) const { return has(k) ? std::stoi(get(k)) : d; }
+  double get_double(const std::string& k, double d) const { return has(k) ? std::stod(get(k)) : d; }
+  float get_float(const std::string& k, float d) const { return has(k) ? std::stof(get(k)) : d; }
+  bool get_bool(const std::string& k, bool d) const {
+    if (!has(k)) return d;
+    std::string v = get(k);
+    std::transform(v.begin(), v.end(), v.begin(), ::tolower);
+    return v == "true" || v == "1";
+  }
+  std::vector<std::string> get_list(const std::string& k, const std::string& sep = ",") const {
+    std::vector<std::string> out;
+    std::string v = get(k);
+    size_t st = 0;
+    while (true) {
+      size_t p = v.find(sep, st);
+      std::string tok = trim(v.substr(st, p == std::string::npos ? std::string::npos : p - st));
+      if (!tok.empty()) out.push_back(tok);
+      if (p == std::string::npos) break;
+      st = p + sep.size();
+    }
+    return out;
+  }
+};
+
+struct Dictionary {
+  std::unordered_map<std::string, int> idx;
+  std::vector<std::string> names;
+  int add(const std::string& n) { auto it = idx.find(n); if (it != idx.end()) return it->second; int i = (int)names.size(); idx.emplace(n, i); names.push_back(n); return i; }
+  int find(const std::string& n) const { auto it = idx.find(n); return it == idx.end() ? -1 : it->second; }
+};
+
+// one prepared record stream in CSR form (global dictionary ids)
+struct Rows {
+  std::vector<std::string> key;
+  std::vector<int32_t> response;
+  std::vector<float> weight, offset;
+  std::vector<int64_t> rowptr{0};
+  std::vector<int32_t> colidx;
+  std::vector<float> vals;
+  size_t n() const { return response.size(); }
+};
+
+inline const std::string INTERCEPT = "(INTERCEPT)";
+
+// Avro binary primitives for the writers that encode records directly (no Value tree)
+inline void put_long(std::string& o, int64_t v) {
+  uint64_t z = ((uint64_t)v << 1) ^ (uint64_t)(v >> 63);
+  while (z & ~0x7FULL) { o.push_back((char)((z & 0x7F) | 0x80)); z >>= 7; }
+  o.push_back((char)z);
+}
+inline void put_str(std::string& o, const char* p, size_t n) { put_long(o, (int64_t)n); o.append(p, n); }
+inline void put_float(std::string& o, float f) { o.append(reinterpret_cast<const char*>(&f), 4); }
+
+extern const char* SCHEMA_TEST_LOGLIK;
+
+// regression_jobs.cpp
+std::string java_float_to_string(float f);
+double num_of(const Value& v);
+const Value* field(const Value& rec, const Schema& s, const std::string& name);
+const Schema& rec_schema(const SchemaP& s);
+bool host_generic_ingest();
+// raw (unprepared) records of one file -> rows; item_key non-empty: rows.key = data.get(item_key).toString()
+void read_raw(const std::string& file, Dictionary& dict, Rows& rows, bool binary_feature, const std::string& item_key = "");
+std::map<std::string, std::unordered_map<std::string, double>> read_linear_models(const std::string& path, bool last_wins = false);
+// RegressionTest-style output schema: input fields with unions removed + pred:float
+std::string test_output_schema(const SchemaP& in, const char* name = "AdmmTestOutput", const char* ns = nullptr);
+// a record's bytes with the union branch indices dropped; throws NotPlain when the record is not plain
+struct NotPlain {};
+void transcode_plain(const Plan& pl, const uint8_t*& p, const uint8_t* e, std::string& o);
+
+// job_class -> job for mlease_job_run; returns true (for use in a namespace-scope initializer)
+using JobFn = void (*)(const JobConfig&);
+bool register_job(const std::string& job_class, JobFn run);
+
+}  // namespace mlease_jobs

@@ -8,6 +8,7 @@
 //   RegressionTest        jobs/RegressionTest.java:65-170
 //   RegressionTestLoglik  jobs/RegressionTestLoglik.java:57-201
 //   RegressionNaiveTrain  jobs/RegressionNaiveTrain.java:99-415 (+ jobs/PartitionIdAssigner.java:41-101)
+//   ItemModelTest, ItemModelTestLoglik: item_model_jobs.cpp
 //   JobConfig             com/linkedin/mapred/JobConfig.java:50-224 (java .properties file)
 // Not mirrored: Hadoop job submission, HDFS, DistributedCache (local files only; is.local is implied).
 #include <algorithm>
@@ -22,78 +23,15 @@
 #include <unordered_map>
 
 #include "../../include/mlease_b200.h"
-#include "avro_io.hpp"
-#include "avro_walk.hpp"
+#include "jobs_common.hpp"
 
-using namespace mlease_host;
-
-namespace {
+namespace mlease_jobs {
 
 thread_local std::string g_job_err;
 
-struct JobError : std::runtime_error { using std::runtime_error::runtime_error; };
 [[noreturn]] void io_error(const std::string& m) { throw JobError(m); }
 void ck(int rc) { if (rc != 0) io_error(std::string(mlease_last_error())); }
 
-// ------------------------------------------------------------------------------------------ JobConfig
-struct JobConfig {
-  std::map<std::string, std::string> kv;
-  static std::string trim(const std::string& s) {
-    size_t a = s.find_first_not_of(" \t\r\n"), b = s.find_last_not_of(" \t\r\n");
-    return a == std::string::npos ? "" : s.substr(a, b - a + 1);
-  }
-  // java.util.Properties subset: key=value | key:value | key value, '#'/'!' comments, trailing '\' continuation
-  static JobConfig load(const std::string& file) {
-    std::ifstream f(file);
-    if (!f) io_error("cannot open job config " + file);
-    JobConfig c;
-    std::string line, acc;
-    while (std::getline(f, line)) {
-      std::string t = trim(line);
-      if (acc.empty() && (t.empty() || t[0] == '#' || t[0] == '!')) continue;
-      if (!t.empty() && t.back() == '\\') { acc += t.substr(0, t.size() - 1); continue; }
-      acc += t;
-      size_t p = acc.find_first_of("=: \t");
-      std::string k = p == std::string::npos ? acc : acc.substr(0, p);
-      std::string v = p == std::string::npos ? "" : acc.substr(p);
-      size_t q = v.find_first_not_of(" \t");
-      if (q != std::string::npos && (v[q] == '=' || v[q] == ':')) v = v.substr(q + 1);
-      c.kv[trim(k)] = trim(v);
-      acc.clear();
-    }
-    return c;
-  }
-  bool has(const std::string& k) const { return kv.count(k) > 0; }
-  std::string get(const std::string& k) const {
-    auto it = kv.find(k);
-    if (it == kv.end()) io_error("Key " + k + " is not in the job config");   // JobConfig.getString(key) on a missing key
-    return it->second;
-  }
-  std::string get(const std::string& k, const std::string& d) const { auto it = kv.find(k); return it == kv.end() ? d : it->second; }
-  int get_int(const std::string& k) const { return std::stoi(get(k)); }
-  int get_int(const std::string& k, int d) const { return has(k) ? std::stoi(get(k)) : d; }
-  double get_double(const std::string& k, double d) const { return has(k) ? std::stod(get(k)) : d; }
-  float get_float(const std::string& k, float d) const { return has(k) ? std::stof(get(k)) : d; }
-  bool get_bool(const std::string& k, bool d) const {
-    if (!has(k)) return d;
-    std::string v = get(k);
-    std::transform(v.begin(), v.end(), v.begin(), ::tolower);
-    return v == "true" || v == "1";
-  }
-  std::vector<std::string> get_list(const std::string& k, const std::string& sep = ",") const {
-    std::vector<std::string> out;
-    std::string v = get(k);
-    size_t st = 0;
-    while (true) {
-      size_t p = v.find(sep, st);
-      std::string tok = trim(v.substr(st, p == std::string::npos ? std::string::npos : p - st));
-      if (!tok.empty()) out.push_back(tok);
-      if (p == std::string::npos) break;
-      st = p + sep.size();
-    }
-    return out;
-  }
-};
 
 // ------------------------------------------------------------------------------------------ Java string semantics
 // Float.toString / String.valueOf(float): model keys "1.0", "1.0#3" (jobs/RegressionAdmmTrain.java:184,650)
@@ -182,7 +120,6 @@ const char* SCHEMA_LAMBDA_RHO = "{\"type\":\"record\",\"name\":\"LambdaRhoMap\",
 const char* SCHEMA_SAMPLE_LOGLIK = "{\"type\":\"record\",\"name\":\"SampleTestLoglik\",\"namespace\":\"com.linkedin.mlease.regression.avro\",\"fields\":[{\"name\":\"lambda\",\"type\":\"string\"},{\"name\":\"iter\",\"type\":\"int\"},{\"name\":\"testLoglik\",\"type\":\"float\"}]}";
 const char* SCHEMA_TEST_LOGLIK = "{\"type\":\"record\",\"name\":\"RegressionTestLoglikOutput\",\"namespace\":\"com.linkedin.mlease.regression.avro\",\"fields\":[{\"name\":\"key\",\"type\":\"string\"},{\"name\":\"testLoglik\",\"type\":\"float\"},{\"name\":\"count\",\"type\":\"double\"}]}";
 const char* SCHEMA_PARTITION_ID = "{\"type\":\"record\",\"name\":\"Pair\",\"namespace\":\"org.apache.avro.mapred\",\"fields\":[{\"name\":\"key\",\"type\":\"string\"},{\"name\":\"value\",\"type\":\"int\"}]}";
-const std::string INTERCEPT = "(INTERCEPT)";
 
 // ------------------------------------------------------------------------------------------ generic record access
 double num_of(const Value& v) { return (v.type == Schema::Float || v.type == Schema::Double) ? v.d : (double)v.i; }
@@ -216,23 +153,6 @@ int get_response(const Value& rec, const Schema& s) {
 }
 std::string feature_key(const std::string& name, const std::string& term) { return term.empty() ? name : name + "\x01" + term; }
 
-struct Dictionary {
-  std::unordered_map<std::string, int> idx;
-  std::vector<std::string> names;
-  int add(const std::string& n) { auto it = idx.find(n); if (it != idx.end()) return it->second; int i = (int)names.size(); idx.emplace(n, i); names.push_back(n); return i; }
-  int find(const std::string& n) const { auto it = idx.find(n); return it == idx.end() ? -1 : it->second; }
-};
-
-// one prepared record stream in CSR form (global dictionary ids)
-struct Rows {
-  std::vector<std::string> key;
-  std::vector<int32_t> response;
-  std::vector<float> weight, offset;
-  std::vector<int64_t> rowptr{0};
-  std::vector<int32_t> colidx;
-  std::vector<float> vals;
-  size_t n() const { return response.size(); }
-};
 
 // generic (Value-tree) reader: the reference implementation of read_prepared, and its fallback for unusual schemas
 void read_prepared_generic(const std::string& path, Dictionary& dict, Rows& rows, bool binary_feature) {
@@ -269,14 +189,6 @@ void read_prepared_generic(const std::string& path, Dictionary& dict, Rows& rows
 }
 
 
-// Avro binary primitives for the writers that encode records directly (no Value tree)
-inline void put_long(std::string& o, int64_t v) {
-  uint64_t z = ((uint64_t)v << 1) ^ (uint64_t)(v >> 63);
-  while (z & ~0x7FULL) { o.push_back((char)((z & 0x7F) | 0x80)); z >>= 7; }
-  o.push_back((char)z);
-}
-inline void put_str(std::string& o, const char* p, size_t n) { put_long(o, (int64_t)n); o.append(p, n); }
-inline void put_float(std::string& o, float f) { o.append(reinterpret_cast<const char*>(&f), 4); }
 
 // ------------------------------------------------------------------------------------------ block-parallel ingest (avro_walk.hpp)
 // Slots of the record plan.  The per-record logic below restates the generic readers field by field (same defaults, same casts,
@@ -371,7 +283,7 @@ void reset_record_slots(Slot* sl) {
 thread_local bool g_force_generic = false;   // tests: compare the two readers in one process
 bool host_generic_ingest() { if (g_force_generic) return true; const char* e = getenv("MLEASE_HOST_GENERIC_INGEST"); return e && atoi(e); }
 
-void read_raw_generic(const std::string& file, Dictionary& dict, Rows& rows, bool binary_feature);
+void read_raw_generic(const std::string& file, Dictionary& dict, Rows& rows, bool binary_feature, const std::string& item_key = "");
 
 // rows of one block with block-local feature ids
 struct BlockRows {
@@ -379,12 +291,13 @@ struct BlockRows {
   StrTable names;
 };
 // One file -> rows (appended) with global dictionary ids, decoded block-parallel.  mode 0: prepared records (read_prepared), 1: raw
-// records (read_raw).  Returns false (nothing touched) when the schema is left to the generic reader.
-bool read_rows_fast(const std::string& file, Dictionary& dict, Rows& rows, bool binary_feature, int mode) {
+// records (read_raw); item_key (mode 1 only): rows.key = that column rendered as item_key_string() does.  Returns false (nothing
+// touched) when the schema is left to the generic reader.
+bool read_rows_fast(const std::string& file, Dictionary& dict, Rows& rows, bool binary_feature, int mode, const std::string& item_key = "") {
   if (host_generic_ingest()) return false;
   AvroFile af(file);
   RecPlan rp;
-  if (!build_rec_plan(af.schema(), "", rp)) return false;
+  if (!build_rec_plan(af.schema(), item_key, rp)) return false;
   const size_t nb = af.num_blocks();
   std::vector<BlockRows> outs(nb);
   parallel_blocks(nb, host_threads(), [&](size_t b) {
@@ -405,9 +318,19 @@ bool read_rows_fast(const std::string& file, Dictionary& dict, Rows& rows, bool 
         const Slot& k = sl[S_KEY];
         r.key.push_back(k.is_null() ? std::string() : (k.kind == Slot::Str ? std::string(k.p, k.n) : std::to_string(k.i)));
       }
+      if (mode == 1) {
+        if (item_key.empty()) r.key.push_back("");
+        else {
+          if (rp.mapkey_slot < 0 || sl[rp.mapkey_slot].is_null()) io_error("data does not contain the column" + item_key);   // jobs/ItemModelTest.java:109-114
+          const Slot& k = sl[rp.mapkey_slot];
+          r.key.push_back(k.kind == Slot::Str ? std::string(k.p, k.n)
+                          : k.kind == Slot::Float ? java_float_to_string((float)k.d)
+                          : k.kind == Slot::Double ? java_double_to_string(k.d)
+                          : k.kind == Slot::Bool ? (k.i ? "true" : "false") : std::to_string(k.i));
+        }
+      }
       const int resp = get_response_slots(sl);
       if (resp != 1 && resp != 0 && resp != -1) io_error(mode == 0 ? "response = " + std::to_string(resp) + " (only 1, 0, -1 are allowed)" : "response = " + std::to_string(resp));
-      if (mode == 1) r.key.push_back("");
       r.response.push_back(resp);
       r.weight.push_back(sl[S_WEIGHT].is_null() ? 1.0f : (float)sl[S_WEIGHT].num());
       r.offset.push_back(sl[S_OFFSET].is_null() ? 0.0f : (float)sl[S_OFFSET].num());
@@ -463,9 +386,9 @@ void read_prepared(const std::string& path, Dictionary& dict, Rows& rows, bool b
     read_prepared_generic(f, dict, rows, binary_feature);
   }
 }
-void read_raw(const std::string& file, Dictionary& dict, Rows& rows, bool binary_feature) {
-  if (read_rows_fast(file, dict, rows, binary_feature, 1)) return;
-  read_raw_generic(file, dict, rows, binary_feature);
+void read_raw(const std::string& file, Dictionary& dict, Rows& rows, bool binary_feature, const std::string& item_key) {
+  if (read_rows_fast(file, dict, rows, binary_feature, 1, item_key)) return;
+  read_raw_generic(file, dict, rows, binary_feature, item_key);
 }
 
 // ------------------------------------------------------------------------------------------ model files
@@ -551,7 +474,8 @@ void write_linear_models(const std::string& path, const Dictionary& dict, const 
   write_model_records(path, dict, models);
 }
 // reads LinearModelAvro files -> key -> (feature key -> value), intercept under INTERCEPT
-std::map<std::string, std::unordered_map<std::string, double>> read_linear_models(const std::string& path) {
+// last_wins: a repeated key keeps only its last record (HashMap.put, regression/consumers/ReadLinearModelConsumer.java:54-88)
+std::map<std::string, std::unordered_map<std::string, double>> read_linear_models(const std::string& path, bool last_wins) {
   std::map<std::string, std::unordered_map<std::string, double>> out;
   for (auto& f : list_avro_files(path)) {
     AvroReader rd(f);
@@ -560,6 +484,7 @@ std::map<std::string, std::unordered_map<std::string, double>> read_linear_model
     Value rec;
     while (rd.next(rec)) {
       auto& m = out[rec.items[ki].s];
+      if (last_wins) m.clear();
       for (auto& fv : rec.items[mi].items) m[feature_key(fv.items[0].s, fv.items[1].s)] = fv.items[2].d;
     }
   }
@@ -632,7 +557,7 @@ double sample_test_loglik(const Rows& t, const Dictionary& dict, const std::vect
 }
 
 // raw (unprepared) records -> Rows; used by Test and by the per-iteration loglik (generic reader / fallback)
-void read_raw_generic(const std::string& file, Dictionary& dict, Rows& rows, bool binary_feature) {
+void read_raw_generic(const std::string& file, Dictionary& dict, Rows& rows, bool binary_feature, const std::string& item_key) {
   AvroReader rd(file);
   const Schema& s = rec_schema(rd.schema());
   int fi = s.field_index("features");
@@ -641,9 +566,18 @@ void read_raw_generic(const std::string& file, Dictionary& dict, Rows& rows, boo
   int ni = fs.field_index("name"), ti = fs.field_index("term"), vi = fs.field_index("value");
   Value rec;
   while (rd.next(rec)) {
+    std::string key;
+    if (!item_key.empty()) {   // data.get(item.key).toString() (jobs/ItemModelTest.java:109-114)
+      const Value* k = field(rec, s, item_key);
+      if (!k) io_error("data does not contain the column" + item_key);
+      key = k->type == Schema::String ? k->s
+            : k->type == Schema::Float ? java_float_to_string((float)k->d)
+            : k->type == Schema::Double ? java_double_to_string(k->d)
+            : k->type == Schema::Boolean ? (k->i ? "true" : "false") : std::to_string(k->i);
+    }
     int resp = get_response(rec, s);
     if (resp != 1 && resp != 0 && resp != -1) io_error("response = " + std::to_string(resp));
-    rows.key.push_back("");
+    rows.key.push_back(key);
     rows.response.push_back(resp);
     const Value* w = field(rec, s, "weight"); const Value* o = field(rec, s, "offset");
     rows.weight.push_back(w ? (float)num_of(*w) : 1.0f);
@@ -662,13 +596,18 @@ void read_raw_generic(const std::string& file, Dictionary& dict, Rows& rows, boo
 
 // ------------------------------------------------------------------------------------------ RegressionTest output
 // output = input fields (unions removed, utils/Util.java:377-417) + pred (jobs/RegressionTest.java:198-236)
-std::string test_output_schema(const SchemaP& in) {
+std::string test_output_schema(const SchemaP& in, const char* name, const char* ns) {
   SchemaP os = std::make_shared<Schema>(*schema_remove_union(in));
-  os->name = "AdmmTestOutput";
+  os->name = name;
   auto pf = std::make_shared<Schema>(); pf->type = Schema::Float;
   os->fields.emplace_back("pred", pf);
   std::map<std::string, bool> em;
-  return json_dump(schema_to_json(os, em));
+  Json j = schema_to_json(os, em);
+  if (ns) {
+    Json v; v.kind = Json::Str; v.str = ns;
+    j.obj.insert(j.obj.begin() + 1, {"namespace", v});
+  }
+  return json_dump(j);
 }
 void write_test_output_generic(const std::string& in_file, const std::string& out_file, const std::vector<float>& pred) {
   AvroReader rd(in_file);
@@ -680,7 +619,6 @@ void write_test_output_generic(const std::string& in_file, const std::string& ou
 // Record bytes with the union branch indices dropped -- what encoding the decoded record against the union-free schema gives when
 // every union holds its first non-null branch.  Anything else (a null where the output schema has none, a second non-null branch,
 // a union of nulls) throws NotPlain and the file goes through the generic path, which then behaves exactly as before.
-struct NotPlain {};
 void copy_varint(const uint8_t*& p, const uint8_t* e, std::string& o) {
   const uint8_t* q = p;
   walk_detail::rd_long(p, e);
@@ -1393,12 +1331,19 @@ void run_regression(const JobConfig& c) {
   }
 }
 
-}  // namespace
+// jobs defined in other translation units (register_job)
+std::map<std::string, JobFn>& job_registry() { static std::map<std::string, JobFn> r; return r; }
+bool register_job(const std::string& job_class, JobFn run) { job_registry()[job_class] = run; return true; }
+
+}  // namespace mlease_jobs
+
+using namespace mlease_jobs;
 
 extern "C" {
 const char* mlease_job_last_error(void) { return g_job_err.c_str(); }
 
-// job_class: Regression | RegressionPrepare | RegressionAdmmTrain | RegressionTest | RegressionTestLoglik | RegressionNaiveTrain
+// job_class: Regression | RegressionPrepare | RegressionAdmmTrain | RegressionTest | RegressionTestLoglik | RegressionNaiveTrain |
+// ItemModelTest | ItemModelTestLoglik
 // (the README's names AdmmPrepare / AdmmTrain / AdmmTest / AdmmTestLoglik / NaiveTrain are accepted as aliases).
 int mlease_job_run(const char* job_class, const char* config_path) {
   try {
@@ -1413,6 +1358,7 @@ int mlease_job_run(const char* job_class, const char* config_path) {
     else if (j == "RegressionTest" || j == "AdmmTest") run_test(c);
     else if (j == "RegressionTestLoglik" || j == "AdmmTestLoglik") run_test_loglik(c);
     else if (j == "RegressionNaiveTrain" || j == "NaiveTrain") run_naive_train(c);
+    else if (auto it = job_registry().find(j); it != job_registry().end()) it->second(c);
     else { g_job_err = "unknown job class " + j; return 1; }
     return 0;
   } catch (const std::exception& e) {

@@ -396,6 +396,39 @@ def test_loglik(response, pred, weight=None, combiner_block=0, device=0, stream=
 test_loglik.__test__ = False
 
 
+def score_keyed(vals, key_rowstart, rowptr, colidx, num_features, model_ptr, model_col, model_val, *, offset=None,
+                binary_feature=False, device=0, stream=None, out=None):
+    """ItemModelTest scoring (jobs/ItemModelTest.java:181-211): row i of key k (rows [key_rowstart[k], key_rowstart[k+1]) of the
+    CSR) is scored with model l*K + k for every lambda l.  Models are a CSR over (lambda, key): entries
+    [model_ptr[m], model_ptr[m+1]) of model_col (ascending, num_features = intercept) / model_val.  -> pred [L, nrows] float32."""
+    krs, rp, ci, vals = _keep(key_rowstart, np.int64), _keep(rowptr, np.int64), _keep(colidx, np.int32), _keep(vals, np.float32)
+    mp, mc, mv = _keep(model_ptr, np.int64), _keep(model_col, np.int32), _keep(model_val, np.float32)
+    K = len(krs) - 1
+    if K <= 0 or (len(mp) - 1) % K:
+        raise ValueError("model_ptr must hold num_lambdas * num_keys + 1 entries")
+    L = (len(mp) - 1) // K
+    n = len(rp) - 1
+    o = _keep(offset, np.float32)
+    pred = np.zeros((L, n), np.float32) if out is None else out
+    check(lib().mlease_score_keyed(device, stream, int(num_features), K, ptr(krs), ptr(rp), ptr(ci), ptr(vals), ptr(o), L, ptr(mp),
+                                   ptr(mc), ptr(mv), int(bool(binary_feature)), ptr(pred)))
+    return pred
+
+
+def test_loglik_keyed(entry_key, entry_group, response, pred, num_keys, weight=None, device=0, stream=None):
+    """ItemModelTestLoglik (jobs/ItemModelTestLoglik.java:60-142): one entry per (record, pred-map key), combiner group per entry
+    (non-decreasing) -> (float32 loglik [num_keys], float64 count [num_keys])."""
+    k, g, r = _keep(entry_key, np.int32), _keep(entry_group, np.int32), _keep(response, np.int32)
+    p, w = _keep(pred, np.float32), _keep(weight, np.float32)
+    ll = np.zeros(int(num_keys), np.float32)
+    cnt = np.zeros(int(num_keys), np.float64)
+    check(lib().mlease_test_loglik_keyed(device, stream, len(r), ptr(k), ptr(g), ptr(r), ptr(w), ptr(p), int(num_keys), ptr(ll), ptr(cnt)))
+    return ll, cnt
+
+
+test_loglik_keyed.__test__ = False
+
+
 def naive_train_dense(X, key_rowstart, response, lam, weight=None, offset=None, lambda_map=None, prior_mean=0.0,
                       penalize_intercept=False, has_intercept=True, data_size_threshold=0, device=0, stream=None):
     """RegressionNaiveTrain reducer for K keys (jobs/RegressionNaiveTrain.java:302-415) -> (models [K,D+1], skipped[K])."""
