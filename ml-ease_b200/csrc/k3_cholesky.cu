@@ -777,6 +777,45 @@ __global__ void chol_share_end_kernel(const Problem* __restrict__ probs, int npr
     c->ysym_use = probs[b - b % share].Ysym;   // wide systems: no copy of the factored inverse, the group streams the leader's
   }
 }
+// A follower of the shared cold-start factor must keep reading THAT factor when its owner later refactorises on its own (the
+// "stuck" rule or refresh_next): its secant pairs and h0_scale were built around the old H0, and the owner's new Y is another
+// lambda's Hessian at another point.  Before ysym_kernel overwrites the owner's Ysym, such a follower copies the owner's bytes into
+// its own Ysym (mode 0, grid (chunks, nprob)) and is then pointed at its own copy (mode 1, one thread per problem; a separate launch,
+// so that no CTA of mode 0 sees a follower already repointed).  A follower that refactorises in the same slot needs neither.
+__device__ __forceinline__ int detach_owner(const Problem* __restrict__ probs, int nprob, int b) {
+  const Problem& pb = probs[b];
+  const Ctrl* c = pb.ctrl;
+  const void* use = c->ysym_use;
+  if (!use || use == (const void*)pb.Ysym || (!c->done && c->need_hess)) return -1;
+  for (int j = 0; j < nprob; j++) {
+    if ((const void*)probs[j].Ysym != use) continue;
+    const Ctrl* oc = probs[j].ctrl;
+    return (!oc->done && oc->need_hess) ? j : -1;
+  }
+  return -1;
+}
+__global__ void __launch_bounds__(256) ysym_detach_kernel(const Problem* __restrict__ probs, int nprob, int mode) {
+  if (mode == 1) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b < nprob && detach_owner(probs, nprob, b) >= 0) probs[b].ctrl->ysym_use = probs[b].Ysym;
+    return;
+  }
+  const int b = blockIdx.y;
+  const int o = detach_owner(probs, nprob, b);
+  if (o < 0) return;
+  const size_t n16 = (size_t)probs[b].ldh * probs[b].ldh / 8;   // ldh is a multiple of 32: whole 16-byte words
+  const uint4* __restrict__ src = reinterpret_cast<const uint4*>(probs[o].Ysym);
+  uint4* __restrict__ dst = reinterpret_cast<uint4*>(probs[b].Ysym);
+  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < n16; e += (size_t)gridDim.x * blockDim.x) dst[e] = src[e];
+}
+cudaError_t cholesky_detach_followers(const Problem* d_probs, int nprob, int ldh, cudaStream_t st, int* launches) {
+  if (!cholesky_factored_direction(ldh)) return cudaSuccess;
+  ysym_detach_kernel<<<dim3(64, nprob), 256, 0, st>>>(d_probs, nprob, 0);
+  ysym_detach_kernel<<<(nprob + 255) / 256, 256, 0, st>>>(d_probs, nprob, 1);
+  if (launches) *launches += 2;
+  return cudaGetLastError();
+}
+
 cudaError_t cholesky_share_begin(const Problem* d_probs, int nprob, int share, cudaStream_t st, int* launches) {
   chol_share_begin_kernel<<<(nprob + 127) / 128, 128, 0, st>>>(d_probs, nprob, share);
   if (launches) *launches += 1;

@@ -25,6 +25,8 @@ cudaError_t newton_begin(const Problem* d_probs, int nprob, double xtol, int max
                          int invalidate_hess, int rebuild_is_expensive, cudaStream_t st, int* launches);
 cudaError_t k1_reduce_decide(const Problem* d_probs, int nprob, int Dt, cudaStream_t st, int* launches, int spec = 0);
 cudaError_t newton_solve(const Problem* d_probs, int nprob, int ldh, cudaStream_t st, int* launches, int group_L = 1);
+// the two triangular GEMVs of the factored direction (ldh > 2048) alone, over the whole batch: dir = Y^T (Y qf), t in tf
+cudaError_t newton_gemv_tri(const Problem* d_probs, int nprob, int ldh, int group_L, cudaStream_t st);
 // matrix-free Newton-CG direction (newton.cu): begin (pick the problems that need a direction), the fixed-order reduction of the
 // Hv / diagonal partials (out 0: g_t, 1: cg_Hp, 2: cg_diag), init (after the diagonal pass), one CG step (after an Hv pass), and
 // the poll of the CG flags into *d_any (1 while a problem's CG still runs)
@@ -66,7 +68,9 @@ cudaError_t cholesky_launch(const Problem* d_probs, int nprob, int ldh, cudaStre
 bool cholesky_factored_direction(int ldh);   // wide systems: Ysym holds Y = L^-1 (bf16, symmetric storage), the direction is Y^T (Y q)
 cudaError_t cholesky_share_begin(const Problem* d_probs, int nprob, int share, cudaStream_t st, int* launches);
 cudaError_t cholesky_share_end(const Problem* d_probs, int nprob, int share, cudaStream_t st, int* launches);
-
+// before a rebuild slot of a wide batch whose followers may still read a shared cold-start factor: every follower whose owner
+// refactorises in this slot (and which does not) copies the owner's Ysym into its own and points at it (d_probs: the whole batch)
+cudaError_t cholesky_detach_followers(const Problem* d_probs, int nprob, int ldh, cudaStream_t st, int* launches);
 // K4 (k4_consensus.cu)
 cudaError_t admm_reset(const Problem* d_probs, int nprob, int L, double* d_z, int ldv, const double* d_rho_eff,
                        cudaStream_t st, int* launches);

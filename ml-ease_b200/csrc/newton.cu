@@ -659,13 +659,21 @@ cudaError_t k1_reduce_decide(const Problem* d_probs, int nprob, int Dt, cudaStre
   if (launches) *launches += 2;
   return cudaGetLastError();
 }
+// Both phases of the factored direction, qf -> tf -> dir.  d_probs must be the whole batch (not a compacted subset): the lambda
+// sets of group_L are taken as b % group_L of the array index.
+cudaError_t newton_gemv_tri(const Problem* d_probs, int nprob, int ldh, int group_L, cudaStream_t st) {
+  const int nblk2 = ((ldh + GEMV_RB - 1) / GEMV_RB + 1) / 2;   // row blocks, two (a block and its mirror) per warp
+  const dim3 gtri((nblk2 + NT / 32 - 1) / (NT / 32), nprob);
+  newton_gemv_tri_kernel<<<gtri, NT, 0, st>>>(d_probs, 0, group_L);
+  newton_gemv_tri_kernel<<<gtri, NT, 0, st>>>(d_probs, 1, group_L);
+  return cudaGetLastError();
+}
+
 cudaError_t newton_solve(const Problem* d_probs, int nprob, int ldh, cudaStream_t st, int* launches, int group_L) {
   const dim3 grid((ldh + NT / 32 - 1) / (NT / 32), nprob);
   if (cholesky_factored_direction(ldh)) {
-    const int nblk2 = ((ldh + GEMV_RB - 1) / GEMV_RB + 1) / 2;   // row blocks, two (a block and its mirror) per warp
-    const dim3 gtri((nblk2 + NT / 32 - 1) / (NT / 32), nprob);
-    newton_gemv_tri_kernel<<<gtri, NT, 0, st>>>(d_probs, 0, group_L);
-    newton_gemv_tri_kernel<<<gtri, NT, 0, st>>>(d_probs, 1, group_L);
+    const cudaError_t e = newton_gemv_tri(d_probs, nprob, ldh, group_L, st);
+    if (e != cudaSuccess) return e;
     if (launches) *launches += 1;
   } else {
     newton_gemv_kernel<<<grid, NT, 0, st>>>(d_probs);

@@ -169,6 +169,7 @@ struct Batch {
   int k1_dyn = 0;                 // > 0: K1 CTAs are dealt to the running problems at run time (value = nprob, <= 32); k1_grid = whole grid
   int rebuild_is_expensive = 0;   // cost model: Gram + Cholesky + inverse vs one K1 pass (set in batch_alloc)
   int matfree = 0;                // Newton-CG directions from Hv passes: no Gram, factor or inverse is allocated (set in batch_alloc)
+  bool ysym_shared = false;       // a wide batch whose followers were pointed at their leader's Ysym (chol_share_end_kernel)
   std::vector<Problem> h;
   Problem* d = nullptr;
   Problem* d_compact = nullptr;   // large batches: Problem structs of the problems that may rebuild in the next slot
@@ -379,7 +380,10 @@ int batch_alloc(Batch& B, int num_sms, int hessian_policy, int csr_gram_force = 
     B.gram_slices = best;
   }
   // matrix-free: the CG vectors r, p, z, Hp and diag(H) per problem instead of the L-BFGS pairs (no secant pairs are kept there)
-  const size_t nd = (size_t)nprob * ((9 + (B.matfree ? 5 : 2 * BFGS_M)) * (size_t)ldx + 2 * BFGS_M + (size_t)gpart_rows * ldx + (size_t)B.k1_grid + 8);
+  // doubles per problem, rounded up to a multiple of 4: every problem's vectors start 32-byte aligned (the triangular GEMVs and the
+  // Hv passes read qf / tf / hv_vf as float4); the K1 partial count k1_grid (fused: its segment count) may be odd
+  const size_t nd_prob = ((9 + (B.matfree ? 5 : 2 * BFGS_M)) * (size_t)ldx + 2 * BFGS_M + (size_t)gpart_rows * ldx + (size_t)B.k1_grid + 8 + 3) & ~(size_t)3;
+  const size_t nd = (size_t)nprob * nd_prob;
   const size_t nf = (size_t)nprob * 4 * ldx;
   double* dd; float* ff; float* hp = nullptr; double* lc = nullptr; double* ld = nullptr; double* ldi = nullptr; double* yi = nullptr; double* hi = nullptr;
   if (int rc = dev_alloc(B, (void**)&dd, nd * sizeof(double))) return rc;
@@ -423,6 +427,7 @@ int batch_alloc(Batch& B, int num_sms, int hessian_policy, int csr_gram_force = 
     p.ldx = ldx; p.Dt = B.Dt; p.Dp = B.Dp; p.ldh = B.ldh; p.self_idx = b;
     p.k1_ctas = B.k1_grid;
     p.gram_slices = B.gram_slices;
+    double* const q0 = dd;
     double* q = dd;
     p.beta = q; q += ldx; p.beta_t = q; q += ldx; p.m = q; q += ldx; p.q = q; q += ldx;
     p.g_t = q; q += ldx; p.g_acc = q; q += ldx; p.dir = q; q += ldx; p.x_d = q; q += ldx;
@@ -434,7 +439,7 @@ int batch_alloc(Batch& B, int num_sms, int hessian_policy, int csr_gram_force = 
     if (B.matfree) { p.cg_r = q; q += ldx; p.cg_p = q; q += ldx; p.cg_z = q; q += ldx; p.cg_Hp = q; q += ldx; p.cg_diag = q; q += ldx; }
     p.gpart_f = gpf ? gpf + (size_t)b * B.k1_grid * ldx : nullptr;
     p.fpart = q; q += B.k1_grid + 8;
-    dd = q;
+    dd = q0 + nd_prob;
     float* f = ff;
     p.beta_tf = f; f += ldx; p.u_f = f; f += ldx; p.uplusx_f = f; f += ldx; p.x_f = f; f += ldx;
     ff = f;
@@ -557,10 +562,13 @@ int batch_xupdate(Batch& B, cudaStream_t st, double xtol, int max_newton, int po
       pf.end(st);
       pf.begin(3, st);
       const bool share_fact = share > 1 && share_first_factor;   // same rho too: same H, one factorisation per group
+      // a follower still on a shared factor whose owner refactorises here takes a copy of the owner's bytes first
+      if (B.ysym_shared) CK(cholesky_detach_followers(B.d, B.nprob, B.ldh, st, &launches));
       if (share_fact) CK(cholesky_share_begin(B.d, B.nprob, share, st, &launches));
       CK(cholesky_launch(d_hess, n_hess, B.ldh, st, &launches, share));
       if (share_fact) {
         CK(cholesky_share_end(B.d, B.nprob, share, st, &launches));
+        if (cholesky_factored_direction(B.ldh)) B.ysym_shared = true;
         const size_t hh = (size_t)B.ldh * B.ldh;
         for (int b = 0; b < B.nprob; b++) {
           if (b % share == 0) continue;
@@ -1625,6 +1633,125 @@ int mlease_internal_batch_hv(mlease_session* s, int32_t mode, const double* w, c
   if (int rc = set_ctrl(0, -1)) return rc;
   B.mirror.clear();
   s->cnt.launches += launches;
+  return 0;
+}
+
+// Test hooks of the factored direction of wide systems (ldh > 2048), not part of the C ABI.  Each refuses, before any launch, a
+// batch that has no Ysym (ldh <= 2048, or matrix-free), since the kernels they run dereference it.
+//
+// mlease_internal_factor: the caller's Dt x Dt H (row-major; its lower triangle is read) goes into the scratch problem's Lc of
+// partition pid as chol_prep leaves it (lower triangle, identity on the padding, zero above), then the factorisation the solver
+// runs for its direction: fp64 Cholesky, recursive inverse with TF32 merges, bf16 symmetric packing.  Read back, each if not NULL:
+// Lc (Dt x Dt), Yinv (ldh x ldh, whole) and the raw bits of Ysym (ldh x ldh).  The scratch problem's x-update state is consumed.
+int mlease_internal_factor(mlease_session* s, int32_t pid, const double* H, double* L_out, double* Y_out, uint16_t* ysym_out) {
+  if (!s || !H) return fail(MLEASE_ERR_INVALID, "null argument");
+  CK(cudaSetDevice(s->cfg.device));
+  const int pi = find_part(s, pid);
+  if (pi < 0) return fail(MLEASE_ERR_INVALID, "partition not resident in this session");
+  if (s->cfg.hessian_policy == 2) return fail(MLEASE_ERR_INVALID, "a matrix-free session forms no factor");
+  if (!cholesky_factored_direction(round_up(s->Dt, 32))) return fail(MLEASE_ERR_INVALID, "only systems wider than 2048 (ldh) use the factored direction");
+  if (int rc = ensure_scratch(s, pi)) return rc;
+  Batch* B = s->scratch;
+  if (B->matfree) return fail(MLEASE_ERR_INVALID, "a matrix-free session forms no factor");   // (made so by the memory rule)
+  if (!cholesky_factored_direction(B->ldh) || !B->h[0].Ysym) return fail(MLEASE_ERR_INVALID, "only systems wider than 2048 (ldh) use the factored direction");
+  const Problem& p = B->h[0];
+  const int Dt = s->Dt, ldh = B->ldh;
+  const size_t hh = (size_t)ldh * ldh;
+  std::vector<double> lc(hh, 0.0);
+  for (int i = 0; i < ldh; i++)
+    for (int j = 0; j <= i; j++) lc[(size_t)i * ldh + j] = i < Dt ? H[(size_t)i * Dt + j] : (i == j ? 1.0 : 0.0);
+  CK(cudaMemcpy(p.Lc, lc.data(), hh * sizeof(double), cudaMemcpyHostToDevice));
+  Ctrl c; std::memset(&c, 0, sizeof(c)); c.need_hess = 1;
+  CK(cudaMemcpy(B->d_ctrl, &c, sizeof(Ctrl), cudaMemcpyHostToDevice));
+  int launches = 0;
+  CK(cholesky_launch(B->d, 1, ldh, s->stream, &launches, 0, 1, 0));
+  CK(cudaStreamSynchronize(s->stream));
+  CK(cudaMemcpy(&c, B->d_ctrl, sizeof(Ctrl), cudaMemcpyDeviceToHost));
+  if (L_out) {
+    CK(cudaMemcpy(lc.data(), p.Lc, hh * sizeof(double), cudaMemcpyDeviceToHost));
+    for (int i = 0; i < Dt; i++) std::memcpy(L_out + (size_t)i * Dt, &lc[(size_t)i * ldh], (size_t)Dt * sizeof(double));
+  }
+  if (Y_out) CK(cudaMemcpy(Y_out, p.Yinv, hh * sizeof(double), cudaMemcpyDeviceToHost));
+  if (ysym_out) CK(cudaMemcpy(ysym_out, p.Ysym, hh * sizeof(uint16_t), cudaMemcpyDeviceToHost));
+  // as after mlease_posterior_variance: the scratch problem's bookkeeping no longer matches its factor
+  Ctrl c2; std::memset(&c2, 0, sizeof(c2));
+  CK(cudaMemcpy(B->d_ctrl, &c2, sizeof(Ctrl), cudaMemcpyHostToDevice));
+  B->mirror.clear();
+  s->cnt.launches += launches;
+  if (c.fail) return fail(MLEASE_ERR_NUMERIC, "Hessian not positive definite");
+  return 0;
+}
+
+// mlease_internal_factored_direction: on the ADMM batch (after begin() and at least one iterate()), the two triangular GEMV phases of
+// the direction for the problems with active[b] != 0, each on its q[b] (Dt entries; b = local partition * L + lambda), over the
+// whole problem array with the batch's group_L, exactly as newton_solve launches them.  t_out[b] / dir_out[b] (Dt entries each, if
+// not NULL) receive tf and dir; dir is filled with NaN beforehand, so an inactive problem keeps NaN.  The batch's x-update state
+// is consumed (every problem is left done): begin() again before iterating.
+int mlease_internal_factored_direction(mlease_session* s, const int32_t* active, const float* q, float* t_out, double* dir_out) {
+  if (!s || !active || !q) return fail(MLEASE_ERR_INVALID, "null argument");
+  if (!s->batch || !s->begun || s->iter < 1) return fail(MLEASE_ERR_STATE, "needs the ADMM batch after mlease_admm_begin and one iteration");
+  CK(cudaSetDevice(s->cfg.device));
+  Batch& B = *s->batch;
+  if (B.matfree) return fail(MLEASE_ERR_INVALID, "a matrix-free session forms no factor");
+  if (!cholesky_factored_direction(B.ldh) || !B.h[0].Ysym) return fail(MLEASE_ERR_INVALID, "only systems wider than 2048 (ldh) use the factored direction");
+  const int nprob = B.nprob, ldx = s->ldx, Dt = s->Dt;
+  std::vector<Ctrl> c(nprob);
+  CK(cudaMemcpy(c.data(), B.d_ctrl, (size_t)nprob * sizeof(Ctrl), cudaMemcpyDeviceToHost));
+  for (int b = 0; b < nprob; b++) { c[b].done = active[b] ? 0 : 1; c[b].need_solve = active[b] ? 1 : 0; }
+  CK(cudaMemcpy(B.d_ctrl, c.data(), (size_t)nprob * sizeof(Ctrl), cudaMemcpyHostToDevice));
+  std::vector<float> qt(2 * (size_t)ldx, 0.f);   // qf then tf: qf = float(q) on [0, Dt) and 0 on [Dt, ldx) (as the decide kernel leaves it)
+  const std::vector<double> nan(ldx, std::nan(""));
+  for (int b = 0; b < nprob; b++) {
+    for (int k = 0; k < ldx; k++) { qt[k] = k < Dt ? q[(size_t)b * Dt + k] : 0.f; qt[ldx + k] = k < Dt ? std::nanf("") : 0.f; }
+    CK(cudaMemcpy(B.h[b].qf, qt.data(), 2 * (size_t)ldx * sizeof(float), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(B.h[b].dir, nan.data(), (size_t)ldx * sizeof(double), cudaMemcpyHostToDevice));
+  }
+  CK(newton_gemv_tri(B.d, nprob, B.ldh, B.group_L, s->stream));
+  CK(cudaStreamSynchronize(s->stream));
+  for (int b = 0; b < nprob; b++) {
+    if (t_out) CK(cudaMemcpy(t_out + (size_t)b * Dt, B.h[b].tf, (size_t)Dt * sizeof(float), cudaMemcpyDeviceToHost));
+    if (dir_out) CK(cudaMemcpy(dir_out + (size_t)b * Dt, B.h[b].dir, (size_t)Dt * sizeof(double), cudaMemcpyDeviceToHost));
+  }
+  for (auto& x : c) { x.done = 1; x.need_solve = 0; }
+  CK(cudaMemcpy(B.d_ctrl, c.data(), (size_t)nprob * sizeof(Ctrl), cudaMemcpyHostToDevice));
+  B.mirror.clear();
+  s->cnt.launches += 2;
+  return 0;
+}
+
+// mlease_internal_ysym: the bytes problem b of the ADMM batch streams in its direction (Ctrl::ysym_use, else its own Ysym; ldh x ldh
+// bf16 bits), the index of the problem that owns them, and b's factorisation count (Ctrl::tot_hess).  Reads only.
+int mlease_internal_ysym(mlease_session* s, int32_t b, uint16_t* out, int32_t* owner, int32_t* tot_hess) {
+  if (!s) return fail(MLEASE_ERR_INVALID, "null session");
+  if (!s->batch) return fail(MLEASE_ERR_STATE, "mlease_admm_begin was not called");
+  CK(cudaSetDevice(s->cfg.device));
+  Batch& B = *s->batch;
+  if (b < 0 || b >= B.nprob) return fail(MLEASE_ERR_INVALID, "problem index out of range");
+  if (B.matfree) return fail(MLEASE_ERR_INVALID, "a matrix-free session forms no factor");
+  if (!cholesky_factored_direction(B.ldh) || !B.h[0].Ysym) return fail(MLEASE_ERR_INVALID, "only systems wider than 2048 (ldh) use the factored direction");
+  Ctrl c;
+  CK(cudaMemcpy(&c, B.d_ctrl + b, sizeof(Ctrl), cudaMemcpyDeviceToHost));
+  const void* use = c.ysym_use ? c.ysym_use : (const void*)B.h[b].Ysym;
+  int own = -1;
+  for (int j = 0; j < B.nprob; j++) if ((const void*)B.h[j].Ysym == use) own = j;
+  if (own < 0) return fail(MLEASE_ERR_STATE, "problem's factor pointer matches no problem of the batch");
+  if (out) CK(cudaMemcpy(out, use, (size_t)B.ldh * B.ldh * sizeof(uint16_t), cudaMemcpyDeviceToHost));
+  if (owner) *owner = own;
+  if (tot_hess) *tot_hess = (int32_t)c.tot_hess;
+  return 0;
+}
+
+// mlease_internal_request_refresh: problem b of the ADMM batch refactorises at the start point of its next x-update, as after a
+// slow x-update (Ctrl::refresh_next), whatever the other problems do.  Lets a test make one lambda rebuild on its own.
+int mlease_internal_request_refresh(mlease_session* s, int32_t b) {
+  if (!s) return fail(MLEASE_ERR_INVALID, "null session");
+  if (!s->batch) return fail(MLEASE_ERR_STATE, "mlease_admm_begin was not called");
+  Batch& B = *s->batch;
+  if (b < 0 || b >= B.nprob) return fail(MLEASE_ERR_INVALID, "problem index out of range");
+  CK(cudaSetDevice(s->cfg.device));
+  const int one = 1;
+  CK(cudaMemcpy(&B.d_ctrl[b].refresh_next, &one, sizeof(int), cudaMemcpyHostToDevice));
+  if ((int)B.mirror.size() > b) B.mirror[b].refresh_next = 1;   // the host's prediction of slot 0: a rebuild is due
   return 0;
 }
 
