@@ -253,6 +253,21 @@ int mlease_naive_train_dense(int32_t device, void* stream, int32_t num_keys, int
                              float prior_mean, int32_t penalize_intercept, int32_t has_intercept,
                              int32_t data_size_threshold, double* out_model, int32_t* skipped);
 
+/* ItemModelTrain (jobs/ItemModelTrain.java:226-276): num_keys x IL x DL independent fits on the CSR input of mlease_naive_train
+ * (rowptr, colidx, vals, key_rowstart, response, weight, offset; binary_feature), always with an intercept and no size threshold.
+ * Fit (a, b) of key k: priorVar = 1/lambda_map[j] for a listed feature (lambda_map [num_features] or NULL, entries > 0, 0 = none),
+ * 1/intercept_lambdas[a] for the intercept, 1/default_lambdas[b] otherwise (every lambda > 0, checked, naming its list); prior mean
+ * intercept_prior_mean[k] for the intercept, 0 otherwise; start 0.  out_model [IL][DL][num_keys][num_features+1] double, intercept
+ * last, features absent from the key's rows 0.  compute_var: out_var of the same shape receives the diagonal posterior variance
+ * 1 / (1/priorVar[j] + sum_i weight_i p_i (1-p_i) x_ij^2) at the fit (llf/LibLinear.java:328-333), 1/q = priorVar[j] for an absent
+ * feature.  All inputs host-or-device; intercept_prior_mean, out_model and out_var host.  With IL = DL = 1, intercept_lambdas[0] =
+ * default_lambdas[0] and zero means the models are bitwise those of mlease_naive_train(prior_mean 0, penalize_intercept 1). */
+int mlease_item_model_train(int32_t device, void* stream, int32_t num_keys, int32_t num_features, const int64_t* key_rowstart,
+                            const int64_t* rowptr, const int32_t* colidx, const float* vals, const int32_t* response, const float* weight,
+                            const float* offset, const double* intercept_prior_mean, int32_t num_intercept_lambdas,
+                            const float* intercept_lambdas, int32_t num_default_lambdas, const float* default_lambdas,
+                            const float* lambda_map, int32_t binary_feature, int32_t compute_var, double* out_model, double* out_var);
+
 /* ---------------------------------------------------------------------------------------
  * RegressionTest / RegressionTestLoglik.
  * score: pred = float(offset + interceptTerm + sum beta_k x_k), interceptTerm = -log(n-1+n*exp(-b)),

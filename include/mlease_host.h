@@ -12,7 +12,7 @@
 extern "C" {
 #endif
 /* job_class: Regression | RegressionPrepare | RegressionAdmmTrain | RegressionTest | RegressionTestLoglik |
- * RegressionNaiveTrain | ItemModelTest | ItemModelTestLoglik (README aliases AdmmPrepare/AdmmTrain/AdmmTest/AdmmTestLoglik/NaiveTrain
+ * RegressionNaiveTrain | ItemModelTest | ItemModelTestLoglik | ItemModelTrain (README aliases AdmmPrepare/AdmmTrain/AdmmTest/AdmmTestLoglik/NaiveTrain
  * accepted).
  * Returns 0, or non-zero with the message (the reference's IOException / RuntimeException text) in mlease_job_last_error(). */
 int mlease_job_run(const char* job_class, const char* config_path);

@@ -6,17 +6,37 @@
 //     full     : postVar = diag(H^-1), H = LogisticRegressionL2.hessian (:258-297), inverted by Cholesky
 //                (commons-math CholeskyDecomposition in the reference, :321-325; K3's fp64 factorisation + explicit inverse here).
 // The tensor-core Gram (bf16 operands) is a preconditioner-grade H; a reported variance needs the Hessian itself, so these
-// kernels accumulate it in fp64 from the fp32 data (SIMT; n D'^2 / 2 fp64 FMA -- ItemModel-sized problems, not the hot path).
+// kernels accumulate it in fp64 from the fp32 data (SIMT; n D'^2 / 2 fp64 FMA for the full matrix).  The diagonal runs over a
+// batch of problems (ItemModelTrain's keys, one launch per key chunk and prior) or over a session's one partition.
+#include <algorithm>
+
 #include "kernels.cuh"
 
 namespace mlease {
 
-// d_i = weight_i p_i (1 - p_i) at w (double), one warp per row.  Same score as LogisticRegressionL2.hessian (:261-269).
-__global__ void postvar_rowweight_kernel(const Problem* __restrict__ probs, const double* __restrict__ w, int has_bias, double* __restrict__ dvec) {
-  const Problem& pb = probs[0];
+// A batch's rows are numbered across its problems: problem b owns rows [row_start[b], row_start[b+1]) (empty problems allowed).
+// One warp per row of the whole batch, so a batch of thousands of keys of a few hundred rows keeps every SM busy; the row's
+// problem is the last b with row_start[b] <= r.
+__device__ __forceinline__ int postvar_problem_of(const long long* __restrict__ row_start, int nprob, long long r) {
+  int lo = 0, hi = nprob - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (row_start[mid] <= r) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+
+// d_r = weight_i p_i (1 - p_i) at the problem's beta (double).  Same score as LogisticRegressionL2.hessian (:261-269).
+__global__ void postvar_rowweight_kernel(const Problem* __restrict__ probs, int nprob, const long long* __restrict__ row_start,
+                                         int has_bias, double* __restrict__ dvec) {
   const int lane = threadIdx.x & 31;
   const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
-  for (long long i = warp; i < pb.n; i += nwarps) {
+  const long long nrows = row_start[nprob];
+  for (long long r = warp; r < nrows; r += nwarps) {
+    const int b = postvar_problem_of(row_start, nprob, r);
+    const Problem& pb = probs[b];
+    const long long i = r - row_start[b];
+    const double* w = pb.beta;
     double s = 0.0;
     if (pb.X) {
       const float* xr = pb.X + (size_t)i * pb.ldx;
@@ -29,18 +49,29 @@ __global__ void postvar_rowweight_kernel(const Problem* __restrict__ probs, cons
       if (!pb.X && has_bias) s += w[pb.Dt - 1];
       s += (double)pb.o[i];
       const double p = 1.0 / (1.0 + exp(-(double)pb.y[i] * s));
-      dvec[i] = (double)pb.w[i] * p * (1.0 - p);
+      dvec[r] = (double)pb.w[i] * p * (1.0 - p);
     }
   }
 }
 
-// H[k] += d_i x_ik^2 (k < Dt): per-CTA shared-memory accumulation when Dt fits, flushed with fp64 global atomics.
-__global__ void postvar_diag_kernel(const Problem* __restrict__ probs, const double* __restrict__ dvec, int has_bias, double* __restrict__ H) {
-  const Problem& pb = probs[0];
+// g_t = q over [0, ldx): the prior precision the diagonal starts from
+__global__ void postvar_diag_init_kernel(const Problem* __restrict__ probs) {
+  const Problem& pb = probs[blockIdx.x];
+  for (int k = threadIdx.x; k < pb.ldx; k += blockDim.x) pb.g_t[k] = pb.q[k];
+}
+
+// g_t[k] += d_r x_ik^2 (k < Dt) of each problem, fp64 global atomics.
+__global__ void postvar_diag_kernel(const Problem* __restrict__ probs, int nprob, const long long* __restrict__ row_start,
+                                    const double* __restrict__ dvec, int has_bias) {
   const int lane = threadIdx.x & 31;
   const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
-  for (long long i = warp; i < pb.n; i += nwarps) {
-    const double d = dvec[i];
+  const long long nrows = row_start[nprob];
+  for (long long r = warp; r < nrows; r += nwarps) {
+    const int b = postvar_problem_of(row_start, nprob, r);
+    const Problem& pb = probs[b];
+    const long long i = r - row_start[b];
+    double* H = pb.g_t;
+    const double d = dvec[r];
     if (pb.X) {
       const float* xr = pb.X + (size_t)i * pb.ldx;
       for (int k = lane; k < pb.Dt; k += 32) { const double x = (double)xr[k]; atomicAdd(&H[k], d * x * x); }
@@ -117,14 +148,18 @@ __global__ void postvar_init_kernel(const Problem* __restrict__ probs, const dou
   }
 }
 
-cudaError_t postvar_rowweights(const Problem* d_prob, const double* d_w, int has_bias, double* d_dvec, cudaStream_t st, int* launches) {
-  postvar_rowweight_kernel<<<1184, 256, 0, st>>>(d_prob, d_w, has_bias, d_dvec);
+static int postvar_grid(long long nrows) { return (int)std::max(1LL, std::min(1184LL, (nrows + 7) / 8)); }   // 8 warps per CTA
+cudaError_t postvar_rowweights(const Problem* d_probs, int nprob, const long long* d_row_start, long long nrows, int has_bias, double* d_dvec,
+                               cudaStream_t st, int* launches) {
+  postvar_rowweight_kernel<<<postvar_grid(nrows), 256, 0, st>>>(d_probs, nprob, d_row_start, has_bias, d_dvec);
   if (launches) *launches += 1;
   return cudaGetLastError();
 }
-cudaError_t postvar_diag(const Problem* d_prob, const double* d_dvec, int has_bias, double* d_H, cudaStream_t st, int* launches) {
-  postvar_diag_kernel<<<1184, 256, 0, st>>>(d_prob, d_dvec, has_bias, d_H);
-  if (launches) *launches += 1;
+cudaError_t postvar_diag(const Problem* d_probs, int nprob, const long long* d_row_start, long long nrows, const double* d_dvec, int has_bias,
+                         cudaStream_t st, int* launches) {
+  postvar_diag_init_kernel<<<nprob, 128, 0, st>>>(d_probs);
+  postvar_diag_kernel<<<postvar_grid(nrows), 256, 0, st>>>(d_probs, nprob, d_row_start, d_dvec, has_bias);
+  if (launches) *launches += 2;
   return cudaGetLastError();
 }
 cudaError_t postvar_hessian(const Problem* d_prob, bool csr, int ldh, const double* d_dvec, const double* d_q, int has_bias, cudaStream_t st, int* launches) {

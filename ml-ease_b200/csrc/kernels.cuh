@@ -82,8 +82,12 @@ cudaError_t admm_consensus(const Problem* d_probs, int nlocal_parts, int L, int 
                            int* launches, const double* d_l1_thr = nullptr);
 
 // posterior variance (k6_postvar.cu): exact fp64 Hessian diagonal / full Hessian into Lc
-cudaError_t postvar_rowweights(const Problem* d_prob, const double* d_w, int has_bias, double* d_dvec, cudaStream_t st, int* launches);
-cudaError_t postvar_diag(const Problem* d_prob, const double* d_dvec, int has_bias, double* d_H, cudaStream_t st, int* launches);
+// rowweights / diag run over the problems d_probs[0 .. nprob): problem b owns rows [d_row_start[b], d_row_start[b+1]) of d_dvec
+// (nrows = d_row_start[nprob]); d_dvec[r] = w_i p_i (1 - p_i) at the problem's beta; diag leaves q + sum_i d_i x_ik^2 in each g_t
+cudaError_t postvar_rowweights(const Problem* d_probs, int nprob, const long long* d_row_start, long long nrows, int has_bias, double* d_dvec,
+                               cudaStream_t st, int* launches);
+cudaError_t postvar_diag(const Problem* d_probs, int nprob, const long long* d_row_start, long long nrows, const double* d_dvec, int has_bias,
+                         cudaStream_t st, int* launches);
 cudaError_t postvar_hessian(const Problem* d_prob, bool csr, int ldh, const double* d_dvec, const double* d_q, int has_bias, cudaStream_t st,
                             int* launches);
 

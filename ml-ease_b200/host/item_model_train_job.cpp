@@ -1,0 +1,173 @@
+// item_model_train_job.cpp -- ItemModelTrain (jobs/ItemModelTrain.java:89-321): per key, one LibLinear fit for every (intercept lambda,
+// default lambda) pair, written as LinearModelWithVarAvro records under output.model.path/models.  Reached through mlease_job_run
+// (register_job); the fits and their posterior variance are one mlease_item_model_train call.
+#include <cmath>
+
+#include "jobs_common.hpp"
+
+namespace mlease_jobs {
+namespace {
+
+const char* SCHEMA_MODEL_WITH_VAR =
+    "{\"type\":\"record\",\"name\":\"LinearModelWithVarAvro\",\"namespace\":\"com.linkedin.mlease.avro\",\"doc\":\"Linear Model with posterior variance in Avro\","
+    "\"fields\":[{\"name\":\"key\",\"type\":\"string\"},"
+    "{\"name\":\"model\",\"type\":{\"type\":\"array\",\"items\":{\"type\":\"record\",\"name\":\"feature\",\"fields\":["
+    "{\"name\":\"name\",\"type\":\"string\"},{\"name\":\"term\",\"type\":\"string\"},{\"name\":\"value\",\"type\":\"float\"}]}}},"
+    "{\"name\":\"posteriorVar\",\"type\":{\"type\":\"array\",\"items\":{\"type\":\"record\",\"name\":\"featureVar\",\"fields\":["
+    "{\"name\":\"name\",\"type\":\"string\"},{\"name\":\"term\",\"type\":\"string\"},{\"name\":\"value\",\"type\":\"float\"}]}}}]}";
+
+// intercept.lambdas / default.lambdas: Float.parseFloat of the comma list, in order, repeats kept (:313-321).  The reference divides
+// by every lambda (:262), so a lambda <= 0 or NaN is refused here instead of producing infinite prior variances.
+std::vector<float> lambda_list(const JobConfig& c, const std::string& key) {
+  std::vector<float> out;
+  for (auto& t : c.get_list(key)) {
+    const float v = std::stof(t);
+    if (!(v > 0.f)) io_error(key + ": every lambda must be > 0 (got " + t + ")");
+    out.push_back(v);
+  }
+  if (out.empty()) io_error(key + ": no lambda given");
+  return out;
+}
+
+// intercept.prior.mean.map: Pair records {key, value}, value = Double.parseDouble(value.toString()) (:293-301), so a float value
+// is read through its Float.toString digits
+std::unordered_map<std::string, double> read_prior_mean_map(const std::string& path) {
+  std::unordered_map<std::string, double> out;
+  for (auto& f : list_avro_files(path)) {
+    AvroReader rd(f);
+    const Schema& s = rec_schema(rd.schema());
+    Value rec;
+    while (rd.next(rec)) {
+      const Value* k = field(rec, s, "key");
+      const Value* v = field(rec, s, "value");
+      if (!k || !v) io_error("intercept.prior.mean.map: a record without key or value");
+      double d;
+      if (v->type == Schema::String) {
+        try { d = std::stod(JobConfig::trim(v->s)); } catch (const std::exception&) { io_error("For input string: \"" + v->s + "\""); }
+      } else if (v->type == Schema::Float) d = std::stod(java_float_to_string((float)v->d));
+      else if (v->type == Schema::Double) d = v->d;
+      else if (v->type == Schema::Int || v->type == Schema::Long) d = (double)v->i;
+      else io_error("intercept.prior.mean.map: value of key " + k->s + " is not a number or a string");
+      out[k->s] = d;   // HashMap.put: the last record of a key wins
+    }
+  }
+  return out;
+}
+
+void run_item_model_train(const JobConfig& c) {
+  const std::string out = c.get("output.model.path");
+  const bool binary = c.get_bool("binary.feature", false);
+  const bool compute_var = c.get_bool("compute.var", false);
+  const std::vector<float> il = lambda_list(c, "intercept.lambdas"), dl = lambda_list(c, "default.lambdas");
+  // conf.setFloat / getFloat (:112, :165): the default intercept prior mean is float-rounded
+  const double default_mean = (double)(float)c.get_double("intercept.default.prior.mean", 0.0);
+  std::unordered_map<std::string, double> mean_map;
+  if (!c.get("intercept.prior.mean.map", "").empty()) mean_map = read_prior_mean_map(c.get("intercept.prior.mean.map"));
+  // liblinear.epsilon, report.frequency and short.feature.index are accepted; the fit is an exact Newton solve
+  Dictionary dict; Rows rows;
+  read_prepared(c.get("input.paths"), dict, rows, binary);
+  const int D = (int)dict.names.size(), Dt = D + 1;
+  std::vector<std::pair<std::string, float>> lm_entries;
+  std::vector<float> lambda_map;
+  if (!c.get("lambda.map", "").empty()) {
+    lm_entries = read_lambda_map_entries(c.get("lambda.map"));
+    lambda_map.assign(D, 0.f);
+    for (auto& e : lm_entries) if (const int k = dict.find(e.first); k >= 0) lambda_map[k] = e.second;
+  }
+  // one dataset per key (:227-239), keys in Avro string order; a row's features sorted by id (llf/LibLinearDataset.java:481-482)
+  std::map<std::string, std::vector<size_t>> by_key;
+  for (size_t i = 0; i < rows.n(); i++) by_key[rows.key[i]].push_back(i);
+  const int K = (int)by_key.size();
+  std::vector<int64_t> krs{0}, rp{0}; std::vector<std::string> knames;
+  std::vector<int32_t> ci, rr; std::vector<float> vv, ww, oo;
+  std::vector<double> means;
+  for (auto& kv : by_key) {
+    knames.push_back(kv.first);
+    auto it = mean_map.find(kv.first);
+    means.push_back(it != mean_map.end() ? it->second : default_mean);   // :240-248
+    for (size_t i : kv.second) {
+      std::vector<std::pair<int32_t, float>> ent;
+      for (int64_t j = rows.rowptr[i]; j < rows.rowptr[i + 1]; j++) ent.emplace_back(rows.colidx[j], rows.vals[j]);
+      std::sort(ent.begin(), ent.end(), [](auto& a, auto& b) { return a.first < b.first; });
+      for (auto& e : ent) { ci.push_back(e.first); vv.push_back(e.second); }
+      rp.push_back((int64_t)ci.size());
+      rr.push_back(rows.response[i]); ww.push_back(rows.weight[i]); oo.push_back(rows.offset[i]);
+    }
+    krs.push_back((int64_t)rr.size());
+  }
+  // a key's model lists the intercept and the features its rows list (llf/LibLinear.java:343-350)
+  std::vector<std::vector<int32_t>> present(K);
+  for (int k = 0; k < K; k++) {
+    std::vector<int32_t>& pk = present[k];
+    pk.assign(ci.begin() + rp[krs[k]], ci.begin() + rp[krs[k + 1]]);
+    std::sort(pk.begin(), pk.end());
+    pk.erase(std::unique(pk.begin(), pk.end()), pk.end());
+  }
+  const int IL = (int)il.size(), DL = (int)dl.size();
+  std::vector<double> m((size_t)IL * DL * K * Dt), var(compute_var ? m.size() : 0);
+  if (K > 0)
+    ck(mlease_item_model_train(c.get_int("gpu.device", 0), nullptr, K, D, krs.data(), rp.data(), ci.data(), vv.data(), rr.data(), ww.data(), oo.data(),
+                               means.data(), IL, il.data(), DL, dl.data(), lambda_map.empty() ? nullptr : lambda_map.data(), binary ? 1 : 0,
+                               compute_var ? 1 : 0, m.data(), compute_var ? var.data() : nullptr));
+  // posteriorVar also lists every lambda.map feature the key's rows do not, at its prior variance 1/lambda (llf/LibLinear.java:384-397),
+  // after the dataset's features, in the map's order; the intercept's entry is always the dataset's
+  auto absent_map_entries = [&](int k) {
+    std::vector<std::pair<std::string, float>> ex;
+    for (auto& e : lm_entries) {
+      if (e.first == INTERCEPT) continue;
+      const int id = dict.find(e.first);
+      if (id >= 0 && std::binary_search(present[k].begin(), present[k].end(), id)) continue;
+      ex.emplace_back(e.first, (float)(1.0 / (double)e.second));
+    }
+    return ex;
+  };
+  AvroWriter w(out + "/models/part-r-00000.avro", SCHEMA_MODEL_WITH_VAR);
+  const bool generic = host_generic_ingest();
+  const FeaturePrefix fp(dict);
+  std::vector<float> mf(Dt), vf(Dt);
+  std::string rec;
+  for (int k = 0; k < K; k++) {
+    const auto extra = compute_var ? absent_map_entries(k) : std::vector<std::pair<std::string, float>>();
+    for (int a = 0; a < IL; a++)
+      for (int b = 0; b < DL; b++) {
+        const size_t base = (((size_t)a * DL + b) * K + k) * Dt;
+        for (int j = 0; j < Dt; j++) { mf[j] = (float)m[base + j]; vf[j] = compute_var ? (float)var[base + j] : 0.f; }
+        const std::string key = java_float_to_string(il[a]) + ":" + java_float_to_string(dl[b]) + "#" + knames[k];   // :265
+        if (generic) {   // Value-tree encoder: the reference implementation the tests compare with
+          Value r; r.type = Schema::Record; r.items.resize(3);
+          r.items[0] = Value::of_string(key);
+          Value& ml = r.items[1]; ml.type = Schema::Array;
+          ml.items.push_back(feature_value(INTERCEPT, mf[D]));
+          for (int32_t j : present[k]) ml.items.push_back(feature_value(dict.names[j], mf[j]));
+          Value& vl = r.items[2]; vl.type = Schema::Array;
+          vl.items.push_back(feature_value(INTERCEPT, vf[D]));   // without compute.var: new LinearModel().toAvro, (INTERCEPT) 0 (:271-274)
+          if (compute_var) {
+            for (int32_t j : present[k]) vl.items.push_back(feature_value(dict.names[j], vf[j]));
+            for (auto& e : extra) vl.items.push_back(feature_value(e.first, e.second));
+          }
+          w.append(r);
+        } else {
+          rec.clear();
+          put_str(rec, key.data(), key.size());
+          fp.encode_subset(rec, mf.data(), present[k]);
+          if (compute_var) {
+            put_long(rec, (int64_t)(1 + present[k].size() + extra.size()));
+            rec.append(fp.bytes, fp.off[0], fp.off[1] - fp.off[0]); put_float(rec, vf[D]);
+            for (int32_t j : present[k]) { rec.append(fp.bytes, fp.off[(size_t)j + 1], fp.off[(size_t)j + 2] - fp.off[(size_t)j + 1]); put_float(rec, vf[j]); }
+            for (auto& e : extra) { put_feature_key(rec, e.first); put_float(rec, e.second); }
+            put_long(rec, 0);
+          } else {
+            put_long(rec, 1); put_feature_key(rec, INTERCEPT); put_float(rec, 0.f); put_long(rec, 0);
+          }
+          w.append_encoded(rec.data(), rec.size(), 1);
+        }
+      }
+  }
+  w.close();
+  if (c.get_bool("remove.tmp.dir", true)) remove_tree(out + "/tmp-data");   // :122-127
+}
+
+[[maybe_unused]] const bool registered = register_job("ItemModelTrain", run_item_model_train);
+
+}  // namespace
+}  // namespace mlease_jobs

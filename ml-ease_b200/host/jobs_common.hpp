@@ -110,6 +110,40 @@ inline void put_long(std::string& o, int64_t v) {
 inline void put_str(std::string& o, const char* p, size_t n) { put_long(o, (int64_t)n); o.append(p, n); }
 inline void put_float(std::string& o, float f) { o.append(reinterpret_cast<const char*>(&f), 4); }
 
+// the (name, term) strings of a feature key (name, or name\u0001term)
+inline void put_feature_key(std::string& o, const std::string& key) {
+  const size_t p = key.find('\x01');
+  if (p == std::string::npos) { put_str(o, key.data(), key.size()); put_long(o, 0); }
+  else { put_str(o, key.data(), p); put_str(o, key.data() + p + 1, key.size() - p - 1); }
+}
+
+// The (name, term) part of every feature record of a model list in Avro binary, intercept first (models/LinearModel.java:697-720):
+// built once per file, after which a model is a run of [prefix, 4-byte float] appends instead of a Value tree per feature.
+struct FeaturePrefix {
+  std::string bytes;
+  std::vector<size_t> off;   // [D + 2]: entry 0 = intercept, entry k + 1 = dictionary feature k
+  explicit FeaturePrefix(const Dictionary& dict) {
+    off.push_back(bytes.size()); put_feature_key(bytes, INTERCEPT);
+    for (auto& n : dict.names) { off.push_back(bytes.size()); put_feature_key(bytes, n); }
+    off.push_back(bytes.size());
+  }
+  // one model list: coef[D] (intercept) first, then coef[0..D)
+  void encode(std::string& o, const float* coef) const {
+    const size_t D = off.size() - 2;
+    put_long(o, (int64_t)(D + 1));
+    o.append(bytes, off[0], off[1] - off[0]); put_float(o, coef[D]);
+    for (size_t k = 0; k < D; k++) { o.append(bytes, off[k + 1], off[k + 2] - off[k + 1]); put_float(o, coef[k]); }
+    put_long(o, 0);
+  }
+  // the intercept and the listed features only (a NaiveTrain model holds the features its key's rows list, llf/LibLinear.java:343-350)
+  void encode_subset(std::string& o, const float* coef, const std::vector<int32_t>& subset) const {
+    const size_t D = off.size() - 2;
+    put_long(o, (int64_t)(subset.size() + 1));
+    o.append(bytes, off[0], off[1] - off[0]); put_float(o, coef[D]);
+    for (int32_t k : subset) { o.append(bytes, off[(size_t)k + 1], off[(size_t)k + 2] - off[(size_t)k + 1]); put_float(o, coef[k]); }
+    put_long(o, 0);
+  }
+};
 extern const char* SCHEMA_TEST_LOGLIK;
 
 // regression_jobs.cpp
@@ -120,6 +154,11 @@ const Schema& rec_schema(const SchemaP& s);
 bool host_generic_ingest();
 // raw (unprepared) records of one file -> rows; item_key non-empty: rows.key = data.get(item_key).toString()
 void read_raw(const std::string& file, Dictionary& dict, Rows& rows, bool binary_feature, const std::string& item_key = "");
+// prepared records (RegressionPrepareOutput) of every file under path -> rows (appended), global dictionary ids
+void read_prepared(const std::string& path, Dictionary& dict, Rows& rows, bool binary_feature);
+std::vector<std::pair<std::string, float>> read_lambda_map_entries(const std::string& path);
+// {name, term, value} feature record of a model list (Value tree), value cast to float
+Value feature_value(const std::string& key, float v);
 std::map<std::string, std::unordered_map<std::string, double>> read_linear_models(const std::string& path, bool last_wins = false);
 // RegressionTest-style output schema: input fields with unions removed + pred:float
 std::string test_output_schema(const SchemaP& in, const char* name = "AdmmTestOutput", const char* ns = nullptr);

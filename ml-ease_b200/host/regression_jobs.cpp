@@ -9,6 +9,7 @@
 //   RegressionTestLoglik  jobs/RegressionTestLoglik.java:57-201
 //   RegressionNaiveTrain  jobs/RegressionNaiveTrain.java:99-415 (+ jobs/PartitionIdAssigner.java:41-101)
 //   ItemModelTest, ItemModelTestLoglik: item_model_jobs.cpp
+//   ItemModelTrain: item_model_train_job.cpp
 //   JobConfig             com/linkedin/mapred/JobConfig.java:50-224 (java .properties file)
 // Not mirrored: Hadoop job submission, HDFS, DistributedCache (local files only; is.local is implied).
 #include <algorithm>
@@ -409,39 +410,6 @@ Value model_list(const Dictionary& dict, const float* coef /*[D+1], intercept la
   else for (int k = 0; k < D; k++) a.items.push_back(feature_value(dict.names[k], coef[k]));
   return a;
 }
-// The (name, term) part of every feature record of a model list in Avro binary, intercept first (models/LinearModel.java:697-720):
-// built once per file, after which a model is a run of [prefix, 4-byte float] appends instead of a Value tree per feature.
-struct FeaturePrefix {
-  std::string bytes;
-  std::vector<size_t> off;   // [D + 2]: entry 0 = intercept, entry k + 1 = dictionary feature k
-  explicit FeaturePrefix(const Dictionary& dict) {
-    auto add = [&](const std::string& key) {
-      off.push_back(bytes.size());
-      const size_t p = key.find('\x01');
-      if (p == std::string::npos) { put_str(bytes, key.data(), key.size()); put_long(bytes, 0); }
-      else { put_str(bytes, key.data(), p); put_str(bytes, key.data() + p + 1, key.size() - p - 1); }
-    };
-    add(INTERCEPT);
-    for (auto& n : dict.names) add(n);
-    off.push_back(bytes.size());
-  }
-  // one model list: coef[D] (intercept) first, then coef[0..D)
-  void encode(std::string& o, const float* coef) const {
-    const size_t D = off.size() - 2;
-    put_long(o, (int64_t)(D + 1));
-    o.append(bytes, off[0], off[1] - off[0]); put_float(o, coef[D]);
-    for (size_t k = 0; k < D; k++) { o.append(bytes, off[k + 1], off[k + 2] - off[k + 1]); put_float(o, coef[k]); }
-    put_long(o, 0);
-  }
-  // the intercept and the listed features only (a NaiveTrain model holds the features its key's rows list, llf/LibLinear.java:343-350)
-  void encode_subset(std::string& o, const float* coef, const std::vector<int32_t>& subset) const {
-    const size_t D = off.size() - 2;
-    put_long(o, (int64_t)(subset.size() + 1));
-    o.append(bytes, off[0], off[1] - off[0]); put_float(o, coef[D]);
-    for (int32_t k : subset) { o.append(bytes, off[(size_t)k + 1], off[(size_t)k + 2] - off[(size_t)k + 1]); put_float(o, coef[k]); }
-    put_long(o, 0);
-  }
-};
 // LinearModelAvro records {key, model}; with uplusx: RegressionTrainOutput records {key, model, uplusx} (:706-711).
 // subsets (one entry per model, NULL = all features): the dictionary ids a model lists, ascending.
 void write_model_records(const std::string& path, const Dictionary& dict, const std::vector<std::pair<std::string, std::vector<float>>>& models,
@@ -510,11 +478,11 @@ std::vector<int32_t> gpu_devices(const JobConfig& c) {
 }
 
 // lambda.map file (ReadLambdaMapConsumer, regression/consumers/ReadLambdaMapConsumer.java:33-52; jobs/RegressionAdmmTrain.java:186-196,
-// jobs/RegressionNaiveTrain.java:318-332): records {name, term, value}; key = name or name\u0001term; value cast to float.
-// Returned as a dense [D] vector over the job's feature dictionary, 0 = not listed (features outside the dictionary cannot
-// occur in any model of this job and are dropped).
-std::vector<float> read_lambda_map(const std::string& path, const Dictionary& dict) {
-  std::vector<float> lm(dict.names.size(), 0.f);
+// jobs/RegressionNaiveTrain.java:318-332, jobs/ItemModelTrain.java:194-212): records {name, term, value}; key = name or name\u0001term;
+// value cast to float.  The map's keys in order of first appearance, a repeated key keeping its last value (HashMap.put).
+std::vector<std::pair<std::string, float>> read_lambda_map_entries(const std::string& path) {
+  std::vector<std::pair<std::string, float>> out;
+  std::unordered_map<std::string, size_t> at;
   for (auto& f : list_avro_files(path)) {
     AvroReader rd(f);
     const Schema& s = rec_schema(rd.schema());
@@ -525,9 +493,21 @@ std::vector<float> read_lambda_map(const std::string& path, const Dictionary& di
       const Value* tm = field(rec, s, "term");
       const float lam = (float)num_of(*vl);
       if (!(lam > 0.f)) io_error("lambda.map: lambda of feature " + nm->s + " must be > 0 (it becomes the prior variance 1/lambda)");
-      int k = dict.find(feature_key(nm->s, tm ? tm->s : ""));
-      if (k >= 0) lm[k] = lam;
+      const std::string key = feature_key(nm->s, tm ? tm->s : "");
+      auto it = at.find(key);
+      if (it != at.end()) out[it->second].second = lam;
+      else { at.emplace(key, out.size()); out.emplace_back(key, lam); }
     }
+  }
+  return out;
+}
+// The same as a dense [D] vector over the job's feature dictionary, 0 = not listed (features outside the dictionary cannot occur in
+// any model of the job and are dropped).
+std::vector<float> read_lambda_map(const std::string& path, const Dictionary& dict) {
+  std::vector<float> lm(dict.names.size(), 0.f);
+  for (auto& e : read_lambda_map_entries(path)) {
+    const int k = dict.find(e.first);
+    if (k >= 0) lm[k] = e.second;
   }
   return lm;
 }
@@ -1343,7 +1323,7 @@ extern "C" {
 const char* mlease_job_last_error(void) { return g_job_err.c_str(); }
 
 // job_class: Regression | RegressionPrepare | RegressionAdmmTrain | RegressionTest | RegressionTestLoglik | RegressionNaiveTrain |
-// ItemModelTest | ItemModelTestLoglik
+// ItemModelTest | ItemModelTestLoglik | ItemModelTrain
 // (the README's names AdmmPrepare / AdmmTrain / AdmmTest / AdmmTestLoglik / NaiveTrain are accepted as aliases).
 int mlease_job_run(const char* job_class, const char* config_path) {
   try {

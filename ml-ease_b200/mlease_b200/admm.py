@@ -470,3 +470,25 @@ def naive_train(vals, key_rowstart, response, lambdas, *, rowptr=None, colidx=No
                                    float(prior_mean), int(penalize_intercept), int(has_intercept), int(data_size_threshold),
                                    int(bool(binary_feature)), ptr(out), ptr(skipped)))
     return out, skipped.astype(bool)
+
+
+def item_model_train(vals, key_rowstart, response, intercept_lambdas, default_lambdas, *, rowptr, colidx, num_features,
+                     intercept_prior_mean=None, weight=None, offset=None, lambda_map=None, binary_feature=False, compute_var=False,
+                     device=0, stream=None):
+    """ItemModelTrain reducers (jobs/ItemModelTrain.java:226-276) for K keys on one CSR upload: one fit per (intercept lambda, default
+    lambda), in list order.  intercept_prior_mean [K] float64 (None = 0).
+    -> (models [IL, DL, K, D+1] float64, posterior variance of the same shape or None)."""
+    krs = np.ascontiguousarray(key_rowstart, np.int64)
+    K, D = len(krs) - 1, int(num_features)
+    il, dl = _f32(np.atleast_1d(intercept_lambdas)), _f32(np.atleast_1d(default_lambdas))
+    rp, ci, vals = _keep(rowptr, np.int64), _keep(colidx, np.int32), _keep(vals, np.float32)
+    r, w, o, lm = _keep(response, np.int32), _keep(weight, np.float32), _keep(offset, np.float32), _keep(lambda_map, np.float32)
+    im = np.zeros(K, np.float64) if intercept_prior_mean is None else np.ascontiguousarray(intercept_prior_mean, np.float64)
+    if len(im) != K:
+        raise ValueError("intercept_prior_mean must hold one entry per key")
+    out = np.zeros((len(il), len(dl), K, D + 1), np.float64)
+    var = np.zeros_like(out) if compute_var else None
+    check(lib().mlease_item_model_train(device, stream, K, D, ptr(krs), ptr(rp), ptr(ci), ptr(vals), ptr(r), ptr(w), ptr(o), ptr(im),
+                                        len(il), ptr(il), len(dl), ptr(dl), ptr(lm), int(bool(binary_feature)), int(bool(compute_var)),
+                                        ptr(out), ptr(var)))
+    return out, var
