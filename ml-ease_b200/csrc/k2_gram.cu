@@ -14,8 +14,9 @@
 // Warpgroup roles (384 threads): warpgroup 0 = TMA producer (one lane), warpgroups 1-2 = consumers,
 // each issuing m64n256k16 wgmma for its 64 rows of the tile (128 fp32 accumulators a thread).
 //
-// CSR partitions have two kernels on the same e4m3 operand bytes: gram_csr_wgmma_kernel (operand blocks assembled in shared
-// memory, wgmma) and gram_csr_sparse_kernel (only the nonzero products of each row, exact int64 sums).  session.cu batch_alloc
+// CSR partitions have two kernels on the same e4m3 operand values: gram_csr_wgmma_kernel (operand blocks assembled in shared
+// memory, wgmma; one byte an entry) and gram_csr_sparse_kernel (only the nonzero products of each row, exact int64 sums; one
+// pre-decoded 32-bit word an entry).  session.cu batch_alloc
 // picks one per batch from the data: the sparse one wins below about 3 % density at 10k features.
 //
 // A fp32 SIMT kernel computing the same partials from the same bf16 operand is kept ONLY as a
@@ -364,9 +365,30 @@ gram_csr_wgmma_kernel(const Problem* __restrict__ probs, const GramTile* __restr
   }
 }
 
-// Gram operand of the CSR kernel, once per build: for every entry of the block-major list, the e4m3 byte
-// e4m3(value * (sqrt(d_row) * gram_scale)).  gram_scale is a power of two that keeps sqrt(d) x in e4m3's normal range (chol_prep
-// undoes it exactly).  sdvec is rewritten by K1 between builds, so this runs immediately before each build, gated like it.
+// e4m3 byte -> signed integer number of units of 2^-9 (subnormal m: m units; normal (e, m): (8 + m) << (e - 1)).  0x7F / 0xFF
+// (NaN) never occur: the operand pass converts with __NV_SATFINITE.
+__device__ __forceinline__ int e4m3_units(uint32_t b) {
+  const int e = (int)((b >> 3) & 15u), m = (int)(b & 7u);
+  const int mag = e ? (8 | m) << (e - 1) : m;
+  return (b & 0x80u) ? -mag : mag;
+}
+
+// The sparse kernel's operand word of an entry: everything it needs, decoded once per build instead of once per tile reading it.
+// The e4m3 value in units of 2^-9 is an integer of at most 4 significant bits below 2^18, so as an fp32 its low 20 mantissa bits
+// are zero; the low 15 carry the entry's row in its span (8 bits: 32 (group mod span) + row in group) and column in its 128-block
+// (7 bits).  Bits 15 .. 19 stay zero.  Decoding is a mask and one float-to-int conversion, a shift and two masks.
+constexpr uint32_t SW_VALUE_MASK = 0xFFFF8000u;
+__device__ __forceinline__ uint32_t sparse_word(uint32_t byte, int row_in_span, int col) {
+  return __float_as_uint((float)e4m3_units(byte)) | ((uint32_t)row_in_span << 7) | (uint32_t)col;
+}
+__device__ __forceinline__ int sw_units(uint32_t w) { return __float2int_rz(__uint_as_float(w & SW_VALUE_MASK)); }
+__device__ __forceinline__ int sw_row(uint32_t w) { return (int)((w >> 7) & 255u); }
+__device__ __forceinline__ int sw_col(uint32_t w) { return (int)(w & 127u); }
+
+// Gram operand of the CSR kernels, once per build: for every entry of the block-major list, the e4m3 byte
+// e4m3(value * (sqrt(d_row) * gram_scale)), or for a sparse-kernel batch (csr_gram == CSR_GRAM_SPARSE) the same value as
+// sparse_word.  gram_scale is a power of two that keeps sqrt(d) x in e4m3's normal range (chol_prep undoes it exactly).  sdvec
+// is rewritten by K1 between builds, so this runs immediately before each build, gated like it.
 // One warp per 32-row group: lane l holds sqrt(d) of row 32 g + l, and the group's runs of every column block follow.
 __global__ void __launch_bounds__(256) gram_csr_operand_kernel(const Problem* __restrict__ probs, int force, int share) {
   if (share > 1 && blockIdx.y % share != 0) return;   // see gram_wgmma_kernel
@@ -380,11 +402,15 @@ __global__ void __launch_bounds__(256) gram_csr_operand_kernel(const Problem* __
   const unsigned short* __restrict__ keys = pb.bm_keys;
   const float* __restrict__ vals = pb.bm_vals;
   unsigned char* __restrict__ out = pb.bm_e4m3;
+  uint32_t* __restrict__ out_w = pb.bm_word;
+  const bool word = pb.csr_gram == CSR_GRAM_SPARSE;
+  const int span = gram_sparse_span(pb.bm_entries, nblk, ngroups);   // as gram_csr_sparse_kernel computes it
   const float gscale = pb.gram_scale;
   const long long nw = ((long long)gridDim.x * blockDim.x) >> 5;
   for (long long g = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; g < ngroups; g += nw) {
     const long long r = g * SK + lane;
     const float sd = r < n ? pb.sdvec[r] * gscale : 0.f;
+    const int row0 = 32 * (int)(g % span);   // the group's first row in its span
     for (int b = 0; b < nblk; b++) {
       const uint32_t lo = (uint32_t)offs[(size_t)b * ngroups + g], hi = (uint32_t)offs[(size_t)b * ngroups + g + 1];
       for (uint32_t e0 = lo; e0 < hi; e0 += 32) {
@@ -392,15 +418,19 @@ __global__ void __launch_bounds__(256) gram_csr_operand_kernel(const Problem* __
         const bool v = e < hi;
         const uint32_t key = v ? (uint32_t)keys[e] : 0u;
         const float val = v ? vals[e] : 0.f;
-        const float sdk = __shfl_sync(0xffffffffu, sd, kmaj_row(key));
-        if (v) out[e] = (unsigned char)__nv_cvt_float_to_fp8(val * sdk, __NV_SATFINITE, __NV_E4M3);
+        const int k = kmaj_row(key);
+        const float sdk = __shfl_sync(0xffffffffu, sd, k);
+        const uint32_t byte = __nv_cvt_float_to_fp8(val * sdk, __NV_SATFINITE, __NV_E4M3);
+        if (!v) continue;
+        if (word) out_w[e] = sparse_word(byte, row0 + k, (int)(key >> 5));
+        else out[e] = (unsigned char)byte;
       }
     }
   }
 }
 
 // ------------------------------------------------------------------------------------------
-// Sparse CSR Gram: the same partial from the same e4m3 operand bytes, but only the nonzero products of each row are formed.  At
+// Sparse CSR Gram: the same partial from the same e4m3 operand values, but only the nonzero products of each row are formed.  At
 // 1 % density a 32-row x 128-column operand block holds ~1 % nonzeros, so the wgmma kernel above spends ~10^4 multiply-adds per
 // nonzero product; here each product is one integer multiply and (mostly) one native shared-memory atomic add.
 // Exact and deterministic: an e4m3 value is an integer number of units of 2^-9 (|v| <= 448 = 229376 units < 2^18), so a product
@@ -416,8 +446,10 @@ __global__ void __launch_bounds__(256) gram_csr_operand_kernel(const Problem* __
 // SP_SPAN (256 rows), fewer on denser data (gram_sparse_span: the mean range of a span must fit 3/4 of a stage chunk, since each
 // further chunk re-reads the bi range); warp w takes the spans w, w + SP_WARPS, ...  The list is block-major with ascending
 // groups, so a block's entries for a span are one contiguous range [offs[b][g0], offs[b][g0 + span]), in row order (group, then
-// row in group: csr_bm_fill_kernel writes lane 0's entries, then lane 1's, ...), and an entry's row in the span is
-// 32 (group - g0) + kmaj_row(key), its group found by walking the span's warp-uniform group bounds as the entries go by.  Per
+// row in group: csr_bm_fill_kernel writes lane 0's entries, then lane 1's, ...).  The operand pass, which visits every entry once
+// per build anyway, writes each entry as one sparse_word holding its value in units, its row in the span
+// (32 (group - g0) + row in group) and its column, so that the 80-odd tiles reading an entry each decode it with a few masks and
+// one conversion (before: a key and a byte load, the e4m3 decode, the swizzle decode and a walk over the span's group bounds).  Per
 // span the warp stages the bj range's nonzero entries in shared memory with each row's [start, end), then enumerates the
 // (bi entry, staged partner of its row) pairs in a flat index space: per 32 bi entries an inclusive warp scan of the partner
 // counts, then steps of 32 pairs, one per lane, each lane finding its owner entry from one OR-reduction of the owners' end
@@ -425,11 +457,11 @@ __global__ void __launch_bounds__(256) gram_csr_operand_kernel(const Problem* __
 // over the rows, and a row with 128 entries in both blocks (128^2 pairs) is as many full steps.  A bj range longer than SP_STAGE
 // entries is staged in chunks (boundaries may fall inside a row: each chunk pairs with its own part of the row), the bi range
 // re-read for each.
-// What bounds it (1M x 10k x 1 %, H100 at 400 W, 46.5 ms a build): the per-entry work, not the products.  Each batch of 32
-// entries is ~90 instructions to stage (load, decode, group, ballot, row table) and as many to scan on the bi side, for ~1.3
-// products per entry.  In a 52 ms form of the kernel (fixed 8-group spans, loads consumed as soon as issued), leaving out the pair
-// steps left 35 ms, and leaving out the whole bi side too left 18 ms.
-// Diagonal tiles keep the pairs with c2 <= c1 only (predicated) and mirror them in the epilogue.  Zero operand bytes (w = 0
+// What bounds it (1M x 10k x 1 %, H100 80GB HBM3 at 700 W, 36.5 ms a build): the per-entry work, not the products.  Each batch
+// of 32 entries is 50 warp instructions to stage (load, decode, ballot, row table) and 76 to scan on the bi side up to the pair
+// steps (row-table lookup, partner-count scan, owner table), for ~1.3 products per entry; with the byte operand they were 89 and
+// 114, plus ~12 for every group bound a batch crossed.
+// Diagonal tiles keep the pairs with c2 <= c1 only (predicated) and mirror them in the epilogue.  Zero operand values (w = 0
 // rows, the end of a range) are skipped.
 // Same-cell contention: every row's intercept entry pairs with itself in the intercept's diagonal tile, so consecutive rows'
 // (intercept, intercept) products would be one step of 32 same-address atomics.  A lane sums that cell's products in an int64
@@ -448,16 +480,9 @@ constexpr size_t SP_ACC_BYTES = (size_t)SN * SN * 2 * sizeof(uint32_t);   // 128
 constexpr size_t SP_WARP_BYTES = (size_t)SP_STAGE * 4 + (size_t)SP_ROWS * 4 + 32 * 8;
 constexpr size_t SP_SMEM = SP_ACC_BYTES + (size_t)SP_WARPS * SP_WARP_BYTES;
 static_assert(SP_SMEM <= 227 * 1024, "sparse Gram shared memory");
-static_assert(SP_STAGE % 16 == 0 && SP_SPAN + 1 <= 16, "layout of the stage and of the span bounds");
+static_assert(SP_STAGE % 16 == 0, "layout of the stage");
 static_assert(SP_SPAN == 8 && SP_STAGE == 448, "gram_sparse_span (kernels.cuh) assumes these");
-
-// e4m3 byte -> signed integer number of units of 2^-9 (subnormal m: m units; normal (e, m): (8 + m) << (e - 1)).  0x7F / 0xFF
-// (NaN) never occur: the operand pass converts with __NV_SATFINITE.
-__device__ __forceinline__ int e4m3_units(uint32_t b) {
-  const int e = (int)((b >> 3) & 15u), m = (int)(b & 7u);
-  const int mag = e ? (8 | m) << (e - 1) : m;
-  return (b & 0x80u) ? -mag : mag;
-}
+static_assert(SP_ROWS <= 256, "sparse_word holds the row in the span in 8 bits");
 
 __global__ void __launch_bounds__(SP_THREADS, 1)
 gram_csr_sparse_kernel(const Problem* __restrict__ probs, const GramTile* __restrict__ tiles, int force, int share) {
@@ -491,8 +516,7 @@ gram_csr_sparse_kernel(const Problem* __restrict__ probs, const GramTile* __rest
   const bool valid = bi < pb.nblk128 && bj < pb.nblk128;
   const long long* __restrict__ offs_i = pb.bm_offs + (size_t)bi * ngroups;
   const long long* __restrict__ offs_j = pb.bm_offs + (size_t)bj * ngroups;
-  const unsigned short* __restrict__ keys = pb.bm_keys;
-  const unsigned char* __restrict__ bytes = pb.bm_e4m3;
+  const uint32_t* __restrict__ words = pb.bm_word;
   const uint32_t lt = (1u << lane) - 1u;
   // a cell gets the product p (units of 2^-18, int64): the low word with a native atomic add that returns the old word, the high
   // word plus the carry out of the low add when that is not 0
@@ -502,50 +526,28 @@ gram_csr_sparse_kernel(const Problem* __restrict__ probs, const GramTile* __rest
     const int hi = (int)(p >> 32) + (old + lo < old ? 1 : 0);
     if (hi != 0) atomicAdd(acc_hi + cell, hi);
   };
-  // the list holds < 2^32 entries (checked at upload): entry numbers are 32-bit.  A span's group bounds, lane-distributed: lane k
-  // (k <= span) holds offs_i[g0 + k], lane 16 + k offs_j[g0 + k], clamped to the last group (a short last span's missing groups
-  // are empty).  Fetched two spans ahead, and the first SP_AHEAD batches of 32 entries of both ranges one span ahead: a warp has
-  // one span in flight.  Inside a range the entries are loaded SP_AHEAD batches ahead: most bj ranges are not in L2 (a wave's
-  // tiles read ~80 different bj blocks), so a batch's loads need the time of several batches' work to arrive.
+  // the list holds < 2^32 entries (checked at upload): entry numbers are 32-bit.  A span's ranges, lane-distributed: lanes 0, 1
+  // hold offs_i[g0], offs_i[g0 + span], lanes 2, 3 the same of offs_j, clamped to the last group (a short last span's missing
+  // groups are empty).  Fetched two spans ahead, and the first SP_AHEAD batches of 32 entries of both ranges one span ahead: a
+  // warp has one span in flight.  Inside a range the entries are loaded SP_AHEAD batches ahead: most bj ranges are not in L2 (a
+  // wave's tiles read ~80 different bj blocks), so a batch's loads need the time of several batches' work to arrive.
   auto ld_bounds = [&](long long s) -> uint32_t {
-    const int k = lane & 15;
-    if (!valid || s >= nspans || k > span) return 0u;
-    return (uint32_t)__ldg((lane < 16 ? offs_i : offs_j) + min(s * span + k, ngroups));
+    if (!valid || s >= nspans || lane >= 4) return 0u;
+    return (uint32_t)__ldg((lane < 2 ? offs_i : offs_j) + min(s * span + (lane & 1) * span, ngroups));
   };
-  // an entry's key and e4m3 byte, both 0 past the end of its range (a zero byte: skipped like any zero operand).  Kept as the two
-  // loaded registers until the entry is used: an instruction that combined them at the load would wait for the load right there
-  struct Entry { uint32_t key, byte; };
-  auto ld_entry = [&](uint32_t e, uint32_t hi) -> Entry {
-    Entry x = {0u, 0u};
-    if (e < hi) { x.key = __ldg(keys + e); x.byte = __ldg(bytes + e); }
-    return x;
-  };
-  struct Span { uint32_t b; Entry i[SP_AHEAD], j[SP_AHEAD]; };
+  // an entry's operand word, 0 past the end of its range (a zero value: skipped like any zero operand)
+  auto ld_entry = [&](uint32_t e, uint32_t hi) -> uint32_t { return e < hi ? __ldg(words + e) : 0u; };
+  struct Span { uint32_t ilo, ihi, jlo, jhi, i[SP_AHEAD], j[SP_AHEAD]; };
   auto take = [&](Span& q, uint32_t b) {
-    q.b = b;
-    const uint32_t ilo = __shfl_sync(0xffffffffu, b, 0), ihi = __shfl_sync(0xffffffffu, b, span);
-    const uint32_t jlo = __shfl_sync(0xffffffffu, b, 16), jhi = __shfl_sync(0xffffffffu, b, 16 + span);
+    q.ilo = __shfl_sync(0xffffffffu, b, 0); q.ihi = __shfl_sync(0xffffffffu, b, 1);
+    q.jlo = __shfl_sync(0xffffffffu, b, 2); q.jhi = __shfl_sync(0xffffffffu, b, 3);
 #pragma unroll
-    for (int k = 0; k < SP_AHEAD; k++) { q.i[k] = ld_entry(ilo + lane + 32 * k, ihi); q.j[k] = ld_entry(jlo + lane + 32 * k, jhi); }
-  };
-  // group of entry e of a range, from its bounds (lane 16 * side + k): k is the next bound not yet passed and nb its value, so the
-  // batch's first entry is in group k - 1; every bound below lim (the end of the batch) adds one to the entries at or past it
-  auto group_of = [&](uint32_t e, uint32_t lim, const Span& q, int side, int& k, uint32_t& nb) -> int {
-    int g = k - 1;
-    while (k < span && nb < lim) {
-      g += e >= nb ? 1 : 0;
-      k++;
-      nb = __shfl_sync(0xffffffffu, q.b, 16 * side + k);
-    }
-    return g;
+    for (int k = 0; k < SP_AHEAD; k++) { q.i[k] = ld_entry(q.ilo + lane + 32 * k, q.ihi); q.j[k] = ld_entry(q.jlo + lane + 32 * k, q.jhi); }
   };
   long long hot_sum = 0;   // this lane's products of the intercept's cell
   auto run = [&](const Span& q) {
-    const uint32_t ilo = __shfl_sync(0xffffffffu, q.b, 0), ihi = __shfl_sync(0xffffffffu, q.b, span);
-    const uint32_t jlo = __shfl_sync(0xffffffffu, q.b, 16), jhi = __shfl_sync(0xffffffffu, q.b, 16 + span);
+    const uint32_t ilo = q.ilo, ihi = q.ihi, jlo = q.jlo, jhi = q.jhi;
     if (ilo == ihi || jlo == jhi) return;
-    int jk = 1;
-    uint32_t jnb = __shfl_sync(0xffffffffu, q.b, 17);
     for (uint32_t c0 = jlo; c0 < jhi; c0 += SP_STAGE) {
       const uint32_t c1 = min(jhi, c0 + SP_STAGE);   // >= jlo + 32 * SP_AHEAD or = jhi: the prefetched batches lie in the first chunk
       __syncwarp();   // the previous chunk's readers are done
@@ -554,15 +556,14 @@ gram_csr_sparse_kernel(const Problem* __restrict__ probs, const GramTile* __rest
       __syncwarp();
       // ---- stage the chunk's nonzero entries; a kept entry whose row differs from the previous kept one starts its row
       int nst = 0, prev_row = -1;
-      Entry x[SP_AHEAD + 1];   // the batches base, base + 32, ...
+      uint32_t x[SP_AHEAD + 1];   // the batches base, base + 32, ...
 #pragma unroll
       for (int k = 0; k < SP_AHEAD; k++) x[k] = c0 == jlo ? q.j[k] : ld_entry(c0 + 32 * k + lane, c1);
       for (uint32_t base = c0; base < c1; base += 32) {
         x[SP_AHEAD] = ld_entry(base + 32 * SP_AHEAD + lane, c1);
-        const int g = group_of(base + lane, min(base + 32, c1), q, 1, jk, jnb);
-        const int v = e4m3_units(x[0].byte);
-        const uint32_t key = x[0].key;
-        const int r = 32 * g + kmaj_row(key);
+        const uint32_t w = x[0];
+        const int v = sw_units(w);
+        const int r = sw_row(w);
         const bool keep = v != 0;
         const uint32_t m = __ballot_sync(0xffffffffu, keep);
         const uint32_t below = m & lt;
@@ -570,7 +571,7 @@ gram_csr_sparse_kernel(const Problem* __restrict__ probs, const GramTile* __rest
         const int pr = below ? up : prev_row;
         const int s = nst + __popc(below);
         if (keep) {
-          stage[s] = v * 128 + (int)(key >> 5);
+          stage[s] = v * 128 + sw_col(w);
           if (r != pr) { rtab16[2 * r] = (unsigned short)s; if (pr >= 0) rtab16[2 * pr + 1] = (unsigned short)s; }
         }
         if (m) prev_row = __shfl_sync(0xffffffffu, r, 31 - __clz(m));
@@ -582,16 +583,13 @@ gram_csr_sparse_kernel(const Problem* __restrict__ probs, const GramTile* __rest
       if (lane == 0) rtab16[2 * prev_row + 1] = (unsigned short)nst;
       __syncwarp();
       // ---- the (bi entry, staged partner) pairs, 32 bi entries at a time
-      int ik = 1;
-      uint32_t inb = __shfl_sync(0xffffffffu, q.b, 1);
 #pragma unroll
       for (int k = 0; k < SP_AHEAD; k++) x[k] = q.i[k];
       for (uint32_t base = ilo; base < ihi; base += 32) {
         x[SP_AHEAD] = ld_entry(base + 32 * SP_AHEAD + lane, ihi);
-        const int g = group_of(base + lane, min(base + 32, ihi), q, 0, ik, inb);
-        const int a = e4m3_units(x[0].byte);
-        const uint32_t key = x[0].key;
-        const uint32_t t = a != 0 ? rtab[32 * g + kmaj_row(key)] : 0u;
+        const uint32_t w = x[0];
+        const int a = sw_units(w);
+        const uint32_t t = a != 0 ? rtab[sw_row(w)] : 0u;
         const int s0 = (int)(t & 0xFFFFu), cnt = (int)(t >> 16) - s0;
         int incl = cnt;   // inclusive warp scan of the partner counts
 #pragma unroll
@@ -606,7 +604,7 @@ gram_csr_sparse_kernel(const Problem* __restrict__ probs, const GramTile* __rest
         // owners (entries with partners) in lane order: pair p belongs to the owner of rank #{owners whose pairs end at or before p}
         const uint32_t owners = __ballot_sync(0xffffffffu, cnt > 0);
         __syncwarp();   // the previous batch's readers of own[] are done
-        if (cnt > 0) own[__popc(owners & lt)] = make_int2(a * 128 + (int)(key >> 5), s0 - (incl - cnt));
+        if (cnt > 0) own[__popc(owners & lt)] = make_int2(a * 128 + sw_col(w), s0 - (incl - cnt));
         __syncwarp();
         int before = 0;   // owners whose pairs end before this step
         for (int p0 = 0; p0 < total; p0 += 32) {

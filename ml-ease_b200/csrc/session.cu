@@ -238,12 +238,14 @@ int dev_alloc(Batch& B, void** p, size_t bytes, bool zero = true) {
 }
 
 // Bytes the Gram path allocates for a batch beyond the O(D') solver state: split-K Gram partials (one slice at least), the fp64
-// factor, L^-1 and H^-1, the diagonal-block side buffers, the bf16 Y of wide systems and the e4m3 operands (~26 D'^2 per problem).
+// factor, L^-1 and H^-1, the diagonal-block side buffers, the bf16 Y of wide systems (~26 D'^2 per problem) and the CSR operands
+// (B.csr_gram must be set: one byte an entry for the wgmma kernel, one 32-bit word for the sparse kernel).
+static int csr_operand_bytes(int csr_gram) { return csr_gram == CSR_GRAM_SPARSE ? 4 : 1; }
 static double gram_path_bytes(const Batch& B) {
   const double Dp = round_up(B.ldx, 128), ldh = round_up(B.Dt, 32);
   double per = Dp * Dp * 4.0 + 3.0 * ldh * ldh * 8.0 + 2.0 * ldh * 32 * 8.0 + (cholesky_factored_direction((int)ldh) ? ldh * ldh * 2.0 : 0.0);
   double bytes = per * B.nprob;
-  for (auto& p : B.h) bytes += (double)p.bm_entries;
+  for (auto& p : B.h) bytes += (double)csr_operand_bytes(B.csr_gram) * (double)p.bm_entries;
   return bytes;
 }
 
@@ -251,13 +253,15 @@ static double gram_path_bytes(const Batch& B) {
 // run of every 32-row group once per tile it belongs to (nblk + 1 tiles: `reads` entries in all).  wgmma: every 128 x 128 lower
 // tile times every 32-row group on the tensor pipe, plus the producers' run loads, which is what makes its rate fall at small n
 // and high density.  Sparse: per product (integer multiply + native shared atomic add), per (tile, span) visit (gram_sparse_span
-// groups: fetching and walking the span's bounds) and per entry read (loading, decoding and staging or scanning it), with the
-// whole device busy; a grid of fewer CTAs than SMs is that much slower.  Relative least-squares fits of tools/time_gram.py on an
-// H100 80GB HBM3 at a 400 W power limit over 0.3 - 20 % density at 10k features (DESIGN.md section 4): the sparse model is within
-// 3.5 % and the wgmma model within 9.5 % of every measured shape, so near the crossover (~3 % at 10k features) the rule may pick
-// a kernel up to ~10 % slower than the other.
+// groups: fetching the span's two bounds per block) and per entry read (loading its pre-decoded word and staging or scanning it),
+// with the whole device busy; a grid of fewer CTAs than SMs is that much slower.  Relative least-squares fits of
+// tools/time_gram.py (REPS=3) over 0.3 - 20 % density at 10k features (DESIGN.md section 4): the wgmma constants on an H100 80GB
+// HBM3 at a 400 W power limit, the sparse ones, refitted for the one-word operand, on an H100 80GB HBM3 at a 700 W power limit
+// (the wgmma times there are within 3.5 % of the 400 W ones).  The sparse model is within 2.5 % and the wgmma model within 9.5 %
+// of every measured shape, so near the crossover (~3 % at 10k features) the rule may pick a kernel up to ~10 % slower than the
+// other.
 constexpr double GRAM_WGMMA_S_PER_MAC = 1.317e-15, GRAM_WGMMA_S_PER_READ = 4.315e-12;
-constexpr double GRAM_SPARSE_S_PER_PAIR = 1.822e-12, GRAM_SPARSE_S_PER_VISIT = 4.652e-10, GRAM_SPARSE_S_PER_READ = 3.716e-12;
+constexpr double GRAM_SPARSE_S_PER_PAIR = 1.808e-12, GRAM_SPARSE_S_PER_VISIT = 2.548e-10, GRAM_SPARSE_S_PER_READ = 2.915e-12;
 static double gram_cost(const Problem& p, int Dp, int kind, double ctas, int num_sms) {
   const double nblk = Dp / 128, tiles = nblk * (nblk + 1) / 2, groups = (double)((p.n + 31) / 32);
   const int span = gram_sparse_span(p.bm_entries, Dp / 128, (p.n + 31) / 32);
@@ -319,29 +323,7 @@ int batch_alloc(Batch& B, int num_sms, int hessian_policy, int csr_gram_force = 
   if (hessian_policy == 2 && !B.csr_fx)
     return fail(MLEASE_ERR_INVALID, "hessian_policy 2 (matrix-free Newton-CG) needs CSR rows with strictly increasing column ids");
   B.matfree = hessian_policy == 2 ? 1 : 0;
-  if (!B.matfree && B.csr && B.gram_from_csr) {
-    // the Gram path's bytes plus the O(D') state allocated with it (vectors, L-BFGS pairs, per-CTA partials, sqrt(d) per row) and
-    // a margin for the session's own vectors: a Gram path that would only just fit is not taken
-    double state = 0;
-    for (auto& p : B.h) state += 8.0 * (double)p.n;
-    state += (double)nprob * (8.0 * ((9 + 2 * BFGS_M + gpart_rows) * (double)ldx + B.k1_grid + 8) + 16.0 * ldx +
-                              (B.k1_fused ? 4.0 * B.k1_grid * ldx : 0.0));
-    size_t free_b = 0, total_b = 0;
-    CK(cudaMemGetInfo(&free_b, &total_b));
-    if (gram_path_bytes(B) + state + (256.0 * 1024 * 1024) > (double)free_b) B.matfree = 1;
-  }
-  // Cost model for the rebuild policy (seconds, order of magnitude only: the policy compares the two with a factor of 8): one K1
-  // pass streams the partition at ~5 TB/s; a rebuild is n*Dt^2 flop at ~1 PFLOP/s (tensor-core Gram, lower triangle) plus
-  // ~Dt^3 fp64 flop at ~5 TFLOP/s (Cholesky + inverse).
-  {
-    double bytes = 0;
-    for (auto& p : B.h) bytes = std::max(bytes, B.csr ? 8.0 * (double)p.nnz_hint + 17.0 * (double)p.n : (double)p.n * 4.0 * ldx);
-    const double t_pass = bytes / 5e12 + 20e-6;
-    const double t_rebuild = (double)maxn * B.Dt * B.Dt / 1e15 + (double)B.Dt * B.Dt * B.Dt / 5e12 + 300e-6;
-    // only wide systems qualify: small ones (NaiveTrain's per-key fits, cold-started every time) are launch-bound, not
-    // flop-bound, and a mid-update rebuild saves them many lock-step slots
-    B.rebuild_is_expensive = (t_rebuild > 8.0 * t_pass && B.Dt > 2048 && !B.matfree) ? 1 : 0;
-  }
+  // the CSR Gram kernel first: its operand's size enters the memory check below
   B.csr_gram = 0;
   if (B.gram_from_csr && !B.matfree) {
     double t_sparse = 0, t_wgmma = 0;
@@ -356,6 +338,29 @@ int batch_alloc(Batch& B, int num_sms, int hessian_policy, int csr_gram_force = 
     if (csr_gram_force == CSR_GRAM_SPARSE && !fits)
       return fail(MLEASE_ERR_INVALID, "the sparse CSR Gram's int64 sums hold at most 2^27 rows per partition");
     if (csr_gram_force) B.csr_gram = csr_gram_force;
+  }
+  if (!B.matfree && B.csr && B.gram_from_csr) {
+    // the Gram path's bytes plus the O(D') state allocated with it (vectors, L-BFGS pairs, per-CTA partials, sqrt(d) per row) and
+    // a margin for the session's own vectors: a Gram path that would only just fit is not taken
+    double state = 0;
+    for (auto& p : B.h) state += 8.0 * (double)p.n;
+    state += (double)nprob * (8.0 * ((9 + 2 * BFGS_M + gpart_rows) * (double)ldx + B.k1_grid + 8) + 16.0 * ldx +
+                              (B.k1_fused ? 4.0 * B.k1_grid * ldx : 0.0));
+    size_t free_b = 0, total_b = 0;
+    CK(cudaMemGetInfo(&free_b, &total_b));
+    if (gram_path_bytes(B) + state + (256.0 * 1024 * 1024) > (double)free_b) { B.matfree = 1; B.csr_gram = 0; }
+  }
+  // Cost model for the rebuild policy (seconds, order of magnitude only: the policy compares the two with a factor of 8): one K1
+  // pass streams the partition at ~5 TB/s; a rebuild is n*Dt^2 flop at ~1 PFLOP/s (tensor-core Gram, lower triangle) plus
+  // ~Dt^3 fp64 flop at ~5 TFLOP/s (Cholesky + inverse).
+  {
+    double bytes = 0;
+    for (auto& p : B.h) bytes = std::max(bytes, B.csr ? 8.0 * (double)p.nnz_hint + 17.0 * (double)p.n : (double)p.n * 4.0 * ldx);
+    const double t_pass = bytes / 5e12 + 20e-6;
+    const double t_rebuild = (double)maxn * B.Dt * B.Dt / 1e15 + (double)B.Dt * B.Dt * B.Dt / 5e12 + 300e-6;
+    // only wide systems qualify: small ones (NaiveTrain's per-key fits, cold-started every time) are launch-bound, not
+    // flop-bound, and a mid-update rebuild saves them many lock-step slots
+    B.rebuild_is_expensive = (t_rebuild > 8.0 * t_pass && B.Dt > 2048 && !B.matfree) ? 1 : 0;
   }
   // Gram decomposition
   constexpr int MAX_TILES = 1 << 18;   // lower 128x128 tiles of Dp up to ~90k
@@ -415,8 +420,10 @@ int batch_alloc(Batch& B, int num_sms, int hessian_policy, int csr_gram_force = 
   for (int b = 0; b < nprob; b++) {
     pool_off[b] = pool_bytes;
     const bool windows = B.csr_fx && k1_csr_window(ldx) > 0;   // then a second [n] vector (row residuals) follows sdvec
-    // CSR: sdvec (+ rvec), then the e4m3 operand bytes of the entry list (none in a matrix-free batch); else the bf16 operand Xt
-    const size_t need = B.csr_fx ? (((size_t)B.h[b].n * sizeof(float) * (windows ? 2 : 1) + 255) & ~(size_t)255) + (B.matfree ? 0 : (size_t)B.h[b].bm_entries)
+    // CSR: sdvec (+ rvec), then the operand of the entry list (e4m3 bytes or sparse-kernel words; none in a matrix-free batch);
+    // else the bf16 operand Xt
+    const size_t need = B.csr_fx ? (((size_t)B.h[b].n * sizeof(float) * (windows ? 2 : 1) + 255) & ~(size_t)255) +
+                                       (B.matfree ? 0 : (size_t)csr_operand_bytes(B.csr_gram) * (size_t)B.h[b].bm_entries)
                                         : (size_t)B.h[b].n * B.Dp * sizeof(__nv_bfloat16);
     pool_bytes += (need + 255) & ~(size_t)255;
   }
@@ -456,7 +463,9 @@ int batch_alloc(Batch& B, int num_sms, int hessian_policy, int csr_gram_force = 
     if (B.csr_fx) {
       p.sdvec = reinterpret_cast<float*>(pool + pool_off[b]);
       p.rvec = k1_csr_window(ldx) > 0 ? p.sdvec + p.n : nullptr;
-      p.bm_e4m3 = B.matfree ? nullptr : pool + pool_off[b] + (((size_t)p.n * sizeof(float) * (p.rvec ? 2 : 1) + 255) & ~(size_t)255);
+      unsigned char* op = B.matfree ? nullptr : pool + pool_off[b] + (((size_t)p.n * sizeof(float) * (p.rvec ? 2 : 1) + 255) & ~(size_t)255);
+      p.bm_e4m3 = B.csr_gram == CSR_GRAM_SPARSE ? nullptr : op;
+      p.bm_word = B.csr_gram == CSR_GRAM_SPARSE ? reinterpret_cast<uint32_t*>(op) : nullptr;
       p.gram_from_csr = B.gram_from_csr;
       p.csr_gram = B.csr_gram;
       std::memset(&maps[b], 0, sizeof(CUtensorMap));
