@@ -22,9 +22,9 @@
 #include <thread>
 #include <vector>
 
-#include "../../include/mlease_b200.h"
+#include "host.cuh"
 
-extern "C" int mlease_internal_set_error(int code, const char* msg);   // session.cu: writes the thread-local error string
+using mlease::fail;
 
 namespace {
 
@@ -62,7 +62,6 @@ NcclApi* nccl() {
   return &api;
 }
 
-int fail(int code, const std::string& m) { return mlease_internal_set_error(code, m.c_str()); }
 int nccl_ready() {
   NcclApi* a = nccl();
   if (!a->err.empty()) return fail(MLEASE_ERR_CUDA, a->err);
@@ -118,15 +117,14 @@ int mlease_comm_info(const mlease_comm* c, int32_t* rank, int32_t* nranks, int32
   return 0;
 }
 
-// used by session.cu: in-place sum of `count` doubles on `stream`
-int mlease_internal_allreduce(mlease_comm* c, double* buf, size_t count, void* stream) {
+}  // extern "C"
+
+int mlease::comm_allreduce(mlease_comm* c, double* buf, size_t count, cudaStream_t st) {
   if (!c || !c->comm) return fail(MLEASE_ERR_STATE, "no communicator attached");
-  ncclResult_t r = nccl()->AllReduce(buf, buf, count, ncclDouble, ncclSum, c->comm, (cudaStream_t)stream);
+  ncclResult_t r = nccl()->AllReduce(buf, buf, count, ncclDouble, ncclSum, c->comm, st);
   if (r != ncclSuccess) return fail(MLEASE_ERR_CUDA, std::string("ncclAllReduce: ") + nccl()->GetErrorString(r));
   return 0;
 }
-
-}  // extern "C"
 
 // ============================================================================================ mlease_world
 struct mlease_world {

@@ -7,7 +7,11 @@
 // HBM-bound streaming kernels (one read of the test matrix).
 #include <cub/device/device_radix_sort.cuh>
 
-#include "kernels.cuh"
+#include <cmath>
+#include <string>
+#include <vector>
+
+#include "host.cuh"
 
 namespace mlease {
 
@@ -123,10 +127,10 @@ __global__ void __launch_bounds__(256) keyed_table_scatter_kernel(int Dg, int K,
   }
 }
 
-cudaError_t score_keyed_chunk(int Dg, int K, int k0, int k1, long long r0, long long r1, const long long* krs, const long long* rowptr,
-                              const int* colidx, const float* vals, const float* offset, int G, const long long* mp, const int* mc,
-                              const float* mv, const double* term, int binary_feature, long long nrows, float* table, float* pred,
-                              int* d_bad, cudaStream_t st) {
+static cudaError_t score_keyed_chunk(int Dg, int K, int k0, int k1, long long r0, long long r1, const long long* krs, const long long* rowptr,
+                                     const int* colidx, const float* vals, const float* offset, int G, const long long* mp, const int* mc,
+                                     const float* mv, const double* term, int binary_feature, long long nrows, float* table, float* pred,
+                                     int* d_bad, cudaStream_t st) {
   const int LP = G == 1 ? 1 : G == 2 ? 2 : 4;
   const int nk = k1 - k0;
   cudaError_t e = cudaMemsetAsync(table, 0, (size_t)nk * Dg * LP * sizeof(float), st);
@@ -191,10 +195,10 @@ __global__ void __launch_bounds__(256) keyed_loglik_reduce_kernel(long long n, i
   if (lane == 0) { out_ll[k] = (float)(sum / cnt); out_cnt[k] = cnt; }
 }
 
-cudaError_t loglik_keyed_launch(long long n, int nkeys, long long ngroups, const int* key, const int* group, const int* response,
-                                const float* weight, const float* pred, float* d_ll, long long* d_skey, long long* d_skey_sorted,
-                                int* d_idx, int* d_idx_sorted, void* d_tmp, size_t* tmp_bytes, int* d_bad, float* d_out_ll,
-                                double* d_out_cnt, cudaStream_t st) {
+static cudaError_t loglik_keyed_launch(long long n, int nkeys, long long ngroups, const int* key, const int* group, const int* response,
+                                       const float* weight, const float* pred, float* d_ll, long long* d_skey, long long* d_skey_sorted,
+                                       int* d_idx, int* d_idx_sorted, void* d_tmp, size_t* tmp_bytes, int* d_bad, float* d_out_ll,
+                                       double* d_out_cnt, cudaStream_t st) {
   int end_bit = 1;
   while (end_bit < 63 && ((long long)nkeys * ngroups - 1) >> end_bit) end_bit++;
   if (!d_tmp)   // size query
@@ -206,9 +210,9 @@ cudaError_t loglik_keyed_launch(long long n, int nkeys, long long ngroups, const
   return cudaGetLastError();
 }
 
-cudaError_t score_launch(int Dg, long long nrows, const long long* rowptr, const int* colidx, const float* vals, long long ldx,
-                         const float* offset, const double* d_model, double intercept_term, int binary_feature, float* pred,
-                         cudaStream_t st) {
+static cudaError_t score_launch(int Dg, long long nrows, const long long* rowptr, const int* colidx, const float* vals, long long ldx,
+                                const float* offset, const double* d_model, double intercept_term, int binary_feature, float* pred,
+                                cudaStream_t st) {
   if (nrows == 0) return cudaSuccess;
   long long blocks = (nrows + 7) / 8;
   if (blocks > 132 * 16) blocks = 132 * 16;
@@ -216,8 +220,8 @@ cudaError_t score_launch(int Dg, long long nrows, const long long* rowptr, const
   return cudaGetLastError();
 }
 
-cudaError_t loglik_launch(long long nrows, const int* response, const float* pred, const float* weight, long long combiner_block,
-                          float* d_ll, double* d_block_sum, double* d_block_cnt, int* d_bad, cudaStream_t st) {
+static cudaError_t loglik_launch(long long nrows, const int* response, const float* pred, const float* weight, long long combiner_block,
+                                 float* d_ll, double* d_block_sum, double* d_block_cnt, int* d_bad, cudaStream_t st) {
   if (nrows == 0) return cudaSuccess;
   loglik_record_kernel<<<(int)((nrows + 255) / 256), 256, 0, st>>>(nrows, response, pred, weight, d_ll, d_bad);
   const long long nb = (nrows + combiner_block - 1) / combiner_block;
@@ -226,3 +230,205 @@ cudaError_t loglik_launch(long long nrows, const int* response, const float* pre
 }
 
 }  // namespace mlease
+
+using namespace mlease;
+
+extern "C" {
+
+int mlease_score(int32_t device, void* stream, int32_t Dg, int64_t nrows, const int64_t* rowptr, const int32_t* colidx, const float* vals,
+                 int64_t ldx, const float* offset, const double* model, int32_t num_click_replicates, int32_t binary_feature, float* pred) {
+  if (!vals || !model || !pred || nrows < 0) return fail(MLEASE_ERR_INVALID, "bad argument");
+  if (int rc = open_device(device, nullptr)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  DevMem t;
+  const long long* d_rp = nullptr; const int* d_ci = nullptr; const float* d_v = nullptr; const float* d_o = nullptr; const double* d_m = nullptr;
+  long long nnz = nrows * ldx;
+  if (colidx) {
+    if (!rowptr) return fail(MLEASE_ERR_INVALID, "null rowptr");
+    long long last;
+    CK(cudaMemcpy(&last, rowptr + nrows, 8, cudaMemcpyDefault));
+    nnz = last;
+    if (int rc = to_device(t, (const long long*)rowptr, (size_t)nrows + 1, &d_rp, st)) return rc;
+    if (int rc = to_device(t, colidx, (size_t)nnz, &d_ci, st)) return rc;
+  }
+  if (int rc = to_device(t, vals, (size_t)nnz, &d_v, st)) return rc;
+  if (int rc = to_device(t, offset, (size_t)nrows, &d_o, st)) return rc;
+  if (int rc = to_device(t, model, (size_t)Dg + 1, &d_m, st)) return rc;
+  double b;
+  CK(cudaMemcpy(&b, model + Dg, 8, cudaMemcpyDefault));
+  // intercept term  -log(n - 1 + n exp(-b))  (models/LinearModel.java:243-244)
+  const double ic = -std::log((double)num_click_replicates - 1 + (double)num_click_replicates * std::exp(-b));
+  const bool pred_dev = is_device_ptr(pred);
+  float* d_pred = pred;
+  if (!pred_dev) { if (int rc = t.get(&d_pred, (size_t)nrows, false)) return rc; }
+  CK(score_launch(Dg, nrows, d_rp, d_ci, d_v, ldx, d_o, d_m, ic, binary_feature, d_pred, st));
+  if (!pred_dev) CK(cudaMemcpyAsync(pred, d_pred, (size_t)nrows * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return 0;
+}
+
+int mlease_test_loglik(int32_t device, void* stream, int64_t nrows, const int32_t* response, const float* pred, const float* weight,
+                       int64_t combiner_block, float* out_loglik, double* out_count) {
+  if (!response || !pred || !out_loglik || !out_count || nrows <= 0) return fail(MLEASE_ERR_INVALID, "bad argument");
+  if (int rc = open_device(device, nullptr)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  DevMem t;
+  const int* d_r; const float* d_p; const float* d_w;
+  if (int rc = to_device(t, (const int*)response, (size_t)nrows, &d_r, st)) return rc;
+  if (int rc = to_device(t, pred, (size_t)nrows, &d_p, st)) return rc;
+  if (int rc = to_device(t, weight, (size_t)nrows, &d_w, st)) return rc;
+  const bool combine = combiner_block > 0;
+  const long long blk = combine ? combiner_block : 4096;
+  const long long nb = (nrows + blk - 1) / blk;
+  float* d_ll; double *d_bs, *d_bc; int* d_bad;
+  if (int rc = t.get(&d_ll, (size_t)nrows, false)) return rc;
+  if (int rc = t.get(&d_bs, (size_t)nb, false)) return rc;
+  if (int rc = t.get(&d_bc, (size_t)nb, false)) return rc;
+  if (int rc = t.get(&d_bad, 1, false)) return rc;
+  CK(cudaMemsetAsync(d_bad, 0, 4, st));
+  CK(loglik_launch(nrows, d_r, d_p, d_w, blk, d_ll, d_bs, d_bc, d_bad, st));
+  std::vector<double> bs(nb), bc(nb);
+  int bad = 0;
+  CK(cudaMemcpyAsync(bs.data(), d_bs, nb * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(bc.data(), d_bc, nb * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  if (bad) return fail(MLEASE_ERR_INVALID, "response should be 1,0 or -1!");
+  double sum = 0, n = 0;
+  for (long long b = 0; b < nb; b++) {
+    sum += combine ? (double)(float)bs[b] : bs[b];   // combiner casts its partial sum to float (jobs/RegressionTestLoglik.java:197)
+    n += bc[b];
+  }
+  *out_loglik = (float)(sum / n);                    // reducer (:173)
+  *out_count = n;
+  return 0;
+}
+
+// ItemModelTest.  The rows are uploaded once for every lambda.  Keys are taken in chunks whose dense coefficient table fits
+// SCORE_KEYED_TABLE_CAP and a quarter of the free device memory; a chunk's rows are one contiguous range because rows come grouped
+// by key.  A key's table slice (Dg * 16 B) is reused by all its rows from L2 while the rows stream from HBM once per group of
+// four lambdas.
+static constexpr size_t SCORE_KEYED_TABLE_CAP = size_t(1) << 30;
+
+int mlease_score_keyed(int32_t device, void* stream, int32_t Dg, int32_t K, const int64_t* key_rowstart, const int64_t* rowptr,
+                       const int32_t* colidx, const float* vals, const float* offset, int32_t L, const int64_t* model_ptr,
+                       const int32_t* model_col, const float* model_val, int32_t binary_feature, float* pred) {
+  if (Dg <= 0 || K < 0 || L <= 0 || !key_rowstart || !rowptr || !colidx || !vals || !model_ptr || !pred) return fail(MLEASE_ERR_INVALID, "bad argument");
+  if (int rc = open_device(device, nullptr)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  // host copies of the index arrays that decide the chunks and of the models, which are checked and give the intercept terms
+  std::vector<long long> krs((size_t)K + 1);
+  CK(cudaMemcpy(krs.data(), key_rowstart, krs.size() * 8, cudaMemcpyDefault));
+  if (krs[0] != 0) return fail(MLEASE_ERR_INVALID, "key_rowstart[0] must be 0");
+  for (int k = 0; k < K; k++) if (krs[k + 1] < krs[k]) return fail(MLEASE_ERR_INVALID, "key_rowstart must be non-decreasing");
+  const long long nrows = krs[K], M = (long long)L * K;
+  std::vector<long long> mp((size_t)M + 1);
+  CK(cudaMemcpy(mp.data(), model_ptr, mp.size() * 8, cudaMemcpyDefault));
+  if (mp[0] != 0) return fail(MLEASE_ERR_INVALID, "model_ptr[0] must be 0");
+  for (long long m = 0; m < M; m++) if (mp[m + 1] < mp[m]) return fail(MLEASE_ERR_INVALID, "model_ptr must be non-decreasing");
+  const long long nme = mp[M];
+  if (nme > 0 && (!model_col || !model_val)) return fail(MLEASE_ERR_INVALID, "null model_col / model_val");
+  std::vector<int> mc((size_t)nme);
+  std::vector<float> mv((size_t)nme);
+  if (nme > 0) {
+    CK(cudaMemcpy(mc.data(), model_col, (size_t)nme * 4, cudaMemcpyDefault));
+    CK(cudaMemcpy(mv.data(), model_val, (size_t)nme * 4, cudaMemcpyDefault));
+  }
+  // intercept term -log(0 + 1 exp(-b)) of LinearModel.eval with num_click_replicates = 1 (models/LinearModel.java:243-244), b = 0 for
+  // a model without an intercept entry, the empty model included (jobs/ItemModelTest.java:189-197)
+  std::vector<double> term((size_t)M);
+  for (long long m = 0; m < M; m++) {
+    for (long long e = mp[m]; e < mp[m + 1]; e++) {
+      if (mc[e] < 0 || mc[e] > Dg) return fail(MLEASE_ERR_INVALID, "model_col out of range (model " + std::to_string(m) + ")");
+      if (e > mp[m] && mc[e] <= mc[e - 1]) return fail(MLEASE_ERR_INVALID, "model_col must be strictly ascending within a model (model " + std::to_string(m) + ")");
+    }
+    const double b = (mp[m + 1] > mp[m] && mc[mp[m + 1] - 1] == Dg) ? (double)mv[mp[m + 1] - 1] : 0.0;
+    term[m] = -std::log(1.0 - 1 + 1.0 * std::exp(-b));
+  }
+  if (nrows == 0) return 0;
+  DevMem t;
+  const long long *d_rp, *d_krs, *d_mp; const int *d_ci, *d_mc; const float *d_v, *d_o, *d_mv; const double* d_term;
+  long long nnz;
+  CK(cudaMemcpy(&nnz, rowptr + nrows, 8, cudaMemcpyDefault));
+  if (int rc = to_device(t, (const long long*)rowptr, (size_t)nrows + 1, &d_rp, st)) return rc;
+  if (int rc = to_device(t, colidx, (size_t)nnz, &d_ci, st)) return rc;
+  if (int rc = to_device(t, vals, (size_t)nnz, &d_v, st)) return rc;
+  if (int rc = to_device(t, offset, (size_t)nrows, &d_o, st)) return rc;
+  if (int rc = to_device(t, (const long long*)krs.data(), krs.size(), &d_krs, st)) return rc;
+  if (int rc = to_device(t, (const long long*)mp.data(), mp.size(), &d_mp, st)) return rc;
+  if (int rc = to_device(t, (const int*)mc.data(), mc.size(), &d_mc, st)) return rc;
+  if (int rc = to_device(t, (const float*)mv.data(), mv.size(), &d_mv, st)) return rc;
+  if (int rc = to_device(t, (const double*)term.data(), term.size(), &d_term, st)) return rc;
+  const bool pred_dev = is_device_ptr(pred);
+  float* d_pred = pred;
+  if (!pred_dev) { if (int rc = t.get(&d_pred, (size_t)L * nrows, false)) return rc; }
+  int* d_bad;
+  if (int rc = t.get(&d_bad, 1, false)) return rc;
+  CK(cudaMemsetAsync(d_bad, 0, 4, st));
+  size_t free_b = 0, total_b = 0;
+  CK(cudaMemGetInfo(&free_b, &total_b));
+  const size_t key_bytes = (size_t)Dg * (L >= 3 ? 4 : L) * sizeof(float);
+  const long long kpc = std::max<long long>(1, std::min<long long>(K, (long long)(std::min(SCORE_KEYED_TABLE_CAP, free_b / 4) / key_bytes)));
+  float* d_table;
+  if (int rc = t.get(&d_table, (size_t)kpc * key_bytes / sizeof(float), false)) return rc;
+  for (long long k0 = 0; k0 < K; k0 += kpc) {
+    const int k1 = (int)std::min<long long>(K, k0 + kpc);
+    if (krs[k1] == krs[k0]) continue;
+    for (int l0 = 0; l0 < L; l0 += 4)
+      CK(score_keyed_chunk(Dg, K, (int)k0, k1, krs[k0], krs[k1], d_krs, d_rp, d_ci, d_v, d_o, std::min(4, L - l0), d_mp + (size_t)l0 * K,
+                           d_mc, d_mv, d_term + (size_t)l0 * K, binary_feature, nrows, d_table, d_pred + (size_t)l0 * nrows, d_bad, st));
+  }
+  int bad = 0;
+  CK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, st));
+  if (!pred_dev) CK(cudaMemcpyAsync(pred, d_pred, (size_t)L * nrows * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  if (bad) return fail(MLEASE_ERR_INVALID, "colidx out of range [0, num_features)");
+  return 0;
+}
+
+int mlease_test_loglik_keyed(int32_t device, void* stream, int64_t n, const int32_t* entry_key, const int32_t* entry_group,
+                             const int32_t* response, const float* weight, const float* pred, int32_t num_keys, float* out_loglik,
+                             double* out_count) {
+  if (n <= 0 || n > INT32_MAX || num_keys <= 0 || !entry_key || !entry_group || !response || !pred || !out_loglik || !out_count)
+    return fail(MLEASE_ERR_INVALID, "bad argument");
+  if (int rc = open_device(device, nullptr)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  DevMem t;
+  const int *d_k, *d_g, *d_r; const float *d_p, *d_w;
+  if (int rc = to_device(t, (const int*)entry_key, (size_t)n, &d_k, st)) return rc;
+  if (int rc = to_device(t, (const int*)entry_group, (size_t)n, &d_g, st)) return rc;
+  if (int rc = to_device(t, (const int*)response, (size_t)n, &d_r, st)) return rc;
+  if (int rc = to_device(t, pred, (size_t)n, &d_p, st)) return rc;
+  if (int rc = to_device(t, weight, (size_t)n, &d_w, st)) return rc;
+  int last_group = 0;
+  CK(cudaMemcpy(&last_group, entry_group + n - 1, 4, cudaMemcpyDefault));
+  if (last_group < 0) return fail(MLEASE_ERR_INVALID, "entry_group must be non-decreasing and >= 0");
+  const long long ngroups = (long long)last_group + 1;
+  float* d_ll; long long *d_skey, *d_skey_s; int *d_idx, *d_idx_s, *d_bad; float* d_oll; double* d_ocnt; char* d_tmp;
+  size_t tmp_bytes = 0;
+  CK(loglik_keyed_launch(n, num_keys, ngroups, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                         nullptr, &tmp_bytes, nullptr, nullptr, nullptr, st));
+  if (int rc = t.get(&d_ll, (size_t)n, false)) return rc;
+  if (int rc = t.get(&d_skey, (size_t)n, false)) return rc;
+  if (int rc = t.get(&d_skey_s, (size_t)n, false)) return rc;
+  if (int rc = t.get(&d_idx, (size_t)n, false)) return rc;
+  if (int rc = t.get(&d_idx_s, (size_t)n, false)) return rc;
+  if (int rc = t.get(&d_bad, 1, false)) return rc;
+  if (int rc = t.get(&d_oll, (size_t)num_keys, false)) return rc;
+  if (int rc = t.get(&d_ocnt, (size_t)num_keys, false)) return rc;
+  if (int rc = t.get(&d_tmp, tmp_bytes, false)) return rc;
+  CK(cudaMemsetAsync(d_bad, 0, 4, st));
+  CK(loglik_keyed_launch(n, num_keys, ngroups, d_k, d_g, d_r, d_w, d_p, d_ll, d_skey, d_skey_s, d_idx, d_idx_s, d_tmp, &tmp_bytes, d_bad,
+                         d_oll, d_ocnt, st));
+  int bad = 0;
+  CK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(out_loglik, d_oll, (size_t)num_keys * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(out_count, d_ocnt, (size_t)num_keys * 8, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  if (bad & 1) return fail(MLEASE_ERR_INVALID, "response should be 1,0 or -1!");   // jobs/ItemModelTestLoglik.java:74-77
+  if (bad & 2) return fail(MLEASE_ERR_INVALID, "entry_key out of range [0, num_keys)");
+  if (bad & 4) return fail(MLEASE_ERR_INVALID, "entry_group must be non-decreasing and >= 0");
+  return 0;
+}
+
+}  // extern "C"

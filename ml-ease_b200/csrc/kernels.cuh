@@ -91,22 +91,4 @@ cudaError_t postvar_diag(const Problem* d_probs, int nprob, const long long* d_r
 cudaError_t postvar_hessian(const Problem* d_prob, bool csr, int ldh, const double* d_dvec, const double* d_q, int has_bias, cudaStream_t st,
                             int* launches);
 
-// K5 (k5_score.cu)
-cudaError_t score_launch(int Dg, long long nrows, const long long* rowptr, const int* colidx, const float* vals, long long ldx,
-                         const float* offset, const double* d_model, double intercept_term, int binary_feature, float* pred,
-                         cudaStream_t st);
-cudaError_t loglik_launch(long long nrows, const int* response, const float* pred, const float* weight, long long combiner_block,
-                          float* d_ll, double* d_block_sum, double* d_block_cnt, int* d_bad, cudaStream_t st);
-// keys [k0, k1) (rows [r0, r1)) against the G <= 4 lambdas whose models start at mp / term / pred; table holds (k1-k0)*Dg*4 floats
-cudaError_t score_keyed_chunk(int Dg, int K, int k0, int k1, long long r0, long long r1, const long long* krs, const long long* rowptr,
-                              const int* colidx, const float* vals, const float* offset, int G, const long long* mp, const int* mc,
-                              const float* mv, const double* term, int binary_feature, long long nrows, float* table, float* pred,
-                              int* d_bad, cudaStream_t st);
-// d_tmp == nullptr: only sets *tmp_bytes (the sort's scratch)
-cudaError_t loglik_keyed_launch(long long n, int nkeys, long long ngroups, const int* key, const int* group, const int* response,
-                                const float* weight, const float* pred, float* d_ll, long long* d_skey, long long* d_skey_sorted,
-                                int* d_idx, int* d_idx_sorted, void* d_tmp, size_t* tmp_bytes, int* d_bad, float* d_out_ll,
-                                double* d_out_cnt, cudaStream_t st);
-
-// upload helpers (session.cu)
 }  // namespace mlease

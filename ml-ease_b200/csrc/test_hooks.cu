@@ -1,0 +1,187 @@
+// test_hooks.cu -- the mlease_internal_* test hooks: not part of the C ABI (include/mlease_b200.h does not declare them), exported
+// for the tests and tools that drive single kernels of a session's batches.
+#include <cmath>
+#include <cstring>
+#include <vector>
+
+#include "host.cuh"
+
+using namespace mlease;
+
+extern "C" {
+
+// Test hook, not part of the C ABI (include/mlease_b200.h does not declare it): one Hv (mode 1) or Hessian-diagonal (mode 2) pass
+// over the session's ADMM batch -- every (partition, lambda) problem at its own point w[b] and vector v[b] (b = local partition * L
+// + lambda, Dt entries each), through the kernels a matrix-free x-update runs (fused multi-lambda or per-problem).  out[b] = the data
+// term X^T D X v resp. sum_i d_i x_ic^2, without the prior.  The batch's x-update state is consumed: begin() again before iterating.
+int mlease_internal_batch_hv(mlease_session* s, int32_t mode, const double* w, const double* v, double* out) {
+  if (!s || !w || !v || !out || (mode != K1_HV && mode != K1_DIAG)) return fail(MLEASE_ERR_INVALID, "bad argument");
+  if (!s->batch) return fail(MLEASE_ERR_STATE, "mlease_admm_begin was not called");
+  CK(cudaSetDevice(s->cfg.device));
+  Batch& B = *s->batch;
+  if (!(B.csr && B.csr_fx)) return fail(MLEASE_ERR_INVALID, "Hessian-vector passes need CSR rows with strictly increasing column ids");
+  const int nprob = B.nprob, ldx = s->ldx, Dt = s->Dt;
+  std::vector<Ctrl> c(nprob);
+  auto set_ctrl = [&](int skip_clear, int active) -> int {
+    CK(cudaMemcpy(c.data(), B.d_ctrl, (size_t)nprob * sizeof(Ctrl), cudaMemcpyDeviceToHost));
+    for (auto& x : c) { if (skip_clear) x.skip_eval = 0; x.cg_active = active; if (active < 0) { x.cg_active = 0; x.done = 1; } }
+    CK(cudaMemcpy(B.d_ctrl, c.data(), (size_t)nprob * sizeof(Ctrl), cudaMemcpyHostToDevice));
+    return 0;
+  };
+  std::vector<double> wb(ldx, 0.0);
+  for (int b = 0; b < nprob; b++) {
+    std::memcpy(wb.data(), w + (size_t)b * Dt, (size_t)Dt * sizeof(double));
+    CK(cudaMemcpy(B.h[b].beta, wb.data(), (size_t)ldx * sizeof(double), cudaMemcpyHostToDevice));
+  }
+  if (int rc = set_ctrl(1, 0)) return rc;
+  int launches = 0;
+  CK(newton_begin(B.d, nprob, 1e-8, 1, 2, 1, 0, s->stream, &launches));   // beta_t = float(w), every problem running
+  CK(batch_k1(B, 1, s->stream, &launches));                               // sqrt(d) at w
+  CK(cudaStreamSynchronize(s->stream));
+  for (int b = 0; b < nprob; b++)
+    if (int rc = load_hv(B, b, v + (size_t)b * Dt, s->stream)) return rc;
+  CK(batch_k1(B, 0, s->stream, &launches, mode));
+  CK(hv_reduce(B.d, nprob, Dt, 0, s->stream, &launches));
+  CK(cudaStreamSynchronize(s->stream));
+  for (int b = 0; b < nprob; b++) CK(cudaMemcpy(out + (size_t)b * Dt, B.h[b].g_t, (size_t)Dt * sizeof(double), cudaMemcpyDeviceToHost));
+  if (int rc = set_ctrl(0, -1)) return rc;
+  B.mirror.clear();
+  s->cnt.launches += launches;
+  return 0;
+}
+
+// Test hooks of the factored direction of wide systems (ldh > 2048), not part of the C ABI.  Each refuses, before any launch, a
+// batch that has no Ysym (ldh <= 2048, or matrix-free), since the kernels they run dereference it.
+//
+// mlease_internal_factor: the caller's Dt x Dt H (row-major; its lower triangle is read) goes into the scratch problem's Lc of
+// partition pid as chol_prep leaves it (lower triangle, identity on the padding, zero above), then the factorisation the solver
+// runs for its direction: fp64 Cholesky, recursive inverse with TF32 merges, bf16 symmetric packing.  Read back, each if not NULL:
+// Lc (Dt x Dt), Yinv (ldh x ldh, whole) and the raw bits of Ysym (ldh x ldh).  The scratch problem's x-update state is consumed.
+int mlease_internal_factor(mlease_session* s, int32_t pid, const double* H, double* L_out, double* Y_out, uint16_t* ysym_out) {
+  if (!s || !H) return fail(MLEASE_ERR_INVALID, "null argument");
+  if (s->cfg.hessian_policy == 2) return fail(MLEASE_ERR_INVALID, "a matrix-free session forms no factor");
+  if (!cholesky_factored_direction(round_up(s->Dt, 32))) return fail(MLEASE_ERR_INVALID, "only systems wider than 2048 (ldh) use the factored direction");
+  Batch* B;
+  if (int rc = scratch_for(s, pid, &B)) return rc;
+  if (B->matfree) return fail(MLEASE_ERR_INVALID, "a matrix-free session forms no factor");   // (made so by the memory rule)
+  if (!cholesky_factored_direction(B->ldh) || !B->h[0].Ysym) return fail(MLEASE_ERR_INVALID, "only systems wider than 2048 (ldh) use the factored direction");
+  const Problem& p = B->h[0];
+  const int Dt = s->Dt, ldh = B->ldh;
+  const size_t hh = (size_t)ldh * ldh;
+  std::vector<double> lc(hh, 0.0);
+  for (int i = 0; i < ldh; i++)
+    for (int j = 0; j <= i; j++) lc[(size_t)i * ldh + j] = i < Dt ? H[(size_t)i * Dt + j] : (i == j ? 1.0 : 0.0);
+  CK(cudaMemcpy(p.Lc, lc.data(), hh * sizeof(double), cudaMemcpyHostToDevice));
+  Ctrl c; std::memset(&c, 0, sizeof(c)); c.need_hess = 1;
+  CK(cudaMemcpy(B->d_ctrl, &c, sizeof(Ctrl), cudaMemcpyHostToDevice));
+  int launches = 0;
+  CK(cholesky_launch(B->d, 1, ldh, s->stream, &launches, 0, 1, 0));
+  CK(cudaStreamSynchronize(s->stream));
+  CK(cudaMemcpy(&c, B->d_ctrl, sizeof(Ctrl), cudaMemcpyDeviceToHost));
+  if (L_out) {
+    CK(cudaMemcpy(lc.data(), p.Lc, hh * sizeof(double), cudaMemcpyDeviceToHost));
+    for (int i = 0; i < Dt; i++) std::memcpy(L_out + (size_t)i * Dt, &lc[(size_t)i * ldh], (size_t)Dt * sizeof(double));
+  }
+  if (Y_out) CK(cudaMemcpy(Y_out, p.Yinv, hh * sizeof(double), cudaMemcpyDeviceToHost));
+  if (ysym_out) CK(cudaMemcpy(ysym_out, p.Ysym, hh * sizeof(uint16_t), cudaMemcpyDeviceToHost));
+  if (int rc = reset_ctrl(*B)) return rc;
+  s->cnt.launches += launches;
+  if (c.fail) return fail(MLEASE_ERR_NUMERIC, "Hessian not positive definite");
+  return 0;
+}
+
+// mlease_internal_factored_direction: on the ADMM batch (after begin() and at least one iterate()), the two triangular GEMV phases of
+// the direction for the problems with active[b] != 0, each on its q[b] (Dt entries; b = local partition * L + lambda), over the
+// whole problem array with the batch's group_L, exactly as newton_solve launches them.  t_out[b] / dir_out[b] (Dt entries each, if
+// not NULL) receive tf and dir; dir is filled with NaN beforehand, so an inactive problem keeps NaN.  The batch's x-update state
+// is consumed (every problem is left done): begin() again before iterating.
+int mlease_internal_factored_direction(mlease_session* s, const int32_t* active, const float* q, float* t_out, double* dir_out) {
+  if (!s || !active || !q) return fail(MLEASE_ERR_INVALID, "null argument");
+  if (!s->batch || !s->begun || s->iter < 1) return fail(MLEASE_ERR_STATE, "needs the ADMM batch after mlease_admm_begin and one iteration");
+  CK(cudaSetDevice(s->cfg.device));
+  Batch& B = *s->batch;
+  if (B.matfree) return fail(MLEASE_ERR_INVALID, "a matrix-free session forms no factor");
+  if (!cholesky_factored_direction(B.ldh) || !B.h[0].Ysym) return fail(MLEASE_ERR_INVALID, "only systems wider than 2048 (ldh) use the factored direction");
+  const int nprob = B.nprob, ldx = s->ldx, Dt = s->Dt;
+  std::vector<Ctrl> c(nprob);
+  CK(cudaMemcpy(c.data(), B.d_ctrl, (size_t)nprob * sizeof(Ctrl), cudaMemcpyDeviceToHost));
+  for (int b = 0; b < nprob; b++) { c[b].done = active[b] ? 0 : 1; c[b].need_solve = active[b] ? 1 : 0; }
+  CK(cudaMemcpy(B.d_ctrl, c.data(), (size_t)nprob * sizeof(Ctrl), cudaMemcpyHostToDevice));
+  std::vector<float> qt(2 * (size_t)ldx, 0.f);   // qf then tf: qf = float(q) on [0, Dt) and 0 on [Dt, ldx) (as the decide kernel leaves it)
+  const std::vector<double> nan(ldx, std::nan(""));
+  for (int b = 0; b < nprob; b++) {
+    for (int k = 0; k < ldx; k++) { qt[k] = k < Dt ? q[(size_t)b * Dt + k] : 0.f; qt[ldx + k] = k < Dt ? std::nanf("") : 0.f; }
+    CK(cudaMemcpy(B.h[b].qf, qt.data(), 2 * (size_t)ldx * sizeof(float), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(B.h[b].dir, nan.data(), (size_t)ldx * sizeof(double), cudaMemcpyHostToDevice));
+  }
+  CK(newton_gemv_tri(B.d, nprob, B.ldh, B.group_L, s->stream));
+  CK(cudaStreamSynchronize(s->stream));
+  for (int b = 0; b < nprob; b++) {
+    if (t_out) CK(cudaMemcpy(t_out + (size_t)b * Dt, B.h[b].tf, (size_t)Dt * sizeof(float), cudaMemcpyDeviceToHost));
+    if (dir_out) CK(cudaMemcpy(dir_out + (size_t)b * Dt, B.h[b].dir, (size_t)Dt * sizeof(double), cudaMemcpyDeviceToHost));
+  }
+  for (auto& x : c) { x.done = 1; x.need_solve = 0; }
+  CK(cudaMemcpy(B.d_ctrl, c.data(), (size_t)nprob * sizeof(Ctrl), cudaMemcpyHostToDevice));
+  B.mirror.clear();
+  s->cnt.launches += 2;
+  return 0;
+}
+
+// mlease_internal_ysym: the bytes problem b of the ADMM batch streams in its direction (Ctrl::ysym_use, else its own Ysym; ldh x ldh
+// bf16 bits), the index of the problem that owns them, and b's factorisation count (Ctrl::tot_hess).  Reads only.
+int mlease_internal_ysym(mlease_session* s, int32_t b, uint16_t* out, int32_t* owner, int32_t* tot_hess) {
+  if (!s) return fail(MLEASE_ERR_INVALID, "null session");
+  if (!s->batch) return fail(MLEASE_ERR_STATE, "mlease_admm_begin was not called");
+  CK(cudaSetDevice(s->cfg.device));
+  Batch& B = *s->batch;
+  if (b < 0 || b >= B.nprob) return fail(MLEASE_ERR_INVALID, "problem index out of range");
+  if (B.matfree) return fail(MLEASE_ERR_INVALID, "a matrix-free session forms no factor");
+  if (!cholesky_factored_direction(B.ldh) || !B.h[0].Ysym) return fail(MLEASE_ERR_INVALID, "only systems wider than 2048 (ldh) use the factored direction");
+  Ctrl c;
+  CK(cudaMemcpy(&c, B.d_ctrl + b, sizeof(Ctrl), cudaMemcpyDeviceToHost));
+  const void* use = c.ysym_use ? c.ysym_use : (const void*)B.h[b].Ysym;
+  int own = -1;
+  for (int j = 0; j < B.nprob; j++) if ((const void*)B.h[j].Ysym == use) own = j;
+  if (own < 0) return fail(MLEASE_ERR_STATE, "problem's factor pointer matches no problem of the batch");
+  if (out) CK(cudaMemcpy(out, use, (size_t)B.ldh * B.ldh * sizeof(uint16_t), cudaMemcpyDeviceToHost));
+  if (owner) *owner = own;
+  if (tot_hess) *tot_hess = (int32_t)c.tot_hess;
+  return 0;
+}
+
+// mlease_internal_request_refresh: problem b of the ADMM batch refactorises at the start point of its next x-update, as after a
+// slow x-update (Ctrl::refresh_next), whatever the other problems do.  Lets a test make one lambda rebuild on its own.
+int mlease_internal_request_refresh(mlease_session* s, int32_t b) {
+  if (!s) return fail(MLEASE_ERR_INVALID, "null session");
+  if (!s->batch) return fail(MLEASE_ERR_STATE, "mlease_admm_begin was not called");
+  Batch& B = *s->batch;
+  if (b < 0 || b >= B.nprob) return fail(MLEASE_ERR_INVALID, "problem index out of range");
+  CK(cudaSetDevice(s->cfg.device));
+  const int one = 1;
+  CK(cudaMemcpy(&B.d_ctrl[b].refresh_next, &one, sizeof(int), cudaMemcpyHostToDevice));
+  if ((int)B.mirror.size() > b) B.mirror[b].refresh_next = 1;   // the host's prediction of slot 0: a rebuild is due
+  return 0;
+}
+
+// Test hooks, not part of the C ABI: the CSR Gram kernel of the batches allocated from now on -- 0 = picked from the data,
+// CSR_GRAM_WGMMA (1), CSR_GRAM_SPARSE (2).  Must be called before the ADMM batch exists; the one-problem scratch batch (objective,
+// timing) is rebuilt with the new setting on its next use.  The query returns the kind of the ADMM batch and of the scratch batch
+// (0: no such batch, or no CSR Gram).
+int mlease_internal_set_csr_gram(mlease_session* s, int32_t kind) {
+  if (!s || kind < 0 || kind > CSR_GRAM_SPARSE) return fail(MLEASE_ERR_INVALID, "bad argument");
+  if (s->batch) return fail(MLEASE_ERR_STATE, "the CSR Gram kernel is chosen when the ADMM batch is allocated: set it before");
+  s->csr_gram_force = kind;
+  delete s->scratch;
+  s->scratch = nullptr;
+  s->scratch_part = -1;
+  return 0;
+}
+
+int mlease_internal_csr_gram(mlease_session* s, int32_t* batch_kind, int32_t* scratch_kind) {
+  if (!s || !batch_kind || !scratch_kind) return fail(MLEASE_ERR_INVALID, "null argument");
+  *batch_kind = s->batch ? s->batch->csr_gram : 0;
+  *scratch_kind = s->scratch ? s->scratch->csr_gram : 0;
+  return 0;
+}
+
+}  // extern "C"
