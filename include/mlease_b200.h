@@ -240,6 +240,15 @@ int mlease_posterior_variance(mlease_session* s, int32_t partition_id, const dou
  * 100000 unless penalize_intercept (:333-343), prior.mean, has.intercept, data.size.threshold (skipped keys -> skipped[k]=1,
  * model 0, :379-382).  out_model [num_lambdas][num_keys][num_features+1] double, intercept last.  All pointers host-or-device
  * except out_model / skipped (host).  A fit that does not converge -> MLEASE_ERR_NUMERIC ("Model fitting error!", :400-412).
+ *
+ * Inputs larger than the device: when the rows, labels and key boundaries do not fit next to the first chunk's solver state, the
+ * keyed calls (mlease_naive_train, mlease_naive_train_dense, mlease_item_model_train, mlease_score_keyed) stream contiguous key
+ * ranges through the device, the next range's rows copied while the current one is solved.  A key's fit then matches the resident
+ * call's within the run-to-run spread of the CSR kernels (their gradient sums use float atomics); scores are bitwise the same.
+ * In that mode "rows sorted and unique" (which selects the CSR kernels) is decided per key range, not per call, so one key with
+ * unsorted rows changes the kernels of its range only.
+ * Several devices: these four calls may run at the same time from several host threads, one device per thread (keys are
+ * independent; a caller shards them into contiguous ranges, each with its own key_rowstart and rowptr from 0).
  * ------------------------------------------------------------------------------------- */
 int mlease_naive_train(int32_t device, void* stream, int32_t num_keys, int32_t num_features, const int64_t* key_rowstart,
                        const int64_t* rowptr, const int32_t* colidx, const float* vals, int64_t ldx, const int32_t* response,

@@ -173,6 +173,18 @@ void check_csr(cudaStream_t st, long long n, long long nnz, const long long* row
 // n rows of Dg floats, ld_in apart, from host or device into dst with ldx floats a row; column Dg is 1 (has_bias) or 0, like the
 // rest of the padding.
 int upload_dense_rows(float* dst, int ldx, const float* src, long long ld_in, long long n, int Dg, int has_bias, cudaStream_t st);
+// dst[i] = src[i] - base for i in [0, n]: the row pointers of a row range copied out of a larger CSR, made range-local
+void rebase_rowptr(cudaStream_t st, long long n, const long long* src, long long base, long long* dst);
+
+// Keyed calls (keyed_fit.cu, k5_score.cu).  keyed_budget: the device bytes the mode decision and the chunk plan of a keyed call may
+// use, min(free, the test cap of mlease_internal_set_keyed_budget).  keyed_record: the key boundaries of the chunks the call ran and
+// whether it streamed, with the host time the streamed rows took to stage and the time the solve waited for them.
+size_t keyed_budget(size_t free_b);
+void keyed_record(const std::vector<long long>& bounds, bool streamed, double stage_ms, double wait_ms);
+// host copies of rowptr[idx[i]] (host or device rowptr)
+int gather_rowptr(const int64_t* rowptr, const std::vector<long long>& idx, std::vector<long long>& out);
+// whether the CUDA copy engines can read p directly (device, managed or pinned host memory)
+bool is_dma_ptr(const void* p);
 
 }  // namespace mlease
 

@@ -62,6 +62,13 @@ __global__ void check_csr_kernel(long long nnz, const int* colidx, float* vals, 
     if (binary) vals[j] = 1.0f;
   }
 }
+__global__ void gather_i64_kernel(const long long* src, const long long* idx, int n, long long* out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) out[i] = src[idx[i]];
+}
+__global__ void rebase_rowptr_kernel(long long n, const long long* src, long long base, long long* dst) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i <= n; i += (long long)gridDim.x * blockDim.x) dst[i] = src[i] - base;
+}
 __global__ void repack_rows_kernel(float* dst, int ldx, const float* src, long long ld_in, long long rows, int Dg) {
   const long long total = rows * Dg;
   for (long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long long)gridDim.x * blockDim.x) {
@@ -78,6 +85,30 @@ bool is_device_ptr(const void* p) {
   const bool dev = cudaPointerGetAttributes(&a, p) == cudaSuccess && (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged);
   cudaGetLastError();
   return dev;
+}
+
+bool is_dma_ptr(const void* p) {
+  cudaPointerAttributes a;
+  const bool dma = cudaPointerGetAttributes(&a, p) == cudaSuccess &&
+                   (a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged || a.type == cudaMemoryTypeHost);
+  cudaGetLastError();
+  return dma;
+}
+
+int gather_rowptr(const int64_t* rowptr, const std::vector<long long>& idx, std::vector<long long>& out) {
+  out.resize(idx.size());
+  if (!is_device_ptr(rowptr)) {
+    for (size_t i = 0; i < idx.size(); i++) out[i] = rowptr[idx[i]];
+    return 0;
+  }
+  DevMem t;
+  long long *d_idx, *d_out;
+  if (int rc = t.get(&d_idx, idx.size(), false)) return rc;
+  if (int rc = t.get(&d_out, idx.size(), false)) return rc;
+  CK(cudaMemcpy(d_idx, idx.data(), idx.size() * 8, cudaMemcpyHostToDevice));
+  gather_i64_kernel<<<(int)((idx.size() + 255) / 256), 256>>>((const long long*)rowptr, d_idx, (int)idx.size(), d_out);
+  CK(cudaMemcpy(out.data(), d_out, idx.size() * 8, cudaMemcpyDeviceToHost));
+  return 0;
 }
 
 int ingest_labels(cudaStream_t st, long long n, const int32_t* response, const float* weight, const float* offset, signed char* y, float* w,
@@ -105,6 +136,10 @@ void check_csr(cudaStream_t st, long long n, long long nnz, const long long* row
   if (nnz <= 0) return;
   check_csr_kernel<<<(int)std::min<long long>((nnz + 255) / 256, 4096), 256, 0, st>>>(nnz, colidx, vals, Dg, binary, d_flag);
   check_rows_sorted_kernel<<<(int)std::min<long long>((n + 255) / 256, 4096), 256, 0, st>>>(n, rowptr, colidx, d_flag + 1);
+}
+
+void rebase_rowptr(cudaStream_t st, long long n, const long long* src, long long base, long long* dst) {
+  rebase_rowptr_kernel<<<(int)std::min<long long>((n + 256) / 256, 4096), 256, 0, st>>>(n, src, base, dst);
 }
 
 int upload_dense_rows(float* dst, int ldx, const float* src, long long ld_in, long long n, int Dg, int has_bias, cudaStream_t st) {

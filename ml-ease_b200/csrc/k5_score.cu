@@ -81,7 +81,12 @@ __global__ void __launch_bounds__(256) score_keyed_kernel(int Dg, int k0, int k1
                                                           const long long* __restrict__ rowptr, const int* __restrict__ colidx,
                                                           const float* __restrict__ vals, const float* __restrict__ offset,
                                                           const float* __restrict__ table, const double* __restrict__ term, int K, int G,
-                                                          int binary_feature, long long nrows, float* __restrict__ pred, int* __restrict__ bad) {
+                                                          int binary_feature, long long nrows, long long row_base, float* __restrict__ pred,
+                                                          int* __restrict__ bad) {
+  // rowptr, offset and pred hold rows [row_base, ...): a streamed key range indexes its own copy of them
+  rowptr -= row_base;
+  if (offset) offset -= row_base;
+  pred -= row_base;
   const int lane = threadIdx.x & 31;
   const long long wg = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
@@ -129,8 +134,8 @@ __global__ void __launch_bounds__(256) keyed_table_scatter_kernel(int Dg, int K,
 
 static cudaError_t score_keyed_chunk(int Dg, int K, int k0, int k1, long long r0, long long r1, const long long* krs, const long long* rowptr,
                                      const int* colidx, const float* vals, const float* offset, int G, const long long* mp, const int* mc,
-                                     const float* mv, const double* term, int binary_feature, long long nrows, float* table, float* pred,
-                                     int* d_bad, cudaStream_t st) {
+                                     const float* mv, const double* term, int binary_feature, long long nrows, long long row_base, float* table,
+                                     float* pred, int* d_bad, cudaStream_t st) {
   const int LP = G == 1 ? 1 : G == 2 ? 2 : 4;
   const int nk = k1 - k0;
   cudaError_t e = cudaMemsetAsync(table, 0, (size_t)nk * Dg * LP * sizeof(float), st);
@@ -140,9 +145,9 @@ static cudaError_t score_keyed_chunk(int Dg, int K, int k0, int k1, long long r0
   if (r1 > r0) {
     long long blocks = (r1 - r0 + 7) / 8;
     if (blocks > 132 * 16) blocks = 132 * 16;
-    if (LP == 1) score_keyed_kernel<1><<<(int)blocks, 256, 0, st>>>(Dg, k0, k1, r0, r1, krs, rowptr, colidx, vals, offset, table, term, K, G, binary_feature, nrows, pred, d_bad);
-    else if (LP == 2) score_keyed_kernel<2><<<(int)blocks, 256, 0, st>>>(Dg, k0, k1, r0, r1, krs, rowptr, colidx, vals, offset, table, term, K, G, binary_feature, nrows, pred, d_bad);
-    else score_keyed_kernel<4><<<(int)blocks, 256, 0, st>>>(Dg, k0, k1, r0, r1, krs, rowptr, colidx, vals, offset, table, term, K, G, binary_feature, nrows, pred, d_bad);
+    if (LP == 1) score_keyed_kernel<1><<<(int)blocks, 256, 0, st>>>(Dg, k0, k1, r0, r1, krs, rowptr, colidx, vals, offset, table, term, K, G, binary_feature, nrows, row_base, pred, d_bad);
+    else if (LP == 2) score_keyed_kernel<2><<<(int)blocks, 256, 0, st>>>(Dg, k0, k1, r0, r1, krs, rowptr, colidx, vals, offset, table, term, K, G, binary_feature, nrows, row_base, pred, d_bad);
+    else score_keyed_kernel<4><<<(int)blocks, 256, 0, st>>>(Dg, k0, k1, r0, r1, krs, rowptr, colidx, vals, offset, table, term, K, G, binary_feature, nrows, row_base, pred, d_bad);
   }
   return cudaGetLastError();
 }
@@ -229,6 +234,114 @@ static cudaError_t loglik_launch(long long nrows, const int* response, const flo
   return cudaGetLastError();
 }
 
+// ItemModelTest.  The rows are uploaded once for every lambda.  Keys are taken in chunks whose dense coefficient table fits
+// SCORE_KEYED_TABLE_CAP and a quarter of the free device memory; a chunk's rows are one contiguous range because rows come grouped
+// by key.  A key's table slice (Dg * 16 B) is reused by all its rows from L2 while the rows stream from HBM once per group of
+// four lambdas.
+static constexpr size_t SCORE_KEYED_TABLE_CAP = size_t(1) << 30;
+
+// mlease_score_keyed over key ranges whose rows, offsets and pred slice fit a quarter of the budget, next to the models (uploaded
+// once).  The rows of range r+1 are copied on a second stream while range r is scored, and each pred slice goes back as soon as
+// it is done.  A pred is a function of its row and its key's model only, so it is bitwise the resident call's.
+static int score_keyed_streamed(cudaStream_t st, int Dg, int K, const std::vector<long long>& krs, const int64_t* rowptr, const int32_t* colidx,
+                                const float* vals, const float* offset, int L, const std::vector<long long>& mp, const std::vector<int>& mc,
+                                const std::vector<float>& mv, const std::vector<double>& term, int binary_feature, float* pred, size_t budget) {
+  const long long nrows = krs[K];
+  std::vector<long long> off;   // rowptr at the key boundaries
+  if (int rc = gather_rowptr(rowptr, krs, off)) return rc;
+  const size_t key_bytes = (size_t)Dg * (L >= 3 ? 4 : L) * sizeof(float);
+  const long long kpc = std::max<long long>(1, std::min<long long>(K, (long long)(std::min(SCORE_KEYED_TABLE_CAP, budget / 4) / key_bytes)));
+  const size_t cap = budget / 4;
+  std::vector<long long> bounds{0};
+  long long max_rows = 0, max_nnz = 0;
+  for (int k = 0; k < K;) {
+    int e = k;
+    size_t bytes = 0;
+    while (e < K) {
+      const size_t need = (size_t)(krs[e + 1] - krs[e]) * (16 + 4 + 4 * (size_t)L) + (size_t)(off[e + 1] - off[e]) * 8;
+      if (e > k && (bytes + need > cap || e - k >= kpc)) break;
+      bytes += need; e++;
+    }
+    max_rows = std::max(max_rows, krs[e] - krs[k]);
+    max_nnz = std::max(max_nnz, off[e] - off[k]);
+    bounds.push_back(e);
+    k = e;
+  }
+  const int nr = (int)bounds.size() - 1;
+  DevMem t;
+  const long long *d_krs, *d_mp; const int* d_mc; const float* d_mv; const double* d_term;
+  if (int rc = to_device(t, (const long long*)krs.data(), krs.size(), &d_krs, st)) return rc;
+  if (int rc = to_device(t, (const long long*)mp.data(), mp.size(), &d_mp, st)) return rc;
+  if (int rc = to_device(t, (const int*)mc.data(), mc.size(), &d_mc, st)) return rc;
+  if (int rc = to_device(t, (const float*)mv.data(), mv.size(), &d_mv, st)) return rc;
+  if (int rc = to_device(t, (const double*)term.data(), term.size(), &d_term, st)) return rc;
+  long long* rp_raw[2]; int* ci[2]; float* v[2]; float* o[2] = {nullptr, nullptr};
+  for (int b = 0; b < 2; b++) {
+    if (int rc = t.get(&rp_raw[b], (size_t)max_rows + 1, false)) return rc;
+    if (int rc = t.get(&ci[b], (size_t)max_nnz, false)) return rc;
+    if (int rc = t.get(&v[b], (size_t)max_nnz, false)) return rc;
+    if (offset) { if (int rc = t.get(&o[b], (size_t)max_rows, false)) return rc; }
+  }
+  long long* d_rp; float *d_table, *d_pred; int* d_bad;
+  if (int rc = t.get(&d_rp, (size_t)max_rows + 1, false)) return rc;
+  if (int rc = t.get(&d_table, (size_t)kpc * key_bytes / sizeof(float), false)) return rc;
+  if (int rc = t.get(&d_pred, (size_t)L * max_rows, false)) return rc;
+  if (int rc = t.get(&d_bad, 1, false)) return rc;
+  CK(cudaMemsetAsync(d_bad, 0, 4, st));
+  struct Ring {   // the copy stream and its events, released on every return path
+    cudaStream_t cs = nullptr;
+    cudaEvent_t up[2] = {nullptr, nullptr}, done[2] = {nullptr, nullptr}, in = nullptr;
+    ~Ring() {
+      for (int b = 0; b < 2; b++) { if (up[b]) cudaEventDestroy(up[b]); if (done[b]) cudaEventDestroy(done[b]); }
+      if (in) cudaEventDestroy(in);
+      if (cs) cudaStreamDestroy(cs);
+    }
+  } ring;
+  CK(cudaStreamCreateWithFlags(&ring.cs, cudaStreamNonBlocking));
+  for (int b = 0; b < 2; b++) {
+    CK(cudaEventCreateWithFlags(&ring.up[b], cudaEventDisableTiming));
+    CK(cudaEventCreateWithFlags(&ring.done[b], cudaEventDisableTiming));
+  }
+  CK(cudaEventCreateWithFlags(&ring.in, cudaEventDisableTiming));
+  CK(cudaEventRecord(ring.in, st));   // device input may be produced by work the caller queued on st
+  CK(cudaStreamWaitEvent(ring.cs, ring.in, 0));
+  auto upload = [&](int r) -> int {
+    const int b = r & 1;
+    const long long r0 = krs[bounds[r]], n = krs[bounds[r + 1]] - r0, o0 = off[bounds[r]], nz = off[bounds[r + 1]] - o0;
+    if (r >= 2) CK(cudaStreamWaitEvent(ring.cs, ring.done[b], 0));   // range r - 2 is scored: its slot is free
+    CK(cudaMemcpyAsync(rp_raw[b], rowptr + r0, (size_t)(n + 1) * 8, cudaMemcpyDefault, ring.cs));
+    if (nz > 0) {
+      CK(cudaMemcpyAsync(ci[b], colidx + o0, (size_t)nz * 4, cudaMemcpyDefault, ring.cs));
+      CK(cudaMemcpyAsync(v[b], vals + o0, (size_t)nz * 4, cudaMemcpyDefault, ring.cs));
+    }
+    if (offset && n > 0) CK(cudaMemcpyAsync(o[b], offset + r0, (size_t)n * 4, cudaMemcpyDefault, ring.cs));
+    CK(cudaEventRecord(ring.up[b], ring.cs));
+    return 0;
+  };
+  if (int rc = upload(0)) return rc;
+  for (int r = 0; r < nr; r++) {
+    const int b = r & 1, k0 = (int)bounds[r], k1 = (int)bounds[r + 1];
+    const long long r0 = krs[k0], n = krs[k1] - r0;
+    CK(cudaStreamWaitEvent(st, ring.up[b], 0));
+    if (n > 0) {
+      rebase_rowptr(st, n, rp_raw[b], off[k0], d_rp);
+      for (int l0 = 0; l0 < L; l0 += 4)
+        CK(score_keyed_chunk(Dg, K, k0, k1, r0, r0 + n, d_krs, d_rp, ci[b], v[b], o[b], std::min(4, L - l0), d_mp + (size_t)l0 * K, d_mc, d_mv,
+                             d_term + (size_t)l0 * K, binary_feature, n, r0, d_table, d_pred + (size_t)l0 * n, d_bad, st));
+    }
+    CK(cudaEventRecord(ring.done[b], st));
+    if (r + 1 < nr) { if (int rc = upload(r + 1)) return rc; }
+    if (n > 0) CK(cudaMemcpy2DAsync(pred + r0, (size_t)nrows * 4, d_pred, (size_t)n * 4, (size_t)n * 4, L, cudaMemcpyDefault, st));
+  }
+  int bad = 0;
+  CK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  CK(cudaStreamSynchronize(ring.cs));
+  keyed_record(bounds, true, 0, 0);
+  if (bad) return fail(MLEASE_ERR_INVALID, "colidx out of range [0, num_features)");
+  return 0;
+}
+
 }  // namespace mlease
 
 using namespace mlease;
@@ -304,11 +417,6 @@ int mlease_test_loglik(int32_t device, void* stream, int64_t nrows, const int32_
   return 0;
 }
 
-// ItemModelTest.  The rows are uploaded once for every lambda.  Keys are taken in chunks whose dense coefficient table fits
-// SCORE_KEYED_TABLE_CAP and a quarter of the free device memory; a chunk's rows are one contiguous range because rows come grouped
-// by key.  A key's table slice (Dg * 16 B) is reused by all its rows from L2 while the rows stream from HBM once per group of
-// four lambdas.
-static constexpr size_t SCORE_KEYED_TABLE_CAP = size_t(1) << 30;
 
 int mlease_score_keyed(int32_t device, void* stream, int32_t Dg, int32_t K, const int64_t* key_rowstart, const int64_t* rowptr,
                        const int32_t* colidx, const float* vals, const float* offset, int32_t L, const int64_t* model_ptr,
@@ -346,10 +454,28 @@ int mlease_score_keyed(int32_t device, void* stream, int32_t Dg, int32_t K, cons
     term[m] = -std::log(1.0 - 1 + 1.0 * std::exp(-b));
   }
   if (nrows == 0) return 0;
-  DevMem t;
-  const long long *d_rp, *d_krs, *d_mp; const int *d_ci, *d_mc; const float *d_v, *d_o, *d_mv; const double* d_term;
   long long nnz;
   CK(cudaMemcpy(&nnz, rowptr + nrows, 8, cudaMemcpyDefault));
+  const bool pred_dev = is_device_ptr(pred);
+  const size_t key_bytes = (size_t)Dg * (L >= 3 ? 4 : L) * sizeof(float);
+  size_t free_b = 0, total_b = 0;
+  CK(cudaMemGetInfo(&free_b, &total_b));
+  const size_t budget = keyed_budget(free_b);
+  {
+    // resident when the rows, the pred array and the model table fit the budget next to the models; else key ranges stream
+    const size_t models = ((size_t)M + 1) * 8 + (size_t)nme * 8 + (size_t)M * 8 + ((size_t)K + 1) * 8;
+    size_t rows = 0;
+    if (!is_device_ptr(rowptr)) rows += ((size_t)nrows + 1) * 8;
+    if (!is_device_ptr(colidx)) rows += (size_t)nnz * 4;
+    if (!is_device_ptr(vals)) rows += (size_t)nnz * 4;
+    if (offset && !is_device_ptr(offset)) rows += (size_t)nrows * 4;
+    if (!pred_dev) rows += (size_t)L * nrows * 4;
+    const size_t table = std::min(SCORE_KEYED_TABLE_CAP, budget / 4);
+    if (models + rows + table > budget)
+      return score_keyed_streamed(st, Dg, K, krs, rowptr, colidx, vals, offset, L, mp, mc, mv, term, binary_feature, pred, budget);
+  }
+  DevMem t;
+  const long long *d_rp, *d_krs, *d_mp; const int *d_ci, *d_mc; const float *d_v, *d_o, *d_mv; const double* d_term;
   if (int rc = to_device(t, (const long long*)rowptr, (size_t)nrows + 1, &d_rp, st)) return rc;
   if (int rc = to_device(t, colidx, (size_t)nnz, &d_ci, st)) return rc;
   if (int rc = to_device(t, vals, (size_t)nnz, &d_v, st)) return rc;
@@ -359,29 +485,30 @@ int mlease_score_keyed(int32_t device, void* stream, int32_t Dg, int32_t K, cons
   if (int rc = to_device(t, (const int*)mc.data(), mc.size(), &d_mc, st)) return rc;
   if (int rc = to_device(t, (const float*)mv.data(), mv.size(), &d_mv, st)) return rc;
   if (int rc = to_device(t, (const double*)term.data(), term.size(), &d_term, st)) return rc;
-  const bool pred_dev = is_device_ptr(pred);
   float* d_pred = pred;
   if (!pred_dev) { if (int rc = t.get(&d_pred, (size_t)L * nrows, false)) return rc; }
   int* d_bad;
   if (int rc = t.get(&d_bad, 1, false)) return rc;
   CK(cudaMemsetAsync(d_bad, 0, 4, st));
-  size_t free_b = 0, total_b = 0;
   CK(cudaMemGetInfo(&free_b, &total_b));
-  const size_t key_bytes = (size_t)Dg * (L >= 3 ? 4 : L) * sizeof(float);
+  free_b = keyed_budget(free_b);
   const long long kpc = std::max<long long>(1, std::min<long long>(K, (long long)(std::min(SCORE_KEYED_TABLE_CAP, free_b / 4) / key_bytes)));
   float* d_table;
   if (int rc = t.get(&d_table, (size_t)kpc * key_bytes / sizeof(float), false)) return rc;
+  std::vector<long long> bounds{0};
   for (long long k0 = 0; k0 < K; k0 += kpc) {
     const int k1 = (int)std::min<long long>(K, k0 + kpc);
+    bounds.push_back(k1);
     if (krs[k1] == krs[k0]) continue;
     for (int l0 = 0; l0 < L; l0 += 4)
       CK(score_keyed_chunk(Dg, K, (int)k0, k1, krs[k0], krs[k1], d_krs, d_rp, d_ci, d_v, d_o, std::min(4, L - l0), d_mp + (size_t)l0 * K,
-                           d_mc, d_mv, d_term + (size_t)l0 * K, binary_feature, nrows, d_table, d_pred + (size_t)l0 * nrows, d_bad, st));
+                           d_mc, d_mv, d_term + (size_t)l0 * K, binary_feature, nrows, 0, d_table, d_pred + (size_t)l0 * nrows, d_bad, st));
   }
   int bad = 0;
   CK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, st));
   if (!pred_dev) CK(cudaMemcpyAsync(pred, d_pred, (size_t)L * nrows * 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
+  keyed_record(bounds, false, 0, 0);
   if (bad) return fail(MLEASE_ERR_INVALID, "colidx out of range [0, num_features)");
   return 0;
 }

@@ -1,8 +1,10 @@
 // keyed_fit.cu -- K independent fits per prior over one upload of the rows: RegressionNaiveTrain (mlease_naive_train,
 // mlease_naive_train_dense) and ItemModelTrain (mlease_item_model_train).
 #include <algorithm>
+#include <chrono>
 #include <cstring>
 #include <string>
+#include <thread>
 #include <vector>
 
 #include "host.cuh"
@@ -54,23 +56,108 @@ int keyed_fit_check(int32_t device, int32_t Dg, const int64_t* rowptr, const int
   if (!csr && ldx_in < Dg) return fail(MLEASE_ERR_INVALID, "ldx < num_features");
   return open_device(device, num_sms);
 }
-// callers run keyed_fit_check first
-int keyed_fit(int num_sms, cudaStream_t st, int32_t K, int32_t Dg, const int64_t* key_rowstart, const int64_t* rowptr, const int32_t* colidx,
-              const float* vals, int64_t ldx_in, const int32_t* response, const float* weight, const float* offset, bool has_intercept,
-              int32_t data_size_threshold, int32_t binary_feature, const std::vector<KeyedPrior>& priors, const double* intercept_mean,
-              double* out_model, double* out_var, int32_t* skipped) {
-  const bool csr = rowptr != nullptr;
-  const int L = (int)priors.size();
-  const int Dt = Dg + 1, ldx = round_up(Dt, 4);
-  std::vector<long long> krs(K + 1);
+
+// The device arrays the problems of a chunk point into; element 0 of the row arrays is row row0 of the call (0 when resident)
+struct ChunkRows {
+  long long row0 = 0;
+  signed char* y = nullptr; float* w = nullptr; float* o = nullptr;
+  float* X = nullptr;
+  const long long* rp = nullptr; const int* ci = nullptr; float* v = nullptr;   // rp: offsets into ci / v
+  int csr_unique = 0;
+};
+
+// n bytes from src to dst (pageable host to pinned host) by several threads: one memcpy thread does not keep up with the H2D copy
+void parallel_memcpy(void* dst, const void* src, size_t n) {
+  const size_t per = size_t(8) << 20;
+  const size_t hw = std::max(1u, std::min(8u, std::thread::hardware_concurrency()));
+  const int nt = (int)std::min(hw, (n + per - 1) / per);
+  if (nt <= 1) { if (n) std::memcpy(dst, src, n); return; }
+  std::vector<std::thread> ts;
+  const size_t step = (n + nt - 1) / nt;
+  for (int t = 0; t < nt; t++) {
+    const size_t a = std::min(n, t * step), b = std::min(n, a + step);
+    try {
+      ts.emplace_back([=] { std::memcpy((char*)dst + a, (const char*)src + a, b - a); });
+    } catch (const std::exception&) {   // no thread to spare: this slice on the calling thread
+      std::memcpy((char*)dst + a, (const char*)src + a, b - a);
+    }
+  }
+  for (auto& t : ts) t.join();
+}
+
+// One keyed fit call.  Resident mode (the whole upload and the first chunk's state fit the budget): every row is uploaded once,
+// then solved in chunks of keys.  Streamed mode: contiguous key ranges, each holding its own rows next to its solver state within a
+// quarter of the budget; the rows of range c+1 are staged (pageable input through a pinned ring, by several host threads) and
+// copied on a second stream while range c is solved, and each range passes the row checks before any of its rows is read.  Rows
+// sorted and unique (csr_unique) is then a property of the range.  Neither mode changes what a key's fit computes: a streamed range
+// solves exactly as a resident call on that range's keys alone.  The mode and the plan are host arithmetic on the shapes, the CSR
+// offsets at the key boundaries and the free memory, never on the values.
+struct KeyedFit {
+  int num_sms; cudaStream_t st; int32_t K, Dg; const int64_t* key_rowstart; const int64_t* rowptr; const int32_t* colidx; const float* vals;
+  int64_t ldx_in; const int32_t* response; const float* weight; const float* offset; bool has_intercept; int32_t data_size_threshold;
+  int32_t binary_feature; const std::vector<KeyedPrior>& priors; const double* intercept_mean; double* out_model; double* out_var;
+  int32_t* skipped;
+  bool csr = false;
+  int L = 0, Dt = 0, ldx = 0, Dp = 0, ldh = 0;
+  std::vector<long long> krs, key_nnz0;   // key_nnz0: CSR rowptr at the key boundaries
+  std::vector<int> todo;                  // the keys that are fitted
+  Counters cnt;
+
+  bool solves(int k) const { const long long nk = krs[k + 1] - krs[k]; return !(nk < data_size_threshold || nk <= 0); }   // (:379-382)
+  // device bytes of a fitted key of n rows: Xt (n*Dp*2) + Hpart + Lc per problem (+ the row weights of the variance)
+  size_t state_bytes(long long n) const {
+    return (size_t)n * Dp * 2 + (size_t)Dp * Dp * 4 + 3 * (size_t)ldh * ldh * 8 + 2 * (size_t)ldh * 32 * 8 + 64 * (size_t)ldx +
+           (out_var ? (size_t)n * 8 : 0);
+  }
+  void init_outputs() {
+    for (size_t e = 0; e < (size_t)L * K * Dt; e++) out_model[e] = 0.0;
+    if (skipped) for (int k = 0; k < K; k++) skipped[k] = solves(k) ? 0 : 1;   // "data size < threshold": no model
+    if (out_var)   // a key without rows has no fit: every variance is the prior's
+      for (int l = 0; l < L; l++)
+        for (int k = 0; k < K; k++)
+          for (int j = 0; j < Dt; j++) out_var[((size_t)l * K + k) * Dt + j] = 1.0 / priors[l].q[j];
+  }
+  int finish(const std::vector<long long>& bounds, bool streamed, double stage_ms, double wait_ms) {
+    keyed_record(bounds, streamed, stage_ms, wait_ms);
+    if (cnt.not_converged) return fail(MLEASE_ERR_NUMERIC, "Model fitting error! (" + std::to_string(cnt.not_converged) + " fits did not converge)");
+    return 0;
+  }
+  int run();
+  int resident();
+  int streamed(size_t budget);
+  int solve_chunk(const int* keys, int nprob, const ChunkRows& cr, int* dflag, int* hflag);
+};
+
+int KeyedFit::run() {
+  csr = rowptr != nullptr;
+  L = (int)priors.size();
+  Dt = Dg + 1; ldx = round_up(Dt, 4); Dp = round_up(ldx, 128); ldh = round_up(Dt, 32);
+  krs.resize(K + 1);
   CK(cudaMemcpy(krs.data(), key_rowstart, (size_t)(K + 1) * 8, cudaMemcpyDefault));
   const long long ntot = krs[K];
   for (int k = 0; k < K; k++) if (krs[k + 1] < krs[k]) return fail(MLEASE_ERR_INVALID, "key_rowstart must be non-decreasing");
+  for (int k = 0; k < K; k++) if (solves(k)) todo.push_back(k);
+  // the bytes of the resident upload (rows, labels, key boundaries, the temporaries of host input) and of the first chunk's state
+  size_t free_b, total_b;
+  CK(cudaMemGetInfo(&free_b, &total_b));
+  const size_t budget = keyed_budget(free_b);
+  long long nnz = 0;
+  if (csr) CK(cudaMemcpy(&nnz, rowptr + ntot, 8, cudaMemcpyDefault));
+  const bool host_rows = !is_device_ptr(csr ? (const void*)colidx : (const void*)vals);
+  size_t up = (size_t)ntot * 9 + (is_device_ptr(response) ? 0 : (size_t)ntot * 12);
+  if (csr) up += (size_t)nnz * 4 + (host_rows ? (size_t)nnz * 4 + (size_t)(ntot + 1) * 8 : 0) + (size_t)(K + 1) * 16;
+  else up += (size_t)ntot * ldx * 4 + (host_rows ? (size_t)256 << 20 : 0);
+  const size_t first = todo.empty() ? 0 : state_bytes(krs[todo[0] + 1] - krs[todo[0]]);
+  return up + first <= budget ? resident() : streamed(budget);
+}
+
+int KeyedFit::resident() {
+  const long long ntot = krs[K];
   DevMem t;
   PinnedMem pinned;
   float* dX = nullptr; signed char* dy; float *dw, *dofs; int* dflag; int* hflag;
   const long long* d_rp = nullptr; const int* d_ci = nullptr; float* d_v = nullptr;
-  std::vector<long long> key_nnz0(K + 1, 0);   // CSR: rowptr at the key boundaries
+  key_nnz0.assign(K + 1, 0);
   int csr_unique = 0;
   if (int rc = t.get(&dy, (size_t)ntot, false)) return rc;
   if (int rc = t.get(&dw, (size_t)ntot, false)) return rc;
@@ -106,111 +193,269 @@ int keyed_fit(int num_sms, cudaStream_t st, int32_t K, int32_t Dg, const int64_t
     csr_unique = hflag[1] ? 0 : 1;
   }
   if (int rc = ingest_labels(st, ntot, response, weight, offset, dy, dw, dofs, dflag, hflag, nullptr)) return rc;
-  for (size_t e = 0; e < (size_t)L * K * Dt; e++) out_model[e] = 0.0;
-  std::vector<int> todo;
-  for (int k = 0; k < K; k++) {
-    const long long nk = krs[k + 1] - krs[k];
-    if (skipped) skipped[k] = 0;
-    if (nk < data_size_threshold || nk <= 0) { if (skipped) skipped[k] = 1; }   // "data size < threshold": no model (:379-382)
-    else todo.push_back(k);
-  }
-  if (out_var)   // a key without rows has no fit: every variance is the prior's
-    for (int l = 0; l < L; l++)
-      for (int k = 0; k < K; k++)
-        for (int j = 0; j < Dt; j++) out_var[((size_t)l * K + k) * Dt + j] = 1.0 / priors[l].q[j];
-  // chunk size bounded by memory: Xt (n*Dp*2) + Hpart + Lc per problem (+ the row weights of the variance)
-  const int Dp = round_up(ldx, 128), ldh = round_up(Dt, 32);
+  init_outputs();
+  ChunkRows cr;
+  cr.y = dy; cr.w = dw; cr.o = dofs; cr.X = dX; cr.rp = d_rp; cr.ci = d_ci; cr.v = d_v; cr.csr_unique = csr_unique;
+  // chunk size bounded by memory
   size_t free_b, total_b;
   CK(cudaMemGetInfo(&free_b, &total_b));
-  Counters cnt;
+  free_b = keyed_budget(free_b);
+  std::vector<long long> bounds{0};
   size_t pos = 0;
   while (pos < todo.size()) {
     size_t bytes = 0;
     size_t end = pos;
     while (end < todo.size() && end - pos < 16384) {
-      const long long nk = krs[todo[end] + 1] - krs[todo[end]];
-      const size_t need = (size_t)nk * Dp * 2 + (size_t)Dp * Dp * 4 + 3 * (size_t)ldh * ldh * 8 + 2 * (size_t)ldh * 32 * 8 + 64 * (size_t)ldx +
-                          (out_var ? (size_t)nk * 8 : 0);
+      const size_t need = state_bytes(krs[todo[end] + 1] - krs[todo[end]]);
       if (end > pos && bytes + need > free_b / 2) break;
       bytes += need;
       end++;
     }
-    Batch B;
-    B.nprob = (int)(end - pos); B.Dt = Dt; B.ldx = ldx; B.csr = csr; B.has_bias = has_intercept ? 1 : 0;
-    B.h.resize(B.nprob);
-    std::vector<long long> row_start(B.nprob + 1, 0);   // the chunk's rows numbered across its problems (batched variance)
-    for (int b = 0; b < B.nprob; b++) {
-      const int k = todo[pos + b];
-      Problem& p = B.h[b];
-      std::memset(&p, 0, sizeof(Problem));
-      p.n = krs[k + 1] - krs[k];
-      p.y = dy + krs[k]; p.w = dw + krs[k]; p.o = dofs + krs[k];
-      if (csr) {
-        // a key = a row range of the one CSR: the row pointers keep their absolute offsets into colidx / vals
-        p.rowptr = d_rp + krs[k]; p.colidx = d_ci; p.vals = d_v; p.nnz_hint = key_nnz0[k + 1] - key_nnz0[k]; p.csr_unique = csr_unique;
-      } else {
-        p.X = dX + (size_t)krs[k] * ldx;
-      }
-      row_start[b + 1] = row_start[b] + p.n;
+    if (int rc = solve_chunk(todo.data() + pos, (int)(end - pos), cr, dflag, hflag)) return rc;
+    bounds.push_back(end < todo.size() ? todo[end] : K);
+    pos = end;
+  }
+  if (bounds.back() != K) bounds.push_back(K);
+  return finish(bounds, false, 0, 0);
+}
+
+// the problems keys[0, nprob) over the rows of cr, every prior, into out_model / out_var
+int KeyedFit::solve_chunk(const int* keys, int nprob, const ChunkRows& cr, int* dflag, int* hflag) {
+  Batch B;
+  B.nprob = nprob; B.Dt = Dt; B.ldx = ldx; B.csr = csr; B.has_bias = has_intercept ? 1 : 0;
+  B.h.resize(B.nprob);
+  std::vector<long long> row_start(B.nprob + 1, 0);   // the chunk's rows numbered across its problems (batched variance)
+  for (int b = 0; b < B.nprob; b++) {
+    const int k = keys[b];
+    const long long r = krs[k] - cr.row0;
+    Problem& p = B.h[b];
+    std::memset(&p, 0, sizeof(Problem));
+    p.n = krs[k + 1] - krs[k];
+    p.y = cr.y + r; p.w = cr.w + r; p.o = cr.o + r;
+    if (csr) {
+      // a key = a row range of the CSR: the row pointers keep their offsets into colidx / vals
+      p.rowptr = cr.rp + r; p.colidx = cr.ci; p.vals = cr.v; p.nnz_hint = key_nnz0[k + 1] - key_nnz0[k]; p.csr_unique = cr.csr_unique;
+    } else {
+      p.X = cr.X + (size_t)r * ldx;
     }
-    if (int rc = batch_alloc(B, num_sms, 0)) return rc;
-    DevMem ct;   // the chunk's temporaries: freed with the chunk, before the next chunk's batch_alloc
-    double *dm, *dq, *dout, *dim = nullptr, *dvec = nullptr; long long* drs = nullptr; unsigned char* dmask = nullptr;
-    if (int rc = ct.get(&dm, (size_t)ldx, false)) return rc;
-    if (int rc = ct.get(&dq, (size_t)ldx, false)) return rc;
-    if (int rc = ct.get(&dout, (size_t)B.nprob * Dt, false)) return rc;
-    if (intercept_mean) {
-      std::vector<double> im(B.nprob);
-      for (int b = 0; b < B.nprob; b++) im[b] = intercept_mean[todo[pos + b]];
-      if (int rc = ct.get(&dim, (size_t)B.nprob, false)) return rc;
-      CK(cudaMemcpyAsync(dim, im.data(), im.size() * 8, cudaMemcpyHostToDevice, st));
-      CK(cudaStreamSynchronize(st));   // im is released here
+    row_start[b + 1] = row_start[b] + p.n;
+  }
+  if (int rc = batch_alloc(B, num_sms, 0)) return rc;
+  DevMem ct;   // the chunk's temporaries: freed with the chunk, before the next chunk's batch_alloc
+  double *dm, *dq, *dout, *dim = nullptr, *dvec = nullptr; long long* drs = nullptr; unsigned char* dmask = nullptr;
+  if (int rc = ct.get(&dm, (size_t)ldx, false)) return rc;
+  if (int rc = ct.get(&dq, (size_t)ldx, false)) return rc;
+  if (int rc = ct.get(&dout, (size_t)B.nprob * Dt, false)) return rc;
+  if (intercept_mean) {
+    std::vector<double> im(B.nprob);
+    for (int b = 0; b < B.nprob; b++) im[b] = intercept_mean[keys[b]];
+    if (int rc = ct.get(&dim, (size_t)B.nprob, false)) return rc;
+    CK(cudaMemcpyAsync(dim, im.data(), im.size() * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaStreamSynchronize(st));   // im is released here
+  }
+  if (out_var) {
+    if (int rc = ct.get(&dvec, (size_t)row_start[B.nprob], false)) return rc;
+    if (int rc = ct.get(&drs, row_start.size(), false)) return rc;
+    CK(cudaMemcpyAsync(drs, row_start.data(), row_start.size() * 8, cudaMemcpyHostToDevice, st));
+  }
+  if (csr) {
+    // features absent from a key's rows are not part of its dataset, hence not of its model (llf/LibLinear.java:343-350; the only
+    // prior mean a caller may set per key is the intercept's, which every dataset holds, so :374-383 adds nothing): mask them out
+    if (int rc = ct.get(&dmask, (size_t)B.nprob * Dt, false)) return rc;
+    CK(cudaMemsetAsync(dmask, 0, (size_t)B.nprob * Dt, st));
+    naive_present_kernel<<<B.nprob, 256, 0, st>>>(B.d, Dt, has_intercept ? 1 : 0, dmask);
+  }
+  std::vector<double> xs((size_t)B.nprob * Dt);
+  for (int l = 0; l < L; l++) {
+    CK(cudaMemcpyAsync(dm, priors[l].m.data(), ldx * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(dq, priors[l].q.data(), ldx * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaStreamSynchronize(st));   // dq / dm are reused by the next prior
+    naive_init_kernel<<<B.nprob, 128, 0, st>>>(B.d, dm, dq, dim);
+    B.mirror.clear();                // the factors of the previous prior belong to another prior
+    if (int rc = batch_xupdate(B, st, 2e-7, 100, 0, 1, hflag, dflag, cnt)) return rc;
+    gather_beta_kernel<<<B.nprob, 128, 0, st>>>(B.d, Dt, dout, dmask, 0);
+    CK(cudaMemcpyAsync(xs.data(), dout, xs.size() * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    for (int b = 0; b < B.nprob; b++) {
+      double* dst = out_model + ((size_t)l * K + keys[b]) * Dt;
+      std::memcpy(dst, xs.data() + (size_t)b * Dt, Dt * 8);
+      if (!has_intercept) dst[Dg] = 0.0;
     }
     if (out_var) {
-      if (int rc = ct.get(&dvec, (size_t)row_start[B.nprob], false)) return rc;
-      if (int rc = ct.get(&drs, row_start.size(), false)) return rc;
-      CK(cudaMemcpyAsync(drs, row_start.data(), row_start.size() * 8, cudaMemcpyHostToDevice, st));
-    }
-    if (csr) {
-      // features absent from a key's rows are not part of its dataset, hence not of its model (llf/LibLinear.java:343-350; the only
-      // prior mean a caller may set per key is the intercept's, which every dataset holds, so :374-383 adds nothing): mask them out
-      if (int rc = ct.get(&dmask, (size_t)B.nprob * Dt, false)) return rc;
-      CK(cudaMemsetAsync(dmask, 0, (size_t)B.nprob * Dt, st));
-      naive_present_kernel<<<B.nprob, 256, 0, st>>>(B.d, Dt, has_intercept ? 1 : 0, dmask);
-    }
-    std::vector<double> xs((size_t)B.nprob * Dt);
-    for (int l = 0; l < L; l++) {
-      CK(cudaMemcpyAsync(dm, priors[l].m.data(), ldx * 8, cudaMemcpyHostToDevice, st));
-      CK(cudaMemcpyAsync(dq, priors[l].q.data(), ldx * 8, cudaMemcpyHostToDevice, st));
-      CK(cudaStreamSynchronize(st));   // dq / dm are reused by the next prior
-      naive_init_kernel<<<B.nprob, 128, 0, st>>>(B.d, dm, dq, dim);
-      B.mirror.clear();                // the factors of the previous prior belong to another prior
-      if (int rc = batch_xupdate(B, st, 2e-7, 100, 0, 1, hflag, dflag, cnt)) return rc;
-      gather_beta_kernel<<<B.nprob, 128, 0, st>>>(B.d, Dt, dout, dmask, 0);
+      // posteriorVar, diagonal (llf/LibLinear.java:328-333): one pass over the chunk's rows for all of its keys
+      CK(postvar_rowweights(B.d, B.nprob, drs, row_start[B.nprob], B.has_bias, dvec, st, nullptr));
+      CK(postvar_diag(B.d, B.nprob, drs, row_start[B.nprob], dvec, B.has_bias, st, nullptr));
+      gather_beta_kernel<<<B.nprob, 128, 0, st>>>(B.d, Dt, dout, nullptr, 1);
       CK(cudaMemcpyAsync(xs.data(), dout, xs.size() * 8, cudaMemcpyDeviceToHost, st));
       CK(cudaStreamSynchronize(st));
       for (int b = 0; b < B.nprob; b++) {
-        double* dst = out_model + ((size_t)l * K + todo[pos + b]) * Dt;
-        std::memcpy(dst, xs.data() + (size_t)b * Dt, Dt * 8);
-        if (!has_intercept) dst[Dg] = 0.0;
-      }
-      if (out_var) {
-        // posteriorVar, diagonal (llf/LibLinear.java:328-333): one pass over the chunk's rows for all of its keys
-        CK(postvar_rowweights(B.d, B.nprob, drs, row_start[B.nprob], B.has_bias, dvec, st, nullptr));
-        CK(postvar_diag(B.d, B.nprob, drs, row_start[B.nprob], dvec, B.has_bias, st, nullptr));
-        gather_beta_kernel<<<B.nprob, 128, 0, st>>>(B.d, Dt, dout, nullptr, 1);
-        CK(cudaMemcpyAsync(xs.data(), dout, xs.size() * 8, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-        for (int b = 0; b < B.nprob; b++) {
-          double* dst = out_var + ((size_t)l * K + todo[pos + b]) * Dt;
-          for (int j = 0; j < Dt; j++) dst[j] = 1.0 / xs[(size_t)b * Dt + j];
-        }
+        double* dst = out_var + ((size_t)l * K + keys[b]) * Dt;
+        for (int j = 0; j < Dt; j++) dst[j] = 1.0 / xs[(size_t)b * Dt + j];
       }
     }
-    pos = end;
   }
-  if (cnt.not_converged) return fail(MLEASE_ERR_NUMERIC, "Model fitting error! (" + std::to_string(cnt.not_converged) + " fits did not converge)");
   return 0;
+}
+
+int KeyedFit::streamed(size_t budget) {
+  if (csr) {
+    // rowptr at the key boundaries and at row 0, read without uploading the rows
+    std::vector<long long> idx(krs);
+    idx.push_back(0);
+    if (int rc = gather_rowptr(rowptr, idx, key_nnz0)) return rc;
+    if (key_nnz0.back() != 0) return fail(MLEASE_ERR_INVALID, "rowptr[0] must be 0");
+    key_nnz0.pop_back();
+  }
+  // the plan: contiguous key ranges whose rows (staged copy + the solver's layout) and fitted keys' state fit a quarter of the budget
+  auto row_bytes = [&](int k) -> size_t {
+    const size_t n = (size_t)(krs[k + 1] - krs[k]);
+    size_t b = n * (12 + 9);
+    b += csr ? n * 16 + (size_t)(key_nnz0[k + 1] - key_nnz0[k]) * 8 : n * ((size_t)ldx_in + ldx) * 4;
+    return b;
+  };
+  const size_t cap = budget / 4;
+  std::vector<long long> bounds{0};
+  long long max_rows = 0, max_nnz = 0;
+  for (int k = 0; k < K;) {
+    int e = k, fitted = 0;
+    size_t bytes = 0;
+    while (e < K) {
+      const size_t need = row_bytes(e) + (solves(e) ? state_bytes(krs[e + 1] - krs[e]) : 0);
+      if (e > k && (bytes + need > cap || (solves(e) && fitted >= 16384))) break;
+      bytes += need; fitted += solves(e) ? 1 : 0; e++;
+    }
+    max_rows = std::max(max_rows, krs[e] - krs[k]);
+    if (csr) max_nnz = std::max(max_nnz, key_nnz0[e] - key_nnz0[k]);
+    bounds.push_back(e);
+    k = e;
+  }
+  const int nch = (int)bounds.size() - 1;
+  // the ring: two staged ranges on the device (+ pinned host copies of pageable input), one solver layout
+  struct Src { const void* p; size_t esize; size_t per_row; bool per_nnz; bool dma; void* dev[2]; void* host[2]; };
+  std::vector<Src> srcs;
+  auto add = [&](const void* p, size_t esize, size_t per_row, bool per_nnz) {
+    if (p) srcs.push_back(Src{p, esize, per_row, per_nnz, is_dma_ptr(p), {nullptr, nullptr}, {nullptr, nullptr}});
+  };
+  if (csr) { add(rowptr, 8, 1, false); add(colidx, 4, 0, true); add(vals, 4, 0, true); }
+  else add(vals, 4, (size_t)ldx_in, false);
+  add(response, 4, 1, false); add(weight, 4, 1, false); add(offset, 4, 1, false);
+  DevMem t;
+  PinnedMem pinned;
+  for (auto& s : srcs) {
+    const size_t count = s.per_nnz ? (size_t)max_nnz : (size_t)max_rows * s.per_row + (s.esize == 8 ? 1 : 0);
+    for (int b = 0; b < 2; b++) {
+      char* d; if (int rc = t.get(&d, count * s.esize, false)) return rc;
+      s.dev[b] = d;
+      if (!s.dma) { char* h; if (int rc = pinned.get(&h, count * s.esize, false)) return rc; s.host[b] = h; }
+    }
+  }
+  signed char* dy; float *dw, *dofs; int* dflag; int* hflag; float* dX = nullptr; long long* d_rp = nullptr;
+  if (int rc = t.get(&dy, (size_t)max_rows, false)) return rc;
+  if (int rc = t.get(&dw, (size_t)max_rows, false)) return rc;
+  if (int rc = t.get(&dofs, (size_t)max_rows, false)) return rc;
+  if (int rc = t.get(&dflag, 16, false)) return rc;
+  if (int rc = pinned.get(&hflag, 16, false)) return rc;
+  if (csr) { if (int rc = t.get(&d_rp, (size_t)max_rows + 1, false)) return rc; }
+  else { if (int rc = t.get(&dX, (size_t)max_rows * ldx, false)) return rc; }
+  struct Ring {   // the copy stream and its events, released on every return path
+    cudaStream_t cs = nullptr;
+    cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};   // slot 0 / 1 staged; [2]: what the caller queued on st before the call
+    ~Ring() { for (auto e : ev) if (e) cudaEventDestroy(e); if (cs) cudaStreamDestroy(cs); }
+  } ring;
+  CK(cudaStreamCreateWithFlags(&ring.cs, cudaStreamNonBlocking));
+  for (auto& e : ring.ev) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  CK(cudaEventRecord(ring.ev[2], st));   // device input may be produced by work the caller queued on st
+  int device = 0;
+  CK(cudaGetDevice(&device));
+  // stage range c into ring slot c & 1, on its own host thread: it returns once the rows are on the device
+  auto stage = [&](int c) -> cudaError_t {
+    cudaError_t e = cudaSetDevice(device);
+    if (e == cudaSuccess) e = cudaStreamWaitEvent(ring.cs, ring.ev[2], 0);
+    const int b = c & 1;
+    const long long r0 = krs[bounds[c]], r1 = krs[bounds[c + 1]], n = r1 - r0;
+    for (auto& s : srcs) {
+      if (e != cudaSuccess) break;
+      size_t first, count;
+      if (s.per_nnz) { first = (size_t)key_nnz0[bounds[c]]; count = (size_t)(key_nnz0[bounds[c + 1]] - key_nnz0[bounds[c]]); }
+      else if (s.esize == 8) { first = (size_t)r0; count = (size_t)n + 1; }   // rowptr: n + 1 entries
+      else if (s.per_row > 1) { first = (size_t)r0 * s.per_row; count = n > 0 ? (size_t)(n - 1) * s.per_row + Dg : 0; }   // dense rows
+      else { first = (size_t)r0; count = (size_t)n; }
+      const char* src = (const char*)s.p + first * s.esize;
+      const size_t bytes = count * s.esize;
+      if (!bytes) continue;
+      if (s.dma) { e = cudaMemcpyAsync(s.dev[b], src, bytes, cudaMemcpyDefault, ring.cs); continue; }
+      parallel_memcpy(s.host[b], src, bytes);
+      e = cudaMemcpyAsync(s.dev[b], s.host[b], bytes, cudaMemcpyHostToDevice, ring.cs);
+    }
+    if (e == cudaSuccess) e = cudaEventRecord(ring.ev[b], ring.cs);
+    if (e == cudaSuccess) e = cudaEventSynchronize(ring.ev[b]);
+    return e;
+  };
+  // what the stager thread writes outlives it: declared before the guard that joins it on every return path
+  cudaError_t stage_err = cudaSuccess;
+  double stage_ms = 0, wait_ms = 0;
+  std::thread stager;
+  struct Join { std::thread& t; ~Join() { if (t.joinable()) t.join(); } } join{stager};
+  using clk = std::chrono::steady_clock;
+  auto start = [&](int c) -> int {
+    try {
+      stager = std::thread([&, c] {
+        const auto t0 = clk::now();
+        stage_err = stage(c);
+        stage_ms += std::chrono::duration<double, std::milli>(clk::now() - t0).count();
+      });
+    } catch (const std::exception& e) {   // no exception leaves the C ABI
+      return fail(MLEASE_ERR_CUDA, std::string("cannot start the staging thread: ") + e.what());
+    }
+    return 0;
+  };
+  init_outputs();
+  if (int rc = start(0)) return rc;
+  for (int c = 0; c < nch; c++) {
+    const auto t0 = clk::now();
+    stager.join();
+    wait_ms += std::chrono::duration<double, std::milli>(clk::now() - t0).count();
+    if (stage_err != cudaSuccess) return fail(MLEASE_ERR_CUDA, std::string("staging the rows of a key range: ") + cudaGetErrorString(stage_err));
+    const int b = c & 1;
+    const long long r0 = krs[bounds[c]], n = krs[bounds[c + 1]] - r0;
+    auto slot = [&](const void* p) -> void* { for (auto& s : srcs) if (s.p == p) return s.dev[b]; return nullptr; };
+    ChunkRows cr;
+    cr.row0 = r0; cr.y = dy; cr.w = dw; cr.o = dofs;
+    // the range's checks, before any kernel reads its rows
+    if (csr) {
+      const long long nnz = key_nnz0[bounds[c + 1]] - key_nnz0[bounds[c]];
+      rebase_rowptr(st, n, (const long long*)slot(rowptr), key_nnz0[bounds[c]], d_rp);
+      cr.rp = d_rp; cr.ci = (const int*)slot(colidx); cr.v = (float*)slot(vals);
+      CK(cudaMemsetAsync(dflag, 0, 8, st));
+      check_csr(st, n, nnz, cr.rp, cr.ci, cr.v, Dg, binary_feature, dflag);
+      CK(cudaMemcpyAsync(hflag, dflag, 8, cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
+      if (hflag[0]) return fail(MLEASE_ERR_INVALID, "feature index out of range");
+      cr.csr_unique = hflag[1] ? 0 : 1;
+    } else {
+      if (int rc = upload_dense_rows(dX, ldx, (const float*)slot(vals), ldx_in, n, Dg, has_intercept ? 1 : 0, st)) return rc;
+      cr.X = dX;
+    }
+    if (int rc = ingest_labels(st, n, (const int32_t*)slot(response), (const float*)slot(weight), (const float*)slot(offset), dy, dw, dofs,
+                               dflag, hflag, nullptr))
+      return rc;
+    if (c + 1 < nch) { if (int rc = start(c + 1)) return rc; }
+    std::vector<int> keys;
+    for (long long k = bounds[c]; k < bounds[c + 1]; k++) if (solves((int)k)) keys.push_back((int)k);
+    if (!keys.empty())
+      if (int rc = solve_chunk(keys.data(), (int)keys.size(), cr, dflag, hflag)) return rc;
+  }
+  return finish(bounds, true, stage_ms, wait_ms);
+}
+
+// callers run keyed_fit_check first
+int keyed_fit(int num_sms, cudaStream_t st, int32_t K, int32_t Dg, const int64_t* key_rowstart, const int64_t* rowptr, const int32_t* colidx,
+              const float* vals, int64_t ldx_in, const int32_t* response, const float* weight, const float* offset, bool has_intercept,
+              int32_t data_size_threshold, int32_t binary_feature, const std::vector<KeyedPrior>& priors, const double* intercept_mean,
+              double* out_model, double* out_var, int32_t* skipped) {
+  KeyedFit f{num_sms, st, K, Dg, key_rowstart, rowptr, colidx, vals, ldx_in, response, weight, offset, has_intercept, data_size_threshold,
+             binary_feature, priors, intercept_mean, out_model, out_var, skipped};
+  return f.run();
 }
 // host copy of a host-or-device array (NULL -> empty)
 template <class T> int host_copy(const T* in, size_t count, std::vector<T>& out) {

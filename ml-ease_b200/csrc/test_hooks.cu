@@ -1,14 +1,61 @@
 // test_hooks.cu -- the mlease_internal_* test hooks: not part of the C ABI (include/mlease_b200.h does not declare them), exported
 // for the tests and tools that drive single kernels of a session's batches.
+#include <algorithm>
+#include <atomic>
 #include <cmath>
 #include <cstring>
+#include <mutex>
 #include <vector>
 
 #include "host.cuh"
 
 using namespace mlease;
 
+namespace {
+std::atomic<unsigned long long> g_keyed_budget{0};
+std::mutex g_keyed_mu;   // the keyed calls of several host threads (one device each) record here
+std::vector<long long> g_keyed_bounds;
+bool g_keyed_streamed = false;
+double g_keyed_stage_ms = 0, g_keyed_wait_ms = 0;
+}  // namespace
+
+namespace mlease {
+size_t keyed_budget(size_t free_b) {
+  const unsigned long long cap = g_keyed_budget.load();
+  return cap ? std::min<size_t>(free_b, (size_t)cap) : free_b;
+}
+void keyed_record(const std::vector<long long>& bounds, bool streamed, double stage_ms, double wait_ms) {
+  std::lock_guard<std::mutex> g(g_keyed_mu);
+  g_keyed_bounds = bounds;
+  g_keyed_streamed = streamed;
+  g_keyed_stage_ms = stage_ms;
+  g_keyed_wait_ms = wait_ms;
+}
+}  // namespace mlease
+
 extern "C" {
+
+// Test hooks, not part of the C ABI: mlease_internal_set_keyed_budget caps, process-wide, the device bytes the keyed calls
+// (mlease_naive_train*, mlease_item_model_train, mlease_score_keyed) plan with (0 = the free memory only), so that small inputs stream
+// through many chunks.  mlease_internal_keyed_last_call reports the most recent keyed call of the process: the key boundaries of its
+// chunks (*count of them, the first 0 and the last K; up to cap are written), whether it streamed, and for a streamed fit the host
+// milliseconds its rows took to stage (copy into the pinned ring and H2D, all chunks) and the milliseconds the solve waited for them.
+int mlease_internal_set_keyed_budget(int64_t bytes) {
+  if (bytes < 0) return fail(MLEASE_ERR_INVALID, "bad argument");
+  g_keyed_budget.store((unsigned long long)bytes);
+  return 0;
+}
+
+int mlease_internal_keyed_last_call(int64_t* bounds, int32_t cap, int32_t* count, int32_t* streamed, double* stage_ms, double* wait_ms) {
+  if (!count || cap < 0 || (cap > 0 && !bounds)) return fail(MLEASE_ERR_INVALID, "bad argument");
+  std::lock_guard<std::mutex> g(g_keyed_mu);
+  *count = (int32_t)g_keyed_bounds.size();
+  for (size_t i = 0; i < g_keyed_bounds.size() && (int)i < cap; i++) bounds[i] = g_keyed_bounds[i];
+  if (streamed) *streamed = g_keyed_streamed ? 1 : 0;
+  if (stage_ms) *stage_ms = g_keyed_stage_ms;
+  if (wait_ms) *wait_ms = g_keyed_wait_ms;
+  return 0;
+}
 
 // Test hook, not part of the C ABI (include/mlease_b200.h does not declare it): one Hv (mode 1) or Hessian-diagonal (mode 2) pass
 // over the session's ADMM batch -- every (partition, lambda) problem at its own point w[b] and vector v[b] (b = local partition * L

@@ -89,8 +89,30 @@ void run_item_model_test(const JobConfig& c) {
     }
   }
   std::vector<float> pred((size_t)L * n);
-  ck(mlease_score_keyed(c.get_int("gpu.device", 0), nullptr, Dg, K, krs.data(), rp.data(), ci.data(), vv.data(), oo.data(), L, mp.data(),
-                        mc.data(), mv.data(), ignore_value ? 1 : 0, pred.data()));
+  const std::vector<int32_t> devs = gpu_devices(c);
+  if (devs.size() == 1 || K == 0) {
+    ck(mlease_score_keyed(devs[0], nullptr, Dg, K, krs.data(), rp.data(), ci.data(), vv.data(), oo.data(), L, mp.data(),
+                          mc.data(), mv.data(), ignore_value ? 1 : 0, pred.data()));
+  } else {
+    // one key range per device (shard_keys) with its models; each range's preds go to their slice of pred
+    run_shards(devs, shard_keys(krs, rp, Dg, (int)devs.size()), [&](int32_t dev, int k0, int k1) {
+      const KeySlice s(krs, rp, k0, k1);
+      const int Ks = k1 - k0;
+      const int64_t ns = s.krs[Ks];
+      std::vector<int64_t> smp{0}; std::vector<int32_t> smc; std::vector<float> smv;
+      for (int l = 0; l < L; l++)
+        for (int k = k0; k < k1; k++) {
+          const size_t m = (size_t)l * K + k;
+          smc.insert(smc.end(), mc.begin() + mp[m], mc.begin() + mp[m + 1]);
+          smv.insert(smv.end(), mv.begin() + mp[m], mv.begin() + mp[m + 1]);
+          smp.push_back((int64_t)smc.size());
+        }
+      std::vector<float> sp((size_t)L * ns);
+      ck(mlease_score_keyed(dev, nullptr, Dg, Ks, s.krs.data(), s.rowptr.data(), ci.data() + s.nz0, vv.data() + s.nz0, oo.data() + s.row0, L,
+                            smp.data(), smc.data(), smv.data(), ignore_value ? 1 : 0, sp.data()));
+      for (int l = 0; l < L; l++) std::copy(sp.begin() + (size_t)l * ns, sp.begin() + (size_t)(l + 1) * ns, pred.begin() + (size_t)l * n + s.row0);
+    });
+  }
   // output: every input field (unions removed) + pred, schema PerItemTestOutput (:214-248)
   AvroReader first(files[0]);
   for (size_t f = 1; f < files.size(); f++)

@@ -105,10 +105,26 @@ void run_item_model_train(const JobConfig& c) {
   }
   const int IL = (int)il.size(), DL = (int)dl.size();
   std::vector<double> m((size_t)IL * DL * K * Dt), var(compute_var ? m.size() : 0);
-  if (K > 0)
-    ck(mlease_item_model_train(c.get_int("gpu.device", 0), nullptr, K, D, krs.data(), rp.data(), ci.data(), vv.data(), rr.data(), ww.data(), oo.data(),
+  const std::vector<int32_t> devs = gpu_devices(c);
+  if (K > 0 && devs.size() == 1)
+    ck(mlease_item_model_train(devs[0], nullptr, K, D, krs.data(), rp.data(), ci.data(), vv.data(), rr.data(), ww.data(), oo.data(),
                                means.data(), IL, il.data(), DL, dl.data(), lambda_map.empty() ? nullptr : lambda_map.data(), binary ? 1 : 0,
                                compute_var ? 1 : 0, m.data(), compute_var ? var.data() : nullptr));
+  else if (K > 0)
+    // one key range per device (shard_keys); each range's models and variances go to their slices
+    run_shards(devs, shard_keys(krs, rp, D, (int)devs.size()), [&](int32_t dev, int k0, int k1) {
+      const KeySlice s(krs, rp, k0, k1);
+      const int Ks = k1 - k0;
+      std::vector<double> ms((size_t)IL * DL * Ks * Dt), vs(compute_var ? ms.size() : 0);
+      ck(mlease_item_model_train(dev, nullptr, Ks, D, s.krs.data(), s.rowptr.data(), ci.data() + s.nz0, vv.data() + s.nz0, rr.data() + s.row0,
+                                 ww.data() + s.row0, oo.data() + s.row0, means.data() + k0, IL, il.data(), DL, dl.data(),
+                                 lambda_map.empty() ? nullptr : lambda_map.data(), binary ? 1 : 0, compute_var ? 1 : 0, ms.data(),
+                                 compute_var ? vs.data() : nullptr));
+      for (int g = 0; g < IL * DL; g++) {
+        std::copy(ms.begin() + (size_t)g * Ks * Dt, ms.begin() + (size_t)(g + 1) * Ks * Dt, m.begin() + ((size_t)g * K + k0) * Dt);
+        if (compute_var) std::copy(vs.begin() + (size_t)g * Ks * Dt, vs.begin() + (size_t)(g + 1) * Ks * Dt, var.begin() + ((size_t)g * K + k0) * Dt);
+      }
+    });
   // posteriorVar also lists every lambda.map feature the key's rows do not, at its prior variance 1/lambda (llf/LibLinear.java:384-397),
   // after the dataset's features, in the map's order; the intercept's entry is always the dataset's
   auto absent_map_entries = [&](int k) {

@@ -3,10 +3,12 @@
 // regression_jobs.cpp are reached by mlease_job_run.
 #pragma once
 #include <algorithm>
+#include <exception>
 #include <fstream>
 #include <map>
 #include <stdexcept>
 #include <string>
+#include <thread>
 #include <unordered_map>
 #include <vector>
 
@@ -165,6 +167,63 @@ std::string test_output_schema(const SchemaP& in, const char* name = "AdmmTestOu
 // a record's bytes with the union branch indices dropped; throws NotPlain when the record is not plain
 struct NotPlain {};
 void transcode_plain(const Plan& pl, const uint8_t*& p, const uint8_t* e, std::string& o);
+
+// gpu.devices = 0,1,2,...  (falls back to the single gpu.device, default 0)
+std::vector<int32_t> gpu_devices(const JobConfig& c);
+
+// ------------------------------------------------------------------------------------------ keyed jobs on several GPUs
+// Keys are independent, so a keyed job (NaiveTrain, ItemModelTrain, ItemModelTest) cuts them into one contiguous range per device,
+// runs the single-device library call of each range on its own thread, and writes the results into disjoint slices of its output.
+//
+// shard_keys: cuts[s] .. cuts[s + 1] is shard s's key range, balanced by the estimated cost of a key, rows * (D + 1)^2 + nnz (a
+// shard's cost exceeds the mean by less than the largest key's).  Ranges may be empty when there are more shards than keys.
+inline std::vector<int> shard_keys(const std::vector<int64_t>& krs, const std::vector<int64_t>& rowptr, int D, int nshards) {
+  const int K = (int)krs.size() - 1;
+  const double d2 = (double)(D + 1) * (double)(D + 1);
+  std::vector<double> pre(K + 1, 0.0);
+  for (int k = 0; k < K; k++)
+    pre[k + 1] = pre[k] + (double)(krs[k + 1] - krs[k]) * d2 + (double)(rowptr[krs[k + 1]] - rowptr[krs[k]]);
+  std::vector<int> cuts{0};
+  int k = 0;
+  for (int s = 1; s < nshards; s++) {
+    const double target = pre[K] * s / nshards;
+    while (k < K && pre[k] < target) k++;   // the key that crosses the target closes the shard
+    cuts.push_back(k);
+  }
+  cuts.push_back(K);
+  return cuts;
+}
+
+// The rows of keys [k0, k1) of a CSR grouped by key: their own key_rowstart and rowptr (both from 0); row0 / nz0 locate the
+// range's rows and entries in the arrays of the whole job.
+struct KeySlice {
+  std::vector<int64_t> krs, rowptr;
+  int64_t row0 = 0, nz0 = 0;
+  KeySlice(const std::vector<int64_t>& krs_all, const std::vector<int64_t>& rp_all, int k0, int k1) {
+    row0 = krs_all[k0]; nz0 = rp_all[row0];
+    for (int k = k0; k <= k1; k++) krs.push_back(krs_all[k] - row0);
+    for (int64_t i = row0; i <= krs_all[k1]; i++) rowptr.push_back(rp_all[i] - nz0);
+  }
+};
+
+// fn(device, k0, k1) for every non-empty shard of cuts, one thread per device (on the calling thread when there is one device).
+// Every thread is joined; the first failing shard's error (in shard order) is the job's.
+template <class F> void run_shards(const std::vector<int32_t>& devs, const std::vector<int>& cuts, F fn) {
+  if (devs.size() == 1) { fn(devs[0], cuts[0], cuts[1]); return; }
+  std::vector<std::exception_ptr> err(devs.size());
+  std::vector<std::thread> ts;
+  for (size_t s = 0; s < devs.size(); s++) {
+    if (cuts[s] == cuts[s + 1]) continue;
+    try {
+      ts.emplace_back([&, s] { try { fn(devs[s], cuts[s], cuts[s + 1]); } catch (...) { err[s] = std::current_exception(); } });
+    } catch (...) {   // no thread for this shard: the job fails, after the running shards are joined
+      err[s] = std::current_exception();
+      break;
+    }
+  }
+  for (auto& t : ts) t.join();
+  for (auto& e : err) if (e) std::rethrow_exception(e);
+}
 
 // job_class -> job for mlease_job_run; returns true (for use in a namespace-scope initializer)
 using JobFn = void (*)(const JobConfig&);

@@ -470,6 +470,7 @@ struct World {
 };
 // gpu.devices = 0,1,2,...  (falls back to the single gpu.device, default 0).  Not a reference key: the reference's
 // parallelism is Hadoop's (one reducer per (partition, lambda), jobs/RegressionAdmmTrain.java:355).
+// The keyed jobs shard their keys over the same list (run_shards).
 std::vector<int32_t> gpu_devices(const JobConfig& c) {
   std::vector<int32_t> d;
   if (c.has("gpu.devices")) for (auto& t : c.get_list("gpu.devices")) d.push_back(std::stoi(t));
@@ -1269,9 +1270,27 @@ void run_naive_train(const JobConfig& c) {
   std::vector<const std::vector<int32_t>*> model_feats;
   std::map<std::string, std::pair<int, std::vector<double>>> sums;
   std::vector<double> m((size_t)L * K * Dt); std::vector<int32_t> skipped(K);
-  ck(mlease_naive_train(gpu_devices(c)[0], nullptr, K, D, krs.data(), rp.data(), ci.data(), vv.data(), 0, rr.data(), ww.data(), oo.data(), L, lambdas.data(),
-                        lambda_map.empty() ? nullptr : lambda_map.data(), c.get_float("prior.mean", 0.0f), penalize_intercept,
-                        c.get_bool("has.intercept", true), c.get_int("data.size.threshold", 0), ignore_value ? 1 : 0, m.data(), skipped.data()));
+  const std::vector<int32_t> devs = gpu_devices(c);
+  const float prior_mean = c.get_float("prior.mean", 0.0f);
+  const bool has_intercept = c.get_bool("has.intercept", true);
+  const int threshold = c.get_int("data.size.threshold", 0);
+  if (devs.size() == 1 || K == 0) {
+    ck(mlease_naive_train(devs[0], nullptr, K, D, krs.data(), rp.data(), ci.data(), vv.data(), 0, rr.data(), ww.data(), oo.data(), L, lambdas.data(),
+                          lambda_map.empty() ? nullptr : lambda_map.data(), prior_mean, penalize_intercept, has_intercept, threshold, ignore_value ? 1 : 0,
+                          m.data(), skipped.data()));
+  } else {
+    // one key range per device (shard_keys); each range's models go to their slice of m
+    run_shards(devs, shard_keys(krs, rp, D, (int)devs.size()), [&](int32_t dev, int k0, int k1) {
+      const KeySlice s(krs, rp, k0, k1);
+      const int Ks = k1 - k0;
+      std::vector<double> ms((size_t)L * Ks * Dt);
+      ck(mlease_naive_train(dev, nullptr, Ks, D, s.krs.data(), s.rowptr.data(), ci.data() + s.nz0, vv.data() + s.nz0, 0, rr.data() + s.row0,
+                            ww.data() + s.row0, oo.data() + s.row0, L, lambdas.data(), lambda_map.empty() ? nullptr : lambda_map.data(), prior_mean,
+                            penalize_intercept, has_intercept, threshold, ignore_value ? 1 : 0, ms.data(), skipped.data() + k0));
+      for (int l = 0; l < L; l++)
+        std::copy(ms.begin() + (size_t)l * Ks * Dt, ms.begin() + (size_t)(l + 1) * Ks * Dt, m.begin() + ((size_t)l * K + k0) * Dt);
+    });
+  }
   for (int l = 0; l < L; l++) {
     const std::string ls = java_float_to_string(lambdas[l]);
     auto& acc = sums[ls]; acc.second.assign(Dt, 0.0);

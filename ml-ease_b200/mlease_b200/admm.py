@@ -492,3 +492,23 @@ def item_model_train(vals, key_rowstart, response, intercept_lambdas, default_la
                                         len(il), ptr(il), len(dl), ptr(dl), ptr(lm), int(bool(binary_feature)), int(bool(compute_var)),
                                         ptr(out), ptr(var)))
     return out, var
+
+
+def _internal_set_keyed_budget(nbytes):
+    """Test hook (not part of the C ABI): caps, process-wide, the device bytes the keyed calls plan with (0 = free memory only),
+    so that small inputs stream through many chunks."""
+    fn = lib().mlease_internal_set_keyed_budget
+    fn.argtypes, fn.restype = [C.c_int64], C.c_int
+    check(fn(int(nbytes)))
+
+
+def _internal_keyed_last_call():
+    """Test hook: the most recent keyed call of the process -> (key boundaries of its chunks, streamed, stage ms, wait ms)."""
+    fn = lib().mlease_internal_keyed_last_call
+    fn.argtypes, fn.restype = [C.c_void_p, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_double),
+                               C.POINTER(C.c_double)], C.c_int
+    n, s, a, b = C.c_int32(), C.c_int32(), C.c_double(), C.c_double()
+    check(fn(None, 0, C.byref(n), None, None, None))
+    bounds = np.zeros(max(n.value, 1), np.int64)
+    check(fn(bounds.ctypes.data, n.value, C.byref(n), C.byref(s), C.byref(a), C.byref(b)))
+    return bounds[:n.value], bool(s.value), a.value, b.value
