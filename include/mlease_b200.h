@@ -242,7 +242,7 @@ int mlease_posterior_variance(mlease_session* s, int32_t partition_id, const dou
  * except out_model / skipped (host).  A fit that does not converge -> MLEASE_ERR_NUMERIC ("Model fitting error!", :400-412).
  *
  * Inputs larger than the device: when the rows, labels and key boundaries do not fit next to the first chunk's solver state, the
- * keyed calls (mlease_naive_train, mlease_naive_train_dense, mlease_item_model_train, mlease_score_keyed) stream contiguous key
+ * keyed calls (mlease_naive_train, mlease_naive_train_dense, mlease_item_model_train, mlease_score_keyed[_var]) stream contiguous key
  * ranges through the device, the next range's rows copied while the current one is solved.  A key's fit then matches the resident
  * call's within the run-to-run spread of the CSR kernels (their gradient sums use float atomics); scores are bitwise the same.
  * In that mode "rows sorted and unique" (which selects the CSR kernels) is decided per key range, not per call, so one key with
@@ -300,6 +300,19 @@ int mlease_test_loglik(int32_t device, void* stream, int64_t nrows, const int32_
 int mlease_score_keyed(int32_t device, void* stream, int32_t num_features, int32_t num_keys, const int64_t* key_rowstart,
                        const int64_t* rowptr, const int32_t* colidx, const float* vals, const float* offset, int32_t num_lambdas,
                        const int64_t* model_ptr, const int32_t* model_col, const float* model_val, int32_t binary_feature, float* pred);
+/* mlease_score_keyed with each record's predictive variance under the diagonal posterior of its key's model (ItemModelTrain with
+ * compute.var).  Rows, keys and models as in mlease_score_keyed, model m = g*num_keys + k for grid point g of
+ * num_models_per_key; rows must list strictly ascending columns (checked).  Model m's variance list is entries
+ * [var_ptr[m], var_ptr[m+1]) of var_col (strictly ascending, <= num_features = the intercept, checked) and var_val; var_default[m]
+ * is the variance of every column the list does not name; every variance finite and >= 0 (checked).
+ * pred [G][nrows] is bitwise mlease_score_keyed's; pred_var [G][nrows] = float(sum_e v(c_e) x_e^2 + v_b) accumulated in double,
+ * x_e = 1 under binary_feature, v_b = the listed intercept variance or 0; a model with an empty variance list gives NaN (no
+ * posterior).  All pointers host-or-device; streams over key ranges and runs on several devices like mlease_score_keyed. */
+int mlease_score_keyed_var(int32_t device, void* stream, int32_t num_features, int32_t num_keys, const int64_t* key_rowstart,
+                           const int64_t* rowptr, const int32_t* colidx, const float* vals, const float* offset,
+                           int32_t num_models_per_key, const int64_t* model_ptr, const int32_t* model_col, const float* model_val,
+                           const int64_t* var_ptr, const int32_t* var_col, const float* var_val, const float* var_default,
+                           int32_t binary_feature, float* pred, float* pred_var);
 /* ItemModelTestLoglik (jobs/ItemModelTestLoglik.java:60-142): entry e = one (record, pred-map key) pair: entry_key[e] in
  * [0, num_keys), entry_group[e] = combiner group (non-decreasing), the record's response (1, 0, -1) and weight (NULL = 1), pred[e].
  * out_loglik / out_count [num_keys] (host): reducer float(sum of float combiner partials / sum of counts), partials added in group

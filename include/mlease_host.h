@@ -12,8 +12,11 @@
 extern "C" {
 #endif
 /* job_class: Regression | RegressionPrepare | RegressionAdmmTrain | RegressionTest | RegressionTestLoglik |
- * RegressionNaiveTrain | ItemModelTest | ItemModelTestLoglik | ItemModelTrain (README aliases AdmmPrepare/AdmmTrain/AdmmTest/AdmmTestLoglik/NaiveTrain
- * accepted).
+ * RegressionNaiveTrain | ItemModelTest | ItemModelTestLoglik | ItemModelTrain | ItemModelGridTest (README aliases
+ * AdmmPrepare/AdmmTrain/AdmmTest/AdmmTestLoglik/NaiveTrain accepted).  ItemModelGridTest is not a reference job: it scores held-out
+ * records with every (intercept lambda, default lambda) model ItemModelTrain wrote for their key, writes pred (and predVar, the
+ * predictive variance under the diagonal posterior, with compute.var) per grid point under output.base.path/lambda-<il>_<dl>/, and
+ * one test log-likelihood per grid point under output.base.path/_loglik/.
  * Returns 0, or non-zero with the message (the reference's IOException / RuntimeException text) in mlease_job_last_error(). */
 int mlease_job_run(const char* job_class, const char* config_path);
 const char* mlease_job_last_error(void);

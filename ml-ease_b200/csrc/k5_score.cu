@@ -3,7 +3,8 @@
 //           float cast of RegressionTest (jobs/RegressionTest.java:163).  One warp per record, fp64 accumulate.
 //   loglik: RegressionTestLoglik mapper/combiner/reducer (jobs/RegressionTestLoglik.java:124-200) with its float
 //           rounding points: per-record float, per-combiner-block float, final float(sum/count).
-//   keyed : ItemModelTest / ItemModelTestLoglik, the same two computations with one model (and one reducer) per key.
+//   keyed : ItemModelTest / ItemModelTestLoglik, the same two computations with one model (and one reducer) per key; with a
+//           variance list per model (ItemModelTrain's posteriorVar), also each record's predictive variance.
 // HBM-bound streaming kernels (one read of the test matrix).
 #include <cub/device/device_radix_sort.cuh>
 
@@ -76,17 +77,22 @@ __device__ __forceinline__ void load_lp(const float* p, float (&t)[LP]) {
   else t[0] = *p;
 }
 
-template <int LP>
+// WITH_VAR (mlease_score_keyed_var): a second [key - k0][Dg][LP] table holds each model's diagonal posterior variance (var_default
+// where its list names no column), and pred_var = float(sum v x^2 + vterm) beside pred, in fp64 with the same lane stride.  Rows
+// must then list strictly ascending columns (bad |= 2): a repeated column would count as two independent terms of the variance.
+template <int LP, bool WITH_VAR>
 __global__ void __launch_bounds__(256) score_keyed_kernel(int Dg, int k0, int k1, long long r0, long long r1, const long long* __restrict__ krs,
                                                           const long long* __restrict__ rowptr, const int* __restrict__ colidx,
                                                           const float* __restrict__ vals, const float* __restrict__ offset,
                                                           const float* __restrict__ table, const double* __restrict__ term, int K, int G,
                                                           int binary_feature, long long nrows, long long row_base, float* __restrict__ pred,
-                                                          int* __restrict__ bad) {
+                                                          int* __restrict__ bad, const float* __restrict__ vtable,
+                                                          const double* __restrict__ vterm, float* __restrict__ pred_var) {
   // rowptr, offset and pred hold rows [row_base, ...): a streamed key range indexes its own copy of them
   rowptr -= row_base;
   if (offset) offset -= row_base;
   pred -= row_base;
+  if constexpr (WITH_VAR) pred_var -= row_base;
   const int lane = threadIdx.x & 31;
   const long long wg = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
@@ -94,60 +100,105 @@ __global__ void __launch_bounds__(256) score_keyed_kernel(int Dg, int k0, int k1
     int lo = k0, hi = k1;   // krs[lo] <= i < krs[hi]: row i belongs to key lo once hi = lo + 1
     while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (krs[mid] <= i) lo = mid; else hi = mid; }
     const float* tk = table + (size_t)(lo - k0) * Dg * LP;
-    double a[LP];
+    double a[LP], va[LP];
 #pragma unroll
-    for (int q = 0; q < LP; q++) a[q] = 0.0;
-    for (long long j = rowptr[i] + lane; j < rowptr[i + 1]; j += 32) {
+    for (int q = 0; q < LP; q++) { a[q] = 0.0; if constexpr (WITH_VAR) va[q] = 0.0; }
+    const long long j0 = rowptr[i];
+    for (long long j = j0 + lane; j < rowptr[i + 1]; j += 32) {
       const int c = colidx[j];
       if ((unsigned)c >= (unsigned)Dg) { *bad = 1; continue; }
+      if constexpr (WITH_VAR) { if (j > j0 && colidx[j - 1] >= c) { atomicOr(bad, 2); continue; } }
       float t[LP];
       load_lp<LP>(tk + (size_t)c * LP, t);
       const double v = binary_feature ? 1.0 : (double)vals[j];
 #pragma unroll
       for (int q = 0; q < LP; q++) a[q] += (double)t[q] * v;
+      if constexpr (WITH_VAR) {
+        float s[LP];
+        load_lp<LP>(vtable + ((size_t)(lo - k0) * Dg + c) * LP, s);
+        const double v2 = v * v;
+#pragma unroll
+        for (int q = 0; q < LP; q++) va[q] += (double)s[q] * v2;
+      }
     }
 #pragma unroll
-    for (int q = 0; q < LP; q++) a[q] = warp_sum(a[q]);
+    for (int q = 0; q < LP; q++) { a[q] = warp_sum(a[q]); if constexpr (WITH_VAR) va[q] = warp_sum(va[q]); }
     if (lane == 0) {
       const double o = offset ? (double)offset[i] : 0.0;
 #pragma unroll
       for (int q = 0; q < LP; q++)
-        if (q < G) pred[(size_t)q * nrows + i] = (float)(o + (term[(size_t)q * K + lo] + a[q]));
+        if (q < G) {
+          pred[(size_t)q * nrows + i] = (float)(o + (term[(size_t)q * K + lo] + a[q]));
+          if constexpr (WITH_VAR) pred_var[(size_t)q * nrows + i] = (float)(va[q] + vterm[(size_t)q * K + lo]);
+        }
     }
   }
 }
 
 // one warp per (lambda of the group, key of the chunk): its model's coefficients into the table; the intercept (column Dg)
-// is not a table column, it enters through term
+// is not a table column, it enters through term.  fill (variance lists): every column of the model's slice starts at fill[m].
 __global__ void __launch_bounds__(256) keyed_table_scatter_kernel(int Dg, int K, int k0, int nk, int G, int LP, const long long* __restrict__ mp,
-                                                                  const int* __restrict__ mc, const float* __restrict__ mv, float* __restrict__ table) {
+                                                                  const int* __restrict__ mc, const float* __restrict__ mv, float* __restrict__ table,
+                                                                  const float* __restrict__ fill) {
   const int lane = threadIdx.x & 31;
   const long long w = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   if (w >= (long long)nk * G) return;
   const int q = (int)(w / nk), kk = (int)(w % nk);
   const long long m = (long long)q * K + k0 + kk;
+  if (fill) {
+    for (int c = lane; c < Dg; c += 32) table[((size_t)kk * Dg + c) * LP + q] = fill[m];
+    __syncwarp();
+  }
   for (long long e = mp[m] + lane; e < mp[m + 1]; e += 32) {
     const int c = mc[e];
     if (c < Dg) table[((size_t)kk * Dg + c) * LP + q] = mv[e];
   }
 }
 
+// The variance lists of mlease_score_keyed_var on the device, for one group of up to four lambdas (at()); all null for
+// mlease_score_keyed.  vterm[m]: the listed intercept variance, 0 without one, NaN for an empty list.
+struct KeyedVar {
+  const long long* vp = nullptr;
+  const int* vc = nullptr;
+  const float* vv = nullptr;
+  const float* vdef = nullptr;
+  const double* vterm = nullptr;
+  float* vtable = nullptr;
+  float* pred_var = nullptr;
+  explicit operator bool() const { return vp != nullptr; }
+  KeyedVar at(int l0, int K, long long nrows) const {
+    if (!vp) return *this;
+    KeyedVar r = *this;
+    r.vp += (size_t)l0 * K; r.vdef += (size_t)l0 * K; r.vterm += (size_t)l0 * K; r.pred_var += (size_t)l0 * nrows;
+    return r;
+  }
+};
+
 static cudaError_t score_keyed_chunk(int Dg, int K, int k0, int k1, long long r0, long long r1, const long long* krs, const long long* rowptr,
                                      const int* colidx, const float* vals, const float* offset, int G, const long long* mp, const int* mc,
                                      const float* mv, const double* term, int binary_feature, long long nrows, long long row_base, float* table,
-                                     float* pred, int* d_bad, cudaStream_t st) {
+                                     float* pred, int* d_bad, const KeyedVar& var, cudaStream_t st) {
   const int LP = G == 1 ? 1 : G == 2 ? 2 : 4;
   const int nk = k1 - k0;
-  cudaError_t e = cudaMemsetAsync(table, 0, (size_t)nk * Dg * LP * sizeof(float), st);
+  const size_t tbytes = (size_t)nk * Dg * LP * sizeof(float);
+  cudaError_t e = cudaMemsetAsync(table, 0, tbytes, st);
+  if (e == cudaSuccess && var) e = cudaMemsetAsync(var.vtable, 0, tbytes, st);   // the unused lanes of a group of three
   if (e != cudaSuccess) return e;
   const long long warps = (long long)nk * G;
-  keyed_table_scatter_kernel<<<(int)((warps + 7) / 8), 256, 0, st>>>(Dg, K, k0, nk, G, LP, mp, mc, mv, table);
+  keyed_table_scatter_kernel<<<(int)((warps + 7) / 8), 256, 0, st>>>(Dg, K, k0, nk, G, LP, mp, mc, mv, table, nullptr);
+  if (var) keyed_table_scatter_kernel<<<(int)((warps + 7) / 8), 256, 0, st>>>(Dg, K, k0, nk, G, LP, var.vp, var.vc, var.vv, var.vtable, var.vdef);
   if (r1 > r0) {
     long long blocks = (r1 - r0 + 7) / 8;
     if (blocks > 132 * 16) blocks = 132 * 16;
-    if (LP == 1) score_keyed_kernel<1><<<(int)blocks, 256, 0, st>>>(Dg, k0, k1, r0, r1, krs, rowptr, colidx, vals, offset, table, term, K, G, binary_feature, nrows, row_base, pred, d_bad);
-    else if (LP == 2) score_keyed_kernel<2><<<(int)blocks, 256, 0, st>>>(Dg, k0, k1, r0, r1, krs, rowptr, colidx, vals, offset, table, term, K, G, binary_feature, nrows, row_base, pred, d_bad);
-    else score_keyed_kernel<4><<<(int)blocks, 256, 0, st>>>(Dg, k0, k1, r0, r1, krs, rowptr, colidx, vals, offset, table, term, K, G, binary_feature, nrows, row_base, pred, d_bad);
+#define MLEASE_SCORE_KEYED(LP_, V_)                                                                                                     \
+  score_keyed_kernel<LP_, V_><<<(int)blocks, 256, 0, st>>>(Dg, k0, k1, r0, r1, krs, rowptr, colidx, vals, offset, table, term, K, G,   \
+                                                           binary_feature, nrows, row_base, pred, d_bad, var.vtable, var.vterm, var.pred_var)
+    if (var) {
+      if (LP == 1) MLEASE_SCORE_KEYED(1, true); else if (LP == 2) MLEASE_SCORE_KEYED(2, true); else MLEASE_SCORE_KEYED(4, true);
+    } else {
+      if (LP == 1) MLEASE_SCORE_KEYED(1, false); else if (LP == 2) MLEASE_SCORE_KEYED(2, false); else MLEASE_SCORE_KEYED(4, false);
+    }
+#undef MLEASE_SCORE_KEYED
   }
   return cudaGetLastError();
 }
@@ -240,25 +291,51 @@ static cudaError_t loglik_launch(long long nrows, const int* response, const flo
 // four lambdas.
 static constexpr size_t SCORE_KEYED_TABLE_CAP = size_t(1) << 30;
 
+// the row checks of score_keyed_kernel, read back
+static int keyed_bad(int bad) {
+  if (bad & 1) return fail(MLEASE_ERR_INVALID, "colidx out of range [0, num_features)");
+  if (bad & 2) return fail(MLEASE_ERR_INVALID, "colidx must be strictly ascending within a row");
+  return 0;
+}
+
+// Host copies of mlease_score_keyed_var's variance lists, checked, and its pred_var output; absent for mlease_score_keyed.
+struct KeyedVarHost {
+  std::vector<long long> vp;
+  std::vector<int> vc;
+  std::vector<float> vv, vdef;
+  std::vector<double> vterm;
+  float* pred_var = nullptr;
+  size_t bytes() const { return vp.size() * 8 + vc.size() * 4 + vv.size() * 4 + vdef.size() * 4 + vterm.size() * 8; }
+  int upload(DevMem& t, KeyedVar& d, cudaStream_t st) const {
+    if (int rc = to_device(t, (const long long*)vp.data(), vp.size(), &d.vp, st)) return rc;
+    if (int rc = to_device(t, (const int*)vc.data(), vc.size(), &d.vc, st)) return rc;
+    if (int rc = to_device(t, (const float*)vv.data(), vv.size(), &d.vv, st)) return rc;
+    if (int rc = to_device(t, (const float*)vdef.data(), vdef.size(), &d.vdef, st)) return rc;
+    return to_device(t, (const double*)vterm.data(), vterm.size(), &d.vterm, st);
+  }
+};
+
 // mlease_score_keyed over key ranges whose rows, offsets and pred slice fit a quarter of the budget, next to the models (uploaded
 // once).  The rows of range r+1 are copied on a second stream while range r is scored, and each pred slice goes back as soon as
-// it is done.  A pred is a function of its row and its key's model only, so it is bitwise the resident call's.
+// it is done.  A pred is a function of its row and its key's model only, so it is bitwise the resident call's; so is a pred_var.
 static int score_keyed_streamed(cudaStream_t st, int Dg, int K, const std::vector<long long>& krs, const int64_t* rowptr, const int32_t* colidx,
                                 const float* vals, const float* offset, int L, const std::vector<long long>& mp, const std::vector<int>& mc,
-                                const std::vector<float>& mv, const std::vector<double>& term, int binary_feature, float* pred, size_t budget) {
+                                const std::vector<float>& mv, const std::vector<double>& term, int binary_feature, float* pred,
+                                const KeyedVarHost* var, size_t budget) {
   const long long nrows = krs[K];
   std::vector<long long> off;   // rowptr at the key boundaries
   if (int rc = gather_rowptr(rowptr, krs, off)) return rc;
-  const size_t key_bytes = (size_t)Dg * (L >= 3 ? 4 : L) * sizeof(float);
+  const size_t key_bytes = (size_t)Dg * (L >= 3 ? 4 : L) * sizeof(float) * (var ? 2 : 1);
   const long long kpc = std::max<long long>(1, std::min<long long>(K, (long long)(std::min(SCORE_KEYED_TABLE_CAP, budget / 4) / key_bytes)));
   const size_t cap = budget / 4;
+  const size_t pred_bytes = 4 * (size_t)L * (var ? 2 : 1);   // a row's pred (and pred_var) slice
   std::vector<long long> bounds{0};
   long long max_rows = 0, max_nnz = 0;
   for (int k = 0; k < K;) {
     int e = k;
     size_t bytes = 0;
     while (e < K) {
-      const size_t need = (size_t)(krs[e + 1] - krs[e]) * (16 + 4 + 4 * (size_t)L) + (size_t)(off[e + 1] - off[e]) * 8;
+      const size_t need = (size_t)(krs[e + 1] - krs[e]) * (16 + 4 + pred_bytes) + (size_t)(off[e + 1] - off[e]) * 8;
       if (e > k && (bytes + need > cap || e - k >= kpc)) break;
       bytes += need; e++;
     }
@@ -275,6 +352,8 @@ static int score_keyed_streamed(cudaStream_t st, int Dg, int K, const std::vecto
   if (int rc = to_device(t, (const int*)mc.data(), mc.size(), &d_mc, st)) return rc;
   if (int rc = to_device(t, (const float*)mv.data(), mv.size(), &d_mv, st)) return rc;
   if (int rc = to_device(t, (const double*)term.data(), term.size(), &d_term, st)) return rc;
+  KeyedVar dvar;
+  if (var) { if (int rc = var->upload(t, dvar, st)) return rc; }
   long long* rp_raw[2]; int* ci[2]; float* v[2]; float* o[2] = {nullptr, nullptr};
   for (int b = 0; b < 2; b++) {
     if (int rc = t.get(&rp_raw[b], (size_t)max_rows + 1, false)) return rc;
@@ -286,6 +365,10 @@ static int score_keyed_streamed(cudaStream_t st, int Dg, int K, const std::vecto
   if (int rc = t.get(&d_rp, (size_t)max_rows + 1, false)) return rc;
   if (int rc = t.get(&d_table, (size_t)kpc * key_bytes / sizeof(float), false)) return rc;
   if (int rc = t.get(&d_pred, (size_t)L * max_rows, false)) return rc;
+  if (var) {   // the second half of the table and a pred_var slice
+    dvar.vtable = d_table + (size_t)kpc * key_bytes / 2 / sizeof(float);
+    if (int rc = t.get(&dvar.pred_var, (size_t)L * max_rows, false)) return rc;
+  }
   if (int rc = t.get(&d_bad, 1, false)) return rc;
   CK(cudaMemsetAsync(d_bad, 0, 4, st));
   struct Ring {   // the copy stream and its events, released on every return path
@@ -327,19 +410,20 @@ static int score_keyed_streamed(cudaStream_t st, int Dg, int K, const std::vecto
       rebase_rowptr(st, n, rp_raw[b], off[k0], d_rp);
       for (int l0 = 0; l0 < L; l0 += 4)
         CK(score_keyed_chunk(Dg, K, k0, k1, r0, r0 + n, d_krs, d_rp, ci[b], v[b], o[b], std::min(4, L - l0), d_mp + (size_t)l0 * K, d_mc, d_mv,
-                             d_term + (size_t)l0 * K, binary_feature, n, r0, d_table, d_pred + (size_t)l0 * n, d_bad, st));
+                             d_term + (size_t)l0 * K, binary_feature, n, r0, d_table, d_pred + (size_t)l0 * n, d_bad, dvar.at(l0, K, n), st));
     }
     CK(cudaEventRecord(ring.done[b], st));
     if (r + 1 < nr) { if (int rc = upload(r + 1)) return rc; }
     if (n > 0) CK(cudaMemcpy2DAsync(pred + r0, (size_t)nrows * 4, d_pred, (size_t)n * 4, (size_t)n * 4, L, cudaMemcpyDefault, st));
+    if (n > 0 && var)
+      CK(cudaMemcpy2DAsync(var->pred_var + r0, (size_t)nrows * 4, dvar.pred_var, (size_t)n * 4, (size_t)n * 4, L, cudaMemcpyDefault, st));
   }
   int bad = 0;
   CK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   CK(cudaStreamSynchronize(ring.cs));
   keyed_record(bounds, true, 0, 0);
-  if (bad) return fail(MLEASE_ERR_INVALID, "colidx out of range [0, num_features)");
-  return 0;
+  return keyed_bad(bad);
 }
 
 }  // namespace mlease
@@ -417,11 +501,18 @@ int mlease_test_loglik(int32_t device, void* stream, int64_t nrows, const int32_
   return 0;
 }
 
+}  // extern "C"
 
-int mlease_score_keyed(int32_t device, void* stream, int32_t Dg, int32_t K, const int64_t* key_rowstart, const int64_t* rowptr,
+namespace mlease {
+
+// mlease_score_keyed, and mlease_score_keyed_var when var_ptr is given: the variance lists are copied to the host and checked
+// like the models, and every table, slice and copy of pred gets its variance twin.
+static int score_keyed(int32_t device, void* stream, int32_t Dg, int32_t K, const int64_t* key_rowstart, const int64_t* rowptr,
                        const int32_t* colidx, const float* vals, const float* offset, int32_t L, const int64_t* model_ptr,
-                       const int32_t* model_col, const float* model_val, int32_t binary_feature, float* pred) {
+                       const int32_t* model_col, const float* model_val, const int64_t* var_ptr, const int32_t* var_col,
+                       const float* var_val, const float* var_default, int32_t binary_feature, float* pred, float* pred_var) {
   if (Dg <= 0 || K < 0 || L <= 0 || !key_rowstart || !rowptr || !colidx || !vals || !model_ptr || !pred) return fail(MLEASE_ERR_INVALID, "bad argument");
+  if (var_ptr && (!var_default || !pred_var)) return fail(MLEASE_ERR_INVALID, "bad argument");
   if (int rc = open_device(device, nullptr)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   // host copies of the index arrays that decide the chunks and of the models, which are checked and give the intercept terms
@@ -453,26 +544,60 @@ int mlease_score_keyed(int32_t device, void* stream, int32_t Dg, int32_t K, cons
     const double b = (mp[m + 1] > mp[m] && mc[mp[m + 1] - 1] == Dg) ? (double)mv[mp[m + 1] - 1] : 0.0;
     term[m] = -std::log(1.0 - 1 + 1.0 * std::exp(-b));
   }
+  KeyedVarHost vh;
+  const KeyedVarHost* var = var_ptr ? &vh : nullptr;
+  if (var) {
+    // the same checks for the variance lists, and every variance finite and >= 0; vterm = the listed intercept variance, 0 when the
+    // list does not name the intercept (as term), NaN for an empty list (no posterior for this model)
+    vh.pred_var = pred_var;
+    vh.vp.resize((size_t)M + 1);
+    vh.vdef.resize((size_t)M);
+    CK(cudaMemcpy(vh.vp.data(), var_ptr, vh.vp.size() * 8, cudaMemcpyDefault));
+    if (M > 0) CK(cudaMemcpy(vh.vdef.data(), var_default, (size_t)M * 4, cudaMemcpyDefault));
+    if (vh.vp[0] != 0) return fail(MLEASE_ERR_INVALID, "var_ptr[0] must be 0");
+    for (long long m = 0; m < M; m++) if (vh.vp[m + 1] < vh.vp[m]) return fail(MLEASE_ERR_INVALID, "var_ptr must be non-decreasing");
+    const long long nve = vh.vp[M];
+    if (nve > 0 && (!var_col || !var_val)) return fail(MLEASE_ERR_INVALID, "null var_col / var_val");
+    vh.vc.resize((size_t)nve);
+    vh.vv.resize((size_t)nve);
+    if (nve > 0) {
+      CK(cudaMemcpy(vh.vc.data(), var_col, (size_t)nve * 4, cudaMemcpyDefault));
+      CK(cudaMemcpy(vh.vv.data(), var_val, (size_t)nve * 4, cudaMemcpyDefault));
+    }
+    vh.vterm.resize((size_t)M);
+    for (long long m = 0; m < M; m++) {
+      auto bad = [m](const char* what) { return fail(MLEASE_ERR_INVALID, std::string(what) + " (model " + std::to_string(m) + ")"); };
+      if (!(std::isfinite(vh.vdef[m]) && vh.vdef[m] >= 0.f)) return bad("var_default must be finite and >= 0");
+      for (long long e = vh.vp[m]; e < vh.vp[m + 1]; e++) {
+        if (vh.vc[e] < 0 || vh.vc[e] > Dg) return bad("var_col out of range");
+        if (e > vh.vp[m] && vh.vc[e] <= vh.vc[e - 1]) return bad("var_col must be strictly ascending within a model");
+        if (!(std::isfinite(vh.vv[e]) && vh.vv[e] >= 0.f)) return bad("var_val must be finite and >= 0");
+      }
+      const long long e1 = vh.vp[m + 1];
+      vh.vterm[m] = e1 == vh.vp[m] ? std::nan("") : vh.vc[e1 - 1] == Dg ? (double)vh.vv[e1 - 1] : 0.0;
+    }
+  }
   if (nrows == 0) return 0;
   long long nnz;
   CK(cudaMemcpy(&nnz, rowptr + nrows, 8, cudaMemcpyDefault));
-  const bool pred_dev = is_device_ptr(pred);
-  const size_t key_bytes = (size_t)Dg * (L >= 3 ? 4 : L) * sizeof(float);
+  const bool pred_dev = is_device_ptr(pred), pred_var_dev = var && is_device_ptr(pred_var);
+  const size_t key_bytes = (size_t)Dg * (L >= 3 ? 4 : L) * sizeof(float) * (var ? 2 : 1);   // var: the variance table too
   size_t free_b = 0, total_b = 0;
   CK(cudaMemGetInfo(&free_b, &total_b));
   const size_t budget = keyed_budget(free_b);
   {
     // resident when the rows, the pred array and the model table fit the budget next to the models; else key ranges stream
-    const size_t models = ((size_t)M + 1) * 8 + (size_t)nme * 8 + (size_t)M * 8 + ((size_t)K + 1) * 8;
+    const size_t models = ((size_t)M + 1) * 8 + (size_t)nme * 8 + (size_t)M * 8 + ((size_t)K + 1) * 8 + (var ? var->bytes() : 0);
     size_t rows = 0;
     if (!is_device_ptr(rowptr)) rows += ((size_t)nrows + 1) * 8;
     if (!is_device_ptr(colidx)) rows += (size_t)nnz * 4;
     if (!is_device_ptr(vals)) rows += (size_t)nnz * 4;
     if (offset && !is_device_ptr(offset)) rows += (size_t)nrows * 4;
     if (!pred_dev) rows += (size_t)L * nrows * 4;
+    if (var && !pred_var_dev) rows += (size_t)L * nrows * 4;
     const size_t table = std::min(SCORE_KEYED_TABLE_CAP, budget / 4);
     if (models + rows + table > budget)
-      return score_keyed_streamed(st, Dg, K, krs, rowptr, colidx, vals, offset, L, mp, mc, mv, term, binary_feature, pred, budget);
+      return score_keyed_streamed(st, Dg, K, krs, rowptr, colidx, vals, offset, L, mp, mc, mv, term, binary_feature, pred, var, budget);
   }
   DevMem t;
   const long long *d_rp, *d_krs, *d_mp; const int *d_ci, *d_mc; const float *d_v, *d_o, *d_mv; const double* d_term;
@@ -485,8 +610,14 @@ int mlease_score_keyed(int32_t device, void* stream, int32_t Dg, int32_t K, cons
   if (int rc = to_device(t, (const int*)mc.data(), mc.size(), &d_mc, st)) return rc;
   if (int rc = to_device(t, (const float*)mv.data(), mv.size(), &d_mv, st)) return rc;
   if (int rc = to_device(t, (const double*)term.data(), term.size(), &d_term, st)) return rc;
+  KeyedVar dvar;
+  if (var) { if (int rc = var->upload(t, dvar, st)) return rc; }
   float* d_pred = pred;
   if (!pred_dev) { if (int rc = t.get(&d_pred, (size_t)L * nrows, false)) return rc; }
+  if (var) {
+    dvar.pred_var = pred_var;
+    if (!pred_var_dev) { if (int rc = t.get(&dvar.pred_var, (size_t)L * nrows, false)) return rc; }
+  }
   int* d_bad;
   if (int rc = t.get(&d_bad, 1, false)) return rc;
   CK(cudaMemsetAsync(d_bad, 0, 4, st));
@@ -495,6 +626,7 @@ int mlease_score_keyed(int32_t device, void* stream, int32_t Dg, int32_t K, cons
   const long long kpc = std::max<long long>(1, std::min<long long>(K, (long long)(std::min(SCORE_KEYED_TABLE_CAP, free_b / 4) / key_bytes)));
   float* d_table;
   if (int rc = t.get(&d_table, (size_t)kpc * key_bytes / sizeof(float), false)) return rc;
+  if (var) dvar.vtable = d_table + (size_t)kpc * key_bytes / 2 / sizeof(float);
   std::vector<long long> bounds{0};
   for (long long k0 = 0; k0 < K; k0 += kpc) {
     const int k1 = (int)std::min<long long>(K, k0 + kpc);
@@ -502,15 +634,36 @@ int mlease_score_keyed(int32_t device, void* stream, int32_t Dg, int32_t K, cons
     if (krs[k1] == krs[k0]) continue;
     for (int l0 = 0; l0 < L; l0 += 4)
       CK(score_keyed_chunk(Dg, K, (int)k0, k1, krs[k0], krs[k1], d_krs, d_rp, d_ci, d_v, d_o, std::min(4, L - l0), d_mp + (size_t)l0 * K,
-                           d_mc, d_mv, d_term + (size_t)l0 * K, binary_feature, nrows, 0, d_table, d_pred + (size_t)l0 * nrows, d_bad, st));
+                           d_mc, d_mv, d_term + (size_t)l0 * K, binary_feature, nrows, 0, d_table, d_pred + (size_t)l0 * nrows, d_bad,
+                           dvar.at(l0, K, nrows), st));
   }
   int bad = 0;
   CK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, st));
   if (!pred_dev) CK(cudaMemcpyAsync(pred, d_pred, (size_t)L * nrows * 4, cudaMemcpyDeviceToHost, st));
+  if (var && !pred_var_dev) CK(cudaMemcpyAsync(pred_var, dvar.pred_var, (size_t)L * nrows * 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   keyed_record(bounds, false, 0, 0);
-  if (bad) return fail(MLEASE_ERR_INVALID, "colidx out of range [0, num_features)");
-  return 0;
+  return keyed_bad(bad);
+}
+
+}  // namespace mlease
+
+extern "C" {
+
+int mlease_score_keyed(int32_t device, void* stream, int32_t Dg, int32_t K, const int64_t* key_rowstart, const int64_t* rowptr,
+                       const int32_t* colidx, const float* vals, const float* offset, int32_t L, const int64_t* model_ptr,
+                       const int32_t* model_col, const float* model_val, int32_t binary_feature, float* pred) {
+  return score_keyed(device, stream, Dg, K, key_rowstart, rowptr, colidx, vals, offset, L, model_ptr, model_col, model_val, nullptr, nullptr,
+                     nullptr, nullptr, binary_feature, pred, nullptr);
+}
+
+int mlease_score_keyed_var(int32_t device, void* stream, int32_t Dg, int32_t K, const int64_t* key_rowstart, const int64_t* rowptr,
+                           const int32_t* colidx, const float* vals, const float* offset, int32_t G, const int64_t* model_ptr,
+                           const int32_t* model_col, const float* model_val, const int64_t* var_ptr, const int32_t* var_col,
+                           const float* var_val, const float* var_default, int32_t binary_feature, float* pred, float* pred_var) {
+  if (!var_ptr) return fail(MLEASE_ERR_INVALID, "bad argument");
+  return score_keyed(device, stream, Dg, K, key_rowstart, rowptr, colidx, vals, offset, G, model_ptr, model_col, model_val, var_ptr, var_col,
+                     var_val, var_default, binary_feature, pred, pred_var);
 }
 
 int mlease_test_loglik_keyed(int32_t device, void* stream, int64_t n, const int32_t* entry_key, const int32_t* entry_group,

@@ -36,7 +36,7 @@ void keyed_record(const std::vector<long long>& bounds, bool streamed, double st
 extern "C" {
 
 // Test hooks, not part of the C ABI: mlease_internal_set_keyed_budget caps, process-wide, the device bytes the keyed calls
-// (mlease_naive_train*, mlease_item_model_train, mlease_score_keyed) plan with (0 = the free memory only), so that small inputs stream
+// (mlease_naive_train*, mlease_item_model_train, mlease_score_keyed[_var]) plan with (0 = the free memory only), so that small inputs stream
 // through many chunks.  mlease_internal_keyed_last_call reports the most recent keyed call of the process: the key boundaries of its
 // chunks (*count of them, the first 0 and the last K; up to cap are written), whether it streamed, and for a streamed fit the host
 // milliseconds its rows took to stage (copy into the pinned ring and H2D, all chunks) and the milliseconds the solve waited for them.

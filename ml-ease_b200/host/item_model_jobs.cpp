@@ -1,7 +1,6 @@
 // item_model_jobs.cpp -- ItemModelTest (jobs/ItemModelTest.java:53-248) and ItemModelTestLoglik (jobs/ItemModelTestLoglik.java:40-142):
 // per-key scoring of RegressionNaiveTrain's "<lambda>#<key>" models and one test log-likelihood per key.  Reached through
 // mlease_job_run (register_job).
-#include <atomic>
 #include <cmath>
 
 #include "jobs_common.hpp"
@@ -10,34 +9,6 @@ namespace mlease_jobs {
 namespace {
 
 // ============================================================================================ ItemModelTest
-// The records of one file as union-free bytes (transcode_plain), one string per record.  False when the schema or a record is
-// not plain; the generic encoder then writes the job's output.
-bool plain_records(const std::string& file, std::vector<std::string>& out) {
-  AvroFile af(file);
-  Plan plan;
-  try { plan = plan_build(*af.schema()); } catch (const std::exception&) { return false; }
-  {
-    const Plan* p = &plan;
-    while (p->type == Schema::Union) { const Plan* nx = nullptr; for (auto& k : p->kids) if (k.type != Schema::Null) { nx = &k; break; } if (!nx) return false; p = nx; }
-    if (p->type != Schema::Record) return false;
-  }
-  const size_t nb = af.num_blocks();
-  std::vector<std::vector<std::string>> parts(nb);
-  std::atomic<bool> plain{true};
-  parallel_blocks(nb, host_threads(), [&](size_t b) {
-    if (!plain.load()) return;
-    const std::string data = af.block_data(b);
-    const uint8_t* p = reinterpret_cast<const uint8_t*>(data.data());
-    const uint8_t* e = p + data.size();
-    try {
-      for (int64_t q = 0; q < af.block_records(b); q++) { std::string o; transcode_plain(plan, p, e, o); parts[b].push_back(std::move(o)); }
-    } catch (const NotPlain&) { plain.store(false); }
-  });
-  if (!plain.load()) return false;
-  for (auto& v : parts) for (auto& r : v) out.push_back(std::move(r));
-  return true;
-}
-
 // jobs/ItemModelTest.java:65-248.  Records are grouped by item key in Avro string order (unsigned bytes); inside a key they keep
 // input order (files in listing order, records in file order).  One mlease_score_keyed call scores every lambda.
 void run_item_model_test(const JobConfig& c) {
@@ -50,21 +21,12 @@ void run_item_model_test(const JobConfig& c) {
   Dictionary td; Rows rows;
   for (auto& f : files) read_raw(f, td, rows, ignore_value, itemKey);
   const size_t n = rows.n();
-  std::vector<size_t> order(n);
-  for (size_t i = 0; i < n; i++) order[i] = i;
-  std::stable_sort(order.begin(), order.end(), [&](size_t a, size_t b) { return rows.key[a] < rows.key[b]; });
-  std::vector<std::string> knames;
-  std::vector<int64_t> krs{0}, rp{0};
-  std::vector<int32_t> ci; std::vector<float> vv, oo;
-  for (size_t q = 0; q < n; q++) {
-    const size_t i = order[q];
-    if (q > 0 && rows.key[i] != rows.key[order[q - 1]]) krs.push_back((int64_t)q);
-    if (q == 0 || rows.key[i] != rows.key[order[q - 1]]) knames.push_back(rows.key[i]);
-    for (int64_t j = rows.rowptr[i]; j < rows.rowptr[i + 1]; j++) { ci.push_back(rows.colidx[j]); vv.push_back(rows.vals[j]); }
-    rp.push_back((int64_t)ci.size());
-    oo.push_back(rows.offset[i]);
-  }
-  if (n) krs.push_back((int64_t)n);
+  const KeyedRows kr(rows);
+  const std::vector<size_t>& order = kr.order;
+  const std::vector<std::string>& knames = kr.knames;
+  const std::vector<int64_t> &krs = kr.krs, &rp = kr.rp;
+  const std::vector<int32_t>& ci = kr.ci;
+  const std::vector<float> &vv = kr.vv, &oo = kr.oo;
   const int K = (int)knames.size();
   // model "String.valueOf(float lambda)#itemKey" (:187); its features mapped to the test dictionary, the ones the test data never
   // lists dropped (they cannot contribute), "(INTERCEPT)" to column Dg.  A key without a model gets the empty model (:189-197).
@@ -99,14 +61,8 @@ void run_item_model_test(const JobConfig& c) {
       const KeySlice s(krs, rp, k0, k1);
       const int Ks = k1 - k0;
       const int64_t ns = s.krs[Ks];
-      std::vector<int64_t> smp{0}; std::vector<int32_t> smc; std::vector<float> smv;
-      for (int l = 0; l < L; l++)
-        for (int k = k0; k < k1; k++) {
-          const size_t m = (size_t)l * K + k;
-          smc.insert(smc.end(), mc.begin() + mp[m], mc.begin() + mp[m + 1]);
-          smv.insert(smv.end(), mv.begin() + mp[m], mv.begin() + mp[m + 1]);
-          smp.push_back((int64_t)smc.size());
-        }
+      std::vector<int64_t> smp; std::vector<int32_t> smc; std::vector<float> smv;
+      slice_model_lists(mp, mc, mv, L, K, k0, k1, smp, smc, smv);
       std::vector<float> sp((size_t)L * ns);
       ck(mlease_score_keyed(dev, nullptr, Dg, Ks, s.krs.data(), s.rowptr.data(), ci.data() + s.nz0, vv.data() + s.nz0, oo.data() + s.row0, L,
                             smp.data(), smc.data(), smv.data(), ignore_value ? 1 : 0, sp.data()));

@@ -16,19 +16,6 @@ const char* SCHEMA_MODEL_WITH_VAR =
     "{\"name\":\"posteriorVar\",\"type\":{\"type\":\"array\",\"items\":{\"type\":\"record\",\"name\":\"featureVar\",\"fields\":["
     "{\"name\":\"name\",\"type\":\"string\"},{\"name\":\"term\",\"type\":\"string\"},{\"name\":\"value\",\"type\":\"float\"}]}}}]}";
 
-// intercept.lambdas / default.lambdas: Float.parseFloat of the comma list, in order, repeats kept (:313-321).  The reference divides
-// by every lambda (:262), so a lambda <= 0 or NaN is refused here instead of producing infinite prior variances.
-std::vector<float> lambda_list(const JobConfig& c, const std::string& key) {
-  std::vector<float> out;
-  for (auto& t : c.get_list(key)) {
-    const float v = std::stof(t);
-    if (!(v > 0.f)) io_error(key + ": every lambda must be > 0 (got " + t + ")");
-    out.push_back(v);
-  }
-  if (out.empty()) io_error(key + ": no lambda given");
-  return out;
-}
-
 // intercept.prior.mean.map: Pair records {key, value}, value = Double.parseDouble(value.toString()) (:293-301), so a float value
 // is read through its Float.toString digits
 std::unordered_map<std::string, double> read_prior_mean_map(const std::string& path) {

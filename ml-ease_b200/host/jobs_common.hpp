@@ -3,6 +3,7 @@
 // regression_jobs.cpp are reached by mlease_job_run.
 #pragma once
 #include <algorithm>
+#include <atomic>
 #include <exception>
 #include <fstream>
 #include <map>
@@ -162,8 +163,8 @@ std::vector<std::pair<std::string, float>> read_lambda_map_entries(const std::st
 // {name, term, value} feature record of a model list (Value tree), value cast to float
 Value feature_value(const std::string& key, float v);
 std::map<std::string, std::unordered_map<std::string, double>> read_linear_models(const std::string& path, bool last_wins = false);
-// RegressionTest-style output schema: input fields with unions removed + pred:float
-std::string test_output_schema(const SchemaP& in, const char* name = "AdmmTestOutput", const char* ns = nullptr);
+// RegressionTest-style output schema: input fields with unions removed + pred:float (+ predVar:float)
+std::string test_output_schema(const SchemaP& in, const char* name = "AdmmTestOutput", const char* ns = nullptr, bool pred_var = false);
 // a record's bytes with the union branch indices dropped; throws NotPlain when the record is not plain
 struct NotPlain {};
 void transcode_plain(const Plan& pl, const uint8_t*& p, const uint8_t* e, std::string& o);
@@ -172,7 +173,7 @@ void transcode_plain(const Plan& pl, const uint8_t*& p, const uint8_t* e, std::s
 std::vector<int32_t> gpu_devices(const JobConfig& c);
 
 // ------------------------------------------------------------------------------------------ keyed jobs on several GPUs
-// Keys are independent, so a keyed job (NaiveTrain, ItemModelTrain, ItemModelTest) cuts them into one contiguous range per device,
+// Keys are independent, so a keyed job (NaiveTrain, ItemModelTrain, ItemModelTest, ItemModelGridTest) cuts them into one contiguous range per device,
 // runs the single-device library call of each range on its own thread, and writes the results into disjoint slices of its output.
 //
 // shard_keys: cuts[s] .. cuts[s + 1] is shard s's key range, balanced by the estimated cost of a key, rows * (D + 1)^2 + nnz (a
@@ -223,6 +224,87 @@ template <class F> void run_shards(const std::vector<int32_t>& devs, const std::
   }
   for (auto& t : ts) t.join();
   for (auto& e : err) if (e) std::rethrow_exception(e);
+}
+
+// ------------------------------------------------------------------------------------------ ItemModelTest and ItemModelGridTest
+// The records of one file as union-free bytes (transcode_plain), one string per record.  False when the schema or a record is
+// not plain; the generic encoder then writes the job's output.
+inline bool plain_records(const std::string& file, std::vector<std::string>& out) {
+  AvroFile af(file);
+  Plan plan;
+  try { plan = plan_build(*af.schema()); } catch (const std::exception&) { return false; }
+  {
+    const Plan* p = &plan;
+    while (p->type == Schema::Union) { const Plan* nx = nullptr; for (auto& k : p->kids) if (k.type != Schema::Null) { nx = &k; break; } if (!nx) return false; p = nx; }
+    if (p->type != Schema::Record) return false;
+  }
+  const size_t nb = af.num_blocks();
+  std::vector<std::vector<std::string>> parts(nb);
+  std::atomic<bool> plain{true};
+  parallel_blocks(nb, host_threads(), [&](size_t b) {
+    if (!plain.load()) return;
+    const std::string data = af.block_data(b);
+    const uint8_t* p = reinterpret_cast<const uint8_t*>(data.data());
+    const uint8_t* e = p + data.size();
+    try {
+      for (int64_t q = 0; q < af.block_records(b); q++) { std::string o; transcode_plain(plan, p, e, o); parts[b].push_back(std::move(o)); }
+    } catch (const NotPlain&) { plain.store(false); }
+  });
+  if (!plain.load()) return false;
+  for (auto& v : parts) for (auto& r : v) out.push_back(std::move(r));
+  return true;
+}
+
+// Records grouped by item key in Avro string order (unsigned bytes), input order inside a key (jobs/ItemModelTest.java:65-248):
+// position q holds record order[q]; keys knames with their rows [krs[k], krs[k+1]) of the CSR (rp, ci, vv) and offsets oo.
+struct KeyedRows {
+  std::vector<size_t> order;
+  std::vector<std::string> knames;
+  std::vector<int64_t> krs{0}, rp{0};
+  std::vector<int32_t> ci;
+  std::vector<float> vv, oo;
+  explicit KeyedRows(const Rows& rows) {
+    const size_t n = rows.n();
+    order.resize(n);
+    for (size_t i = 0; i < n; i++) order[i] = i;
+    std::stable_sort(order.begin(), order.end(), [&](size_t a, size_t b) { return rows.key[a] < rows.key[b]; });
+    for (size_t q = 0; q < n; q++) {
+      const size_t i = order[q];
+      if (q > 0 && rows.key[i] != rows.key[order[q - 1]]) krs.push_back((int64_t)q);
+      if (q == 0 || rows.key[i] != rows.key[order[q - 1]]) knames.push_back(rows.key[i]);
+      for (int64_t j = rows.rowptr[i]; j < rows.rowptr[i + 1]; j++) { ci.push_back(rows.colidx[j]); vv.push_back(rows.vals[j]); }
+      rp.push_back((int64_t)ci.size());
+      oo.push_back(rows.offset[i]);
+    }
+    if (n) krs.push_back((int64_t)n);
+  }
+};
+
+// Lists of L x K models as a CSR over (l, key), m = l*K + k: the lists of keys [k0, k1) of every l, as their own CSR.
+inline void slice_model_lists(const std::vector<int64_t>& mp, const std::vector<int32_t>& mc, const std::vector<float>& mv, int L, int K,
+                              int k0, int k1, std::vector<int64_t>& smp, std::vector<int32_t>& smc, std::vector<float>& smv) {
+  smp.assign(1, 0); smc.clear(); smv.clear();
+  for (int l = 0; l < L; l++)
+    for (int k = k0; k < k1; k++) {
+      const size_t m = (size_t)l * K + k;
+      smc.insert(smc.end(), mc.begin() + mp[m], mc.begin() + mp[m + 1]);
+      smv.insert(smv.end(), mv.begin() + mp[m], mv.begin() + mp[m + 1]);
+      smp.push_back((int64_t)smc.size());
+    }
+}
+
+// intercept.lambdas / default.lambdas of ItemModelTrain: Float.parseFloat of the comma list, in order, repeats kept
+// (jobs/ItemModelTrain.java:313-321).  The reference divides by every lambda (:262), so a lambda <= 0 or NaN is refused instead of
+// producing infinite prior variances.
+inline std::vector<float> lambda_list(const JobConfig& c, const std::string& key) {
+  std::vector<float> out;
+  for (auto& t : c.get_list(key)) {
+    const float v = std::stof(t);
+    if (!(v > 0.f)) io_error(key + ": every lambda must be > 0 (got " + t + ")");
+    out.push_back(v);
+  }
+  if (out.empty()) io_error(key + ": no lambda given");
+  return out;
 }
 
 // job_class -> job for mlease_job_run; returns true (for use in a namespace-scope initializer)

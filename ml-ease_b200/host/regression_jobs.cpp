@@ -10,6 +10,7 @@
 //   RegressionNaiveTrain  jobs/RegressionNaiveTrain.java:99-415 (+ jobs/PartitionIdAssigner.java:41-101)
 //   ItemModelTest, ItemModelTestLoglik: item_model_jobs.cpp
 //   ItemModelTrain: item_model_train_job.cpp
+//   ItemModelGridTest (scores ItemModelTrain's grid models with their posterior variance): item_model_grid_test_job.cpp
 //   JobConfig             com/linkedin/mapred/JobConfig.java:50-224 (java .properties file)
 // Not mirrored: Hadoop job submission, HDFS, DistributedCache (local files only; is.local is implied).
 #include <algorithm>
@@ -577,11 +578,12 @@ void read_raw_generic(const std::string& file, Dictionary& dict, Rows& rows, boo
 
 // ------------------------------------------------------------------------------------------ RegressionTest output
 // output = input fields (unions removed, utils/Util.java:377-417) + pred (jobs/RegressionTest.java:198-236)
-std::string test_output_schema(const SchemaP& in, const char* name, const char* ns) {
+std::string test_output_schema(const SchemaP& in, const char* name, const char* ns, bool pred_var) {
   SchemaP os = std::make_shared<Schema>(*schema_remove_union(in));
   os->name = name;
   auto pf = std::make_shared<Schema>(); pf->type = Schema::Float;
   os->fields.emplace_back("pred", pf);
+  if (pred_var) os->fields.emplace_back("predVar", pf);
   std::map<std::string, bool> em;
   Json j = schema_to_json(os, em);
   if (ns) {
@@ -1342,7 +1344,7 @@ extern "C" {
 const char* mlease_job_last_error(void) { return g_job_err.c_str(); }
 
 // job_class: Regression | RegressionPrepare | RegressionAdmmTrain | RegressionTest | RegressionTestLoglik | RegressionNaiveTrain |
-// ItemModelTest | ItemModelTestLoglik | ItemModelTrain
+// ItemModelTest | ItemModelTestLoglik | ItemModelTrain | ItemModelGridTest
 // (the README's names AdmmPrepare / AdmmTrain / AdmmTest / AdmmTestLoglik / NaiveTrain are accepted as aliases).
 int mlease_job_run(const char* job_class, const char* config_path) {
   try {

@@ -415,6 +415,29 @@ def score_keyed(vals, key_rowstart, rowptr, colidx, num_features, model_ptr, mod
     return pred
 
 
+def score_keyed_var(vals, key_rowstart, rowptr, colidx, num_features, model_ptr, model_col, model_val, var_ptr, var_col, var_val,
+                    var_default, *, offset=None, binary_feature=False, device=0, stream=None, out=None, out_var=None):
+    """score_keyed with each record's predictive variance under the diagonal posterior of its model (ItemModelTrain, compute.var).
+    Rows must list strictly ascending columns.  Variance lists are a CSR over (grid point, key) like the models: entries
+    [var_ptr[m], var_ptr[m+1]) of var_col (ascending, num_features = intercept) / var_val; var_default[m] for every unlisted
+    column.  -> (pred [G, nrows] float32, pred_var [G, nrows] float32); an empty variance list gives NaN."""
+    krs, rp, ci, vals = _keep(key_rowstart, np.int64), _keep(rowptr, np.int64), _keep(colidx, np.int32), _keep(vals, np.float32)
+    mp, mc, mv = _keep(model_ptr, np.int64), _keep(model_col, np.int32), _keep(model_val, np.float32)
+    vp, vc, vv, vd = _keep(var_ptr, np.int64), _keep(var_col, np.int32), _keep(var_val, np.float32), _keep(var_default, np.float32)
+    K = len(krs) - 1
+    if K <= 0 or (len(mp) - 1) % K or len(vp) != len(mp) or len(vd) != len(mp) - 1:
+        raise ValueError("model_ptr and var_ptr must hold G * num_keys + 1 entries, var_default G * num_keys")
+    G = (len(mp) - 1) // K
+    n = len(rp) - 1
+    o = _keep(offset, np.float32)
+    pred = np.zeros((G, n), np.float32) if out is None else out
+    pred_var = np.zeros((G, n), np.float32) if out_var is None else out_var
+    check(lib().mlease_score_keyed_var(device, stream, int(num_features), K, ptr(krs), ptr(rp), ptr(ci), ptr(vals), ptr(o), G, ptr(mp),
+                                       ptr(mc), ptr(mv), ptr(vp), ptr(vc), ptr(vv), ptr(vd), int(bool(binary_feature)), ptr(pred),
+                                       ptr(pred_var)))
+    return pred, pred_var
+
+
 def test_loglik_keyed(entry_key, entry_group, response, pred, num_keys, weight=None, device=0, stream=None):
     """ItemModelTestLoglik (jobs/ItemModelTestLoglik.java:60-142): one entry per (record, pred-map key), combiner group per entry
     (non-decreasing) -> (float32 loglik [num_keys], float64 count [num_keys])."""
