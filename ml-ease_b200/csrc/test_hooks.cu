@@ -97,6 +97,88 @@ int mlease_internal_batch_hv(mlease_session* s, int32_t mode, const double* w, c
   return 0;
 }
 
+// Test hook, not part of the C ABI: one gradient pass over the session's ADMM batch (after begin()) through exactly the K1 kernels
+// batch_k1 runs for it.  Problem b (= local partition * L + lambda) is evaluated at float(w[b]) (Dt entries) when active[b] != 0; the
+// others are marked done before the launch, as problems that converged earlier are in an x-update.  skip_eval is cleared and the
+// pass emits its Gram operand (force_emit = 1).  The per-chunk partials are reduced by the fixed-order reduction of the solver.
+// Outputs (inactive problems: NaN): f_out[b] = the loss (fpart summed in chunk order), g_out[b] (Dt) = the data-term gradient without
+// the prior; if not NULL, sd_out = sqrt(d_i) of every problem's rows, problem after problem (csr_fx batches: sdvec), and xt_out = the
+// bf16 bits of the Xt operand, n x Dp per problem (dense and general-CSR batches).  info (8 + nprob ints): [0] kernel kind
+// (1 dense, 2 CSR fixed point, 3 CSR fixed point with column windows, 4 general CSR, 5 fused multi-lambda CSR), [1] G (dense), LP
+// (fused), beta in shared memory (fixed point, general CSR), [2] k1_dyn, [3] k1_grid, [4] rows per thread RT (dense), rows per
+// segment (fused), column window width (windows), [5] row slices nsl (dense), [6] nprob, [7] 0, [8 + b] Ctrl::k1_chunks of an
+// active problem (0 otherwise).  The batch's x-update state is consumed (every problem is left done): begin() again before iterating.
+int mlease_internal_batch_grad(mlease_session* s, const int32_t* active, const double* w, double* f_out, double* g_out, float* sd_out,
+                               uint16_t* xt_out, int32_t* info) {
+  if (!s || !active || !w || !f_out || !g_out || !info) return fail(MLEASE_ERR_INVALID, "null argument");
+  if (!s->batch || !s->begun) return fail(MLEASE_ERR_STATE, "mlease_admm_begin was not called");
+  Batch& B = *s->batch;
+  if (sd_out && !(B.csr && B.csr_fx)) return fail(MLEASE_ERR_INVALID, "sqrt(d) goes to sdvec only on CSR batches with sorted unique rows");
+  if (xt_out && B.csr && B.csr_fx) return fail(MLEASE_ERR_INVALID, "this batch emits no Xt operand (its Gram reads sdvec)");
+  CK(cudaSetDevice(s->cfg.device));
+  const int nprob = B.nprob, ldx = s->ldx, Dt = s->Dt;
+  std::vector<int32_t> inf(8 + (size_t)nprob, 0);
+  inf[2] = B.k1_dyn; inf[3] = B.k1_grid; inf[6] = nprob;
+  if (B.k1_fused) {
+    inf[0] = 5; inf[1] = B.k1f_LP; inf[4] = B.h[0].sg_rows;
+  } else if (B.csr && B.csr_fx) {
+    const int W = k1_csr_window(ldx);
+    inf[0] = W > 0 ? 3 : 2;
+    inf[1] = (W == 0 && (size_t)2 * (ldx + 32) * 4 + (size_t)ldx * 4 <= 220 * 1024) ? 1 : 0;   // as k1_csr_fx_launch decides
+    inf[4] = W;
+  } else if (B.csr) {
+    inf[0] = 4; inf[1] = (size_t)2 * ldx * 4 <= 200 * 1024 ? 1 : 0;   // as k1_launch decides
+  } else {
+    int R, S, G, cps; size_t smem;
+    if (!k1_dense_plan(ldx, &R, &S, &G, &smem, &cps)) return fail(MLEASE_ERR_INVALID, "no dense K1 plan for this width");
+    inf[0] = 1; inf[1] = G; inf[4] = G == 4 ? 4 : 8; inf[5] = R / inf[4];
+  }
+  std::vector<float> bf(ldx, 0.f);
+  for (int b = 0; b < nprob; b++) {
+    for (int k = 0; k < Dt; k++) bf[k] = (float)w[(size_t)b * Dt + k];
+    CK(cudaMemcpy(B.h[b].beta_tf, bf.data(), (size_t)ldx * sizeof(float), cudaMemcpyHostToDevice));
+  }
+  std::vector<Ctrl> c(nprob);
+  CK(cudaMemcpy(c.data(), B.d_ctrl, (size_t)nprob * sizeof(Ctrl), cudaMemcpyDeviceToHost));
+  for (int b = 0; b < nprob; b++) { c[b].done = active[b] ? 0 : 1; c[b].skip_eval = 0; c[b].cg_active = active[b] ? 1 : 0; c[b].k1_chunks = 0; }
+  CK(cudaMemcpy(B.d_ctrl, c.data(), (size_t)nprob * sizeof(Ctrl), cudaMemcpyHostToDevice));
+  int launches = 0;
+  CK(batch_k1(B, 1, s->stream, &launches));
+  CK(hv_reduce(B.d, nprob, Dt, 0, s->stream, &launches));
+  CK(cudaStreamSynchronize(s->stream));
+  CK(cudaMemcpy(c.data(), B.d_ctrl, (size_t)nprob * sizeof(Ctrl), cudaMemcpyDeviceToHost));
+  const double nan = std::nan("");
+  std::vector<double> fp;
+  size_t row0 = 0;
+  for (int b = 0; b < nprob; b++) {
+    const Problem& p = B.h[b];
+    const size_t n = (size_t)p.n;
+    if (active[b]) {
+      inf[8 + b] = c[b].k1_chunks;
+      fp.resize(std::max(1, c[b].k1_chunks));
+      CK(cudaMemcpy(fp.data(), p.fpart, (size_t)c[b].k1_chunks * sizeof(double), cudaMemcpyDeviceToHost));
+      double f = 0.0;
+      for (int t = 0; t < c[b].k1_chunks; t++) f += fp[t];
+      f_out[b] = f;
+      CK(cudaMemcpy(g_out + (size_t)b * Dt, p.g_t, (size_t)Dt * sizeof(double), cudaMemcpyDeviceToHost));
+      if (sd_out) CK(cudaMemcpy(sd_out + row0, p.sdvec, n * sizeof(float), cudaMemcpyDeviceToHost));
+      if (xt_out) CK(cudaMemcpy(xt_out + row0 * B.Dp, p.Xt, n * B.Dp * sizeof(uint16_t), cudaMemcpyDeviceToHost));
+    } else {
+      f_out[b] = nan;
+      std::fill(g_out + (size_t)b * Dt, g_out + (size_t)(b + 1) * Dt, nan);
+      if (sd_out) std::fill(sd_out + row0, sd_out + row0 + n, std::nanf(""));
+      if (xt_out) std::fill(xt_out + row0 * B.Dp, xt_out + (row0 + n) * B.Dp, (uint16_t)0x7FC0);   // bf16 NaN
+    }
+    row0 += n;
+  }
+  for (auto& x : c) { x.done = 1; x.cg_active = 0; }
+  CK(cudaMemcpy(B.d_ctrl, c.data(), (size_t)nprob * sizeof(Ctrl), cudaMemcpyHostToDevice));
+  B.mirror.clear();
+  s->cnt.launches += launches;
+  std::copy(inf.begin(), inf.end(), info);
+  return 0;
+}
+
 // Test hooks of the factored direction of wide systems (ldh > 2048), not part of the C ABI.  Each refuses, before any launch, a
 // batch that has no Ysym (ldh <= 2048, or matrix-free), since the kernels they run dereference it.
 //

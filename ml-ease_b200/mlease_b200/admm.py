@@ -525,6 +525,38 @@ def _internal_set_keyed_budget(nbytes):
     check(fn(int(nbytes)))
 
 
+K1_KINDS = {1: "dense", 2: "fx", 3: "fx_window", 4: "csr", 5: "fused"}
+
+
+def _internal_batch_grad(session, w, active=None, rows=None, want_sd=False, want_xt=False):
+    """Test hook (not part of the C ABI): one K1 gradient pass over the ADMM batch of `session` (after begin()), problem b =
+    partition * L + lambda at float(w[b]) when active[b] (default: all).  rows: the row count of each partition (needed for
+    want_sd / want_xt).  Consumes the batch's x-update state.
+    -> dict(f [nprob], g [nprob, Dt] (data term, no prior; NaN for inactive problems), sd (list of [n] float32 or None),
+    xt (list of [n, Dp] uint16 bf16 bits or None), kind, G (dense G / fused LP / beta in shared memory), dyn, grid, RT (dense rows
+    per thread / fused segment rows / column window), nsl, chunks [nprob])."""
+    nprob, Dt = session.num_blocks * session.L, session.Dt
+    w = np.ascontiguousarray(w, np.float64).reshape(nprob, Dt)
+    act = np.ones(nprob, np.int32) if active is None else np.ascontiguousarray(active, np.int32)
+    if len(act) != nprob:
+        raise ValueError("active must hold one entry per problem")
+    Dp = ((Dt + 3) // 4 * 4 + 127) // 128 * 128
+    n_b = [int(rows[b // session.L]) for b in range(nprob)] if (want_sd or want_xt) else None
+    f = np.zeros(nprob, np.float64)
+    g = np.zeros((nprob, Dt), np.float64)
+    sd = np.zeros(sum(n_b), np.float32) if want_sd else None
+    xt = np.zeros(sum(n_b) * Dp, np.uint16) if want_xt else None
+    info = np.zeros(8 + nprob, np.int32)
+    fn = lib().mlease_internal_batch_grad
+    fn.argtypes, fn.restype = [C.c_void_p] * 8, C.c_int
+    check(fn(session._h, act.ctypes.data, w.ctypes.data, f.ctypes.data, g.ctypes.data, ptr(sd), ptr(xt), info.ctypes.data))
+    split = np.cumsum([0] + (n_b or []))
+    return dict(f=f, g=g, sd=[sd[split[b]:split[b + 1]] for b in range(nprob)] if want_sd else None,
+                xt=[xt[split[b] * Dp:split[b + 1] * Dp].reshape(-1, Dp) for b in range(nprob)] if want_xt else None,
+                kind=K1_KINDS[int(info[0])], G=int(info[1]), dyn=int(info[2]), grid=int(info[3]), RT=int(info[4]), nsl=int(info[5]),
+                chunks=info[8:].copy())
+
+
 def _internal_keyed_last_call():
     """Test hook: the most recent keyed call of the process -> (key boundaries of its chunks, streamed, stage ms, wait ms)."""
     fn = lib().mlease_internal_keyed_last_call

@@ -76,15 +76,19 @@ def _part_csr(part, D):
 
 # (partitions, rows, features, stored values per row, lambdas, no segment lists): the ADMM batch of a policy-2 session through the
 # kernels its CG runs -- fused multi-lambda with 4- and 2-wide interleaved vectors, the per-problem fixed-point kernel with its
-# accumulators and v in shared memory (5 lambdas: no fused kernel) under the dynamic CTA mapping, and the column windows (2 lambdas
-# at 30 001 columns: no segment lists, see test_hessian_vector_matches_oracle)
+# accumulators and v in shared memory (5 lambdas: no fused kernel) under the dynamic CTA mapping, the same kernel reading v from
+# global memory (3 lambdas at 20 003 columns: the 4-wide interleaved vectors of the fused kernel do not fit), and the column windows
+# (2 lambdas at 30 001 columns: no segment lists, see test_hessian_vector_matches_oracle)
 @pytest.mark.parametrize("P,n,D,nnz,L,no_fused", [(2, 3000, 300, 12, 3, False), (2, 3000, 300, 12, 2, False), (2, 3000, 300, 12, 5, False),
-                                                  (2, 2000, 30001, 60, 2, True)])
+                                                  (1, 2000, 20003, 40, 3, True), (2, 2000, 30001, 60, 2, True)])
 def test_batch_hv_and_diagonal_match_oracle(mb, P, n, D, nnz, L, no_fused):
     """Every (partition, lambda) problem at its own point w and vector v: a wrong lambda's v or d, or a wrong diagonal, fails here (the
-    ADMM parity cases could not see it: any SPD model leads the line search to the same minimiser)."""
+    ADMM parity cases could not see it: any SPD model leads the line search to the same minimiser).  Each column is also held to the
+    bound of tests/k1_reference.py, with the pass's chunking as the gradient hook reports it for the same batch."""
     import ctypes as C
+    import k1_reference as kr
     from mlease_b200._native import lib, ptr, check
+    from mlease_b200.admm import _internal_batch_grad
     parts, _, _ = _sparse_parts(P, n, D, nnz, seed=D + L)
     rng = np.random.default_rng(L)
     nprob = P * L
@@ -98,6 +102,8 @@ def test_batch_hv_and_diagonal_match_oracle(mb, P, n, D, nnz, L, no_fused):
             s.add_partition_csr(p, *part)
         s.begin()
         assert s.stats()["k1_fused"] == (0 if no_fused or L > 4 else 1)
+        info = _internal_batch_grad(s, w)   # all problems, as in the Hv / diagonal passes: the same CTA mapping
+        assert info["kind"] == ("fused" if s.stats()["k1_fused"] else "fx_window" if D > 28000 else "fx")
         for mode, name in ((1, "Hv"), (2, "hessian_diag")):
             outs = []
             for rep in range(2):
@@ -110,6 +116,14 @@ def test_batch_hv_and_diagonal_match_oracle(mb, P, n, D, nnz, L, no_fused):
                 ref = orc.objective(name, data, w[b], np.zeros(D + 1), big, vec=v[b] if mode == 1 else None)
                 err = np.abs(outs[0][b] - ref).max() / np.abs(ref).max()
                 assert err <= 1e-5, (name, b, err)
+                rp, ci, vv, yy, ww, oo = parts[b // L]
+                part = kr.Part.from_csr(rp, ci, vv, yy, ww, oo, D)
+                rowl1 = np.float32(np.bincount(part.rows, np.abs(vv.astype(np.float64)), part.n).max() * (1 + 1e-5))
+                vinf = np.abs(v[b].astype(np.float32)).max()
+                ref64, bnd = kr.hv_reference_and_bound(part, w[b], v[b], mode, kr.plan_from_info(info, b, part.n), rowl1, vinf)
+                r = kr.ratio(outs[0][b] - ref64, bnd)
+                assert np.all(r <= 1.0), (name, b, int(np.argmax(r)), float(r.max()))
+                print("Hv bound %s %s L=%d D=%d: worst error/bound %.3e" % (name, info["kind"], L, D, r.max()))
 
 
 def test_policy2_session_builds_no_gram_list(mb):
