@@ -10,6 +10,7 @@
 // throughput-bound on the fp64 pipe.
 #include <algorithm>
 #include <cstdlib>
+#include <mutex>
 
 #include "kernels.cuh"
 
@@ -43,32 +44,32 @@ __global__ void chol_prep_kernel(const Problem* __restrict__ probs, int share) {
   pb.Lc[(size_t)i * ldh + j] = v;
 }
 
-// Panel step k, part 1: ONE warp per problem factorises the NBxNB diagonal block in registers and inverts it.
-// lane i holds row i; column j is scaled by lane-j's pivot and every L[kk][j] reaches the other rows by shuffle: ~500 double
-// shuffles + FMAs (a few microseconds) instead of 32 rounds of block-wide barriers.  This kernel and the two below are one link
-// of a chain of ldh/32 dependent steps: latency is what counts.  The factor and its inverse go to the side buffers Ldiag / Ldinv
-// (chol_finish_kernel copies the diagonal blocks back into Lc).
+// Panel step k: the diagonal block, then rows of L21 = A21 * L11^-T, RB rows at a time.
+// The NBxNB diagonal block is factorised in registers by one warp and inverted: lane i holds row i; column j is scaled by
+// lane-j's pivot and every L[kk][j] reaches the other rows by shuffle: ~500 double shuffles + FMAs instead of 32 rounds of
+// block-wide barriers.  Every CTA of the panel kernel repeats it in its warp 0 (the same instructions, so the same bits) while
+// its other warps stage the CTA's first rows of A21: the step is one launch, not two.  This kernel and chol_update_kernel are the
+// links of a chain of ldh/32 dependent steps: latency is what counts.  CTA 0 stores the factor and its inverse in the side
+// buffers Ldiag / Ldinv (chol_finish_kernel copies the diagonal blocks back into Lc; trinv_kernel reads Ldinv).
 constexpr int RB = 64;
-__global__ void __launch_bounds__(32) chol_diag_kernel(const Problem* __restrict__ probs, int k) {
-  const Problem& pb = probs[blockIdx.x];
-  Ctrl* c = pb.ctrl;
-  if (c->done || !c->need_hess) return;
-  __shared__ double A[NB][NB + 1];
+constexpr int PANEL_CTAS = 32;   // CTAs per problem at most (one per SM: 168 registers): each walks row blocks x, x + gridDim.x, ...
+__device__ __forceinline__ void chol_diag_block(const Problem& pb, int c0, bool store, double (&A)[NB][NB + 1], double (&Li)[NB][NB + 1],
+                                                double (&dinv)[NB]) {
   const int ldh = pb.ldh;
-  const int c0 = k * NB;
   const double* H = pb.Lc;
   const int lane = threadIdx.x;
   double a[NB];
 #pragma unroll
   for (int kk = 0; kk < NB; kk++) a[kk] = (kk <= lane) ? H[(size_t)(c0 + lane) * ldh + c0 + kk] : 0.0;
   int bad = 0;
-  double dinv[NB];   // 1 / L[j][j]: one rsqrt per pivot serves the column scaling here and the substitution below (no divisions)
+  // dinv[j] = 1 / L[j][j] (shared memory, every lane computes the same): one rsqrt per pivot serves the column scaling here and
+  // the substitution below (no divisions)
 #pragma unroll
   for (int j = 0; j < NB; j++) {
     double djj = __shfl_sync(0xffffffffu, a[j], j);
     if (!(djj > 0.0)) { bad = 1; djj = 1.0; }
     const double r = rsqrt(djj);
-    dinv[j] = r;
+    if (lane == j) dinv[j] = r;
     if (lane == j) a[j] = djj * r;
     else if (lane > j) a[j] = a[j] * r;
 #pragma unroll
@@ -80,53 +81,64 @@ __global__ void __launch_bounds__(32) chol_diag_kernel(const Problem* __restrict
 #pragma unroll
   for (int kk = 0; kk < NB; kk++) {
     A[lane][kk] = (kk <= lane) ? a[kk] : 0.0;
-    pb.Ldiag[(size_t)(c0 + lane) * NB + kk] = (kk <= lane) ? a[kk] : 0.0;
+    if (store) pb.Ldiag[(size_t)(c0 + lane) * NB + kk] = (kk <= lane) ? a[kk] : 0.0;
   }
   __syncwarp();
-  // inverse of the lower-triangular factor: lane cc solves column cc by forward substitution (A is read as a broadcast)
+  // inverse of the lower-triangular factor: lane cc solves column cc of Li by forward substitution (A is read as a broadcast,
+  // column cc of Li only by lane cc)
   {
     const int cc = lane;
-    double li[NB];
 #pragma unroll
     for (int i = 0; i < NB; i++) {
       double sacc = 0.0;
 #pragma unroll
       for (int kk = 0; kk < NB; kk++)
-        if (kk < i) sacc += A[i][kk] * li[kk];     // li[kk] = 0 for kk < cc
-      li[i] = i < cc ? 0.0 : (i == cc ? dinv[i] : -sacc * dinv[i]);
+        if (kk < i) sacc += A[i][kk] * Li[kk][cc];     // Li[kk][cc] = 0 for kk < cc
+      const double li = i < cc ? 0.0 : (i == cc ? dinv[i] : -sacc * dinv[i]);
+      Li[i][cc] = li;
+      if (store) pb.Ldinv[(size_t)(c0 + i) * NB + cc] = li;
     }
-#pragma unroll
-    for (int i = 0; i < NB; i++) pb.Ldinv[(size_t)(c0 + i) * NB + cc] = li[i];
   }
-  if (lane == 0 && bad) c->fail = 1;
+  if (store && lane == 0 && bad) pb.ctrl->fail = 1;
 }
 
-// Panel step k, part 2: rows of L21 = A21 * L11^-T, RB rows per CTA, with the inverse of the diagonal block from Ldinv.
 __global__ void __launch_bounds__(256) chol_panel_kernel(const Problem* __restrict__ probs, int k) {
   const Problem& pb = probs[blockIdx.y];
   Ctrl* c = pb.ctrl;
   if (c->done || !c->need_hess) return;
+  __shared__ double A[NB][NB + 1];
   __shared__ double Li[NB][NB + 1];
   __shared__ double P[RB][NB + 1];
+  __shared__ double dinv[NB];
   const int ldh = pb.ldh;
   const int c0 = k * NB;
   double* H = pb.Lc;
   const int tid = threadIdx.x;
-  const int r0 = c0 + NB + blockIdx.x * RB;
-  if (r0 >= ldh) return;
-  const int rows = min(RB, ldh - r0);
-  for (int e = tid; e < NB * NB; e += 256) Li[e / NB][e % NB] = pb.Ldinv[(size_t)(c0 + e / NB) * NB + e % NB];
-  for (int e = tid; e < rows * NB; e += 256) {
-    const int i = e / NB, j = e % NB;
-    P[i][j] = H[(size_t)(r0 + i) * ldh + c0 + j];
-  }
+  const int rfirst = c0 + NB + blockIdx.x * RB;
+  if (tid < 32) chol_diag_block(pb, c0, blockIdx.x == 0, A, Li, dinv);
+  else if (rfirst < ldh)
+    for (int e = tid - 32; e < min(RB, ldh - rfirst) * NB; e += 224) P[e / NB][e % NB] = H[(size_t)(rfirst + e / NB) * ldh + c0 + e % NB];
   __syncthreads();
-  for (int e = tid; e < rows * NB; e += 256) {
-    const int i = e / NB, j = e % NB;
-    double sacc = 0.0;
-    for (int kk = 0; kk <= j; kk++) sacc += P[i][kk] * Li[j][kk];   // (A21 * L11^-T)[i][j]
-    H[(size_t)(r0 + i) * ldh + c0 + j] = sacc;
+  for (int r0 = rfirst; r0 < ldh; r0 += gridDim.x * RB) {
+    const int rows = min(RB, ldh - r0);
+    if (r0 != rfirst) {
+      __syncthreads();   // every thread is done with the previous row block
+      for (int e = tid; e < rows * NB; e += 256) P[e / NB][e % NB] = H[(size_t)(r0 + e / NB) * ldh + c0 + e % NB];
+      __syncthreads();
+    }
+    for (int e = tid; e < rows * NB; e += 256) {
+      const int i = e / NB, j = e % NB;
+      double sacc = 0.0;
+      for (int kk = 0; kk <= j; kk++) sacc += P[i][kk] * Li[j][kk];   // (A21 * L11^-T)[i][j]
+      H[(size_t)(r0 + i) * ldh + c0 + j] = sacc;
+    }
   }
+}
+static void chol_panel_launch(const Problem* d_probs, int nprob, int ldh, int k, cudaStream_t st, int* launches) {
+  const int below = ldh - (k + 1) * NB;
+  const int gx = below > 0 ? std::min(PANEL_CTAS, (below + RB - 1) / RB) : 1;
+  chol_panel_kernel<<<dim3(gx, nprob), 256, 0, st>>>(d_probs, k);
+  if (launches) *launches += 1;
 }
 
 // Trailing update A22 -= L21 L21^T on lower-triangular TBxTB tiles.
@@ -326,15 +338,21 @@ __global__ void __launch_bounds__(256) hinv_syrk_kernel(const Problem* __restric
 
 // ------------------------------------------------------------------------------------------
 // Wide systems (ldh > 1000): the same factorisation / inverse / product, restructured so that almost all flops are
-// fp64 tensor-core GEMMs (DMMA m8n8k4) on 128x64 tiles with K chunks of 16 staged through shared memory:
+// fp64 tensor-core GEMMs (DMMA m16n8k4) with K chunks of 16 staged through shared memory:
 //   Cholesky : outer panels of WNB columns; inside a panel the NB=32 steps above (panel kernel + K=32 updates limited
-//              to the panel's columns), then one K=WNB trailing update             C -= A A^T      (mode 0)
+//              to the panel's columns), then one K=WNB trailing update C -= A A^T (syrk_kernel, 128x128 tiles)
+//              in two launches, the next panel's columns first (look-ahead, cholesky_launch_wide)
+//   (dgemm_kernel, 128x64 tiles:)
 //   Y = L^-1 : leaves of WLEAF columns by trinv_kernel, then pairwise merges bottom-up
 //              T = L21 * Y11 (mode 1, T in the Hinv buffer), Y21 = -Y22 * T          (mode 2)
 //   Hinv     : Y^T Y over k >= max(i, j)                                            (mode 3)
 // Operand tiles live in shared memory either [row][k] (stride 20) or [k][row] (stride tile+4), whichever matches the
 // contiguous direction in global memory; both strides are = 4 mod 16 doubles, which makes the DMMA fragment loads
 // (thread t: row t/4, k t%4) bank-conflict free.
+// m16n8k4 is two m8n8k4 stacked in M (rows g and g + 8 of a 16-row fragment, one B fragment) at twice the issue rate of the
+// m8n8k4 (tools/dmma_rate.cu: 67 vs 34 TFLOP/s on an H100 SXM at 700 W); every element still takes one 4-product DMMA step
+// per k4 chunk in ascending k from a zero accumulator, and tests/test_gpu_chol_wide.py checks that the two shapes agree bit for
+// bit.  The symmetric results (the trailing update, mode 3) launch their lower-triangle tiles only.
 // ------------------------------------------------------------------------------------------
 constexpr int WNB = 256;     // outer panel width of the wide Cholesky
 constexpr int WLEAF = 256;   // leaf size of the recursive inverse
@@ -342,25 +360,43 @@ constexpr int DM = 128, DN = 64, DK = 16;
 constexpr int DA_SZ = DM * 20 > DK * (DM + 4) ? DM * 20 : DK * (DM + 4);   // doubles per A stage
 constexpr int DB_SZ = DN * 20 > DK * (DN + 4) ? DN * 20 : DK * (DN + 4);
 constexpr size_t DGEMM_SMEM = (size_t)2 * (DA_SZ + DB_SZ) * sizeof(double);
+static_assert(DM == 2 * DN, "dgemm_tile: a 128x128 block of a symmetric result is two tiles");
 
 __device__ __forceinline__ void dmma_8x8x4(double& c0, double& c1, double a, double b) {
   asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};" : "+d"(c0), "+d"(c1) : "d"(a), "d"(b));
 }
+// rows g (c0, c1; a0) and g + 8 (c2, c3; a1) of a 16x8 tile, columns 2 tg, 2 tg + 1; b: (k tg, column g)
+__device__ __forceinline__ void dmma_16x8x4(double& c0, double& c1, double& c2, double& c3, double a0, double a1, double b) {
+  asm volatile("mma.sync.aligned.m16n8k4.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5}, {%6}, {%0,%1,%2,%3};"
+               : "+d"(c0), "+d"(c1), "+d"(c2), "+d"(c3) : "d"(a0), "d"(a1), "d"(b));
+}
+
+// Tile (i0, j0) of CTA x.  A symmetric result (M == N, lower triangle wanted) enumerates the 128x128 blocks bi >= bj, two
+// 64-column tiles each, so that no CTA is launched for the strictly upper part; returns false for a tile past N.
+__device__ __forceinline__ bool dgemm_tile(bool tri, int x, int M, int N, int& i0, int& j0) {
+  if (tri) {
+    const int t = x >> 1;
+    int bi = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
+    while (bi * (bi + 1) / 2 > t) bi--;
+    while ((bi + 1) * (bi + 2) / 2 <= t) bi++;
+    i0 = bi * DM;
+    j0 = (t - bi * (bi + 1) / 2) * DM + (x & 1) * DN;
+    return j0 < N;
+  }
+  const int tiles_n = (N + DN - 1) / DN;
+  i0 = (x / tiles_n) * DM; j0 = (x % tiles_n) * DN;
+  return i0 < M;
+}
 
 template <bool A_KC, bool B_KC>
-__global__ void __launch_bounds__(256, 2) dgemm_kernel(const Problem* __restrict__ probs, int mode, int p0, int p1) {
+__global__ void __launch_bounds__(256, 2) dgemm_kernel(const Problem* __restrict__ probs, int mode, int p0) {
   const Problem& pb = probs[blockIdx.z];
   Ctrl* ctl = pb.ctrl;
   if (ctl->done || !ctl->need_hess) return;
   const int ldh = pb.ldh;
   const double* A; const double* B; double* C;
   int M, N, K;
-  if (mode == 0) {            // trailing update after the outer panel at column p0 of width p1
-    const int c = p0, w = p1;
-    M = N = ldh - c - w; K = w;
-    A = B = pb.Lc + (size_t)(c + w) * ldh + c;
-    C = pb.Lc + (size_t)(c + w) * ldh + (c + w);
-  } else if (mode == 1 || mode == 2) {   // merge of the diagonal blocks [r0, r0+m) and [r0+m, r0+m+m2)
+  if (mode == 1 || mode == 2) {   // merge of the diagonal blocks [r0, r0+m) and [r0+m, r0+m+m2)
     const int m = p0, r0 = 2 * blockIdx.y * m;
     const int m2 = min(m, ldh - r0 - m);
     if (m2 <= 0) return;
@@ -381,10 +417,8 @@ __global__ void __launch_bounds__(256, 2) dgemm_kernel(const Problem* __restrict
     A = B = pb.Yinv;
     C = pb.Hinv;
   }
-  const int tiles_n = (N + DN - 1) / DN;
-  const int i0 = (blockIdx.x / tiles_n) * DM, j0 = (blockIdx.x % tiles_n) * DN;
-  if (i0 >= M) return;
-  if ((mode == 0 || mode == 3) && j0 >= i0 + DM) return;   // strictly upper tile of a symmetric result
+  int i0, j0;
+  if (!dgemm_tile(mode == 3, blockIdx.x, M, N, i0, j0)) return;
   int klo = 0, khi = K;
   if (mode == 1) klo = j0;                      // Y11 is lower triangular: Y11[k][j] = 0 for k < j
   if (mode == 2) khi = min(K, i0 + DM);         // Y22 is lower triangular: Y22[i][k] = 0 for k > i
@@ -460,9 +494,10 @@ __global__ void __launch_bounds__(256, 2) dgemm_kernel(const Problem* __restrict
           fb[f] = B_KC ? b[(wn + f * 8 + g) * 20 + k4 + tg] : b[(k4 + tg) * (DN + 4) + wn + f * 8 + g];
         }
 #pragma unroll
-        for (int fm = 0; fm < 4; fm++)
+        for (int fm = 0; fm < 4; fm += 2)
 #pragma unroll
-          for (int fn = 0; fn < 4; fn++) dmma_8x8x4(acc[fm][fn][0], acc[fm][fn][1], fa[fm], fb[fn]);
+          for (int fn = 0; fn < 4; fn++)
+            dmma_16x8x4(acc[fm][fn][0], acc[fm][fn][1], acc[fm + 1][fn][0], acc[fm + 1][fn][1], fa[fm], fa[fm + 1], fb[fn]);
       }
       if (more) sstore(buf ^ 1);
       __syncthreads();
@@ -479,11 +514,7 @@ __global__ void __launch_bounds__(256, 2) dgemm_kernel(const Problem* __restrict
       const int j = j0 + wn + fn * 8 + 2 * tg;
       if (j >= N) continue;
       const double v0 = acc[fm][fn][0], v1 = acc[fm][fn][1];
-      if (mode == 0) {
-        double* d = C + (size_t)i * ldh + j;
-        if (j + 1 <= i) { double2 o = *reinterpret_cast<double2*>(d); o.x -= v0; o.y -= v1; *reinterpret_cast<double2*>(d) = o; }
-        else if (j <= i) d[0] -= v0;
-      } else if (mode == 1) {
+      if (mode == 1) {
         *reinterpret_cast<double2*>(C + (size_t)i * ldh + j) = make_double2(v0, v1);
       } else if (mode == 2) {
         *reinterpret_cast<double2*>(C + (size_t)i * ldh + j) = make_double2(-v0, -v1);
@@ -496,7 +527,7 @@ __global__ void __launch_bounds__(256, 2) dgemm_kernel(const Problem* __restrict
 }
 
 template <bool A_KC, bool B_KC>
-static cudaError_t dgemm_launch(const Problem* d_probs, int nprob, int mode, int p0, int p1, int M, int N, int nmerge, cudaStream_t st,
+static cudaError_t dgemm_launch(const Problem* d_probs, int nprob, int mode, int p0, int M, int N, int nmerge, cudaStream_t st,
                                 int* launches) {
   {
     // the attribute is per device: set it once for every device this process launches on
@@ -509,10 +540,174 @@ static cudaError_t dgemm_launch(const Problem* d_probs, int nprob, int mode, int
       if (dev >= 0 && dev < 64) configured[dev] = true;
     }
   }
-  const int tiles = ((M + DM - 1) / DM) * ((N + DN - 1) / DN);
+  const int tm = (M + DM - 1) / DM;
+  const int tiles = mode == 3 ? tm * (tm + 1) : tm * ((N + DN - 1) / DN);   // see dgemm_tile
   if (tiles <= 0 || nmerge <= 0) return cudaSuccess;
-  dgemm_kernel<A_KC, B_KC><<<dim3(tiles, nmerge, nprob), 256, DGEMM_SMEM, st>>>(d_probs, mode, p0, p1);
+  dgemm_kernel<A_KC, B_KC><<<dim3(tiles, nmerge, nprob), 256, DGEMM_SMEM, st>>>(d_probs, mode, p0);
   if (launches) *launches += 1;
+  return cudaGetLastError();
+}
+
+// Trailing update after the outer panel [c, c + w) (w = WNB): C -= A A^T on the columns [o, o + n) of the trailing block, o = c + w
+// + off, rows o.. (the lower triangle of the n x n block at o and everything below it); A = rows o.. of the panel's columns.
+// 128x64 tiles, 8 warps of 32x32, two CTAs per SM, fed by a 3-stage cp.async ring (zero-filled past the matrix) with one barrier
+// per stage instead of dgemm_kernel's register-staged double buffer; the tile of C is prefetched into L2 at the start, since
+// with K = 256 a tile's read-modify-write of C is a third of its traffic.  (128x128 tiles, one CTA per SM, were slower on an
+// H100: 75 against 57 ms for the trailing updates of 4 problems of ldh 10016.)  Each element's accumulator starts at 0, takes
+// the k4 chunks in ascending k (one m16n8k4 each) and is subtracted from C once.
+constexpr int SY_T = 128, SY_TN = 64, SY_LD = DK + 4, SY_STAGES = 3;
+constexpr int SY_WM = 4;                           // warps along M
+constexpr int SY_FM = SY_T / SY_WM / 16;           // m16 fragments per warp
+constexpr int SY_STAGE = (SY_T + SY_TN) * SY_LD;   // doubles per stage (A tile, then B tile; [row][k], stride 20)
+constexpr size_t SYRK_SMEM = (size_t)SY_STAGES * SY_STAGE * sizeof(double);
+__device__ __forceinline__ void cp_async16(double* dst, const double* src, bool ok) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"((uint32_t)__cvta_generic_to_shared(dst)), "l"(src), "r"(ok ? 16 : 0)
+               : "memory");
+}
+__global__ void __launch_bounds__(256, 2) syrk_kernel(const Problem* __restrict__ probs, int c, int w, int off, int n) {
+  const Problem& pb = probs[blockIdx.z];
+  Ctrl* ctl = pb.ctrl;
+  if (ctl->done || !ctl->need_hess) return;
+  const int ldh = pb.ldh, o = c + w + off, M = ldh - o, N = n;
+  int i0, j0;
+  if (M == N) {   // the lower triangle: 128x128 blocks bi >= bj, 128 / SY_TN tiles each
+    const int t = blockIdx.x / (SY_T / SY_TN);
+    int bi = (int)((sqrt(8.0 * t + 1.0) - 1.0) * 0.5);
+    while (bi * (bi + 1) / 2 > t) bi--;
+    while ((bi + 1) * (bi + 2) / 2 <= t) bi++;
+    i0 = bi * SY_T; j0 = (t - bi * (bi + 1) / 2) * SY_T + (blockIdx.x % (SY_T / SY_TN)) * SY_TN;
+    if (j0 >= N) return;
+  } else {
+    const int tn = (N + SY_TN - 1) / SY_TN;
+    i0 = (blockIdx.x / tn) * SY_T; j0 = (blockIdx.x % tn) * SY_TN;
+    if (j0 >= i0 + SY_T) return;   // strictly upper
+  }
+  const double* A = pb.Lc + (size_t)o * ldh + c;
+  double* C = pb.Lc + (size_t)o * ldh + o;
+  extern __shared__ __align__(16) double sy_smem[];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int g = lane >> 2, tg = lane & 3;
+  const int wm = (warp % SY_WM) * (SY_T / SY_WM), wn = (warp / SY_WM) * 32;
+  // staging: thread t copies 16 bytes (k 2 (t & 7), + 1) of rows (t >> 3) + 32 q of each operand tile
+  const int sr = tid >> 3, sk = (tid & 7) * 2;
+  auto issue = [&](int kc) {
+    if (kc < w / DK) {
+      double* st = sy_smem + (kc % SY_STAGES) * SY_STAGE;
+#pragma unroll
+      for (int q = 0; q < SY_T / 32; q++) {
+        const int r = sr + 32 * q;
+        const bool oka = i0 + r < M;
+        cp_async16(st + r * SY_LD + sk, A + (size_t)(oka ? i0 + r : 0) * ldh + kc * DK + sk, oka);
+      }
+#pragma unroll
+      for (int q = 0; q < SY_TN / 32; q++) {
+        const int r = sr + 32 * q;
+        const bool okb = j0 + r < N;
+        cp_async16(st + (SY_T + r) * SY_LD + sk, A + (size_t)(okb ? j0 + r : 0) * ldh + kc * DK + sk, okb);
+      }
+    }
+    asm volatile("cp.async.commit_group;" ::: "memory");
+  };
+  // the tile of C is read back only after the last K chunk: ask for it in L2 now, so that the epilogue does not wait on HBM
+  for (int e = tid; e < SY_T * (SY_TN / 16); e += 256) {   // 128-byte lines: SY_TN / 16 per row
+    const int r = e / (SY_TN / 16), q = e % (SY_TN / 16);
+    if (i0 + r < M && j0 + q * 16 < N && j0 + q * 16 <= i0 + r)
+      asm volatile("prefetch.global.L2 [%0];" ::"l"(C + (size_t)(i0 + r) * ldh + j0 + q * 16));
+  }
+  double acc[SY_FM][4][4];
+#pragma unroll
+  for (int a = 0; a < SY_FM; a++)
+#pragma unroll
+    for (int b = 0; b < 4; b++)
+#pragma unroll
+      for (int e = 0; e < 4; e++) acc[a][b][e] = 0.0;
+  issue(0);
+  issue(1);
+  for (int kc = 0; kc < w / DK; kc++) {
+    asm volatile("cp.async.wait_group 1;" ::: "memory");   // this thread's copies of stage kc have landed
+    __syncthreads();                                       // everyone's have, and stage kc - 1 is no longer read
+    issue(kc + 2);
+    const double* a = sy_smem + (kc % SY_STAGES) * SY_STAGE;
+    const double* b = a + SY_T * SY_LD;
+#pragma unroll
+    for (int k4 = 0; k4 < DK; k4 += 4) {
+      double fa[SY_FM][2], fb[4];
+#pragma unroll
+      for (int f = 0; f < SY_FM; f++) {
+        fa[f][0] = a[(wm + f * 16 + g) * SY_LD + k4 + tg];
+        fa[f][1] = a[(wm + f * 16 + 8 + g) * SY_LD + k4 + tg];
+      }
+#pragma unroll
+      for (int f = 0; f < 4; f++) fb[f] = b[(wn + f * 8 + g) * SY_LD + k4 + tg];
+#pragma unroll
+      for (int fm = 0; fm < SY_FM; fm++)
+#pragma unroll
+        for (int fn = 0; fn < 4; fn++)
+          dmma_16x8x4(acc[fm][fn][0], acc[fm][fn][1], acc[fm][fn][2], acc[fm][fn][3], fa[fm][0], fa[fm][1], fb[fn]);
+    }
+  }
+  asm volatile("cp.async.wait_group 0;" ::: "memory");
+#pragma unroll
+  for (int fm = 0; fm < SY_FM; fm++)
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      const int i = i0 + wm + fm * 16 + 8 * h + g;
+      if (i >= M) continue;
+#pragma unroll
+      for (int fn = 0; fn < 4; fn++) {
+        const int j = j0 + wn + fn * 8 + 2 * tg;
+        if (j >= N) continue;
+        const double v0 = acc[fm][fn][2 * h], v1 = acc[fm][fn][2 * h + 1];
+        double* d = C + (size_t)i * ldh + j;
+        if (j + 1 <= i) { double2 x = *reinterpret_cast<double2*>(d); x.x -= v0; x.y -= v1; *reinterpret_cast<double2*>(d) = x; }
+        else if (j <= i) d[0] -= v0;
+      }
+    }
+}
+static cudaError_t syrk_launch(const Problem* d_probs, int nprob, int c, int w, int off, int n, int M, cudaStream_t st, int* launches) {
+  {
+    static bool configured[64] = {};   // per device, as in dgemm_launch
+    int dev = 0;
+    cudaGetDevice(&dev);
+    if (dev < 0 || dev >= 64 || !configured[dev]) {
+      cudaError_t e = cudaFuncSetAttribute(syrk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SYRK_SMEM);
+      if (e != cudaSuccess) return e;
+      if (dev >= 0 && dev < 64) configured[dev] = true;
+    }
+  }
+  const int tm = (M + SY_T - 1) / SY_T;
+  const int tiles = M == n ? tm * (tm + 1) / 2 * (SY_T / SY_TN) : tm * ((n + SY_TN - 1) / SY_TN);
+  if (tiles <= 0) return cudaSuccess;
+  syrk_kernel<<<dim3(tiles, 1, nprob), 256, SYRK_SMEM, st>>>(d_probs, c, w, off, n);
+  if (launches) *launches += 1;
+  return cudaGetLastError();
+}
+
+// Test support (mlease_internal_dmma_shapes): for n 16x8 tiles, D = A B^T with A [n][16][K], B [n][8][K] (row-major), accumulated
+// the way dgemm_kernel accumulates -- zero start, one DMMA per k4 chunk, k ascending -- once as two m8n8k4 per chunk (D8) and once
+// as one m16n8k4 (D16).  One warp per tile.
+__global__ void __launch_bounds__(32) dmma_shapes_kernel(const double* __restrict__ A, const double* __restrict__ B, int K,
+                                                         double* __restrict__ D8, double* __restrict__ D16) {
+  const int t = blockIdx.x, g = threadIdx.x >> 2, tg = threadIdx.x & 3;
+  const double* a = A + (size_t)t * 16 * K;
+  const double* b = B + (size_t)t * 8 * K;
+  double p[4] = {0.0, 0.0, 0.0, 0.0}, q[4] = {0.0, 0.0, 0.0, 0.0};
+  for (int k = 0; k < K; k += 4) {
+    const double a0 = a[g * K + k + tg], a1 = a[(g + 8) * K + k + tg], bb = b[g * K + k + tg];
+    dmma_8x8x4(p[0], p[1], a0, bb);
+    dmma_8x8x4(p[2], p[3], a1, bb);
+    dmma_16x8x4(q[0], q[1], q[2], q[3], a0, a1, bb);
+  }
+  for (int h = 0; h < 2; h++)
+    for (int e = 0; e < 2; e++) {
+      const size_t o = (size_t)t * 128 + (g + 8 * h) * 8 + 2 * tg + e;
+      D8[o] = p[2 * h + e];
+      D16[o] = q[2 * h + e];
+    }
+}
+cudaError_t dmma_shapes(const double* A, const double* B, int n, int K, double* D8, double* D16, cudaStream_t st) {
+  if (n <= 0 || K <= 0 || K % 4) return cudaErrorInvalidValue;
+  dmma_shapes_kernel<<<n, 32, 0, st>>>(A, B, K, D8, D16);
   return cudaGetLastError();
 }
 
@@ -713,25 +908,70 @@ __global__ void __launch_bounds__(256) ysym_kernel(const Problem* __restrict__ p
 
 bool cholesky_factored_direction(int ldh) { return ldh > 2048; }   // = the problems that carry Ysym (batch_alloc)
 
+// The look-ahead's second stream and its fork / join events, one set per device.  The stream has the highest priority: the panel
+// chain is latency-bound, and its CTAs take the SM slots the trailing update frees before that update's next CTAs do.
+struct ChainStream {
+  cudaStream_t s = nullptr;
+  cudaEvent_t fork = nullptr, join = nullptr;
+};
+static std::mutex chain_mu;   // held while a factorisation is enqueued: the events are shared by every caller on the device
+static cudaError_t chain_stream(ChainStream** out) {
+  static ChainStream per_dev[64];
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  if (dev < 0 || dev >= 64) return cudaErrorInvalidDevice;
+  ChainStream& cs = per_dev[dev];
+  if (!cs.s) {
+    int lo = 0, hi = 0;
+    if ((e = cudaDeviceGetStreamPriorityRange(&lo, &hi)) != cudaSuccess) return e;
+    if ((e = cudaEventCreateWithFlags(&cs.fork, cudaEventDisableTiming)) != cudaSuccess) return e;
+    if ((e = cudaEventCreateWithFlags(&cs.join, cudaEventDisableTiming)) != cudaSuccess) return e;
+    if ((e = cudaStreamCreateWithPriority(&cs.s, cudaStreamNonBlocking, hi)) != cudaSuccess) return e;
+  }
+  *out = &cs;
+  return cudaSuccess;
+}
+
+// The NB = 32 steps inside the outer panel [c, c + w): panel kernel, then the K = 32 update of the panel's remaining columns.
+static cudaError_t panel_chain(const Problem* d_probs, int nprob, int ldh, int c, int w, cudaStream_t st, int* launches) {
+  for (int k = c / NB; k < (c + w) / NB; k++) {
+    chol_panel_launch(d_probs, nprob, ldh, k, st, launches);
+    const int below = ldh - (k + 1) * NB;
+    const int inner = c + w - (k + 1) * NB;   // panel columns still to be updated
+    if (inner > 0) {
+      chol_update_kernel<<<dim3((inner + TB - 1) / TB, (below + TB - 1) / TB, nprob), 256, 0, st>>>(d_probs, k, c + w);
+      if (launches) *launches += 1;
+    }
+  }
+  return cudaGetLastError();
+}
+
 static cudaError_t cholesky_launch_wide(const Problem* d_probs, int nprob, int ldh, cudaStream_t st, int* launches, bool factored_direction) {
   cudaError_t e;
-  // ---- factorisation
-  for (int c = 0; c < ldh; c += WNB) {
-    const int w = std::min(WNB, ldh - c);
-    for (int k = c / NB; k < (c + w) / NB; k++) {
-      const int below = ldh - (k + 1) * NB;
-      const int gx = below > 0 ? (below + RB - 1) / RB : 1;
-      chol_diag_kernel<<<nprob, 32, 0, st>>>(d_probs, k);
-      if (below > 0) chol_panel_kernel<<<dim3(gx, nprob), 256, 0, st>>>(d_probs, k);
-      if (launches) *launches += 2;
-      const int inner = c + w - (k + 1) * NB;   // panel columns still to be updated
-      if (inner > 0) {
-        chol_update_kernel<<<dim3((inner + TB - 1) / TB, (below + TB - 1) / TB, nprob), 256, 0, st>>>(d_probs, k, c + w);
-        if (launches) *launches += 1;
+  // ---- factorisation, with a look-ahead of one outer panel: the trailing update after panel c first updates the columns of
+  // panel c + 1 (all rows below), then the chain of panel c + 1 runs on the second stream while the rest of that update runs
+  // on st.  The two write disjoint columns and read the finished panel c, and st waits for the chain before the next trailing
+  // update, so every element takes the same subtractions in the same order as with no look-ahead.
+  {
+    std::lock_guard<std::mutex> lock(chain_mu);
+    ChainStream* cs = nullptr;
+    if ((e = chain_stream(&cs)) != cudaSuccess) return e;
+    if ((e = panel_chain(d_probs, nprob, ldh, 0, std::min(WNB, ldh), st, launches)) != cudaSuccess) return e;
+    for (int c = 0; c + WNB < ldh; c += WNB) {
+      const int w = WNB, rest = ldh - c - w, nw = std::min(WNB, rest);
+      if ((e = syrk_launch(d_probs, nprob, c, w, 0, nw, rest, st, launches)) != cudaSuccess) return e;
+      if (rest == nw) {   // the last panel: nothing left to overlap with
+        if ((e = panel_chain(d_probs, nprob, ldh, c + w, nw, st, launches)) != cudaSuccess) return e;
+        continue;
       }
+      if ((e = cudaEventRecord(cs->fork, st)) != cudaSuccess) return e;
+      if ((e = cudaStreamWaitEvent(cs->s, cs->fork, 0)) != cudaSuccess) return e;
+      if ((e = panel_chain(d_probs, nprob, ldh, c + w, nw, cs->s, launches)) != cudaSuccess) return e;
+      if ((e = cudaEventRecord(cs->join, cs->s)) != cudaSuccess) return e;
+      if ((e = syrk_launch(d_probs, nprob, c, w, nw, rest - nw, rest - nw, st, launches)) != cudaSuccess) return e;
+      if ((e = cudaStreamWaitEvent(st, cs->join, 0)) != cudaSuccess) return e;
     }
-    const int rest = ldh - c - w;
-    if (rest > 0 && (e = dgemm_launch<true, true>(d_probs, nprob, 0, c, w, rest, rest, 1, st, launches)) != cudaSuccess) return e;
   }
   // ---- inverse: leaves, then merges
   trinv_kernel<64><<<dim3((ldh + 63) / 64, nprob), 256, 0, st>>>(d_probs, WLEAF);
@@ -746,8 +986,8 @@ static cudaError_t cholesky_launch_wide(const Problem* d_probs, int nprob, int l
       if ((e = merge_tf32_launch(d_probs, nprob, 2, m, nmerge, st, launches)) != cudaSuccess) return e;
       continue;
     }
-    if ((e = dgemm_launch<true, false>(d_probs, nprob, 1, m, 0, m, m, nmerge, st, launches)) != cudaSuccess) return e;
-    if ((e = dgemm_launch<true, false>(d_probs, nprob, 2, m, 0, m, m, nmerge, st, launches)) != cudaSuccess) return e;
+    if ((e = dgemm_launch<true, false>(d_probs, nprob, 1, m, m, m, nmerge, st, launches)) != cudaSuccess) return e;
+    if ((e = dgemm_launch<true, false>(d_probs, nprob, 2, m, m, m, nmerge, st, launches)) != cudaSuccess) return e;
   }
   if (factored_direction) {
     ysym_kernel<<<dim3(ldh / 32, ldh / 32, nprob), 256, 0, st>>>(d_probs);
@@ -755,7 +995,7 @@ static cudaError_t cholesky_launch_wide(const Problem* d_probs, int nprob, int l
     return cudaGetLastError();
   }
   // ---- Hinv = Y^T Y
-  return dgemm_launch<false, false>(d_probs, nprob, 3, 0, 0, ldh, ldh, 1, st, launches);
+  return dgemm_launch<false, false>(d_probs, nprob, 3, 0, ldh, ldh, 1, st, launches);
 }
 
 // Cold start of a multi-lambda run with equal rho: the L problems of a partition have the same H = G + rho I, so only
@@ -844,10 +1084,7 @@ cudaError_t cholesky_launch(const Problem* d_probs, int nprob, int ldh, cudaStre
   } else {
     for (int k = 0; k < nb; k++) {
       const int below = ldh - (k + 1) * NB;
-      const int gx = below > 0 ? (below + RB - 1) / RB : 1;
-      chol_diag_kernel<<<nprob, 32, 0, st>>>(d_probs, k);
-      if (below > 0) chol_panel_kernel<<<dim3(gx, nprob), 256, 0, st>>>(d_probs, k);
-      if (launches) *launches += 2;
+      chol_panel_launch(d_probs, nprob, ldh, k, st, launches);
       if (below > 0) {
         const int T = (below + TB - 1) / TB;
         chol_update_kernel<<<dim3(T, T, nprob), 256, 0, st>>>(d_probs, k, ldh);

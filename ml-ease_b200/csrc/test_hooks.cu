@@ -313,4 +313,21 @@ int mlease_internal_csr_gram(mlease_session* s, int32_t* batch_kind, int32_t* sc
   return 0;
 }
 
+// Test hook, not part of the C ABI: on the current device, n 16x8 tiles D = A B^T (A: n x 16 x K, B: n x 8 x K, row-major,
+// K a multiple of 4) accumulated as dgemm_kernel accumulates, once through DMMA m8n8k4 (D8) and once through m16n8k4 (D16).
+int mlease_internal_dmma_shapes(const double* A, const double* B, int32_t n, int32_t K, double* D8, double* D16) {
+  if (!A || !B || !D8 || !D16 || n <= 0 || K <= 0 || K % 4) return fail(MLEASE_ERR_INVALID, "bad argument");
+  const size_t na = (size_t)n * 16 * K, nb = (size_t)n * 8 * K, nd = (size_t)n * 128;
+  double* d = nullptr;
+  CK(cudaMalloc(&d, (na + nb + 2 * nd) * sizeof(double)));
+  cudaError_t e = cudaMemcpy(d, A, na * sizeof(double), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(d + na, B, nb * sizeof(double), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = dmma_shapes(d, d + na, n, K, d + na + nb, d + na + nb + nd, 0);
+  if (e == cudaSuccess) e = cudaMemcpy(D8, d + na + nb, nd * sizeof(double), cudaMemcpyDeviceToHost);
+  if (e == cudaSuccess) e = cudaMemcpy(D16, d + na + nb + nd, nd * sizeof(double), cudaMemcpyDeviceToHost);
+  cudaFree(d);
+  CK(e);
+  return 0;
+}
+
 }  // extern "C"
