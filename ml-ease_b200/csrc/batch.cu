@@ -297,6 +297,29 @@ cudaError_t batch_k1(Batch& B, int force_emit, cudaStream_t st, int* launches, i
   return k1_launch(B.d, B.nprob, B.csr, B.ldx, B.has_bias, B.k1_grid, force_emit, st, launches, B.csr_fx, B.k1_dyn, mode);
 }
 
+// The factorisation of a rebuild slot over d_hess[0 .. n_hess) (the whole batch, or poll2_kernel's compacted copies).  share =
+// group_L > 1 (cold start, d_hess = B.d): every problem's H is its group leader's Gram + its own diag(q); share_fact (equal rho
+// too): only the leaders factorise, the followers take the leader's outcome and a copy of its H^-1.  skip_prep: Lc already holds H.
+int batch_factor(Batch& B, const Problem* d_hess, int n_hess, int share, bool share_fact, int skip_prep, cudaStream_t st, int* launches) {
+  // a follower still on a shared factor whose owner refactorises here takes a copy of the owner's bytes first
+  if (B.ysym_shared) CK(cholesky_detach_followers(B.d, B.nprob, B.ldh, st, launches));
+  if (share_fact) CK(cholesky_share_begin(B.d, B.nprob, share, st, launches));
+  CK(cholesky_launch(d_hess, n_hess, B.ldh, st, launches, share, skip_prep));
+  if (share_fact) {
+    CK(cholesky_share_end(B.d, B.nprob, share, st, launches));
+    if (cholesky_factored_direction(B.ldh)) B.ysym_shared = true;
+    const size_t hh = (size_t)B.ldh * B.ldh;
+    for (int b = 0; b < B.nprob; b++) {
+      if (b % share == 0) continue;
+      const Problem& lead = B.h[b - b % share];
+      // wide systems work on the factored form Y = L^-1 (bf16, Ysym): that is all a follower needs
+      if (!cholesky_factored_direction(B.ldh)) CK(cudaMemcpyAsync(B.h[b].Hinv, lead.Hinv, hh * sizeof(double), cudaMemcpyDeviceToDevice, st));
+      // (Ysym is not copied: chol_share_end_kernel points the follower's Ctrl::ysym_use at the leader's)
+    }
+  }
+  return 0;
+}
+
 // One x-update for every problem of the batch: beta (init), m, q must already be on the device.
 int batch_xupdate(Batch& B, cudaStream_t st, double xtol, int max_newton, int policy, int invalidate, int* h_flag, int* d_flag,
                   Counters& cnt, Profiler* prof, int share_first_gram, int share_first_factor) {
@@ -364,22 +387,7 @@ int batch_xupdate(Batch& B, cudaStream_t st, double xtol, int max_newton, int po
       pf.end(st);
       pf.begin(3, st);
       const bool share_fact = share > 1 && share_first_factor;   // same rho too: same H, one factorisation per group
-      // a follower still on a shared factor whose owner refactorises here takes a copy of the owner's bytes first
-      if (B.ysym_shared) CK(cholesky_detach_followers(B.d, B.nprob, B.ldh, st, &launches));
-      if (share_fact) CK(cholesky_share_begin(B.d, B.nprob, share, st, &launches));
-      CK(cholesky_launch(d_hess, n_hess, B.ldh, st, &launches, share));
-      if (share_fact) {
-        CK(cholesky_share_end(B.d, B.nprob, share, st, &launches));
-        if (cholesky_factored_direction(B.ldh)) B.ysym_shared = true;
-        const size_t hh = (size_t)B.ldh * B.ldh;
-        for (int b = 0; b < B.nprob; b++) {
-          if (b % share == 0) continue;
-          const Problem& lead = B.h[b - b % share];
-          // wide systems work on the factored form Y = L^-1 (bf16, Ysym): that is all a follower needs
-          if (!cholesky_factored_direction(B.ldh)) CK(cudaMemcpyAsync(B.h[b].Hinv, lead.Hinv, hh * sizeof(double), cudaMemcpyDeviceToDevice, st));
-          // (Ysym is not copied: chol_share_end_kernel points the follower's Ctrl::ysym_use at the leader's)
-        }
-      }
+      if (int rc = batch_factor(B, d_hess, n_hess, share, share_fact, 0, st, &launches)) return rc;
       pf.end(st);
     }
     if (B.matfree)

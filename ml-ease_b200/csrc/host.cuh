@@ -158,6 +158,7 @@ struct Profiler {
 int batch_alloc(Batch& B, int num_sms, int hessian_policy, int csr_gram_force = 0);
 cudaError_t batch_gram(const Batch& B, const Problem* d_probs, int n, int force, cudaStream_t st, int* launches, int share = 0);
 cudaError_t batch_k1(Batch& B, int force_emit, cudaStream_t st, int* launches, int mode = K1_GRAD);
+int batch_factor(Batch& B, const Problem* d_hess, int n_hess, int share, bool share_fact, int skip_prep, cudaStream_t st, int* launches);
 int batch_xupdate(Batch& B, cudaStream_t st, double xtol, int max_newton, int policy, int invalidate, int* h_flag, int* d_flag,
                   Counters& cnt, Profiler* prof = nullptr, int share_first_gram = 0, int share_first_factor = 0);
 

@@ -1070,12 +1070,18 @@ cudaError_t cholesky_share_end(const Problem* d_probs, int nprob, int share, cud
 // skip_prep: Lc already holds H (lower triangle + diag(q) + identity padding), e.g. the exact fp64 Hessian of k6_postvar.cu
 // want_hinv: the caller reads the explicit H^-1 afterwards (posterior variance, the inverse parity test): wide systems then run
 // the Y^T Y product even where the solver's direction works on the factored form (see ysym_kernel).
+cudaError_t cholesky_prep(const Problem* d_probs, int nprob, int ldh, int share, cudaStream_t st, int* launches) {
+  dim3 blk(32, 8);
+  dim3 grd((ldh + 31) / 32, (ldh + 7) / 8, nprob);
+  chol_prep_kernel<<<grd, blk, 0, st>>>(d_probs, share);
+  if (launches) *launches += 1;
+  return cudaGetLastError();
+}
+
 cudaError_t cholesky_launch(const Problem* d_probs, int nprob, int ldh, cudaStream_t st, int* launches, int share, int skip_prep, int want_hinv) {
   if (!skip_prep) {
-    dim3 blk(32, 8);
-    dim3 grd((ldh + 31) / 32, (ldh + 7) / 8, nprob);
-    chol_prep_kernel<<<grd, blk, 0, st>>>(d_probs, share);
-    if (launches) *launches += 1;
+    cudaError_t e = cholesky_prep(d_probs, nprob, ldh, share, st, launches);
+    if (e != cudaSuccess) return e;
   }
   const int nb = ldh / NB;
   if (ldh > CHOL_WIDE_MIN) {

@@ -65,6 +65,8 @@ cudaError_t gram_launch_simt(const Problem* d_probs, int nprob, int Dp, int forc
 // K3 (k3_cholesky.cu)
 cudaError_t cholesky_launch(const Problem* d_probs, int nprob, int ldh, cudaStream_t st, int* launches, int share = 0, int skip_prep = 0,
                             int want_hinv = 0);
+// the first launch of cholesky_launch: Lc = sum of the Gram partials (the group leader's when share > 1) + diag(q), identity padding
+cudaError_t cholesky_prep(const Problem* d_probs, int nprob, int ldh, int share, cudaStream_t st, int* launches);
 // test support: the same fp64 products through DMMA m8n8k4 and m16n8k4 (k3_cholesky.cu, mlease_internal_dmma_shapes)
 cudaError_t dmma_shapes(const double* A, const double* B, int n, int K, double* D8, double* D16, cudaStream_t st);
 bool cholesky_factored_direction(int ldh);   // wide systems: Ysym holds Y = L^-1 (bf16, symmetric storage), the direction is Y^T (Y q)

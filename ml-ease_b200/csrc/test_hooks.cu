@@ -179,6 +179,232 @@ int mlease_internal_batch_grad(mlease_session* s, const int32_t* active, const d
   return 0;
 }
 
+// Test hook, not part of the C ABI: one factorisation of the session's ADMM batch (after begin()) with an explicit inverse (ldh
+// <= 2048), through batch_factor -- the code of the solver's rebuild slot.  Problem b (= local partition * L + lambda):
+//   mode[b] = 0: done, no kernel may touch it;  1: Lc = H[b] (Dt x Dt row-major, lower triangle read) as chol_prep leaves it,
+//   then the factorisation without prep;  2: the fp32 Gram G[b] (Dt x Dt) goes into Hpart slice 0 (the other slices are zeroed),
+//   q[b] (Dt) into q, gram_unscale = 1, and chol_prep_kernel forms H with the batch's share.
+// order (norder entries, NULL: the batch order): the grids run over a device array of Problem copies in that order, as they run
+// over poll2_kernel's compacted array in batches of more than 64 problems.  share (0 or group_L > 1) and share_factor mirror the
+// cold start of a rebuild slot: share alone = distinct rho (every problem factorises the leader's Gram + its own q), share_factor
+// too = equal rho (the leaders factorise, chol_share_end_kernel and the Hinv copies serve the followers).  A batch mixing modes 1
+// and 2 runs chol_prep_kernel on its own first, with the mode-1 problems parked (need_hess = 0), then batch_factor without prep.
+// Before the launch every problem's Lc, Ldiag, Ldinv, Yinv and Hinv are filled with a NaN sentinel (all bits set), except the
+// strict upper triangle of Yinv, which stays 0: the DMMA merges and Y^T Y of systems wider than 1000 read it as the zeros of a
+// triangular matrix.  Outputs, each if not NULL: L_out (Dt x Dt), Y_out and Hinv_out (ldh x ldh), Ldinv_out (ldh x 32), ctrl_out
+// (4 per problem: fail, done, hess_valid, tot_hess as the kernels left them; the hook starts every problem from 0, 0/1, 0, 0).
+// Every argument is checked before any launch.  gram_unscale and q are restored; the batch's x-update state is consumed (every
+// problem is left done without a factor): begin() again before iterating.
+int mlease_internal_batch_factor(mlease_session* s, const int32_t* mode, const double* H, const float* G, const double* q,
+                                 const int32_t* order, int32_t norder, int32_t share, int32_t share_factor, double* L_out,
+                                 double* Y_out, double* Hinv_out, double* Ldinv_out, int32_t* ctrl_out) {
+  if (!s || !mode) return fail(MLEASE_ERR_INVALID, "null argument");
+  if (!s->batch || !s->begun) return fail(MLEASE_ERR_STATE, "mlease_admm_begin was not called");
+  Batch& B = *s->batch;
+  if (B.matfree || !B.h[0].Hinv) return fail(MLEASE_ERR_INVALID, "a matrix-free session forms no factor");
+  if (cholesky_factored_direction(B.ldh)) return fail(MLEASE_ERR_INVALID, "only systems up to 2048 (ldh) form the explicit inverse");
+  const int nprob = B.nprob, Dt = s->Dt, ldh = B.ldh, Dp = B.Dp;
+  bool any1 = false, any2 = false, any0 = false;
+  for (int b = 0; b < nprob; b++) {
+    if (mode[b] < 0 || mode[b] > 2) return fail(MLEASE_ERR_INVALID, "mode must be 0, 1 or 2");
+    any0 |= mode[b] == 0; any1 |= mode[b] == 1; any2 |= mode[b] == 2;
+  }
+  if (any1 && !H) return fail(MLEASE_ERR_INVALID, "mode 1 needs H");
+  if (any2 && (!G || !q)) return fail(MLEASE_ERR_INVALID, "mode 2 needs G and q");
+  if (order) {
+    if (norder < 0 || norder > nprob) return fail(MLEASE_ERR_INVALID, "launch order longer than the batch");
+    std::vector<char> seen(nprob, 0);
+    for (int i = 0; i < norder; i++) {
+      if (order[i] < 0 || order[i] >= nprob) return fail(MLEASE_ERR_INVALID, "launch order leaves the batch");
+      if (seen[order[i]]++) return fail(MLEASE_ERR_INVALID, "launch order repeats a problem");
+    }
+  }
+  if (share != 0 && !(share > 1 && share == B.group_L)) return fail(MLEASE_ERR_INVALID, "share must be 0 or the batch's group_L (> 1)");
+  if (share && order) return fail(MLEASE_ERR_INVALID, "a shared cold start runs over the batch order");
+  if (share_factor && !share) return fail(MLEASE_ERR_INVALID, "share_factor needs share");
+  if (share_factor && (any0 || (any1 && any2))) return fail(MLEASE_ERR_INVALID, "share_factor needs every problem in one mode, 1 or 2");
+  if (share)
+    for (int b = 0; b < nprob; b++)
+      if (mode[b] != mode[b - b % share]) return fail(MLEASE_ERR_INVALID, "with share, every problem of a group has its leader's mode");
+  CK(cudaSetDevice(s->cfg.device));
+  const size_t hh = (size_t)ldh * ldh;
+  std::vector<Ctrl> c0(nprob), c(nprob);
+  CK(cudaMemcpy(c0.data(), B.d_ctrl, (size_t)nprob * sizeof(Ctrl), cudaMemcpyDeviceToHost));
+  std::vector<double> qsave((size_t)nprob * Dt);
+  // sentinel: all bits set (a NaN) everywhere, but 0 in the strict upper triangle of Yinv
+  std::vector<double> ypat(hh);
+  {
+    double nan; std::memset(&nan, 0xFF, sizeof(nan));
+    for (int i = 0; i < ldh; i++)
+      for (int j = 0; j < ldh; j++) ypat[(size_t)i * ldh + j] = j > i ? 0.0 : nan;
+  }
+  std::vector<double> lc(hh);
+  std::vector<float> gp((size_t)Dp * Dp, 0.f);
+  std::vector<Problem> ph = B.h;
+  for (int b = 0; b < nprob; b++) {
+    const Problem& p = B.h[b];
+    CK(cudaMemset(p.Lc, 0xFF, hh * sizeof(double)));
+    CK(cudaMemset(p.Hinv, 0xFF, hh * sizeof(double)));
+    CK(cudaMemset(p.Ldiag, 0xFF, (size_t)ldh * 32 * sizeof(double)));
+    CK(cudaMemset(p.Ldinv, 0xFF, (size_t)ldh * 32 * sizeof(double)));
+    CK(cudaMemcpy(p.Yinv, ypat.data(), hh * sizeof(double), cudaMemcpyHostToDevice));
+    if (mode[b] == 1) {
+      const double* h = H + (size_t)b * Dt * Dt;
+      std::fill(lc.begin(), lc.end(), 0.0);
+      for (int i = 0; i < ldh; i++)
+        for (int j = 0; j <= i; j++) lc[(size_t)i * ldh + j] = i < Dt ? h[(size_t)i * Dt + j] : (i == j ? 1.0 : 0.0);
+      CK(cudaMemcpy(p.Lc, lc.data(), hh * sizeof(double), cudaMemcpyHostToDevice));
+    } else if (mode[b] == 2) {
+      const float* g = G + (size_t)b * Dt * Dt;
+      for (int i = 0; i < Dt; i++) std::memcpy(&gp[(size_t)i * Dp], g + (size_t)i * Dt, (size_t)Dt * sizeof(float));
+      CK(cudaMemset(p.Hpart, 0, (size_t)B.gram_slices * Dp * Dp * sizeof(float)));
+      CK(cudaMemcpy(p.Hpart, gp.data(), gp.size() * sizeof(float), cudaMemcpyHostToDevice));
+      CK(cudaMemcpy(&qsave[(size_t)b * Dt], p.q, (size_t)Dt * sizeof(double), cudaMemcpyDeviceToHost));
+      CK(cudaMemcpy(p.q, q + (size_t)b * Dt, (size_t)Dt * sizeof(double), cudaMemcpyHostToDevice));
+      ph[b].gram_unscale = 1.f;
+    }
+    c[b] = c0[b];
+    c[b].done = mode[b] ? 0 : 1; c[b].need_hess = 1; c[b].fail = 0; c[b].hess_valid = 0; c[b].tot_hess = 0;
+  }
+  CK(cudaMemcpy(B.d, ph.data(), (size_t)nprob * sizeof(Problem), cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(B.d_ctrl, c.data(), (size_t)nprob * sizeof(Ctrl), cudaMemcpyHostToDevice));
+  Problem* d_ord = nullptr;
+  int launches = 0;
+  auto run = [&]() -> int {
+    const Problem* d_hess = B.d;
+    int n_hess = nprob;
+    if (order) {
+      std::vector<Problem> po(std::max(1, (int)norder));
+      for (int i = 0; i < norder; i++) po[i] = ph[order[i]];
+      CK(cudaMalloc(&d_ord, po.size() * sizeof(Problem)));
+      CK(cudaMemcpy(d_ord, po.data(), (size_t)norder * sizeof(Problem), cudaMemcpyHostToDevice));
+      d_hess = d_ord; n_hess = norder;
+    }
+    int skip_prep = any2 ? 0 : 1;
+    if (any1 && any2 && n_hess > 0) {
+      std::vector<Ctrl> cp = c;
+      for (int b = 0; b < nprob; b++) if (mode[b] == 1) cp[b].need_hess = 0;
+      CK(cudaMemcpy(B.d_ctrl, cp.data(), (size_t)nprob * sizeof(Ctrl), cudaMemcpyHostToDevice));
+      CK(cholesky_prep(d_hess, n_hess, ldh, share, s->stream, &launches));
+      CK(cudaStreamSynchronize(s->stream));
+      CK(cudaMemcpy(B.d_ctrl, c.data(), (size_t)nprob * sizeof(Ctrl), cudaMemcpyHostToDevice));
+      skip_prep = 1;
+    }
+    if (n_hess > 0)
+      if (int rc = batch_factor(B, d_hess, n_hess, share, share_factor != 0, skip_prep, s->stream, &launches)) return rc;
+    CK(cudaStreamSynchronize(s->stream));
+    return 0;
+  };
+  // read back, then restore q, gram_unscale and Ctrl (also after a failed launch)
+  auto read = [&]() -> int {
+    if (int rc = run()) return rc;
+    CK(cudaMemcpy(c.data(), B.d_ctrl, (size_t)nprob * sizeof(Ctrl), cudaMemcpyDeviceToHost));
+    for (int b = 0; b < nprob; b++) {
+    const Problem& p = B.h[b];
+    if (L_out) {
+      CK(cudaMemcpy(lc.data(), p.Lc, hh * sizeof(double), cudaMemcpyDeviceToHost));
+      for (int i = 0; i < Dt; i++) std::memcpy(L_out + (size_t)b * Dt * Dt + (size_t)i * Dt, &lc[(size_t)i * ldh], (size_t)Dt * sizeof(double));
+    }
+    if (Y_out) CK(cudaMemcpy(Y_out + (size_t)b * hh, p.Yinv, hh * sizeof(double), cudaMemcpyDeviceToHost));
+    if (Hinv_out) CK(cudaMemcpy(Hinv_out + (size_t)b * hh, p.Hinv, hh * sizeof(double), cudaMemcpyDeviceToHost));
+    if (Ldinv_out) CK(cudaMemcpy(Ldinv_out + (size_t)b * ldh * 32, p.Ldinv, (size_t)ldh * 32 * sizeof(double), cudaMemcpyDeviceToHost));
+    if (ctrl_out) {
+      int32_t* o = ctrl_out + 4 * (size_t)b;
+      o[0] = c[b].fail; o[1] = c[b].done; o[2] = c[b].hess_valid; o[3] = (int32_t)c[b].tot_hess;
+    }
+    }
+    return 0;
+  };
+  const int rc = read();
+  if (d_ord) cudaFree(d_ord);
+  cudaStreamSynchronize(s->stream);
+  for (int b = 0; b < nprob; b++)
+    if (mode[b] == 2) CK(cudaMemcpy(B.h[b].q, &qsave[(size_t)b * Dt], (size_t)Dt * sizeof(double), cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(B.d, B.h.data(), (size_t)nprob * sizeof(Problem), cudaMemcpyHostToDevice));
+  for (int b = 0; b < nprob; b++) { c0[b].done = 1; c0[b].hess_valid = 0; c0[b].need_hess = 0; c0[b].fail = 0; }
+  CK(cudaMemcpy(B.d_ctrl, c0.data(), (size_t)nprob * sizeof(Ctrl), cudaMemcpyHostToDevice));
+  B.mirror.clear();
+  s->cnt.launches += launches;
+  return rc;
+}
+
+// Test hook, not part of the C ABI: the quasi-Newton direction on the explicit inverse (ldh <= 2048) of the problems with active[b]
+// != 0, through the kernels of a chord slot: k1_reduce_decide (its first L-BFGS loop) and newton_solve (newton_gemv_kernel, the
+// second loop, h0_scale, the trial point).  Run it after mlease_internal_batch_factor: it multiplies whatever Hinv holds.  Per
+// active problem: the data-term gradient g[b] (Dt), the secant ring S[b], Y[b] (BFGS_M x Dt each, slot-major), rho[b] (BFGS_M),
+// count[b] = Ctrl::bfgs_count (>= 0; above BFGS_M the ring has wrapped), h0[b] = Ctrl::h0_scale and the point beta[b] (Dt).
+// The decide kernel takes its accept path with no pass over the rows: skip_eval = 1 (k1_partial_reduce_kernel leaves g_t alone,
+// no loss partials: k1_chunks = 0), beta_t = m = beta (the prior term is 0), have_dir = 0 (no line search, no new secant pair),
+// hess_valid = 1, emit = 0 (no rebuild), newton_steps = evals = 0 and max_newton >= 1 (no stop test can end the x-update).  Outputs, each if not NULL:
+// dir_out (Dt per problem), phi0_out = Ctrl::phi0, dirnorm_out = Ctrl::dirnorm, beta_t_out (Dt; float(beta + dir) as stored);
+// an inactive problem's are NaN.  Checked before any launch; the batch's x-update state is consumed: begin() again before iterating.
+int mlease_internal_direction(mlease_session* s, const int32_t* active, const double* g, const double* S, const double* Y,
+                              const double* rho, const int32_t* count, const double* h0, const double* beta, double* dir_out,
+                              double* phi0_out, double* dirnorm_out, double* beta_t_out) {
+  if (!s || !active || !g || !S || !Y || !rho || !count || !h0 || !beta) return fail(MLEASE_ERR_INVALID, "null argument");
+  if (!s->batch || !s->begun) return fail(MLEASE_ERR_STATE, "mlease_admm_begin was not called");
+  Batch& B = *s->batch;
+  if (B.matfree || !B.h[0].Hinv) return fail(MLEASE_ERR_INVALID, "a matrix-free session forms no factor");
+  if (cholesky_factored_direction(B.ldh)) return fail(MLEASE_ERR_INVALID, "only systems up to 2048 (ldh) form the explicit inverse");
+  const int nprob = B.nprob, Dt = s->Dt, ldx = s->ldx;
+  for (int b = 0; b < nprob; b++)
+    if (active[b] && count[b] < 0) return fail(MLEASE_ERR_INVALID, "bfgs_count must be >= 0");
+  CK(cudaSetDevice(s->cfg.device));
+  std::vector<Ctrl> c(nprob);
+  CK(cudaMemcpy(c.data(), B.d_ctrl, (size_t)nprob * sizeof(Ctrl), cudaMemcpyDeviceToHost));
+  std::vector<double> v(ldx), ring((size_t)BFGS_M * ldx);
+  for (int b = 0; b < nprob; b++) {
+    Ctrl& x = c[b];
+    x.done = active[b] ? 0 : 1;
+    if (!active[b]) continue;
+    const Problem& p = B.h[b];
+    x.skip_eval = 1; x.k1_chunks = 0; x.have_dir = 0; x.hess_valid = 1; x.emit = 0; x.need_hess = 0; x.need_solve = 0;
+    x.newton_steps = 0; x.evals = 0; x.fail = 0; x.bfgs_count = count[b]; x.h0_scale = h0[b];
+    x.max_newton = std::max(1, s->max_newton);   // (a batch that never ran an x-update has 0: the decide kernel would stop it)
+    std::fill(v.begin(), v.end(), 0.0);
+    std::memcpy(v.data(), g + (size_t)b * Dt, (size_t)Dt * sizeof(double));
+    CK(cudaMemcpy(p.g_t, v.data(), (size_t)ldx * sizeof(double), cudaMemcpyHostToDevice));
+    std::memcpy(v.data(), beta + (size_t)b * Dt, (size_t)Dt * sizeof(double));
+    CK(cudaMemcpy(p.beta_t, v.data(), (size_t)ldx * sizeof(double), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(p.m, v.data(), (size_t)ldx * sizeof(double), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(p.beta, v.data(), (size_t)ldx * sizeof(double), cudaMemcpyHostToDevice));
+    std::fill(v.begin(), v.end(), std::nan(""));
+    CK(cudaMemcpy(p.dir, v.data(), (size_t)ldx * sizeof(double), cudaMemcpyHostToDevice));
+    for (int pass = 0; pass < 2; pass++) {
+      const double* src = (pass ? Y : S) + (size_t)b * BFGS_M * Dt;
+      std::fill(ring.begin(), ring.end(), 0.0);
+      for (int j = 0; j < BFGS_M; j++) std::memcpy(&ring[(size_t)j * ldx], src + (size_t)j * Dt, (size_t)Dt * sizeof(double));
+      CK(cudaMemcpy(pass ? p.bfgs_Y : p.bfgs_S, ring.data(), ring.size() * sizeof(double), cudaMemcpyHostToDevice));
+    }
+    CK(cudaMemcpy(p.bfgs_rho, rho + (size_t)b * BFGS_M, BFGS_M * sizeof(double), cudaMemcpyHostToDevice));
+  }
+  CK(cudaMemcpy(B.d_ctrl, c.data(), (size_t)nprob * sizeof(Ctrl), cudaMemcpyHostToDevice));
+  int launches = 0;
+  CK(k1_reduce_decide(B.d, nprob, Dt, s->stream, &launches, 0));
+  CK(newton_solve(B.d, nprob, B.ldh, s->stream, &launches, B.group_L));
+  CK(cudaStreamSynchronize(s->stream));
+  CK(cudaMemcpy(c.data(), B.d_ctrl, (size_t)nprob * sizeof(Ctrl), cudaMemcpyDeviceToHost));
+  const double nan = std::nan("");
+  for (int b = 0; b < nprob; b++) {
+    const Problem& p = B.h[b];
+    if (dir_out) {
+      if (active[b]) CK(cudaMemcpy(dir_out + (size_t)b * Dt, p.dir, (size_t)Dt * sizeof(double), cudaMemcpyDeviceToHost));
+      else std::fill(dir_out + (size_t)b * Dt, dir_out + (size_t)(b + 1) * Dt, nan);
+    }
+    if (beta_t_out) {
+      if (active[b]) CK(cudaMemcpy(beta_t_out + (size_t)b * Dt, p.beta_t, (size_t)Dt * sizeof(double), cudaMemcpyDeviceToHost));
+      else std::fill(beta_t_out + (size_t)b * Dt, beta_t_out + (size_t)(b + 1) * Dt, nan);
+    }
+    if (phi0_out) phi0_out[b] = active[b] ? c[b].phi0 : nan;
+    if (dirnorm_out) dirnorm_out[b] = active[b] ? c[b].dirnorm : nan;
+  }
+  for (auto& x : c) { x.done = 1; x.hess_valid = 0; x.need_solve = 0; x.need_hess = 0; x.have_dir = 0; x.bfgs_count = 0; x.h0_scale = 1.0; }
+  CK(cudaMemcpy(B.d_ctrl, c.data(), (size_t)nprob * sizeof(Ctrl), cudaMemcpyHostToDevice));
+  B.mirror.clear();
+  s->cnt.launches += launches;
+  return 0;
+}
+
 // Test hooks of the factored direction of wide systems (ldh > 2048), not part of the C ABI.  Each refuses, before any launch, a
 // batch that has no Ysym (ldh <= 2048, or matrix-free), since the kernels they run dereference it.
 //

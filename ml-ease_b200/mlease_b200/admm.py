@@ -557,6 +557,58 @@ def _internal_batch_grad(session, w, active=None, rows=None, want_sd=False, want
                 chunks=info[8:].copy())
 
 
+def _internal_batch_factor(session, mode, H=None, G=None, q=None, order=None, share=0, share_factor=False):
+    """Test hook (not part of the C ABI): one factorisation of the ADMM batch of `session` (after begin(), ldh <= 2048) through
+    the solver's rebuild code.  mode[b]: 0 = done (untouched), 1 = factorise H[b] (Dt x Dt fp64), 2 = factorise the fp32 Gram G[b]
+    plus diag(q[b]) through chol_prep_kernel.  order: launch order (a permutation or subset of the problems; default: batch
+    order).  share / share_factor: the cold start of a rebuild slot (see mlease_internal_batch_factor).  Consumes the batch's
+    x-update state.  -> dict(L [nprob, Dt, Dt], Y, Hinv [nprob, ldh, ldh], Ldinv [nprob, ldh, 32],
+    fail, done, hess_valid, tot_hess [nprob]); buffers no kernel wrote hold the all-ones NaN sentinel."""
+    nprob, Dt = session.num_blocks * session.L, session.Dt
+    ldh = (Dt + 31) // 32 * 32
+    md = np.ascontiguousarray(mode, np.int32)
+    if md.shape != (nprob,):
+        raise ValueError("mode must hold one entry per problem")
+    Hc = None if H is None else np.ascontiguousarray(H, np.float64).reshape(nprob, Dt, Dt)
+    Gc = None if G is None else np.ascontiguousarray(G, np.float32).reshape(nprob, Dt, Dt)
+    qc = None if q is None else np.ascontiguousarray(q, np.float64).reshape(nprob, Dt)
+    oc = None if order is None else np.ascontiguousarray(order, np.int32)
+    out = dict(L=np.empty((nprob, Dt, Dt)), Y=np.empty((nprob, ldh, ldh)), Hinv=np.empty((nprob, ldh, ldh)),
+               Ldinv=np.empty((nprob, ldh, 32)))
+    ctrl = np.zeros((nprob, 4), np.int32)
+    fn = lib().mlease_internal_batch_factor
+    vp = C.c_void_p
+    fn.argtypes, fn.restype = [vp] * 6 + [C.c_int32] * 3 + [vp] * 5, C.c_int
+    check(fn(session._h, md.ctypes.data, ptr(Hc), ptr(Gc), ptr(qc), ptr(oc), 0 if oc is None else len(oc), int(share),
+             int(bool(share_factor)), out["L"].ctypes.data, out["Y"].ctypes.data, out["Hinv"].ctypes.data, out["Ldinv"].ctypes.data,
+             ctrl.ctypes.data))
+    out.update(fail=ctrl[:, 0].copy(), done=ctrl[:, 1].copy(), hess_valid=ctrl[:, 2].copy(), tot_hess=ctrl[:, 3].copy())
+    return out
+
+
+BFGS_M = 6   # secant pairs kept per problem (common.cuh)
+
+
+def _internal_direction(session, active, g, S, Y, rho, count, h0, beta):
+    """Test hook (not part of the C ABI): the quasi-Newton direction on the explicit inverse H^-1 (ldh <= 2048) of the active
+    problems of the ADMM batch, through the kernels of a chord slot, after _internal_batch_factor.  Per problem: g [Dt] data-term
+    gradient, S, Y [BFGS_M, Dt] secant ring (slot-major), rho [BFGS_M], count (bfgs_count), h0 (h0_scale), beta [Dt] point.
+    Consumes the batch's x-update state.  -> dict(dir [nprob, Dt], phi0, dirnorm [nprob], beta_t [nprob, Dt]); NaN where inactive."""
+    nprob, Dt = session.num_blocks * session.L, session.Dt
+    act = np.ascontiguousarray(active, np.int32)
+    g, beta = (np.ascontiguousarray(a, np.float64).reshape(nprob, Dt) for a in (g, beta))
+    S, Y = (np.ascontiguousarray(a, np.float64).reshape(nprob, BFGS_M, Dt) for a in (S, Y))
+    rho = np.ascontiguousarray(rho, np.float64).reshape(nprob, BFGS_M)
+    cnt = np.ascontiguousarray(count, np.int32).reshape(nprob)
+    h0 = np.ascontiguousarray(h0, np.float64).reshape(nprob)
+    out = dict(dir=np.empty((nprob, Dt)), phi0=np.empty(nprob), dirnorm=np.empty(nprob), beta_t=np.empty((nprob, Dt)))
+    fn = lib().mlease_internal_direction
+    fn.argtypes, fn.restype = [C.c_void_p] * 13, C.c_int
+    check(fn(session._h, act.ctypes.data, g.ctypes.data, S.ctypes.data, Y.ctypes.data, rho.ctypes.data, cnt.ctypes.data, h0.ctypes.data,
+             beta.ctypes.data, out["dir"].ctypes.data, out["phi0"].ctypes.data, out["dirnorm"].ctypes.data, out["beta_t"].ctypes.data))
+    return out
+
+
 def _internal_keyed_last_call():
     """Test hook: the most recent keyed call of the process -> (key boundaries of its chunks, streamed, stage ms, wait ms)."""
     fn = lib().mlease_internal_keyed_last_call

@@ -669,13 +669,15 @@ def test_errors_follow_reference_conventions(mb):
             s.run(1)
 
 
+@pytest.mark.parametrize("d", [45, 1100])
 @pytest.mark.parametrize("sparse", [False, True])
-def test_posterior_variance_diag_and_full(mb, sparse):
+def test_posterior_variance_diag_and_full(mb, sparse, d):
     """ItemModelTrain's "posteriorVar" (jobs/ItemModelTrain.java:257-266): LibLinear.train's computePosteriorVar tail
     (llf/LibLinear.java:315-334).  Diagonal mode = 1 / hessianDiagonal (llf/LogisticRegressionL2.java:304-327); full mode =
     diag of the inverse of hessian() (:258-297).  The GPU accumulates the Hessian in fp64 from the fp32 data, so the
-    tolerance is 1e-9 / 1e-8 relative, not the bf16 Gram's."""
-    n, d = 2500, 45
+    tolerance is 1e-9 / 1e-8 relative, not the bf16 Gram's.  d = 1100 (ldh 1120) runs the inverse of systems wider than 1000:
+    256-wide leaves, the fp64 DMMA merges and Y^T Y."""
+    n = 2500
     X, y, w, o = _mk(n, d, seed=17, sparse=sparse, density=0.25)
     rng = np.random.default_rng(2)
     pm = rng.normal(0, 0.2, d + 1); pv = rng.uniform(0.3, 3.0, d + 1)
