@@ -317,6 +317,73 @@ int batch_factor(Batch& B, const Problem* d_hess, int n_hess, int share, bool sh
       // (Ysym is not copied: chol_share_end_kernel points the follower's Ctrl::ysym_use at the leader's)
     }
   }
+  B.has_factor = true;
+  return 0;
+}
+
+// Matrix-free direction of the problems that accepted a point this slot: diagonal pass, then CG steps in chunks of CG_CHUNK
+// (Hv pass -> fixed-order reduction -> CG update each), one pinned read-back of the "any CG running" flag per chunk.
+// Problems whose CG has finished return at once from every kernel of a chunk.
+static int mf_direction(Batch& B, const SlotCtx& x) {
+  constexpr int CG_CHUNK = 4;
+  Profiler& pf = *x.pf;
+  cudaStream_t st = x.st;
+  int& launches = *x.launches;
+  pf.begin(2, st);
+  CK(cg_begin(B.d, B.nprob, st, &launches));
+  CK(batch_k1(B, 0, st, &launches, K1_DIAG));
+  CK(hv_reduce(B.d, B.nprob, B.Dt, 2, st, &launches));
+  CK(cg_init(B.d, B.nprob, B.Dt, st, &launches));
+  pf.end(st);
+  for (int steps = 0; steps < CG_MAX_STEPS; steps += CG_CHUNK) {
+    for (int j = 0; j < CG_CHUNK; j++) {
+      pf.begin(2, st);
+      CK(batch_k1(B, 0, st, &launches, K1_HV));
+      CK(hv_reduce(B.d, B.nprob, B.Dt, 1, st, &launches));
+      CK(cg_step(B.d, B.nprob, B.Dt, st, &launches));
+      pf.end(st);
+    }
+    CK(cg_poll(B.d, B.nprob, x.d_flag + 2, st, &launches));
+    CK(cudaMemcpyAsync(x.h_flag + 2, x.d_flag + 2, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (!x.h_flag[2]) break;
+  }
+  return 0;
+}
+
+// One slot's launches of an x-update: K1, the decide kernel, the Gram / Cholesky launches of a rebuild (with_hess), the
+// matrix-free direction, newton_solve / newton_finish and, for large batches (x.poll), the end-of-slot poll.  spec: see
+// k1_reduce_decide_kernel.  batch_xupdate and the slot-trace test hook both run their slots through this function.
+int batch_slot(Batch& B, const SlotCtx& x, int slot_idx, bool with_hess, bool spec) {
+  Profiler& pf = *x.pf;
+  cudaStream_t st = x.st;
+  int& launches = *x.launches;
+  pf.begin(0, st);
+  CK(batch_k1(B, B.matfree ? 1 : -1, st, &launches));   // matrix-free: every pass leaves sqrt(d) of its point for the Hv passes
+  pf.end(st);
+  pf.begin(1, st);
+  CK(k1_reduce_decide(B.d, B.nprob, B.Dt, st, &launches, spec ? 1 : 0));
+  pf.end(st);
+  if (with_hess && x.n_hess > 0) {
+    pf.begin(2, st);
+    // cold start of a multi-lambda run: the L problems of a partition all sit at beta = 0, their Grams are the same
+    const int share = (slot_idx == 0) ? x.share_first_gram : 0;
+    if (share > 1)
+      for (int b = 0; b < B.nprob; b++) if (b % share != 0) *x.shared_flops += gram_build_flops(B, B.h[b]);
+    CK(batch_gram(B, x.d_hess, x.n_hess, 0, st, &launches, share));
+    pf.end(st);
+    pf.begin(3, st);
+    const bool share_fact = share > 1 && x.share_first_factor;   // same rho too: same H, one factorisation per group
+    if (int rc = batch_factor(B, x.d_hess, x.n_hess, share, share_fact, 0, st, &launches)) return rc;
+    pf.end(st);
+  }
+  if (B.matfree)
+    if (int rc = mf_direction(B, x)) return rc;
+  pf.begin(1, st);
+  if (B.matfree) CK(newton_finish(B.d, B.nprob, B.Dt, st, &launches));
+  else CK(newton_solve(B.d, B.nprob, B.ldh, st, &launches, B.group_L));
+  if (x.poll) { poll2_kernel<<<1, 256, 0, st>>>(B.d, B.nprob, x.d_flag, B.d_compact); launches++; }
+  pf.end(st);
   return 0;
 }
 
@@ -343,61 +410,10 @@ int batch_xupdate(Batch& B, cudaStream_t st, double xtol, int max_newton, int po
   const Problem* d_hess = B.d;   // problems the Gram / Cholesky grids run over (large batches: compacted by poll2_kernel)
   int n_hess = B.nprob;
   double shared_flops = 0;   // Gram builds that were not run because the group's first problem stood in for them
-  // Matrix-free direction of the problems that accepted a point this slot: diagonal pass, then CG steps in chunks of CG_CHUNK
-  // (Hv pass -> fixed-order reduction -> CG update each), one pinned read-back of the "any CG running" flag per chunk.
-  // Problems whose CG has finished return at once from every kernel of a chunk.
-  auto mf_direction = [&]() -> int {
-    constexpr int CG_CHUNK = 4;
-    pf.begin(2, st);
-    CK(cg_begin(B.d, B.nprob, st, &launches));
-    CK(batch_k1(B, 0, st, &launches, K1_DIAG));
-    CK(hv_reduce(B.d, B.nprob, B.Dt, 2, st, &launches));
-    CK(cg_init(B.d, B.nprob, B.Dt, st, &launches));
-    pf.end(st);
-    for (int steps = 0; steps < CG_MAX_STEPS; steps += CG_CHUNK) {
-      for (int j = 0; j < CG_CHUNK; j++) {
-        pf.begin(2, st);
-        CK(batch_k1(B, 0, st, &launches, K1_HV));
-        CK(hv_reduce(B.d, B.nprob, B.Dt, 1, st, &launches));
-        CK(cg_step(B.d, B.nprob, B.Dt, st, &launches));
-        pf.end(st);
-      }
-      CK(cg_poll(B.d, B.nprob, d_flag + 2, st, &launches));
-      CK(cudaMemcpyAsync(h_flag + 2, d_flag + 2, sizeof(int), cudaMemcpyDeviceToHost, st));
-      CK(cudaStreamSynchronize(st));
-      if (!h_flag[2]) break;
-    }
-    return 0;
-  };
-  // One slot's launches.  with_hess: the Gram / Cholesky launches of a rebuild are included; spec: see k1_reduce_decide_kernel.
+  // One slot's launches (batch_slot).  with_hess: the Gram / Cholesky launches of a rebuild are included; spec: see k1_reduce_decide_kernel.
   auto enqueue_slot = [&](int slot_idx, bool with_hess, bool spec) -> int {
-    pf.begin(0, st);
-    CK(batch_k1(B, B.matfree ? 1 : -1, st, &launches));   // matrix-free: every pass leaves sqrt(d) of its point for the Hv passes
-    pf.end(st);
-    pf.begin(1, st);
-    CK(k1_reduce_decide(B.d, B.nprob, B.Dt, st, &launches, spec ? 1 : 0));
-    pf.end(st);
-    if (with_hess && n_hess > 0) {
-      pf.begin(2, st);
-      // cold start of a multi-lambda run: the L problems of a partition all sit at beta = 0, their Grams are the same
-      const int share = (slot_idx == 0) ? share_first_gram : 0;
-      if (share > 1)
-        for (int b = 0; b < B.nprob; b++) if (b % share != 0) shared_flops += gram_build_flops(B, B.h[b]);
-      CK(batch_gram(B, d_hess, n_hess, 0, st, &launches, share));
-      pf.end(st);
-      pf.begin(3, st);
-      const bool share_fact = share > 1 && share_first_factor;   // same rho too: same H, one factorisation per group
-      if (int rc = batch_factor(B, d_hess, n_hess, share, share_fact, 0, st, &launches)) return rc;
-      pf.end(st);
-    }
-    if (B.matfree)
-      if (int rc = mf_direction()) return rc;
-    pf.begin(1, st);
-    if (B.matfree) CK(newton_finish(B.d, B.nprob, B.Dt, st, &launches));
-    else CK(newton_solve(B.d, B.nprob, B.ldh, st, &launches, B.group_L));
-    if (!small) { poll2_kernel<<<1, 256, 0, st>>>(B.d, B.nprob, d_flag, B.d_compact); launches++; }
-    pf.end(st);
-    return 0;
+    const SlotCtx x{st, &pf, &launches, d_hess, n_hess, share_first_gram, share_first_factor, &shared_flops, h_flag, d_flag, !small};
+    return batch_slot(B, x, slot_idx, with_hess, spec);
   };
   if (small) {
     // Slot pipeline: the host runs ONE slot ahead of what it knows.  While slot s executes, slot s+1 is already enqueued in

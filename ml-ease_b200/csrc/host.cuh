@@ -93,6 +93,7 @@ struct Batch {
   int k1_dyn = 0;                 // > 0: K1 CTAs are dealt to the running problems at run time (value = nprob, <= 32); k1_grid = whole grid
   int rebuild_is_expensive = 0;   // cost model: Gram + Cholesky + inverse vs one K1 pass (set in batch_alloc)
   int matfree = 0;                // Newton-CG directions from Hv passes: no Gram, factor or inverse is allocated (set in batch_alloc)
+  bool has_factor = false;        // batch_factor has run on this batch: Hinv / Ysym hold a factorisation
   bool ysym_shared = false;       // a wide batch whose followers were pointed at their leader's Ysym (chol_share_end_kernel)
   std::vector<Problem> h;
   Problem* d = nullptr;
@@ -159,6 +160,17 @@ int batch_alloc(Batch& B, int num_sms, int hessian_policy, int csr_gram_force = 
 cudaError_t batch_gram(const Batch& B, const Problem* d_probs, int n, int force, cudaStream_t st, int* launches, int share = 0);
 cudaError_t batch_k1(Batch& B, int force_emit, cudaStream_t st, int* launches, int mode = K1_GRAD);
 int batch_factor(Batch& B, const Problem* d_hess, int n_hess, int share, bool share_fact, int skip_prep, cudaStream_t st, int* launches);
+// what one slot of an x-update runs with: the stream, profiler and launch counter, the problems its rebuild launches run over,
+// the cold-start sharing of slot 0 (with the flops it saved), the flag words, and whether the end-of-slot poll kernel runs
+struct SlotCtx {
+  cudaStream_t st; Profiler* pf; int* launches;
+  const Problem* d_hess; int n_hess;
+  int share_first_gram, share_first_factor;
+  double* shared_flops;
+  int* h_flag; int* d_flag;
+  bool poll;
+};
+int batch_slot(Batch& B, const SlotCtx& x, int slot_idx, bool with_hess, bool spec);
 int batch_xupdate(Batch& B, cudaStream_t st, double xtol, int max_newton, int policy, int invalidate, int* h_flag, int* d_flag,
                   Counters& cnt, Profiler* prof = nullptr, int share_first_gram = 0, int share_first_factor = 0);
 

@@ -69,7 +69,9 @@ __global__ void __launch_bounds__(256) admm_consensus_kernel(const Problem* __re
   const double invP = 1.0 / (double)P;
   // regularizer = 1 (l1_thr != NULL): z = xbar + ubar, then the reference's "iterative thresholding" of the coefficients
   // (jobs/RegressionAdmmTrain.java:406-437): val > t -> val - t, val < -t -> val + t, values inside [-t, t] stay as they are
-  // (the reference does not zero them); the intercept (not in getCoefficients()) is the plain mean (:438-449).
+  // (the reference does not zero them); the intercept (not in getCoefficients()) is the plain mean (:438-449).  Column Dt - 1 IS
+  // the intercept in every batch this kernel sees: a session's batches are built with has_bias = 1 and Dt = num_features + 1
+  // (session.cu), there is no ADMM session without an intercept column, so k == Dt - 1 needs no flag.
   const double thr = l1_thr ? l1_thr[l] : 0.0;
   for (int k = blockIdx.x * 256 + threadIdx.x; k < Dt; k += gridDim.x * 256) {   // one element per thread: the grid covers Dt
     double zn;

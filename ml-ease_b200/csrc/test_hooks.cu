@@ -405,6 +405,258 @@ int mlease_internal_direction(mlease_session* s, const int32_t* active, const do
   return 0;
 }
 
+}  // extern "C"
+
+namespace {
+// The x-update fields of Ctrl as mlease_internal_newton_stage exchanges them, per problem: 24 ints, 14 reals, then the cumulative
+// counters (read back only).  The Ctrl pointers and ysym_use are never taken from the caller.
+#define STAGE_INTS(X)                                                                                                              \
+  X(done) X(have_dir) X(need_solve) X(need_hess) X(emit) X(hess_valid) X(fail) X(newton_steps) X(evals) X(rejects) X(hess_builds) \
+  X(stall) X(bfgs_count) X(k1_chunks) X(refresh_next) X(skip_eval) X(warm_used) X(build_step) X(max_newton) X(hess_policy)        \
+  X(rebuild_is_expensive) X(cg_active) X(cg_iter)
+#define STAGE_REALS(X) \
+  X(h0_scale) X(worst_ratio) X(alpha) X(phi0) X(f_acc) X(f_t) X(gnorm) X(gnorm_prev) X(dirnorm) X(dirnorm_prev) X(xtol) X(cg_rz) X(cg_g2) X(hv_vinf)
+#define STAGE_TOTALS(X) X(tot_evals) X(tot_newton) X(tot_rejects) X(tot_hess)
+struct StageCtrl {
+#define X(f) int32_t f;
+  STAGE_INTS(X)
+#undef X
+  int32_t pad_;
+#define X(f) double f;
+  STAGE_REALS(X)
+  STAGE_TOTALS(X)
+#undef X
+};
+static_assert(sizeof(StageCtrl) == 24 * 4 + 18 * 8, "StageCtrl is packed: 24 ints, 18 doubles");
+void stage_to_ctrl(const StageCtrl& a, Ctrl& c) {
+#define X(f) c.f = (decltype(c.f))a.f;
+  STAGE_INTS(X)
+  STAGE_REALS(X)
+#undef X
+}
+void ctrl_to_stage(const Ctrl& c, StageCtrl& a) {
+#define X(f) a.f = c.f;
+  STAGE_INTS(X)
+#undef X
+#define X(f) a.f = (double)c.f;
+  STAGE_REALS(X)
+  STAGE_TOTALS(X)
+#undef X
+  a.pad_ = 0;
+}
+enum { ST_BEGIN = 1, ST_DECIDE = 2, ST_SOLVE = 4, ST_FINISH = 8, ST_CG_BEGIN = 16, ST_CG_INIT = 32, ST_CG_STEP = 64, ST_CG_POLL = 128 };
+constexpr int STAGE_NVEC = 12;
+// Every problem's vectors, secant ring and fp32 vectors to the device (h2d) or back, in the layout of mlease_internal_newton_stage.
+int stage_exchange(Batch& B, int ldx, bool h2d, double* vec, double* ring, float* fvec) {
+  const size_t vb = (size_t)ldx * sizeof(double), ring_n = 2 * (size_t)BFGS_M * ldx + 2 * BFGS_M;
+  const int nvec = B.matfree ? STAGE_NVEC : 7;
+  auto cp = [&](void* dev, void* host, size_t bytes) {
+    return h2d ? cudaMemcpy(dev, host, bytes, cudaMemcpyHostToDevice) : cudaMemcpy(host, dev, bytes, cudaMemcpyDeviceToHost);
+  };
+  for (int b = 0; b < B.nprob; b++) {
+    const Problem& p = B.h[b];
+    double* v[STAGE_NVEC] = {p.beta, p.beta_t, p.m, p.q, p.g_t, p.g_acc, p.dir, p.cg_r, p.cg_p, p.cg_z, p.cg_Hp, p.cg_diag};
+    for (int i = 0; i < nvec; i++) CK(cp(v[i], vec + ((size_t)b * STAGE_NVEC + i) * ldx, vb));
+    double* r = ring + (size_t)b * ring_n;
+    if (!B.matfree) {
+      CK(cp(p.bfgs_S, r, (size_t)BFGS_M * vb));
+      CK(cp(p.bfgs_Y, r + (size_t)BFGS_M * ldx, (size_t)BFGS_M * vb));
+    }
+    CK(cp(p.bfgs_rho, r + 2 * (size_t)BFGS_M * ldx, BFGS_M * sizeof(double)));
+    CK(cp(p.bfgs_alpha, r + 2 * (size_t)BFGS_M * ldx + BFGS_M, BFGS_M * sizeof(double)));
+    float* f = fvec + (size_t)b * 3 * ldx;
+    CK(cp(p.beta_tf, f, (size_t)ldx * sizeof(float)));
+    CK(cp(p.qf, f + ldx, 2 * (size_t)ldx * sizeof(float)));   // qf and tf are adjacent
+  }
+  return 0;
+}
+}  // namespace
+
+extern "C" {
+
+// Test hook, not part of the C ABI: injects an x-update state into every problem of the begun ADMM batch, runs the selected kernels
+// of the Newton state machine (newton.cu) once, each through the solver's own launcher, and reads the whole state back.
+//   stages: ST_BEGIN newton_begin(begin_args = {xtol, max_newton, policy, invalidate, rebuild_is_expensive}); ST_DECIDE
+//   k1_reduce_decide(spec) -- the fixed-order reduction of the partials and the decide kernel, no pass over the rows; ST_CG_BEGIN,
+//   ST_CG_INIT, ST_CG_STEP, ST_CG_POLL (matrix-free batches; *cg_any = the poll's flag) -- cg_init finds the diagonal's data term in
+//   cg_diag and cg_step finds X^T D X p in cg_Hp, as the reductions of their passes leave them; ST_SOLVE newton_solve (the GEMV on
+//   whatever Hinv / Ysym the batch holds, then newton_solve_kernel) or ST_FINISH newton_finish (newton_solve_kernel alone, on the r
+//   = H0^-1 q the caller put into dir).  They run in that order.  stages = 0 injects and runs nothing: info only.
+//   ctrl: nprob StageCtrl, in and out.  vec: nprob x 12 x ldx doubles (beta, beta_t, m, q, g_t, g_acc, dir, cg_r, cg_p, cg_z, cg_Hp,
+//   cg_diag; the last five only on a matrix-free batch), ring: nprob x (2 BFGS_M ldx + 2 BFGS_M) doubles (bfgs_S, bfgs_Y -- not on
+//   a matrix-free batch --, bfgs_rho, bfgs_alpha), fvec: nprob x 3 x ldx floats (beta_tf, qf = hv_vf, tf); all in and out, whole
+//   vectors, padding included, copied as bytes (a caller marks what no kernel may write with any pattern it likes).
+//   gpart (nprob x nct_cap x ldx doubles; stored as fp32 into gpart_f on a fused batch) and fpart (nprob x nct_cap), or both NULL
+//   when every k1_chunks is 0.
+//   info (12 ints): nprob, Dt, ldx, ldh, partial rows allocated per problem (k1_grid), fused K1, matrix-free, Ysym present,
+//   rebuild_is_expensive, group_L, 0, 0.
+// Refused before any launch: a state the kernels would index memory with (k1_chunks beyond the allocated rows or nct_cap,
+// bfgs_count < 0, a policy other than 2 or secant pairs on a matrix-free batch, which has no ring), ST_SOLVE on a batch that never
+// factorised (no batch_factor ran on it: mlease_internal_batch_factor or a rebuild slot), ST_SOLVE together with ST_FINISH, CG stages on a batch without CG vectors.  The batch's x-update state is consumed
+// (every problem is left done, without a factor or pairs): begin() again before iterating.
+int mlease_internal_newton_stage(mlease_session* s, int32_t stages, int32_t spec, const double* begin_args, void* ctrl, double* vec,
+                                 double* ring, float* fvec, const double* gpart, const double* fpart, int32_t nct_cap, int32_t* info,
+                                 int32_t* cg_any) {
+  if (!s || !info) return fail(MLEASE_ERR_INVALID, "null argument");
+  if (!s->batch || !s->begun) return fail(MLEASE_ERR_STATE, "mlease_admm_begin was not called");
+  Batch& B = *s->batch;
+  const int nprob = B.nprob, Dt = s->Dt, ldx = s->ldx;
+  const bool wide = cholesky_factored_direction(B.ldh);
+  const int32_t inf[12] = {nprob, Dt, ldx, B.ldh, B.k1_grid, B.k1_fused, B.matfree, (!B.matfree && B.h[0].Ysym) ? 1 : 0,
+                           B.rebuild_is_expensive, B.group_L, 0, 0};
+  std::copy(inf, inf + 12, info);
+  if (stages == 0) return 0;
+  if (stages < 0 || stages > 255 || (spec != 0 && spec != 1)) return fail(MLEASE_ERR_INVALID, "stage mask or spec out of range");
+  if (!ctrl || !vec || !ring || !fvec) return fail(MLEASE_ERR_INVALID, "null argument");
+  if ((gpart == nullptr) != (fpart == nullptr) || nct_cap < 0) return fail(MLEASE_ERR_INVALID, "gpart and fpart come together");
+  if ((stages & ST_SOLVE) && (stages & ST_FINISH)) return fail(MLEASE_ERR_INVALID, "newton_solve and newton_finish are alternatives");
+  if ((stages & ST_SOLVE) && (B.matfree || !B.h[0].Hinv || (wide && !B.h[0].Ysym) || !B.has_factor))
+    return fail(MLEASE_ERR_INVALID, "newton_solve needs a batch that has factorised (batch_factor ran; a matrix-free batch forms no factor)");
+  if ((stages & (ST_CG_BEGIN | ST_CG_INIT | ST_CG_STEP | ST_CG_POLL)) && (!B.matfree || !B.h[0].cg_r))
+    return fail(MLEASE_ERR_INVALID, "the CG kernels need a matrix-free batch");
+  if ((stages & ST_CG_POLL) && !cg_any) return fail(MLEASE_ERR_INVALID, "cg_poll needs cg_any");
+  if (stages & ST_BEGIN) {
+    if (!begin_args) return fail(MLEASE_ERR_INVALID, "newton_begin needs its arguments");
+    const double pol = begin_args[2];
+    if (!(begin_args[0] >= 0.0) || !(begin_args[1] >= 0.0 && begin_args[1] <= 1e6) || !(pol == 0.0 || pol == 1.0 || pol == 2.0) ||
+        (B.matfree && pol != 2.0))
+      return fail(MLEASE_ERR_INVALID, "newton_begin arguments out of range (a matrix-free batch runs policy 2 only)");
+  }
+  const StageCtrl* in = static_cast<const StageCtrl*>(ctrl);
+  for (int b = 0; b < nprob; b++) {
+    const StageCtrl& a = in[b];
+    if (a.k1_chunks < 0 || a.k1_chunks > B.k1_grid) return fail(MLEASE_ERR_INVALID, "k1_chunks beyond the partial rows the batch allocated");
+    if (a.k1_chunks > (gpart ? nct_cap : 0)) return fail(MLEASE_ERR_INVALID, "k1_chunks beyond the partials passed");
+    if (a.bfgs_count < 0 || a.bfgs_count > (1 << 20)) return fail(MLEASE_ERR_INVALID, "bfgs_count must be >= 0");
+    if (a.hess_policy < 0 || a.hess_policy > 2 || a.max_newton < 0 || a.cg_iter < 0) return fail(MLEASE_ERR_INVALID, "policy, max_newton or cg_iter out of range");
+    if (B.matfree && (a.hess_policy != 2 || a.bfgs_count != 0)) return fail(MLEASE_ERR_INVALID, "a matrix-free batch keeps no secant pairs: policy 2, bfgs_count 0");
+  }
+  CK(cudaSetDevice(s->cfg.device));
+  std::vector<Ctrl> c0(nprob), c(nprob);
+  CK(cudaMemcpy(c0.data(), B.d_ctrl, (size_t)nprob * sizeof(Ctrl), cudaMemcpyDeviceToHost));
+  const size_t vb = (size_t)ldx * sizeof(double);
+  if (int rc = stage_exchange(B, ldx, true, vec, ring, fvec)) return rc;
+  if (gpart) {
+    std::vector<float> gf;
+    for (int b = 0; b < nprob; b++) {
+      const Problem& p = B.h[b];
+      const int nct = in[b].k1_chunks;
+      if (nct == 0) continue;
+      const double* src = gpart + (size_t)b * nct_cap * ldx;
+      if (p.gpart_f) {
+        gf.assign(src, src + (size_t)nct * ldx);
+        CK(cudaMemcpy(p.gpart_f, gf.data(), gf.size() * sizeof(float), cudaMemcpyHostToDevice));
+      } else {
+        CK(cudaMemcpy(p.gpart, src, (size_t)nct * vb, cudaMemcpyHostToDevice));
+      }
+      CK(cudaMemcpy(p.fpart, fpart + (size_t)b * nct_cap, (size_t)nct * sizeof(double), cudaMemcpyHostToDevice));
+    }
+  }
+  for (int b = 0; b < nprob; b++) { c[b] = c0[b]; stage_to_ctrl(in[b], c[b]); }
+  CK(cudaMemcpy(B.d_ctrl, c.data(), (size_t)nprob * sizeof(Ctrl), cudaMemcpyHostToDevice));
+  int launches = 0;
+  auto run = [&]() -> int {
+    if (stages & ST_BEGIN)
+      CK(newton_begin(B.d, nprob, begin_args[0], (int)begin_args[1], (int)begin_args[2], begin_args[3] != 0.0, begin_args[4] != 0.0, s->stream, &launches));
+    if (stages & ST_DECIDE) CK(k1_reduce_decide(B.d, nprob, Dt, s->stream, &launches, spec));
+    if (stages & ST_CG_BEGIN) CK(cg_begin(B.d, nprob, s->stream, &launches));
+    if (stages & ST_CG_INIT) CK(cg_init(B.d, nprob, Dt, s->stream, &launches));
+    if (stages & ST_CG_STEP) CK(cg_step(B.d, nprob, Dt, s->stream, &launches));
+    if (stages & ST_CG_POLL) {
+      CK(cg_poll(B.d, nprob, s->d_flag + 2, s->stream, &launches));
+      CK(cudaMemcpyAsync(s->h_flag + 2, s->d_flag + 2, sizeof(int), cudaMemcpyDeviceToHost, s->stream));
+    }
+    if (stages & ST_SOLVE) CK(newton_solve(B.d, nprob, B.ldh, s->stream, &launches, B.group_L));
+    if (stages & ST_FINISH) CK(newton_finish(B.d, nprob, Dt, s->stream, &launches));
+    CK(cudaStreamSynchronize(s->stream));
+    if (stages & ST_CG_POLL) *cg_any = s->h_flag[2];
+    CK(cudaMemcpy(c.data(), B.d_ctrl, (size_t)nprob * sizeof(Ctrl), cudaMemcpyDeviceToHost));
+    StageCtrl* out = static_cast<StageCtrl*>(ctrl);
+    for (int b = 0; b < nprob; b++) ctrl_to_stage(c[b], out[b]);
+    return stage_exchange(B, ldx, false, vec, ring, fvec);
+  };
+  const int rc = run();
+  cudaStreamSynchronize(s->stream);
+  for (int b = 0; b < nprob; b++) {
+    Ctrl& x = c0[b];
+    x.done = 1; x.hess_valid = 0; x.need_solve = 0; x.need_hess = 0; x.have_dir = 0; x.bfgs_count = 0; x.h0_scale = 1.0;
+    x.skip_eval = 0; x.refresh_next = 0; x.cg_active = 0; x.k1_chunks = 0; x.fail = 0;
+  }
+  CK(cudaMemcpy(B.d_ctrl, c0.data(), (size_t)nprob * sizeof(Ctrl), cudaMemcpyHostToDevice));
+  B.mirror.clear();
+  s->cnt.launches += launches;
+  return rc;
+}
+
+// Test hook, not part of the C ABI: one real x-update of the begun ADMM batch (at most 64 problems), slot by slot, through batch_slot
+// -- the slot code batch_xupdate runs: K1, the decide kernel, the Gram / Cholesky launches of a rebuild, the matrix-free direction,
+// newton_solve / newton_finish.  args = {xtol (<= 0: the session's), max_newton (<= 0: the session's), policy, invalidate}; a
+// matrix-free batch runs policy 2 whatever is asked, as in batch_xupdate.  newton_begin, then slots until every problem is done or
+// max_slots have run.  spec[i] != 0 asks for slot i in speculative form (no rebuild launches); it is honoured as batch_xupdate
+// would: only when, as of the state before slot i - 1, every running problem had a valid factor and no rebuild was due.  A regular
+// slot includes the rebuild launches iff a running problem has emit set.  Refused before any launch: spec under a policy other than
+// 0, spec for slot 0, a batch of more than 64 problems (batch_xupdate never speculates there).
+// The trace has max_slots + 1 entries, entry 0 the state newton_begin left and entry i + 1 the state after slot i, each in the
+// layout of mlease_internal_newton_stage (ctrl: nprob StageCtrl; vec, ring, fvec); slot_info (2 ints per slot): ran speculatively,
+// included the rebuild launches; *nslots = slots run.  The batch is left as after an x-update (beta = x).
+int mlease_internal_xupdate_trace(mlease_session* s, const double* args, const int32_t* spec, int32_t max_slots, void* ctrl_trace,
+                                  double* vec_trace, double* ring_trace, float* fvec_trace, int32_t* slot_info, int32_t* nslots) {
+  if (!s || !args || !spec || !ctrl_trace || !vec_trace || !ring_trace || !fvec_trace || !slot_info || !nslots) return fail(MLEASE_ERR_INVALID, "null argument");
+  if (!s->batch || !s->begun) return fail(MLEASE_ERR_STATE, "mlease_admm_begin was not called");
+  Batch& B = *s->batch;
+  if (max_slots < 1 || max_slots > 400) return fail(MLEASE_ERR_INVALID, "max_slots out of range");
+  if (B.nprob > 64) return fail(MLEASE_ERR_INVALID, "the slot trace follows batches of at most 64 problems");
+  if (!(args[2] == 0.0 || args[2] == 1.0 || args[2] == 2.0)) return fail(MLEASE_ERR_INVALID, "policy must be 0, 1 or 2");
+  const int policy = B.matfree ? 2 : (int)args[2];
+  if (policy == 2 && !B.matfree) return fail(MLEASE_ERR_INVALID, "policy 2 needs a matrix-free batch");
+  for (int i = 0; i < max_slots; i++)
+    if (spec[i] && (policy != 0 || i == 0)) return fail(MLEASE_ERR_INVALID, "batch_xupdate speculates only under policy 0 and never on slot 0");
+  CK(cudaSetDevice(s->cfg.device));
+  const int nprob = B.nprob, ldx = s->ldx;
+  const double xtol = args[0] > 0.0 ? args[0] : s->xtol;
+  const int max_newton = args[1] > 0.0 ? (int)args[1] : s->max_newton;
+  const size_t ring_n = 2 * (size_t)BFGS_M * ldx + 2 * BFGS_M;
+  Profiler nop;
+  int launches = 0;
+  double shared_flops = 0;
+  std::vector<Ctrl> c(nprob);
+  auto record = [&](int entry) -> int {
+    CK(cudaStreamSynchronize(s->stream));
+    CK(cudaMemcpy(c.data(), B.d_ctrl, (size_t)nprob * sizeof(Ctrl), cudaMemcpyDeviceToHost));
+    StageCtrl* out = static_cast<StageCtrl*>(ctrl_trace) + (size_t)entry * nprob;
+    for (int b = 0; b < nprob; b++) ctrl_to_stage(c[b], out[b]);
+    return stage_exchange(B, ldx, false, vec_trace + (size_t)entry * nprob * STAGE_NVEC * ldx, ring_trace + (size_t)entry * nprob * ring_n,
+                          fvec_trace + (size_t)entry * nprob * 3 * ldx);
+  };
+  // flags of the read-back state: 1 a problem runs, 2 a rebuild is due; *valid: every running problem has a factor
+  auto flags = [&](bool* valid) {
+    int f = 0; *valid = true;
+    for (int b = 0; b < nprob; b++) if (!c[b].done) { f |= 1; if (c[b].emit) f |= 2; if (!c[b].hess_valid) *valid = false; }
+    return f;
+  };
+  CK(newton_begin(B.d, nprob, xtol, max_newton, policy, args[3] != 0.0, B.rebuild_is_expensive, s->stream, &launches));
+  if (int rc = record(0)) return rc;
+  bool valid_now, valid_before = false;
+  int flag_now = flags(&valid_now), flag_before = 2;   // nothing is known before slot 0: no speculation on slot 1 unless slot 0's outcome allows it
+  if (!B.matfree) { valid_before = valid_now; flag_before = flag_now; }   // (the host's prediction of slot 0 equals what newton_begin left)
+  int slots = 0;
+  while ((flag_now & 1) && slots < max_slots) {
+    const bool sp = spec[slots] && valid_before && !(flag_before & 2);
+    const bool with_hess = !sp && (flag_now & 2) && !B.matfree;
+    const SlotCtx x{s->stream, &nop, &launches, B.d, nprob, 0, 0, &shared_flops, s->h_flag, s->d_flag, false};
+    if (int rc = batch_slot(B, x, slots, with_hess, sp)) return rc;
+    slot_info[2 * slots] = sp ? 1 : 0; slot_info[2 * slots + 1] = with_hess ? 1 : 0;
+    valid_before = valid_now; flag_before = flag_now;
+    if (int rc = record(slots + 1)) return rc;
+    flag_now = flags(&valid_now);
+    slots++;
+  }
+  *nslots = slots;
+  B.mirror = c;
+  s->cnt.launches += launches;
+  return 0;
+}
+
 // Test hooks of the factored direction of wide systems (ldh > 2048), not part of the C ABI.  Each refuses, before any launch, a
 // batch that has no Ysym (ldh <= 2048, or matrix-free), since the kernels they run dereference it.
 //

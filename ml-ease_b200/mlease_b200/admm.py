@@ -609,6 +609,80 @@ def _internal_direction(session, active, g, S, Y, rho, count, h0, beta):
     return out
 
 
+STAGE_INTS = ("done", "have_dir", "need_solve", "need_hess", "emit", "hess_valid", "fail", "newton_steps", "evals", "rejects",
+              "hess_builds", "stall", "bfgs_count", "k1_chunks", "refresh_next", "skip_eval", "warm_used", "build_step", "max_newton",
+              "hess_policy", "rebuild_is_expensive", "cg_active", "cg_iter", "pad_")
+STAGE_REALS = ("h0_scale", "worst_ratio", "alpha", "phi0", "f_acc", "f_t", "gnorm", "gnorm_prev", "dirnorm", "dirnorm_prev", "xtol",
+               "cg_rz", "cg_g2", "hv_vinf", "tot_evals", "tot_newton", "tot_rejects", "tot_hess")
+STAGE_CTRL = np.dtype([(k, np.int32) for k in STAGE_INTS] + [(k, np.float64) for k in STAGE_REALS])   # StageCtrl of test_hooks.cu
+STAGE_VECS = ("beta", "beta_t", "m", "q", "g_t", "g_acc", "dir", "cg_r", "cg_p", "cg_z", "cg_Hp", "cg_diag")
+STAGES = dict(begin=1, decide=2, solve=4, finish=8, cg_begin=16, cg_init=32, cg_step=64, cg_poll=128)
+
+
+def _internal_newton_stage(session, stages=(), ctrl=None, vec=None, ring=None, fvec=None, gpart=None, fpart=None, spec=0, begin_args=None):
+    """Test hook (not part of the C ABI): inject an x-update state into every problem of the ADMM batch (after begin()), run the
+    kernels named in `stages` (keys of STAGES) once through the solver's launchers, read the state back.  ctrl [nprob] STAGE_CTRL;
+    vec [nprob, 12, ldx] (STAGE_VECS); ring [nprob, 2 BFGS_M ldx + 2 BFGS_M] (S, Y, rho, alpha); fvec [nprob, 3, ldx] float32
+    (beta_tf, qf = hv_vf, tf); gpart [nprob, nct, ldx], fpart [nprob, nct] or None; begin_args (xtol, max_newton, policy,
+    invalidate, expensive).  Without stages: info only.  Consumes the batch's x-update state.
+    -> dict(info=dict(nprob, Dt, ldx, ldh, part_rows, fused, matrix_free, ysym, expensive, group_L), ctrl, vec, ring, fvec, cg_any)."""
+    mask = 0
+    for k in stages:
+        mask |= STAGES[k]
+    info = np.zeros(12, np.int32)
+    cg_any = C.c_int32(-1)
+    fn = lib().mlease_internal_newton_stage
+    vp = C.c_void_p
+    fn.argtypes, fn.restype = [vp, C.c_int32, C.c_int32] + [vp] * 7 + [C.c_int32, vp, C.POINTER(C.c_int32)], C.c_int
+    out = {}
+    nct = 0
+    if mask:
+        out["ctrl"] = np.array(ctrl, STAGE_CTRL, copy=True)
+        out["vec"] = np.array(vec, np.float64, copy=True, order="C")
+        out["ring"] = np.array(ring, np.float64, copy=True, order="C")
+        out["fvec"] = np.array(fvec, np.float32, copy=True, order="C")
+        gpart = None if gpart is None else np.ascontiguousarray(gpart, np.float64)
+        fpart = None if fpart is None else np.ascontiguousarray(fpart, np.float64)
+        nct = 0 if fpart is None else fpart.shape[1]
+        begin_args = None if begin_args is None else np.ascontiguousarray(begin_args, np.float64)
+    check(fn(session._h, mask, int(spec), ptr(begin_args) if mask else None, ptr(out.get("ctrl")), ptr(out.get("vec")),
+             ptr(out.get("ring")), ptr(out.get("fvec")), ptr(gpart) if mask else None, ptr(fpart) if mask else None, nct,
+             info.ctypes.data, C.byref(cg_any)))
+    out["info"] = dict(zip(("nprob", "Dt", "ldx", "ldh", "part_rows", "fused", "matrix_free", "ysym", "expensive", "group_L"),
+                           (int(x) for x in info)))
+    out["cg_any"] = cg_any.value
+    return out
+
+
+def _internal_xupdate_trace(session, policy=0, invalidate=0, spec=(), max_slots=60, xtol=0.0, max_newton=0):
+    """Test hook (not part of the C ABI): one real x-update of the ADMM batch, slot by slot through the solver's own slot code.
+    spec: slot indices asked to run speculatively (policy 0 only, never slot 0).  xtol / max_newton 0: the session's.
+    -> dict(nslots, spec [nslots], with_hess [nslots], ctrl [nslots + 1, nprob] STAGE_CTRL, vec [nslots + 1, nprob, 12, ldx],
+    ring [nslots + 1, nprob, 2 BFGS_M ldx + 2 BFGS_M], fvec [nslots + 1, nprob, 3, ldx]); entry 0 is the state newton_begin left,
+    entry i + 1 the state after slot i."""
+    info = _internal_newton_stage(session)["info"]
+    nprob, ldx = info["nprob"], info["ldx"]
+    sp = np.zeros(max_slots, np.int32)
+    for i in spec:
+        if i < max_slots:
+            sp[i] = 1
+    ctrl = np.zeros((max_slots + 1, nprob), STAGE_CTRL)
+    vec = np.zeros((max_slots + 1, nprob, 12, ldx))
+    ring = np.zeros((max_slots + 1, nprob, 2 * BFGS_M * ldx + 2 * BFGS_M))
+    fvec = np.zeros((max_slots + 1, nprob, 3, ldx), np.float32)
+    sinfo = np.zeros((max_slots, 2), np.int32)
+    n = C.c_int32(0)
+    args = np.array([xtol, max_newton, policy, invalidate], np.float64)
+    fn = lib().mlease_internal_xupdate_trace
+    vp = C.c_void_p
+    fn.argtypes, fn.restype = [vp, vp, vp, C.c_int32, vp, vp, vp, vp, vp, C.POINTER(C.c_int32)], C.c_int
+    check(fn(session._h, args.ctypes.data, sp.ctypes.data, int(max_slots), ctrl.ctypes.data, vec.ctypes.data, ring.ctypes.data,
+             fvec.ctypes.data, sinfo.ctypes.data, C.byref(n)))
+    k = n.value
+    return dict(nslots=k, spec=sinfo[:k, 0].copy(), with_hess=sinfo[:k, 1].copy(), ctrl=ctrl[:k + 1], vec=vec[:k + 1], ring=ring[:k + 1],
+                fvec=fvec[:k + 1], info=info)
+
+
 def _internal_keyed_last_call():
     """Test hook: the most recent keyed call of the process -> (key boundaries of its chunks, streamed, stage ms, wait ms)."""
     fn = lib().mlease_internal_keyed_last_call
