@@ -254,6 +254,12 @@ namespace mlease {
 int scratch_for(mlease_session* s, int pid, Batch** B);
 int load_hv(Batch& B, int b, const double* v, cudaStream_t st);
 int reset_ctrl(Batch& B);
+// session.cu: the reducers' rho of iteration `iter` for lambda l (the boost at iteration 1, then rho.adapt.coefficient), and the z/u
+// update of an iteration around the caller's one stream synchronisation: consensus_enqueue (rho of the next iteration to d_rho, K4 on
+// the summed exchange, read-back of the per-lambda diff), consensus_finish (maxdiff, mindiff, the stop rule)
+double rho_eff_for_iter(mlease_session* s, int l, int iter);
+int consensus_enqueue(mlease_session* s, const double* exchange_sum_dev);
+void consensus_finish(mlease_session* s, double* maxdiff, int32_t* stop);
 // ingest.cu: checks and derived lists of one uploaded CSR partition
 int csr_build_layout(mlease_session* s, PartData& pd);
 // comm.cu: in-place sum of `count` doubles over the communicator's ranks on `st`

@@ -85,7 +85,12 @@ __global__ void __launch_bounds__(256) admm_consensus_kernel(const Problem* __re
       zn = wz[(size_t)l * ldv + k] * (exch[(size_t)l * Dt + k] * invP);
     }
     const double zo = z[(size_t)l * ldv + k];
-    dmax = fmax(dmax, fabs(zo - zn));
+    const double dk = fabs(zo - zn);
+    dmax = fmax(dmax, dk);
+    // LinearModel.maxAbsValue (models/LinearModel.java:728-740) starts from |intercept diff| and skips a NaN coefficient diff
+    // (`maxabs < v` is false), as fmax does; a NaN at the intercept is the lambda's diff whatever follows.  fabs leaves a positive
+    // NaN, whose bit pattern orders above every other non-negative double in the atomicMax below.
+    if (k == Dt - 1 && dk != dk) atomicMax(reinterpret_cast<unsigned long long*>(diff + l), (unsigned long long)__double_as_longlong(dk));
     z[(size_t)l * ldv + k] = zn;
     const float zf = (float)zn;
     for (int p = 0; p < nparts; p++) {

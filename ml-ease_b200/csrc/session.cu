@@ -127,19 +127,21 @@ int ensure_scratch(mlease_session* s, int part_idx) {
   return batch_alloc(*B, s->num_sms, s->cfg.hessian_policy, s->csr_gram_force);
 }
 
-double rho_eff_for_iter(mlease_session* s, int l, int iter) {
+}  // namespace
+
+double mlease::rho_eff_for_iter(mlease_session* s, int l, int iter) {
   // reducer: rho = lambdaRho[lambda] (float -> double), times rho.adapt.rate if != 1 (jobs/RegressionAdmmTrain.java:652-658);
   // rate = (float) exp(-(i-1)*coef) for i > 1 (:323-327)
   double r = (double)s->rhos[l];
   // rho.adapt.rate is a key of the per-iteration JobConf, which the driver re-creates every iteration (:286-291 ->
   // com/linkedin/mapred/AbstractAvroJob.java:101-115): the boost is seen by the reducers of iteration 1 only (:313-316)
   float rate = (iter == 1 && s->boost_rate > 0.f) ? s->boost_rate : 1.0f;
-  if (iter > 1 && s->cfg.rho_adapt_coefficient > 0) rate = (float)std::exp(-(iter - 1) * s->cfg.rho_adapt_coefficient);
+  // the product is float (int times float), the exponential double (Math.exp): std::exp of the float would be expf, which rounds
+  // differently for some arguments (coefficient 0.289 at iteration 2: 0.74901223f instead of 0.7490122f)
+  if (iter > 1 && s->cfg.rho_adapt_coefficient > 0) rate = (float)std::exp((double)(-(iter - 1) * s->cfg.rho_adapt_coefficient));
   if (rate != 1.0f) r = r * (double)rate;
   return r;
 }
-
-}  // namespace
 
 int mlease::scratch_for(mlease_session* s, int pid, Batch** B) {
   CK(cudaSetDevice(s->cfg.device));
@@ -375,9 +377,11 @@ int mlease_admm_local_step(mlease_session* s, double* exchange_dev) {
   return 0;
 }
 
+}  // extern "C"
+
 // z/u update of the iteration: enqueue (kernel + read-back of the per-lambda |z - z_prev| into pinned memory), then, after the
 // caller's ONE stream synchronisation, finish (convergence scalars, stop rule :493-496).
-static int consensus_enqueue(mlease_session* s, const double* exchange_sum_dev) {
+int mlease::consensus_enqueue(mlease_session* s, const double* exchange_sum_dev) {
   for (int l = 0; l < s->L; l++) s->h_small[l] = rho_eff_for_iter(s, l, s->iter + 1);
   CK(cudaMemcpyAsync(s->d_rho, s->h_small, s->L * sizeof(double), cudaMemcpyHostToDevice, s->stream));
   int launches = 0;
@@ -386,7 +390,7 @@ static int consensus_enqueue(mlease_session* s, const double* exchange_sum_dev) 
   CK(cudaMemcpyAsync(s->h_small + s->L, s->d_diff, s->L * sizeof(double), cudaMemcpyDeviceToHost, s->stream));
   return 0;
 }
-static void consensus_finish(mlease_session* s, double* maxdiff, int32_t* stop) {
+void mlease::consensus_finish(mlease_session* s, double* maxdiff, int32_t* stop) {
   const double* hd = s->h_small + s->L;
   double mx = 0, mn = 99999999;
   for (int l = 0; l < s->L; l++) { mx = std::max(mx, hd[l]); mn = std::min(mn, hd[l]); }
@@ -395,6 +399,8 @@ static void consensus_finish(mlease_session* s, double* maxdiff, int32_t* stop) 
   const double eps = s->cfg.epsilon >= 0 ? s->cfg.epsilon : 0.0001;   // default 1e-4 (:473); 0 = never stop early
   if (stop) *stop = (mx < eps && s->liblinear_eps <= 0.00001) ? 1 : 0;   // :493-496
 }
+
+extern "C" {
 
 int mlease_admm_consensus(mlease_session* s, const double* exchange_sum_dev, double* maxdiff, int32_t* stop) {
   if (!s || !exchange_sum_dev) return fail(MLEASE_ERR_INVALID, "null argument");

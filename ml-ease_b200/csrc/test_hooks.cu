@@ -809,3 +809,138 @@ int mlease_internal_dmma_shapes(const double* A, const double* B, int32_t n, int
 }
 
 }  // extern "C"
+
+namespace {
+enum { CS_RESET = 1, CS_INIT = 2, CS_PACK = 4, CS_CONSENSUS = 8 };
+constexpr int CS_NVEC = 5, CS_NFVEC = 3, CS_NCTRL = 3;
+// Every problem's K4 vectors and the session's z / exchange / diff to the device (h2d) or back, in the layout of
+// mlease_internal_consensus.
+int consensus_exchange(mlease_session* s, bool h2d, double* vec, float* fvec, double* z, double* exch, double* diff) {
+  Batch& B = *s->batch;
+  const int ldx = s->ldx;
+  auto cp = [&](void* dev, void* host, size_t bytes) {
+    return h2d ? cudaMemcpy(dev, host, bytes, cudaMemcpyHostToDevice) : cudaMemcpy(host, dev, bytes, cudaMemcpyDeviceToHost);
+  };
+  for (int b = 0; b < B.nprob; b++) {
+    const Problem& p = B.h[b];
+    double* v[CS_NVEC] = {p.beta, p.m, p.q, p.g_t, p.x_d};
+    float* f[CS_NFVEC] = {p.u_f, p.uplusx_f, p.x_f};
+    for (int i = 0; i < CS_NVEC; i++) CK(cp(v[i], vec + ((size_t)b * CS_NVEC + i) * ldx, (size_t)ldx * sizeof(double)));
+    for (int i = 0; i < CS_NFVEC; i++) CK(cp(f[i], fvec + ((size_t)b * CS_NFVEC + i) * ldx, (size_t)ldx * sizeof(float)));
+  }
+  CK(cp(s->d_z, z, (size_t)s->L * ldx * sizeof(double)));
+  CK(cp(s->d_exch, exch, ((size_t)s->L * s->Dt + 1) * sizeof(double)));
+  CK(cp(s->d_diff, diff, (size_t)s->L * sizeof(double)));
+  return 0;
+}
+}  // namespace
+
+extern "C" {
+
+// Test hook, not part of the C ABI: the consensus step (K4, k4_consensus.cu) of the begun ADMM batch on an injected state.
+//   stages: CS_RESET (d_rho = rho of iteration 1, then admm_reset, as begin() runs them), CS_INIT (admm_init on the injected z, as
+//   begin_initialized() runs it; not on an L1 session), CS_PACK (admm_pack into the session's exchange buffer), CS_CONSENSUS (the
+//   session's own consensus_enqueue on that buffer, one stream synchronisation, consensus_finish, with s->iter = args[0] >= 1 and
+//   s->liblinear_eps = (float)args[1]).  They run in that order.  stages = 0 injects and runs nothing: it reads the state back
+//   (or only info when vec is NULL).
+//   vec: nprob x 5 x ldx doubles (beta, m, q, g_t, x_d), fvec: nprob x 3 x ldx floats (u_f, uplusx_f, x_f), z: L x ldx, exch: L Dt + 1
+//   (the last slot is the failed-fit count), diff: L, ctrl: nprob x 3 ints (Ctrl::hess_valid, skip_eval, k1_chunks); all in and out,
+//   whole vectors, padding included, copied as bytes.  ctrl_raw (out, may be NULL): 2 x nprob x sizeof(Ctrl) bytes, every problem's
+//   Ctrl just before the first stage and after the last one, with the three fields of ctrl zeroed in both.  wz (L x ldx), l1thr (L;
+//   NULL on an L2 session) and rho (L): the z-weights, L1 thresholds and d_rho the kernels read, as the last stage left d_rho.
+//   res (3 doubles, CS_CONSENSUS): maxdiff, the session's mindiff, stop.
+//   info (12 ints): nprob, Dt, ldx, L, P, local partitions, CSR, fused K1 (gpart_f present), matrix-free, regularizer, k1_grid,
+//   sizeof(Ctrl).
+// Every kernel of K4 indexes by Dt, ldx, L and the problem count alone; k1_chunks is still refused beyond the partial rows the batch
+// allocated.  Refused before any launch: no begun batch, a stage mask outside [0, 15], CS_INIT on an L1 session, CS_CONSENSUS
+// without args or with args[0] < 1, a null array.  With stages set, the batch's x-update state is consumed (every problem is left
+// done, as by mlease_internal_newton_stage): begin() again before iterating; s->iter, liblinear_eps, mindiff and last_maxdiff are
+// restored.
+int mlease_internal_consensus(mlease_session* s, int32_t stages, const double* args, double* vec, float* fvec, double* z, double* exch,
+                              double* diff, int32_t* ctrl, uint8_t* ctrl_raw, double* wz, double* l1thr, double* rho, double* res,
+                              int32_t* info) {
+  if (!s || !info) return fail(MLEASE_ERR_INVALID, "null argument");
+  if (!s->batch || !s->begun) return fail(MLEASE_ERR_STATE, "mlease_admm_begin was not called");
+  Batch& B = *s->batch;
+  const int nprob = B.nprob, L = s->L, ldx = s->ldx;
+  const int32_t inf[12] = {nprob, s->Dt, ldx, L, s->P, (int)s->parts.size(), B.csr ? 1 : 0, B.h[0].gpart_f ? 1 : 0, B.matfree,
+                           s->cfg.regularizer, B.k1_grid, (int)sizeof(Ctrl)};
+  std::copy(inf, inf + 12, info);
+  if (stages < 0 || stages > 15) return fail(MLEASE_ERR_INVALID, "stage mask out of range");
+  if (stages == 0 && !vec) return 0;
+  if (!vec || !fvec || !z || !exch || !diff || !ctrl || !wz || !rho || !res || (s->cfg.regularizer == 1 && !l1thr))
+    return fail(MLEASE_ERR_INVALID, "null argument");
+  if ((stages & CS_INIT) && s->cfg.regularizer != 2) return fail(MLEASE_ERR_INVALID, "admm_init runs on L2 sessions only (begin_initialized)");
+  if ((stages & CS_CONSENSUS) && (!args || !(args[0] >= 1.0 && args[0] <= 1e9)))
+    return fail(MLEASE_ERR_INVALID, "the consensus step needs args = {iter >= 1, liblinear_eps}");
+  if (stages)
+    for (int b = 0; b < nprob; b++)
+      if (ctrl[3 * b + 2] < 0 || ctrl[3 * b + 2] > B.k1_grid) return fail(MLEASE_ERR_INVALID, "k1_chunks beyond the partial rows the batch allocated");
+  CK(cudaSetDevice(s->cfg.device));
+  std::vector<Ctrl> c0(nprob), c(nprob);
+  auto raw = [&](int which) {   // Ctrl bytes without the three fields the caller exchanges
+    if (!ctrl_raw) return;
+    for (int b = 0; b < nprob; b++) {
+      Ctrl x = c[b];
+      x.hess_valid = 0; x.skip_eval = 0; x.k1_chunks = 0;
+      std::memcpy(ctrl_raw + ((size_t)which * nprob + b) * sizeof(Ctrl), &x, sizeof(Ctrl));
+    }
+  };
+  CK(cudaStreamSynchronize(s->stream));
+  CK(cudaMemcpy(c0.data(), B.d_ctrl, (size_t)nprob * sizeof(Ctrl), cudaMemcpyDeviceToHost));
+  c = c0;
+  const int iter0 = s->iter;
+  const float eps0 = s->liblinear_eps;
+  const double mindiff0 = s->mindiff, maxdiff0 = s->last_maxdiff;
+  int launches = 0;
+  auto run = [&]() -> int {
+    if (stages) {
+      if (int rc = consensus_exchange(s, true, vec, fvec, z, exch, diff)) return rc;
+      for (int b = 0; b < nprob; b++) { c[b].hess_valid = ctrl[3 * b]; c[b].skip_eval = ctrl[3 * b + 1]; c[b].k1_chunks = ctrl[3 * b + 2]; }
+      CK(cudaMemcpy(B.d_ctrl, c.data(), (size_t)nprob * sizeof(Ctrl), cudaMemcpyHostToDevice));
+    }
+    raw(0);
+    if (stages & CS_RESET) {
+      for (int l = 0; l < L; l++) s->h_small[l] = rho_eff_for_iter(s, l, 1);
+      CK(cudaMemcpyAsync(s->d_rho, s->h_small, L * sizeof(double), cudaMemcpyHostToDevice, s->stream));
+      CK(admm_reset(B.d, nprob, L, s->d_z, ldx, s->d_rho, s->stream, &launches));
+      CK(cudaStreamSynchronize(s->stream));   // h_small is reused below
+    }
+    if (stages & CS_INIT) CK(admm_init(B.d, nprob, s->d_z, ldx, s->stream, &launches));
+    if (stages & CS_PACK) CK(admm_pack(B.d, (int)s->parts.size(), L, s->Dt, s->d_exch, s->stream, &launches));
+    if (stages & CS_CONSENSUS) {
+      s->iter = (int)args[0];
+      s->liblinear_eps = (float)args[1];
+      double md = 0;
+      int32_t stop = 0;
+      if (int rc = consensus_enqueue(s, s->d_exch)) return rc;
+      CK(cudaStreamSynchronize(s->stream));
+      consensus_finish(s, &md, &stop);
+      res[0] = md; res[1] = s->mindiff; res[2] = stop;
+    }
+    CK(cudaStreamSynchronize(s->stream));
+    if (int rc = consensus_exchange(s, false, vec, fvec, z, exch, diff)) return rc;
+    CK(cudaMemcpy(c.data(), B.d_ctrl, (size_t)nprob * sizeof(Ctrl), cudaMemcpyDeviceToHost));
+    for (int b = 0; b < nprob; b++) { ctrl[3 * b] = c[b].hess_valid; ctrl[3 * b + 1] = c[b].skip_eval; ctrl[3 * b + 2] = c[b].k1_chunks; }
+    raw(1);
+    CK(cudaMemcpy(wz, s->d_wz, (size_t)L * ldx * sizeof(double), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(rho, s->d_rho, (size_t)L * sizeof(double), cudaMemcpyDeviceToHost));
+    if (s->d_l1thr) CK(cudaMemcpy(l1thr, s->d_l1thr, (size_t)L * sizeof(double), cudaMemcpyDeviceToHost));
+    return 0;
+  };
+  const int rc = run();
+  cudaStreamSynchronize(s->stream);
+  s->iter = iter0; s->liblinear_eps = eps0; s->mindiff = mindiff0; s->last_maxdiff = maxdiff0;
+  s->cnt.launches += launches;
+  if (!stages) return rc;
+  for (int b = 0; b < nprob; b++) {
+    Ctrl& x = c0[b];
+    x.done = 1; x.hess_valid = 0; x.need_solve = 0; x.need_hess = 0; x.have_dir = 0; x.bfgs_count = 0; x.h0_scale = 1.0;
+    x.skip_eval = 0; x.refresh_next = 0; x.cg_active = 0; x.k1_chunks = 0; x.fail = 0;
+  }
+  CK(cudaMemcpy(B.d_ctrl, c0.data(), (size_t)nprob * sizeof(Ctrl), cudaMemcpyHostToDevice));
+  B.mirror.clear();
+  return rc;
+}
+
+}  // extern "C"

@@ -683,6 +683,55 @@ def _internal_xupdate_trace(session, policy=0, invalidate=0, spec=(), max_slots=
                 fvec=fvec[:k + 1], info=info)
 
 
+CONSENSUS_VECS = ("beta", "m", "q", "g_t", "x_d")
+CONSENSUS_FVECS = ("u_f", "uplusx_f", "x_f")
+CONSENSUS_CTRL = ("hess_valid", "skip_eval", "k1_chunks")
+CONSENSUS_STAGES = dict(reset=1, init=2, pack=4, consensus=8)
+CONSENSUS_INFO = ("nprob", "Dt", "ldx", "L", "P", "nlocal", "csr", "fused", "matrix_free", "regularizer", "k1_grid", "ctrl_bytes")
+
+
+def _internal_consensus(session, stages=(), state=None, iter=1, liblinear_eps=0.01, read=True):
+    """Test hook (not part of the C ABI): inject a K4 state into the begun ADMM batch, run the stages named in `stages` (keys of
+    CONSENSUS_STAGES, run in the order reset, init, pack, consensus) through the solver's own code, read everything back.  state:
+    dict(vec [nprob, 5, ldx] (CONSENSUS_VECS), fvec [nprob, 3, ldx] float32 (CONSENSUS_FVECS), z [L, ldx], exch [L Dt + 1],
+    diff [L], ctrl [nprob, 3] int32 (CONSENSUS_CTRL)), whole vectors with their padding.  The consensus stage runs with the session's
+    iteration counter at `iter` and its liblinear epsilon at `liblinear_eps`.  Without stages nothing is injected: the state is read
+    (read=False: info only).  With stages the batch's x-update state is consumed: begin() again before iterating.
+    -> dict(info, the state's keys after the last stage, ctrl_raw [2, nprob, ctrl_bytes] uint8 (before / after, the three ctrl
+    fields zeroed), wz [L, ldx], l1thr [L] or None, rho [L], maxdiff, mindiff, stop)."""
+    mask = stages if isinstance(stages, int) else 0   # (a raw mask: lets a test pass one the hook must refuse)
+    for k in ([] if isinstance(stages, int) else stages):
+        mask |= CONSENSUS_STAGES[k]
+    info = np.zeros(12, np.int32)
+    fn = lib().mlease_internal_consensus
+    vp = C.c_void_p
+    fn.argtypes, fn.restype = [vp, C.c_int32] + [vp] * 13, C.c_int
+    check(fn(session._h, 0, None, None, None, None, None, None, None, None, None, None, None, None, info.ctypes.data))
+    inf = dict(zip(CONSENSUS_INFO, (int(x) for x in info)))
+    if not mask and not read:
+        return dict(info=inf)
+    nprob, L, Dt, ldx = inf["nprob"], inf["L"], inf["Dt"], inf["ldx"]
+    if mask:
+        out = dict(vec=np.array(state["vec"], np.float64, copy=True, order="C"), fvec=np.array(state["fvec"], np.float32, copy=True, order="C"),
+                   z=np.array(state["z"], np.float64, copy=True, order="C"), exch=np.array(state["exch"], np.float64, copy=True, order="C"),
+                   diff=np.array(state["diff"], np.float64, copy=True, order="C"), ctrl=np.array(state["ctrl"], np.int32, copy=True, order="C"))
+        if out["vec"].shape != (nprob, 5, ldx) or out["fvec"].shape != (nprob, 3, ldx) or out["z"].shape != (L, ldx) or \
+                out["exch"].shape != (L * Dt + 1,) or out["diff"].shape != (L,) or out["ctrl"].shape != (nprob, 3):
+            raise ValueError("state arrays do not match the batch")
+    else:
+        out = dict(vec=np.zeros((nprob, 5, ldx)), fvec=np.zeros((nprob, 3, ldx), np.float32), z=np.zeros((L, ldx)),
+                   exch=np.zeros(L * Dt + 1), diff=np.zeros(L), ctrl=np.zeros((nprob, 3), np.int32))
+    out.update(ctrl_raw=np.zeros((2, nprob, inf["ctrl_bytes"]), np.uint8), wz=np.zeros((L, ldx)),
+               l1thr=np.zeros(L) if inf["regularizer"] == 1 else None, rho=np.zeros(L))
+    res = np.zeros(3)
+    args = np.array([iter, liblinear_eps], np.float64)
+    check(fn(session._h, mask, args.ctypes.data, out["vec"].ctypes.data, out["fvec"].ctypes.data, out["z"].ctypes.data,
+             out["exch"].ctypes.data, out["diff"].ctypes.data, out["ctrl"].ctypes.data, out["ctrl_raw"].ctypes.data, out["wz"].ctypes.data,
+             ptr(out["l1thr"]), out["rho"].ctypes.data, res.ctypes.data, info.ctypes.data))
+    out.update(info=inf, maxdiff=float(res[0]), mindiff=float(res[1]), stop=int(res[2]))
+    return out
+
+
 def _internal_keyed_last_call():
     """Test hook: the most recent keyed call of the process -> (key boundaries of its chunks, streamed, stage ms, wait ms)."""
     fn = lib().mlease_internal_keyed_last_call

@@ -622,7 +622,7 @@ int orc_admm_run(int P, int Dg, const int64_t* part_rowstart, const int64_t* row
       for (int p = 0; p < P; p++)
         for (int l = 0; l < L; l++)
           for (int k = 0; k < Dt; k++) u[p * L + l][k] = (float)((double)uplusx[p * L + l][k] + (-1.0) * z[l][k]);
-      if (rho_adapt_coefficient > 0) rhoAdaptRate = (float)std::exp(-(i - 1) * rho_adapt_coefficient);  // :323-327
+      if (rho_adapt_coefficient > 0) rhoAdaptRate = (float)std::exp((double)(-(i - 1) * rho_adapt_coefficient));  // :323-327 (Math.exp: double)
     }
     // z as the reducers see it: float (:330-331)
     std::vector<std::vector<float>> zf(L, std::vector<float>(Dt));
