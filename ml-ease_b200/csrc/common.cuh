@@ -111,6 +111,7 @@ struct Problem {
   const long long* sg_goff;         // [sg_S][sg_ngrp] first 32-lane row of the group in sg_row16 / sg_val
   const unsigned short* sg_row16;   // [..][32] row inside the segment
   const float* sg_val;              // [..][32] value (0 in padding slots)
+  const unsigned short* sg_col16;   // [nnz] colidx as 16-bit ids (the fused kernel's phase A reads these: 6 instead of 8 B per value)
   float* gpart_f;                   // [sg_S][ldx] per-segment partial gradients when the fused K1 runs (else NULL; gpart is used)
   float* sdvec;            // [n] sqrt(d_i) written by K1 when the Gram is assembled straight from CSR (no Xt)
   float* rvec;             // [n] row residuals r_i, only for CSR partitions wider than one K1 column window (else NULL)

@@ -228,11 +228,12 @@ int csr_build_layout(mlease_session* s, PartData& pd) {
     // segment lists of the fused multi-lambda K1
     int S = 0, rows = 0, LP = 0; size_t smem = 0;
     if (k1f_plan(nrows, s->ldx, s->L, s->num_sms, &S, &rows, &LP, &smem)) {
-      int *perm, *depth; long long* goff; unsigned short* row16; float* val; long long total;
-      CK(k1f_build(nrows, s->Dg, nnz, d.rowptr, d.colidx, d.vals, S, rows, &d.sg_ngrp, &perm, &depth, &goff, &row16, &val, &total, s->stream));
+      int *perm, *depth; long long* goff; unsigned short *row16, *col16; float* val; long long total;
+      CK(k1f_build(nrows, s->Dg, nnz, d.rowptr, d.colidx, d.vals, S, rows, &d.sg_ngrp, &perm, &depth, &goff, &row16, &val, &total, &col16,
+                   s->stream));
       d.sg_S = S; d.sg_rows = rows;
-      d.sg_perm = perm; d.sg_depth = depth; d.sg_goff = goff; d.sg_row16 = row16; d.sg_val = val;
-      for (void* p : {(void*)perm, (void*)depth, (void*)goff, (void*)row16, (void*)val}) s->mem.adopt(p);
+      d.sg_perm = perm; d.sg_depth = depth; d.sg_goff = goff; d.sg_row16 = row16; d.sg_val = val; d.sg_col16 = col16;
+      for (void* p : {(void*)perm, (void*)depth, (void*)goff, (void*)row16, (void*)val, (void*)col16}) s->mem.adopt(p);
     }
   }
   return 0;

@@ -14,8 +14,8 @@
 //            group: coalesced loads, r gathered from shared memory, g_c += v r in registers -- a segmented sum with no
 //            atomics and a fixed order (row order): deterministic like the dense kernel.
 // Per-segment partial gradients go to gpart_f[segment][column] (fp32, one writer per element); k1_partial_reduce_kernel adds
-// the segments in fp64 in segment order.  HBM traffic per partition pass: 8 B (CSR) + ~6.2 B (segment list) per stored value
-// + 9 B per row, for ALL lambdas together.
+// the segments in fp64 in segment order.  HBM traffic per partition pass: 6 B (the CSR values + a 16-bit copy of the column ids,
+// sg_col16) + ~6.2 B (segment list) per stored value + 9 B per row, for ALL lambdas together.
 // MODE K1_HV / K1_DIAG (matrix-free solver, common.cuh): phase A computes t_il = d_il (x_i . v_l) (v_l = hv_vf, interleaved like
 // beta) or t_il = d_il, with d_il = sqrt(d_il)^2 from sdvec of the last gradient pass; phase B is the same column sum of
 // x_ic t_il (x_ic^2 t_il for the diagonal).  The problems taking part are those with Ctrl::cg_active.
@@ -67,11 +67,26 @@ __global__ void __launch_bounds__(K1F_THREADS, 1) k1_csr_fused_kernel(const Prob
   V* r_s = beta_s + ldx;                                  // [sg_rows] interleaved residuals
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nw = K1F_THREADS >> 5;
   {
-    float* bs = reinterpret_cast<float*>(beta_s);
-    for (int e = tid; e < ldx * LP; e += K1F_THREADS) {
-      const int k = e / LP, l = e - k * LP;
-      if constexpr (MODE == K1_GRAD) bs[e] = (l < L && ((act >> l) & 1)) ? probs[b0 + l].beta_tf[k] : 0.f;
-      else bs[e] = (MODE == K1_HV && l < L && ((act >> l) & 1)) ? probs[b0 + l].hv_vf[k] : 0.f;
+    // 4 columns per thread: one 16-byte load per lambda, written as the LP-wide interleaved vectors of the 4 columns
+    const float* src[LP];
+#pragma unroll
+    for (int l = 0; l < LP; l++)
+      src[l] = (MODE != K1_DIAG && l < L && ((act >> l) & 1)) ? (MODE == K1_GRAD ? probs[b0 + l].beta_tf : probs[b0 + l].hv_vf) : nullptr;
+    float4* bs4 = reinterpret_cast<float4*>(k1f_sm);
+    for (int k4 = tid; k4 < (ldx >> 2); k4 += K1F_THREADS) {
+      float q[LP][4];
+#pragma unroll
+      for (int l = 0; l < LP; l++) {
+        const float4 t = src[l] ? __ldg(reinterpret_cast<const float4*>(src[l]) + k4) : make_float4(0.f, 0.f, 0.f, 0.f);
+        q[l][0] = t.x; q[l][1] = t.y; q[l][2] = t.z; q[l][3] = t.w;
+      }
+#pragma unroll
+      for (int m = 0; m < LP; m++) {   // float e = 4m..4m+3 of the 4 LP values: column e / LP, lambda e % LP
+        float o[4];
+#pragma unroll
+        for (int u = 0; u < 4; u++) o[u] = q[(4 * m + u) % LP][(4 * m + u) / LP];
+        bs4[(size_t)k4 * LP + m] = make_float4(o[0], o[1], o[2], o[3]);
+      }
     }
   }
   __syncthreads();
@@ -102,14 +117,14 @@ __global__ void __launch_bounds__(K1F_THREADS, 1) k1_csr_fused_kernel(const Prob
   for (long long ib = rb + 2 * warp; ib < re; ib += rstep) {
     const bool has_row = i < re;
     const float* __restrict__ vr = p0.vals + j0;
-    const int* __restrict__ cr = p0.colidx + j0;
+    const unsigned short* __restrict__ cr = p0.sg_col16 + j0;
     float v[K1F_NCH];
     int c[K1F_NCH];
 #pragma unroll
     for (int q = 0; q < K1F_NCH; q++) {
       const bool ok = sl + K1F_HW * q < len;
       v[q] = ok ? __ldg(vr + sl + K1F_HW * q) : 0.f;
-      c[q] = ok ? __ldg(cr + sl + K1F_HW * q) : 0;
+      c[q] = ok ? (int)__ldg(cr + sl + K1F_HW * q) : 0;   // unsigned: ids >= 32768 stay positive
     }
     float yy = 0.f, ww = 0.f, oo = 0.f;
     if (has_row) { yy = (float)__ldg(yv + i); ww = __ldg(wv + i); oo = __ldg(ov + i); }
@@ -128,7 +143,7 @@ __global__ void __launch_bounds__(K1F_THREADS, 1) k1_csr_fused_kernel(const Prob
     }
     for (int j = K1F_NCH * K1F_HW + sl; j < len; j += K1F_HW) {
       const float vj = __ldg(vr + j);
-      const V bb = beta_s[__ldg(cr + j)];
+      const V bb = beta_s[(int)__ldg(cr + j)];
 #pragma unroll
       for (int l = 0; l < LP; l++) a[l] = fmaf(vj, vget(bb, l), a[l]);
     }
@@ -311,6 +326,11 @@ __global__ void k1f_rowid_kernel(long long n, int sg_rows, int Dg, int ngrp, con
     }
   }
 }
+// 16-bit copy of the column ids for phase A (k1f_plan admits no partition wider than 55 296 columns)
+__global__ void k1f_col16_kernel(long long nnz, const int* __restrict__ colidx, unsigned short* __restrict__ col16) {
+  for (long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x; j < nnz; j += (long long)gridDim.x * blockDim.x)
+    col16[j] = (unsigned short)colidx[j];
+}
 // pass 2a: column histogram of every chunk of a segment's stored values (K1F_CHUNKS chunks per segment, consecutive in the CSR)
 constexpr int K1F_CHUNKS = 8;
 __device__ __forceinline__ void k1f_chunk_range(long long j0, long long j1, int chunk, long long* a, long long* b) {
@@ -410,12 +430,13 @@ static cudaError_t k1f_tmp_alloc(T** p, cudaStream_t st, size_t bytes) { return 
 // Builds the segment list of one partition.  All outputs are cudaMalloc'ed here and owned by the caller.
 cudaError_t k1f_build(long long n, int Dg, long long nnz, const long long* rowptr, const int* colidx, const float* vals, int S, int sg_rows, int* ngrp_out,
                       int** perm_out, int** depth_out, long long** goff_out, unsigned short** row16_out, float** val_out, long long* total_out,
-                      cudaStream_t st) {
+                      unsigned short** col16_out, cudaStream_t st) {
   const int ngrp = (Dg + 31) / 32;
   cudaError_t e;
   int *cnt = nullptr, *cnt_s = nullptr, *ids = nullptr, *ids_s = nullptr, *offs = nullptr, *inv = nullptr, *perm = nullptr, *depth = nullptr;
   long long *goff = nullptr, *d64 = nullptr;
   unsigned short* row16 = nullptr;
+  unsigned short* col16 = nullptr;
   unsigned short* ent_row = nullptr;
   unsigned* ent_base = nullptr;
   unsigned short* hist = nullptr;
@@ -426,7 +447,7 @@ cudaError_t k1f_build(long long n, int Dg, long long nnz, const long long* rowpt
     // temporaries come from the stream-ordered allocator: cudaFree would wait for the whole device, including the next partition's H2D copy
     void* tmps[] = {cnt, cnt_s, ids, ids_s, offs, inv, d64, tmp, ent_row, ent_base, hist};
     for (void* t : tmps) if (t) cudaFreeAsync(t, st);
-    if (all) { cudaFree(perm); cudaFree(depth); cudaFree(goff); cudaFree(row16); cudaFree(sval); }
+    if (all) { cudaFree(perm); cudaFree(depth); cudaFree(goff); cudaFree(row16); cudaFree(sval); cudaFree(col16); }
   };
 #define K1F_CK(x) do { e = (x); if (e != cudaSuccess) { cleanup(true); return e; } } while (0)
   K1F_CK(k1f_tmp_alloc(&cnt, st, sd * 4)); K1F_CK(k1f_tmp_alloc(&cnt_s, st, sd * 4)); K1F_CK(k1f_tmp_alloc(&ids, st, sd * 4)); K1F_CK(k1f_tmp_alloc(&ids_s, st, sd * 4));
@@ -463,11 +484,13 @@ cudaError_t k1f_build(long long n, int Dg, long long nnz, const long long* rowpt
   k1f_hist_kernel<<<dim3(S, K1F_CHUNKS), 256, (size_t)Dg * 4, st>>>(n, sg_rows, Dg, rowptr, colidx, hist);
   K1F_CK(cudaFuncSetAttribute(k1f_fill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Dg * 2));
   k1f_fill_kernel<<<dim3(S, K1F_CHUNKS), 32, (size_t)Dg * 2, st>>>(n, sg_rows, Dg, rowptr, colidx, vals, ent_row, ent_base, hist, row16, sval);
+  K1F_CK(cudaMalloc(&col16, std::max<size_t>((size_t)nnz * 2, 16)));
+  k1f_col16_kernel<<<2048, 256, 0, st>>>(nnz, colidx, col16);
   K1F_CK(cudaGetLastError());
   K1F_CK(cudaStreamSynchronize(st));
 #undef K1F_CK
   cleanup(false);
-  *ngrp_out = ngrp; *perm_out = perm; *depth_out = depth; *goff_out = goff; *row16_out = row16; *val_out = sval; *total_out = total;
+  *ngrp_out = ngrp; *perm_out = perm; *depth_out = depth; *goff_out = goff; *row16_out = row16; *val_out = sval; *total_out = total; *col16_out = col16;
   return cudaSuccess;
 }
 

@@ -14,7 +14,7 @@ cudaError_t k1_launch(const Problem* d_probs, int nprob, bool csr, int ldx, int 
 bool k1f_plan(long long n, int ldx, int L, int num_sms, int* S_out, int* rows_out, int* LP_out, size_t* smem_out);
 cudaError_t k1f_build(long long n, int Dg, long long nnz, const long long* rowptr, const int* colidx, const float* vals, int S, int sg_rows, int* ngrp_out,
                       int** perm_out, int** depth_out, long long** goff_out, unsigned short** row16_out, float** val_out, long long* total_out,
-                      cudaStream_t st);
+                      unsigned short** col16_out, cudaStream_t st);
 cudaError_t k1f_launch(const Problem* d_probs, int ngroups, int L, int S, int LP, size_t smem, int has_bias, int force_emit, cudaStream_t st, int* launches,
                        int mode = K1_GRAD);
 // max over rows of sum_j |v_ij| (float bits, non-negative: order preserving) -> *out (k1_score_grad.cu)
