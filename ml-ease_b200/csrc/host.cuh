@@ -233,6 +233,7 @@ struct mlease_session {
   double mindiff = 99999999;
   double last_maxdiff = 0;
   bool begun = false;
+  bool hook_consumed = false;   // a test hook parked the ADMM batch (mlease_internal.h): no x-update before the next begin
   float boost_rate = 0.f;    // initialize.boost.rate of the current run (0: cold start from z = {})
   mlease::Counters cnt;
   mlease::Profiler prof;

@@ -332,6 +332,7 @@ static int admm_begin_impl(mlease_session* s, const double* z0, float boost_rate
   s->cnt.launches += launches;
   s->rho_fact.assign(s->L, -1.0);
   s->begun = true;
+  s->hook_consumed = false;
   return 0;
 }
 
@@ -347,6 +348,7 @@ int mlease_admm_begin_initialized(mlease_session* s, const double* z0, float boo
 int mlease_admm_local_step(mlease_session* s, double* exchange_dev) {
   if (!s || !exchange_dev) return fail(MLEASE_ERR_INVALID, "null argument");
   if (!s->begun) return fail(MLEASE_ERR_STATE, "mlease_admm_begin was not called");
+  if (s->hook_consumed) return fail(MLEASE_ERR_STATE, "a test hook consumed the x-update state: call mlease_admm_begin again");
   CK(cudaSetDevice(s->cfg.device));
   s->iter++;
   const int i = s->iter;

@@ -74,18 +74,16 @@ def make_case(L):
 def run_case(mb, L):
     """The gradient pass (with sqrt(d)), the Hv pass and the Hessian-diagonal pass of case L through the solver's launchers.
     -> dict(g, f, sd [P L, n], hv, diag, info (of the gradient pass), digest)."""
-    import ctypes as C
-    from mlease_b200._native import lib, check, ptr
-    from mlease_b200.admm import _internal_batch_grad
+    from mlease_b200._native import check, ptr
+    from mlease_b200 import _hooks
     P, D, lambdas = case_shape(L)
     arrs, parts, W, V, digest = make_case(L)
-    fn = lib().mlease_internal_batch_hv
-    fn.argtypes, fn.restype = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p], C.c_int
+    fn = _hooks.bound().mlease_internal_batch_hv
     with mb.AdmmSession(P, D, lambdas, hessian_policy=2) as s:
         for p, a in enumerate(arrs):
             s.add_partition_csr(p, a["rowptr"], a["colidx"], a["vals"], a["response"], a["weight"], a["offset"])
         s.begin()
-        info = _internal_batch_grad(s, W, rows=[N_ROWS] * P, want_sd=True)
+        info = _hooks.batch_grad(s, W, rows=[N_ROWS] * P, want_sd=True)
         out = dict(g=info["g"], f=info["f"], sd=np.stack(info["sd"]), info=info, digest=digest)
         for mode, name in ((1, "hv"), (2, "diag")):
             o = np.zeros_like(W)

@@ -204,7 +204,7 @@ class Plan:
 
 
 def plan_from_info(info, b, n):
-    """The Plan of problem b from mlease_b200.admm._internal_batch_grad's result."""
+    """The Plan of problem b from mlease_b200._hooks.batch_grad's result."""
     k = info["kind"]
     if k == "dense":
         return Plan("dense", RT=info["RT"], chunks=int(info["chunks"][b]))

@@ -51,9 +51,9 @@ class _Sess:
         self.nprob, self.Dt, self.ldh = P * L, D + 1, ldh_of(D + 1)
 
     def factor(self, mode, **kw):
-        from mlease_b200.admm import _internal_batch_factor
+        from mlease_b200 import _hooks
         self.s.begin()
-        return _internal_batch_factor(self.s, mode, **kw)
+        return _hooks.batch_factor(self.s, mode, **kw)
 
     def close(self):
         self.s.__exit__(None, None, None)
@@ -299,9 +299,9 @@ def test_real_hessians_within_fp64_bounds(mb, D, dense):
         w = r.normal(0, 0.5, Dt)
         _, _, Hr = s.objective(0, w, np.zeros(Dt), np.full(Dt, 0.3), want_grad=False, want_hessian=True, tensor=True)
         Hr = (np.tril(Hr) + np.tril(Hr, -1).T)
-        from mlease_b200.admm import _internal_batch_factor
+        from mlease_b200 import _hooks
         s.begin()
-        out = _internal_batch_factor(s, np.array([1, 1], np.int32), H=np.stack([Hr, Hr]))
+        out = _hooks.batch_factor(s, np.array([1, 1], np.int32), H=np.stack([Hr, Hr]))
     assert (out["fail"] == 0).all()
     for k in _KEYS:
         assert np.array_equal(out[k][0].view(np.uint64), out[k][1].view(np.uint64)), k
@@ -314,7 +314,7 @@ def test_real_hessians_within_fp64_bounds(mb, D, dense):
 
 def test_hook_refusals(mb):
     """Every bad argument is refused before any launch, each with its own text, and the session still works after."""
-    from mlease_b200.admm import _internal_batch_factor, _internal_direction
+    from mlease_b200 import _hooks
     D, Dt = 40, 41
     H = np.stack([np.eye(Dt)] * 4)
     with mb.AdmmSession(2, D, [1.0, 2.0]) as s:
@@ -322,7 +322,7 @@ def test_hook_refusals(mb):
             s.add_partition_csr(p, *_part(D, 64, 6, p))
         one = np.ones(4, np.int32)
         with pytest.raises(mb.MleaseError, match="mlease_admm_begin was not called"):
-            _internal_batch_factor(s, one, H=H)
+            _hooks.batch_factor(s, one, H=H)
         s.begin()
         cases = [
             (dict(mode=np.array([1, 3, 1, 1], np.int32), H=H), "mode must be 0, 1 or 2"),
@@ -341,18 +341,18 @@ def test_hook_refusals(mb):
         for kw, text in cases:
             mode = kw.pop("mode")
             with pytest.raises(mb.MleaseError, match=text.replace("(", r"\(")):
-                _internal_batch_factor(s, mode, **kw)
+                _hooks.batch_factor(s, mode, **kw)
         with pytest.raises(mb.MleaseError, match="launch order leaves the batch"):   # refused before q or Ctrl are touched
-            _internal_batch_factor(s, np.array([1, 2, 1, 2], np.int32), H=H, G=H.astype(np.float32), q=np.ones((4, Dt)), order=[9])
+            _hooks.batch_factor(s, np.array([1, 2, 1, 2], np.int32), H=H, G=H.astype(np.float32), q=np.ones((4, Dt)), order=[9])
         with pytest.raises(mb.MleaseError, match=r"bfgs_count must be >= 0"):
             args = _dir_args(4, Dt)
             args[5][2] = -1
-            _internal_direction(s, *args)
+            _hooks.direction(s, *args)
         # an empty launch order on a batch mixing modes 1 and 2: nothing runs, nothing is written
-        out = _internal_batch_factor(s, np.array([1, 2, 1, 2], np.int32), H=H, G=H.astype(np.float32), q=np.ones((4, Dt)),
+        out = _hooks.batch_factor(s, np.array([1, 2, 1, 2], np.int32), H=H, G=H.astype(np.float32), q=np.ones((4, Dt)),
                                      order=np.zeros(0, np.int32))
         assert all(cr.is_sentinel(out["Hinv"][b]) for b in range(4)) and (out["tot_hess"] == 0).all()
-        out = _internal_batch_factor(s, one, H=H)
+        out = _hooks.batch_factor(s, one, H=H)
         assert (out["hess_valid"] == 1).all() and np.array_equal(out["Hinv"][:, :Dt, :Dt], H)
         s.begin()
         s.run(2)   # the solver still runs on the batch the hook used
@@ -360,16 +360,16 @@ def test_hook_refusals(mb):
         s.add_partition_csr(0, *_part(D, 64, 6, 0))
         s.begin()
         with pytest.raises(mb.MleaseError, match="a matrix-free session forms no factor"):
-            _internal_batch_factor(s, np.ones(1, np.int32), H=H[:1])
+            _hooks.batch_factor(s, np.ones(1, np.int32), H=H[:1])
         with pytest.raises(mb.MleaseError, match="a matrix-free session forms no factor"):
-            _internal_direction(s, *_dir_args(1, Dt))
+            _hooks.direction(s, *_dir_args(1, Dt))
     with mb.AdmmSession(1, 3000, [1.0]) as s:   # ldh 3008: the factored direction, no explicit inverse
         s.add_partition_csr(0, *_part(3000, 64, 6, 0))
         s.begin()
         with pytest.raises(mb.MleaseError, match="only systems up to 2048"):
-            _internal_batch_factor(s, np.ones(1, np.int32), H=np.eye(3001)[None])
+            _hooks.batch_factor(s, np.ones(1, np.int32), H=np.eye(3001)[None])
         with pytest.raises(mb.MleaseError, match="only systems up to 2048"):
-            _internal_direction(s, *_dir_args(1, 3001))
+            _hooks.direction(s, *_dir_args(1, 3001))
 
 
 def _dir_args(nprob, Dt):
@@ -386,7 +386,7 @@ def test_direction_on_the_explicit_inverse(mb, D, L):
     bfgs_count in {0, 1, 6, 7, 13} (13: the ring has wrapped twice) and h0_scale in {1, 2.5}, every combination on every problem
     position of an L-lambda batch.  dir, phi0 = dir . g and dirnorm = max |dir| within the running-error bounds; beta_t is
     float(beta + dir) bit for bit."""
-    from mlease_b200.admm import _internal_batch_factor, _internal_direction
+    from mlease_b200 import _hooks
     Dt, M = D + 1, cr.BFGS_M
     combos = [(c, h) for c in (0, 1, 6, 7, 13) for h in (1.0, 2.5)]
     Hs = np.stack([_spd(Dt, 50 + b) for b in range(L)])
@@ -394,7 +394,7 @@ def test_direction_on_the_explicit_inverse(mb, D, L):
     with mb.AdmmSession(1, D, [1.0 + l for l in range(L)]) as s:
         s.add_partition_csr(0, *_part(D, 64, 6, D))
         s.begin()
-        Hinv = _internal_batch_factor(s, np.ones(L, np.int32), H=Hs)["Hinv"]
+        Hinv = _hooks.batch_factor(s, np.ones(L, np.int32), H=Hs)["Hinv"]
         worst = np.zeros(3)
         for i in range(len(combos)):
             cnt = np.array([combos[(i + b) % len(combos)][0] for b in range(L)], np.int32)
@@ -404,7 +404,7 @@ def test_direction_on_the_explicit_inverse(mb, D, L):
             Y = np.einsum("bjk,bkl->bjl", S, Hs) + 1e-3 * r.normal(size=(L, M, Dt))
             rho = 1.0 / np.einsum("bjk,bjk->bj", S, Y)
             beta = r.normal(0, 0.5, (L, Dt))
-            out = _internal_direction(s, np.ones(L, np.int32), g, S, Y, rho, cnt, h0, beta)
+            out = _hooks.direction(s, np.ones(L, np.int32), g, S, Y, rho, cnt, h0, beta)
             for b in range(L):
                 ref, bound = cr.two_loop(Hinv[b], g[b], S[b], Y[b], rho[b], cnt[b], h0[b])
                 e = cr.direction_excess(out["dir"][b], out["phi0"][b], out["dirnorm"][b], g[b], ref, bound)

@@ -2,7 +2,6 @@
 and mid-tile, run-to-run bit equality of the factor and the inverse (the look-ahead overlaps the panel chain with the trailing
 update on a second stream), and bit equality of the two DMMA shapes the trailing update may issue (m16n8k4 is two m8n8k4
 stacked in M).  The hooks are test entry points of the library, not part of its C ABI."""
-import ctypes as C
 import os
 import sys
 
@@ -23,14 +22,8 @@ def mb():
 
 @pytest.fixture(scope="module")
 def hooks(mb):
-    from mlease_b200._native import lib
-    L = lib()
-    vp = C.c_void_p
-    L.mlease_internal_factor.argtypes = [vp, C.c_int32, vp, vp, vp, vp]
-    L.mlease_internal_factor.restype = C.c_int
-    L.mlease_internal_dmma_shapes.argtypes = [vp, vp, C.c_int32, C.c_int32, vp, vp]
-    L.mlease_internal_dmma_shapes.restype = C.c_int
-    return L
+    from mlease_b200 import _hooks
+    return _hooks.bound()
 
 
 def _check(rc):

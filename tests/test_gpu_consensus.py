@@ -71,8 +71,8 @@ class _Sess:
     "fused" (sorted unique CSR rows, fused multi-lambda K1 when L <= 4) or "mf" (matrix-free, hessian_policy 2)."""
 
     def __init__(self, mb, kind, D, P, L, parts=None, n=400, reg=2, lmap=None, pen=False, coef=0.0, epsilon=1e-4, seed=0):
-        from mlease_b200.admm import _internal_consensus
-        self.hook = _internal_consensus
+        from mlease_b200 import _hooks
+        self.hook = _hooks.consensus
         r = np.random.default_rng(seed + D + 7 * P + 31 * L)
         self.kind, self.D, self.P, self.L, self.reg, self.pen, self.coef, self.eps = kind, D, P, L, reg, pen, coef, epsilon
         self.parts = list(range(P)) if parts is None else sorted(parts)
@@ -340,27 +340,27 @@ def _check_estimate(S, pre, post, tag):
 
 def test_refusals(mb):
     from mlease_b200._native import MleaseError, lib
-    from mlease_b200.admm import _internal_consensus
+    from mlease_b200 import _hooks
     r = np.random.default_rng(9)
     arr, _ = _rows(r, "fused", 200, 20)
     with mb.AdmmSession(2, 20, [1.0], regularizer=1) as s:
         s.add_partition_csr(0, arr["rowptr"], arr["colidx"], arr["vals"], arr["response"])
         with pytest.raises(MleaseError, match="begin"):
-            _internal_consensus(s, read=False)
+            _hooks.consensus(s, read=False)
         s.begin()
-        S = _internal_consensus(s)   # a read without stages
+        S = _hooks.consensus(s)   # a read without stages
         st = {k: S[k] for k in ("vec", "fvec", "z", "exch", "diff", "ctrl")}
         for mask in (16, -1):
             with pytest.raises(MleaseError, match="stage mask"):
-                _internal_consensus(s, mask, st)
+                _hooks.consensus(s, mask, st)
         with pytest.raises(MleaseError, match="L2"):
-            _internal_consensus(s, ["init"], st)
+            _hooks.consensus(s, ["init"], st)
         with pytest.raises(MleaseError, match="iter >= 1"):
-            _internal_consensus(s, ["consensus"], st, iter=0)
+            _hooks.consensus(s, ["consensus"], st, iter=0)
         bad = dict(st, ctrl=np.tile([0, 0, S["info"]["k1_grid"] + 1], (S["info"]["nprob"], 1)))
         with pytest.raises(MleaseError, match="k1_chunks"):
-            _internal_consensus(s, ["pack"], bad)
+            _hooks.consensus(s, ["pack"], bad)
         info = np.zeros(12, np.int32)
-        fn = lib().mlease_internal_consensus
+        fn = _hooks.bound().mlease_internal_consensus
         rc = fn(s._h, 4, None, None, None, None, None, None, None, None, None, None, None, None, info.ctypes.data)
         assert rc != 0 and b"null" in lib().mlease_last_error()

@@ -26,16 +26,8 @@ def mb():
 
 @pytest.fixture(scope="module")
 def hooks(mb):
-    from mlease_b200._native import lib
-    L = lib()
-    vp = C.c_void_p
-    L.mlease_internal_factor.argtypes = [vp, C.c_int32, vp, vp, vp, vp]
-    L.mlease_internal_factored_direction.argtypes = [vp, vp, vp, vp, vp]
-    L.mlease_internal_ysym.argtypes = [vp, C.c_int32, vp, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
-    L.mlease_internal_request_refresh.argtypes = [vp, C.c_int32]
-    for f in (L.mlease_internal_factor, L.mlease_internal_factored_direction, L.mlease_internal_ysym, L.mlease_internal_request_refresh):
-        f.restype = C.c_int
-    return L
+    from mlease_b200 import _hooks
+    return _hooks.bound()
 
 
 def _check(rc):

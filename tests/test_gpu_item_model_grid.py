@@ -26,9 +26,9 @@ def _ndev():
 
 @pytest.fixture
 def budget():
-    from mlease_b200 import admm
-    yield admm._internal_set_keyed_budget
-    admm._internal_set_keyed_budget(0)
+    from mlease_b200 import _hooks
+    yield _hooks.set_keyed_budget
+    _hooks.set_keyed_budget(0)
 
 
 def _problem(rng, K, D, G, max_rows=40, density=0.05):
@@ -119,21 +119,21 @@ def test_score_keyed_var_pred_is_score_keyed_and_var_is_fp64(G):
 def test_streamed_score_keyed_var_is_bitwise_resident(budget, G):
     import torch
 
-    from mlease_b200 import admm
+    from mlease_b200 import _hooks
     pb = _problem(np.random.default_rng(80 + G), K=40, D=120, G=G, max_rows=300, density=0.1)
     budget(0)
     want_p, want_v = _call(pb)
-    assert not admm._internal_keyed_last_call()[1]
+    assert not _hooks.keyed_last_call()[1]
     budget(256 << 10)
     got_p, got_v = _call(pb)
-    bounds, streamed, _, _ = admm._internal_keyed_last_call()
+    bounds, streamed, _, _ = _hooks.keyed_last_call()
     assert streamed and len(bounds) - 1 >= 4, bounds
     assert np.array_equal(got_p.view(np.uint32), want_p.view(np.uint32)) and np.array_equal(got_v.view(np.uint32), want_v.view(np.uint32))
     n = int(pb["krs"][-1])
     dp = torch.zeros((G, n), dtype=torch.float32, device="cuda")
     dv = torch.zeros((G, n), dtype=torch.float32, device="cuda")
     _call(pb, out=dp, out_var=dv)
-    assert admm._internal_keyed_last_call()[1]
+    assert _hooks.keyed_last_call()[1]
     assert np.array_equal(dp.cpu().numpy().view(np.uint32), want_p.view(np.uint32))
     assert np.array_equal(dv.cpu().numpy().view(np.uint32), want_v.view(np.uint32))
 

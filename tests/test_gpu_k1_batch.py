@@ -27,8 +27,8 @@ def report():
 
 
 def _grad(s, W, active=None, rows=None, sd=False, xt=False):
-    from mlease_b200.admm import _internal_batch_grad
-    return _internal_batch_grad(s, W, active=active, rows=rows, want_sd=sd, want_xt=xt)
+    from mlease_b200 import _hooks
+    return _hooks.batch_grad(s, W, active=active, rows=rows, want_sd=sd, want_xt=xt)
 
 
 def _session(mb, D, L, cases, policy=0, binary=False):

@@ -27,9 +27,9 @@ def _ndev():
 
 @pytest.fixture
 def budget():
-    from mlease_b200 import admm
-    yield admm._internal_set_keyed_budget
-    admm._internal_set_keyed_budget(0)
+    from mlease_b200 import _hooks
+    yield _hooks.set_keyed_budget
+    _hooks.set_keyed_budget(0)
 
 
 def _keyed(rng, rows, D, nnz, absent=8):
@@ -66,17 +66,17 @@ def _naive(pb, budget_bytes, budget, lams=(0.5, 3.0), thr=40):
 
 
 def test_streamed_naive_train_csr_matches_resident_per_chunk(budget):
-    from mlease_b200 import admm
+    from mlease_b200 import _hooks
     rng = np.random.default_rng(71)
     rows = rng.integers(400, 1200, 36); rows[[3, 17, 30]] = [5, 0, 20]          # skipped by data.size.threshold = 40, and a key with no rows
     pb = _keyed(rng, rows, 48, 30)
     models, skipped = _naive(pb, 5 << 20, budget)
-    bounds, streamed, _, _ = admm._internal_keyed_last_call()
+    bounds, streamed, _, _ = _hooks.keyed_last_call()
     assert streamed and len(bounds) - 1 >= 6 and bounds[0] == 0 and bounds[-1] == pb["K"], bounds
     assert list(np.nonzero(skipped)[0]) == [3, 17, 30] and np.all(models[:, [3, 17, 30]] == 0)
     for k0, k1 in zip(bounds[:-1], bounds[1:]):
         m1, s1 = _naive(_slice(pb, k0, k1), 0, budget)
-        assert not admm._internal_keyed_last_call()[1]
+        assert not _hooks.keyed_last_call()[1]
         _close(models[:, k0:k1], m1)
         assert np.array_equal(skipped[k0:k1], s1)
     full, _ = _naive(pb, 0, budget)
@@ -88,11 +88,11 @@ def test_streamed_naive_train_csr_matches_resident_per_chunk(budget):
 
 def test_streamed_naive_train_one_row_keys_are_bitwise(budget):
     """keys of one row: every gradient sum is one addition, so a streamed chunk is bitwise its resident call"""
-    from mlease_b200 import admm
+    from mlease_b200 import _hooks
     rng = np.random.default_rng(72)
     pb = _keyed(rng, np.ones(300, np.int64), 30, 6)
     models, _ = _naive(pb, 120 << 10, budget, thr=0)
-    bounds, streamed, _, _ = admm._internal_keyed_last_call()
+    bounds, streamed, _, _ = _hooks.keyed_last_call()
     assert streamed and len(bounds) - 1 >= 6, bounds
     for k0, k1 in list(zip(bounds[:-1], bounds[1:]))[::10]:
         m1, _ = _naive(_slice(pb, k0, k1), 0, budget, thr=0)
@@ -101,7 +101,7 @@ def test_streamed_naive_train_one_row_keys_are_bitwise(budget):
 
 def test_streamed_naive_train_dense(budget):
     import mlease_b200 as mb
-    from mlease_b200 import admm
+    from mlease_b200 import _hooks
     rng = np.random.default_rng(73)
     K, D = 24, 40
     rows = rng.integers(300, 900, K)
@@ -110,7 +110,7 @@ def test_streamed_naive_train_dense(budget):
     y = (rng.random(krs[-1]) < 1 / (1 + np.exp(-X[:, :5].sum(1)))).astype(np.int32)
     budget(3 << 20)
     got, _ = mb.naive_train(X, krs, y, [1.0, 4.0])
-    bounds, streamed, _, _ = admm._internal_keyed_last_call()
+    bounds, streamed, _, _ = _hooks.keyed_last_call()
     assert streamed and len(bounds) - 1 >= 4, bounds
     budget(0)
     for k0, k1 in zip(bounds[:-1], bounds[1:]):
@@ -121,7 +121,7 @@ def test_streamed_naive_train_dense(budget):
 
 def test_streamed_item_model_train_matches_resident_per_chunk(budget):
     import mlease_b200 as mb
-    from mlease_b200 import admm
+    from mlease_b200 import _hooks
     rng = np.random.default_rng(74)
     rows = rng.integers(300, 900, 30); rows[11] = 0
     pb = _keyed(rng, rows, 40, 8)
@@ -134,7 +134,7 @@ def test_streamed_item_model_train_matches_resident_per_chunk(budget):
         return mb.item_model_train(p["v"], p["krs"], p["y"], il, dl, rowptr=p["rp"], colidx=p["ci"], num_features=p["D"], intercept_prior_mean=m,
                                    weight=p["w"], offset=p["o"], lambda_map=lm, compute_var=True)
     models, var = fit(pb, means, 3 << 19)
-    bounds, streamed, _, _ = admm._internal_keyed_last_call()
+    bounds, streamed, _, _ = _hooks.keyed_last_call()
     assert streamed and len(bounds) - 1 >= 6, bounds
     for k0, k1 in zip(bounds[:-1], bounds[1:]):
         m1, v1 = fit(_slice(pb, k0, k1), means[k0:k1], 0)
@@ -177,16 +177,16 @@ def test_streamed_naive_train_from_device_and_pinned_input(budget, where):
     """device or pinned rows are copied into the ring directly (no pinned staging copy); same fits as pageable input"""
     import torch
 
-    from mlease_b200 import admm
+    from mlease_b200 import _hooks
     rng = np.random.default_rng(78)
     rows = rng.integers(400, 1200, 24); rows[5] = 10
     pb = _keyed(rng, rows, 48, 30)
     want, ws = _naive(pb, 2 << 20, budget)
-    assert admm._internal_keyed_last_call()[1]
+    assert _hooks.keyed_last_call()[1]
     conv = (lambda a: torch.from_numpy(a).cuda()) if where == "device" else (lambda a: torch.from_numpy(a).pin_memory())
     pt = dict(pb, rp=conv(pb["rp"]), ci=conv(pb["ci"]), v=conv(pb["v"]), y=conv(pb["y"]), w=conv(pb["w"]), o=conv(pb["o"]))
     got, gs = _naive(pt, 2 << 20, budget)   # below the device input's resident upload (rows, labels) + first state
-    bounds, streamed, _, _ = admm._internal_keyed_last_call()
+    bounds, streamed, _, _ = _hooks.keyed_last_call()
     assert streamed and len(bounds) - 1 >= 6, bounds
     assert np.array_equal(gs, ws)
     _close(got, want)
@@ -216,21 +216,21 @@ def test_streamed_score_keyed_is_bitwise_resident(budget, L, binary):
     import torch
 
     import mlease_b200 as mb
-    from mlease_b200 import admm
+    from mlease_b200 import _hooks
     rng = np.random.default_rng(76 + L)
     K, D = 40, 120
     krs, rp, ci, v, o, mp, mc, mv = _scoring_data(rng, K, D, L)
     budget(0)
     want = mb.score_keyed(v, krs, rp, ci, D, mp, mc, mv, offset=o, binary_feature=binary)
-    assert not admm._internal_keyed_last_call()[1]
+    assert not _hooks.keyed_last_call()[1]
     budget(256 << 10)
     got = mb.score_keyed(v, krs, rp, ci, D, mp, mc, mv, offset=o, binary_feature=binary)
-    bounds, streamed, _, _ = admm._internal_keyed_last_call()
+    bounds, streamed, _, _ = _hooks.keyed_last_call()
     assert streamed and len(bounds) - 1 >= 4, bounds
     assert np.array_equal(got.view(np.uint32), want.view(np.uint32))
     dev = torch.zeros((L, int(krs[-1])), dtype=torch.float32, device="cuda")
     mb.score_keyed(v, krs, rp, ci, D, mp, mc, mv, offset=o, binary_feature=binary, out=dev)
-    assert admm._internal_keyed_last_call()[1]
+    assert _hooks.keyed_last_call()[1]
     assert np.array_equal(dev.cpu().numpy().view(np.uint32), want.view(np.uint32))
 
 

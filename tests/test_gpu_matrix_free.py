@@ -85,24 +85,21 @@ def test_batch_hv_and_diagonal_match_oracle(mb, P, n, D, nnz, L, no_fused):
     """Every (partition, lambda) problem at its own point w and vector v: a wrong lambda's v or d, or a wrong diagonal, fails here (the
     ADMM parity cases could not see it: any SPD model leads the line search to the same minimiser).  Each column is also held to the
     bound of tests/k1_reference.py, with the pass's chunking as the gradient hook reports it for the same batch."""
-    import ctypes as C
     import k1_reference as kr
-    from mlease_b200._native import lib, ptr, check
-    from mlease_b200.admm import _internal_batch_grad
+    from mlease_b200._native import ptr, check
+    from mlease_b200 import _hooks
     parts, _, _ = _sparse_parts(P, n, D, nnz, seed=D + L)
     rng = np.random.default_rng(L)
     nprob = P * L
     w = rng.normal(0, 0.3, (nprob, D + 1)); v = rng.normal(size=(nprob, D + 1))
     big = np.full(D + 1, 1e30)   # prior variance: the oracle's prior term vanishes, the hook returns the data term
-    fn = lib().mlease_internal_batch_hv
-    fn.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-    fn.restype = C.c_int
+    fn = _hooks.bound().mlease_internal_batch_hv
     with mb.AdmmSession(P, D, [0.5 * (l + 1) for l in range(L)], hessian_policy=2) as s:
         for p, part in enumerate(parts):
             s.add_partition_csr(p, *part)
         s.begin()
         assert s.stats()["k1_fused"] == (0 if no_fused or L > 4 else 1)
-        info = _internal_batch_grad(s, w)   # all problems, as in the Hv / diagonal passes: the same CTA mapping
+        info = _hooks.batch_grad(s, w)   # all problems, as in the Hv / diagonal passes: the same CTA mapping
         assert info["kind"] == ("fused" if s.stats()["k1_fused"] else "fx_window" if D > 28000 else "fx")
         for mode, name in ((1, "Hv"), (2, "hessian_diag")):
             outs = []

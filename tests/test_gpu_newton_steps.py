@@ -51,9 +51,9 @@ class _Sess:
     """A begun ADMM session of P partitions x L lambdas: kind "dense", "csr" (Gram path) or "mf" (matrix-free, policy 2)."""
 
     def __init__(self, mb, kind, D, P=1, L=1, policy=0):
-        from mlease_b200.admm import _internal_newton_stage
+        from mlease_b200 import _hooks
         import k1_reference as k1
-        self.hook = _internal_newton_stage
+        self.hook = _hooks.newton_stage
         r = np.random.default_rng(D + 7 * P + L)
         self.s = mb.AdmmSession(P, D, [1.0 + l for l in range(L)], hessian_policy=2 if kind == "mf" else policy, epsilon=0.0)
         self.s.__enter__()
@@ -81,7 +81,7 @@ class _Sess:
 
     def pack(self, states):
         """The hook's arrays for one state per problem (None: a done problem, every byte the sentinel)."""
-        from mlease_b200.admm import STAGE_CTRL
+        from mlease_b200._hooks import STAGE_CTRL
         n, Dt, ldx = self.nprob, self.Dt, self.ldx
         ctrl = np.zeros(n, STAGE_CTRL)
         vec = np.zeros((n, 12, ldx))
@@ -101,7 +101,7 @@ class _Sess:
                 ctrl[b][k] = st[k]
             for k in nr.REAL_FIELDS:
                 ctrl[b][k] = st[k]
-            from mlease_b200.admm import STAGE_VECS
+            from mlease_b200._hooks import STAGE_VECS
             for i, k in enumerate(STAGE_VECS):
                 if k in st:
                     vec[b, i, :len(st[k])] = st[k]   # (a state may carry whole ldx-long vectors: its padding then)
@@ -130,7 +130,7 @@ class _Sess:
 
     def compare(self, states, refs, inp, out, ints=nr.INT_FIELDS, reals=nr.REAL_FIELDS, tag=""):
         """Every output of every problem against the replica's state by bits; a done problem keeps its bytes."""
-        from mlease_b200.admm import STAGE_VECS
+        from mlease_b200._hooks import STAGE_VECS
         Dt, ldx = self.Dt, self.ldx
         for b, (st, ref) in enumerate(zip(states, refs)):
             where = "%s problem %d %s" % (tag, b, sorted(ref["branch"]) if ref else "done")
@@ -651,7 +651,7 @@ def test_cg_kernels_bit_for_bit(mb, D, P, L):
 
 def _state_of(tr, e, b, Dt, ldx, wide, mf):
     """The replica state of problem b at trace entry e."""
-    from mlease_b200.admm import STAGE_VECS
+    from mlease_b200._hooks import STAGE_VECS
     st = nr.new_state(Dt, wide=wide, matrix_free=mf)
     c = tr["ctrl"][e, b]
     for k in nr.INT_FIELDS + nr.TOTALS:
@@ -774,7 +774,7 @@ AUDIT = [("dense", 100, 2, 1), ("csr", 1000, 2, 3), ("csr", 2301, 1, 1), ("mf", 
 def test_slot_audit_of_real_xupdates(mb, kind, D, P, L, warm):
     """Cold and after `warm` ADMM iterations (fused batches then start from the estimated gradient: skip_eval), under the
     session's policy without and with speculative slots, and rebuilding at every step."""
-    from mlease_b200.admm import _internal_xupdate_trace
+    from mlease_b200 import _hooks
     seen = set()
     runs = [(2, ())] if kind == "mf" else [(0, ()), (0, tuple(range(1, 60))), (1, ())]
     for policy, spec in runs:
@@ -782,7 +782,7 @@ def test_slot_audit_of_real_xupdates(mb, kind, D, P, L, warm):
         try:
             for _ in range(warm):
                 t.s.iterate()
-            tr = _internal_xupdate_trace(t.s, policy=policy, invalidate=int(warm == 0), spec=spec)
+            tr = _hooks.xupdate_trace(t.s, policy=policy, invalidate=int(warm == 0), spec=spec)
             _audit(t, tr, seen)
             if spec:
                 assert tr["spec"].any() or tr["nslots"] < 3, "no slot ran speculatively"
@@ -812,12 +812,12 @@ def test_slot_audit_of_real_xupdates(mb, kind, D, P, L, warm):
 
 
 def test_trace_refusals(mb):
-    from mlease_b200.admm import _internal_xupdate_trace
+    from mlease_b200 import _hooks
     t = _Sess(mb, "csr", 36, 2, 2, policy=1)
     try:
         for kw in (dict(policy=1, spec=(1,)), dict(policy=0, spec=(0,)), dict(policy=2), dict(policy=3), dict(policy=0, max_slots=0)):
             with pytest.raises(mb.MleaseError) as e:
-                _internal_xupdate_trace(t.s, **kw)
+                _hooks.xupdate_trace(t.s, **kw)
             assert e.value.code == 1, kw
         t.s.begin()
         for _ in range(2):
@@ -946,7 +946,7 @@ def test_partial_reduction_bit_for_bit_on_order_sensitive_data(mb):
 def test_newton_solve_on_a_real_factor(mb):
     """newton_solve (the GEMV on the explicit inverse, then newton_solve_kernel) after a factorisation: the direction against the
     replica on the device's own Hinv; refused before any factorisation."""
-    from mlease_b200.admm import _internal_batch_factor
+    from mlease_b200 import _hooks
     t = _Sess(mb, "csr", 199, 2, 2)
     try:
         r = np.random.default_rng(77)
@@ -962,7 +962,7 @@ def test_newton_solve_on_a_real_factor(mb):
             A = r.normal(size=(Dt, 2 * Dt))
             H[b] = A @ A.T / (2 * Dt) + np.eye(Dt)
         t.s.begin()
-        fac = _internal_batch_factor(t.s, np.ones(t.nprob, np.int32), H=H)
+        fac = _hooks.batch_factor(t.s, np.ones(t.nprob, np.int32), H=H)
         inp, out = t.stage(states, ["decide", "solve"])
         for b, st in enumerate(states):
             d = nr.decide(st, [])
@@ -978,7 +978,7 @@ def test_newton_solve_on_a_real_factor(mb):
 
 
 def test_hook_refusals(mb):
-    from mlease_b200.admm import _internal_newton_stage
+    from mlease_b200 import _hooks
 
     def refused(t, states, stages, **kw):
         with pytest.raises(mb.MleaseError) as e:

@@ -39,13 +39,8 @@ def num_sms():
 
 
 def _hooks():
-    from mlease_b200._native import lib
-    L = lib()
-    L.mlease_internal_set_csr_gram.argtypes = [C.c_void_p, C.c_int32]
-    L.mlease_internal_set_csr_gram.restype = C.c_int
-    L.mlease_internal_csr_gram.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
-    L.mlease_internal_csr_gram.restype = C.c_int
-    return L
+    from mlease_b200._hooks import bound
+    return bound()
 
 
 def _set_kind(s, kind):

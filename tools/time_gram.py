@@ -17,20 +17,12 @@ import torch  # noqa: E402
 
 import bench  # noqa: E402
 import mlease_b200 as mb  # noqa: E402
-from mlease_b200._native import check, lib  # noqa: E402
+from mlease_b200 import _hooks  # noqa: E402
+from mlease_b200._native import check  # noqa: E402
 
 WGMMA, SPARSE = 1, 2
 dev = torch.device("cuda:0")
 REPS = int(os.environ.get("REPS", 3))
-
-
-def hooks():
-    L = lib()
-    L.mlease_internal_set_csr_gram.argtypes = [C.c_void_p, C.c_int32]
-    L.mlease_internal_set_csr_gram.restype = C.c_int
-    L.mlease_internal_csr_gram.argtypes = [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
-    L.mlease_internal_csr_gram.restype = C.c_int
-    return L
 
 
 def session(n, D, nnz):
@@ -45,7 +37,7 @@ def session(n, D, nnz):
 
 def time_gram(s, kind):
     """ms per build with the kernel `kind` (0: the automatic choice), and the kind that ran"""
-    L = hooks()
+    L = _hooks.bound()
     check(L.mlease_internal_set_csr_gram(s._h, kind))
     ms = s.time_kernel(0, "gram", reps=REPS)
     b, sc = C.c_int32(), C.c_int32()

@@ -6,7 +6,6 @@ passes of the matrix-free solver.  Kernel time = the summed CUDA time of the k1_
 Byte model of one pass (what the kernel moves for all lambdas together, per-row terms and the gpart_f partials left out):
 phase A reads the CSR rows, COLBYTES (2 for 16-bit column ids, 4 for int32) + 4 B per stored value; phase B the segment list,
 6 B per slot incl. its padding.  Scratch tool for kernel work on a GPU box, not part of the product."""
-import ctypes as C
 import os
 import sys
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "ml-ease_b200"))
@@ -15,8 +14,7 @@ import numpy as np
 import torch
 from torch.profiler import ProfilerActivity, profile
 import mlease_b200 as mb
-from mlease_b200._native import lib
-from mlease_b200.admm import _internal_batch_grad
+from mlease_b200 import _hooks
 import bench
 
 REPS = int(os.environ.get("REPS", 20))
@@ -45,8 +43,7 @@ def kernel_ms(fn, tag):
     return us / cnt / 1e3
 
 
-hv = lib().mlease_internal_batch_hv
-hv.argtypes, hv.restype = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p], C.c_int
+hv = _hooks.bound().mlease_internal_batch_hv
 for L in (3, 1):
     lambdas = [0.1, 1.0, 10.0][:L] if L == 3 else [1.0]
     for policy in (0, 2):
@@ -54,7 +51,7 @@ for L in (3, 1):
             s.add_partition_csr(0, rp, ci, vv, y)
             s.begin()
             W = np.tile(np.append(beta, -1.0).astype(np.float64), (L, 1))
-            info = _internal_batch_grad(s, W)
+            info = _hooks.batch_grad(s, W)
             assert info["kind"] == "fused", info["kind"]
             LP = info["G"]
             S, rows = info["chunks"][0], info["RT"]
@@ -62,7 +59,7 @@ for L in (3, 1):
             # (not known here; the byte model counts the stored values, i.e. it is a lower bound on what phase B reads)
             nbytes = (COLBYTES + 4.0) * n * nnz + 6.0 * n * nnz
             if policy == 0:
-                ms = kernel_ms(lambda: _internal_batch_grad(s, W), "k1_csr_fused_kernel<%d, 0>" % LP)
+                ms = kernel_ms(lambda: _hooks.batch_grad(s, W), "k1_csr_fused_kernel<%d, 0>" % LP)
                 print("gradient pass L=%d (LP=%d, %d segments x %d rows): %.3f ms, %.0f GB/s of the byte model" %
                       (L, LP, S, rows, ms, nbytes / ms / 1e6), flush=True)
             else:

@@ -63,7 +63,7 @@ def main():
     a = ap.parse_args()
     import torch
 
-    from mlease_b200 import admm
+    from mlease_b200 import _hooks
     ndev = torch.cuda.device_count()
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
     print(json.dumps({"card": card.splitlines(), "devices": ndev}), flush=True)
@@ -75,7 +75,7 @@ def main():
         if g > ndev:
             print(json.dumps({"run": name, "keys": K, "gpus": g, "measured": False, "reason": "only %d devices" % ndev}), flush=True)
             continue
-        admm._internal_set_keyed_budget(a.budget if name == "streamed" else 0)
+        _hooks.set_keyed_budget(a.budget if name == "streamed" else 0)
         if cached[0] != K:
             cached[:] = [K, None]          # the previous data set is released before the next one is made
             cached[1] = data(K, a.rows, a.features)
@@ -84,7 +84,7 @@ def main():
         t0 = time.perf_counter()
         fit(X, y, krs, list(range(g)))
         dt = time.perf_counter() - t0
-        bounds, streamed, stage_ms, wait_ms = admm._internal_keyed_last_call()
+        bounds, streamed, stage_ms, wait_ms = _hooks.keyed_last_call()
         rec = {"run": name, "keys": K, "rows": a.rows, "features": a.features, "gpus": g, "seconds": round(dt, 3), "fits_per_s": round(K / dt, 1),
                "streamed": streamed, "chunks": len(bounds) - 1}
         if streamed:
