@@ -235,6 +235,12 @@ int mlease_posterior_variance(mlease_session* s, int32_t partition_id, const dou
  *         (:360-398).  A feature that no row of a key lists is not in that key's dataset, hence not in its model
  *         (regression/liblinearfunc/LibLinear.java:343-350): its output coefficient is 0, whatever prior.mean is.
  *         binary_feature: every listed feature counts as 1 (LibLinearBinaryDataset).
+ *         Each key is solved in its own column space when that is narrower: with Dk the distinct columns its rows list, a key with
+ *         round_up(Dk + 1, 32) < round_up(num_features + 1, 32) is fitted over those Dk columns and the intercept only, and its
+ *         model is scattered back to the global columns.  Device memory then scales with each key's own width, not with
+ *         num_features (a 200 000-feature dictionary whose keys list a few hundred features each fits easily); the dense host
+ *         output, num_lambdas * num_keys * (num_features+1) doubles, is the limit that remains.  Which width a key runs at depends
+ *         on its own rows alone.
  *   dense (rowptr == NULL): vals = X row-major [nrows x num_features], leading dimension ldx; every feature is present.
  * priorVar = 1/lambda, 1/lambda_map[k] for listed features (lambda_map [num_features] or NULL, entries > 0), intercept variance
  * 100000 unless penalize_intercept (:333-343), prior.mean, has.intercept, data.size.threshold (skipped keys -> skipped[k]=1,
@@ -269,7 +275,9 @@ int mlease_naive_train_dense(int32_t device, void* stream, int32_t num_keys, int
  * intercept_prior_mean[k] for the intercept, 0 otherwise; start 0.  out_model [IL][DL][num_keys][num_features+1] double, intercept
  * last, features absent from the key's rows 0.  compute_var: out_var of the same shape receives the diagonal posterior variance
  * 1 / (1/priorVar[j] + sum_i weight_i p_i (1-p_i) x_ij^2) at the fit (llf/LibLinear.java:328-333), 1/q = priorVar[j] for an absent
- * feature.  All inputs host-or-device; intercept_prior_mean, out_model and out_var host.  With IL = DL = 1, intercept_lambdas[0] =
+ * feature.  Each key is solved in its own column space when that is narrower, as mlease_naive_train's CSR keys are: device memory
+ * scales with each key's own width, and the dense host outputs (IL * DL * num_keys * (num_features+1) doubles, twice with
+ * compute_var) are the limit that remains.  All inputs host-or-device; intercept_prior_mean, out_model and out_var host.  With IL = DL = 1, intercept_lambdas[0] =
  * default_lambdas[0] and zero means the models are bitwise those of mlease_naive_train(prior_mean 0, penalize_intercept 1). */
 int mlease_item_model_train(int32_t device, void* stream, int32_t num_keys, int32_t num_features, const int64_t* key_rowstart,
                             const int64_t* rowptr, const int32_t* colidx, const float* vals, const int32_t* response, const float* weight,

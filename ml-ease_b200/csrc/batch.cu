@@ -202,7 +202,7 @@ int batch_alloc(Batch& B, int num_sms, int hessian_policy, int csr_gram_force) {
   }
   if (int rc = B.mem.get(&B.d_ctrl, (size_t)nprob, true)) return rc;
   if (int rc = B.mem.get(&B.d, (size_t)nprob, true)) return rc;
-  if (nprob > 64)
+  if (nprob > 64 || B.lockstep)
     if (int rc = B.mem.get(&B.d_compact, (size_t)nprob, true)) return rc;
   if (int rc = B.mem.get(&B.d_tmaps, nprob, true)) return rc;
   if (int rc = B.mem.get(&B.d_tiles, (size_t)B.ntiles * 2, true)) return rc;
@@ -397,7 +397,8 @@ int batch_xupdate(Batch& B, cudaStream_t st, double xtol, int max_newton, int po
   CK(newton_begin(B.d, B.nprob, xtol, max_newton, policy, invalidate, B.rebuild_is_expensive, st, &launches));
   // The first slot's flags are known on the host: every problem is running, and a rebuild is due iff the policy says
   // always, the factors were invalidated, or the mirrored control blocks say so (no factor yet / refresh requested).
-  const bool small = B.nprob <= 64;   // small batches read the whole control array back each slot (one sync, no poll kernel)
+  // small batches read the whole control array back each slot (one sync, no poll kernel) and pipeline their slots
+  const bool small = B.nprob <= 64 && !B.lockstep;
   int flag = 1;
   {
     bool emit0 = policy == 1 || invalidate || B.mirror.empty();

@@ -95,6 +95,8 @@ struct Batch {
   int matfree = 0;                // Newton-CG directions from Hv passes: no Gram, factor or inverse is allocated (set in batch_alloc)
   bool has_factor = false;        // batch_factor has run on this batch: Hinv / Ysym hold a factorisation
   bool ysym_shared = false;       // a wide batch whose followers were pointed at their leader's Ysym (chol_share_end_kernel)
+  bool lockstep = false;          // set before batch_alloc: every slot is awaited before the next is enqueued, whatever nprob, so no
+                                  // problem's rebuild is deferred by a speculative slot and each fit is independent of the batch's others
   std::vector<Problem> h;
   Problem* d = nullptr;
   Problem* d_compact = nullptr;   // large batches: Problem structs of the problems that may rebuild in the next slot
@@ -198,6 +200,21 @@ void keyed_record(const std::vector<long long>& bounds, bool streamed, double st
 int gather_rowptr(const int64_t* rowptr, const std::vector<long long>& idx, std::vector<long long>& out);
 // whether the CUDA copy engines can read p directly (device, managed or pinned host memory)
 bool is_dma_ptr(const void* p);
+
+// keyed_cols.cu: the column space of each key of a CSR key range, built after check_csr has accepted the range's rows.  koff[k] ..
+// koff[k + 1]: key k's entries in ci (koff[0] = 0).  Key k's sorted distinct columns are cols[start[k] .. start[k + 1]) (host copy;
+// d_cols on the device), and d_lci[j] is entry j's index in its key's list: the map is monotone, so sorted unique rows stay so.
+// listed[k] = 0 only for a key of more than 2^31 - 1 entries (one sort cannot take it): it has no list.
+struct KeyCols {
+  std::vector<long long> start;
+  std::vector<int> cols;
+  std::vector<unsigned char> listed;
+  int* d_cols = nullptr;
+  int* d_lci = nullptr;
+};
+int key_columns(cudaStream_t st, DevMem& mem, const std::vector<long long>& koff, const int* ci, KeyCols* kc);
+// device bytes key_columns may hold at once for nnz entries of nkeys keys, the largest of max_key_nnz
+size_t key_columns_bytes(long long nnz, long long max_key_nnz, int nkeys);
 
 }  // namespace mlease
 

@@ -36,9 +36,20 @@ __global__ void naive_present_kernel(const Problem* probs, int Dt, int has_bias,
   for (long long j = j0 + threadIdx.x; j < j1; j += blockDim.x) mk[pb.colidx[j]] = 1;
   if (threadIdx.x == 0 && has_bias) mk[Dt - 1] = 1;
 }
-__global__ void gather_i64_kernel(const long long* src, const long long* idx, int n, long long* out) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) out[i] = src[idx[i]];
+// naive_init_kernel for problems in their keys' own column spaces: column c < Dk of problem b is global column cols[span[2b] + c]
+// (Dk = span[2b + 1] - span[2b]) and takes its q and m from the global [ldx] vectors; the intercept (column Dt - 1) takes the global
+// column Dg's (or intercept_mean[b]); the padding between them and beyond Dt gets q = 1, m = 0, which no row touches
+__global__ void local_init_kernel(const Problem* probs, const double* m, const double* q, const double* intercept_mean, const int* cols,
+                                  const long long* span, int Dg) {
+  const Problem& pb = probs[blockIdx.x];
+  const int* c = cols + span[2 * blockIdx.x];
+  const int dk = (int)(span[2 * blockIdx.x + 1] - span[2 * blockIdx.x]);
+  for (int k = threadIdx.x; k < pb.ldx; k += blockDim.x) {
+    pb.beta[k] = 0.0;
+    if (k < dk) { pb.q[k] = q[c[k]]; pb.m[k] = m[c[k]]; }
+    else if (k == pb.Dt - 1) { pb.q[k] = q[Dg]; pb.m[k] = intercept_mean ? intercept_mean[blockIdx.x] : m[Dg]; }
+    else { pb.q[k] = 1.0; pb.m[k] = 0.0; }
+  }
 }
 // One prior of a keyed fit: precision q and mean m of every coefficient ([ldx], the intercept at Dg, 1 / 0 on the padding)
 struct KeyedPrior { std::vector<double> q, m; };
@@ -64,6 +75,8 @@ struct ChunkRows {
   float* X = nullptr;
   const long long* rp = nullptr; const int* ci = nullptr; float* v = nullptr;   // rp: offsets into ci / v
   int csr_unique = 0;
+  const KeyCols* kc = nullptr;   // the column spaces of keys kbase.. (CSR calls wider than 32 columns), else NULL
+  int kbase = 0;
 };
 
 // n bytes from src to dst (pageable host to pinned host) by several threads: one memcpy thread does not keep up with the H2D copy
@@ -92,6 +105,12 @@ void parallel_memcpy(void* dst, const void* src, size_t n) {
 // sorted and unique (csr_unique) is then a property of the range.  Neither mode changes what a key's fit computes: a streamed range
 // solves exactly as a resident call on that range's keys alone.  The mode and the plan are host arithmetic on the shapes, the CSR
 // offsets at the key boundaries and the free memory, never on the values.
+// Column spaces (CSR): a key whose Dk distinct listed columns give round_up(Dk + 1, 32) < round_up(Dg + 1, 32) is solved in its own
+// space of Dt_k = round_up(Dk + 1, 32) columns: its Dk listed features in ascending order, padding (q = 1, m = 0, no row touches it,
+// so beta stays 0 there) and the intercept at Dt_k - 1.  Every other key runs at the global width Dt = Dg + 1.  The choice and the
+// shape depend on the key's own rows alone, never on which keys share its call, chunk or streamed range; each chunk runs one batch
+// per width.  Outputs are scattered back to the global columns: a feature the key does not list keeps 0 in the model and 1/q in the
+// variance.
 struct KeyedFit {
   int num_sms; cudaStream_t st; int32_t K, Dg; const int64_t* key_rowstart; const int64_t* rowptr; const int32_t* colidx; const float* vals;
   int64_t ldx_in; const int32_t* response; const float* weight; const float* offset; bool has_intercept; int32_t data_size_threshold;
@@ -101,13 +120,34 @@ struct KeyedFit {
   int L = 0, Dt = 0, ldx = 0, Dp = 0, ldh = 0;
   std::vector<long long> krs, key_nnz0;   // key_nnz0: CSR rowptr at the key boundaries
   std::vector<int> todo;                  // the keys that are fitted
+  bool lists = false;                     // CSR with Dt > 32: a key may be narrower than Dt, so every range builds its column lists
+  std::vector<int> kdt;                   // the width (Dt or Dt_k) of each key's problems, known once its range's lists exist
   Counters cnt;
 
   bool solves(int k) const { const long long nk = krs[k + 1] - krs[k]; return !(nk < data_size_threshold || nk <= 0); }   // (:379-382)
-  // device bytes of a fitted key of n rows: Xt (n*Dp*2) + Hpart + Lc per problem (+ the row weights of the variance)
-  size_t state_bytes(long long n) const {
-    return (size_t)n * Dp * 2 + (size_t)Dp * Dp * 4 + 3 * (size_t)ldh * ldh * 8 + 2 * (size_t)ldh * 32 * 8 + 64 * (size_t)ldx +
-           (out_var ? (size_t)n * 8 : 0);
+  // the width of a key of dk distinct columns; with dk = its stored entries, a bound on it before the lists exist
+  int local_dt(long long dk) const { const int w = round_up((int)std::min<long long>(dk, Dg) + 1, 32); return w < ldh ? w : Dt; }
+  int bound_dt(int k) const { return lists ? local_dt(key_nnz0[k + 1] - key_nnz0[k]) : Dt; }
+  // device bytes of a fitted key of n rows at width w: Xt (n*Dp*2) + Hpart + Lc per problem (+ the row weights of the variance)
+  size_t state_bytes(long long n, int w) const {
+    const size_t x = (size_t)round_up(w, 4), p = (size_t)round_up((int)x, 128), h = (size_t)round_up(w, 32);
+    return (size_t)n * p * 2 + p * p * 4 + 3 * h * h * 8 + 2 * h * 32 * 8 + 64 * x + (out_var ? (size_t)n * 8 : 0);
+  }
+  // the lists of keys [k0, k1) over the range's colidx ci (entries from key_nnz0[k0] on), and the widths they give
+  int build_lists(int k0, int k1, const int* ci, cudaStream_t s, DevMem& mem, KeyCols* kc) {
+    std::vector<long long> koff(key_nnz0.begin() + k0, key_nnz0.begin() + k1 + 1);
+    for (auto& o : koff) o -= key_nnz0[k0];
+    if (int rc = key_columns(s, mem, koff, ci, kc)) return rc;
+    for (int k = k0; k < k1; k++)
+      kdt[k] = kc->listed[k - k0] ? local_dt(kc->start[k - k0 + 1] - kc->start[k - k0]) : Dt;
+    return 0;
+  }
+  // device bytes of the lists of keys [k0, k1)
+  size_t list_bytes(int k0, int k1) const {
+    if (!lists) return 0;
+    long long mx = 0;
+    for (int k = k0; k < k1; k++) mx = std::max(mx, key_nnz0[k + 1] - key_nnz0[k]);
+    return key_columns_bytes(key_nnz0[k1] - key_nnz0[k0], mx, k1 - k0);
   }
   void init_outputs() {
     for (size_t e = 0; e < (size_t)L * K * Dt; e++) out_model[e] = 0.0;
@@ -126,6 +166,7 @@ struct KeyedFit {
   int resident();
   int streamed(size_t budget);
   int solve_chunk(const int* keys, int nprob, const ChunkRows& cr, int* dflag, int* hflag);
+  int solve_batch(const int* keys, int nprob, int width, const ChunkRows& cr, int* dflag, int* hflag);
 };
 
 int KeyedFit::run() {
@@ -137,17 +178,28 @@ int KeyedFit::run() {
   const long long ntot = krs[K];
   for (int k = 0; k < K; k++) if (krs[k + 1] < krs[k]) return fail(MLEASE_ERR_INVALID, "key_rowstart must be non-decreasing");
   for (int k = 0; k < K; k++) if (solves(k)) todo.push_back(k);
-  // the bytes of the resident upload (rows, labels, key boundaries, the temporaries of host input) and of the first chunk's state
+  kdt.assign(K, Dt);
+  if (csr) {
+    // rowptr at the key boundaries and at row 0, read without uploading the rows: each key's stored entries bound its width
+    std::vector<long long> idx(krs);
+    idx.push_back(0);
+    if (int rc = gather_rowptr(rowptr, idx, key_nnz0)) return rc;
+    if (key_nnz0.back() != 0) return fail(MLEASE_ERR_INVALID, "rowptr[0] must be 0");
+    key_nnz0.pop_back();
+    // any key may list fewer columns than the dictionary holds (the bound above only caps its width): every range builds its lists
+    lists = ldh > 32 && !todo.empty();
+  }
+  // the bytes of the resident upload (rows, labels, key boundaries, the temporaries of host input, the column lists) and of the
+  // first chunk's state
   size_t free_b, total_b;
   CK(cudaMemGetInfo(&free_b, &total_b));
   const size_t budget = keyed_budget(free_b);
-  long long nnz = 0;
-  if (csr) CK(cudaMemcpy(&nnz, rowptr + ntot, 8, cudaMemcpyDefault));
+  const long long nnz = csr ? key_nnz0[K] : 0;
   const bool host_rows = !is_device_ptr(csr ? (const void*)colidx : (const void*)vals);
   size_t up = (size_t)ntot * 9 + (is_device_ptr(response) ? 0 : (size_t)ntot * 12);
-  if (csr) up += (size_t)nnz * 4 + (host_rows ? (size_t)nnz * 4 + (size_t)(ntot + 1) * 8 : 0) + (size_t)(K + 1) * 16;
+  if (csr) up += (size_t)nnz * 4 + (host_rows ? (size_t)nnz * 4 + (size_t)(ntot + 1) * 8 : 0) + (size_t)(K + 1) * 16 + list_bytes(0, K);
   else up += (size_t)ntot * ldx * 4 + (host_rows ? (size_t)256 << 20 : 0);
-  const size_t first = todo.empty() ? 0 : state_bytes(krs[todo[0] + 1] - krs[todo[0]]);
+  const size_t first = todo.empty() ? 0 : state_bytes(krs[todo[0] + 1] - krs[todo[0]], bound_dt(todo[0]));
   return up + first <= budget ? resident() : streamed(budget);
 }
 
@@ -157,7 +209,7 @@ int KeyedFit::resident() {
   PinnedMem pinned;
   float* dX = nullptr; signed char* dy; float *dw, *dofs; int* dflag; int* hflag;
   const long long* d_rp = nullptr; const int* d_ci = nullptr; float* d_v = nullptr;
-  key_nnz0.assign(K + 1, 0);
+  KeyCols kc;
   int csr_unique = 0;
   if (int rc = t.get(&dy, (size_t)ntot, false)) return rc;
   if (int rc = t.get(&dw, (size_t)ntot, false)) return rc;
@@ -169,11 +221,7 @@ int KeyedFit::resident() {
     if (int rc = upload_dense_rows(dX, ldx, vals, ldx_in, ntot, Dg, has_intercept ? 1 : 0, st)) return rc;
   } else {
     if (int rc = to_device(t, (const long long*)rowptr, (size_t)ntot + 1, &d_rp, st)) return rc;
-    long long nnz = 0, first = 0;
-    CK(cudaMemcpyAsync(&nnz, d_rp + ntot, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&first, d_rp, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (first != 0) return fail(MLEASE_ERR_INVALID, "rowptr[0] must be 0");
+    const long long nnz = key_nnz0[K];
     if (int rc = to_device(t, colidx, (size_t)nnz, &d_ci, st)) return rc;
     // values are copied even when they already live on the device: binary.feature rewrites them
     if (int rc = t.get(&d_v, (size_t)nnz, false)) return rc;
@@ -181,21 +229,17 @@ int KeyedFit::resident() {
     CK(cudaMemsetAsync(dflag, 0, 8, st));
     check_csr(st, ntot, nnz, d_rp, d_ci, d_v, Dg, binary_feature, dflag);
     CK(cudaMemcpyAsync(hflag, dflag, 8, cudaMemcpyDeviceToHost, st));
-    // rowptr at the key boundaries (nnz per key for the cost model and the byte accounting)
-    long long* d_kn; long long* d_krs;
-    if (int rc = t.get(&d_kn, (size_t)K + 1, false)) return rc;
-    if (int rc = t.get(&d_krs, (size_t)K + 1, false)) return rc;
-    CK(cudaMemcpyAsync(d_krs, krs.data(), (size_t)(K + 1) * 8, cudaMemcpyHostToDevice, st));
-    gather_i64_kernel<<<(K + 256) / 256, 256, 0, st>>>(d_rp, d_krs, K + 1, d_kn);
-    CK(cudaMemcpyAsync(key_nnz0.data(), d_kn, (size_t)(K + 1) * 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     if (hflag[0]) return fail(MLEASE_ERR_INVALID, "feature index out of range");
     csr_unique = hflag[1] ? 0 : 1;
+    if (lists)
+      if (int rc = build_lists(0, K, d_ci, st, t, &kc)) return rc;
   }
   if (int rc = ingest_labels(st, ntot, response, weight, offset, dy, dw, dofs, dflag, hflag, nullptr)) return rc;
   init_outputs();
   ChunkRows cr;
   cr.y = dy; cr.w = dw; cr.o = dofs; cr.X = dX; cr.rp = d_rp; cr.ci = d_ci; cr.v = d_v; cr.csr_unique = csr_unique;
+  cr.kc = lists ? &kc : nullptr;
   // chunk size bounded by memory
   size_t free_b, total_b;
   CK(cudaMemGetInfo(&free_b, &total_b));
@@ -206,7 +250,7 @@ int KeyedFit::resident() {
     size_t bytes = 0;
     size_t end = pos;
     while (end < todo.size() && end - pos < 16384) {
-      const size_t need = state_bytes(krs[todo[end] + 1] - krs[todo[end]]);
+      const size_t need = state_bytes(krs[todo[end] + 1] - krs[todo[end]], kdt[todo[end]]);
       if (end > pos && bytes + need > free_b / 2) break;
       bytes += need;
       end++;
@@ -219,11 +263,31 @@ int KeyedFit::resident() {
   return finish(bounds, false, 0, 0);
 }
 
-// the problems keys[0, nprob) over the rows of cr, every prior, into out_model / out_var
+// the problems keys[0, nprob) over the rows of cr, every prior, into out_model / out_var: one batch per width, narrowest first
 int KeyedFit::solve_chunk(const int* keys, int nprob, const ChunkRows& cr, int* dflag, int* hflag) {
+  std::vector<int> widths;
+  for (int b = 0; b < nprob; b++) widths.push_back(kdt[keys[b]]);
+  std::sort(widths.begin(), widths.end());
+  widths.erase(std::unique(widths.begin(), widths.end()), widths.end());
+  std::vector<int> group;
+  for (int w : widths) {
+    group.clear();
+    for (int b = 0; b < nprob; b++) if (kdt[keys[b]] == w) group.push_back(keys[b]);
+    if (int rc = solve_batch(group.data(), (int)group.size(), w, cr, dflag, hflag)) return rc;
+  }
+  return 0;
+}
+
+// the problems keys[0, nprob) of width w: Dt (today's global-width problems), or the keys' own column spaces (w < Dt)
+int KeyedFit::solve_batch(const int* keys, int nprob, int w, const ChunkRows& cr, int* dflag, int* hflag) {
+  const bool local = w != Dt;
   Batch B;
-  B.nprob = nprob; B.Dt = Dt; B.ldx = ldx; B.csr = csr; B.has_bias = has_intercept ? 1 : 0;
+  B.nprob = nprob; B.Dt = w; B.ldx = round_up(w, 4); B.csr = csr; B.has_bias = has_intercept ? 1 : 0;
+  // a local batch's members depend on the call (its chunk, its width group): without the slot pipeline a key's path, hence a one-row
+  // key's bits, do not depend on them
+  B.lockstep = local;
   B.h.resize(B.nprob);
+  std::vector<long long> span(local ? 2 * (size_t)nprob : 0);   // each problem's list in cr.kc's columns
   std::vector<long long> row_start(B.nprob + 1, 0);   // the chunk's rows numbered across its problems (batched variance)
   for (int b = 0; b < B.nprob; b++) {
     const int k = keys[b];
@@ -235,17 +299,21 @@ int KeyedFit::solve_chunk(const int* keys, int nprob, const ChunkRows& cr, int* 
     if (csr) {
       // a key = a row range of the CSR: the row pointers keep their offsets into colidx / vals
       p.rowptr = cr.rp + r; p.colidx = cr.ci; p.vals = cr.v; p.nnz_hint = key_nnz0[k + 1] - key_nnz0[k]; p.csr_unique = cr.csr_unique;
+      if (local) {   // the same entries, each naming its index in the key's list
+        p.colidx = cr.kc->d_lci;
+        span[2 * b] = cr.kc->start[k - cr.kbase]; span[2 * b + 1] = cr.kc->start[k - cr.kbase + 1];
+      }
     } else {
       p.X = cr.X + (size_t)r * ldx;
     }
     row_start[b + 1] = row_start[b] + p.n;
   }
   if (int rc = batch_alloc(B, num_sms, 0)) return rc;
-  DevMem ct;   // the chunk's temporaries: freed with the chunk, before the next chunk's batch_alloc
-  double *dm, *dq, *dout, *dim = nullptr, *dvec = nullptr; long long* drs = nullptr; unsigned char* dmask = nullptr;
+  DevMem ct;   // the batch's temporaries: freed with it, before the next batch_alloc
+  double *dm, *dq, *dout, *dim = nullptr, *dvec = nullptr; long long *drs = nullptr, *dspan = nullptr; unsigned char* dmask = nullptr;
   if (int rc = ct.get(&dm, (size_t)ldx, false)) return rc;
   if (int rc = ct.get(&dq, (size_t)ldx, false)) return rc;
-  if (int rc = ct.get(&dout, (size_t)B.nprob * Dt, false)) return rc;
+  if (int rc = ct.get(&dout, (size_t)B.nprob * w, false)) return rc;
   if (intercept_mean) {
     std::vector<double> im(B.nprob);
     for (int b = 0; b < B.nprob; b++) im[b] = intercept_mean[keys[b]];
@@ -258,39 +326,52 @@ int KeyedFit::solve_chunk(const int* keys, int nprob, const ChunkRows& cr, int* 
     if (int rc = ct.get(&drs, row_start.size(), false)) return rc;
     CK(cudaMemcpyAsync(drs, row_start.data(), row_start.size() * 8, cudaMemcpyHostToDevice, st));
   }
-  if (csr) {
+  if (local) {
+    if (int rc = ct.get(&dspan, span.size(), false)) return rc;
+    CK(cudaMemcpyAsync(dspan, span.data(), span.size() * 8, cudaMemcpyHostToDevice, st));
+  } else if (csr) {
     // features absent from a key's rows are not part of its dataset, hence not of its model (llf/LibLinear.java:343-350; the only
     // prior mean a caller may set per key is the intercept's, which every dataset holds, so :374-383 adds nothing): mask them out
     if (int rc = ct.get(&dmask, (size_t)B.nprob * Dt, false)) return rc;
     CK(cudaMemsetAsync(dmask, 0, (size_t)B.nprob * Dt, st));
     naive_present_kernel<<<B.nprob, 256, 0, st>>>(B.d, Dt, has_intercept ? 1 : 0, dmask);
   }
-  std::vector<double> xs((size_t)B.nprob * Dt);
+  // a local problem's column c < Dk is global column cols[c]; its intercept (column w - 1) is global column Dg
+  auto scatter = [&](double* dst, const double* x, int b, bool inv) {
+    const long long s0 = span[2 * b], dk = span[2 * b + 1] - s0;
+    const int* cols = cr.kc->cols.data() + s0;
+    for (long long c = 0; c < dk; c++) dst[cols[c]] = inv ? 1.0 / x[c] : x[c];
+    dst[Dg] = inv ? 1.0 / x[w - 1] : x[w - 1];
+  };
+  std::vector<double> xs((size_t)B.nprob * w);
   for (int l = 0; l < L; l++) {
     CK(cudaMemcpyAsync(dm, priors[l].m.data(), ldx * 8, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(dq, priors[l].q.data(), ldx * 8, cudaMemcpyHostToDevice, st));
     CK(cudaStreamSynchronize(st));   // dq / dm are reused by the next prior
-    naive_init_kernel<<<B.nprob, 128, 0, st>>>(B.d, dm, dq, dim);
+    if (local) local_init_kernel<<<B.nprob, 128, 0, st>>>(B.d, dm, dq, dim, cr.kc->d_cols, dspan, Dg);
+    else naive_init_kernel<<<B.nprob, 128, 0, st>>>(B.d, dm, dq, dim);
     B.mirror.clear();                // the factors of the previous prior belong to another prior
     if (int rc = batch_xupdate(B, st, 2e-7, 100, 0, 1, hflag, dflag, cnt)) return rc;
-    gather_beta_kernel<<<B.nprob, 128, 0, st>>>(B.d, Dt, dout, dmask, 0);
+    gather_beta_kernel<<<B.nprob, 128, 0, st>>>(B.d, w, dout, dmask, 0);
     CK(cudaMemcpyAsync(xs.data(), dout, xs.size() * 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     for (int b = 0; b < B.nprob; b++) {
       double* dst = out_model + ((size_t)l * K + keys[b]) * Dt;
-      std::memcpy(dst, xs.data() + (size_t)b * Dt, Dt * 8);
+      if (local) scatter(dst, xs.data() + (size_t)b * w, b, false);
+      else std::memcpy(dst, xs.data() + (size_t)b * Dt, Dt * 8);
       if (!has_intercept) dst[Dg] = 0.0;
     }
     if (out_var) {
-      // posteriorVar, diagonal (llf/LibLinear.java:328-333): one pass over the chunk's rows for all of its keys
+      // posteriorVar, diagonal (llf/LibLinear.java:328-333): one pass over the batch's rows for all of its keys
       CK(postvar_rowweights(B.d, B.nprob, drs, row_start[B.nprob], B.has_bias, dvec, st, nullptr));
       CK(postvar_diag(B.d, B.nprob, drs, row_start[B.nprob], dvec, B.has_bias, st, nullptr));
-      gather_beta_kernel<<<B.nprob, 128, 0, st>>>(B.d, Dt, dout, nullptr, 1);
+      gather_beta_kernel<<<B.nprob, 128, 0, st>>>(B.d, w, dout, nullptr, 1);
       CK(cudaMemcpyAsync(xs.data(), dout, xs.size() * 8, cudaMemcpyDeviceToHost, st));
       CK(cudaStreamSynchronize(st));
       for (int b = 0; b < B.nprob; b++) {
         double* dst = out_var + ((size_t)l * K + keys[b]) * Dt;
-        for (int j = 0; j < Dt; j++) dst[j] = 1.0 / xs[(size_t)b * Dt + j];
+        if (local) scatter(dst, xs.data() + (size_t)b * w, b, true);   // unlisted features keep init_outputs' 1/q
+        else for (int j = 0; j < Dt; j++) dst[j] = 1.0 / xs[(size_t)b * Dt + j];
       }
     }
   }
@@ -298,19 +379,12 @@ int KeyedFit::solve_chunk(const int* keys, int nprob, const ChunkRows& cr, int* 
 }
 
 int KeyedFit::streamed(size_t budget) {
-  if (csr) {
-    // rowptr at the key boundaries and at row 0, read without uploading the rows
-    std::vector<long long> idx(krs);
-    idx.push_back(0);
-    if (int rc = gather_rowptr(rowptr, idx, key_nnz0)) return rc;
-    if (key_nnz0.back() != 0) return fail(MLEASE_ERR_INVALID, "rowptr[0] must be 0");
-    key_nnz0.pop_back();
-  }
-  // the plan: contiguous key ranges whose rows (staged copy + the solver's layout) and fitted keys' state fit a quarter of the budget
+  // the plan: contiguous key ranges whose rows (staged copy + the solver's layout, the column lists) and fitted keys' state (at the
+  // bound of their widths) fit a quarter of the budget
   auto row_bytes = [&](int k) -> size_t {
     const size_t n = (size_t)(krs[k + 1] - krs[k]);
     size_t b = n * (12 + 9);
-    b += csr ? n * 16 + (size_t)(key_nnz0[k + 1] - key_nnz0[k]) * 8 : n * ((size_t)ldx_in + ldx) * 4;
+    b += csr ? n * 16 + (size_t)(key_nnz0[k + 1] - key_nnz0[k]) * 8 + list_bytes(k, k + 1) : n * ((size_t)ldx_in + ldx) * 4;
     return b;
   };
   const size_t cap = budget / 4;
@@ -320,7 +394,7 @@ int KeyedFit::streamed(size_t budget) {
     int e = k, fitted = 0;
     size_t bytes = 0;
     while (e < K) {
-      const size_t need = row_bytes(e) + (solves(e) ? state_bytes(krs[e + 1] - krs[e]) : 0);
+      const size_t need = row_bytes(e) + (solves(e) ? state_bytes(krs[e + 1] - krs[e], bound_dt(e)) : 0);
       if (e > k && (bytes + need > cap || (solves(e) && fitted >= 16384))) break;
       bytes += need; fitted += solves(e) ? 1 : 0; e++;
     }
@@ -421,6 +495,8 @@ int KeyedFit::streamed(size_t budget) {
     auto slot = [&](const void* p) -> void* { for (auto& s : srcs) if (s.p == p) return s.dev[b]; return nullptr; };
     ChunkRows cr;
     cr.row0 = r0; cr.y = dy; cr.w = dw; cr.o = dofs;
+    DevMem lmem;   // the range's column lists
+    KeyCols kc;
     // the range's checks, before any kernel reads its rows
     if (csr) {
       const long long nnz = key_nnz0[bounds[c + 1]] - key_nnz0[bounds[c]];
@@ -432,6 +508,10 @@ int KeyedFit::streamed(size_t budget) {
       CK(cudaStreamSynchronize(st));
       if (hflag[0]) return fail(MLEASE_ERR_INVALID, "feature index out of range");
       cr.csr_unique = hflag[1] ? 0 : 1;
+      if (lists) {
+        if (int rc = build_lists((int)bounds[c], (int)bounds[c + 1], cr.ci, st, lmem, &kc)) return rc;
+        cr.kc = &kc; cr.kbase = (int)bounds[c];
+      }
     } else {
       if (int rc = upload_dense_rows(dX, ldx, (const float*)slot(vals), ldx_in, n, Dg, has_intercept ? 1 : 0, st)) return rc;
       cr.X = dX;
