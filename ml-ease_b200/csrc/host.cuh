@@ -5,7 +5,9 @@
 #include <cuda.h>
 
 #include <cstring>
+#include <functional>
 #include <string>
+#include <thread>
 #include <vector>
 
 #include "../../include/mlease_b200.h"
@@ -193,13 +195,67 @@ void rebase_rowptr(cudaStream_t st, long long n, const long long* src, long long
 
 // Keyed calls (keyed_fit.cu, k5_score.cu).  keyed_budget: the device bytes the mode decision and the chunk plan of a keyed call may
 // use, min(free, the test cap of mlease_internal_set_keyed_budget).  keyed_record: the key boundaries of the chunks the call ran and
-// whether it streamed, with the host time the streamed rows took to stage and the time the solve waited for them.
+// whether it streamed, with the host time the streamed rows took to stage and the time the fit or the scoring waited for them.
 size_t keyed_budget(size_t free_b);
 void keyed_record(const std::vector<long long>& bounds, bool streamed, double stage_ms, double wait_ms);
 // host copies of rowptr[idx[i]] (host or device rowptr)
 int gather_rowptr(const int64_t* rowptr, const std::vector<long long>& idx, std::vector<long long>& out);
 // whether the CUDA copy engines can read p directly (device, managed or pinned host memory)
 bool is_dma_ptr(const void* p);
+
+// key_ranges.cu: the one pipeline of the keyed calls.  A call cuts its keys into contiguous ranges; a range's rows get onto the
+// device, pass their checks and are then fitted or scored.  The resident call is the plan of exactly one range.
+// plan_ranges: [0, n) cut greedily: item e joins the current range while the range's cost plus cost(e) stays within cap and, if
+// e is counted (NULL: every item), the range holds fewer than limit counted items; the first item of a range always joins.
+// -> the bounds {0, .., n} ({0} for n = 0).
+std::vector<long long> plan_ranges(long long n, size_t cap, long long limit, const std::function<size_t(long long)>& cost,
+                                   const std::function<bool(long long)>& counted);
+// n bytes from src to dst (pageable host to pinned host) by several threads: one memcpy thread does not keep up with the H2D copy
+void parallel_memcpy(void* dst, const void* src, size_t n);
+// One input array of a keyed call (p NULL: absent) and how a range's part is cut from it: ROW one element per row, ROWPTR the
+// range's n + 1 row pointers, ENTRY its stored CSR entries, DENSE its rows ld elements apart (the last one Dg long).
+struct RangeSrc { const void* p; size_t esize; enum { ROW, ROWPTR, ENTRY, DENSE } cut; };
+// The staging ring over ranges c with rows row_at[c] .. row_at[c + 1] and entries nnz_at[c] .. nnz_at[c + 1] of a call whose mode
+// decision chose to stream (staged), whatever the number of its ranges.  A resident call stages nothing: view() hands the caller's
+// pointers through, and no slot, stream, event or thread is made.  A streamed call holds two device slots per source; open() stages
+// range 0 and start(c + 1) stages range c + 1 while range c runs, H2D on a copy stream that first waits for what the caller queued on
+// st.  With bounce, a host thread stages it, pageable input through a pinned buffer filled by parallel_memcpy; without, the calling
+// thread queues direct copies of every source.  view(c) gives each source's slot of range c, with st ordered after its copies;
+// done(c) records on st that the caller has finished with range c's slot.  stage_ms: host time spent staging; wait_ms: the time
+// view() waited for the staging thread (0 without bounce, where staging runs on the calling thread).
+class RangeRing {
+ public:
+  RangeRing(cudaStream_t st, std::vector<RangeSrc> srcs, std::vector<long long> row_at, std::vector<long long> nnz_at, long long ld, int Dg,
+            bool staged, bool bounce)
+      : st_(st), srcs_(std::move(srcs)), row_at_(std::move(row_at)), nnz_at_(std::move(nnz_at)), ld_(ld), Dg_(Dg), staged_(staged),
+        bounce_(bounce) {}
+  RangeRing(const RangeRing&) = delete;
+  RangeRing& operator=(const RangeRing&) = delete;
+  ~RangeRing();
+  bool staged() const { return staged_; }
+  int open();
+  int start(int c);
+  int view(int c, const void** v);
+  int done(int c);
+  double stage_ms = 0, wait_ms = 0;
+
+ private:
+  struct Slot { bool dma = false; char* dev[2] = {nullptr, nullptr}; char* host[2] = {nullptr, nullptr}; };
+  void cut(const RangeSrc& s, int c, size_t* first, size_t* count) const;
+  cudaError_t stage(int c);
+  cudaStream_t st_, cs_ = nullptr;
+  std::vector<RangeSrc> srcs_;
+  std::vector<long long> row_at_, nnz_at_;
+  long long ld_;
+  int Dg_, device_ = 0;
+  bool staged_, bounce_;
+  std::vector<Slot> slot_;
+  DevMem mem_;
+  PinnedMem pinned_;
+  cudaEvent_t up_[2] = {nullptr, nullptr}, done_[2] = {nullptr, nullptr}, in_ = nullptr;
+  std::thread stager_;
+  cudaError_t stage_err_ = cudaSuccess;
+};
 
 // keyed_cols.cu: the column space of each key of a CSR key range, built after check_csr has accepted the range's rows.  koff[k] ..
 // koff[k + 1]: key k's entries in ci (koff[0] = 0).  Key k's sorted distinct columns are cols[start[k] .. start[k + 1]) (host copy;

@@ -1,10 +1,8 @@
 // keyed_fit.cu -- K independent fits per prior over one upload of the rows: RegressionNaiveTrain (mlease_naive_train,
 // mlease_naive_train_dense) and ItemModelTrain (mlease_item_model_train).
 #include <algorithm>
-#include <chrono>
 #include <cstring>
 #include <string>
-#include <thread>
 #include <vector>
 
 #include "host.cuh"
@@ -68,7 +66,7 @@ int keyed_fit_check(int32_t device, int32_t Dg, const int64_t* rowptr, const int
   return open_device(device, num_sms);
 }
 
-// The device arrays the problems of a chunk point into; element 0 of the row arrays is row row0 of the call (0 when resident)
+// The device arrays the problems of a chunk point into; element 0 of the row arrays is row row0 of the call (its range's first)
 struct ChunkRows {
   long long row0 = 0;
   signed char* y = nullptr; float* w = nullptr; float* o = nullptr;
@@ -79,30 +77,11 @@ struct ChunkRows {
   int kbase = 0;
 };
 
-// n bytes from src to dst (pageable host to pinned host) by several threads: one memcpy thread does not keep up with the H2D copy
-void parallel_memcpy(void* dst, const void* src, size_t n) {
-  const size_t per = size_t(8) << 20;
-  const size_t hw = std::max(1u, std::min(8u, std::thread::hardware_concurrency()));
-  const int nt = (int)std::min(hw, (n + per - 1) / per);
-  if (nt <= 1) { if (n) std::memcpy(dst, src, n); return; }
-  std::vector<std::thread> ts;
-  const size_t step = (n + nt - 1) / nt;
-  for (int t = 0; t < nt; t++) {
-    const size_t a = std::min(n, t * step), b = std::min(n, a + step);
-    try {
-      ts.emplace_back([=] { std::memcpy((char*)dst + a, (const char*)src + a, b - a); });
-    } catch (const std::exception&) {   // no thread to spare: this slice on the calling thread
-      std::memcpy((char*)dst + a, (const char*)src + a, b - a);
-    }
-  }
-  for (auto& t : ts) t.join();
-}
-
-// One keyed fit call.  Resident mode (the whole upload and the first chunk's state fit the budget): every row is uploaded once,
-// then solved in chunks of keys.  Streamed mode: contiguous key ranges, each holding its own rows next to its solver state within a
-// quarter of the budget; the rows of range c+1 are staged (pageable input through a pinned ring, by several host threads) and
-// copied on a second stream while range c is solved, and each range passes the row checks before any of its rows is read.  Rows
-// sorted and unique (csr_unique) is then a property of the range.  Neither mode changes what a key's fit computes: a streamed range
+// One keyed fit call, over the key ranges of the keyed pipeline (key_ranges.cu).  Resident (the whole upload and the first chunk's
+// state fit the budget): one range, every row uploaded once, then solved in chunks of keys.  Streamed: contiguous key ranges, each
+// holding its own rows next to its solver state within a quarter of the budget and solved as one chunk, the rows of range c+1
+// staged through the ring while range c is solved.  Each range passes the row checks before any of its rows is read, so rows
+// sorted and unique (csr_unique) is a property of the range.  Neither mode changes what a key's fit computes: a streamed range
 // solves exactly as a resident call on that range's keys alone.  The mode and the plan are host arithmetic on the shapes, the CSR
 // offsets at the key boundaries and the free memory, never on the values.
 // Column spaces (CSR): a key whose Dk distinct listed columns give round_up(Dk + 1, 32) < round_up(Dg + 1, 32) is solved in its own
@@ -157,14 +136,7 @@ struct KeyedFit {
         for (int k = 0; k < K; k++)
           for (int j = 0; j < Dt; j++) out_var[((size_t)l * K + k) * Dt + j] = 1.0 / priors[l].q[j];
   }
-  int finish(const std::vector<long long>& bounds, bool streamed, double stage_ms, double wait_ms) {
-    keyed_record(bounds, streamed, stage_ms, wait_ms);
-    if (cnt.not_converged) return fail(MLEASE_ERR_NUMERIC, "Model fitting error! (" + std::to_string(cnt.not_converged) + " fits did not converge)");
-    return 0;
-  }
   int run();
-  int resident();
-  int streamed(size_t budget);
   int solve_chunk(const int* keys, int nprob, const ChunkRows& cr, int* dflag, int* hflag);
   int solve_batch(const int* keys, int nprob, int width, const ChunkRows& cr, int* dflag, int* hflag);
 };
@@ -189,8 +161,8 @@ int KeyedFit::run() {
     // any key may list fewer columns than the dictionary holds (the bound above only caps its width): every range builds its lists
     lists = ldh > 32 && !todo.empty();
   }
-  // the bytes of the resident upload (rows, labels, key boundaries, the temporaries of host input, the column lists) and of the
-  // first chunk's state
+  // resident (one range) when the whole upload (rows, labels, key boundaries, the temporaries of host input, the column lists) and
+  // the first chunk's state fit the budget
   size_t free_b, total_b;
   CK(cudaMemGetInfo(&free_b, &total_b));
   const size_t budget = keyed_budget(free_b);
@@ -200,67 +172,93 @@ int KeyedFit::run() {
   if (csr) up += (size_t)nnz * 4 + (host_rows ? (size_t)nnz * 4 + (size_t)(ntot + 1) * 8 : 0) + (size_t)(K + 1) * 16 + list_bytes(0, K);
   else up += (size_t)ntot * ldx * 4 + (host_rows ? (size_t)256 << 20 : 0);
   const size_t first = todo.empty() ? 0 : state_bytes(krs[todo[0] + 1] - krs[todo[0]], bound_dt(todo[0]));
-  return up + first <= budget ? resident() : streamed(budget);
-}
-
-int KeyedFit::resident() {
-  const long long ntot = krs[K];
+  const bool streamed = up + first > budget;
+  std::vector<long long> ranges{0, K};
+  if (streamed) {
+    // streamed: ranges whose rows (staged copy + the solver's layout, the column lists) and fitted keys' state (at the bound of
+    // their widths) fit a quarter of the budget
+    ranges = plan_ranges(K, budget / 4, 16384, [&](long long k) -> size_t {
+      const size_t n = (size_t)(krs[k + 1] - krs[k]);
+      size_t b = n * (12 + 9);
+      b += csr ? n * 16 + (size_t)(key_nnz0[k + 1] - key_nnz0[k]) * 8 + list_bytes(k, k + 1) : n * ((size_t)ldx_in + ldx) * 4;
+      return b + (solves(k) ? state_bytes(n, bound_dt(k)) : 0);
+    }, [&](long long k) { return solves(k); });
+  }
+  const int nr = (int)ranges.size() - 1;
+  std::vector<long long> row_at, nnz_at;
+  for (long long k : ranges) { row_at.push_back(krs[k]); if (csr) nnz_at.push_back(key_nnz0[k]); }
+  enum { RP, CI, V, Y, W, O };   // the sources; the dense rows are V
+  RangeRing ring(st, {{rowptr, 8, RangeSrc::ROWPTR}, {colidx, 4, RangeSrc::ENTRY}, {vals, 4, csr ? RangeSrc::ENTRY : RangeSrc::DENSE},
+                      {response, 4, RangeSrc::ROW}, {weight, 4, RangeSrc::ROW}, {offset, 4, RangeSrc::ROW}}, row_at, nnz_at, ldx_in, Dg,
+                      streamed, true);
+  long long max_rows = 0;
+  for (int c = 0; c < nr; c++) max_rows = std::max(max_rows, row_at[c + 1] - row_at[c]);
   DevMem t;
   PinnedMem pinned;
-  float* dX = nullptr; signed char* dy; float *dw, *dofs; int* dflag; int* hflag;
-  const long long* d_rp = nullptr; const int* d_ci = nullptr; float* d_v = nullptr;
-  KeyCols kc;
-  int csr_unique = 0;
-  if (int rc = t.get(&dy, (size_t)ntot, false)) return rc;
-  if (int rc = t.get(&dw, (size_t)ntot, false)) return rc;
-  if (int rc = t.get(&dofs, (size_t)ntot, false)) return rc;
+  signed char* dy; float *dw, *dofs, *dX = nullptr; int* dflag; int* hflag;
+  if (int rc = t.get(&dy, (size_t)max_rows, false)) return rc;
+  if (int rc = t.get(&dw, (size_t)max_rows, false)) return rc;
+  if (int rc = t.get(&dofs, (size_t)max_rows, false)) return rc;
   if (int rc = t.get(&dflag, 16, false)) return rc;
   if (int rc = pinned.get(&hflag, 16, false)) return rc;
-  if (!csr) {
-    if (int rc = t.get(&dX, (size_t)ntot * ldx, false)) return rc;
-    if (int rc = upload_dense_rows(dX, ldx, vals, ldx_in, ntot, Dg, has_intercept ? 1 : 0, st)) return rc;
-  } else {
-    if (int rc = to_device(t, (const long long*)rowptr, (size_t)ntot + 1, &d_rp, st)) return rc;
-    const long long nnz = key_nnz0[K];
-    if (int rc = to_device(t, colidx, (size_t)nnz, &d_ci, st)) return rc;
-    // values are copied even when they already live on the device: binary.feature rewrites them
-    if (int rc = t.get(&d_v, (size_t)nnz, false)) return rc;
-    CK(cudaMemcpyAsync(d_v, vals, (size_t)nnz * 4, cudaMemcpyDefault, st));
-    CK(cudaMemsetAsync(dflag, 0, 8, st));
-    check_csr(st, ntot, nnz, d_rp, d_ci, d_v, Dg, binary_feature, dflag);
-    CK(cudaMemcpyAsync(hflag, dflag, 8, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    if (hflag[0]) return fail(MLEASE_ERR_INVALID, "feature index out of range");
-    csr_unique = hflag[1] ? 0 : 1;
-    if (lists)
-      if (int rc = build_lists(0, K, d_ci, st, t, &kc)) return rc;
-  }
-  if (int rc = ingest_labels(st, ntot, response, weight, offset, dy, dw, dofs, dflag, hflag, nullptr)) return rc;
-  init_outputs();
-  ChunkRows cr;
-  cr.y = dy; cr.w = dw; cr.o = dofs; cr.X = dX; cr.rp = d_rp; cr.ci = d_ci; cr.v = d_v; cr.csr_unique = csr_unique;
-  cr.kc = lists ? &kc : nullptr;
-  // chunk size bounded by memory
-  size_t free_b, total_b;
-  CK(cudaMemGetInfo(&free_b, &total_b));
-  free_b = keyed_budget(free_b);
+  if (!csr) { if (int rc = t.get(&dX, (size_t)max_rows * ldx, false)) return rc; }
+  if (int rc = ring.open()) return rc;
   std::vector<long long> bounds{0};
-  size_t pos = 0;
-  while (pos < todo.size()) {
-    size_t bytes = 0;
-    size_t end = pos;
-    while (end < todo.size() && end - pos < 16384) {
-      const size_t need = state_bytes(krs[todo[end] + 1] - krs[todo[end]], kdt[todo[end]]);
-      if (end > pos && bytes + need > free_b / 2) break;
-      bytes += need;
-      end++;
+  for (int c = 0; c < nr; c++) {
+    const void* v[6];
+    if (int rc = ring.view(c, v)) return rc;
+    const int k0 = (int)ranges[c], k1 = (int)ranges[c + 1];
+    const long long n = row_at[c + 1] - row_at[c];
+    DevMem rt;   // the range's device copies of host input and its column lists
+    KeyCols kc;
+    ChunkRows cr;
+    cr.row0 = row_at[c]; cr.y = dy; cr.w = dw; cr.o = dofs; cr.X = dX;
+    // the range's checks, before any kernel reads its rows
+    if (csr) {
+      const long long z0 = nnz_at[c], nz = nnz_at[c + 1] - z0;
+      if (int rc = to_device(rt, (const long long*)v[RP], (size_t)n + 1, &cr.rp, st)) return rc;
+      if (int rc = to_device(rt, (const int*)v[CI], (size_t)nz, &cr.ci, st)) return rc;
+      cr.v = (float*)v[V];   // a ring slot: the range's own copy
+      if (!ring.staged()) {  // the caller's values are copied even when they live on the device: binary.feature rewrites them
+        if (int rc = rt.get(&cr.v, (size_t)nz, false)) return rc;
+        CK(cudaMemcpyAsync(cr.v, vals, (size_t)nz * 4, cudaMemcpyDefault, st));
+      }
+      if (z0) rebase_rowptr(st, n, cr.rp, z0, (long long*)cr.rp);   // in place: a range after the first is in a ring slot
+      CK(cudaMemsetAsync(dflag, 0, 8, st));
+      check_csr(st, n, nz, cr.rp, cr.ci, cr.v, Dg, binary_feature, dflag);
+      CK(cudaMemcpyAsync(hflag, dflag, 8, cudaMemcpyDeviceToHost, st));
+      CK(cudaStreamSynchronize(st));
+      if (hflag[0]) return fail(MLEASE_ERR_INVALID, "feature index out of range");
+      cr.csr_unique = hflag[1] ? 0 : 1;
+      if (lists) {
+        if (int rc = build_lists(k0, k1, cr.ci, st, rt, &kc)) return rc;
+        cr.kc = &kc; cr.kbase = k0;
+      }
+    } else {
+      if (int rc = upload_dense_rows(dX, ldx, (const float*)v[V], ldx_in, n, Dg, has_intercept ? 1 : 0, st)) return rc;
     }
-    if (int rc = solve_chunk(todo.data() + pos, (int)(end - pos), cr, dflag, hflag)) return rc;
-    bounds.push_back(end < todo.size() ? todo[end] : K);
-    pos = end;
+    if (int rc = ingest_labels(st, n, (const int32_t*)v[Y], (const float*)v[W], (const float*)v[O], dy, dw, dofs, dflag, hflag, nullptr))
+      return rc;
+    if (c == 0) init_outputs();   // the first range's rows passed their checks
+    if (int rc = ring.start(c + 1)) return rc;
+    // the range's fitted keys in chunks: a streamed range is one chunk, a resident call's chunks fit the memory left after its upload
+    std::vector<int> keys;
+    for (int k = k0; k < k1; k++) if (solves(k)) keys.push_back(k);
+    size_t cap = SIZE_MAX;
+    if (!ring.staged()) { CK(cudaMemGetInfo(&free_b, &total_b)); cap = keyed_budget(free_b) / 2; }
+    const std::vector<long long> chunks = plan_ranges((long long)keys.size(), cap, 16384, [&](long long i) {
+      return state_bytes(krs[keys[i] + 1] - krs[keys[i]], kdt[keys[i]]);
+    }, nullptr);
+    for (size_t j = 1; j < chunks.size(); j++) {
+      if (int rc = solve_chunk(keys.data() + chunks[j - 1], (int)(chunks[j] - chunks[j - 1]), cr, dflag, hflag)) return rc;
+      bounds.push_back(chunks[j] < (long long)keys.size() ? keys[chunks[j]] : k1);
+    }
+    if (bounds.back() != k1) bounds.push_back(k1);
+    if (int rc = ring.done(c)) return rc;
   }
-  if (bounds.back() != K) bounds.push_back(K);
-  return finish(bounds, false, 0, 0);
+  keyed_record(bounds, ring.staged(), ring.stage_ms, ring.wait_ms);
+  if (cnt.not_converged) return fail(MLEASE_ERR_NUMERIC, "Model fitting error! (" + std::to_string(cnt.not_converged) + " fits did not converge)");
+  return 0;
 }
 
 // the problems keys[0, nprob) over the rows of cr, every prior, into out_model / out_var: one batch per width, narrowest first
@@ -376,156 +374,6 @@ int KeyedFit::solve_batch(const int* keys, int nprob, int w, const ChunkRows& cr
     }
   }
   return 0;
-}
-
-int KeyedFit::streamed(size_t budget) {
-  // the plan: contiguous key ranges whose rows (staged copy + the solver's layout, the column lists) and fitted keys' state (at the
-  // bound of their widths) fit a quarter of the budget
-  auto row_bytes = [&](int k) -> size_t {
-    const size_t n = (size_t)(krs[k + 1] - krs[k]);
-    size_t b = n * (12 + 9);
-    b += csr ? n * 16 + (size_t)(key_nnz0[k + 1] - key_nnz0[k]) * 8 + list_bytes(k, k + 1) : n * ((size_t)ldx_in + ldx) * 4;
-    return b;
-  };
-  const size_t cap = budget / 4;
-  std::vector<long long> bounds{0};
-  long long max_rows = 0, max_nnz = 0;
-  for (int k = 0; k < K;) {
-    int e = k, fitted = 0;
-    size_t bytes = 0;
-    while (e < K) {
-      const size_t need = row_bytes(e) + (solves(e) ? state_bytes(krs[e + 1] - krs[e], bound_dt(e)) : 0);
-      if (e > k && (bytes + need > cap || (solves(e) && fitted >= 16384))) break;
-      bytes += need; fitted += solves(e) ? 1 : 0; e++;
-    }
-    max_rows = std::max(max_rows, krs[e] - krs[k]);
-    if (csr) max_nnz = std::max(max_nnz, key_nnz0[e] - key_nnz0[k]);
-    bounds.push_back(e);
-    k = e;
-  }
-  const int nch = (int)bounds.size() - 1;
-  // the ring: two staged ranges on the device (+ pinned host copies of pageable input), one solver layout
-  struct Src { const void* p; size_t esize; size_t per_row; bool per_nnz; bool dma; void* dev[2]; void* host[2]; };
-  std::vector<Src> srcs;
-  auto add = [&](const void* p, size_t esize, size_t per_row, bool per_nnz) {
-    if (p) srcs.push_back(Src{p, esize, per_row, per_nnz, is_dma_ptr(p), {nullptr, nullptr}, {nullptr, nullptr}});
-  };
-  if (csr) { add(rowptr, 8, 1, false); add(colidx, 4, 0, true); add(vals, 4, 0, true); }
-  else add(vals, 4, (size_t)ldx_in, false);
-  add(response, 4, 1, false); add(weight, 4, 1, false); add(offset, 4, 1, false);
-  DevMem t;
-  PinnedMem pinned;
-  for (auto& s : srcs) {
-    const size_t count = s.per_nnz ? (size_t)max_nnz : (size_t)max_rows * s.per_row + (s.esize == 8 ? 1 : 0);
-    for (int b = 0; b < 2; b++) {
-      char* d; if (int rc = t.get(&d, count * s.esize, false)) return rc;
-      s.dev[b] = d;
-      if (!s.dma) { char* h; if (int rc = pinned.get(&h, count * s.esize, false)) return rc; s.host[b] = h; }
-    }
-  }
-  signed char* dy; float *dw, *dofs; int* dflag; int* hflag; float* dX = nullptr; long long* d_rp = nullptr;
-  if (int rc = t.get(&dy, (size_t)max_rows, false)) return rc;
-  if (int rc = t.get(&dw, (size_t)max_rows, false)) return rc;
-  if (int rc = t.get(&dofs, (size_t)max_rows, false)) return rc;
-  if (int rc = t.get(&dflag, 16, false)) return rc;
-  if (int rc = pinned.get(&hflag, 16, false)) return rc;
-  if (csr) { if (int rc = t.get(&d_rp, (size_t)max_rows + 1, false)) return rc; }
-  else { if (int rc = t.get(&dX, (size_t)max_rows * ldx, false)) return rc; }
-  struct Ring {   // the copy stream and its events, released on every return path
-    cudaStream_t cs = nullptr;
-    cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};   // slot 0 / 1 staged; [2]: what the caller queued on st before the call
-    ~Ring() { for (auto e : ev) if (e) cudaEventDestroy(e); if (cs) cudaStreamDestroy(cs); }
-  } ring;
-  CK(cudaStreamCreateWithFlags(&ring.cs, cudaStreamNonBlocking));
-  for (auto& e : ring.ev) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-  CK(cudaEventRecord(ring.ev[2], st));   // device input may be produced by work the caller queued on st
-  int device = 0;
-  CK(cudaGetDevice(&device));
-  // stage range c into ring slot c & 1, on its own host thread: it returns once the rows are on the device
-  auto stage = [&](int c) -> cudaError_t {
-    cudaError_t e = cudaSetDevice(device);
-    if (e == cudaSuccess) e = cudaStreamWaitEvent(ring.cs, ring.ev[2], 0);
-    const int b = c & 1;
-    const long long r0 = krs[bounds[c]], r1 = krs[bounds[c + 1]], n = r1 - r0;
-    for (auto& s : srcs) {
-      if (e != cudaSuccess) break;
-      size_t first, count;
-      if (s.per_nnz) { first = (size_t)key_nnz0[bounds[c]]; count = (size_t)(key_nnz0[bounds[c + 1]] - key_nnz0[bounds[c]]); }
-      else if (s.esize == 8) { first = (size_t)r0; count = (size_t)n + 1; }   // rowptr: n + 1 entries
-      else if (s.per_row > 1) { first = (size_t)r0 * s.per_row; count = n > 0 ? (size_t)(n - 1) * s.per_row + Dg : 0; }   // dense rows
-      else { first = (size_t)r0; count = (size_t)n; }
-      const char* src = (const char*)s.p + first * s.esize;
-      const size_t bytes = count * s.esize;
-      if (!bytes) continue;
-      if (s.dma) { e = cudaMemcpyAsync(s.dev[b], src, bytes, cudaMemcpyDefault, ring.cs); continue; }
-      parallel_memcpy(s.host[b], src, bytes);
-      e = cudaMemcpyAsync(s.dev[b], s.host[b], bytes, cudaMemcpyHostToDevice, ring.cs);
-    }
-    if (e == cudaSuccess) e = cudaEventRecord(ring.ev[b], ring.cs);
-    if (e == cudaSuccess) e = cudaEventSynchronize(ring.ev[b]);
-    return e;
-  };
-  // what the stager thread writes outlives it: declared before the guard that joins it on every return path
-  cudaError_t stage_err = cudaSuccess;
-  double stage_ms = 0, wait_ms = 0;
-  std::thread stager;
-  struct Join { std::thread& t; ~Join() { if (t.joinable()) t.join(); } } join{stager};
-  using clk = std::chrono::steady_clock;
-  auto start = [&](int c) -> int {
-    try {
-      stager = std::thread([&, c] {
-        const auto t0 = clk::now();
-        stage_err = stage(c);
-        stage_ms += std::chrono::duration<double, std::milli>(clk::now() - t0).count();
-      });
-    } catch (const std::exception& e) {   // no exception leaves the C ABI
-      return fail(MLEASE_ERR_CUDA, std::string("cannot start the staging thread: ") + e.what());
-    }
-    return 0;
-  };
-  init_outputs();
-  if (int rc = start(0)) return rc;
-  for (int c = 0; c < nch; c++) {
-    const auto t0 = clk::now();
-    stager.join();
-    wait_ms += std::chrono::duration<double, std::milli>(clk::now() - t0).count();
-    if (stage_err != cudaSuccess) return fail(MLEASE_ERR_CUDA, std::string("staging the rows of a key range: ") + cudaGetErrorString(stage_err));
-    const int b = c & 1;
-    const long long r0 = krs[bounds[c]], n = krs[bounds[c + 1]] - r0;
-    auto slot = [&](const void* p) -> void* { for (auto& s : srcs) if (s.p == p) return s.dev[b]; return nullptr; };
-    ChunkRows cr;
-    cr.row0 = r0; cr.y = dy; cr.w = dw; cr.o = dofs;
-    DevMem lmem;   // the range's column lists
-    KeyCols kc;
-    // the range's checks, before any kernel reads its rows
-    if (csr) {
-      const long long nnz = key_nnz0[bounds[c + 1]] - key_nnz0[bounds[c]];
-      rebase_rowptr(st, n, (const long long*)slot(rowptr), key_nnz0[bounds[c]], d_rp);
-      cr.rp = d_rp; cr.ci = (const int*)slot(colidx); cr.v = (float*)slot(vals);
-      CK(cudaMemsetAsync(dflag, 0, 8, st));
-      check_csr(st, n, nnz, cr.rp, cr.ci, cr.v, Dg, binary_feature, dflag);
-      CK(cudaMemcpyAsync(hflag, dflag, 8, cudaMemcpyDeviceToHost, st));
-      CK(cudaStreamSynchronize(st));
-      if (hflag[0]) return fail(MLEASE_ERR_INVALID, "feature index out of range");
-      cr.csr_unique = hflag[1] ? 0 : 1;
-      if (lists) {
-        if (int rc = build_lists((int)bounds[c], (int)bounds[c + 1], cr.ci, st, lmem, &kc)) return rc;
-        cr.kc = &kc; cr.kbase = (int)bounds[c];
-      }
-    } else {
-      if (int rc = upload_dense_rows(dX, ldx, (const float*)slot(vals), ldx_in, n, Dg, has_intercept ? 1 : 0, st)) return rc;
-      cr.X = dX;
-    }
-    if (int rc = ingest_labels(st, n, (const int32_t*)slot(response), (const float*)slot(weight), (const float*)slot(offset), dy, dw, dofs,
-                               dflag, hflag, nullptr))
-      return rc;
-    if (c + 1 < nch) { if (int rc = start(c + 1)) return rc; }
-    std::vector<int> keys;
-    for (long long k = bounds[c]; k < bounds[c + 1]; k++) if (solves((int)k)) keys.push_back((int)k);
-    if (!keys.empty())
-      if (int rc = solve_chunk(keys.data(), (int)keys.size(), cr, dflag, hflag)) return rc;
-  }
-  return finish(bounds, true, stage_ms, wait_ms);
 }
 
 // callers run keyed_fit_check first

@@ -10,7 +10,7 @@ ROOT = os.path.dirname(PKG)            # ml-ease_b200/
 CSRC = os.path.join(ROOT, "csrc")
 LIBDIR = os.path.join(ROOT, "lib")
 SO = os.path.join(LIBDIR, "libmlease_b200.so")
-SOURCES = ["session.cu", "batch.cu", "ingest.cu", "keyed_fit.cu", "keyed_cols.cu", "test_hooks.cu", "k1_score_grad.cu", "k1_csr_fused.cu", "newton.cu", "k2_gram.cu", "k3_cholesky.cu", "k4_consensus.cu", "k5_score.cu", "k6_postvar.cu", "comm.cu"]
+SOURCES = ["session.cu", "batch.cu", "ingest.cu", "keyed_fit.cu", "keyed_cols.cu", "key_ranges.cu", "test_hooks.cu", "k1_score_grad.cu", "k1_csr_fused.cu", "newton.cu", "k2_gram.cu", "k3_cholesky.cu", "k4_consensus.cu", "k5_score.cu", "k6_postvar.cu", "comm.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-Xptxas", "-v"]
