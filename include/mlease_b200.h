@@ -239,8 +239,9 @@ int mlease_posterior_variance(mlease_session* s, int32_t partition_id, const dou
  *         round_up(Dk + 1, 32) < round_up(num_features + 1, 32) is fitted over those Dk columns and the intercept only, and its
  *         model is scattered back to the global columns.  Device memory then scales with each key's own width, not with
  *         num_features (a 200 000-feature dictionary whose keys list a few hundred features each fits easily); the dense host
- *         output, num_lambdas * num_keys * (num_features+1) doubles, is the limit that remains.  Which width a key runs at depends
- *         on its own rows alone.
+ *         output, num_lambdas * num_keys * (num_features+1) doubles, is what remains proportional to the dictionary:
+ *         mlease_naive_train_sparse below returns each key's listed columns only.  Which width a key runs at depends on its own
+ *         rows alone.
  *   dense (rowptr == NULL): vals = X row-major [nrows x num_features], leading dimension ldx; every feature is present.
  * priorVar = 1/lambda, 1/lambda_map[k] for listed features (lambda_map [num_features] or NULL, entries > 0), intercept variance
  * 100000 unless penalize_intercept (:333-343), prior.mean, has.intercept, data.size.threshold (skipped keys -> skipped[k]=1,
@@ -277,13 +278,46 @@ int mlease_naive_train_dense(int32_t device, void* stream, int32_t num_keys, int
  * 1 / (1/priorVar[j] + sum_i weight_i p_i (1-p_i) x_ij^2) at the fit (llf/LibLinear.java:328-333), 1/q = priorVar[j] for an absent
  * feature.  Each key is solved in its own column space when that is narrower, as mlease_naive_train's CSR keys are: device memory
  * scales with each key's own width, and the dense host outputs (IL * DL * num_keys * (num_features+1) doubles, twice with
- * compute_var) are the limit that remains.  All inputs host-or-device; intercept_prior_mean, out_model and out_var host.  With IL = DL = 1, intercept_lambdas[0] =
+ * compute_var) are what remains proportional to the dictionary (mlease_item_model_train_sparse below avoids them).  All inputs
+ * host-or-device; intercept_prior_mean, out_model and out_var host.  With IL = DL = 1, intercept_lambdas[0] =
  * default_lambdas[0] and zero means the models are bitwise those of mlease_naive_train(prior_mean 0, penalize_intercept 1). */
 int mlease_item_model_train(int32_t device, void* stream, int32_t num_keys, int32_t num_features, const int64_t* key_rowstart,
                             const int64_t* rowptr, const int32_t* colidx, const float* vals, const int32_t* response, const float* weight,
                             const float* offset, const double* intercept_prior_mean, int32_t num_intercept_lambdas,
                             const float* intercept_lambdas, int32_t num_default_lambdas, const float* default_lambdas,
                             const float* lambda_map, int32_t binary_feature, int32_t compute_var, double* out_model, double* out_var);
+
+/* Sparse outputs of the two keyed CSR fits above: the same fits (same plan, kernels and priors), each key's model returned as the
+ * columns its rows list instead of a num_features + 1 row.  Inputs, checks, errors, streaming, budgets and several-device use are
+ * those of mlease_naive_train (CSR only: rowptr and colidx required) and mlease_item_model_train.
+ *   lists:    key k's list is entries [out_key_ptr[k], out_key_ptr[k+1]) of out_col (out_key_ptr [num_keys+1], out_key_ptr[0] = 0):
+ *             the distinct columns its rows list, ascending, then the intercept as column num_features (always for ItemModelTrain,
+ *             for NaiveTrain when has_intercept), so strictly ascending as mlease_score_keyed requires.  A key that is not fitted
+ *             (skipped by data_size_threshold, also flagged in skipped; or without rows) has an empty list.  A key's list is the
+ *             same for every prior.
+ *   values:   prior p's value of entry e is out_model[p * capacity + e] (out_var likewise with compute_var), priors in the dense
+ *             calls' order (lambda; a * num_default_lambdas + b).  Each value is the one the dense call computes at that column
+ *             (the same fit; for a one-row key in its own column space, bit for bit; otherwise within the run-to-run spread the
+ *             dense call has from call to call); the variance is 1 / hessianDiagonal in fp64.  Unlisted features are not reported: their
+ *             coefficient is 0 and their variance 1/q.
+ *   capacity: the entries out_col holds (and each prior's stride in out_model / out_var).  Checked before any row is read against
+ *             the bound sum over fitted keys of min(stored entries of the key, num_features) + 1 for the intercept (read from
+ *             rowptr at the key boundaries); a smaller capacity is MLEASE_ERR_INVALID, the message giving the bound.  The lists hold
+ *             out_key_ptr[num_keys] <= bound entries; nothing past them is written.
+ * Host and device memory are proportional to the data (the lists, one chunk of keys at a time on the device), never to
+ * num_keys * num_features.  out_key_ptr, out_col, out_model, out_var and skipped are host memory. */
+int mlease_naive_train_sparse(int32_t device, void* stream, int32_t num_keys, int32_t num_features, const int64_t* key_rowstart,
+                              const int64_t* rowptr, const int32_t* colidx, const float* vals, const int32_t* response,
+                              const float* weight, const float* offset, int32_t num_lambdas, const float* lambdas,
+                              const float* lambda_map, float prior_mean, int32_t penalize_intercept, int32_t has_intercept,
+                              int32_t data_size_threshold, int32_t binary_feature,
+                              int64_t capacity, int64_t* out_key_ptr, int32_t* out_col, double* out_model, int32_t* skipped);
+int mlease_item_model_train_sparse(int32_t device, void* stream, int32_t num_keys, int32_t num_features, const int64_t* key_rowstart,
+                                   const int64_t* rowptr, const int32_t* colidx, const float* vals, const int32_t* response,
+                                   const float* weight, const float* offset, const double* intercept_prior_mean,
+                                   int32_t num_intercept_lambdas, const float* intercept_lambdas, int32_t num_default_lambdas,
+                                   const float* default_lambdas, const float* lambda_map, int32_t binary_feature, int32_t compute_var,
+                                   int64_t capacity, int64_t* out_key_ptr, int32_t* out_col, double* out_model, double* out_var);
 
 /* ---------------------------------------------------------------------------------------
  * RegressionTest / RegressionTestLoglik.

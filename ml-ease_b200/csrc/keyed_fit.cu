@@ -1,5 +1,7 @@
 // keyed_fit.cu -- K independent fits per prior over one upload of the rows: RegressionNaiveTrain (mlease_naive_train,
-// mlease_naive_train_dense) and ItemModelTrain (mlease_item_model_train).
+// mlease_naive_train_dense) and ItemModelTrain (mlease_item_model_train), and both with sparse outputs (mlease_*_train_sparse).
+#include <cub/block/block_scan.cuh>
+
 #include <algorithm>
 #include <cstring>
 #include <string>
@@ -49,8 +51,80 @@ __global__ void local_init_kernel(const Problem* probs, const double* m, const d
     else { pb.q[k] = 1.0; pb.m[k] = 0.0; }
   }
 }
+// mask[b][c] = 1 for every column the rows rows[2b] .. rows[2b + 1] of rp / ci list (+ the intercept, column Dt - 1); count[b] = the
+// mask's ones.  The keys of a sparse chunk that have no column list (sparse_gather_kernel compacts the same mask rows).
+__global__ void span_present_kernel(const long long* rp, const int* ci, const long long* rows, int Dt, int has_bias, unsigned char* mask,
+                                    int* count) {
+  unsigned char* mk = mask + (size_t)blockIdx.x * Dt;
+  const long long j0 = rp[rows[2 * blockIdx.x]], j1 = rp[rows[2 * blockIdx.x + 1]];
+  for (long long j = j0 + threadIdx.x; j < j1; j += blockDim.x) mk[ci[j]] = 1;
+  if (threadIdx.x == 0 && has_bias) mk[Dt - 1] = 1;
+  __syncthreads();
+  __shared__ int total;
+  if (threadIdx.x == 0) total = 0;
+  __syncthreads();
+  int c = 0;
+  for (int k = threadIdx.x; k < Dt; k += blockDim.x) c += mk[k];
+  atomicAdd(&total, c);
+  __syncthreads();
+  if (threadIdx.x == 0) count[blockIdx.x] = total;
+}
+// Where problem b of a batch writes its list in a chunk's slab: entries dst .. of out.  dk >= 0: the list is cols[s0 .. s0 + dk)
+// (then the intercept); dk < 0: no list, the ones of mask row mrow in column order (the intercept's included)
+struct GatherJob { long long dst, s0; int dk, mrow; };
+constexpr int GATHER_THREADS = 256;
+// One problem per block: beta (hdiag: 1 / g_t, IEEE fp64 like the host's 1.0 / x) at the problem's listed columns into out, and the
+// global column ids into out_col (NULL: already written).  A local problem (local = 1) holds its list's columns at 0 .. dk - 1 and
+// the intercept at Dt - 1; a global-width one holds global column c at c.
+__global__ void sparse_gather_kernel(const Problem* probs, const GatherJob* jobs, const int* cols, const unsigned char* mask, int local,
+                                     int Dg, int has_bias, int hdiag, double* out, int* out_col) {
+  using Scan = cub::BlockScan<int, GATHER_THREADS>;
+  __shared__ typename Scan::TempStorage scan;
+  __shared__ int carry;
+  const Problem& pb = probs[blockIdx.x];
+  const GatherJob jb = jobs[blockIdx.x];
+  const double* v = hdiag ? pb.g_t : pb.beta;
+  auto put = [&](long long e, int src, int col) {
+    out[jb.dst + e] = hdiag ? __ddiv_rn(1.0, v[src]) : v[src];
+    if (out_col) out_col[jb.dst + e] = col;
+  };
+  if (jb.dk >= 0) {
+    const int* c = cols + jb.s0;
+    for (int i = threadIdx.x; i < jb.dk; i += blockDim.x) put(i, local ? i : c[i], c[i]);
+    if (threadIdx.x == 0 && has_bias) put(jb.dk, pb.Dt - 1, Dg);
+    return;
+  }
+  const unsigned char* mk = mask + (size_t)jb.mrow * pb.Dt;
+  if (threadIdx.x == 0) carry = 0;
+  __syncthreads();
+  for (int t0 = 0; t0 < pb.Dt; t0 += GATHER_THREADS) {
+    const int k = t0 + threadIdx.x;
+    const int f = k < pb.Dt ? mk[k] : 0;
+    int pos, tile;
+    Scan(scan).ExclusiveSum(f, pos, tile);
+    if (f) put(carry + pos, k, k);
+    __syncthreads();
+    if (threadIdx.x == 0) carry += tile;
+    __syncthreads();
+  }
+}
+
 // One prior of a keyed fit: precision q and mean m of every coefficient ([ldx], the intercept at Dg, 1 / 0 on the padding)
 struct KeyedPrior { std::vector<double> q, m; };
+
+// The sparse output of mlease_*_train_sparse: key k's list is entries key_ptr[k] .. key_ptr[k + 1] of col, prior p's values at
+// model[p * cap + e] (and var).  NULL in KeyedFit: the dense [prior][K][Dt] arrays.
+struct SparseOut { int64_t cap; int64_t* key_ptr; int32_t* col; };
+// A chunk's sparse results on the device: the lists of its fitted keys, contiguous in key order, [prior][n] values and n column ids.
+// off / len (by key - k0): a key's entries in the slab; mrow: its row of mask (-1: it has a column list)
+struct Slab {
+  int k0 = 0;
+  long long n = 0;
+  double* model = nullptr; double* var = nullptr; int* col = nullptr;
+  unsigned char* mask = nullptr;
+  std::vector<long long> off, len;
+  std::vector<int> mrow;
+};
 
 // K independent fits per prior, processed in lockstep chunks of keys: the rows are uploaded ONCE and serve every prior (the reference
 // fans each record out once per reducer through the shuffle, jobs/RegressionNaiveTrain.java:228-241, jobs/ItemModelTrain.java:256-258).
@@ -88,19 +162,21 @@ struct ChunkRows {
 // space of Dt_k = round_up(Dk + 1, 32) columns: its Dk listed features in ascending order, padding (q = 1, m = 0, no row touches it,
 // so beta stays 0 there) and the intercept at Dt_k - 1.  Every other key runs at the global width Dt = Dg + 1.  The choice and the
 // shape depend on the key's own rows alone, never on which keys share its call, chunk or streamed range; each chunk runs one batch
-// per width.  Outputs are scattered back to the global columns: a feature the key does not list keeps 0 in the model and 1/q in the
-// variance.
+// per width.  Dense sink: outputs are scattered back to the global columns, a feature the key does not list keeping 0 in the model
+// and 1/q in the variance.  Sparse sink (sp): each chunk's lists are gathered on the device into a slab and copied out once per prior.
 struct KeyedFit {
   int num_sms; cudaStream_t st; int32_t K, Dg; const int64_t* key_rowstart; const int64_t* rowptr; const int32_t* colidx; const float* vals;
   int64_t ldx_in; const int32_t* response; const float* weight; const float* offset; bool has_intercept; int32_t data_size_threshold;
   int32_t binary_feature; const std::vector<KeyedPrior>& priors; const double* intercept_mean; double* out_model; double* out_var;
   int32_t* skipped;
+  const SparseOut* sp;                    // the output sink: NULL = dense out_model / out_var; else the lists (out_model / out_var their values)
   bool csr = false;
   int L = 0, Dt = 0, ldx = 0, Dp = 0, ldh = 0;
   std::vector<long long> krs, key_nnz0;   // key_nnz0: CSR rowptr at the key boundaries
   std::vector<int> todo;                  // the keys that are fitted
   bool lists = false;                     // CSR with Dt > 32: a key may be narrower than Dt, so every range builds its column lists
   std::vector<int> kdt;                   // the width (Dt or Dt_k) of each key's problems, known once its range's lists exist
+  int sp_key = 0;                         // sparse: key_ptr[0 .. sp_key] are written
   Counters cnt;
 
   bool solves(int k) const { const long long nk = krs[k + 1] - krs[k]; return !(nk < data_size_threshold || nk <= 0); }   // (:379-382)
@@ -112,6 +188,10 @@ struct KeyedFit {
     const size_t x = (size_t)round_up(w, 4), p = (size_t)round_up((int)x, 128), h = (size_t)round_up(w, 32);
     return (size_t)n * p * 2 + p * p * 4 + 3 * h * h * 8 + 2 * h * 32 * 8 + 64 * x + (out_var ? (size_t)n * 8 : 0);
   }
+  // entries of a fitted CSR key's list at most: its stored entries or the dictionary, whichever is smaller, and the intercept
+  long long list_bound(int k) const { return std::min<long long>(key_nnz0[k + 1] - key_nnz0[k], Dg) + (has_intercept ? 1 : 0); }
+  // device bytes of a fitted key's entries in its chunk's slab (values of every prior, variances, column ids); 0 for the dense sink
+  size_t slab_bytes(int k) const { return sp ? (size_t)list_bound(k) * ((size_t)L * 8 * (out_var ? 2 : 1) + 4) : 0; }
   // the lists of keys [k0, k1) over the range's colidx ci (entries from key_nnz0[k0] on), and the widths they give
   int build_lists(int k0, int k1, const int* ci, cudaStream_t s, DevMem& mem, KeyCols* kc) {
     std::vector<long long> koff(key_nnz0.begin() + k0, key_nnz0.begin() + k1 + 1);
@@ -129,16 +209,23 @@ struct KeyedFit {
     return key_columns_bytes(key_nnz0[k1] - key_nnz0[k0], mx, k1 - k0);
   }
   void init_outputs() {
-    for (size_t e = 0; e < (size_t)L * K * Dt; e++) out_model[e] = 0.0;
     if (skipped) for (int k = 0; k < K; k++) skipped[k] = solves(k) ? 0 : 1;   // "data size < threshold": no model
+    if (sp) { sp->key_ptr[0] = 0; return; }   // a list is written with its chunk
+    for (size_t e = 0; e < (size_t)L * K * Dt; e++) out_model[e] = 0.0;
     if (out_var)   // a key without rows has no fit: every variance is the prior's
       for (int l = 0; l < L; l++)
         for (int k = 0; k < K; k++)
           for (int j = 0; j < Dt; j++) out_var[((size_t)l * K + k) * Dt + j] = 1.0 / priors[l].q[j];
   }
+  // sparse: empty lists for keys sp_key .. k1 - 1 (the keys before k1 that no chunk fitted)
+  void close_lists(int k1) {
+    for (; sp_key < k1; sp_key++) sp->key_ptr[sp_key + 1] = sp->key_ptr[sp_key];
+  }
   int run();
   int solve_chunk(const int* keys, int nprob, const ChunkRows& cr, int* dflag, int* hflag);
-  int solve_batch(const int* keys, int nprob, int width, const ChunkRows& cr, int* dflag, int* hflag);
+  int solve_batch(const int* keys, int nprob, int width, const ChunkRows& cr, int* dflag, int* hflag, Slab* sl);
+  int open_slab(const int* keys, int nprob, const ChunkRows& cr, DevMem& mem, Slab* sl);
+  int write_slab(const int* keys, int nprob, const Slab& sl);
 };
 
 int KeyedFit::run() {
@@ -161,6 +248,14 @@ int KeyedFit::run() {
     // any key may list fewer columns than the dictionary holds (the bound above only caps its width): every range builds its lists
     lists = ldh > 32 && !todo.empty();
   }
+  if (sp) {   // the lists' room, checked before any row is read
+    long long need = 0;
+    for (int k : todo) need += list_bound(k);
+    if (sp->cap < need)
+      return fail(MLEASE_ERR_INVALID, "capacity " + std::to_string(sp->cap) + " is too small: the keys' lists need up to " +
+                                          std::to_string(need) + " entries (the sum over fitted keys of min(stored entries, num_features)" +
+                                          (has_intercept ? " + 1)" : ")"));
+  }
   // resident (one range) when the whole upload (rows, labels, key boundaries, the temporaries of host input, the column lists) and
   // the first chunk's state fit the budget
   size_t free_b, total_b;
@@ -171,7 +266,7 @@ int KeyedFit::run() {
   size_t up = (size_t)ntot * 9 + (is_device_ptr(response) ? 0 : (size_t)ntot * 12);
   if (csr) up += (size_t)nnz * 4 + (host_rows ? (size_t)nnz * 4 + (size_t)(ntot + 1) * 8 : 0) + (size_t)(K + 1) * 16 + list_bytes(0, K);
   else up += (size_t)ntot * ldx * 4 + (host_rows ? (size_t)256 << 20 : 0);
-  const size_t first = todo.empty() ? 0 : state_bytes(krs[todo[0] + 1] - krs[todo[0]], bound_dt(todo[0]));
+  const size_t first = todo.empty() ? 0 : state_bytes(krs[todo[0] + 1] - krs[todo[0]], bound_dt(todo[0])) + slab_bytes(todo[0]);
   const bool streamed = up + first > budget;
   std::vector<long long> ranges{0, K};
   if (streamed) {
@@ -181,7 +276,7 @@ int KeyedFit::run() {
       const size_t n = (size_t)(krs[k + 1] - krs[k]);
       size_t b = n * (12 + 9);
       b += csr ? n * 16 + (size_t)(key_nnz0[k + 1] - key_nnz0[k]) * 8 + list_bytes(k, k + 1) : n * ((size_t)ldx_in + ldx) * 4;
-      return b + (solves(k) ? state_bytes(n, bound_dt(k)) : 0);
+      return b + (solves(k) ? state_bytes(n, bound_dt(k)) + slab_bytes((int)k) : 0);
     }, [&](long long k) { return solves(k); });
   }
   const int nr = (int)ranges.size() - 1;
@@ -247,7 +342,7 @@ int KeyedFit::run() {
     size_t cap = SIZE_MAX;
     if (!ring.staged()) { CK(cudaMemGetInfo(&free_b, &total_b)); cap = keyed_budget(free_b) / 2; }
     const std::vector<long long> chunks = plan_ranges((long long)keys.size(), cap, 16384, [&](long long i) {
-      return state_bytes(krs[keys[i] + 1] - krs[keys[i]], kdt[keys[i]]);
+      return state_bytes(krs[keys[i] + 1] - krs[keys[i]], kdt[keys[i]]) + slab_bytes(keys[i]);
     }, nullptr);
     for (size_t j = 1; j < chunks.size(); j++) {
       if (int rc = solve_chunk(keys.data() + chunks[j - 1], (int)(chunks[j] - chunks[j - 1]), cr, dflag, hflag)) return rc;
@@ -256,6 +351,7 @@ int KeyedFit::run() {
     if (bounds.back() != k1) bounds.push_back(k1);
     if (int rc = ring.done(c)) return rc;
   }
+  if (sp) close_lists(K);
   keyed_record(bounds, ring.staged(), ring.stage_ms, ring.wait_ms);
   if (cnt.not_converged) return fail(MLEASE_ERR_NUMERIC, "Model fitting error! (" + std::to_string(cnt.not_converged) + " fits did not converge)");
   return 0;
@@ -267,17 +363,73 @@ int KeyedFit::solve_chunk(const int* keys, int nprob, const ChunkRows& cr, int* 
   for (int b = 0; b < nprob; b++) widths.push_back(kdt[keys[b]]);
   std::sort(widths.begin(), widths.end());
   widths.erase(std::unique(widths.begin(), widths.end()), widths.end());
+  DevMem sm;   // the sparse sink's slab
+  Slab slab;
+  if (sp) { if (int rc = open_slab(keys, nprob, cr, sm, &slab)) return rc; }
   std::vector<int> group;
   for (int w : widths) {
     group.clear();
     for (int b = 0; b < nprob; b++) if (kdt[keys[b]] == w) group.push_back(keys[b]);
-    if (int rc = solve_batch(group.data(), (int)group.size(), w, cr, dflag, hflag)) return rc;
+    if (int rc = solve_batch(group.data(), (int)group.size(), w, cr, dflag, hflag, sp ? &slab : nullptr)) return rc;
   }
+  return sp ? write_slab(keys, nprob, slab) : 0;
+}
+
+// The slab of the chunk keys[0, nprob) (ascending, fitted): each key's list length (from its column list, or for a key without one
+// from the presence mask of its rows, read back here), its offset, and the device arrays
+int KeyedFit::open_slab(const int* keys, int nprob, const ChunkRows& cr, DevMem& mem, Slab* sl) {
+  const int k0 = keys[0], nk = keys[nprob - 1] - k0 + 1;
+  sl->k0 = k0;
+  sl->off.assign(nk, 0); sl->len.assign(nk, 0); sl->mrow.assign(nk, -1);
+  std::vector<long long> rows;   // range-local row bounds of the keys without a list
+  for (int b = 0; b < nprob; b++) {
+    const int k = keys[b];
+    if (cr.kc && cr.kc->listed[k - cr.kbase])
+      sl->len[k - k0] = cr.kc->start[k - cr.kbase + 1] - cr.kc->start[k - cr.kbase] + (has_intercept ? 1 : 0);
+    else {
+      sl->mrow[k - k0] = (int)(rows.size() / 2);
+      rows.push_back(krs[k] - cr.row0); rows.push_back(krs[k + 1] - cr.row0);
+    }
+  }
+  const int nu = (int)rows.size() / 2;
+  if (nu) {
+    long long* drows; int* dcount;
+    if (int rc = mem.get(&sl->mask, (size_t)nu * Dt, false)) return rc;
+    if (int rc = mem.get(&drows, rows.size(), false)) return rc;
+    if (int rc = mem.get(&dcount, (size_t)nu, false)) return rc;
+    CK(cudaMemsetAsync(sl->mask, 0, (size_t)nu * Dt, st));
+    CK(cudaMemcpyAsync(drows, rows.data(), rows.size() * 8, cudaMemcpyHostToDevice, st));
+    span_present_kernel<<<nu, 256, 0, st>>>(cr.rp, cr.ci, drows, Dt, has_intercept ? 1 : 0, sl->mask, dcount);
+    CK(cudaGetLastError());
+    std::vector<int> count(nu);
+    CK(cudaMemcpyAsync(count.data(), dcount, (size_t)nu * 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    for (int i = 0; i < nk; i++) if (sl->mrow[i] >= 0) sl->len[i] = count[sl->mrow[i]];
+  }
+  for (int i = 0; i < nk; i++) { sl->off[i] = sl->n; sl->n += sl->len[i]; }
+  if (int rc = mem.get(&sl->model, (size_t)L * sl->n, false)) return rc;
+  if (out_var) { if (int rc = mem.get(&sl->var, (size_t)L * sl->n, false)) return rc; }
+  return mem.get(&sl->col, (size_t)sl->n, false);
+}
+
+// the chunk's slab into the caller's lists: entries key_ptr[keys[0]] .. of every prior, and key_ptr up to the chunk's last key
+int KeyedFit::write_slab(const int* keys, int nprob, const Slab& sl) {
+  close_lists(keys[0]);
+  const long long e0 = sp->key_ptr[keys[0]];
+  for (int l = 0; l < L; l++) {
+    CK(cudaMemcpyAsync(out_model + l * sp->cap + e0, sl.model + l * sl.n, (size_t)sl.n * 8, cudaMemcpyDeviceToHost, st));
+    if (out_var) CK(cudaMemcpyAsync(out_var + l * sp->cap + e0, sl.var + l * sl.n, (size_t)sl.n * 8, cudaMemcpyDeviceToHost, st));
+  }
+  CK(cudaMemcpyAsync(sp->col + e0, sl.col, (size_t)sl.n * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  for (int k = keys[0]; k <= keys[nprob - 1]; k++) sp->key_ptr[k + 1] = sp->key_ptr[k] + sl.len[k - sl.k0];
+  sp_key = keys[nprob - 1] + 1;
   return 0;
 }
 
-// the problems keys[0, nprob) of width w: Dt (today's global-width problems), or the keys' own column spaces (w < Dt)
-int KeyedFit::solve_batch(const int* keys, int nprob, int w, const ChunkRows& cr, int* dflag, int* hflag) {
+// the problems keys[0, nprob) of width w: Dt (today's global-width problems), or the keys' own column spaces (w < Dt); results into
+// the dense outputs, or with sl into the chunk's slab
+int KeyedFit::solve_batch(const int* keys, int nprob, int w, const ChunkRows& cr, int* dflag, int* hflag, Slab* sl) {
   const bool local = w != Dt;
   Batch B;
   B.nprob = nprob; B.Dt = w; B.ldx = round_up(w, 4); B.csr = csr; B.has_bias = has_intercept ? 1 : 0;
@@ -308,10 +460,25 @@ int KeyedFit::solve_batch(const int* keys, int nprob, int w, const ChunkRows& cr
   }
   if (int rc = batch_alloc(B, num_sms, 0)) return rc;
   DevMem ct;   // the batch's temporaries: freed with it, before the next batch_alloc
-  double *dm, *dq, *dout, *dim = nullptr, *dvec = nullptr; long long *drs = nullptr, *dspan = nullptr; unsigned char* dmask = nullptr;
+  double *dm, *dq, *dout = nullptr, *dim = nullptr, *dvec = nullptr; long long *drs = nullptr, *dspan = nullptr; unsigned char* dmask = nullptr;
+  GatherJob* djobs = nullptr;
   if (int rc = ct.get(&dm, (size_t)ldx, false)) return rc;
   if (int rc = ct.get(&dq, (size_t)ldx, false)) return rc;
-  if (int rc = ct.get(&dout, (size_t)B.nprob * w, false)) return rc;
+  if (sl) {
+    // each problem's list: its column list (local, or a global-width key that has one), else its row of the slab's mask
+    std::vector<GatherJob> jobs(B.nprob);
+    for (int b = 0; b < B.nprob; b++) {
+      const int k = keys[b];
+      GatherJob& j = jobs[b];
+      j.dst = sl->off[k - sl->k0]; j.mrow = sl->mrow[k - sl->k0]; j.s0 = 0; j.dk = -1;
+      if (j.mrow < 0) { j.s0 = cr.kc->start[k - cr.kbase]; j.dk = (int)(cr.kc->start[k - cr.kbase + 1] - j.s0); }
+    }
+    if (int rc = ct.get(&djobs, jobs.size(), false)) return rc;
+    CK(cudaMemcpyAsync(djobs, jobs.data(), jobs.size() * sizeof(GatherJob), cudaMemcpyHostToDevice, st));
+    CK(cudaStreamSynchronize(st));   // jobs is released here
+  } else {
+    if (int rc = ct.get(&dout, (size_t)B.nprob * w, false)) return rc;
+  }
   if (intercept_mean) {
     std::vector<double> im(B.nprob);
     for (int b = 0; b < B.nprob; b++) im[b] = intercept_mean[keys[b]];
@@ -327,9 +494,10 @@ int KeyedFit::solve_batch(const int* keys, int nprob, int w, const ChunkRows& cr
   if (local) {
     if (int rc = ct.get(&dspan, span.size(), false)) return rc;
     CK(cudaMemcpyAsync(dspan, span.data(), span.size() * 8, cudaMemcpyHostToDevice, st));
-  } else if (csr) {
+  } else if (csr && !sl) {
     // features absent from a key's rows are not part of its dataset, hence not of its model (llf/LibLinear.java:343-350; the only
     // prior mean a caller may set per key is the intercept's, which every dataset holds, so :374-383 adds nothing): mask them out
+    // (the sparse sink reports only the listed columns)
     if (int rc = ct.get(&dmask, (size_t)B.nprob * Dt, false)) return rc;
     CK(cudaMemsetAsync(dmask, 0, (size_t)B.nprob * Dt, st));
     naive_present_kernel<<<B.nprob, 256, 0, st>>>(B.d, Dt, has_intercept ? 1 : 0, dmask);
@@ -341,7 +509,7 @@ int KeyedFit::solve_batch(const int* keys, int nprob, int w, const ChunkRows& cr
     for (long long c = 0; c < dk; c++) dst[cols[c]] = inv ? 1.0 / x[c] : x[c];
     dst[Dg] = inv ? 1.0 / x[w - 1] : x[w - 1];
   };
-  std::vector<double> xs((size_t)B.nprob * w);
+  std::vector<double> xs(sl ? 0 : (size_t)B.nprob * w);
   for (int l = 0; l < L; l++) {
     CK(cudaMemcpyAsync(dm, priors[l].m.data(), ldx * 8, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(dq, priors[l].q.data(), ldx * 8, cudaMemcpyHostToDevice, st));
@@ -350,6 +518,20 @@ int KeyedFit::solve_batch(const int* keys, int nprob, int w, const ChunkRows& cr
     else naive_init_kernel<<<B.nprob, 128, 0, st>>>(B.d, dm, dq, dim);
     B.mirror.clear();                // the factors of the previous prior belong to another prior
     if (int rc = batch_xupdate(B, st, 2e-7, 100, 0, 1, hflag, dflag, cnt)) return rc;
+    if (sl) {   // the listed values straight into the slab (column ids with the first prior); no read-back until the chunk is done
+      const int* kcols = cr.kc ? cr.kc->d_cols : nullptr;
+      sparse_gather_kernel<<<B.nprob, GATHER_THREADS, 0, st>>>(B.d, djobs, kcols, sl->mask, local ? 1 : 0, Dg, B.has_bias, 0,
+                                                               sl->model + l * sl->n, l == 0 ? sl->col : nullptr);
+      CK(cudaGetLastError());
+      if (out_var) {
+        CK(postvar_rowweights(B.d, B.nprob, drs, row_start[B.nprob], B.has_bias, dvec, st, nullptr));
+        CK(postvar_diag(B.d, B.nprob, drs, row_start[B.nprob], dvec, B.has_bias, st, nullptr));
+        sparse_gather_kernel<<<B.nprob, GATHER_THREADS, 0, st>>>(B.d, djobs, kcols, sl->mask, local ? 1 : 0, Dg, B.has_bias, 1,
+                                                                 sl->var + l * sl->n, nullptr);
+        CK(cudaGetLastError());
+      }
+      continue;
+    }
     gather_beta_kernel<<<B.nprob, 128, 0, st>>>(B.d, w, dout, dmask, 0);
     CK(cudaMemcpyAsync(xs.data(), dout, xs.size() * 8, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
@@ -380,9 +562,9 @@ int KeyedFit::solve_batch(const int* keys, int nprob, int w, const ChunkRows& cr
 int keyed_fit(int num_sms, cudaStream_t st, int32_t K, int32_t Dg, const int64_t* key_rowstart, const int64_t* rowptr, const int32_t* colidx,
               const float* vals, int64_t ldx_in, const int32_t* response, const float* weight, const float* offset, bool has_intercept,
               int32_t data_size_threshold, int32_t binary_feature, const std::vector<KeyedPrior>& priors, const double* intercept_mean,
-              double* out_model, double* out_var, int32_t* skipped) {
+              double* out_model, double* out_var, int32_t* skipped, const SparseOut* sp) {
   KeyedFit f{num_sms, st, K, Dg, key_rowstart, rowptr, colidx, vals, ldx_in, response, weight, offset, has_intercept, data_size_threshold,
-             binary_feature, priors, intercept_mean, out_model, out_var, skipped};
+             binary_feature, priors, intercept_mean, out_model, out_var, skipped, sp};
   return f.run();
 }
 // host copy of a host-or-device array (NULL -> empty)
@@ -393,19 +575,15 @@ template <class T> int host_copy(const T* in, size_t count, std::vector<T>& out)
   CK(cudaMemcpy(out.data(), in, count * sizeof(T), cudaMemcpyDefault));
   return 0;
 }
-}  // namespace
-
-extern "C" {
 
 // ------------------------------------------------------------------------------------------
-// RegressionNaiveTrain: K independent fits per lambda (keyed_fit)
+// RegressionNaiveTrain: K independent fits per lambda (keyed_fit), into the dense outputs or (sp) the sparse lists
 // ------------------------------------------------------------------------------------------
-int mlease_naive_train(int32_t device, void* stream, int32_t K, int32_t Dg, const int64_t* key_rowstart, const int64_t* rowptr,
-                       const int32_t* colidx, const float* vals, int64_t ldx_in, const int32_t* response, const float* weight,
-                       const float* offset, int32_t L, const float* lambdas, const float* lambda_map, float prior_mean,
-                       int32_t penalize_intercept, int32_t has_intercept, int32_t data_size_threshold, int32_t binary_feature,
-                       double* out_model, int32_t* skipped) {
-  if (K <= 0 || Dg <= 0 || L <= 0 || !lambdas || !key_rowstart || !vals || !response || !out_model) return fail(MLEASE_ERR_INVALID, "bad argument");
+int naive_train(int32_t device, void* stream, int32_t K, int32_t Dg, const int64_t* key_rowstart, const int64_t* rowptr,
+                const int32_t* colidx, const float* vals, int64_t ldx_in, const int32_t* response, const float* weight,
+                const float* offset, int32_t L, const float* lambdas, const float* lambda_map, float prior_mean,
+                int32_t penalize_intercept, int32_t has_intercept, int32_t data_size_threshold, int32_t binary_feature,
+                double* out_model, int32_t* skipped, const SparseOut* sp) {
   int num_sms = 0;
   if (int rc = keyed_fit_check(device, Dg, rowptr, colidx, ldx_in, binary_feature, &num_sms)) return rc;
   std::vector<float> lm, lams;
@@ -428,21 +606,18 @@ int mlease_naive_train(int32_t device, void* stream, int32_t K, int32_t Dg, cons
     m[Dg] = has_intercept ? (double)prior_mean : 0.0;
   }
   return keyed_fit(num_sms, (cudaStream_t)stream, K, Dg, key_rowstart, rowptr, colidx, vals, ldx_in, response, weight, offset, has_intercept != 0,
-                   data_size_threshold, binary_feature, priors, nullptr, out_model, nullptr, skipped);
+                   data_size_threshold, binary_feature, priors, nullptr, out_model, nullptr, skipped, sp);
 }
 
 // ------------------------------------------------------------------------------------------
 // ItemModelTrain (jobs/ItemModelTrain.java:226-276): per key, one fit per (intercept lambda, default lambda) in config order, the
-// intercept's prior mean the key's own; diagonal posterior variance on request
+// intercept's prior mean the key's own; diagonal posterior variance on request.  Dense outputs, or (sp) the sparse lists
 // ------------------------------------------------------------------------------------------
-int mlease_item_model_train(int32_t device, void* stream, int32_t K, int32_t Dg, const int64_t* key_rowstart, const int64_t* rowptr,
-                            const int32_t* colidx, const float* vals, const int32_t* response, const float* weight, const float* offset,
-                            const double* intercept_prior_mean, int32_t IL, const float* intercept_lambdas, int32_t DL,
-                            const float* default_lambdas, const float* lambda_map, int32_t binary_feature, int32_t compute_var,
-                            double* out_model, double* out_var) {
-  if (K <= 0 || Dg <= 0 || IL <= 0 || DL <= 0 || !intercept_lambdas || !default_lambdas || !key_rowstart || !rowptr || !vals || !response ||
-      !intercept_prior_mean || !out_model || (compute_var && !out_var))
-    return fail(MLEASE_ERR_INVALID, "bad argument");
+int item_model_train(int32_t device, void* stream, int32_t K, int32_t Dg, const int64_t* key_rowstart, const int64_t* rowptr,
+                     const int32_t* colidx, const float* vals, const int32_t* response, const float* weight, const float* offset,
+                     const double* intercept_prior_mean, int32_t IL, const float* intercept_lambdas, int32_t DL,
+                     const float* default_lambdas, const float* lambda_map, int32_t binary_feature, int32_t compute_var,
+                     double* out_model, double* out_var, const SparseOut* sp) {
   int num_sms = 0;
   if (int rc = keyed_fit_check(device, Dg, rowptr, colidx, 0, binary_feature, &num_sms)) return rc;
   std::vector<float> lm, il, dl;
@@ -467,7 +642,58 @@ int mlease_item_model_train(int32_t device, void* stream, int32_t K, int32_t Dg,
       q[Dg] = 1.0 / (1.0 / (double)il[a]);
     }
   return keyed_fit(num_sms, (cudaStream_t)stream, K, Dg, key_rowstart, rowptr, colidx, vals, 0, response, weight, offset, true, 0, binary_feature,
-                   priors, im.data(), out_model, compute_var ? out_var : nullptr, nullptr);
+                   priors, im.data(), out_model, compute_var ? out_var : nullptr, nullptr, sp);
+}
+}  // namespace
+
+extern "C" {
+
+int mlease_naive_train(int32_t device, void* stream, int32_t K, int32_t Dg, const int64_t* key_rowstart, const int64_t* rowptr,
+                       const int32_t* colidx, const float* vals, int64_t ldx_in, const int32_t* response, const float* weight,
+                       const float* offset, int32_t L, const float* lambdas, const float* lambda_map, float prior_mean,
+                       int32_t penalize_intercept, int32_t has_intercept, int32_t data_size_threshold, int32_t binary_feature,
+                       double* out_model, int32_t* skipped) {
+  if (K <= 0 || Dg <= 0 || L <= 0 || !lambdas || !key_rowstart || !vals || !response || !out_model) return fail(MLEASE_ERR_INVALID, "bad argument");
+  return naive_train(device, stream, K, Dg, key_rowstart, rowptr, colidx, vals, ldx_in, response, weight, offset, L, lambdas, lambda_map,
+                     prior_mean, penalize_intercept, has_intercept, data_size_threshold, binary_feature, out_model, skipped, nullptr);
+}
+
+int mlease_naive_train_sparse(int32_t device, void* stream, int32_t K, int32_t Dg, const int64_t* key_rowstart, const int64_t* rowptr,
+                              const int32_t* colidx, const float* vals, const int32_t* response, const float* weight, const float* offset,
+                              int32_t L, const float* lambdas, const float* lambda_map, float prior_mean, int32_t penalize_intercept,
+                              int32_t has_intercept, int32_t data_size_threshold, int32_t binary_feature, int64_t capacity,
+                              int64_t* out_key_ptr, int32_t* out_col, double* out_model, int32_t* skipped) {
+  if (K <= 0 || Dg <= 0 || L <= 0 || !lambdas || !key_rowstart || !rowptr || !colidx || !vals || !response || capacity < 0 || !out_key_ptr ||
+      !out_col || !out_model)
+    return fail(MLEASE_ERR_INVALID, "bad argument");
+  const SparseOut sp{capacity, out_key_ptr, out_col};
+  return naive_train(device, stream, K, Dg, key_rowstart, rowptr, colidx, vals, 0, response, weight, offset, L, lambdas, lambda_map,
+                     prior_mean, penalize_intercept, has_intercept, data_size_threshold, binary_feature, out_model, skipped, &sp);
+}
+
+int mlease_item_model_train(int32_t device, void* stream, int32_t K, int32_t Dg, const int64_t* key_rowstart, const int64_t* rowptr,
+                            const int32_t* colidx, const float* vals, const int32_t* response, const float* weight, const float* offset,
+                            const double* intercept_prior_mean, int32_t IL, const float* intercept_lambdas, int32_t DL,
+                            const float* default_lambdas, const float* lambda_map, int32_t binary_feature, int32_t compute_var,
+                            double* out_model, double* out_var) {
+  if (K <= 0 || Dg <= 0 || IL <= 0 || DL <= 0 || !intercept_lambdas || !default_lambdas || !key_rowstart || !rowptr || !vals || !response ||
+      !intercept_prior_mean || !out_model || (compute_var && !out_var))
+    return fail(MLEASE_ERR_INVALID, "bad argument");
+  return item_model_train(device, stream, K, Dg, key_rowstart, rowptr, colidx, vals, response, weight, offset, intercept_prior_mean, IL,
+                          intercept_lambdas, DL, default_lambdas, lambda_map, binary_feature, compute_var, out_model, out_var, nullptr);
+}
+
+int mlease_item_model_train_sparse(int32_t device, void* stream, int32_t K, int32_t Dg, const int64_t* key_rowstart, const int64_t* rowptr,
+                                   const int32_t* colidx, const float* vals, const int32_t* response, const float* weight, const float* offset,
+                                   const double* intercept_prior_mean, int32_t IL, const float* intercept_lambdas, int32_t DL,
+                                   const float* default_lambdas, const float* lambda_map, int32_t binary_feature, int32_t compute_var,
+                                   int64_t capacity, int64_t* out_key_ptr, int32_t* out_col, double* out_model, double* out_var) {
+  if (K <= 0 || Dg <= 0 || IL <= 0 || DL <= 0 || !intercept_lambdas || !default_lambdas || !key_rowstart || !rowptr || !colidx || !vals ||
+      !response || !intercept_prior_mean || capacity < 0 || !out_key_ptr || !out_col || !out_model || (compute_var && !out_var))
+    return fail(MLEASE_ERR_INVALID, "bad argument");
+  const SparseOut sp{capacity, out_key_ptr, out_col};
+  return item_model_train(device, stream, K, Dg, key_rowstart, rowptr, colidx, vals, response, weight, offset, intercept_prior_mean, IL,
+                          intercept_lambdas, DL, default_lambdas, lambda_map, binary_feature, compute_var, out_model, out_var, &sp);
 }
 
 int mlease_naive_train_dense(int32_t device, void* stream, int32_t K, int32_t Dg, const int64_t* key_rowstart, const float* X, int64_t ldx_in,

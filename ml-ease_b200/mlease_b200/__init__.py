@@ -1,3 +1,4 @@
 """mlease_b200 -- H100-native ADMM logistic regression behind ml-ease's AdmmTrain/NaiveTrain/Test surface."""
 from ._native import MleaseError, SO_PATH, lib  # noqa: F401
-from .admm import AdmmSession, Comm, World, item_model_train, naive_train, naive_train_dense, score, score_keyed, score_keyed_var, test_loglik, test_loglik_keyed  # noqa: F401
+from .admm import (AdmmSession, Comm, World, item_model_train, item_model_train_sparse, keyed_models_for_scoring,  # noqa: F401
+                   naive_train, naive_train_dense, naive_train_sparse, score, score_keyed, score_keyed_var, test_loglik, test_loglik_keyed)

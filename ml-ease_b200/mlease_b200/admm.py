@@ -522,3 +522,91 @@ def item_model_train(vals, key_rowstart, response, intercept_lambdas, default_la
                                         len(il), ptr(il), len(dl), ptr(dl), ptr(lm), int(bool(binary_feature)), int(bool(compute_var)),
                                         ptr(out), ptr(var)))
     return out, var
+
+
+def _host(a, dtype):
+    """numpy copy of a host array or torch tensor (any device)"""
+    if hasattr(a, "data_ptr"):
+        a = a.detach().cpu().numpy()
+    return np.ascontiguousarray(a, dtype=dtype)
+
+
+def _list_capacity(key_rowstart, rowptr, num_features, fitted, intercept):
+    """entries the keys' lists may need: sum over fitted keys of min(stored entries, num_features) (+ 1 for the intercept), from
+    rowptr at the key boundaries alone"""
+    krs = _host(key_rowstart, np.int64)
+    if hasattr(rowptr, "data_ptr"):
+        import torch
+        at = _host(rowptr[torch.as_tensor(krs, device=rowptr.device)], np.int64)
+    else:
+        at = np.asarray(rowptr, np.int64)[krs]
+    nnz = np.diff(at)
+    return int((np.minimum(nnz, int(num_features))[fitted] + (1 if intercept else 0)).sum())
+
+
+def naive_train_sparse(vals, key_rowstart, response, lambdas, *, rowptr, colidx, num_features, weight=None, offset=None, lambda_map=None,
+                       prior_mean=0.0, penalize_intercept=False, has_intercept=True, data_size_threshold=0, binary_feature=False, device=0,
+                       stream=None, capacity=None):
+    """naive_train on CSR keys with each key's model returned as the columns its rows list (mlease_naive_train_sparse): key k's list
+    is cols[key_ptr[k]:key_ptr[k+1]] (ascending, then num_features for the intercept when has_intercept), its values for lambda l
+    models[l, key_ptr[k]:key_ptr[k+1]], the dense call's fit at those columns; an unlisted feature's coefficient is 0.  Skipped
+    keys and keys without rows have empty lists.  capacity (None: the bound from rowptr at the key boundaries) is the room allocated.
+    -> (key_ptr [K+1] int64, cols [n] int32, models [L, n] float64, skipped [K] bool)."""
+    krs = np.ascontiguousarray(key_rowstart, np.int64)
+    K, D = len(krs) - 1, int(num_features)
+    lam = _f32(np.atleast_1d(lambdas))
+    L = len(lam)
+    rp, ci, vals = _keep(rowptr, np.int64), _keep(colidx, np.int32), _keep(vals, np.float32)
+    r, w, o, lm = _keep(response, np.int32), _keep(weight, np.float32), _keep(offset, np.float32), _keep(lambda_map, np.float32)
+    rows = np.diff(krs)
+    cap = _list_capacity(krs, rp, D, (rows > 0) & (rows >= int(data_size_threshold)), has_intercept) if capacity is None else int(capacity)
+    key_ptr = np.zeros(K + 1, np.int64)
+    cols = np.zeros(max(cap, 1), np.int32)
+    models = np.zeros((L, max(cap, 1)), np.float64)
+    skipped = np.zeros(K, np.int32)
+    check(lib().mlease_naive_train_sparse(device, stream, K, D, ptr(krs), ptr(rp), ptr(ci), ptr(vals), ptr(r), ptr(w), ptr(o), L, ptr(lam),
+                                          ptr(lm), float(prior_mean), int(penalize_intercept), int(has_intercept), int(data_size_threshold),
+                                          int(bool(binary_feature)), cap, ptr(key_ptr), ptr(cols), ptr(models), ptr(skipped)))
+    n = int(key_ptr[K])
+    return key_ptr, cols[:n].copy(), models[:, :n].copy(), skipped.astype(bool)
+
+
+def item_model_train_sparse(vals, key_rowstart, response, intercept_lambdas, default_lambdas, *, rowptr, colidx, num_features,
+                            intercept_prior_mean=None, weight=None, offset=None, lambda_map=None, binary_feature=False, compute_var=False,
+                            device=0, stream=None, capacity=None):
+    """item_model_train with each key's model (and posterior variance) returned as the columns its rows list, then the intercept
+    (mlease_item_model_train_sparse); values the dense call's fit at those columns, an unlisted feature's coefficient 0 and
+    variance 1/q.  -> (key_ptr [K+1] int64, cols [n] int32, models [IL, DL, n] float64, var [IL, DL, n] float64 or None)."""
+    krs = np.ascontiguousarray(key_rowstart, np.int64)
+    K, D = len(krs) - 1, int(num_features)
+    il, dl = _f32(np.atleast_1d(intercept_lambdas)), _f32(np.atleast_1d(default_lambdas))
+    rp, ci, vals = _keep(rowptr, np.int64), _keep(colidx, np.int32), _keep(vals, np.float32)
+    r, w, o, lm = _keep(response, np.int32), _keep(weight, np.float32), _keep(offset, np.float32), _keep(lambda_map, np.float32)
+    im = np.zeros(K, np.float64) if intercept_prior_mean is None else np.ascontiguousarray(intercept_prior_mean, np.float64)
+    if len(im) != K:
+        raise ValueError("intercept_prior_mean must hold one entry per key")
+    cap = _list_capacity(krs, rp, D, np.diff(krs) > 0, True) if capacity is None else int(capacity)
+    G = len(il) * len(dl)
+    key_ptr = np.zeros(K + 1, np.int64)
+    cols = np.zeros(max(cap, 1), np.int32)
+    models = np.zeros((G, max(cap, 1)), np.float64)
+    var = np.zeros_like(models) if compute_var else None
+    check(lib().mlease_item_model_train_sparse(device, stream, K, D, ptr(krs), ptr(rp), ptr(ci), ptr(vals), ptr(r), ptr(w), ptr(o), ptr(im),
+                                               len(il), ptr(il), len(dl), ptr(dl), ptr(lm), int(bool(binary_feature)), int(bool(compute_var)),
+                                               cap, ptr(key_ptr), ptr(cols), ptr(models), ptr(var)))
+    n = int(key_ptr[K])
+    shape = (len(il), len(dl), n)
+    return (key_ptr, cols[:n].copy(), models[:, :n].reshape(shape).copy(),
+            None if var is None else var[:, :n].reshape(shape).copy())
+
+
+def keyed_models_for_scoring(key_ptr, cols, models):
+    """The sparse fits' lists as score_keyed's models: model m = p * K + k (prior p, key k) is key k's list with prior p's values
+    (models [..., n], the priors flattened in order).  -> (model_ptr [P*K+1] int64, model_col int32, model_val float32)."""
+    kp = np.ascontiguousarray(key_ptr, np.int64)
+    n = int(kp[-1])
+    models = np.asarray(models, np.float64)
+    P = int(np.prod(models.shape[:-1]))
+    vals = models.reshape(P, n)
+    model_ptr = np.concatenate([[0], (kp[1:][None, :] + n * np.arange(P, dtype=np.int64)[:, None]).reshape(-1)]).astype(np.int64)
+    return model_ptr, np.tile(np.ascontiguousarray(cols, np.int32)[:n], P), vals.astype(np.float32).reshape(-1)
