@@ -319,6 +319,31 @@ int mlease_item_model_train_sparse(int32_t device, void* stream, int32_t num_key
                                    const float* default_lambdas, const float* lambda_map, int32_t binary_feature, int32_t compute_var,
                                    int64_t capacity, int64_t* out_key_ptr, int32_t* out_col, double* out_model, double* out_var);
 
+/* mlease_item_model_train_sparse with the full posterior of every fit (computeFullPostVar, llf/LibLinear.java:315-326): the same
+ * inputs, plan, fits, lists and several-device use, the models bit for bit those of the sparse call for one-row keys in their own
+ * column spaces (within its run-to-run spread otherwise).  At each fit, H = diag(q) + sum_i w_i p_i (1-p_i) x_i x_i^T is assembled
+ * in fp64 on the device over the key's own columns (deterministically: Sigma depends on the key's rows and fit alone, not on the
+ * chunking, the streaming or the other keys) and inverted by Cholesky (K3's fp64 factorisation and explicit inverse), Sigma = H^-1.
+ *   out_var:  required; prior p's entry e is diag(Sigma) at the list's column, out_var[p * capacity + e], in place of the sparse call's
+ *             1 / hessianDiagonal.  An unlisted feature is uncorrelated with the listed ones: its variance is 1/q.
+ *   out_cov:  NULL (then cov_capacity and out_cov_ptr are ignored), or key k's block is entries [out_cov_ptr[k], out_cov_ptr[k+1])
+ *             (out_cov_ptr [num_keys+1], out_cov_ptr[0] = 0): for a list of n_k entries, n_k (n_k + 1) / 2 values, the lower
+ *             triangle of Sigma over the list's order, row-major -- entry (a, b), a >= b, at out_cov_ptr[k] + a (a+1) / 2 + b.  Prior
+ *             p's values are at out_cov[p * cov_capacity + e].  Keys that are not fitted have empty blocks.  cov_capacity is checked
+ *             chunk by chunk, once the chunk's list lengths are fixed and before it writes anything: a shortfall is
+ *             MLEASE_ERR_INVALID, the message giving the entries needed up to that chunk's last key.
+ * Refused with MLEASE_ERR_INVALID: rows whose columns are not strictly increasing (llf/LogisticRegressionL2.java:277), and a fitted
+ * key whose system (its own column space, or num_features + 1 at the global width) is wider than 2048 columns -- the widest whose
+ * explicit inverse K3 forms -- before that key's chunk is solved, the message naming the key and its width.  A Hessian that is not
+ * positive definite is MLEASE_ERR_NUMERIC.  out_key_ptr, out_col, out_model, out_var, out_cov_ptr and out_cov are host memory. */
+int mlease_item_model_train_cov(int32_t device, void* stream, int32_t num_keys, int32_t num_features, const int64_t* key_rowstart,
+                                const int64_t* rowptr, const int32_t* colidx, const float* vals, const int32_t* response,
+                                const float* weight, const float* offset, const double* intercept_prior_mean,
+                                int32_t num_intercept_lambdas, const float* intercept_lambdas, int32_t num_default_lambdas,
+                                const float* default_lambdas, const float* lambda_map, int32_t binary_feature, int64_t capacity,
+                                int64_t* out_key_ptr, int32_t* out_col, double* out_model, double* out_var, int64_t cov_capacity,
+                                int64_t* out_cov_ptr, double* out_cov);
+
 /* ---------------------------------------------------------------------------------------
  * RegressionTest / RegressionTestLoglik.
  * score: pred = float(offset + interceptTerm + sum beta_k x_k), interceptTerm = -log(n-1+n*exp(-b)),
@@ -355,6 +380,22 @@ int mlease_score_keyed_var(int32_t device, void* stream, int32_t num_features, i
                            int32_t num_models_per_key, const int64_t* model_ptr, const int32_t* model_col, const float* model_val,
                            const int64_t* var_ptr, const int32_t* var_col, const float* var_val, const float* var_default,
                            int32_t binary_feature, float* pred, float* pred_var);
+/* mlease_score_keyed with each record's predictive variance under the FULL posterior of its key's model (mlease_item_model_train_cov's
+ * blocks, ordered by keyed_cov_for_scoring / as the models).  Model m = g * num_keys + k; its covariance is cov_val[cov_ptr[m] ..
+ * cov_ptr[m+1]) (cov_ptr [G * num_keys + 1], cov_ptr[0] = 0), the packed lower triangle of Sigma over model m's own model_col list,
+ * row-major (entry (a, b), a >= b, at cov_ptr[m] + a(a+1)/2 + b), of n_m(n_m+1)/2 finite values for a list of n_m entries, or empty
+ * (no posterior: pred_var is NaN); any other size is MLEASE_ERR_INVALID.  An unlisted column c has variance 1 / lambda_map[c] where
+ * lambda_map ([num_features] or NULL) is > 0, else var_default[m] (ItemModelTrain's own prior).  pred [G][nrows] is bitwise
+ * mlease_score_keyed's; pred_var [G][nrows] = float(x_L^T Sigma_m x_L + sum over unlisted columns of v_c x_c^2), x_L the record's
+ * entries the list names plus the intercept at 1 when the list ends with it, in fp64 in a fixed order (bitwise repeatable, the same
+ * streamed or resident).  Rows must list strictly ascending columns (checked); binary_feature makes every x 1.  Streaming, budgets
+ * and several-device use are mlease_score_keyed's; the blocks are held on the device for the whole call.  All pointers
+ * host-or-device. */
+int mlease_score_keyed_cov(int32_t device, void* stream, int32_t num_features, int32_t num_keys, const int64_t* key_rowstart,
+                           const int64_t* rowptr, const int32_t* colidx, const float* vals, const float* offset, int32_t num_models_per_key,
+                           const int64_t* model_ptr, const int32_t* model_col, const float* model_val, const int64_t* cov_ptr,
+                           const double* cov_val, const float* lambda_map, const float* var_default, int32_t binary_feature, float* pred,
+                           float* pred_var);
 /* ItemModelTestLoglik (jobs/ItemModelTestLoglik.java:60-142): entry e = one (record, pred-map key) pair: entry_key[e] in
  * [0, num_keys), entry_group[e] = combiner group (non-decreasing), the record's response (1, 0, -1) and weight (NULL = 1), pred[e].
  * out_loglik / out_count [num_keys] (host): reducer float(sum of float combiner partials / sum of counts), partials added in group

@@ -174,10 +174,115 @@ struct KeyedVar {
   }
 };
 
+// mlease_score_keyed_cov: each record's predictive variance under the full posterior of its key's model, pred_var = float(x_L^T Sigma
+// x_L + sum over unlisted columns of v_c x_c^2), x_L the record's entries the model lists plus the intercept at 1 when the list ends
+// with it.  Sigma is the model's packed lower triangle over its list (entry (a, b), a >= b, at cov_ptr[m] + a(a+1)/2 + b); an empty
+// block gives NaN.  v_c = 1 / lambda_map[c] where that is > 0, else var_default[m].  One warp per record and model: each entry's
+// position in the list comes from a binary search, then the lanes walk the flat pair space of 256-entry tiles of the row (a tile
+// with itself, then with each earlier tile), fp64, each lane over a fixed set of pairs in a fixed order, then warp_sum: bitwise
+// repeatable, and the same for a record whichever range or chunk scores it.
+constexpr int COV_TILE = 256;
+struct KeyedCov {
+  const long long* cp = nullptr;
+  const double* cv = nullptr;
+  const float* lm = nullptr;
+  const float* vdef = nullptr;
+  float* pred_var = nullptr;
+  explicit operator bool() const { return cp != nullptr; }
+};
+__device__ __forceinline__ int cov_row_of(long long e) {   // the row a of flat lower-triangle entry e
+  int a = (int)((sqrt(8.0 * (double)e + 1.0) - 1.0) * 0.5);
+  while ((long long)a * (a + 1) / 2 > e) a--;
+  while ((long long)(a + 1) * (a + 2) / 2 <= e) a++;
+  return a;
+}
+__global__ void __launch_bounds__(256) score_keyed_cov_kernel(int Dg, int k0, int k1, long long r0, long long r1, const long long* __restrict__ krs,
+                                                              const long long* __restrict__ rowptr, const int* __restrict__ colidx,
+                                                              const float* __restrict__ vals, const long long* __restrict__ mp,
+                                                              const int* __restrict__ mc, const long long* __restrict__ cp,
+                                                              const double* __restrict__ cv, const float* __restrict__ lm,
+                                                              const float* __restrict__ vdef, int K, int G, int binary_feature, long long nrows,
+                                                              long long row_base, float* __restrict__ pred_var, int* __restrict__ bad) {
+  __shared__ int spos[8][2][COV_TILE];
+  __shared__ double sx[8][2][COV_TILE];
+  rowptr -= row_base;
+  pred_var -= row_base;
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const long long wg = (long long)blockIdx.x * (blockDim.x >> 5) + w;
+  const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
+  for (long long i = r0 + wg; i < r1; i += nw) {
+    int lo = k0, hi = k1;
+    while (hi - lo > 1) { const int mid = (lo + hi) >> 1; if (krs[mid] <= i) lo = mid; else hi = mid; }
+    const long long j0 = rowptr[i], j1 = rowptr[i + 1];
+    for (int q = 0; q < G; q++) {
+      const long long m = (long long)q * K + lo;
+      const long long e0 = mp[m];
+      const int n = (int)(mp[m + 1] - e0);
+      const double* S = cv + cp[m];
+      if (cp[m + 1] == cp[m]) { if (lane == 0) pred_var[(size_t)q * nrows + i] = __int_as_float(0x7fc00000); continue; }
+      const int* L = mc + e0;
+      const int pI = (n > 0 && L[n - 1] == Dg) ? n - 1 : -1;
+      const double vd = (double)vdef[m];
+      auto sig = [&](int a, int b) { return a >= b ? S[(long long)a * (a + 1) / 2 + b] : S[(long long)b * (b + 1) / 2 + a]; };
+      // tile t of the row's entries into buffer slot: list positions (-1: unlisted or out of range) and values; first: the diagonal
+      // pass also adds the unlisted terms and the entries' pairs with the intercept
+      auto load = [&](long long t0, int slot, bool first, double& acc) {
+        for (int t = lane; t < COV_TILE; t += 32) {
+          const long long j = t0 + t;
+          int p = -1; double x = 0.0;
+          if (j < j1) {
+            const int c = colidx[j];
+            x = binary_feature ? 1.0 : (double)vals[j];
+            if ((unsigned)c >= (unsigned)Dg) { if (first) atomicOr(bad, 1); x = 0.0; }
+            else {
+              if (first && j > j0 && colidx[j - 1] >= c) atomicOr(bad, 2);
+              int a = 0, b = n;
+              while (a < b) { const int mid = (a + b) >> 1; if (L[mid] < c) a = mid + 1; else b = mid; }
+              if (a < n && L[a] == c) {
+                p = a;
+                if (first && pI >= 0) acc += 2.0 * x * sig(pI, p);
+              } else if (first) {
+                acc += (lm && lm[c] > 0.f ? 1.0 / (double)lm[c] : vd) * x * x;
+              }
+            }
+          }
+          spos[w][slot][t] = p; sx[w][slot][t] = x;
+        }
+        __syncwarp();
+      };
+      double acc = 0.0;
+      for (long long ta = j0; ta < j1; ta += COV_TILE) {
+        const int Ta = (int)min((long long)COV_TILE, j1 - ta);
+        load(ta, 0, true, acc);
+        const long long tri = (long long)Ta * (Ta + 1) / 2;
+        for (long long e = lane; e < tri; e += 32) {
+          const int a = cov_row_of(e), b = (int)(e - (long long)a * (a + 1) / 2);
+          const int pa = spos[w][0][a], pb = spos[w][0][b];
+          if (pa >= 0 && pb >= 0) acc += (a == b ? 1.0 : 2.0) * sx[w][0][a] * sx[w][0][b] * sig(pa, pb);
+        }
+        for (long long tb = j0; tb < ta; tb += COV_TILE) {
+          double unused = 0.0;
+          load(tb, 1, false, unused);
+          for (int e = lane; e < Ta * COV_TILE; e += 32) {
+            const int a = e / COV_TILE, b = e % COV_TILE;
+            const int pa = spos[w][0][a], pb = spos[w][1][b];
+            if (pa >= 0 && pb >= 0) acc += 2.0 * sx[w][0][a] * sx[w][1][b] * sig(pa, pb);
+          }
+          __syncwarp();
+        }
+        __syncwarp();
+      }
+      if (lane == 0 && pI >= 0) acc += sig(pI, pI);
+      acc = warp_sum(acc);
+      if (lane == 0) pred_var[(size_t)q * nrows + i] = (float)acc;
+    }
+  }
+}
+
 static cudaError_t score_keyed_chunk(int Dg, int K, int k0, int k1, long long r0, long long r1, const long long* krs, const long long* rowptr,
                                      const int* colidx, const float* vals, const float* offset, int G, const long long* mp, const int* mc,
                                      const float* mv, const double* term, int binary_feature, long long nrows, long long row_base, float* table,
-                                     float* pred, int* d_bad, const KeyedVar& var, cudaStream_t st) {
+                                     float* pred, int* d_bad, const KeyedVar& var, const KeyedCov& cov, cudaStream_t st) {
   const int LP = G == 1 ? 1 : G == 2 ? 2 : 4;
   const int nk = k1 - k0;
   const size_t tbytes = (size_t)nk * Dg * LP * sizeof(float);
@@ -199,6 +304,9 @@ static cudaError_t score_keyed_chunk(int Dg, int K, int k0, int k1, long long r0
       if (LP == 1) MLEASE_SCORE_KEYED(1, false); else if (LP == 2) MLEASE_SCORE_KEYED(2, false); else MLEASE_SCORE_KEYED(4, false);
     }
 #undef MLEASE_SCORE_KEYED
+    if (cov)
+      score_keyed_cov_kernel<<<(int)blocks, 256, 0, st>>>(Dg, k0, k1, r0, r1, krs, rowptr, colidx, vals, mp, mc, cov.cp, cov.cv, cov.lm,
+                                                          cov.vdef, K, G, binary_feature, nrows, row_base, cov.pred_var, d_bad);
   }
   return cudaGetLastError();
 }
@@ -398,9 +506,10 @@ namespace mlease {
 static int score_keyed(int32_t device, void* stream, int32_t Dg, int32_t K, const int64_t* key_rowstart, const int64_t* rowptr,
                        const int32_t* colidx, const float* vals, const float* offset, int32_t L, const int64_t* model_ptr,
                        const int32_t* model_col, const float* model_val, const int64_t* var_ptr, const int32_t* var_col,
-                       const float* var_val, const float* var_default, int32_t binary_feature, float* pred, float* pred_var) {
+                       const float* var_val, const float* var_default, int32_t binary_feature, float* pred, float* pred_var,
+                       const int64_t* cov_ptr = nullptr, const double* cov_val = nullptr, const float* lambda_map = nullptr) {
   if (Dg <= 0 || K < 0 || L <= 0 || !key_rowstart || !rowptr || !colidx || !vals || !model_ptr || !pred) return fail(MLEASE_ERR_INVALID, "bad argument");
-  if (var_ptr && (!var_default || !pred_var)) return fail(MLEASE_ERR_INVALID, "bad argument");
+  if ((var_ptr || cov_ptr) && (!var_default || !pred_var)) return fail(MLEASE_ERR_INVALID, "bad argument");
   if (int rc = open_device(device, nullptr)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   // host copies of the index arrays that decide the chunks and of the models, which are checked and give the intercept terms
@@ -464,10 +573,41 @@ static int score_keyed(int32_t device, void* stream, int32_t Dg, int32_t K, cons
       vh.vterm[m] = e1 == vh.vp[m] ? std::nan("") : vh.vc[e1 - 1] == Dg ? (double)vh.vv[e1 - 1] : 0.0;
     }
   }
+  // mlease_score_keyed_cov: every block the packed lower triangle over its model's list, or empty; finite values; lambda_map >= 0
+  std::vector<long long> cph;
+  std::vector<double> cvh;
+  std::vector<float> lmh, cdef;
+  if (cov_ptr) {
+    cph.resize((size_t)M + 1);
+    cdef.resize((size_t)M);
+    CK(cudaMemcpy(cph.data(), cov_ptr, cph.size() * 8, cudaMemcpyDefault));
+    if (M > 0) CK(cudaMemcpy(cdef.data(), var_default, (size_t)M * 4, cudaMemcpyDefault));
+    if (cph[0] != 0) return fail(MLEASE_ERR_INVALID, "cov_ptr[0] must be 0");
+    for (long long m = 0; m < M; m++) {
+      auto bad = [m](const std::string& what) { return fail(MLEASE_ERR_INVALID, what + " (model " + std::to_string(m) + ")"); };
+      const long long n = mp[m + 1] - mp[m], sz = cph[m + 1] - cph[m];
+      if (sz != 0 && sz != n * (n + 1) / 2)
+        return bad("covariance block of " + std::to_string(sz) + " entries: a model listing " + std::to_string(n) + " columns needs " +
+                   std::to_string(n * (n + 1) / 2) + ", or 0 for no posterior");
+      if (!(std::isfinite(cdef[m]) && cdef[m] >= 0.f)) return bad("var_default must be finite and >= 0");
+    }
+    const long long nce = cph[M];
+    if (nce > 0 && !cov_val) return fail(MLEASE_ERR_INVALID, "null cov_val");
+    cvh.resize((size_t)nce);
+    if (nce > 0) CK(cudaMemcpy(cvh.data(), cov_val, (size_t)nce * 8, cudaMemcpyDefault));
+    for (long long e = 0; e < nce; e++)
+      if (!std::isfinite(cvh[e])) return fail(MLEASE_ERR_INVALID, "cov_val must be finite (entry " + std::to_string(e) + ")");
+    if (lambda_map) {
+      lmh.resize((size_t)Dg);
+      CK(cudaMemcpy(lmh.data(), lambda_map, (size_t)Dg * 4, cudaMemcpyDefault));
+      for (float x : lmh) if (!(x >= 0.f) || !std::isfinite(x)) return fail(MLEASE_ERR_INVALID, "lambda_map: entries must be > 0, or 0 for a feature without one");
+    }
+  }
   if (nrows == 0) return 0;
   long long nnz;
   CK(cudaMemcpy(&nnz, rowptr + nrows, 8, cudaMemcpyDefault));
-  const bool pred_dev = is_device_ptr(pred), pred_var_dev = var && is_device_ptr(pred_var);
+  const bool with_pv = var || cov_ptr;   // a pred_var output
+  const bool pred_dev = is_device_ptr(pred), pred_var_dev = with_pv && is_device_ptr(pred_var);
   const size_t key_bytes = (size_t)Dg * (L >= 3 ? 4 : L) * sizeof(float) * (var ? 2 : 1);   // var: the variance table too
   // keys per table chunk within a budget
   auto chunk_keys = [&](size_t b) {
@@ -478,21 +618,22 @@ static int score_keyed(int32_t device, void* stream, int32_t Dg, int32_t K, cons
   const size_t budget = keyed_budget(free_b);
   // resident (one range) when the rows, the pred array and the model table fit the budget next to the models; else key ranges whose
   // rows, offsets and pred slice fit a quarter of the budget stream, each one table chunk
-  const size_t models = ((size_t)M + 1) * 8 + (size_t)nme * 8 + (size_t)M * 8 + ((size_t)K + 1) * 8 + (var ? var->bytes() : 0);
+  const size_t models = ((size_t)M + 1) * 8 + (size_t)nme * 8 + (size_t)M * 8 + ((size_t)K + 1) * 8 + (var ? var->bytes() : 0) +
+                        cph.size() * 8 + cvh.size() * 8 + lmh.size() * 4 + cdef.size() * 4;
   size_t rows = 0;
   if (!is_device_ptr(rowptr)) rows += ((size_t)nrows + 1) * 8;
   if (!is_device_ptr(colidx)) rows += (size_t)nnz * 4;
   if (!is_device_ptr(vals)) rows += (size_t)nnz * 4;
   if (offset && !is_device_ptr(offset)) rows += (size_t)nrows * 4;
   if (!pred_dev) rows += (size_t)L * nrows * 4;
-  if (var && !pred_var_dev) rows += (size_t)L * nrows * 4;
+  if (with_pv && !pred_var_dev) rows += (size_t)L * nrows * 4;
   std::vector<long long> ranges{0, K}, nnz_at{0, nnz}, row_at;   // nnz_at / row_at: rowptr / the row at the range bounds
   long long kpc = 0;
   const bool streamed = models + rows + std::min(SCORE_KEYED_TABLE_CAP, budget / 4) > budget;
   if (streamed) {
     std::vector<long long> off;   // rowptr at the key boundaries
     if (int rc = gather_rowptr(rowptr, krs, off)) return rc;
-    const size_t pred_bytes = 4 * (size_t)L * (var ? 2 : 1);   // a row's pred (and pred_var) slice
+    const size_t pred_bytes = 4 * (size_t)L * (with_pv ? 2 : 1);   // a row's pred (and pred_var) slice
     kpc = chunk_keys(budget);
     ranges = plan_ranges(K, budget / 4, kpc, [&](long long k) {
       return (size_t)(krs[k + 1] - krs[k]) * (16 + 4 + pred_bytes) + (size_t)(off[k + 1] - off[k]) * 8;
@@ -525,6 +666,16 @@ static int score_keyed(int32_t device, void* stream, int32_t Dg, int32_t K, cons
     dvar.pred_var = pred_var;
     if (streamed || !pred_var_dev) { if (int rc = t.get(&dvar.pred_var, (size_t)L * max_rows, false)) return rc; }
   }
+  KeyedCov dcov;
+  if (cov_ptr) {
+    if (int rc = to_device(t, (const long long*)cph.data(), cph.size(), &dcov.cp, st)) return rc;
+    if (int rc = to_device(t, (const double*)cvh.data(), cvh.size(), &dcov.cv, st)) return rc;
+    if (int rc = to_device(t, (const float*)cdef.data(), cdef.size(), &dcov.vdef, st)) return rc;
+    if (lambda_map) { if (int rc = to_device(t, (const float*)lmh.data(), lmh.size(), &dcov.lm, st)) return rc; }
+    dcov.pred_var = pred_var;
+    if (streamed || !pred_var_dev) { if (int rc = t.get(&dcov.pred_var, (size_t)L * max_rows, false)) return rc; }
+  }
+  float* const d_pred_var = var ? dvar.pred_var : dcov.pred_var;
   int* d_bad;
   if (int rc = t.get(&d_bad, 1, false)) return rc;
   CK(cudaMemsetAsync(d_bad, 0, 4, st));
@@ -552,15 +703,18 @@ static int score_keyed(int32_t device, void* stream, int32_t Dg, int32_t K, cons
       const int k0 = (int)(ranges[c] + chunks[j - 1]), k1 = (int)(ranges[c] + chunks[j]);
       bounds.push_back(k1);
       if (krs[k1] == krs[k0]) continue;
-      for (int l0 = 0; l0 < L; l0 += 4)
+      for (int l0 = 0; l0 < L; l0 += 4) {
+        KeyedCov cg = dcov;   // the group's models: blocks, defaults and pred_var rows from l0 on
+        if (cg) { cg.cp += (size_t)l0 * K; cg.vdef += (size_t)l0 * K; cg.pred_var += (size_t)l0 * n; }
         CK(score_keyed_chunk(Dg, K, k0, k1, krs[k0], krs[k1], d_krs, rp, ci, vv, o, std::min(4, L - l0), d_mp + (size_t)l0 * K, d_mc, d_mv,
-                             d_term + (size_t)l0 * K, binary_feature, n, r0, d_table, d_pred + (size_t)l0 * n, d_bad, dvar.at(l0, K, n), st));
+                             d_term + (size_t)l0 * K, binary_feature, n, r0, d_table, d_pred + (size_t)l0 * n, d_bad, dvar.at(l0, K, n), cg, st));
+      }
     }
     if (int rc = ring.done(c)) return rc;
     if (int rc = ring.start(c + 1)) return rc;
     if (n > 0 && d_pred != pred) CK(cudaMemcpy2DAsync(pred + r0, (size_t)nrows * 4, d_pred, (size_t)n * 4, (size_t)n * 4, L, cudaMemcpyDefault, st));
-    if (n > 0 && var && dvar.pred_var != pred_var)
-      CK(cudaMemcpy2DAsync(pred_var + r0, (size_t)nrows * 4, dvar.pred_var, (size_t)n * 4, (size_t)n * 4, L, cudaMemcpyDefault, st));
+    if (n > 0 && with_pv && d_pred_var != pred_var)
+      CK(cudaMemcpy2DAsync(pred_var + r0, (size_t)nrows * 4, d_pred_var, (size_t)n * 4, (size_t)n * 4, L, cudaMemcpyDefault, st));
   }
   int bad = 0;
   CK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, st));
@@ -587,6 +741,15 @@ int mlease_score_keyed_var(int32_t device, void* stream, int32_t Dg, int32_t K, 
   if (!var_ptr) return fail(MLEASE_ERR_INVALID, "bad argument");
   return score_keyed(device, stream, Dg, K, key_rowstart, rowptr, colidx, vals, offset, G, model_ptr, model_col, model_val, var_ptr, var_col,
                      var_val, var_default, binary_feature, pred, pred_var);
+}
+
+int mlease_score_keyed_cov(int32_t device, void* stream, int32_t Dg, int32_t K, const int64_t* key_rowstart, const int64_t* rowptr,
+                           const int32_t* colidx, const float* vals, const float* offset, int32_t G, const int64_t* model_ptr,
+                           const int32_t* model_col, const float* model_val, const int64_t* cov_ptr, const double* cov_val,
+                           const float* lambda_map, const float* var_default, int32_t binary_feature, float* pred, float* pred_var) {
+  if (!cov_ptr) return fail(MLEASE_ERR_INVALID, "bad argument");
+  return score_keyed(device, stream, Dg, K, key_rowstart, rowptr, colidx, vals, offset, G, model_ptr, model_col, model_val, nullptr, nullptr,
+                     nullptr, var_default, binary_feature, pred, pred_var, cov_ptr, cov_val, lambda_map);
 }
 
 int mlease_test_loglik_keyed(int32_t device, void* stream, int64_t n, const int32_t* entry_key, const int32_t* entry_group,

@@ -148,6 +148,63 @@ __global__ void postvar_init_kernel(const Problem* __restrict__ probs, const dou
   }
 }
 
+// Full Hessian of every problem of a batch (CSR rows with strictly increasing column ids): Lc = diag(q) + sum_i d_i x_i x_i^T on
+// [0, Dt), the intercept (has_bias) an implicit entry 1 at column Dt - 1, identity on the padding, zero above the diagonal.  CTA =
+// (column block bj, row block bi, problem); a lower 32x32 tile densifies 32-row slabs of the problem's rows into shared memory (each
+// row's entries in the two column blocks found by a binary search) and every thread sums its 4 cells over the rows in row order:
+// no atomics, so each problem's H is a function of its beta and rows alone, whatever else its batch holds.  dvec is numbered
+// across the batch's rows (row_start), as postvar_rowweights leaves it.
+__global__ void __launch_bounds__(256) postvar_hess_batch_kernel(const Problem* __restrict__ probs, const long long* __restrict__ row_start,
+                                                                 const double* __restrict__ dvec, int has_bias) {
+  const Problem& pb = probs[blockIdx.z];
+  const int bi = blockIdx.y, bj = blockIdx.x;
+  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+  double* H = pb.Lc;
+  if (bj > bi) {
+#pragma unroll
+    for (int q = 0; q < 4; q++) H[(size_t)(bi * 32 + ty + 8 * q) * pb.ldh + bj * 32 + tx] = 0.0;
+    return;
+  }
+  __shared__ double xa[32][33], xb[32][33];   // xa = d_i x_i over block bi, xb = x_i over block bj, for 32 rows
+  const double* d = dvec + row_start[blockIdx.z];
+  const int icol = has_bias ? pb.Dt - 1 : -1;
+  double acc[4] = {0, 0, 0, 0};
+  for (long long r0 = 0; r0 < pb.n; r0 += 32) {
+    for (int e = threadIdx.x; e < 32 * 32; e += 256) { xa[e >> 5][e & 31] = 0.0; xb[e >> 5][e & 31] = 0.0; }
+    __syncthreads();
+    for (int t = ty; t < 64; t += 8) {   // warp ty: rows ty, ty + 8, .. of the slab, block bi then bj
+      const int r = t & 31;
+      const long long i = r0 + r;
+      if (i >= pb.n) continue;
+      const bool A = t < 32;
+      const int c0 = (A ? bi : bj) * 32;
+      const double s = A ? d[i] : 1.0;
+      double* x = A ? xa[r] : xb[r];
+      const long long j1 = pb.rowptr[i + 1];
+      long long lo = pb.rowptr[i], hi = j1;
+      while (lo < hi) { const long long mid = (lo + hi) >> 1; if (pb.colidx[mid] < c0) lo = mid + 1; else hi = mid; }
+      const long long j = lo + tx;   // strictly increasing columns: the block's entries are the next 32 at most
+      if (j < j1) { const int c = pb.colidx[j]; if (c < c0 + 32) x[c - c0] = s * (double)pb.vals[j]; }
+      if (tx == 0 && icol >= c0 && icol < c0 + 32) x[icol - c0] = s;
+    }
+    __syncthreads();
+#pragma unroll 8
+    for (int r = 0; r < 32; r++) {
+      const double b = xb[r][tx];
+#pragma unroll
+      for (int q = 0; q < 4; q++) acc[q] += xa[r][ty + 8 * q] * b;
+    }
+    __syncthreads();
+  }
+#pragma unroll
+  for (int q = 0; q < 4; q++) {
+    const int i = bi * 32 + ty + 8 * q, j = bj * 32 + tx;
+    double v = j <= i ? acc[q] : 0.0;
+    if (i == j) v += i < pb.Dt ? pb.q[i] : 1.0;
+    H[(size_t)i * pb.ldh + j] = v;
+  }
+}
+
 static int postvar_grid(long long nrows) { return (int)std::max(1LL, std::min(1184LL, (nrows + 7) / 8)); }   // 8 warps per CTA
 cudaError_t postvar_rowweights(const Problem* d_probs, int nprob, const long long* d_row_start, long long nrows, int has_bias, double* d_dvec,
                                cudaStream_t st, int* launches) {
@@ -167,6 +224,13 @@ cudaError_t postvar_hessian(const Problem* d_prob, bool csr, int ldh, const doub
   if (csr) postvar_hess_csr_kernel<<<1184, 256, 0, st>>>(d_prob, d_dvec, has_bias);
   else { const int T = ldh / 32; postvar_hess_dense_kernel<<<dim3(T, T), 256, 0, st>>>(d_prob, d_dvec); }
   if (launches) *launches += 2;
+  return cudaGetLastError();
+}
+cudaError_t postvar_hessian_batch(const Problem* d_probs, int nprob, int ldh, const long long* d_row_start, const double* d_dvec, int has_bias,
+                                  cudaStream_t st, int* launches) {
+  const int T = ldh / 32;
+  postvar_hess_batch_kernel<<<dim3(T, T, nprob), 256, 0, st>>>(d_probs, d_row_start, d_dvec, has_bias);
+  if (launches) *launches += 1;
   return cudaGetLastError();
 }
 

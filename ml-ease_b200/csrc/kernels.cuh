@@ -94,5 +94,9 @@ cudaError_t postvar_diag(const Problem* d_probs, int nprob, const long long* d_r
                          cudaStream_t st, int* launches);
 cudaError_t postvar_hessian(const Problem* d_prob, bool csr, int ldh, const double* d_dvec, const double* d_q, int has_bias, cudaStream_t st,
                             int* launches);
+// the full Hessian of every problem d_probs[0 .. nprob) of a CSR batch (rows with strictly increasing column ids, width ldh) into its
+// Lc, as chol_prep leaves it; deterministic (no atomics, every cell summed in row order)
+cudaError_t postvar_hessian_batch(const Problem* d_probs, int nprob, int ldh, const long long* d_row_start, const double* d_dvec, int has_bias,
+                                  cudaStream_t st, int* launches);
 
 }  // namespace mlease

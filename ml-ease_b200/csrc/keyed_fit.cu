@@ -1,5 +1,6 @@
 // keyed_fit.cu -- K independent fits per prior over one upload of the rows: RegressionNaiveTrain (mlease_naive_train,
-// mlease_naive_train_dense) and ItemModelTrain (mlease_item_model_train), and both with sparse outputs (mlease_*_train_sparse).
+// mlease_naive_train_dense) and ItemModelTrain (mlease_item_model_train), both with sparse outputs (mlease_*_train_sparse), and
+// ItemModelTrain with each key's full posterior covariance (mlease_item_model_train_cov).
 #include <cub/block/block_scan.cuh>
 
 #include <algorithm>
@@ -108,6 +109,35 @@ __global__ void sparse_gather_kernel(const Problem* probs, const GatherJob* jobs
     __syncthreads();
   }
 }
+// Where problem b of a batch writes its posterior in a chunk's slab: its list of n entries starts at entry dst of the variances (and
+// of the column ids the model gather wrote), the packed lower triangle of its covariance at entry cdst of the covariance slab (cdst
+// < 0: variances only)
+struct CovJob { long long dst, cdst; int n; };
+// One problem per block, from the explicit inverse Hinv = Sigma of its Hessian: the variances diag(Sigma) over its list and (cdst >= 0)
+// the lower triangle of Sigma over it, row-major: entry (a, b), a >= b, at cdst + a(a+1)/2 + b.  A local problem's entry a is its
+// column a, the last entry (the intercept) its column Dt - 1; a global-width problem's entry a is the global column col names.
+__global__ void cov_gather_kernel(const Problem* probs, const CovJob* jobs, int local, const int* col, double* var, double* cov) {
+  const Problem& pb = probs[blockIdx.x];
+  const CovJob jb = jobs[blockIdx.x];
+  auto hcol = [&](int a) -> size_t { return local ? (a < jb.n - 1 ? a : pb.Dt - 1) : col[jb.dst + a]; };
+  for (int a = threadIdx.x; a < jb.n; a += blockDim.x) { const size_t c = hcol(a); var[jb.dst + a] = pb.Hinv[c * pb.ldh + c]; }
+  if (jb.cdst < 0) return;
+  const long long tot = (long long)jb.n * (jb.n + 1) / 2;
+  for (long long e = threadIdx.x; e < tot; e += blockDim.x) {
+    int a = (int)((sqrt(8.0 * (double)e + 1.0) - 1.0) * 0.5);   // the row of entry e, corrected for rounding
+    while ((long long)a * (a + 1) / 2 > e) a--;
+    while ((long long)(a + 1) * (a + 2) / 2 <= e) a++;
+    const int b = (int)(e - (long long)a * (a + 1) / 2);
+    cov[jb.cdst + e] = pb.Hinv[hcol(a) * pb.ldh + hcol(b)];
+  }
+}
+
+// count[0] += the problems whose factorisation found a non-positive pivot (K3 leaves Ctrl::fail = 1)
+__global__ void cov_fail_kernel(const Problem* probs, int nprob, int* count) {
+  int c = 0;
+  for (int b = threadIdx.x; b < nprob; b += blockDim.x) c += probs[b].ctrl->fail == 1 ? 1 : 0;
+  if (c) atomicAdd(count, c);
+}
 
 // One prior of a keyed fit: precision q and mean m of every coefficient ([ldx], the intercept at Dg, 1 / 0 on the padding)
 struct KeyedPrior { std::vector<double> q, m; };
@@ -115,14 +145,22 @@ struct KeyedPrior { std::vector<double> q, m; };
 // The sparse output of mlease_*_train_sparse: key k's list is entries key_ptr[k] .. key_ptr[k + 1] of col, prior p's values at
 // model[p * cap + e] (and var).  NULL in KeyedFit: the dense [prior][K][Dt] arrays.
 struct SparseOut { int64_t cap; int64_t* key_ptr; int32_t* col; };
+// The covariance output of mlease_item_model_train_cov: key k's block is entries ptr[k] .. ptr[k + 1] of val, prior p's at
+// val[p * cap + e]; val NULL: variances only (ptr unused)
+struct CovOut { int64_t cap; int64_t* ptr; double* val; };
+// the widest system whose explicit inverse K3 forms (wider ones keep it factored, cholesky_factored_direction)
+constexpr int COV_MAX_WIDTH = 2048;
+// solve_batch of a covariance call whose batch would be matrix-free: solve_group splits it
+constexpr int SPLIT_BATCH = -1;
 // A chunk's sparse results on the device: the lists of its fitted keys, contiguous in key order, [prior][n] values and n column ids.
-// off / len (by key - k0): a key's entries in the slab; mrow: its row of mask (-1: it has a column list)
+// off / len (by key - k0): a key's entries in the slab; mrow: its row of mask (-1: it has a column list).  Covariance calls: [prior]
+// [ncov] packed blocks, coff a key's block
 struct Slab {
   int k0 = 0;
-  long long n = 0;
-  double* model = nullptr; double* var = nullptr; int* col = nullptr;
+  long long n = 0, ncov = 0;
+  double* model = nullptr; double* var = nullptr; int* col = nullptr; double* cov = nullptr;
   unsigned char* mask = nullptr;
-  std::vector<long long> off, len;
+  std::vector<long long> off, len, coff;
   std::vector<int> mrow;
 };
 
@@ -164,12 +202,15 @@ struct ChunkRows {
 // shape depend on the key's own rows alone, never on which keys share its call, chunk or streamed range; each chunk runs one batch
 // per width.  Dense sink: outputs are scattered back to the global columns, a feature the key does not list keeping 0 in the model
 // and 1/q in the variance.  Sparse sink (sp): each chunk's lists are gathered on the device into a slab and copied out once per prior.
+// Covariance (cv, with sp and out_var): after each prior's fit, every batch assembles its problems' exact fp64 Hessians into Lc, K3
+// factorises and inverts them, and the variances (and packed covariance blocks) over each key's list are gathered from Hinv.
 struct KeyedFit {
   int num_sms; cudaStream_t st; int32_t K, Dg; const int64_t* key_rowstart; const int64_t* rowptr; const int32_t* colidx; const float* vals;
   int64_t ldx_in; const int32_t* response; const float* weight; const float* offset; bool has_intercept; int32_t data_size_threshold;
   int32_t binary_feature; const std::vector<KeyedPrior>& priors; const double* intercept_mean; double* out_model; double* out_var;
   int32_t* skipped;
   const SparseOut* sp;                    // the output sink: NULL = dense out_model / out_var; else the lists (out_model / out_var their values)
+  const CovOut* cv;                       // NULL, or the full posterior (out_var = diag(Sigma)) and its blocks
   bool csr = false;
   int L = 0, Dt = 0, ldx = 0, Dp = 0, ldh = 0;
   std::vector<long long> krs, key_nnz0;   // key_nnz0: CSR rowptr at the key boundaries
@@ -190,8 +231,13 @@ struct KeyedFit {
   }
   // entries of a fitted CSR key's list at most: its stored entries or the dictionary, whichever is smaller, and the intercept
   long long list_bound(int k) const { return std::min<long long>(key_nnz0[k + 1] - key_nnz0[k], Dg) + (has_intercept ? 1 : 0); }
-  // device bytes of a fitted key's entries in its chunk's slab (values of every prior, variances, column ids); 0 for the dense sink
-  size_t slab_bytes(int k) const { return sp ? (size_t)list_bound(k) * ((size_t)L * 8 * (out_var ? 2 : 1) + 4) : 0; }
+  // device bytes of a fitted key's entries in its chunk's slab (values of every prior, variances, column ids, covariance blocks); 0 for
+  // the dense sink.  len: the key's list length when known, else (< 0) its bound
+  size_t slab_bytes(int k, long long len = -1) const {
+    if (!sp) return 0;
+    const size_t n = (size_t)(len < 0 ? list_bound(k) : len);
+    return n * ((size_t)L * 8 * (out_var ? 2 : 1) + 4) + (cv && cv->val ? n * (n + 1) / 2 * 8 * (size_t)L : 0);
+  }
   // the lists of keys [k0, k1) over the range's colidx ci (entries from key_nnz0[k0] on), and the widths they give
   int build_lists(int k0, int k1, const int* ci, cudaStream_t s, DevMem& mem, KeyCols* kc) {
     std::vector<long long> koff(key_nnz0.begin() + k0, key_nnz0.begin() + k1 + 1);
@@ -210,6 +256,7 @@ struct KeyedFit {
   }
   void init_outputs() {
     if (skipped) for (int k = 0; k < K; k++) skipped[k] = solves(k) ? 0 : 1;   // "data size < threshold": no model
+    if (cv && cv->val) cv->ptr[0] = 0;
     if (sp) { sp->key_ptr[0] = 0; return; }   // a list is written with its chunk
     for (size_t e = 0; e < (size_t)L * K * Dt; e++) out_model[e] = 0.0;
     if (out_var)   // a key without rows has no fit: every variance is the prior's
@@ -219,12 +266,18 @@ struct KeyedFit {
   }
   // sparse: empty lists for keys sp_key .. k1 - 1 (the keys before k1 that no chunk fitted)
   void close_lists(int k1) {
-    for (; sp_key < k1; sp_key++) sp->key_ptr[sp_key + 1] = sp->key_ptr[sp_key];
+    for (; sp_key < k1; sp_key++) {
+      sp->key_ptr[sp_key + 1] = sp->key_ptr[sp_key];
+      if (cv && cv->val) cv->ptr[sp_key + 1] = cv->ptr[sp_key];
+    }
   }
   int run();
   int solve_chunk(const int* keys, int nprob, const ChunkRows& cr, int* dflag, int* hflag);
   int solve_batch(const int* keys, int nprob, int width, const ChunkRows& cr, int* dflag, int* hflag, Slab* sl);
+  int solve_group(const int* keys, int nprob, int width, const ChunkRows& cr, int* dflag, int* hflag, Slab* sl);
   int open_slab(const int* keys, int nprob, const ChunkRows& cr, DevMem& mem, Slab* sl);
+  int posterior_cov(Batch& B, bool local, const long long* drs, long long nrows, double* dvec, const CovJob* dcjobs, Slab* sl, int l,
+                    int* dfail, const Ctrl* factor, const Ctrl* reset);
   int write_slab(const int* keys, int nprob, const Slab& sl);
 };
 
@@ -325,6 +378,8 @@ int KeyedFit::run() {
       CK(cudaStreamSynchronize(st));
       if (hflag[0]) return fail(MLEASE_ERR_INVALID, "feature index out of range");
       cr.csr_unique = hflag[1] ? 0 : 1;
+      if (cv && !cr.csr_unique)
+        return fail(MLEASE_ERR_INVALID, "the full Hessian needs rows with strictly increasing column ids (llf/LogisticRegressionL2.java:277)");
       if (lists) {
         if (int rc = build_lists(k0, k1, cr.ci, st, rt, &kc)) return rc;
         cr.kc = &kc; cr.kbase = k0;
@@ -342,7 +397,10 @@ int KeyedFit::run() {
     size_t cap = SIZE_MAX;
     if (!ring.staged()) { CK(cudaMemGetInfo(&free_b, &total_b)); cap = keyed_budget(free_b) / 2; }
     const std::vector<long long> chunks = plan_ranges((long long)keys.size(), cap, 16384, [&](long long i) {
-      return state_bytes(krs[keys[i] + 1] - krs[keys[i]], kdt[keys[i]]) + slab_bytes(keys[i]);
+      const int k = keys[i];
+      // a covariance call counts a listed key's blocks at their exact size: the bound squared overshoots wide keys many times
+      const long long len = cv && cr.kc && cr.kc->listed[k - cr.kbase] ? cr.kc->start[k - cr.kbase + 1] - cr.kc->start[k - cr.kbase] + 1 : -1;
+      return state_bytes(krs[k + 1] - krs[k], kdt[k]) + slab_bytes(k, len);
     }, nullptr);
     for (size_t j = 1; j < chunks.size(); j++) {
       if (int rc = solve_chunk(keys.data() + chunks[j - 1], (int)(chunks[j] - chunks[j - 1]), cr, dflag, hflag)) return rc;
@@ -363,6 +421,12 @@ int KeyedFit::solve_chunk(const int* keys, int nprob, const ChunkRows& cr, int* 
   for (int b = 0; b < nprob; b++) widths.push_back(kdt[keys[b]]);
   std::sort(widths.begin(), widths.end());
   widths.erase(std::unique(widths.begin(), widths.end()), widths.end());
+  if (cv)   // before any of the chunk's keys is solved
+    for (int b = 0; b < nprob; b++)
+      if (round_up(kdt[keys[b]], 32) > COV_MAX_WIDTH)
+        return fail(MLEASE_ERR_INVALID, "key " + std::to_string(keys[b]) + ": its posterior covariance needs the explicit inverse of a " +
+                                            std::to_string(kdt[keys[b]]) + "-column system (" + (kdt[keys[b]] == Dt ? "the global width" : "its own column space") +
+                                            "), which exists for at most " + std::to_string(COV_MAX_WIDTH) + " columns");
   DevMem sm;   // the sparse sink's slab
   Slab slab;
   if (sp) { if (int rc = open_slab(keys, nprob, cr, sm, &slab)) return rc; }
@@ -370,9 +434,22 @@ int KeyedFit::solve_chunk(const int* keys, int nprob, const ChunkRows& cr, int* 
   for (int w : widths) {
     group.clear();
     for (int b = 0; b < nprob; b++) if (kdt[keys[b]] == w) group.push_back(keys[b]);
-    if (int rc = solve_batch(group.data(), (int)group.size(), w, cr, dflag, hflag, sp ? &slab : nullptr)) return rc;
+    if (int rc = solve_group(group.data(), (int)group.size(), w, cr, dflag, hflag, sp ? &slab : nullptr)) return rc;
   }
   return sp ? write_slab(keys, nprob, slab) : 0;
+}
+
+// solve_batch; a covariance call's batch that would be matrix-free (its Hessians, factors and inverses do not fit the device) is
+// solved in halves instead
+int KeyedFit::solve_group(const int* keys, int nprob, int w, const ChunkRows& cr, int* dflag, int* hflag, Slab* sl) {
+  const int rc = solve_batch(keys, nprob, w, cr, dflag, hflag, sl);
+  if (rc != SPLIT_BATCH) return rc;
+  if (nprob == 1)
+    return fail(MLEASE_ERR_CUDA, "key " + std::to_string(keys[0]) + ": its Hessian, factor and inverse (" + std::to_string(w) +
+                                     " columns) do not fit the free device memory");
+  const int h = nprob / 2;
+  if (int r = solve_group(keys, h, w, cr, dflag, hflag, sl)) return r;
+  return solve_group(keys + h, nprob - h, w, cr, dflag, hflag, sl);
 }
 
 // The slab of the chunk keys[0, nprob) (ascending, fitted): each key's list length (from its column list, or for a key without one
@@ -407,6 +484,16 @@ int KeyedFit::open_slab(const int* keys, int nprob, const ChunkRows& cr, DevMem&
     for (int i = 0; i < nk; i++) if (sl->mrow[i] >= 0) sl->len[i] = count[sl->mrow[i]];
   }
   for (int i = 0; i < nk; i++) { sl->off[i] = sl->n; sl->n += sl->len[i]; }
+  if (cv && cv->val) {
+    // the lengths are fixed: the chunk's blocks must fit the room left, checked before the chunk writes anything
+    sl->coff.assign(nk, 0);
+    for (int i = 0; i < nk; i++) { sl->coff[i] = sl->ncov; sl->ncov += sl->len[i] * (sl->len[i] + 1) / 2; }
+    const long long need = cv->ptr[sp_key] + sl->ncov;
+    if (need > cv->cap)
+      return fail(MLEASE_ERR_INVALID, "cov_capacity " + std::to_string(cv->cap) + " is too small: the covariance blocks of keys 0 .. " +
+                                          std::to_string(keys[nprob - 1]) + " need " + std::to_string(need) + " entries");
+    if (int rc = mem.get(&sl->cov, (size_t)L * sl->ncov, false)) return rc;
+  }
   if (int rc = mem.get(&sl->model, (size_t)L * sl->n, false)) return rc;
   if (out_var) { if (int rc = mem.get(&sl->var, (size_t)L * sl->n, false)) return rc; }
   return mem.get(&sl->col, (size_t)sl->n, false);
@@ -420,9 +507,15 @@ int KeyedFit::write_slab(const int* keys, int nprob, const Slab& sl) {
     CK(cudaMemcpyAsync(out_model + l * sp->cap + e0, sl.model + l * sl.n, (size_t)sl.n * 8, cudaMemcpyDeviceToHost, st));
     if (out_var) CK(cudaMemcpyAsync(out_var + l * sp->cap + e0, sl.var + l * sl.n, (size_t)sl.n * 8, cudaMemcpyDeviceToHost, st));
   }
+  if (cv && cv->val)
+    for (int l = 0; l < L; l++)
+      CK(cudaMemcpyAsync(cv->val + l * cv->cap + cv->ptr[keys[0]], sl.cov + l * sl.ncov, (size_t)sl.ncov * 8, cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(sp->col + e0, sl.col, (size_t)sl.n * 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  for (int k = keys[0]; k <= keys[nprob - 1]; k++) sp->key_ptr[k + 1] = sp->key_ptr[k] + sl.len[k - sl.k0];
+  for (int k = keys[0]; k <= keys[nprob - 1]; k++) {
+    sp->key_ptr[k + 1] = sp->key_ptr[k] + sl.len[k - sl.k0];
+    if (cv && cv->val) cv->ptr[k + 1] = cv->ptr[k] + sl.len[k - sl.k0] * (sl.len[k - sl.k0] + 1) / 2;
+  }
   sp_key = keys[nprob - 1] + 1;
   return 0;
 }
@@ -459,9 +552,14 @@ int KeyedFit::solve_batch(const int* keys, int nprob, int w, const ChunkRows& cr
     row_start[b + 1] = row_start[b] + p.n;
   }
   if (int rc = batch_alloc(B, num_sms, 0)) return rc;
+  if (cv && B.matfree) return SPLIT_BATCH;   // the Hessians need the Gram path's Lc and Hinv
   DevMem ct;   // the batch's temporaries: freed with it, before the next batch_alloc
   double *dm, *dq, *dout = nullptr, *dim = nullptr, *dvec = nullptr; long long *drs = nullptr, *dspan = nullptr; unsigned char* dmask = nullptr;
   GatherJob* djobs = nullptr;
+  CovJob* dcjobs = nullptr;
+  int* dfail = nullptr;              // covariance: pivot failures of the batch's factorisations, all priors
+  PinnedMem cp;
+  Ctrl *factor_ctl = nullptr, *reset_ctl = nullptr;
   if (int rc = ct.get(&dm, (size_t)ldx, false)) return rc;
   if (int rc = ct.get(&dq, (size_t)ldx, false)) return rc;
   if (sl) {
@@ -475,7 +573,20 @@ int KeyedFit::solve_batch(const int* keys, int nprob, int w, const ChunkRows& cr
     }
     if (int rc = ct.get(&djobs, jobs.size(), false)) return rc;
     CK(cudaMemcpyAsync(djobs, jobs.data(), jobs.size() * sizeof(GatherJob), cudaMemcpyHostToDevice, st));
-    CK(cudaStreamSynchronize(st));   // jobs is released here
+    std::vector<CovJob> cjobs(cv ? B.nprob : 0);
+    for (size_t b = 0; b < cjobs.size(); b++) {
+      const int i = keys[b] - sl->k0;
+      cjobs[b] = CovJob{sl->off[i], cv->val ? sl->coff[i] : -1, (int)sl->len[i]};
+    }
+    if (cv) {
+      if (int rc = ct.get(&dfail, 1, true)) return rc;
+      if (int rc = cp.get(&factor_ctl, (size_t)B.nprob, true)) return rc;
+      if (int rc = cp.get(&reset_ctl, (size_t)B.nprob, true)) return rc;
+      for (int b = 0; b < B.nprob; b++) factor_ctl[b].need_hess = 1;
+      if (int rc = ct.get(&dcjobs, cjobs.size(), false)) return rc;
+      CK(cudaMemcpyAsync(dcjobs, cjobs.data(), cjobs.size() * sizeof(CovJob), cudaMemcpyHostToDevice, st));
+    }
+    CK(cudaStreamSynchronize(st));   // jobs and cjobs are released here
   } else {
     if (int rc = ct.get(&dout, (size_t)B.nprob * w, false)) return rc;
   }
@@ -523,7 +634,9 @@ int KeyedFit::solve_batch(const int* keys, int nprob, int w, const ChunkRows& cr
       sparse_gather_kernel<<<B.nprob, GATHER_THREADS, 0, st>>>(B.d, djobs, kcols, sl->mask, local ? 1 : 0, Dg, B.has_bias, 0,
                                                                sl->model + l * sl->n, l == 0 ? sl->col : nullptr);
       CK(cudaGetLastError());
-      if (out_var) {
+      if (cv) {
+        if (int rc = posterior_cov(B, local, drs, row_start[B.nprob], dvec, dcjobs, sl, l, dfail, factor_ctl, reset_ctl)) return rc;
+      } else if (out_var) {
         CK(postvar_rowweights(B.d, B.nprob, drs, row_start[B.nprob], B.has_bias, dvec, st, nullptr));
         CK(postvar_diag(B.d, B.nprob, drs, row_start[B.nprob], dvec, B.has_bias, st, nullptr));
         sparse_gather_kernel<<<B.nprob, GATHER_THREADS, 0, st>>>(B.d, djobs, kcols, sl->mask, local ? 1 : 0, Dg, B.has_bias, 1,
@@ -555,6 +668,32 @@ int KeyedFit::solve_batch(const int* keys, int nprob, int w, const ChunkRows& cr
       }
     }
   }
+  if (dfail) {
+    int bad = 0;
+    CK(cudaMemcpyAsync(&bad, dfail, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (bad) return fail(MLEASE_ERR_NUMERIC, "Model fitting error! (Hessian not positive definite in " + std::to_string(bad) + " fit(s))");
+  }
+  return 0;
+}
+
+// The full posterior of prior l's fits, the batch's x-update just done (llf/LibLinear.java:315-326): row weights at each fit, the
+// exact Hessians into Lc, K3's factorisation without prep and its explicit inverse, then the variances and covariance blocks over
+// each key's list into the slab.  The control blocks are left as reset_ctrl leaves them: no factor, so the next prior's x-update
+// rebuilds from its start point exactly as after the sparse call's diagonal variance (the fits do not change).
+// The pivot failures are counted on the device into dfail, which the batch reads once after its last prior; factor / reset: the
+// control blocks before the factorisation (need_hess = 1) and after it (zero), pinned so that the copies stay asynchronous.
+int KeyedFit::posterior_cov(Batch& B, bool local, const long long* drs, long long nrows, double* dvec, const CovJob* dcjobs, Slab* sl, int l,
+                            int* dfail, const Ctrl* factor, const Ctrl* reset) {
+  CK(postvar_rowweights(B.d, B.nprob, drs, nrows, B.has_bias, dvec, st, nullptr));
+  CK(postvar_hessian_batch(B.d, B.nprob, B.ldh, drs, dvec, B.has_bias, st, nullptr));
+  CK(cudaMemcpyAsync(B.d_ctrl, factor, (size_t)B.nprob * sizeof(Ctrl), cudaMemcpyHostToDevice, st));
+  CK(cholesky_launch(B.d, B.nprob, B.ldh, st, nullptr, 0, 1, 1));
+  cov_gather_kernel<<<B.nprob, 256, 0, st>>>(B.d, dcjobs, local ? 1 : 0, sl->col, sl->var + l * sl->n, cv->val ? sl->cov + l * sl->ncov : nullptr);
+  cov_fail_kernel<<<1, 256, 0, st>>>(B.d, B.nprob, dfail);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(B.d_ctrl, reset, (size_t)B.nprob * sizeof(Ctrl), cudaMemcpyHostToDevice, st));
+  B.mirror.clear();
   return 0;
 }
 
@@ -562,9 +701,9 @@ int KeyedFit::solve_batch(const int* keys, int nprob, int w, const ChunkRows& cr
 int keyed_fit(int num_sms, cudaStream_t st, int32_t K, int32_t Dg, const int64_t* key_rowstart, const int64_t* rowptr, const int32_t* colidx,
               const float* vals, int64_t ldx_in, const int32_t* response, const float* weight, const float* offset, bool has_intercept,
               int32_t data_size_threshold, int32_t binary_feature, const std::vector<KeyedPrior>& priors, const double* intercept_mean,
-              double* out_model, double* out_var, int32_t* skipped, const SparseOut* sp) {
+              double* out_model, double* out_var, int32_t* skipped, const SparseOut* sp, const CovOut* cv = nullptr) {
   KeyedFit f{num_sms, st, K, Dg, key_rowstart, rowptr, colidx, vals, ldx_in, response, weight, offset, has_intercept, data_size_threshold,
-             binary_feature, priors, intercept_mean, out_model, out_var, skipped, sp};
+             binary_feature, priors, intercept_mean, out_model, out_var, skipped, sp, cv};
   return f.run();
 }
 // host copy of a host-or-device array (NULL -> empty)
@@ -611,13 +750,14 @@ int naive_train(int32_t device, void* stream, int32_t K, int32_t Dg, const int64
 
 // ------------------------------------------------------------------------------------------
 // ItemModelTrain (jobs/ItemModelTrain.java:226-276): per key, one fit per (intercept lambda, default lambda) in config order, the
-// intercept's prior mean the key's own; diagonal posterior variance on request.  Dense outputs, or (sp) the sparse lists
+// intercept's prior mean the key's own; diagonal posterior variance on request.  Dense outputs, or (sp) the sparse lists, with (cv)
+// the full posterior
 // ------------------------------------------------------------------------------------------
 int item_model_train(int32_t device, void* stream, int32_t K, int32_t Dg, const int64_t* key_rowstart, const int64_t* rowptr,
                      const int32_t* colidx, const float* vals, const int32_t* response, const float* weight, const float* offset,
                      const double* intercept_prior_mean, int32_t IL, const float* intercept_lambdas, int32_t DL,
                      const float* default_lambdas, const float* lambda_map, int32_t binary_feature, int32_t compute_var,
-                     double* out_model, double* out_var, const SparseOut* sp) {
+                     double* out_model, double* out_var, const SparseOut* sp, const CovOut* cv = nullptr) {
   int num_sms = 0;
   if (int rc = keyed_fit_check(device, Dg, rowptr, colidx, 0, binary_feature, &num_sms)) return rc;
   std::vector<float> lm, il, dl;
@@ -642,7 +782,7 @@ int item_model_train(int32_t device, void* stream, int32_t K, int32_t Dg, const 
       q[Dg] = 1.0 / (1.0 / (double)il[a]);
     }
   return keyed_fit(num_sms, (cudaStream_t)stream, K, Dg, key_rowstart, rowptr, colidx, vals, 0, response, weight, offset, true, 0, binary_feature,
-                   priors, im.data(), out_model, compute_var ? out_var : nullptr, nullptr, sp);
+                   priors, im.data(), out_model, compute_var ? out_var : nullptr, nullptr, sp, cv);
 }
 }  // namespace
 
@@ -694,6 +834,22 @@ int mlease_item_model_train_sparse(int32_t device, void* stream, int32_t K, int3
   const SparseOut sp{capacity, out_key_ptr, out_col};
   return item_model_train(device, stream, K, Dg, key_rowstart, rowptr, colidx, vals, response, weight, offset, intercept_prior_mean, IL,
                           intercept_lambdas, DL, default_lambdas, lambda_map, binary_feature, compute_var, out_model, out_var, &sp);
+}
+
+int mlease_item_model_train_cov(int32_t device, void* stream, int32_t K, int32_t Dg, const int64_t* key_rowstart, const int64_t* rowptr,
+                                const int32_t* colidx, const float* vals, const int32_t* response, const float* weight, const float* offset,
+                                const double* intercept_prior_mean, int32_t IL, const float* intercept_lambdas, int32_t DL,
+                                const float* default_lambdas, const float* lambda_map, int32_t binary_feature, int64_t capacity,
+                                int64_t* out_key_ptr, int32_t* out_col, double* out_model, double* out_var, int64_t cov_capacity,
+                                int64_t* out_cov_ptr, double* out_cov) {
+  if (K <= 0 || Dg <= 0 || IL <= 0 || DL <= 0 || !intercept_lambdas || !default_lambdas || !key_rowstart || !rowptr || !colidx || !vals ||
+      !response || !intercept_prior_mean || capacity < 0 || !out_key_ptr || !out_col || !out_model || !out_var ||
+      (out_cov && (cov_capacity < 0 || !out_cov_ptr)))
+    return fail(MLEASE_ERR_INVALID, "bad argument");
+  const SparseOut sp{capacity, out_key_ptr, out_col};
+  const CovOut cv{cov_capacity, out_cov ? out_cov_ptr : nullptr, out_cov};
+  return item_model_train(device, stream, K, Dg, key_rowstart, rowptr, colidx, vals, response, weight, offset, intercept_prior_mean, IL,
+                          intercept_lambdas, DL, default_lambdas, lambda_map, binary_feature, 1, out_model, out_var, &sp, &cv);
 }
 
 int mlease_naive_train_dense(int32_t device, void* stream, int32_t K, int32_t Dg, const int64_t* key_rowstart, const float* X, int64_t ldx_in,

@@ -445,6 +445,29 @@ def score_keyed_var(vals, key_rowstart, rowptr, colidx, num_features, model_ptr,
     return pred, pred_var
 
 
+def score_keyed_cov(vals, key_rowstart, rowptr, colidx, num_features, model_ptr, model_col, model_val, cov_ptr, cov_val, var_default, *,
+                    lambda_map=None, offset=None, binary_feature=False, device=0, stream=None, out=None, out_var=None):
+    """score_keyed with each record's predictive variance under the full posterior of its model (mlease_score_keyed_cov): model m's
+    covariance is cov_val[cov_ptr[m]:cov_ptr[m+1]], the packed lower triangle of Sigma over its model_col list (keyed_cov_for_scoring
+    orders item_model_train_cov's blocks so), or empty (NaN pred_var).  Unlisted columns: 1 / lambda_map[c] where > 0, else
+    var_default[m].  Rows must list strictly ascending columns.  -> (pred [G, nrows] float32, pred_var [G, nrows] float32)."""
+    krs, rp, ci, vals = _keep(key_rowstart, np.int64), _keep(rowptr, np.int64), _keep(colidx, np.int32), _keep(vals, np.float32)
+    mp, mc, mv = _keep(model_ptr, np.int64), _keep(model_col, np.int32), _keep(model_val, np.float32)
+    cp, cv, vd, lm = _keep(cov_ptr, np.int64), _keep(cov_val, np.float64), _keep(var_default, np.float32), _keep(lambda_map, np.float32)
+    K = len(krs) - 1
+    if K <= 0 or (len(mp) - 1) % K or len(cp) != len(mp) or len(vd) != len(mp) - 1:
+        raise ValueError("model_ptr and cov_ptr must hold G * num_keys + 1 entries, var_default G * num_keys")
+    G = (len(mp) - 1) // K
+    n = len(rp) - 1
+    o = _keep(offset, np.float32)
+    pred = np.zeros((G, n), np.float32) if out is None else out
+    pred_var = np.zeros((G, n), np.float32) if out_var is None else out_var
+    check(lib().mlease_score_keyed_cov(device, stream, int(num_features), K, ptr(krs), ptr(rp), ptr(ci), ptr(vals), ptr(o), G, ptr(mp),
+                                       ptr(mc), ptr(mv), ptr(cp), ptr(cv), ptr(lm), ptr(vd), int(bool(binary_feature)), ptr(pred),
+                                       ptr(pred_var)))
+    return pred, pred_var
+
+
 def test_loglik_keyed(entry_key, entry_group, response, pred, num_keys, weight=None, device=0, stream=None):
     """ItemModelTestLoglik (jobs/ItemModelTestLoglik.java:60-142): one entry per (record, pred-map key), combiner group per entry
     (non-decreasing) -> (float32 loglik [num_keys], float64 count [num_keys])."""
@@ -598,6 +621,72 @@ def item_model_train_sparse(vals, key_rowstart, response, intercept_lambdas, def
     shape = (len(il), len(dl), n)
     return (key_ptr, cols[:n].copy(), models[:, :n].reshape(shape).copy(),
             None if var is None else var[:, :n].reshape(shape).copy())
+
+
+def _list_lengths(key_rowstart, rowptr, colidx, num_features):
+    """each key's list length on the host: its distinct columns + 1 for the intercept, 0 for a key without rows"""
+    krs, rp, ci = _host(key_rowstart, np.int64), _host(rowptr, np.int64), _host(colidx, np.int64)
+    K = len(krs) - 1
+    rows = np.diff(krs)
+    row_key = np.repeat(np.arange(K, dtype=np.int64), rows)
+    entry_key = np.repeat(row_key, np.diff(rp[krs[0]:krs[-1] + 1]))
+    pairs = np.unique(entry_key * (int(num_features) + 1) + ci[rp[krs[0]]:rp[krs[-1]]])
+    distinct = np.bincount(pairs // (int(num_features) + 1), minlength=K)
+    return np.where(rows > 0, distinct + 1, 0).astype(np.int64)
+
+
+def item_model_train_cov(vals, key_rowstart, response, intercept_lambdas, default_lambdas, *, rowptr, colidx, num_features,
+                         intercept_prior_mean=None, weight=None, offset=None, lambda_map=None, binary_feature=False, want_cov=True,
+                         device=0, stream=None, capacity=None, cov_capacity=None):
+    """item_model_train_sparse with the full posterior of every fit (mlease_item_model_train_cov): var is diag(Sigma), Sigma the
+    inverse of the key's exact Hessian at its fit, over its list; key k's covariance block is cov[..., cov_ptr[k]:cov_ptr[k+1]], the
+    lower triangle of Sigma over the list's order, row-major (entry (a, b), a >= b, at cov_ptr[k] + a(a+1)/2 + b).  Rows must list
+    strictly ascending columns.  The blocks are allocated at their exact sizes, from each key's distinct columns (cov_capacity
+    overrides that).  want_cov = False: the variances only (cov_ptr and cov None).
+    -> (key_ptr [K+1] int64, cols [n] int32, models [IL, DL, n], var [IL, DL, n], cov_ptr [K+1] int64, cov [IL, DL, m] float64)."""
+    krs = np.ascontiguousarray(key_rowstart, np.int64)
+    K, D = len(krs) - 1, int(num_features)
+    il, dl = _f32(np.atleast_1d(intercept_lambdas)), _f32(np.atleast_1d(default_lambdas))
+    rp, ci, vals = _keep(rowptr, np.int64), _keep(colidx, np.int32), _keep(vals, np.float32)
+    r, w, o, lm = _keep(response, np.int32), _keep(weight, np.float32), _keep(offset, np.float32), _keep(lambda_map, np.float32)
+    im = np.zeros(K, np.float64) if intercept_prior_mean is None else np.ascontiguousarray(intercept_prior_mean, np.float64)
+    if len(im) != K:
+        raise ValueError("intercept_prior_mean must hold one entry per key")
+    cap = _list_capacity(krs, rp, D, np.diff(krs) > 0, True) if capacity is None else int(capacity)
+    if want_cov and cov_capacity is None:
+        n_k = _list_lengths(krs, rp, ci, D)
+        cov_capacity = int((n_k * (n_k + 1) // 2).sum())
+    ccap = int(cov_capacity) if want_cov else 0
+    G = len(il) * len(dl)
+    key_ptr = np.zeros(K + 1, np.int64)
+    cols = np.zeros(max(cap, 1), np.int32)
+    models = np.zeros((G, max(cap, 1)), np.float64)
+    var = np.zeros_like(models)
+    cov_ptr = np.zeros(K + 1, np.int64) if want_cov else None
+    cov = np.zeros((G, max(ccap, 1)), np.float64) if want_cov else None
+    check(lib().mlease_item_model_train_cov(device, stream, K, D, ptr(krs), ptr(rp), ptr(ci), ptr(vals), ptr(r), ptr(w), ptr(o), ptr(im),
+                                            len(il), ptr(il), len(dl), ptr(dl), ptr(lm), int(bool(binary_feature)), cap, ptr(key_ptr),
+                                            ptr(cols), ptr(models), ptr(var), ccap, ptr(cov_ptr), ptr(cov)))
+    n = int(key_ptr[K])
+    shape = (len(il), len(dl), n)
+    out = (key_ptr, cols[:n].copy(), models[:, :n].reshape(shape).copy(), var[:, :n].reshape(shape).copy())
+    if not want_cov:
+        return out + (None, None)
+    m = int(cov_ptr[K])
+    cov = cov.reshape((len(il), len(dl), -1))   # a view; the blocks can be gigabytes, so trim by copying only when over-allocated
+    return out + (cov_ptr, cov if cov.shape[-1] == m else cov[..., :m].copy())
+
+
+def keyed_cov_for_scoring(key_ptr, cov_ptr, cov):
+    """item_model_train_cov's blocks in the (prior, key) order score_keyed_cov takes them, the order keyed_models_for_scoring gives
+    the models: model m = p * K + k is key k's block with prior p's values (cov [..., m_total], the priors flattened in order).
+    -> (cov_ptr [P*K+1] int64, cov_val float64)."""
+    cp = np.ascontiguousarray(cov_ptr, np.int64)
+    m = int(cp[-1])
+    cov = np.asarray(cov, np.float64)
+    P = int(np.prod(cov.shape[:-1]))
+    ptrs = np.concatenate([[0], (cp[1:][None, :] + m * np.arange(P, dtype=np.int64)[:, None]).reshape(-1)]).astype(np.int64)
+    return ptrs, np.ascontiguousarray(cov.reshape(P, m)).reshape(-1)
 
 
 def keyed_models_for_scoring(key_ptr, cols, models):
