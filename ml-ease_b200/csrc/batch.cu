@@ -45,34 +45,32 @@ static double gram_path_bytes(const Batch& B) {
   return bytes;
 }
 
-// Cost of one CSR Gram build of a partition (seconds; only the comparison matters).  Both kernels read each 128-column block's
-// run of every 32-row group once per tile it belongs to (nblk + 1 tiles: `reads` entries in all).  wgmma: every 128 x 128 lower
-// tile times every 32-row group on the tensor pipe, plus the producers' run loads, which is what makes its rate fall at small n
-// and high density.  Sparse: per product (integer multiply + native shared atomic add), per (tile, span) visit (gram_sparse_span
-// groups: fetching the span's two bounds per block) and per entry read (loading its pre-decoded word and staging or scanning it),
-// with the whole device busy; a grid of fewer CTAs than SMs is that much slower.  Relative least-squares fits of
-// tools/time_gram.py (REPS=3) over 0.3 - 20 % density at 10k features (DESIGN.md section 4): the wgmma constants on an H100 80GB
-// HBM3 at a 400 W power limit, the sparse ones, refitted for the one-word operand, on an H100 80GB HBM3 at a 700 W power limit
-// (the wgmma times there are within 3.5 % of the 400 W ones).  The sparse model is within 2.5 % and the wgmma model within 9.5 %
-// of every measured shape, so near the crossover (~3 % at 10k features) the rule may pick a kernel up to ~10 % slower than the
-// other.
+// Cost of one CSR Gram build of a partition (seconds; only the comparison matters).  wgmma: every 128 x 128 lower tile times every
+// 32-row group on the tensor pipe, plus the producers' run loads (each 128-column block's run of every 32-row group is read once per
+// tile it belongs to: nblk + 1 tiles, `reads` entries in all), which is what makes its rate fall at small n and high density.
+// Sparse (column kernel): per product (a suffix word loaded and multiplied, one native shared atomic add), per entry (one position
+// of the column index, the first run of its suffix loaded) and per cell of the lower triangle (each column's clear and epilogue:
+// one rounding and one strided store a cell), with the whole device busy; a grid of fewer CTAs than two an SM is that much slower.
+// Relative least-squares fits of tools/time_gram.py (REPS=3) over 0.3 - 20 % density at 10k features (DESIGN.md section 4): the
+// wgmma constants on an H100 80GB HBM3 at a 400 W power limit, the sparse ones on an H100 80GB HBM3 at a 700 W power limit (the
+// wgmma times there are within 3.5 % of the 400 W ones).  The sparse model is within 10.2 % and the wgmma model within 9.5 % of every
+// measured shape, so near the crossover (~3 % at 10k features) the rule may pick a kernel up to ~10 % slower than the other.
 constexpr double GRAM_WGMMA_S_PER_MAC = 1.317e-15, GRAM_WGMMA_S_PER_READ = 4.315e-12;
-constexpr double GRAM_SPARSE_S_PER_PAIR = 1.808e-12, GRAM_SPARSE_S_PER_VISIT = 2.548e-10, GRAM_SPARSE_S_PER_READ = 2.915e-12;
-static double gram_cost(const Problem& p, int Dp, int kind, double ctas, int num_sms) {
+constexpr double GRAM_SPARSE_S_PER_PAIR = 3.084e-12, GRAM_SPARSE_S_PER_ENTRY = 1.174e-10, GRAM_SPARSE_S_PER_CELL = 5.048e-13;
+static double gram_cost(const Problem& p, int Dp, int kind, int num_sms) {
   const double nblk = Dp / 128, tiles = nblk * (nblk + 1) / 2, groups = (double)((p.n + 31) / 32);
-  const int span = gram_sparse_span(p.bm_entries, Dp / 128, (p.n + 31) / 32);
-  const double spans = (double)(((p.n + 31) / 32 + span - 1) / span);
-  const double reads = (nblk + 1) * (double)p.bm_entries;
-  if (kind == CSR_GRAM_WGMMA) return tiles * 128.0 * 128.0 * 32.0 * groups * GRAM_WGMMA_S_PER_MAC + reads * GRAM_WGMMA_S_PER_READ;
-  return (p.gram_pairs * GRAM_SPARSE_S_PER_PAIR + tiles * spans * GRAM_SPARSE_S_PER_VISIT + reads * GRAM_SPARSE_S_PER_READ) *
-         std::max(1.0, num_sms / std::max(1.0, ctas));
+  if (kind == CSR_GRAM_WGMMA)
+    return tiles * 128.0 * 128.0 * 32.0 * groups * GRAM_WGMMA_S_PER_MAC + (nblk + 1) * (double)p.bm_entries * GRAM_WGMMA_S_PER_READ;
+  const double ctas = std::min(Dp, 2 * num_sms);   // gram_launch_csr_sparse's grid per problem
+  return (p.gram_pairs * GRAM_SPARSE_S_PER_PAIR + (double)p.bm_entries * GRAM_SPARSE_S_PER_ENTRY +
+          0.5 * Dp * (Dp + 1.0) * GRAM_SPARSE_S_PER_CELL) * std::max(1.0, 2.0 * num_sms / ctas);
 }
 
 // Allocate the per-problem solver state.  Data pointers (X, y, ...) and n must be filled in h[] first.
 // hessian_policy 2 builds the batch matrix-free (Newton-CG on Hv passes, O(D') state per problem); with any other policy the batch
 // is built matrix-free when what the Gram path would allocate exceeds the free device memory (it could not run at all).
 // CSR Gram batches pick their kernel from the data: the sparse kernel when its cost model is lower and every partition is within
-// its row limit (gram_sparse_max_rows), else the wgmma kernel.  csr_gram_force (a test hook's setting) overrides the choice.
+// its row and column limits (gram_sparse_max_rows, gram_sparse_max_cols), else the wgmma kernel.  csr_gram_force (a test hook's setting) overrides the choice.
 int batch_alloc(Batch& B, int num_sms, int hessian_policy, int csr_gram_force) {
   const int nprob = B.nprob, ldx = B.ldx;
   B.Dp = round_up(B.ldx, 128);
@@ -120,16 +118,20 @@ int batch_alloc(Batch& B, int num_sms, int hessian_policy, int csr_gram_force) {
   B.csr_gram = 0;
   if (B.gram_from_csr && !B.matfree) {
     double t_sparse = 0, t_wgmma = 0;
-    bool fits = true;
-    const double nblk = B.Dp / 128, ctas = nblk * (nblk + 1) / 2 * nprob;   // the sparse kernel's grid: one CTA per (tile, problem)
+    // the upload builds the sparse kernel's column index wherever both of its limits hold
+    bool rows_fit = true, indexed = true;
     for (auto& p : B.h) {
-      t_sparse += gram_cost(p, B.Dp, CSR_GRAM_SPARSE, ctas, num_sms);
-      t_wgmma += gram_cost(p, B.Dp, CSR_GRAM_WGMMA, ctas, num_sms);
-      if (p.n > gram_sparse_max_rows()) fits = false;
+      t_sparse += gram_cost(p, B.Dp, CSR_GRAM_SPARSE, num_sms);
+      t_wgmma += gram_cost(p, B.Dp, CSR_GRAM_WGMMA, num_sms);
+      if (p.n > gram_sparse_max_rows()) rows_fit = false;
+      if (!p.gc_pos) indexed = false;
     }
+    const bool fits = rows_fit && indexed && B.Dt <= gram_sparse_max_cols();
     B.csr_gram = (fits && t_sparse < t_wgmma) ? CSR_GRAM_SPARSE : CSR_GRAM_WGMMA;
-    if (csr_gram_force == CSR_GRAM_SPARSE && !fits)
+    if (csr_gram_force == CSR_GRAM_SPARSE && !rows_fit)
       return fail(MLEASE_ERR_INVALID, "the sparse CSR Gram's int64 sums hold at most 2^27 rows per partition");
+    if (csr_gram_force == CSR_GRAM_SPARSE && !fits)
+      return fail(MLEASE_ERR_INVALID, "the sparse CSR Gram's operand word holds column ids below 2^20 (features + intercept)");
     if (csr_gram_force) B.csr_gram = csr_gram_force;
   }
   if (!B.matfree && B.csr && B.gram_from_csr) {
@@ -155,12 +157,13 @@ int batch_alloc(Batch& B, int num_sms, int hessian_policy, int csr_gram_force) {
     // flop-bound, and a mid-update rebuild saves them many lock-step slots
     B.rebuild_is_expensive = (t_rebuild > 8.0 * t_pass && B.Dt > 2048 && !B.matfree) ? 1 : 0;
   }
-  // Gram decomposition
+  // Gram decomposition (the sparse kernel walks columns: no tiles)
   constexpr int MAX_TILES = 1 << 18;   // lower 128x128 tiles of Dp up to ~90k
-  std::vector<short> tiles(B.matfree ? 2 : 2 * (size_t)MAX_TILES);
-  B.ntiles = B.matfree ? 0 : gram_tile_list(B.Dp, tiles.data(), MAX_TILES, B.csr_gram == CSR_GRAM_SPARSE ? 2 : B.gram_from_csr);
-  if (B.ntiles <= 0 && !B.matfree) return fail(MLEASE_ERR_INVALID, "Gram tile list overflow");
-  if (!B.matfree && B.csr_gram != CSR_GRAM_SPARSE) {   // the sparse kernel has no split-K: one slice
+  const bool tiled = !B.matfree && B.csr_gram != CSR_GRAM_SPARSE;
+  std::vector<short> tiles(tiled ? 2 * (size_t)MAX_TILES : 2);
+  B.ntiles = tiled ? gram_tile_list(B.Dp, tiles.data(), MAX_TILES, B.gram_from_csr) : 0;
+  if (B.ntiles <= 0 && tiled) return fail(MLEASE_ERR_INVALID, "Gram tile list overflow");
+  if (tiled) {   // the sparse kernel has no split-K: one slice
     const long long ksteps = (maxn + 63) / 64;
     const long long base = (long long)B.ntiles * nprob;   // CTAs
     const long long cap = std::max(1, num_sms);
@@ -277,7 +280,7 @@ int batch_alloc(Batch& B, int num_sms, int hessian_policy, int csr_gram_force) {
 
 // One Gram build of the problems d_probs[0 .. n) with the batch's kernel (force / share: see gram_wgmma_kernel)
 cudaError_t batch_gram(const Batch& B, const Problem* d_probs, int n, int force, cudaStream_t st, int* launches, int share) {
-  if (B.csr_gram == CSR_GRAM_SPARSE) return gram_launch_csr_sparse(d_probs, n, B.d_tiles, B.ntiles, force, st, launches, share);
+  if (B.csr_gram == CSR_GRAM_SPARSE) return gram_launch_csr_sparse(d_probs, n, B.Dp, force, st, launches, share);
   if (B.gram_from_csr) return gram_launch_csr_wgmma(d_probs, n, B.d_tiles, B.ntiles, B.gram_slices, force, st, launches, share);
   return gram_launch_wgmma(d_probs, n, B.d_tmaps, B.d_tiles, B.ntiles, B.gram_slices, force, st, launches, share);
 }

@@ -99,8 +99,11 @@ struct Problem {
   long long bm_entries;           // entries of the list: nnz + n (one bias entry per row)
   unsigned char* bm_e4m3;         // [bm_entries] this problem's Gram operand, e4m3(value * sqrt(d_row) * gram_scale), written by
                                   // gram_csr_operand_kernel before every CSR Gram build (per problem: the list is shared, sdvec is not)
-  uint32_t* bm_word;              // [bm_entries] the same operand for the sparse CSR Gram, pre-decoded (k2_gram.cu sparse_word);
-                                  // a batch has one of the two forms (bm_e4m3 for CSR_GRAM_WGMMA, bm_word for CSR_GRAM_SPARSE)
+  uint32_t* bm_word;              // [bm_entries] the same operand values for the sparse CSR Gram in ROW order (row r at
+                                  // [rowptr[r] + r, rowptr[r + 1] + r], its intercept entry last), pre-decoded (k2_gram.cu
+                                  // gram_word); a batch has one of the two forms (bm_e4m3 for CSR_GRAM_WGMMA, bm_word for CSR_GRAM_SPARSE)
+  const uint32_t* gc_offs;        // [Dt + 1] column index of the sparse CSR Gram: column c's entries are at the positions
+  const uint32_t* gc_pos;         // gc_pos[gc_offs[c] .. gc_offs[c + 1]) of bm_word, ascending (NULL where that kernel cannot run)
   float vmax, wmax;               // max |stored value| and max record weight of the partition (fixed-point scale of the CSR K1)
   int nblk128;             // number of 128-column blocks (Dp / 128)
   // fused multi-lambda CSR K1 (k1_csr_fused.cu): the partition's rows cut into sg_S segments of sg_rows rows; per segment the

@@ -211,6 +211,7 @@ int csr_build_layout(mlease_session* s, PartData& pd) {
   // the Gram producers index the entry list with 32 bits; the list holds one bias entry per row (session batches always have the
   // intercept, column Dg)
   // A matrix-free session (hessian_policy 2) builds no Gram, so it skips the block-major list (n D'/512 offsets + 6 B per entry)
+  // and the column index of the sparse Gram (4 B per entry)
   if (d.csr_unique && nnz + nrows < (1LL << 32) - 64 && s->cfg.hessian_policy != 2) {
     d.nblk128 = round_up(s->ldx, 128) / 128;
     d.bm_groups = (nrows + 31) / 32;
@@ -223,6 +224,14 @@ int csr_build_layout(mlease_session* s, PartData& pd) {
     CK(csr_bm_fill(nrows, d.rowptr, d.colidx, d.vals, s->Dg, d.nblk128, d.bm_groups, bo, bk, bv, s->stream));
     d.bm_offs = bo; d.bm_keys = bk; d.bm_vals = bv;
     d.gram_pairs = (double)pairs;   // products of one sparse Gram build (the kernel choice of batch_alloc)
+    // the sparse Gram's column index (4 B per entry), only where that kernel can run
+    if (nrows <= gram_sparse_max_rows() && s->Dt <= gram_sparse_max_cols()) {
+      uint32_t *co, *cp;
+      if (int rc = s->mem.get(&co, (size_t)s->Dt + 1, true)) return rc;
+      if (int rc = s->mem.get(&cp, (size_t)d.bm_entries, true)) return rc;
+      CK(csr_col_index(nrows, d.rowptr, d.colidx, s->Dg, d.bm_entries, co, cp, s->stream));
+      d.gc_offs = co; d.gc_pos = cp;
+    }
   }
   if (d.csr_unique && nnz + nrows < (1LL << 32) - 64) {
     // segment lists of the fused multi-lambda K1

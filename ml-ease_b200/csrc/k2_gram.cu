@@ -15,9 +15,8 @@
 // each issuing m64n256k16 wgmma for its 64 rows of the tile (128 fp32 accumulators a thread).
 //
 // CSR partitions have two kernels on the same e4m3 operand values: gram_csr_wgmma_kernel (operand blocks assembled in shared
-// memory, wgmma; one byte an entry) and gram_csr_sparse_kernel (only the nonzero products of each row, exact int64 sums; one
-// pre-decoded 32-bit word an entry).  session.cu batch_alloc
-// picks one per batch from the data: the sparse one wins below about 3 % density at 10k features.
+// memory, wgmma; one byte an entry) and gram_csr_column_kernel (only the nonzero products of each row, column by column, exact
+// int64 sums; one pre-decoded 32-bit word an entry, in row order).  batch.cu batch_alloc picks one per batch from the data.
 //
 // A fp32 SIMT kernel computing the same partials from the same bf16 operand is kept ONLY as a
 // debug cross-check reachable through mlease_objective(tensor=0); the product path never uses it.
@@ -25,6 +24,7 @@
 #include <cuda_fp8.h>
 
 #include <algorithm>
+#include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
 #include "kernels.cuh"
@@ -373,44 +373,57 @@ __device__ __forceinline__ int e4m3_units(uint32_t b) {
   return (b & 0x80u) ? -mag : mag;
 }
 
-// The sparse kernel's operand word of an entry: everything it needs, decoded once per build instead of once per tile reading it.
-// The e4m3 value in units of 2^-9 is an integer of at most 4 significant bits below 2^18, so as an fp32 its low 20 mantissa bits
-// are zero; the low 15 carry the entry's row in its span (8 bits: 32 (group mod span) + row in group) and column in its 128-block
-// (7 bits).  Bits 15 .. 19 stay zero.  Decoding is a mask and one float-to-int conversion, a shift and two masks.
-constexpr uint32_t SW_VALUE_MASK = 0xFFFF8000u;
-__device__ __forceinline__ uint32_t sparse_word(uint32_t byte, int row_in_span, int col) {
-  return __float_as_uint((float)e4m3_units(byte)) | ((uint32_t)row_in_span << 7) | (uint32_t)col;
-}
-__device__ __forceinline__ int sw_units(uint32_t w) { return __float2int_rz(__uint_as_float(w & SW_VALUE_MASK)); }
-__device__ __forceinline__ int sw_row(uint32_t w) { return (int)((w >> 7) & 255u); }
-__device__ __forceinline__ int sw_col(uint32_t w) { return (int)(w & 127u); }
+// The sparse kernel's operand word of an entry of the row-order operand: the e4m3 value in units of 2^-9 is an integer of at most
+// 4 significant bits below 2^18, so as an fp32 its low 20 mantissa bits are zero; they carry the entry's column (D' <= 2^20, which
+// the batch rule checks).  Decoding is a mask and one float-to-int conversion, and a mask.
+constexpr uint32_t GW_VALUE_MASK = 0xFFF00000u, GW_COL_MASK = 0x000FFFFFu;
+__device__ __forceinline__ uint32_t gram_word(uint32_t byte, int col) { return __float_as_uint((float)e4m3_units(byte)) | (uint32_t)col; }
+__device__ __forceinline__ int gw_units(uint32_t w) { return __float2int_rz(__uint_as_float(w & GW_VALUE_MASK)); }
+__device__ __forceinline__ int gw_col(uint32_t w) { return (int)(w & GW_COL_MASK); }
 
-// Gram operand of the CSR kernels, once per build: for every entry of the block-major list, the e4m3 byte
-// e4m3(value * (sqrt(d_row) * gram_scale)), or for a sparse-kernel batch (csr_gram == CSR_GRAM_SPARSE) the same value as
-// sparse_word.  gram_scale is a power of two that keeps sqrt(d) x in e4m3's normal range (chol_prep undoes it exactly).  sdvec
-// is rewritten by K1 between builds, so this runs immediately before each build, gated like it.
-// One warp per 32-row group: lane l holds sqrt(d) of row 32 g + l, and the group's runs of every column block follow.
+// Gram operand of the CSR kernels, once per build: e4m3(value * (sqrt(d_row) * gram_scale)).  gram_scale is a power of two that
+// keeps sqrt(d) x in e4m3's normal range (chol_prep undoes it exactly).  sdvec is rewritten by K1 between builds, so this runs
+// immediately before each build, gated like it.
+// wgmma batches: the byte of every entry of the block-major list, one warp per 32-row group (lane l holds sqrt(d) of row 32 g + l,
+// and the group's runs of every column block follow).  Sparse batches (csr_gram == CSR_GRAM_SPARSE): the gram_word of every entry
+// in row order, one warp per row: row r's entries at [rowptr[r] + r, rowptr[r + 1] + r), then its intercept entry (value 1,
+// column Dt - 1), so every row ends with the word of the intercept.
 __global__ void __launch_bounds__(256) gram_csr_operand_kernel(const Problem* __restrict__ probs, int force, int share) {
   if (share > 1 && blockIdx.y % share != 0) return;   // see gram_wgmma_kernel
   const Problem& pb = probs[blockIdx.y];
   const Ctrl* ctrl = pb.ctrl;
   if (!force && (ctrl->done || !ctrl->need_hess)) return;
   const int lane = threadIdx.x & 31;
-  const long long n = pb.n, ngroups = pb.bm_groups;
+  const long long n = pb.n;
+  const float gscale = pb.gram_scale;
+  const long long nw = ((long long)gridDim.x * blockDim.x) >> 5;
+  const long long w0 = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (pb.csr_gram == CSR_GRAM_SPARSE) {
+    const long long* __restrict__ rowptr = pb.rowptr;
+    const int* __restrict__ colidx = pb.colidx;
+    const float* __restrict__ vals = pb.vals;
+    uint32_t* __restrict__ out_w = pb.bm_word;
+    const int bias_col = pb.Dt - 1;
+    for (long long r = w0; r < n; r += nw) {
+      const float sd = pb.sdvec[r] * gscale;
+      const long long j0 = rowptr[r], j1 = rowptr[r + 1];
+      for (long long j = j0 + lane; j <= j1; j += 32) {
+        const bool bias = j == j1;
+        const uint32_t byte = __nv_cvt_float_to_fp8((bias ? 1.f : vals[j]) * sd, __NV_SATFINITE, __NV_E4M3);
+        out_w[j + r] = gram_word(byte, bias ? bias_col : colidx[j]);
+      }
+    }
+    return;
+  }
+  const long long ngroups = pb.bm_groups;
   const int nblk = pb.nblk128;
   const long long* __restrict__ offs = pb.bm_offs;
   const unsigned short* __restrict__ keys = pb.bm_keys;
   const float* __restrict__ vals = pb.bm_vals;
   unsigned char* __restrict__ out = pb.bm_e4m3;
-  uint32_t* __restrict__ out_w = pb.bm_word;
-  const bool word = pb.csr_gram == CSR_GRAM_SPARSE;
-  const int span = gram_sparse_span(pb.bm_entries, nblk, ngroups);   // as gram_csr_sparse_kernel computes it
-  const float gscale = pb.gram_scale;
-  const long long nw = ((long long)gridDim.x * blockDim.x) >> 5;
-  for (long long g = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; g < ngroups; g += nw) {
+  for (long long g = w0; g < ngroups; g += nw) {
     const long long r = g * SK + lane;
     const float sd = r < n ? pb.sdvec[r] * gscale : 0.f;
-    const int row0 = 32 * (int)(g % span);   // the group's first row in its span
     for (int b = 0; b < nblk; b++) {
       const uint32_t lo = (uint32_t)offs[(size_t)b * ngroups + g], hi = (uint32_t)offs[(size_t)b * ngroups + g + 1];
       for (uint32_t e0 = lo; e0 < hi; e0 += 32) {
@@ -418,106 +431,77 @@ __global__ void __launch_bounds__(256) gram_csr_operand_kernel(const Problem* __
         const bool v = e < hi;
         const uint32_t key = v ? (uint32_t)keys[e] : 0u;
         const float val = v ? vals[e] : 0.f;
-        const int k = kmaj_row(key);
-        const float sdk = __shfl_sync(0xffffffffu, sd, k);
+        const float sdk = __shfl_sync(0xffffffffu, sd, kmaj_row(key));
         const uint32_t byte = __nv_cvt_float_to_fp8(val * sdk, __NV_SATFINITE, __NV_E4M3);
-        if (!v) continue;
-        if (word) out_w[e] = sparse_word(byte, row0 + k, (int)(key >> 5));
-        else out[e] = (unsigned char)byte;
+        if (v) out[e] = (unsigned char)byte;
       }
     }
   }
 }
 
 // ------------------------------------------------------------------------------------------
-// Sparse CSR Gram: the same partial from the same e4m3 operand values, but only the nonzero products of each row are formed.  At
-// 1 % density a 32-row x 128-column operand block holds ~1 % nonzeros, so the wgmma kernel above spends ~10^4 multiply-adds per
-// nonzero product; here each product is one integer multiply and (mostly) one native shared-memory atomic add.
+// Sparse CSR Gram, column by column (Gustavson): the lower triangle's column c1 is
+//     G[c2][c1] = sum over the rows r holding c1 of x_{r,c1} x_{r,c2},   c2 >= c1,
+// and since a row's entries are in ascending column order with the intercept last, the partners of the entry (r, c1) are exactly
+// the row's suffix from that entry up to and including its intercept entry.  So a column is a walk over its positions in the
+// row-order operand (the column index gc_offs / gc_pos, built once at upload), each reading a contiguous run of words in which
+// every word read is one product: no tile re-reads a block's entries, and nothing is staged or scanned.  At 1M x 10k x 1 % a
+// build forms 5.2e9 products from 5.2e9 suffix words (21 GB, mostly from HBM: the operand is 404 MB), where the 128 x 128 tile
+// kernel this replaces read 8.1e9 entries and spent most of its time staging and scanning them.
 // Exact and deterministic: an e4m3 value is an integer number of units of 2^-9 (|v| <= 448 = 229376 units < 2^18), so a product
-// is an integer number of units of 2^-18 below 2^35.6, and the tile accumulates them as int64 (integer addition is associative:
+// is an integer number of units of 2^-18 below 2^35.6, and the column accumulates them as int64 (integer addition is associative:
 // the sum does not depend on the warp schedule).  A 64-bit shared atomic add is a compare-and-swap loop on sm_90a, so each cell
 // is a pair of 32-bit words: the product's low word goes in with a native ATOMS.ADD that returns the old word, and its high word
 // plus the carry out of the low add (old + lo < old) goes into the high word -- skipped when that is 0, which is the usual case
 // for |product| < 2^32 of either sign.  The pair holds the two's complement int64 sum exactly.  The epilogue rounds each cell
-// once to fp32.  The sum cannot overflow below
-// 2^27.4 rows (every row adds at most one product to a cell: rows have unique columns); gram_sparse_max_rows() states the limit
-// the batch rule applies.
-// One CTA per (128 x 128 lower tile (bi, bj), problem), one slice.  A warp's unit of work is a span of consecutive 32-row groups:
-// SP_SPAN (256 rows), fewer on denser data (gram_sparse_span: the mean range of a span must fit 3/4 of a stage chunk, since each
-// further chunk re-reads the bi range); warp w takes the spans w, w + SP_WARPS, ...  The list is block-major with ascending
-// groups, so a block's entries for a span are one contiguous range [offs[b][g0], offs[b][g0 + span]), in row order (group, then
-// row in group: csr_bm_fill_kernel writes lane 0's entries, then lane 1's, ...).  The operand pass, which visits every entry once
-// per build anyway, writes each entry as one sparse_word holding its value in units, its row in the span
-// (32 (group - g0) + row in group) and its column, so that the 80-odd tiles reading an entry each decode it with a few masks and
-// one conversion (before: a key and a byte load, the e4m3 decode, the swizzle decode and a walk over the span's group bounds).  Per
-// span the warp stages the bj range's nonzero entries in shared memory with each row's [start, end), then enumerates the
-// (bi entry, staged partner of its row) pairs in a flat index space: per 32 bi entries an inclusive warp scan of the partner
-// counts, then steps of 32 pairs, one per lane, each lane finding its owner entry from one OR-reduction of the owners' end
-// positions in the step (owners are compacted to a per-warp table first).  So lanes stay busy however the partners are spread
-// over the rows, and a row with 128 entries in both blocks (128^2 pairs) is as many full steps.  A bj range longer than SP_STAGE
-// entries is staged in chunks (boundaries may fall inside a row: each chunk pairs with its own part of the row), the bi range
-// re-read for each.
-// What bounds it (1M x 10k x 1 %, H100 80GB HBM3 at 700 W, 36.5 ms a build): the per-entry work, not the products.  Each batch
-// of 32 entries is 50 warp instructions to stage (load, decode, ballot, row table) and 76 to scan on the bi side up to the pair
-// steps (row-table lookup, partner-count scan, owner table), for ~1.3 products per entry; with the byte operand they were 89 and
-// 114, plus ~12 for every group bound a batch crossed.
-// Diagonal tiles keep the pairs with c2 <= c1 only (predicated) and mirror them in the epilogue.  Zero operand values (w = 0
-// rows, the end of a range) are skipped.
-// Same-cell contention: every row's intercept entry pairs with itself in the intercept's diagonal tile, so consecutive rows'
-// (intercept, intercept) products would be one step of 32 same-address atomics.  A lane sums that cell's products in an int64
-// register instead, and the warp adds its total once at the end (the sum is exact, so the order does not matter).  In the other
-// intercept tiles (bi = the intercept's block) the intercept row's products spread over the 128 cells of bj: at ~1 partner per
-// row, a step's 32 lanes meet ~4 same-cell pairs, no worse than a bank conflict, so those are left to the atomics.
+// once to fp32.  The sum cannot overflow below 2^27.4 rows (every row adds at most one product to a cell: rows have unique
+// columns); gram_sparse_max_rows() states the limit the batch rule applies.
+// A CTA takes the columns k = blockIdx.x, + gridDim.x, ... of one problem in the order bias column first (n positions of one
+// product each), then 0, 1, ...: low columns have the longest suffixes, so each CTA starts with its heaviest.  Its accumulator
+// holds the cells [c1, c1 + GC_CELLS) (a column of a wider system is walked once per window of GC_CELLS cells).  A warp takes 32
+// positions of the column at a time and walks them GC_GROUP at a time: the first 32 words of the next group's suffixes are
+// loaded while the current group's are multiplied, and a suffix longer than 32 words loads its next 32 before multiplying these,
+// so a warp has GC_GROUP to 2 GC_GROUP runs in flight (~16 KB an SM).  Lane 0's word is the multiplier; the intercept word ends
+// the walk (the ballot of its column).  Zero operands (w = 0 rows, underflow to 0) are skipped.
+// What bounds it (1M x 10k x 1 %, H100 80GB HBM3 at 700 W, 26.1 ms a build with the 1.2 ms operand pass): the walk's suffix reads
+// and their per-step instructions, ~19 ms; a walk step of 32 lanes reads 4 - 5 sectors whatever its suffix's length.  Loads in
+// flight do not bound it (GC_GROUP 2, 4 and 8 build in 25.2, 26.1 and 25.9 ms).  Timed without them, the shared atomics take ~4.1
+// ms and the epilogue's strided stores ~2.1 ms.
+// The intercept's cell (Dt - 1, c1) gets one product per row of the column: a lane sums it in an int64 register and the warp adds
+// its total once per column, instead of a stream of same-address atomics; the bias column's own positions are one product each
+// (the intercept squared), summed by lanes in parallel.
+// Epilogue: every cell of the column is rounded once and stored to Hpart[c2 Dp + c1], c2 >= c1 (and the cells above the diagonal
+// of c1's 128 x 128 diagonal tile, which chol_prep reads whole, as their mirror Hpart[c1 Dp + c2]), zeros included, so every build
+// writes the whole lower block triangle; reading a cell clears it for the next column.
 // ------------------------------------------------------------------------------------------
-constexpr int SP_THREADS = 1024;
-constexpr int SP_WARPS = SP_THREADS / 32;
-constexpr int SP_SPAN = 8;                                         // 32-row groups per span
-constexpr int SP_ROWS = SP_SPAN * 32;                              // rows per span: the row table's length
-constexpr int SP_AHEAD = 1;                                        // batches of 32 entries loaded ahead of use (2: slower)
-constexpr int SP_STAGE = 448;                                      // staged bj entries per warp and chunk (< 2^16: u16 row table)
-constexpr size_t SP_ACC_BYTES = (size_t)SN * SN * 2 * sizeof(uint32_t);   // 128 KB: low words, then high words
-// per warp: the stage (int), the row table (u32: start | end << 16) and the owner table (int2), 3 KB
-constexpr size_t SP_WARP_BYTES = (size_t)SP_STAGE * 4 + (size_t)SP_ROWS * 4 + 32 * 8;
-constexpr size_t SP_SMEM = SP_ACC_BYTES + (size_t)SP_WARPS * SP_WARP_BYTES;
-static_assert(SP_SMEM <= 227 * 1024, "sparse Gram shared memory");
-static_assert(SP_STAGE % 16 == 0, "layout of the stage");
-static_assert(SP_SPAN == 8 && SP_STAGE == 448, "gram_sparse_span (kernels.cuh) assumes these");
-static_assert(SP_ROWS <= 256, "sparse_word holds the row in the span in 8 bits");
+constexpr int GC_THREADS = 512;
+constexpr int GC_WARPS = GC_THREADS / 32;
+constexpr int GC_GROUP = 4;           // positions a warp walks together (their first runs loaded one group ahead)
+constexpr int GC_CELLS = 112 * 128;   // int64 cells of the accumulator: 112 KB, two CTAs an SM
+constexpr int GC_BIAS_UNROLL = 8;     // positions of the bias column a thread has in flight
 
-__global__ void __launch_bounds__(SP_THREADS, 1)
-gram_csr_sparse_kernel(const Problem* __restrict__ probs, const GramTile* __restrict__ tiles, int force, int share) {
+__global__ void __launch_bounds__(GC_THREADS, 2)
+gram_csr_column_kernel(const Problem* __restrict__ probs, int force, int share) {
   if (share > 1 && blockIdx.z % share != 0) return;   // see gram_wgmma_kernel
   const Problem& pb = probs[blockIdx.z];
   Ctrl* ctrl = pb.ctrl;
   if (!force && (ctrl->done || !ctrl->need_hess)) return;
-  const GramTile tile = tiles[blockIdx.x];
-  const int bi = tile.bi, bj = tile.bj;
-  const bool diag = bi == bj;
-  const int Dp = pb.Dp;
-  const long long ngroups = pb.bm_groups;
-  const int span = gram_sparse_span(pb.bm_entries, pb.nblk128, ngroups);   // groups per span, <= SP_SPAN
-  const long long nspans = (ngroups + span - 1) / span;
-  // the intercept's cell (column Dt - 1, the last entry of every row) when this is its diagonal tile, else -1 (matches no column)
-  const int hot = diag && (pb.Dt - 1) / SN == bi ? (pb.Dt - 1) % SN : -1;
+  const int Dp = pb.Dp, Dt = pb.Dt;
+  const int hot = Dt - 1;   // the intercept's column: every row's last entry
+  const int W = min(Dp, GC_CELLS);
+  const uint32_t nent = (uint32_t)pb.bm_entries;
+  const uint32_t* __restrict__ words = pb.bm_word;
+  const uint32_t* __restrict__ offs = pb.gc_offs;
+  const uint32_t* __restrict__ cpos = pb.gc_pos;
+  float* __restrict__ out = pb.Hpart;
 
   extern __shared__ __align__(16) unsigned char g_smem_raw[];
-  uint32_t* acc_lo = reinterpret_cast<uint32_t*>(g_smem_raw);   // [c1][c2]: low and high 32-bit words of an int64 sum
-  int* acc_hi = reinterpret_cast<int*>(g_smem_raw) + SN * SN;
+  uint32_t* acc_lo = reinterpret_cast<uint32_t*>(g_smem_raw);   // [cell]: low and high 32-bit words of an int64 sum
+  int* acc_hi = reinterpret_cast<int*>(g_smem_raw) + W;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  unsigned char* wsm = g_smem_raw + SP_ACC_BYTES + (size_t)warp * SP_WARP_BYTES;
-  int* stage = reinterpret_cast<int*>(wsm);                                // (units << 7) | c2
-  uint32_t* rtab = reinterpret_cast<uint32_t*>(wsm + SP_STAGE * 4);        // a row's staged entries [start, end): start | end << 16
-  unsigned short* rtab16 = reinterpret_cast<unsigned short*>(rtab);        // start of row r at 2 r, end at 2 r + 1
-  int2* own = reinterpret_cast<int2*>(wsm + SP_STAGE * 4 + SP_ROWS * 4);  // owners of a batch: ((units << 7) | c1, start - first pair)
-
-  for (int e = threadIdx.x; e < SN * SN; e += SP_THREADS) { acc_lo[e] = 0u; acc_hi[e] = 0; }
+  for (int e = threadIdx.x; e < W; e += GC_THREADS) { acc_lo[e] = 0u; acc_hi[e] = 0; }
   __syncthreads();
 
-  const bool valid = bi < pb.nblk128 && bj < pb.nblk128;
-  const long long* __restrict__ offs_i = pb.bm_offs + (size_t)bi * ngroups;
-  const long long* __restrict__ offs_j = pb.bm_offs + (size_t)bj * ngroups;
-  const uint32_t* __restrict__ words = pb.bm_word;
-  const uint32_t lt = (1u << lane) - 1u;
   // a cell gets the product p (units of 2^-18, int64): the low word with a native atomic add that returns the old word, the high
   // word plus the carry out of the low add when that is not 0
   auto add_cell = [&](int cell, long long p) {
@@ -526,134 +510,128 @@ gram_csr_sparse_kernel(const Problem* __restrict__ probs, const GramTile* __rest
     const int hi = (int)(p >> 32) + (old + lo < old ? 1 : 0);
     if (hi != 0) atomicAdd(acc_hi + cell, hi);
   };
-  // the list holds < 2^32 entries (checked at upload): entry numbers are 32-bit.  A span's ranges, lane-distributed: lanes 0, 1
-  // hold offs_i[g0], offs_i[g0 + span], lanes 2, 3 the same of offs_j, clamped to the last group (a short last span's missing
-  // groups are empty).  Fetched two spans ahead, and the first SP_AHEAD batches of 32 entries of both ranges one span ahead: a
-  // warp has one span in flight.  Inside a range the entries are loaded SP_AHEAD batches ahead: most bj ranges are not in L2 (a
-  // wave's tiles read ~80 different bj blocks), so a batch's loads need the time of several batches' work to arrive.
-  auto ld_bounds = [&](long long s) -> uint32_t {
-    if (!valid || s >= nspans || lane >= 4) return 0u;
-    return (uint32_t)__ldg((lane < 2 ? offs_i : offs_j) + min(s * span + (lane & 1) * span, ngroups));
-  };
-  // an entry's operand word, 0 past the end of its range (a zero value: skipped like any zero operand)
-  auto ld_entry = [&](uint32_t e, uint32_t hi) -> uint32_t { return e < hi ? __ldg(words + e) : 0u; };
-  struct Span { uint32_t ilo, ihi, jlo, jhi, i[SP_AHEAD], j[SP_AHEAD]; };
-  auto take = [&](Span& q, uint32_t b) {
-    q.ilo = __shfl_sync(0xffffffffu, b, 0); q.ihi = __shfl_sync(0xffffffffu, b, 1);
-    q.jlo = __shfl_sync(0xffffffffu, b, 2); q.jhi = __shfl_sync(0xffffffffu, b, 3);
+  // the operand holds < 2^32 - 64 words (checked at upload): positions are 32-bit; past its end a word is 0
+  auto word_at = [&](uint32_t q) -> uint32_t { return q < nent ? __ldg(words + q) : 0u; };
+
+  for (int k = blockIdx.x; k < Dp; k += gridDim.x) {
+    const int c1 = k == 0 ? hot : (k <= hot ? k - 1 : k);
+    const uint32_t p0 = c1 < Dt ? __ldg(offs + c1) : 0u, p1 = c1 < Dt ? __ldg(offs + c1 + 1) : 0u;
+    for (int w0 = c1; w0 < Dp; w0 += W) {
+      const int w1 = min(Dp, w0 + W);
+      long long hot_sum = 0;   // this lane's products of the intercept's cell (hot, c1)
+      if (c1 == hot) {
+        // every position is a row's intercept word, its only partner itself
+        for (uint32_t i0 = p0 + threadIdx.x; i0 < p1; i0 += GC_THREADS * GC_BIAS_UNROLL) {
+          uint32_t x[GC_BIAS_UNROLL];
 #pragma unroll
-    for (int k = 0; k < SP_AHEAD; k++) { q.i[k] = ld_entry(q.ilo + lane + 32 * k, q.ihi); q.j[k] = ld_entry(q.jlo + lane + 32 * k, q.jhi); }
-  };
-  long long hot_sum = 0;   // this lane's products of the intercept's cell
-  auto run = [&](const Span& q) {
-    const uint32_t ilo = q.ilo, ihi = q.ihi, jlo = q.jlo, jhi = q.jhi;
-    if (ilo == ihi || jlo == jhi) return;
-    for (uint32_t c0 = jlo; c0 < jhi; c0 += SP_STAGE) {
-      const uint32_t c1 = min(jhi, c0 + SP_STAGE);   // >= jlo + 32 * SP_AHEAD or = jhi: the prefetched batches lie in the first chunk
-      __syncwarp();   // the previous chunk's readers are done
-#pragma unroll
-      for (int k = 0; k < SP_ROWS / 128; k++) reinterpret_cast<uint4*>(rtab)[lane + 32 * k] = make_uint4(0u, 0u, 0u, 0u);
-      __syncwarp();
-      // ---- stage the chunk's nonzero entries; a kept entry whose row differs from the previous kept one starts its row
-      int nst = 0, prev_row = -1;
-      uint32_t x[SP_AHEAD + 1];   // the batches base, base + 32, ...
-#pragma unroll
-      for (int k = 0; k < SP_AHEAD; k++) x[k] = c0 == jlo ? q.j[k] : ld_entry(c0 + 32 * k + lane, c1);
-      for (uint32_t base = c0; base < c1; base += 32) {
-        x[SP_AHEAD] = ld_entry(base + 32 * SP_AHEAD + lane, c1);
-        const uint32_t w = x[0];
-        const int v = sw_units(w);
-        const int r = sw_row(w);
-        const bool keep = v != 0;
-        const uint32_t m = __ballot_sync(0xffffffffu, keep);
-        const uint32_t below = m & lt;
-        const int up = __shfl_sync(0xffffffffu, r, below ? 31 - __clz(below) : 0);
-        const int pr = below ? up : prev_row;
-        const int s = nst + __popc(below);
-        if (keep) {
-          stage[s] = v * 128 + sw_col(w);
-          if (r != pr) { rtab16[2 * r] = (unsigned short)s; if (pr >= 0) rtab16[2 * pr + 1] = (unsigned short)s; }
-        }
-        if (m) prev_row = __shfl_sync(0xffffffffu, r, 31 - __clz(m));
-        nst += __popc(m);
-#pragma unroll
-        for (int k = 0; k < SP_AHEAD; k++) x[k] = x[k + 1];
-      }
-      if (nst == 0) continue;
-      if (lane == 0) rtab16[2 * prev_row + 1] = (unsigned short)nst;
-      __syncwarp();
-      // ---- the (bi entry, staged partner) pairs, 32 bi entries at a time
-#pragma unroll
-      for (int k = 0; k < SP_AHEAD; k++) x[k] = q.i[k];
-      for (uint32_t base = ilo; base < ihi; base += 32) {
-        x[SP_AHEAD] = ld_entry(base + 32 * SP_AHEAD + lane, ihi);
-        const uint32_t w = x[0];
-        const int a = sw_units(w);
-        const uint32_t t = a != 0 ? rtab[sw_row(w)] : 0u;
-        const int s0 = (int)(t & 0xFFFFu), cnt = (int)(t >> 16) - s0;
-        int incl = cnt;   // inclusive warp scan of the partner counts
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-          const int u = __shfl_up_sync(0xffffffffu, incl, d);
-          if (lane >= d) incl += u;
-        }
-        const int total = __shfl_sync(0xffffffffu, incl, 31);
-#pragma unroll
-        for (int k = 0; k < SP_AHEAD; k++) x[k] = x[k + 1];
-        if (total == 0) continue;
-        // owners (entries with partners) in lane order: pair p belongs to the owner of rank #{owners whose pairs end at or before p}
-        const uint32_t owners = __ballot_sync(0xffffffffu, cnt > 0);
-        __syncwarp();   // the previous batch's readers of own[] are done
-        if (cnt > 0) own[__popc(owners & lt)] = make_int2(a * 128 + sw_col(w), s0 - (incl - cnt));
-        __syncwarp();
-        int before = 0;   // owners whose pairs end before this step
-        for (int p0 = 0; p0 < total; p0 += 32) {
-          const int end = incl - p0;
-          const uint32_t ends = __reduce_or_sync(0xffffffffu, cnt > 0 && end >= 0 && end < 32 ? 1u << end : 0u);
-          const int p = p0 + lane;
-          if (p < total) {
-            const int2 o = own[before + __popc(ends & (0xFFFFFFFFu >> (31 - lane)))];
-            const int pv = stage[p + o.y];
-            const int c1 = o.x & 127, c2 = pv & 127;
-            if (!diag || c2 <= c1) {
-              const long long prod = (long long)(o.x >> 7) * (long long)(pv >> 7);
-              if (c2 == hot && c1 == hot) hot_sum += prod;
-              else add_cell(c1 * SN + c2, prod);
-            }
+          for (int u = 0; u < GC_BIAS_UNROLL; u++) {
+            const uint32_t i = i0 + u * GC_THREADS;
+            x[u] = i < p1 ? __ldg(cpos + i) : 0xFFFFFFFFu;
           }
-          before += __popc(ends);
+#pragma unroll
+          for (int u = 0; u < GC_BIAS_UNROLL; u++) x[u] = word_at(x[u]);
+#pragma unroll
+          for (int u = 0; u < GC_BIAS_UNROLL; u++) { const long long v = gw_units(x[u]); hot_sum += v * v; }
+        }
+      } else {
+        // one position q (warp-uniform) with the first 32 words of its suffix in x (lane l: word q + l)
+        auto walk = [&](uint32_t q, uint32_t x) {
+          const int a = gw_units(__shfl_sync(0xffffffffu, x, 0));
+          if (a == 0) return;
+          while (true) {
+            const int c2 = gw_col(x);
+            const uint32_t ends = __ballot_sync(0xffffffffu, c2 == hot);
+            uint32_t nx = 0u;
+            if (!ends) nx = word_at(q + 32 + lane);   // the next 32 words are in flight while these are multiplied
+            const int v = gw_units(x);
+            if ((!ends || lane < __ffs(ends)) && v != 0) {
+              const long long prod = (long long)a * (long long)v;
+              if (c2 == hot) hot_sum += prod;
+              else if (c2 >= w0 && c2 < w1) add_cell(c2 - w0, prod);
+            }
+            if (ends) return;
+            x = nx;
+            q += 32;
+          }
+        };
+        for (uint32_t cb = p0 + 32u * warp; cb < p1; cb += 32u * GC_WARPS) {
+          const int cnt = (int)min(32u, p1 - cb);
+          const uint32_t mine = lane < cnt ? __ldg(cpos + cb + lane) : 0u;   // the chunk's positions, one a lane
+          uint32_t cur[GC_GROUP];
+#pragma unroll
+          for (int g = 0; g < GC_GROUP; g++) {
+            const uint32_t q = __shfl_sync(0xffffffffu, mine, g);
+            cur[g] = g < cnt ? word_at(q + lane) : 0u;
+          }
+          for (int j = 0; j < cnt; j += GC_GROUP) {
+            uint32_t nxt[GC_GROUP];
+#pragma unroll
+            for (int g = 0; g < GC_GROUP; g++) {
+              const int jj = j + GC_GROUP + g;
+              const uint32_t q = __shfl_sync(0xffffffffu, mine, jj & 31);
+              nxt[g] = jj < cnt ? word_at(q + lane) : 0u;
+            }
+#pragma unroll
+            for (int g = 0; g < GC_GROUP; g++) {
+              const uint32_t q = __shfl_sync(0xffffffffu, mine, j + g);
+              if (j + g < cnt) walk(q, cur[g]);
+            }
+#pragma unroll
+            for (int g = 0; g < GC_GROUP; g++) cur[g] = nxt[g];
+          }
         }
       }
-    }
-  };
-  Span cur, nxt;
-  take(cur, ld_bounds(warp));
-  uint32_t nb = ld_bounds(warp + SP_WARPS);
-  for (long long s = warp; s < nspans; s += SP_WARPS) {
-    take(nxt, nb);   // the next span's loads are in flight while this one runs
-    nb = ld_bounds(s + 2 * SP_WARPS);
-    run(cur);
-    cur = nxt;
-  }
-  if (hot >= 0) {
+      if (hot >= w0 && hot < w1) {
 #pragma unroll
-    for (int d = 16; d > 0; d >>= 1) hot_sum += __shfl_down_sync(0xffffffffu, hot_sum, d);
-    if (lane == 0 && hot_sum != 0) add_cell(hot * SN + hot, hot_sum);
-  }
-  __syncthreads();
-  // ---- one rounding per cell: units of 2^-18 -> fp32
-  float* out = pb.Hpart + (size_t)bi * SN * Dp + (size_t)bj * SN;
-  for (int e = threadIdx.x; e < SN * SN; e += SP_THREADS) {
-    const int c1 = e >> 7, c2 = e & 127;
-    const int idx = diag && c2 > c1 ? c2 * SN + c1 : e;
-    const long long v = (long long)(((unsigned long long)(uint32_t)acc_hi[idx] << 32) | acc_lo[idx]);
-    out[(size_t)c1 * Dp + c2] = __ll2float_rn(v) * 0x1p-18f;
+        for (int d = 16; d > 0; d >>= 1) hot_sum += __shfl_down_sync(0xffffffffu, hot_sum, d);
+        if (lane == 0 && hot_sum != 0) add_cell(hot - w0, hot_sum);
+      }
+      __syncthreads();
+      // ---- one rounding per cell: units of 2^-18 -> fp32; the cell is cleared for the next column
+      const int dend = (c1 / 128 + 1) * 128;   // end of c1's diagonal tile
+      for (int e = threadIdx.x; e < w1 - w0; e += GC_THREADS) {
+        const int c2 = w0 + e;
+        const long long v = (long long)(((unsigned long long)(uint32_t)acc_hi[e] << 32) | acc_lo[e]);
+        acc_lo[e] = 0u; acc_hi[e] = 0;
+        const float f = __ll2float_rn(v) * 0x1p-18f;
+        out[(size_t)c2 * Dp + c1] = f;
+        if (c2 > c1 && c2 < dend) out[(size_t)c1 * Dp + c2] = f;
+      }
+      __syncthreads();
+    }
   }
 }
 
-// Largest partition (rows) the sparse kernel's int64 tile sums are safe for: every row adds at most one product of magnitude
+// Largest partition (rows) the sparse kernel's int64 column sums are safe for: every row adds at most one product of magnitude
 // <= 229376^2 < 2^35.62 units to a cell, and 2^27 * 2^35.62 < 2^63
 long long gram_sparse_max_rows() { return 1LL << 27; }
+// Widest system (D', the intercept included) the sparse kernel takes: its operand word holds the column in 20 bits
+int gram_sparse_max_cols() { return 1 << 20; }
+
+// Column index of the sparse CSR Gram: for every column c < D' the positions, in the row-order operand, of its entries, ascending
+// (so in row order): pos[offs[c] .. offs[c + 1]).  Row r's entries sit at [rowptr[r] + r, rowptr[r + 1] + r] with its intercept
+// (column bias_col = D' - 1) last.  Built by a stable radix sort of the entries' columns in row order.
+__global__ void __launch_bounds__(256) csr_col_keys_kernel(long long n, const long long* __restrict__ rowptr, const int* __restrict__ colidx,
+                                                           int bias_col, uint32_t* __restrict__ keys, uint32_t* __restrict__ idx) {
+  const int lane = threadIdx.x & 31;
+  const long long nw = ((long long)gridDim.x * blockDim.x) >> 5;
+  for (long long r = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n; r += nw) {
+    const long long j0 = rowptr[r], j1 = rowptr[r + 1];
+    for (long long j = j0 + lane; j <= j1; j += 32) {
+      keys[j + r] = j == j1 ? (uint32_t)bias_col : (uint32_t)colidx[j];
+      idx[j + r] = (uint32_t)(j + r);
+    }
+  }
+}
+// offs[c] = the first sorted entry of column >= c, for c in [0, ncols]
+__global__ void __launch_bounds__(256) csr_col_offsets_kernel(long long entries, const uint32_t* __restrict__ sorted, int ncols,
+                                                              uint32_t* __restrict__ offs) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i <= entries; i += (long long)gridDim.x * blockDim.x) {
+    const long long lo = i == 0 ? -1 : (long long)sorted[i - 1];
+    const long long hi = i == entries ? (long long)ncols : (long long)sorted[i];
+    for (long long c = lo + 1; c <= hi; c++) offs[c] = (uint32_t)i;
+  }
+}
 
 // Block-major entry list for the CSR Gram.  For every 128-column block b and every 32-row group g the entries
 // (row in group, column in block, value) are stored contiguously at [offs[b*ngroups+g], offs[b*ngroups+g+1]); the key is
@@ -789,15 +767,13 @@ int gram_make_tensor_map(void* out_map_host /*CUtensorMap, 128 B*/, const void* 
 }
 
 // Lower block-triangle tile list for a Dp x Dp output (Dp multiple of 128): 128 x 256 tiles (bi, bj) for the bf16 kernel, or
-// 128 x 128 tiles for the CSR kernels (csr_tiles != 0).  The tiles of one bi are consecutive, so CTAs resident at the same time
-// share the bi run of the entry list in L2; the sparse kernel (csr_tiles == 2) takes the bi in descending order, which puts the
-// tile of the intercept column (every row's last entry: the most contended cell) into the first wave.
+// 128 x 128 tiles for the CSR wgmma kernel (csr_tiles != 0).  The tiles of one bi are consecutive, so CTAs resident at the same
+// time share the bi run of the entry list in L2.
 int gram_tile_list(int Dp, short* bi_bj_pairs /*[2*max]*/, int max_tiles, int csr_tiles) {
   int n = 0;
   const int cols = csr_tiles ? SN : GN;
   const int nbi = (Dp + GM - 1) / GM, nbj = (Dp + cols - 1) / cols;
-  for (int k = 0; k < nbi; k++) {
-    const int bi = csr_tiles == 2 ? nbi - 1 - k : k;
+  for (int bi = 0; bi < nbi; bi++) {
     for (int bj = 0; bj < nbj; bj++)
       if (bj * cols <= bi * GM + GM - 1) {
         if (n >= max_tiles) return -1;
@@ -846,18 +822,56 @@ cudaError_t gram_launch_csr_wgmma(const Problem* d_probs, int nprob, const void*
   return cudaGetLastError();
 }
 
-// One sparse CSR Gram build: the operand pass, then the sparse Gram into slice 0.  d_tiles holds the tiles of
-// gram_tile_list(..., 2)
-cudaError_t gram_launch_csr_sparse(const Problem* d_probs, int nprob, const void* d_tiles, int ntiles, int force, cudaStream_t st,
-                                   int* launches, int share) {
+// One sparse CSR Gram build of Dp x Dp problems: the operand pass, then the column kernel into slice 0, two CTAs an SM for every
+// problem (a gated-off one returns at once)
+cudaError_t gram_launch_csr_sparse(const Problem* d_probs, int nprob, int Dp, int force, cudaStream_t st, int* launches, int share) {
   static bool configured[64] = {};
-  cudaError_t e = set_smem_once(gram_csr_sparse_kernel, SP_SMEM, configured);
+  static int sms[64] = {};
+  cudaError_t e = set_smem_once(gram_csr_column_kernel, (size_t)GC_CELLS * 8, configured);
   if (e != cudaSuccess) return e;
+  int dev = 0, nsm = 0;
+  if ((e = cudaGetDevice(&dev)) != cudaSuccess) return e;
+  if (dev >= 0 && dev < 64 && sms[dev]) nsm = sms[dev];
+  else {
+    if ((e = cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return e;
+    if (dev >= 0 && dev < 64) sms[dev] = nsm;
+  }
   gram_csr_operand_kernel<<<dim3(1024, nprob), 256, 0, st>>>(d_probs, force, share);
   if ((e = cudaGetLastError()) != cudaSuccess) return e;
-  gram_csr_sparse_kernel<<<dim3(ntiles, 1, nprob), SP_THREADS, SP_SMEM, st>>>(d_probs, reinterpret_cast<const GramTile*>(d_tiles), force, share);
+  const size_t smem = (size_t)std::min(Dp, GC_CELLS) * 8;
+  gram_csr_column_kernel<<<dim3(std::min(Dp, 2 * nsm), 1, nprob), GC_THREADS, smem, st>>>(d_probs, force, share);
   if (launches) *launches += 2;
   return cudaGetLastError();
+}
+
+// The column index of the sparse CSR Gram (csr_col_keys_kernel): offs [bias_col + 2], pos [entries = nnz + n]
+cudaError_t csr_col_index(long long n, const long long* rowptr, const int* colidx, int bias_col, long long entries, uint32_t* offs,
+                          uint32_t* pos, cudaStream_t st) {
+  cudaError_t e = cudaSuccess;
+  uint32_t *keys = nullptr, *sorted = nullptr, *idx = nullptr;
+  void* tmp = nullptr;
+  size_t tmp_bytes = 0;
+  int bits = 1;
+  while ((1LL << bits) <= bias_col) bits++;
+  auto run = [&]() -> cudaError_t {
+    cudaError_t r;
+    // stream-ordered temporaries: no device-wide wait
+    if ((r = cudaMallocAsync(&keys, (size_t)entries * 4, st)) != cudaSuccess) return r;
+    if ((r = cudaMallocAsync(&sorted, (size_t)entries * 4, st)) != cudaSuccess) return r;
+    if ((r = cudaMallocAsync(&idx, (size_t)entries * 4, st)) != cudaSuccess) return r;
+    const int grid = (int)std::min<long long>((n + 7) / 8, 132 * 32);
+    csr_col_keys_kernel<<<std::max(grid, 1), 256, 0, st>>>(n, rowptr, colidx, bias_col, keys, idx);
+    if ((r = cudaGetLastError()) != cudaSuccess) return r;
+    if ((r = cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, keys, sorted, idx, pos, entries, 0, bits, st)) != cudaSuccess) return r;
+    if ((r = cudaMallocAsync(&tmp, tmp_bytes ? tmp_bytes : 16, st)) != cudaSuccess) return r;
+    if ((r = cub::DeviceRadixSort::SortPairs(tmp, tmp_bytes, keys, sorted, idx, pos, entries, 0, bits, st)) != cudaSuccess) return r;
+    csr_col_offsets_kernel<<<(int)std::min<long long>((entries + 256) / 256, 132 * 32), 256, 0, st>>>(entries, sorted, bias_col + 1, offs);
+    return cudaGetLastError();
+  };
+  e = run();
+  for (void* p : {(void*)keys, (void*)sorted, (void*)idx, tmp})
+    if (p) { cudaError_t e2 = cudaFreeAsync(p, st); if (e == cudaSuccess) e = e2; }
+  return e;
 }
 
 // counts -> exclusive offsets in place: offs has nblk*ngroups+1 entries (the last one = total entries)

@@ -45,17 +45,14 @@ cudaError_t gram_launch_wgmma(const Problem* d_probs, int nprob, const void* d_t
                               int nslices, int force, cudaStream_t st, int* launches, int share = 0);
 cudaError_t gram_launch_csr_wgmma(const Problem* d_probs, int nprob, const void* d_tiles, int ntiles, int nslices, int force,
                                   cudaStream_t st, int* launches, int share = 0);
-// the exact sparse CSR Gram (one slice; tiles of gram_tile_list(..., 2)) and the largest partition it accepts
-cudaError_t gram_launch_csr_sparse(const Problem* d_probs, int nprob, const void* d_tiles, int ntiles, int force, cudaStream_t st,
-                                   int* launches, int share = 0);
+// the exact sparse CSR Gram of Dp x Dp problems (one slice), the largest partition (rows) and system (D') it accepts, and its
+// column index, built once at upload: for column c < bias_col + 1 the positions pos[offs[c] .. offs[c + 1]) of its entries in
+// the row-order operand (row r at [rowptr[r] + r, rowptr[r + 1] + r], its intercept entry last)
+cudaError_t gram_launch_csr_sparse(const Problem* d_probs, int nprob, int Dp, int force, cudaStream_t st, int* launches, int share = 0);
 long long gram_sparse_max_rows();
-// 32-row groups per span of the sparse CSR Gram (a warp's unit of work): 8, fewer when the mean (block, group) range of the list
-// (entries / (nblk ngroups)) would not fit 3/4 of a warp's 448-entry stage chunk, since every chunk re-reads the other block's range
-__host__ __device__ inline int gram_sparse_span(long long entries, int nblk, long long ngroups) {
-  const double per = (double)entries / ((double)(nblk > 1 ? nblk : 1) * (double)(ngroups > 1 ? ngroups : 1));
-  const int g = (int)(0.75 * 448 / (per > 1.0 ? per : 1.0));
-  return g < 1 ? 1 : (g > 8 ? 8 : g);
-}
+int gram_sparse_max_cols();
+cudaError_t csr_col_index(long long n, const long long* rowptr, const int* colidx, int bias_col, long long entries, uint32_t* offs,
+                          uint32_t* pos, cudaStream_t st);
 cudaError_t csr_bm_offsets(long long n, const long long* rowptr, const int* colidx, int bias_col, int nblk, long long ngroups, long long* offs,
                            cudaStream_t st);
 cudaError_t csr_bm_fill(long long n, const long long* rowptr, const int* colidx, const float* vals, int bias_col, int nblk, long long ngroups,

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Times one CSR Gram build with each kernel (e4m3 wgmma, exact sparse) on the same upload, at several densities at D = 10k plus
 the bench shape (1M x 10k x 1 %) and `bench.py --features 500` (1M x 500 x 20 %), through mlease_time_kernel; prints which kernel
-the automatic rule picks for each and a least-squares fit of the cost constants of batch_alloc's rule (csrc/session.cu).
+the automatic rule picks for each and a least-squares fit of the cost constants of batch_alloc's rule (csrc/batch.cu).
 OUT=path also writes the table as JSON.  SHAPES=bench keeps the bench shape only.
 WHICH=cholesky: times the factorisation + inverse of one 10k-wide system instead (ROWS=100000 keeps the data small).
 Scratch tool for kernel work on a GPU box, not part of the product."""
@@ -68,21 +68,19 @@ def main():
         Dp = (D + 1 + 127) // 128 * 128   # ldx rounds D + 1 up to a multiple of 4; Dp to 128
         nblk = Dp // 128
         tiles, groups = nblk * (nblk + 1) // 2, (n + 31) // 32
-        span = max(1, min(8, int(0.75 * 448 / max(n * (nnz + 1) / (nblk * groups), 1.0))))   # kernels.cuh gram_sparse_span
-        spans = -(-groups // span)
         r = dict(n=n, D=D, nnz=nnz, density=nnz / D, ms_wgmma=ms_w, ms_sparse=ms_s, auto="sparse" if auto == SPARSE else "wgmma",
                  macs_wgmma=tiles * 128.0 * 128.0 * 32.0 * groups, pairs=n * (nnz + 1) * (nnz + 2) / 2.0,
-                 visits=float(tiles * spans), span=span, reads=(nblk + 1.0) * n * (nnz + 1))
+                 entries=float(n * (nnz + 1)), cells=0.5 * Dp * (Dp + 1.0), reads=(nblk + 1.0) * n * (nnz + 1))
         rows.append(r)
         print("n %8d D %6d nnz/row %5d (%5.2f %%): wgmma %9.3f ms  sparse %9.3f ms  auto %s" %
               (n, D, nnz, 100.0 * nnz / D, ms_w, ms_s, r["auto"]), flush=True)
     fit = {}
-    full = [r for r in rows if r["visits"] / -(-((r["n"] + 31) // 32) // r["span"]) >= torch.cuda.get_device_properties(0).multi_processor_count]
+    full = rows   # every shape here has more columns than the sparse kernel's grid
     if len(full) >= 3:
-        # the rule's models on the shapes that fill the device, relative least squares (every shape weighs the same):
-        #   sparse  s = s/pair * pairs + s/visit * (tile, span) visits + s/read * entries read (each block's run by nblk + 1 tiles)
+        # the rule's models, relative least squares (every shape weighs the same):
+        #   sparse  s = s/pair * pairs + s/entry * entries (column positions) + s/cell * cells of the lower triangle (epilogues)
         #   wgmma   s = s/MAC * MACs + s/read * entries read (the producers' run loads)
-        for name, key, cols in (("sparse", "ms_sparse", ("pairs", "visits", "reads")), ("wgmma", "ms_wgmma", ("macs_wgmma", "reads"))):
+        for name, key, cols in (("sparse", "ms_sparse", ("pairs", "entries", "cells")), ("wgmma", "ms_wgmma", ("macs_wgmma", "reads"))):
             A = np.array([[r[c] for c in cols] for r in full])
             t = np.array([r[key] * 1e-3 for r in full])
             c, *_ = np.linalg.lstsq(A / t[:, None], np.ones(len(full)), rcond=None)
