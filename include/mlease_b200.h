@@ -228,6 +228,27 @@ int mlease_hessian_vector(mlease_session* s, int32_t partition_id, const double*
 int mlease_posterior_variance(mlease_session* s, int32_t partition_id, const double* w, const double* q, int32_t full,
                               double* var, double* cov);
 
+/* Posterior of the ADMM model: the Laplace posterior, at z, of the objective the z-update minimises
+ * (jobs/RegressionAdmmTrain.java:377-404) over ALL partitions of the job, for lambda index lambda_index:
+ *   H = sum over partitions, sum_i weight_i p_i (1-p_i) x~_i x~_i^T + diag(q),   x~_i = row i with the intercept entry 1,
+ *   p_i at z with the row's offset, q[k] = lambda (lambda_map[k] where that is > 0), q[intercept] = lambda with
+ *   penalize_intercept, else 0.
+ * z (num_features+1 doubles, intercept last, host or device) or NULL for the session's consensus z of that lambda (after
+ * mlease_admm_begin).  Every partition's H is exact fp64 from the fp32 rows (CSR: built column by column from the rows' suffixes,
+ * no atomics; dense: tiled X^T D X), the partitions are summed in partition-id order whatever order they were uploaded in, and with
+ * a communicator attached the ranks' sums go through one fp64 all-reduce: the call is then collective on every rank, and a
+ * refusal on one rank is returned on all of them.  The result is bitwise repeatable.
+ *   full = 0: var[k] = 1 / (q[k] + sum_i weight_i p_i (1-p_i) x~_ik^2)  -- any width, matrix-free sessions included
+ *   full = 1: var = diag(H^-1), cov (may be NULL) = H^-1, [D+1][D+1] row-major host memory; Cholesky + explicit inverse in fp64 on
+ *             buffers of the call's own (4 x 8 x ldh^2 bytes, ldh = round_up(D+1, 32), checked against the free device memory
+ *             before anything is allocated).
+ * The ADMM batch, its factors and its state are not touched: the session iterates on exactly as it would have.
+ * MLEASE_ERR_INVALID: regularizer 1 (the L1 penalty has no Hessian), lambda_index out of range, CSR rows that are not strictly
+ * increasing, a full posterior that does not fit the device; MLEASE_ERR_NUMERIC: H not positive definite. */
+int mlease_admm_posterior(mlease_session* s, int32_t lambda_index, const double* z, int32_t full, double* var, double* cov);
+/* the same over the devices of a world (collective over its NCCL communicator); var / cov from device 0 */
+int mlease_world_admm_posterior(mlease_world* w, int32_t lambda_index, const double* z, int32_t full, double* var, double* cov);
+
 /* ---------------------------------------------------------------------------------------
  * RegressionNaiveTrain (jobs/RegressionNaiveTrain.java:302-415): num_keys x num_lambdas independent fits ("lambda#key"
  * reducers, :228-241).  Key k owns rows [key_rowstart[k], key_rowstart[k+1]) of ONE matrix, uploaded once for all lambdas:
@@ -355,6 +376,16 @@ int mlease_item_model_train_cov(int32_t device, void* stream, int32_t num_keys, 
 int mlease_score(int32_t device, void* stream, int32_t num_features, int64_t nrows, const int64_t* rowptr,
                  const int32_t* colidx, const float* vals, int64_t ldx, const float* offset, const double* model,
                  int32_t num_click_replicates, int32_t binary_feature, float* pred);
+/* score_var: score's pred, bit for bit, and each record's predictive variance under the posterior of the model,
+ *        pred_var = float(g^T Sigma g) accumulated in fp64 in a fixed order: g holds the record's entries (1 with binary_feature)
+ *        and, at the intercept, d pred / d b = n e^-b / (n - 1 + n e^-b) (1 for n = 1): the delta method through interceptTerm.
+ *        Exactly one of var ([num_features+1], Sigma diagonal: sum_k var_k g_k^2) and cov ([num_features+1]^2 row-major, dense
+ *        Sigma, its lower triangle read; mlease_admm_posterior's output) is given.  CSR rows only, strictly ascending columns
+ *        (checked: MLEASE_ERR_INVALID).  All pointers host-or-device. */
+int mlease_score_var(int32_t device, void* stream, int32_t num_features, int64_t nrows, const int64_t* rowptr,
+                     const int32_t* colidx, const float* vals, const float* offset, const double* model,
+                     int32_t num_click_replicates, int32_t binary_feature, const double* var, const double* cov, float* pred,
+                     float* pred_var);
 int mlease_test_loglik(int32_t device, void* stream, int64_t nrows, const int32_t* response, const float* pred,
                        const float* weight, int64_t combiner_block, float* out_loglik, double* out_count);
 

@@ -274,6 +274,24 @@ int mlease_world_get_uplusx(mlease_world* w, int32_t pid, int32_t l, float* out)
 int mlease_world_fit_partition(mlease_world* w, int32_t pid, double* x, const double* m, const double* q, int32_t* newton_steps) {
   return (w && pid >= 0) ? mlease_fit_partition(w->sess[owner(w, pid)], pid, x, m, q, newton_steps) : fail(MLEASE_ERR_INVALID, "bad argument");
 }
+// every device sums its own partitions, the all-reduce inside mlease_admm_posterior sums the devices, and every device factorises
+// the same sum; device 0's result is returned
+int mlease_world_admm_posterior(mlease_world* w, int32_t lambda_index, const double* z, int32_t full, double* var, double* cov) {
+  if (!w || !var) return fail(MLEASE_ERR_INVALID, "null argument");
+  if (int rc = world_check_complete(w)) return rc;
+  std::vector<std::vector<double>> vd(w->ndev), cd(w->ndev);
+  return on_all(w, [&](int d) {
+    double* v = var;
+    double* c = cov;
+    if (d > 0) {
+      vd[d].resize(w->Dt);
+      v = vd[d].data();
+      if (cov) { cd[d].resize((size_t)w->Dt * w->Dt); c = cd[d].data(); }
+    }
+    return mlease_admm_posterior(w->sess[d], lambda_index, z, full, v, c);
+  });
+}
+
 int mlease_world_get_stats(mlease_world* w, mlease_stats* out) {
   if (!w || !out) return fail(MLEASE_ERR_INVALID, "null argument");
   std::memset(out, 0, sizeof(*out));

@@ -783,19 +783,6 @@ int gram_tile_list(int Dp, short* bi_bj_pairs /*[2*max]*/, int max_tiles, int cs
   return n;
 }
 
-// the attribute is per device: set it once for every device this process launches on
-template <typename K>
-static cudaError_t set_smem_once(K kernel, size_t bytes, bool (&configured)[64]) {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64 || !configured[dev]) {
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-    if (e != cudaSuccess) return e;
-    if (dev >= 0 && dev < 64) configured[dev] = true;
-  }
-  return cudaSuccess;
-}
-
 cudaError_t gram_launch_wgmma(const Problem* d_probs, int nprob, const void* d_tmaps, const void* d_tiles, int ntiles,
                               int nslices, int force, cudaStream_t st, int* launches, int share) {
   static bool configured[64] = {};

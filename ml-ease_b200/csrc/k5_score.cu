@@ -279,6 +279,87 @@ __global__ void __launch_bounds__(256) score_keyed_cov_kernel(int Dg, int k0, in
   }
 }
 
+// mlease_score_var: score_kernel's pred (the same sum, the same rounding) and pred_var = float(g^T Sigma g), g = the record's entries
+// and gI at the intercept (column Dg, after every stored column).  Diagonal Sigma (var): each lane its entries, lane 0 the intercept,
+// then warp_sum.  Dense Sigma (cov, ld Dg + 1, lower triangle read): the pair space of the row's 256-entry tiles as
+// score_keyed_cov_kernel walks it (a tile with itself, then with each earlier tile), the intercept's pairs added in the diagonal
+// tile's pass: each lane a fixed set of pairs in a fixed order, then warp_sum.  bad: 1 column out of range, 2 not ascending.
+__global__ void __launch_bounds__(256) score_var_kernel(int Dg, long long nrows, const long long* __restrict__ rowptr, const int* __restrict__ colidx,
+                                                        const float* __restrict__ vals, const float* __restrict__ offset,
+                                                        const double* __restrict__ model, double intercept_term, double gI, int binary_feature,
+                                                        const double* __restrict__ var, const double* __restrict__ cov, float* __restrict__ pred,
+                                                        float* __restrict__ pred_var, int* __restrict__ bad) {
+  __shared__ int scol[8][2][COV_TILE];
+  __shared__ double sx[8][2][COV_TILE];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const long long wg = (long long)blockIdx.x * (blockDim.x >> 5) + w;
+  const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
+  const size_t ld = (size_t)Dg + 1;
+  for (long long i = wg; i < nrows; i += nw) {
+    const long long j0 = rowptr[i], j1 = rowptr[i + 1];
+    double a = 0.0;
+    for (long long j = j0 + lane; j < j1; j += 32) {
+      const int c = colidx[j];
+      if ((unsigned)c >= (unsigned)Dg) { atomicOr(bad, 1); continue; }   // never read outside the model
+      a += model[c] * (binary_feature ? 1.0 : (double)vals[j]);
+    }
+    a = warp_sum(a);
+    if (lane == 0) pred[i] = (float)((offset ? (double)offset[i] : 0.0) + (intercept_term + a));
+    double acc = 0.0;
+    if (var) {
+      for (long long j = j0 + lane; j < j1; j += 32) {
+        const int c = colidx[j];
+        if ((unsigned)c >= (unsigned)Dg) { atomicOr(bad, 1); continue; }
+        if (j > j0 && colidx[j - 1] >= c) atomicOr(bad, 2);
+        const double x = binary_feature ? 1.0 : (double)vals[j];
+        acc += var[c] * x * x;
+      }
+      if (lane == 0) acc += var[Dg] * gI * gI;
+    } else {
+      auto load = [&](long long t0, int slot, bool first) {
+        for (int t = lane; t < COV_TILE; t += 32) {
+          const long long j = t0 + t;
+          int c = -1; double x = 0.0;
+          if (j < j1) {
+            c = colidx[j];
+            x = binary_feature ? 1.0 : (double)vals[j];
+            if ((unsigned)c >= (unsigned)Dg) { if (first) atomicOr(bad, 1); c = -1; x = 0.0; }
+            else {
+              if (first && j > j0 && colidx[j - 1] >= c) atomicOr(bad, 2);
+              if (first) acc += 2.0 * gI * x * cov[(size_t)Dg * ld + c];
+            }
+          }
+          scol[w][slot][t] = c; sx[w][slot][t] = x;
+        }
+        __syncwarp();
+      };
+      for (long long ta = j0; ta < j1; ta += COV_TILE) {
+        const int Ta = (int)min((long long)COV_TILE, j1 - ta);
+        load(ta, 0, true);
+        const long long tri = (long long)Ta * (Ta + 1) / 2;
+        for (long long e = lane; e < tri; e += 32) {
+          const int p = cov_row_of(e), q = (int)(e - (long long)p * (p + 1) / 2);
+          const int ca = scol[w][0][p], cb = scol[w][0][q];
+          if (ca >= 0 && cb >= 0) acc += (p == q ? 1.0 : 2.0) * sx[w][0][p] * sx[w][0][q] * cov[(size_t)max(ca, cb) * ld + min(ca, cb)];
+        }
+        for (long long tb = j0; tb < ta; tb += COV_TILE) {
+          load(tb, 1, false);
+          for (int e = lane; e < Ta * COV_TILE; e += 32) {
+            const int p = e / COV_TILE, q = e % COV_TILE;
+            const int ca = scol[w][0][p], cb = scol[w][1][q];
+            if (ca >= 0 && cb >= 0) acc += 2.0 * sx[w][0][p] * sx[w][1][q] * cov[(size_t)max(ca, cb) * ld + min(ca, cb)];
+          }
+          __syncwarp();
+        }
+        __syncwarp();
+      }
+      if (lane == 0) acc += gI * gI * cov[(size_t)Dg * ld + Dg];
+    }
+    acc = warp_sum(acc);
+    if (lane == 0) pred_var[i] = (float)acc;
+  }
+}
+
 static cudaError_t score_keyed_chunk(int Dg, int K, int k0, int k1, long long r0, long long r1, const long long* krs, const long long* rowptr,
                                      const int* colidx, const float* vals, const float* offset, int G, const long long* mp, const int* mc,
                                      const float* mv, const double* term, int binary_feature, long long nrows, long long row_base, float* table,
@@ -458,6 +539,49 @@ int mlease_score(int32_t device, void* stream, int32_t Dg, int64_t nrows, const 
   if (!pred_dev) CK(cudaMemcpyAsync(pred, d_pred, (size_t)nrows * 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   return 0;
+}
+
+int mlease_score_var(int32_t device, void* stream, int32_t Dg, int64_t nrows, const int64_t* rowptr, const int32_t* colidx, const float* vals,
+                     const float* offset, const double* model, int32_t num_click_replicates, int32_t binary_feature, const double* var,
+                     const double* cov, float* pred, float* pred_var) {
+  if (!vals || !model || !pred || !pred_var || nrows < 0 || Dg <= 0) return fail(MLEASE_ERR_INVALID, "bad argument");
+  if (!colidx || !rowptr) return fail(MLEASE_ERR_INVALID, "score_var takes CSR rows only (rowptr and colidx), not dense input");
+  if ((var != nullptr) == (cov != nullptr)) return fail(MLEASE_ERR_INVALID, "exactly one of var and cov must be given");
+  if (int rc = open_device(device, nullptr)) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  DevMem t;
+  long long nnz;
+  CK(cudaMemcpy(&nnz, rowptr + nrows, 8, cudaMemcpyDefault));
+  const long long* d_rp; const int* d_ci; const float *d_v, *d_o; const double *d_m, *d_var, *d_cov;
+  if (int rc = to_device(t, (const long long*)rowptr, (size_t)nrows + 1, &d_rp, st)) return rc;
+  if (int rc = to_device(t, colidx, (size_t)nnz, &d_ci, st)) return rc;
+  if (int rc = to_device(t, vals, (size_t)nnz, &d_v, st)) return rc;
+  if (int rc = to_device(t, offset, (size_t)nrows, &d_o, st)) return rc;
+  if (int rc = to_device(t, model, (size_t)Dg + 1, &d_m, st)) return rc;
+  if (int rc = to_device(t, var, (size_t)Dg + 1, &d_var, st)) return rc;
+  if (int rc = to_device(t, cov, (size_t)(Dg + 1) * (Dg + 1), &d_cov, st)) return rc;
+  double b;
+  CK(cudaMemcpy(&b, model + Dg, 8, cudaMemcpyDefault));
+  const double n = (double)num_click_replicates;
+  const double ic = -std::log(n - 1 + n * std::exp(-b));   // as mlease_score
+  const double gI = n * std::exp(-b) / (n - 1 + n * std::exp(-b));
+  float* d_pred = pred;
+  float* d_pv = pred_var;
+  if (!is_device_ptr(pred)) { if (int rc = t.get(&d_pred, (size_t)nrows, false)) return rc; }
+  if (!is_device_ptr(pred_var)) { if (int rc = t.get(&d_pv, (size_t)nrows, false)) return rc; }
+  int* d_bad;
+  if (int rc = t.get(&d_bad, 1, true)) return rc;
+  if (nrows > 0) {
+    const long long blocks = std::min<long long>((nrows + 7) / 8, 132LL * 16);
+    score_var_kernel<<<(int)blocks, 256, 0, st>>>(Dg, nrows, d_rp, d_ci, d_v, d_o, d_m, ic, gI, binary_feature, d_var, d_cov, d_pred, d_pv, d_bad);
+    CK(cudaGetLastError());
+  }
+  int bad = 0;
+  CK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, st));
+  if (d_pred != pred) CK(cudaMemcpyAsync(pred, d_pred, (size_t)nrows * 4, cudaMemcpyDeviceToHost, st));
+  if (d_pv != pred_var) CK(cudaMemcpyAsync(pred_var, d_pv, (size_t)nrows * 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return keyed_bad(bad);
 }
 
 int mlease_test_loglik(int32_t device, void* stream, int64_t nrows, const int32_t* response, const float* pred, const float* weight,

@@ -8,6 +8,8 @@
 // The tensor-core Gram (bf16 operands) is a preconditioner-grade H; a reported variance needs the Hessian itself, so these
 // kernels accumulate it in fp64 from the fp32 data (SIMT; n D'^2 / 2 fp64 FMA for the full matrix).  The diagonal runs over a
 // batch of problems (ItemModelTrain's keys, one launch per key chunk and prior) or over a session's one partition.
+#include <cub/device/device_radix_sort.cuh>
+
 #include <algorithm>
 
 #include "kernels.cuh"
@@ -231,6 +233,256 @@ cudaError_t postvar_hessian_batch(const Problem* d_probs, int nprob, int ldh, co
   const int T = ldh / 32;
   postvar_hess_batch_kernel<<<dim3(T, T, nprob), 256, 0, st>>>(d_probs, d_row_start, d_dvec, has_bias);
   if (launches) *launches += 1;
+  return cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------
+// The ADMM model's posterior (mlease_admm_posterior): the exact fp64 Hessian sum_i d_i x~_i x~_i^T of a whole resident partition,
+// added into a sum over partitions.  CSR rows (strictly increasing columns) are walked column by column as the sparse Gram walks
+// them (gram_csr_column_kernel): with the intercept an implicit last entry of every row, the lower triangle's column c1 is
+//     H[c2][c1] = sum over the rows r listing c1 of d_r x_{r,c1} x_{r,c2},   c2 >= c1 in the row's suffix from c1 to its intercept,
+// so every entry read is a product and the column needs only the positions of its entries.  Positions are those of the row-order
+// operand of the sparse Gram's column index (row r at [rowptr[r] + r, rowptr[r + 1] + r], its intercept last): the session's own
+// index where it built one, else one built for the call; rowof[] maps a position back to its row.
+// Determinism: a column belongs to one CTA, which walks its rows in row order (staged HC_STAGE at a time).  Its cells are dealt to
+// the CTA's warps by 32-column groups ((c2 >> 5) & 7), and a warp adds a row's products to its own cells only -- one lane per cell
+// (a row lists a column once) -- with a __syncwarp between rows: every cell is a plain fp64 sum over its rows in row order, no
+// atomics, whatever CTA runs the column or when.  The CTAs take columns from a counter in descending order of their work (the summed
+// suffix lengths of their rows) so that the costly columns of a skewed dictionary start first.  The intercept's own cell, sum_i d_i,
+// is a fixed-order block reduction.  The work is sum_i n_i (n_i + 1) / 2 fp64 FMAs with n_i the row's entries plus its intercept:
+// ~5e9 at 1M x 10k x 1 %; every warp reads every suffix of its column (from L1 after the first), each adds only its cells' products.
+// ------------------------------------------------------------------------------------------
+constexpr int HC_THREADS = 256;
+constexpr int HC_WARPS = HC_THREADS / 32;
+constexpr int HC_STAGE = 256;        // column positions staged per step
+constexpr int HC_CELLS = 12288;      // fp64 cells of a column window: 96 KB, two CTAs an SM
+
+// rowof[q] = r for every position q of row r (its entries and its intercept)
+__global__ void __launch_bounds__(256) postvar_rowof_kernel(long long n, const long long* __restrict__ rowptr, uint32_t* __restrict__ rowof) {
+  const int lane = threadIdx.x & 31;
+  const long long nw = ((long long)gridDim.x * blockDim.x) >> 5;
+  for (long long r = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < n; r += nw)
+    for (long long j = rowptr[r] + lane; j <= rowptr[r + 1]; j += 32) rowof[j + r] = (uint32_t)r;
+}
+
+// cost[c] = the products column c's walk forms (the suffix lengths of its positions, intercept included), cols[c] = c
+__global__ void __launch_bounds__(256) postvar_colcost_kernel(int Dt, const long long* __restrict__ rowptr, const uint32_t* __restrict__ offs,
+                                                              const uint32_t* __restrict__ pos, const uint32_t* __restrict__ rowof,
+                                                              unsigned long long* __restrict__ cost, int* __restrict__ cols) {
+  const int lane = threadIdx.x & 31;
+  const int nw = (gridDim.x * blockDim.x) >> 5;
+  for (int c = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; c < Dt; c += nw) {
+    unsigned long long s = 0;
+    for (uint32_t i = offs[c] + lane; i < offs[c + 1]; i += 32) {
+      const uint32_t q = pos[i], r = rowof[q];
+      s += (unsigned long long)(rowptr[r + 1] + r + 1 - q);
+    }
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) s += __shfl_down_sync(0xffffffffu, s, d);
+    if (lane == 0) { cost[c] = s; cols[c] = c; }
+  }
+}
+
+struct HessCsr {
+  long long n;
+  const long long* rowptr;
+  const int* colidx;
+  const float* vals;
+  const double* d;
+  const uint32_t *offs, *pos, *rowof;
+  const int* order;   // columns, costliest first
+  int* next;          // column counter (0 before the launch)
+  int Dt, ldh;
+  double* H;          // += into the lower triangle, ld = ldh
+};
+
+__global__ void __launch_bounds__(HC_THREADS, 2) postvar_hess_col_kernel(HessCsr a) {
+  extern __shared__ __align__(16) unsigned char hc_smem_raw[];
+  double* acc = reinterpret_cast<double*>(hc_smem_raw);
+  __shared__ long long sj[HC_STAGE];
+  __shared__ int slen[HC_STAGE];
+  __shared__ double sx[HC_STAGE];
+  __shared__ double red[HC_WARPS];
+  __shared__ int s_k;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int hot = a.Dt - 1, W = min(a.Dt, HC_CELLS);
+  while (true) {
+    if (threadIdx.x == 0) s_k = atomicAdd(a.next, 1);
+    __syncthreads();
+    const int k = s_k;
+    __syncthreads();
+    if (k >= a.Dt) return;
+    const int c1 = a.order[k];
+    if (c1 == hot) {   // every row's intercept squared: sum_i d_i
+      double s = 0.0;
+      for (long long r = threadIdx.x; r < a.n; r += HC_THREADS) s += a.d[r];
+      s = warp_sum(s);
+      if (lane == 0) red[warp] = s;
+      __syncthreads();
+      if (threadIdx.x == 0) {
+        double t = 0.0;
+        for (int w = 0; w < HC_WARPS; w++) t += red[w];
+        a.H[(size_t)hot * a.ldh + hot] += t;
+      }
+      continue;
+    }
+    const uint32_t p0 = a.offs[c1], p1 = a.offs[c1 + 1];
+    for (int w0 = c1; w0 < a.Dt; w0 += W) {
+      const int w1 = min(a.Dt, w0 + W);
+      for (int e = threadIdx.x; e < w1 - w0; e += HC_THREADS) acc[e] = 0.0;
+      __syncthreads();
+      for (uint32_t b0 = p0; b0 < p1; b0 += HC_STAGE) {
+        const int cnt = (int)min((uint32_t)HC_STAGE, p1 - b0);
+        if (threadIdx.x < cnt) {
+          const uint32_t q = a.pos[b0 + threadIdx.x], r = a.rowof[q];
+          const long long j = (long long)q - r;
+          sj[threadIdx.x] = j;
+          slen[threadIdx.x] = (int)(a.rowptr[r + 1] - j);   // stored entries from c1 on; the intercept follows
+          sx[threadIdx.x] = a.d[r] * (double)a.vals[j];
+        }
+        __syncthreads();
+        for (int t = 0; t < cnt; t++) {
+          const long long j = sj[t];
+          const int len = slen[t];
+          const double x = sx[t];
+          for (int e = lane; e <= len; e += 32) {
+            const int c2 = e < len ? a.colidx[j + e] : hot;
+            if (c2 >= w0 && c2 < w1 && ((c2 >> 5) & (HC_WARPS - 1)) == warp) acc[c2 - w0] += x * (e < len ? (double)a.vals[j + e] : 1.0);
+          }
+          __syncwarp();
+        }
+        __syncthreads();
+      }
+      for (int e = threadIdx.x; e < w1 - w0; e += HC_THREADS) a.H[(size_t)(w0 + e) * a.ldh + c1] += acc[e];
+      __syncthreads();
+    }
+  }
+}
+
+// Diagonal mode, CSR: diag[c] += sum over the positions of column c of d_r x_rc^2 (x = 1 at the intercept), in row order per lane
+// then warp_sum
+__global__ void __launch_bounds__(256) postvar_diag_col_kernel(int Dt, const long long* __restrict__ rowptr, const float* __restrict__ vals,
+                                                               const double* __restrict__ d, const uint32_t* __restrict__ offs,
+                                                               const uint32_t* __restrict__ pos, const uint32_t* __restrict__ rowof,
+                                                               double* __restrict__ diag) {
+  const int lane = threadIdx.x & 31;
+  const int nw = (gridDim.x * blockDim.x) >> 5;
+  for (int c = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; c < Dt; c += nw) {
+    double s = 0.0;
+    for (uint32_t i = offs[c] + lane; i < offs[c + 1]; i += 32) {
+      const uint32_t q = pos[i], r = rowof[q];
+      const long long j = (long long)q - r;
+      const double x = j < rowptr[r + 1] ? (double)vals[j] : 1.0;
+      s += d[r] * x * x;
+    }
+    s = warp_sum(s);
+    if (lane == 0) diag[c] += s;
+  }
+}
+
+// Diagonal mode, dense rows (the intercept is the physical column Dt - 1 of 1.0f): diag[k] += sum_i d_i x_ik^2 in row order
+__global__ void __launch_bounds__(256) postvar_diag_dense_kernel(long long n, int Dt, const float* __restrict__ X, int ldx, const double* __restrict__ d,
+                                                                 double* __restrict__ diag) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= Dt) return;
+  double s = 0.0;
+  for (long long i = 0; i < n; i++) { const double x = (double)X[(size_t)i * ldx + k]; s += d[i] * x * x; }
+  diag[k] += s;
+}
+
+// Lc = Hs + diag(q) on the lower triangle of [0, Dt), identity on the padding, zero above the diagonal (as chol_prep leaves it)
+__global__ void postvar_lc_kernel(const double* __restrict__ Hs, const double* __restrict__ q, int Dt, int ldh, double* __restrict__ Lc) {
+  const size_t total = (size_t)ldh * ldh;
+  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
+    const int i = (int)(e / ldh), j = (int)(e % ldh);
+    Lc[e] = (i < Dt && j <= i) ? Hs[e] + (i == j ? q[i] : 0.0) : (i == j ? 1.0 : 0.0);
+  }
+}
+
+// the lower triangle of [0, Dt) (ld ldh) to / from packed rows (i (i + 1) / 2 + j): the all-reduce sends Dt (Dt + 1) / 2 doubles
+__global__ void postvar_pack_kernel(double* __restrict__ H, int Dt, int ldh, double* __restrict__ packed, int unpack) {
+  const size_t total = (size_t)Dt * (Dt + 1) / 2;
+  for (size_t e = (size_t)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (size_t)gridDim.x * blockDim.x) {
+    int i = (int)((sqrt(8.0 * (double)e + 1.0) - 1.0) * 0.5);
+    while ((size_t)i * (i + 1) / 2 > e) i--;
+    while ((size_t)(i + 1) * (i + 2) / 2 <= e) i++;
+    const int j = (int)(e - (size_t)i * (i + 1) / 2);
+    if (unpack) H[(size_t)i * ldh + j] = packed[e];
+    else packed[e] = H[(size_t)i * ldh + j];
+  }
+}
+
+cudaError_t postvar_rowof(long long n, const long long* rowptr, uint32_t* rowof, cudaStream_t st) {
+  postvar_rowof_kernel<<<(int)std::max(1LL, std::min((n + 7) / 8, 132LL * 32)), 256, 0, st>>>(n, rowptr, rowof);
+  return cudaGetLastError();
+}
+
+cudaError_t postvar_hessian_csr_cols(long long n, const long long* rowptr, const int* colidx, const float* vals, const double* d_dvec,
+                                     const uint32_t* offs, const uint32_t* pos, const uint32_t* rowof, int Dt, int ldh, double* H, cudaStream_t st) {
+  static bool configured[64] = {};
+  static int sms[64] = {};
+  cudaError_t e = set_smem_once(postvar_hess_col_kernel, HC_CELLS * sizeof(double), configured);
+  if (e != cudaSuccess) return e;
+  int dev = 0, nsm = 0;
+  if ((e = cudaGetDevice(&dev)) != cudaSuccess) return e;
+  if (dev >= 0 && dev < 64 && sms[dev]) nsm = sms[dev];
+  else {
+    if ((e = cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev)) != cudaSuccess) return e;
+    if (dev >= 0 && dev < 64) sms[dev] = nsm;
+  }
+  const size_t smem = (size_t)std::min(Dt, HC_CELLS) * sizeof(double);
+  // the column order: descending cost, ties in column order (stable sort)
+  unsigned long long *cost = nullptr, *cost_s = nullptr;
+  int *cols = nullptr, *order = nullptr, *next = nullptr;
+  void* tmp = nullptr;
+  size_t tmp_bytes = 0;
+  auto run = [&]() -> cudaError_t {
+    cudaError_t r;
+    if ((r = cudaMallocAsync(&cost, (size_t)Dt * 8, st)) != cudaSuccess) return r;
+    if ((r = cudaMallocAsync(&cost_s, (size_t)Dt * 8, st)) != cudaSuccess) return r;
+    if ((r = cudaMallocAsync(&cols, (size_t)Dt * 4, st)) != cudaSuccess) return r;
+    if ((r = cudaMallocAsync(&order, (size_t)Dt * 4, st)) != cudaSuccess) return r;
+    if ((r = cudaMallocAsync(&next, 4, st)) != cudaSuccess) return r;
+    if ((r = cudaMemsetAsync(next, 0, 4, st)) != cudaSuccess) return r;
+    postvar_colcost_kernel<<<std::max(1, std::min((Dt + 7) / 8, 132 * 32)), 256, 0, st>>>(Dt, rowptr, offs, pos, rowof, cost, cols);
+    if ((r = cudaGetLastError()) != cudaSuccess) return r;
+    if ((r = cub::DeviceRadixSort::SortPairsDescending(nullptr, tmp_bytes, cost, cost_s, cols, order, Dt, 0, 64, st)) != cudaSuccess) return r;
+    if ((r = cudaMallocAsync(&tmp, tmp_bytes ? tmp_bytes : 16, st)) != cudaSuccess) return r;
+    if ((r = cub::DeviceRadixSort::SortPairsDescending(tmp, tmp_bytes, cost, cost_s, cols, order, Dt, 0, 64, st)) != cudaSuccess) return r;
+    HessCsr a{n, rowptr, colidx, vals, d_dvec, offs, pos, rowof, order, next, Dt, ldh, H};
+    postvar_hess_col_kernel<<<std::max(1, std::min(Dt, 2 * nsm)), HC_THREADS, smem, st>>>(a);
+    return cudaGetLastError();
+  };
+  e = run();
+  for (void* p : {(void*)cost, (void*)cost_s, (void*)cols, (void*)order, (void*)next, tmp})
+    if (p) { cudaError_t e2 = cudaFreeAsync(p, st); if (e == cudaSuccess) e = e2; }
+  return e;
+}
+
+cudaError_t postvar_hessian_dense_add(const Problem* d_prob, int ldh, const double* d_dvec, cudaStream_t st) {
+  const int T = ldh / 32;
+  postvar_hess_dense_kernel<<<dim3(T, T), 256, 0, st>>>(d_prob, d_dvec);
+  return cudaGetLastError();
+}
+
+cudaError_t postvar_diag_csr_cols(const long long* rowptr, const float* vals, const double* d_dvec, const uint32_t* offs, const uint32_t* pos,
+                                  const uint32_t* rowof, int Dt, double* diag, cudaStream_t st) {
+  postvar_diag_col_kernel<<<std::max(1, std::min((Dt + 7) / 8, 132 * 32)), 256, 0, st>>>(Dt, rowptr, vals, d_dvec, offs, pos, rowof, diag);
+  return cudaGetLastError();
+}
+
+cudaError_t postvar_diag_dense(long long n, int Dt, const float* X, int ldx, const double* d_dvec, double* diag, cudaStream_t st) {
+  postvar_diag_dense_kernel<<<(Dt + 127) / 128, 128, 0, st>>>(n, Dt, X, ldx, d_dvec, diag);
+  return cudaGetLastError();
+}
+
+cudaError_t postvar_lc(const double* Hs, const double* d_q, int Dt, int ldh, double* Lc, cudaStream_t st) {
+  postvar_lc_kernel<<<1184, 256, 0, st>>>(Hs, d_q, Dt, ldh, Lc);
+  return cudaGetLastError();
+}
+
+cudaError_t postvar_pack(double* H, int Dt, int ldh, double* packed, int unpack, cudaStream_t st) {
+  postvar_pack_kernel<<<1184, 256, 0, st>>>(H, Dt, ldh, packed, unpack);
   return cudaGetLastError();
 }
 

@@ -4,6 +4,19 @@
 
 namespace mlease {
 
+// the dynamic shared-memory attribute is per device: set it once for every device this process launches on
+template <typename K>
+inline cudaError_t set_smem_once(K kernel, size_t bytes, bool (&configured)[64]) {
+  int dev = 0;
+  cudaGetDevice(&dev);
+  if (dev < 0 || dev >= 64 || !configured[dev]) {
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    if (e != cudaSuccess) return e;
+    if (dev >= 0 && dev < 64) configured[dev] = true;
+  }
+  return cudaSuccess;
+}
+
 // K1 (k1_score_grad.cu)
 bool k1_dense_plan(int ldx, int* R_out, int* S_out, int* G_out, size_t* smem_out, int* ctas_per_sm);
 int k1_csr_window(int ldx);
@@ -95,5 +108,20 @@ cudaError_t postvar_hessian(const Problem* d_prob, bool csr, int ldh, const doub
 // Lc, as chol_prep leaves it; deterministic (no atomics, every cell summed in row order)
 cudaError_t postvar_hessian_batch(const Problem* d_probs, int nprob, int ldh, const long long* d_row_start, const double* d_dvec, int has_bias,
                                   cudaStream_t st, int* launches);
+// the ADMM model's posterior (mlease_admm_posterior): every kernel is deterministic (fixed summation order, no atomics on values).
+// rowof: rowof[q] = r for the n + nnz positions of the sparse Gram's row-order operand (row r at [rowptr[r] + r, rowptr[r + 1] + r]).
+// hessian_csr_cols: H[c2][c1] += sum_i d_i x_{i,c1} x_{i,c2} (c2 >= c1, the intercept an implicit column Dt - 1, ld ldh) of one CSR
+// partition with strictly increasing columns, from the column index offs [Dt + 1] / pos and rowof; hessian_dense_add: the same for the
+// dense rows of d_prob[0] into its Lc (ld ldh); diag_*: diag[k] += sum_i d_i x_ik^2; lc: Lc = Hs + diag(q) as chol_prep leaves it;
+// pack: the lower triangle of [0, Dt) to (unpack = 0) or from (1) Dt (Dt + 1) / 2 packed doubles
+cudaError_t postvar_rowof(long long n, const long long* rowptr, uint32_t* rowof, cudaStream_t st);
+cudaError_t postvar_hessian_csr_cols(long long n, const long long* rowptr, const int* colidx, const float* vals, const double* d_dvec,
+                                     const uint32_t* offs, const uint32_t* pos, const uint32_t* rowof, int Dt, int ldh, double* H, cudaStream_t st);
+cudaError_t postvar_hessian_dense_add(const Problem* d_prob, int ldh, const double* d_dvec, cudaStream_t st);
+cudaError_t postvar_diag_csr_cols(const long long* rowptr, const float* vals, const double* d_dvec, const uint32_t* offs, const uint32_t* pos,
+                                  const uint32_t* rowof, int Dt, double* diag, cudaStream_t st);
+cudaError_t postvar_diag_dense(long long n, int Dt, const float* X, int ldx, const double* d_dvec, double* diag, cudaStream_t st);
+cudaError_t postvar_lc(const double* Hs, const double* d_q, int Dt, int ldh, double* Lc, cudaStream_t st);
+cudaError_t postvar_pack(double* H, int Dt, int ldh, double* packed, int unpack, cudaStream_t st);
 
 }  // namespace mlease

@@ -733,3 +733,176 @@ int mlease_time_kernel(mlease_session* s, int32_t pid, int32_t which, int32_t re
 }
 
 }  // extern "C"
+
+// ------------------------------------------------------------------------------------------
+// The ADMM model's posterior (include/mlease_b200.h, mlease_admm_posterior)
+// ------------------------------------------------------------------------------------------
+// The checks a rank makes before it allocates anything; with a communicator every rank then votes, so that a refusal on one rank
+// is a refusal on all of them instead of a hang in the collective.
+static int admm_post_check(mlease_session* s, int l, const double* z, int full, int* ldh) {
+  if (s->cfg.regularizer == 1) return fail(MLEASE_ERR_INVALID, "the L1 penalty has no Hessian: the posterior needs regularizer = 2");
+  if (l < 0 || l >= s->L) return fail(MLEASE_ERR_INVALID, "lambda index " + std::to_string(l) + " out of range [0, " + std::to_string(s->L) + ")");
+  if (!z && !s->batch) return fail(MLEASE_ERR_STATE, "no consensus z yet: call mlease_admm_begin (or pass z)");
+  if (int rc = csr_flush_pending(s)) return rc;
+  for (const PartData& pd : s->parts) {
+    if (!pd.csr) continue;
+    if (pd.data.nnz_hint > 0 && !pd.data.csr_unique)
+      return fail(MLEASE_ERR_INVALID, "partition " + std::to_string(pd.pid) + ": the posterior needs rows with strictly increasing column ids");
+    if (pd.data.nnz_hint + pd.data.n >= (1LL << 32) - 64)
+      return fail(MLEASE_ERR_INVALID, "partition " + std::to_string(pd.pid) + ": the column index holds fewer than 2^32 - 64 entries");
+  }
+  *ldh = round_up(s->Dt, 32);
+  if (full) {
+    // the sum, Lc, Yinv and Hinv, ldh^2 doubles each
+    const double need = 4.0 * 8.0 * (double)*ldh * (double)*ldh;
+    size_t free_b = 0, total_b = 0;
+    CK(cudaMemGetInfo(&free_b, &total_b));
+    if (need + (256.0 * 1024 * 1024) > (double)free_b)
+      return fail(MLEASE_ERR_INVALID, "the full posterior of " + std::to_string(s->Dt) + " columns needs " + std::to_string((long long)need) +
+                                          " bytes of device memory (4 x 8 x ldh^2, ldh = " + std::to_string(*ldh) + "), " + std::to_string(free_b) +
+                                          " are free: use full = 0");
+  }
+  return 0;
+}
+
+extern "C" {
+
+// With a communicator every rank calls this at the same point: a rank whose local work failed (rc_local, its message local_msg)
+// returns that error, the others learn that one failed, and none is left waiting in a later collective.
+static int post_vote(mlease_session* s, int rc_local, const std::string& local_msg) {
+  if (!s->comm) return rc_local ? fail(rc_local, local_msg) : 0;
+  DevMem t;
+  double* d_vote;
+  if (int rc = t.get(&d_vote, 1, false)) return rc;
+  const double vote = rc_local ? 1.0 : 0.0;
+  CK(cudaMemcpy(d_vote, &vote, 8, cudaMemcpyHostToDevice));
+  if (int rc = comm_allreduce(s->comm, d_vote, 1, s->stream)) return rc;
+  double votes = 0;
+  CK(cudaMemcpyAsync(&votes, d_vote, 8, cudaMemcpyDeviceToHost, s->stream));
+  CK(cudaStreamSynchronize(s->stream));
+  if (rc_local) return fail(rc_local, local_msg);
+  if (votes > 0) return fail(MLEASE_ERR_INVALID, "the posterior failed on " + std::to_string((int)votes) + " other rank(s)");
+  return 0;
+}
+
+int mlease_admm_posterior(mlease_session* s, int32_t l, const double* z, int32_t full, double* var, double* cov) {
+  if (!s || !var) return fail(MLEASE_ERR_INVALID, "null argument");
+  if (cov && !full) return fail(MLEASE_ERR_INVALID, "the covariance matrix is only available with full = 1");
+  CK(cudaSetDevice(s->cfg.device));
+  const cudaStream_t st = s->stream;
+  int ldh = 0;
+  int rc_local = admm_post_check(s, l, z, full, &ldh);
+  std::string local_msg = rc_local ? mlease_last_error() : "";
+  DevMem t;
+  if (int rc = post_vote(s, rc_local, local_msg)) return rc;
+  const int Dt = s->Dt, ldx = s->ldx;
+  // q: lambda, lambda_map's own lambda for a listed feature, the intercept's lambda only with penalize_intercept
+  std::vector<double> q(ldh, 1.0);
+  for (int k = 0; k < s->Dg; k++) q[k] = (!s->lambda_map.empty() && s->lambda_map[k] > 0.f) ? (double)s->lambda_map[k] : (double)s->lambdas[l];
+  q[s->Dg] = s->cfg.penalize_intercept ? (double)s->lambdas[l] : 0.0;
+  double *d_z, *d_q, *Hs = nullptr, *Lc = nullptr, *Yi = nullptr, *Hi = nullptr, *diag = nullptr;
+  Problem* d_prob = nullptr;
+  // this rank's sum; every rank votes on its outcome before the all-reduce (an allocation or launch may fail on one rank only)
+  auto local_sum = [&]() -> int {
+    if (int rc = t.get(&d_z, ldx, true)) return rc;
+    if (int rc = t.get(&d_q, ldh, false)) return rc;
+    if (z) CK(cudaMemcpy(d_z, z, (size_t)Dt * 8, cudaMemcpyDefault));
+    else CK(cudaMemcpyAsync(d_z, s->d_z + (size_t)l * ldx, (size_t)Dt * 8, cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync(d_q, q.data(), (size_t)ldh * 8, cudaMemcpyHostToDevice, st));
+    const size_t hh = (size_t)ldh * ldh;
+    if (full) {
+      if (int rc = t.get(&Hs, hh, true)) return rc;
+      if (int rc = t.get(&Lc, hh, false)) return rc;
+      if (int rc = t.get(&Yi, hh, false)) return rc;
+      if (int rc = t.get(&Hi, hh, false)) return rc;
+    } else {
+      if (int rc = t.get(&diag, Dt, true)) return rc;
+    }
+    // the partitions in partition-id order, whatever order they were uploaded in
+    std::vector<int> order(s->parts.size());
+    for (size_t i = 0; i < order.size(); i++) order[i] = (int)i;
+    std::sort(order.begin(), order.end(), [&](int a, int b) { return s->parts[a].pid < s->parts[b].pid; });
+    long long nmax = 1;
+    for (const PartData& pd : s->parts) nmax = std::max(nmax, pd.data.n);
+    double* dvec;
+    long long* drs;
+    if (int rc = t.get(&dvec, (size_t)nmax, false)) return rc;
+    if (int rc = t.get(&drs, 2, false)) return rc;
+    if (int rc = t.get(&d_prob, 1, false)) return rc;
+    for (int pi : order) {
+      const PartData& pd = s->parts[pi];
+      Problem p = pd.data;
+      p.beta = d_z; p.Dt = Dt; p.ldx = ldx; p.Lc = Hs; p.ldh = ldh;
+      const long long rs[2] = {0, p.n};
+      CK(cudaMemcpyAsync(drs, rs, sizeof(rs), cudaMemcpyHostToDevice, st));
+      CK(cudaMemcpyAsync(d_prob, &p, sizeof(Problem), cudaMemcpyHostToDevice, st));
+      CK(postvar_rowweights(d_prob, 1, drs, p.n, 1, dvec, st, nullptr));   // d_i = w_i p_i (1 - p_i) at z, the row's offset included
+      if (!pd.csr) {
+        if (full) CK(postvar_hessian_dense_add(d_prob, ldh, dvec, st));
+        else CK(postvar_diag_dense(p.n, Dt, p.X, ldx, dvec, diag, st));
+      } else {
+        // the sparse Gram's column index where the session built one, else one for this partition alone
+        DevMem ti;
+        const long long entries = p.nnz_hint + p.n;
+        const uint32_t *offs = p.gc_offs, *pos = p.gc_pos;
+        if (!offs) {
+          uint32_t *o, *ps;
+          if (int rc = ti.get(&o, (size_t)Dt + 1, false)) return rc;
+          if (int rc = ti.get(&ps, (size_t)entries, false)) return rc;
+          CK(csr_col_index(p.n, p.rowptr, p.colidx, s->Dg, entries, o, ps, st));
+          offs = o; pos = ps;
+        }
+        uint32_t* rowof;
+        if (int rc = ti.get(&rowof, (size_t)entries, false)) return rc;
+        CK(postvar_rowof(p.n, p.rowptr, rowof, st));
+        if (full) CK(postvar_hessian_csr_cols(p.n, p.rowptr, p.colidx, p.vals, dvec, offs, pos, rowof, Dt, ldh, Hs, st));
+        else CK(postvar_diag_csr_cols(p.rowptr, p.vals, dvec, offs, pos, rowof, Dt, diag, st));
+        CK(cudaStreamSynchronize(st));   // ti is freed on the way out of this scope
+      }
+    }
+    return 0;
+  };
+  rc_local = local_sum();
+  local_msg = rc_local ? mlease_last_error() : "";
+  if (int rc = post_vote(s, rc_local, local_msg)) return rc;
+  // the sum over ranks: one fp64 all-reduce of the packed lower triangle (Lc is free until the factorisation) or of the diagonal
+  if (s->comm) {
+    if (full) {
+      CK(postvar_pack(Hs, Dt, ldh, Lc, 0, st));
+      if (int rc = comm_allreduce(s->comm, Lc, (size_t)Dt * (Dt + 1) / 2, st)) return rc;
+      CK(postvar_pack(Hs, Dt, ldh, Lc, 1, st));
+    } else if (int rc = comm_allreduce(s->comm, diag, (size_t)Dt, st)) {
+      return rc;
+    }
+  }
+  if (!full) {
+    CK(cudaMemcpyAsync(var, diag, (size_t)Dt * 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    for (int k = 0; k < Dt; k++) var[k] = 1.0 / (q[k] + var[k]);
+    return 0;
+  }
+  // diag(q), then K3's fp64 factorisation and explicit inverse on a one-problem batch of the call's own buffers
+  double *Ld, *Ldi;
+  Ctrl* d_ctrl;
+  if (int rc = t.get(&Ld, (size_t)ldh * 32, true)) return rc;
+  if (int rc = t.get(&Ldi, (size_t)ldh * 32, true)) return rc;
+  if (int rc = t.get(&d_ctrl, 1, true)) return rc;
+  Problem f{};
+  f.Dt = Dt; f.ldx = ldx; f.ldh = ldh; f.Dp = round_up(ldx, 128);
+  f.Lc = Lc; f.Yinv = Yi; f.Hinv = Hi; f.Ldiag = Ld; f.Ldinv = Ldi; f.q = d_q; f.ctrl = d_ctrl;
+  Ctrl c; std::memset(&c, 0, sizeof(c)); c.need_hess = 1;
+  CK(cudaMemcpyAsync(d_ctrl, &c, sizeof(Ctrl), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(d_prob, &f, sizeof(Problem), cudaMemcpyHostToDevice, st));
+  CK(postvar_lc(Hs, d_q, Dt, ldh, Lc, st));
+  int launches = 0;
+  CK(cholesky_launch(d_prob, 1, ldh, st, &launches, 0, 1, 1));
+  CK(cudaMemcpyAsync(&c, d_ctrl, sizeof(Ctrl), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpy2DAsync(var, 8, Hi, (size_t)(ldh + 1) * 8, 8, Dt, cudaMemcpyDeviceToHost, st));
+  if (cov) CK(cudaMemcpy2DAsync(cov, (size_t)Dt * 8, Hi, (size_t)ldh * 8, (size_t)Dt * 8, Dt, cudaMemcpyDefault, st));
+  CK(cudaStreamSynchronize(st));
+  s->cnt.launches += launches;
+  if (c.fail) return fail(MLEASE_ERR_NUMERIC, "the ADMM model's Hessian is not positive definite");
+  return 0;
+}
+
+}  // extern "C"

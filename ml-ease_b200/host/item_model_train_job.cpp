@@ -8,14 +8,6 @@
 namespace mlease_jobs {
 namespace {
 
-const char* SCHEMA_MODEL_WITH_VAR =
-    "{\"type\":\"record\",\"name\":\"LinearModelWithVarAvro\",\"namespace\":\"com.linkedin.mlease.avro\",\"doc\":\"Linear Model with posterior variance in Avro\","
-    "\"fields\":[{\"name\":\"key\",\"type\":\"string\"},"
-    "{\"name\":\"model\",\"type\":{\"type\":\"array\",\"items\":{\"type\":\"record\",\"name\":\"feature\",\"fields\":["
-    "{\"name\":\"name\",\"type\":\"string\"},{\"name\":\"term\",\"type\":\"string\"},{\"name\":\"value\",\"type\":\"float\"}]}}},"
-    "{\"name\":\"posteriorVar\",\"type\":{\"type\":\"array\",\"items\":{\"type\":\"record\",\"name\":\"featureVar\",\"fields\":["
-    "{\"name\":\"name\",\"type\":\"string\"},{\"name\":\"term\",\"type\":\"string\"},{\"name\":\"value\",\"type\":\"float\"}]}}}]}";
-
 // intercept.prior.mean.map: Pair records {key, value}, value = Double.parseDouble(value.toString()) (:293-301), so a float value
 // is read through its Float.toString digits
 std::unordered_map<std::string, double> read_prior_mean_map(const std::string& path) {

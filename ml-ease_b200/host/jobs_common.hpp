@@ -148,6 +148,7 @@ struct FeaturePrefix {
   }
 };
 extern const char* SCHEMA_TEST_LOGLIK;
+extern const char* SCHEMA_MODEL_WITH_VAR;
 
 // regression_jobs.cpp
 std::string java_float_to_string(float f);
@@ -171,6 +172,10 @@ void transcode_plain(const Plan& pl, const uint8_t*& p, const uint8_t* e, std::s
 
 // gpu.devices = 0,1,2,...  (falls back to the single gpu.device, default 0)
 std::vector<int32_t> gpu_devices(const JobConfig& c);
+// Integer.parseInt; RegressionAdmmTrain's lambda list (Float.parseFloat); lambda.map as a dense [D] vector over dict (0 = not listed)
+int java_parse_int(const std::string& s);
+std::vector<float> parse_lambdas(const JobConfig& c);
+std::vector<float> read_lambda_map(const std::string& path, const Dictionary& dict);
 
 // ------------------------------------------------------------------------------------------ keyed jobs on several GPUs
 // Keys are independent, so a keyed job (NaiveTrain, ItemModelTrain, ItemModelTest, ItemModelGridTest) cuts them into one contiguous range per device,

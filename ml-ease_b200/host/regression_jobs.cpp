@@ -120,6 +120,14 @@ std::string schema_train_output() {
 }
 const char* SCHEMA_LAMBDA_RHO = "{\"type\":\"record\",\"name\":\"LambdaRhoMap\",\"namespace\":\"com.linkedin.mlease.regression.avro\",\"fields\":[{\"name\":\"lambda\",\"type\":\"float\"},{\"name\":\"rho\",\"type\":\"float\"}]}";
 const char* SCHEMA_SAMPLE_LOGLIK = "{\"type\":\"record\",\"name\":\"SampleTestLoglik\",\"namespace\":\"com.linkedin.mlease.regression.avro\",\"fields\":[{\"name\":\"lambda\",\"type\":\"string\"},{\"name\":\"iter\",\"type\":\"int\"},{\"name\":\"testLoglik\",\"type\":\"float\"}]}";
+// LinearModelWithVarAvro (ItemModelTrain, RegressionPosterior)
+const char* SCHEMA_MODEL_WITH_VAR =
+    "{\"type\":\"record\",\"name\":\"LinearModelWithVarAvro\",\"namespace\":\"com.linkedin.mlease.avro\",\"doc\":\"Linear Model with posterior variance in Avro\","
+    "\"fields\":[{\"name\":\"key\",\"type\":\"string\"},"
+    "{\"name\":\"model\",\"type\":{\"type\":\"array\",\"items\":{\"type\":\"record\",\"name\":\"feature\",\"fields\":["
+    "{\"name\":\"name\",\"type\":\"string\"},{\"name\":\"term\",\"type\":\"string\"},{\"name\":\"value\",\"type\":\"float\"}]}}},"
+    "{\"name\":\"posteriorVar\",\"type\":{\"type\":\"array\",\"items\":{\"type\":\"record\",\"name\":\"featureVar\",\"fields\":["
+    "{\"name\":\"name\",\"type\":\"string\"},{\"name\":\"term\",\"type\":\"string\"},{\"name\":\"value\",\"type\":\"float\"}]}}}]}";
 const char* SCHEMA_TEST_LOGLIK = "{\"type\":\"record\",\"name\":\"RegressionTestLoglikOutput\",\"namespace\":\"com.linkedin.mlease.regression.avro\",\"fields\":[{\"name\":\"key\",\"type\":\"string\"},{\"name\":\"testLoglik\",\"type\":\"float\"},{\"name\":\"count\",\"type\":\"double\"}]}";
 const char* SCHEMA_PARTITION_ID = "{\"type\":\"record\",\"name\":\"Pair\",\"namespace\":\"org.apache.avro.mapred\",\"fields\":[{\"name\":\"key\",\"type\":\"string\"},{\"name\":\"value\",\"type\":\"int\"}]}";
 

@@ -261,6 +261,15 @@ class AdmmSession:
         check(lib().mlease_posterior_variance(self._h, int(partition_id), ptr(w), ptr(q), int(bool(full)), ptr(var), ptr(cov)))
         return (var, cov) if want_cov else var
 
+    def admm_posterior(self, lambda_idx=0, z=None, full=False, want_cov=False):
+        """Posterior of the ADMM model at z (default: the consensus z of lambda_idx) over all partitions (and all ranks of an attached
+        communicator: collective then).  -> var [Dt], or (var, cov [Dt, Dt]) with want_cov (full only)."""
+        zz = None if z is None else np.ascontiguousarray(z, np.float64)
+        var = np.zeros(self.Dt, np.float64)
+        cov = np.zeros((self.Dt, self.Dt), np.float64) if want_cov else None
+        check(lib().mlease_admm_posterior(self._h, int(lambda_idx), ptr(zz), int(bool(full)), ptr(var), ptr(cov)))
+        return (var, cov) if want_cov else var
+
     def profile(self, enable=-1):
         """Per-kernel CUDA-event timing accumulators; enable: 1 on, 0 off, 2 on+reset, -1 read only."""
         ms = np.zeros(4, np.float64); cnt = np.zeros(4, np.int64)
@@ -367,6 +376,14 @@ class World:
     def uplusx(self, partition_id, lambda_idx=0):
         return self._vec(lib().mlease_world_get_uplusx, partition_id, lambda_idx, np.float32)
 
+    def admm_posterior(self, lambda_idx=0, z=None, full=False, want_cov=False):
+        """AdmmSession.admm_posterior over every device of the world."""
+        zz = None if z is None else np.ascontiguousarray(z, np.float64)
+        var = np.zeros(self.Dt, np.float64)
+        cov = np.zeros((self.Dt, self.Dt), np.float64) if want_cov else None
+        check(lib().mlease_world_admm_posterior(self._h, int(lambda_idx), ptr(zz), int(bool(full)), ptr(var), ptr(cov)))
+        return (var, cov) if want_cov else var
+
     def stats(self):
         s = StatsC()
         check(lib().mlease_world_get_stats(self._h, C.byref(s)))
@@ -390,6 +407,23 @@ def score(vals, model, *, rowptr=None, colidx=None, offset=None, num_features=No
     check(lib().mlease_score(device, stream, Dg, n, ptr(rp), ptr(ci), ptr(vals), ld, ptr(o), ptr(model), int(num_click_replicates),
                              int(binary_feature), ptr(pred)))
     return pred
+
+
+def score_var(rowptr, colidx, vals, model, *, var=None, cov=None, offset=None, num_features=None, device=0, stream=None,
+              num_click_replicates=1, binary_feature=False):
+    """score's pred (bit for bit) and each record's predictive variance float(g^T Sigma g) under var (diagonal Sigma, [Dt]) or cov
+    (dense [Dt, Dt]; exactly one of the two).  CSR rows only, strictly ascending columns.  -> (pred, pred_var) float32."""
+    model = _keep(model, np.float64)
+    Dg = int(num_features) if num_features is not None else len(model) - 1
+    rp, ci, v = _keep(rowptr, np.int64), _keep(colidx, np.int32), _keep(vals, np.float32)
+    n = len(rp) - 1
+    o = None if offset is None else _keep(offset, np.float32)
+    va, cv = _keep(var, np.float64), _keep(cov, np.float64)
+    pred = np.zeros(n, np.float32)
+    pvar = np.zeros(n, np.float32)
+    check(lib().mlease_score_var(device, stream, Dg, n, ptr(rp), ptr(ci), ptr(v), ptr(o), ptr(model), int(num_click_replicates),
+                                 int(bool(binary_feature)), ptr(va), ptr(cv), ptr(pred), ptr(pvar)))
+    return pred, pvar
 
 
 def test_loglik(response, pred, weight=None, combiner_block=0, device=0, stream=None):
