@@ -294,23 +294,35 @@ def _ngpus():
 
 @pytest.mark.skipif(_ngpus() < 2, reason="needs 2 GPUs")
 def test_world_two_gpus_against_one():
+    """random partitions at D' = 121, then posterior_cases' window case at D' = 12 289 (the packed all-reduce past one column
+    window), against fp64 and one GPU against two"""
+    import posterior_cases as pc
     Dg, P = 120, 4
-    parts = _parts(P, 300, Dg, 0.08, seed=41)
-    z = np.random.default_rng(3).normal(0, 0.2, Dg + 1)
-    res = []
-    for devs in ([0], [0, 1]):
-        w = mb.World(devs, P, Dg, [1.0])
-        for pid, (rowptr, cols, vals, y, wt, o) in enumerate(parts):
-            w.add_partition_csr(pid, rowptr, cols, vals, y, wt, o)
-        w.begin()
-        res.append(w.admm_posterior(0, z=z, full=True, want_cov=True))
-        w.close()
-    H = _hessian(parts, Dg, z) + np.diag(_q(Dg, 1.0))
-    _check_inverse(res[0][1], H, "1 gpu")
-    _check_inverse(res[1][1], H, "2 gpus")
-    ev = np.linalg.eigvalsh(H)
-    bound = 8 * H.shape[0] * ev[-1] / ev[0] * EPS * np.abs(res[0][1]).max()
-    assert np.abs(res[0][1] - res[1][1]).max() <= bound
+    wc = pc.window_case(12289)
+    for parts, Dg, z, lm in [(_parts(P, 300, Dg, 0.08, seed=41), Dg, np.random.default_rng(3).normal(0, 0.2, Dg + 1), None),
+                             (wc["parts"], wc["Dg"], wc["z"], wc["lambda_map"])]:
+        res = []
+        for devs in ([0], [0, 1]):
+            w = mb.World(devs, len(parts), Dg, [1.0], lambda_map=lm)
+            for pid, (rowptr, cols, vals, y, wt, o) in enumerate(parts):
+                w.add_partition_csr(pid, rowptr, cols, vals, y, wt, o)
+            w.begin()
+            res.append(w.admm_posterior(0, z=z, full=True, want_cov=True))
+            w.close()
+        if lm is None:
+            H = _hessian(parts, Dg, z) + np.diag(_q(Dg, 1.0))
+            _check_inverse(res[0][1], H, "1 gpu")
+            _check_inverse(res[1][1], H, "2 gpus")
+            ev = np.linalg.eigvalsh(H)
+            bound = 8 * H.shape[0] * ev[-1] / ev[0] * EPS * np.abs(res[0][1]).max()
+        else:
+            ref = pc.reference(wc)
+            bound = pc.sigma_bound(wc, ref)
+            for (_, cov), tag in zip(res, ("1 gpu", "2 gpus")):
+                for r0 in range(0, Dg + 1, 2048):
+                    r1 = min(Dg + 1, r0 + 2048)
+                    assert np.abs(cov[r0:r1] - pc.sigma_rows(ref, Dg + 1, r0, r1)).max() <= bound, (tag, r0)
+        assert np.abs(res[0][1] - res[1][1]).max() <= bound
 
 
 def test_job_chain_on_the_fixture(tmp_path):

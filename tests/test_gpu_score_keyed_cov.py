@@ -1,7 +1,7 @@
 """GPU tests of keyed scoring under the full posterior (mlease_score_keyed_cov): pred bit for bit mlease_score_keyed's for 1 - 7 models
-per key; pred_var within 2 float ulps of numpy's fp64 x_L^T Sigma x_L + unlisted terms, with lambda_map and binary_feature; a diagonal
-Sigma within 1 ulp of mlease_score_keyed_var; NaN for an empty block; streamed equal to resident bit for bit, two devices equal to
-one; the refusals; and fit then score of 50 000 keys over 2 000 000 features."""
+per key and for rows of up to 1 100 entries; pred_var within 2 float ulps of numpy's fp64 x_L^T Sigma x_L + unlisted terms, with
+lambda_map and binary_feature; a diagonal Sigma within 1 ulp of mlease_score_keyed_var; NaN for an empty block; streamed equal to
+resident bit for bit, two devices equal to one; the refusals; and fit then score of 50 000 keys over 2 000 000 features."""
 import resource
 import threading
 
@@ -20,17 +20,26 @@ def budget():
     _hooks.set_keyed_budget(0)
 
 
-def _data(rng, K, G, D=5000, empty=()):
+def _data(rng, K, G, D=5000, empty=(), row_lens=None):
     """K keys; model g*K + k lists a sorted pool of the key's columns then the intercept, with a random SPD Sigma; test rows list half
-    their columns from the key's pool and half outside it (unlisted); models in `empty` have no block"""
-    pools = [np.sort(rng.choice(D, int(rng.integers(4, 60)), replace=False)) for _ in range(K)]
-    nk = rng.integers(1, 40, K)
+    their columns from the key's pool and half outside it (unlisted); models in `empty` have no block.  row_lens: pools of 600 - 700
+    columns and 1 - 3 rows per key whose lengths cycle through row_lens (ceil(len / 2) listed, the last among them, the rest
+    unlisted), so that a row's pairs span several 256-entry tiles of score_keyed_cov_kernel"""
+    lo, hi = (600, 700) if row_lens else (4, 60)
+    pools = [np.sort(rng.choice(D, int(rng.integers(lo, hi)), replace=False)) for _ in range(K)]
+    nk = rng.integers(1, 4 if row_lens else 40, K)
     nk[3] = 0
     rp, ci = [0], []
     for k in range(K):
         for _ in range(nk[k]):
-            a = rng.choice(pools[k], min(len(pools[k]), int(rng.integers(1, 12))), replace=False)
-            b = rng.choice(D, int(rng.integers(0, 8)), replace=False)
+            if row_lens:
+                L = row_lens[(len(rp) - 1) % len(row_lens)]
+                a = rng.choice(pools[k], (L + 1) // 2, replace=False)
+                out = np.setdiff1d(np.arange(D), pools[k])
+                b = rng.choice(out[out < a.max()], L // 2, replace=False)   # the row's last entry is listed: it pairs across tiles
+            else:
+                a = rng.choice(pools[k], min(len(pools[k]), int(rng.integers(1, 12))), replace=False)
+                b = rng.choice(D, int(rng.integers(0, 8)), replace=False)
             c = np.unique(np.concatenate([a, b]))
             ci.append(c); rp.append(rp[-1] + len(c))
     ci = np.concatenate(ci).astype(np.int32)
@@ -95,12 +104,16 @@ def _ulps(got, want, n):
     assert np.all(np.abs(got[~ok].astype(np.float64) - w) <= n * np.spacing(np.abs(w).astype(np.float32)).astype(np.float64))
 
 
-@pytest.mark.parametrize("G", [1, 2, 3, 4, 5, 7])
-def test_pred_and_pred_var(G):
+LONG_ROWS = (1, 255, 256, 257, 512, 513, 1100)   # entries per row: one tile, a full tile, one past it, two, two and one, four
+
+
+@pytest.mark.parametrize("G,row_lens", [pytest.param(G, None, id=str(G)) for G in (1, 2, 3, 4, 5, 7)] +
+                         [pytest.param(G, LONG_ROWS, id="long-%d" % G) for G in (1, 3)])
+def test_pred_and_pred_var(G, row_lens):
     import mlease_b200 as mb
-    rng = np.random.default_rng(3100 + G)
+    rng = np.random.default_rng(3100 + G + (100 if row_lens else 0))
     K = 12
-    pb, md = _data(rng, K, G, empty={1, G * K - 1})
+    pb, md = _data(rng, K, G, empty={1, G * K - 1}, row_lens=row_lens)
     lm = np.zeros(pb["D"], np.float32)
     lm[rng.choice(pb["D"], 800, replace=False)] = rng.uniform(0.2, 5.0, 800).astype(np.float32)
     for binary, lmap in [(False, None), (True, lm), (False, lm)]:
