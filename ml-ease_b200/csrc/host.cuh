@@ -183,8 +183,12 @@ int batch_xupdate(Batch& B, cudaStream_t st, double xtol, int max_newton, int po
 // *wmax (if not NULL): the largest weight, from the same read-back.
 int ingest_labels(cudaStream_t st, long long n, const int32_t* response, const float* weight, const float* offset, signed char* y, float* w,
                   float* o, int* d_flag, int* h_flag, float* wmax);
-// Enqueues the checks of device CSR arrays: a column id outside [0, Dg) sets d_flag[0], a row whose column ids are not strictly
-// increasing sets d_flag[1] (both must be 0 before); binary rewrites every stored value to 1.  The caller reads the flags back.
+// Refuses (MLEASE_ERR_INVALID, the message prefixed with who) device row pointers rowptr[0 .. n] that start below 0 or decrease
+// anywhere; reads only them, and back through d_flag[0] before it returns.  Once it passes, every row lies in [rowptr[0], rowptr[n]].
+int check_rowptr(cudaStream_t st, long long n, const long long* rowptr, int* d_flag, const std::string& who);
+// Enqueues the checks of device CSR arrays whose rowptr passed check_rowptr: a column id outside [0, Dg) sets d_flag[0], a row whose
+// column ids are not strictly increasing sets d_flag[1] (both must be 0 before); binary rewrites every stored value to 1.  The caller
+// reads the flags back.
 void check_csr(cudaStream_t st, long long n, long long nnz, const long long* rowptr, const int* colidx, float* vals, int Dg, int binary,
                int* d_flag);
 // n rows of Dg floats, ld_in apart, from host or device into dst with ldx floats a row; column Dg is 1 (has_bias) or 0, like the
@@ -328,6 +332,8 @@ namespace mlease {
 int scratch_for(mlease_session* s, int pid, Batch** B);
 int load_hv(Batch& B, int b, const double* v, cudaStream_t st);
 int reset_ctrl(Batch& B);
+// session.cu: partition pid as uploaded (device made current, pending CSR lists built)
+int resident_part(mlease_session* s, int pid, const PartData** pd);
 // session.cu: the reducers' rho of iteration `iter` for lambda l (the boost at iteration 1, then rho.adapt.coefficient), and the z/u
 // update of an iteration around the caller's one stream synchronisation: consensus_enqueue (rho of the next iteration to d_rho, K4 on
 // the summed exchange, read-back of the per-lambda diff), consensus_finish (maxdiff, mindiff, the stop rule)

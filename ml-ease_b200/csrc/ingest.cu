@@ -32,6 +32,13 @@ __global__ void convert_labels_kernel(long long n, const int* resp, const float*
     o[i] = o_in ? o_in[i] : 0.0f;
   }
 }
+// rowptr[0] >= 0 and rowptr[i] <= rowptr[i + 1]: reads the n + 1 row pointers only, so it is safe on any rowptr
+__global__ void check_rowptr_kernel(long long n, const long long* rowptr, int* bad) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t == 0 && rowptr[0] < 0) atomicOr(bad, 1);
+  for (long long i = t; i < n; i += (long long)gridDim.x * blockDim.x)
+    if (rowptr[i + 1] < rowptr[i]) { atomicOr(bad, 1); break; }
+}
 __global__ void check_rows_sorted_kernel(long long n, const long long* rowptr, const int* colidx, int* bad) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
     for (long long j = rowptr[i] + 1; j < rowptr[i + 1]; j++)
@@ -131,6 +138,17 @@ int ingest_labels(cudaStream_t st, long long n, const int32_t* response, const f
   return 0;
 }
 
+int check_rowptr(cudaStream_t st, long long n, const long long* rowptr, int* d_flag, const std::string& who) {
+  int bad = 0;
+  CK(cudaMemsetAsync(d_flag, 0, 4, st));
+  check_rowptr_kernel<<<(int)std::max<long long>(1, std::min<long long>((n + 255) / 256, 4096)), 256, 0, st>>>(n, rowptr, d_flag);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(&bad, d_flag, 4, cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  if (bad) return fail(MLEASE_ERR_INVALID, who + "rowptr must start at >= 0 and never decrease");
+  return 0;
+}
+
 void check_csr(cudaStream_t st, long long n, long long nnz, const long long* rowptr, const int* colidx, float* vals, int Dg, int binary,
                int* d_flag) {
   if (nnz <= 0) return;
@@ -192,6 +210,9 @@ int csr_build_layout(mlease_session* s, PartData& pd) {
   if (d.nnz_hint <= 0) return 0;
   const long long nrows = d.n, nnz = d.nnz_hint;
   const std::string who = "partition " + std::to_string(pd.pid) + ": ";
+  // every kernel below indexes by rowptr: its rows must lie inside [0, nnz], which a rowptr that starts at 0 and never decreases
+  // guarantees (a decreasing one makes rows overlap, and the block-major list would get more than nnz + nrows entries)
+  if (int rc = check_rowptr(s->stream, nrows, d.rowptr, s->d_flag, who)) return rc;
   // one read-back of the checks and the scalars: d_flag[0] range, [1] sorted, [2] |value| max, [3] row L1 max, [4, 6) Gram products.
   // A range error is reported before the lists below index by colidx; the reductions read column ids as values only.
   int* f = s->d_flag;

@@ -19,15 +19,19 @@ namespace mlease {
 __global__ void __launch_bounds__(256) score_kernel(int Dg, long long nrows, const long long* __restrict__ rowptr,
                                                     const int* __restrict__ colidx, const float* __restrict__ vals, long long ldx,
                                                     const float* __restrict__ offset, const double* __restrict__ model,
-                                                    double intercept_term, int binary_feature, float* __restrict__ pred) {
+                                                    double intercept_term, int binary_feature, float* __restrict__ pred,
+                                                    int* __restrict__ bad) {
   const int lane = threadIdx.x & 31;
   const long long wg = (long long)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const long long nw = (long long)gridDim.x * (blockDim.x >> 5);
   for (long long i = wg; i < nrows; i += nw) {
     double a = 0.0;
     if (colidx) {
-      for (long long j = rowptr[i] + lane; j < rowptr[i + 1]; j += 32)
-        a += model[colidx[j]] * (binary_feature ? 1.0 : (double)vals[j]);
+      for (long long j = rowptr[i] + lane; j < rowptr[i + 1]; j += 32) {
+        const int c = colidx[j];
+        if ((unsigned)c >= (unsigned)Dg) { atomicOr(bad, 1); continue; }   // never read outside the model, nor the intercept
+        a += model[c] * (binary_feature ? 1.0 : (double)vals[j]);
+      }
     } else {
       const float* xr = vals + i * ldx;
       for (int k = lane; k < Dg; k += 32) a += model[k] * (binary_feature ? 1.0 : (double)xr[k]);
@@ -457,11 +461,12 @@ static cudaError_t loglik_keyed_launch(long long n, int nkeys, long long ngroups
 
 static cudaError_t score_launch(int Dg, long long nrows, const long long* rowptr, const int* colidx, const float* vals, long long ldx,
                                 const float* offset, const double* d_model, double intercept_term, int binary_feature, float* pred,
-                                cudaStream_t st) {
+                                int* d_bad, cudaStream_t st) {
   if (nrows == 0) return cudaSuccess;
   long long blocks = (nrows + 7) / 8;
   if (blocks > 132 * 16) blocks = 132 * 16;
-  score_kernel<<<(int)blocks, 256, 0, st>>>(Dg, nrows, rowptr, colidx, vals, ldx, offset, d_model, intercept_term, binary_feature, pred);
+  score_kernel<<<(int)blocks, 256, 0, st>>>(Dg, nrows, rowptr, colidx, vals, ldx, offset, d_model, intercept_term, binary_feature, pred,
+                                            d_bad);
   return cudaGetLastError();
 }
 
@@ -517,12 +522,16 @@ int mlease_score(int32_t device, void* stream, int32_t Dg, int64_t nrows, const 
   DevMem t;
   const long long* d_rp = nullptr; const int* d_ci = nullptr; const float* d_v = nullptr; const float* d_o = nullptr; const double* d_m = nullptr;
   long long nnz = nrows * ldx;
+  int* d_bad;
+  if (int rc = t.get(&d_bad, 1, true)) return rc;
   if (colidx) {
     if (!rowptr) return fail(MLEASE_ERR_INVALID, "null rowptr");
     long long last;
     CK(cudaMemcpy(&last, rowptr + nrows, 8, cudaMemcpyDefault));
+    if (last < 0) return fail(MLEASE_ERR_INVALID, "rowptr[nrows] < 0");
     nnz = last;
     if (int rc = to_device(t, (const long long*)rowptr, (size_t)nrows + 1, &d_rp, st)) return rc;
+    if (int rc = check_rowptr(st, nrows, d_rp, d_bad, "")) return rc;
     if (int rc = to_device(t, colidx, (size_t)nnz, &d_ci, st)) return rc;
   }
   if (int rc = to_device(t, vals, (size_t)nnz, &d_v, st)) return rc;
@@ -535,10 +544,13 @@ int mlease_score(int32_t device, void* stream, int32_t Dg, int64_t nrows, const 
   const bool pred_dev = is_device_ptr(pred);
   float* d_pred = pred;
   if (!pred_dev) { if (int rc = t.get(&d_pred, (size_t)nrows, false)) return rc; }
-  CK(score_launch(Dg, nrows, d_rp, d_ci, d_v, ldx, d_o, d_m, ic, binary_feature, d_pred, st));
+  CK(cudaMemsetAsync(d_bad, 0, 4, st));
+  CK(score_launch(Dg, nrows, d_rp, d_ci, d_v, ldx, d_o, d_m, ic, binary_feature, d_pred, d_bad, st));
+  int bad = 0;
+  CK(cudaMemcpyAsync(&bad, d_bad, 4, cudaMemcpyDeviceToHost, st));
   if (!pred_dev) CK(cudaMemcpyAsync(pred, d_pred, (size_t)nrows * 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  return 0;
+  return keyed_bad(bad);
 }
 
 int mlease_score_var(int32_t device, void* stream, int32_t Dg, int64_t nrows, const int64_t* rowptr, const int32_t* colidx, const float* vals,
@@ -552,8 +564,13 @@ int mlease_score_var(int32_t device, void* stream, int32_t Dg, int64_t nrows, co
   DevMem t;
   long long nnz;
   CK(cudaMemcpy(&nnz, rowptr + nrows, 8, cudaMemcpyDefault));
+  if (nnz < 0) return fail(MLEASE_ERR_INVALID, "rowptr[nrows] < 0");
+  int* d_bad;
+  if (int rc = t.get(&d_bad, 1, true)) return rc;
   const long long* d_rp; const int* d_ci; const float *d_v, *d_o; const double *d_m, *d_var, *d_cov;
   if (int rc = to_device(t, (const long long*)rowptr, (size_t)nrows + 1, &d_rp, st)) return rc;
+  if (int rc = check_rowptr(st, nrows, d_rp, d_bad, "")) return rc;
+  CK(cudaMemsetAsync(d_bad, 0, 4, st));
   if (int rc = to_device(t, colidx, (size_t)nnz, &d_ci, st)) return rc;
   if (int rc = to_device(t, vals, (size_t)nnz, &d_v, st)) return rc;
   if (int rc = to_device(t, offset, (size_t)nrows, &d_o, st)) return rc;
@@ -569,8 +586,6 @@ int mlease_score_var(int32_t device, void* stream, int32_t Dg, int64_t nrows, co
   float* d_pv = pred_var;
   if (!is_device_ptr(pred)) { if (int rc = t.get(&d_pred, (size_t)nrows, false)) return rc; }
   if (!is_device_ptr(pred_var)) { if (int rc = t.get(&d_pv, (size_t)nrows, false)) return rc; }
-  int* d_bad;
-  if (int rc = t.get(&d_bad, 1, true)) return rc;
   if (nrows > 0) {
     const long long blocks = std::min<long long>((nrows + 7) / 8, 132LL * 16);
     score_var_kernel<<<(int)blocks, 256, 0, st>>>(Dg, nrows, d_rp, d_ci, d_v, d_o, d_m, ic, gI, binary_feature, d_var, d_cov, d_pred, d_pv, d_bad);
@@ -730,6 +745,7 @@ static int score_keyed(int32_t device, void* stream, int32_t Dg, int32_t K, cons
   if (nrows == 0) return 0;
   long long nnz;
   CK(cudaMemcpy(&nnz, rowptr + nrows, 8, cudaMemcpyDefault));
+  if (nnz < 0) return fail(MLEASE_ERR_INVALID, "rowptr[nrows] < 0");
   const bool with_pv = var || cov_ptr;   // a pred_var output
   const bool pred_dev = is_device_ptr(pred), pred_var_dev = with_pv && is_device_ptr(pred_var);
   const size_t key_bytes = (size_t)Dg * (L >= 3 ? 4 : L) * sizeof(float) * (var ? 2 : 1);   // var: the variance table too
@@ -757,6 +773,10 @@ static int score_keyed(int32_t device, void* stream, int32_t Dg, int32_t K, cons
   if (streamed) {
     std::vector<long long> off;   // rowptr at the key boundaries
     if (int rc = gather_rowptr(rowptr, krs, off)) return rc;
+    // the ranges' entry counts come from these; every range's own rows are checked on the device before a kernel indexes by them
+    if (off[0] < 0) return fail(MLEASE_ERR_INVALID, "rowptr[0] < 0");
+    for (int k = 0; k < K; k++)
+      if (off[k + 1] < off[k]) return fail(MLEASE_ERR_INVALID, "rowptr must never decrease (key " + std::to_string(k) + ")");
     const size_t pred_bytes = 4 * (size_t)L * (with_pv ? 2 : 1);   // a row's pred (and pred_var) slice
     kpc = chunk_keys(budget);
     ranges = plan_ranges(K, budget / 4, kpc, [&](long long k) {
@@ -800,8 +820,8 @@ static int score_keyed(int32_t device, void* stream, int32_t Dg, int32_t K, cons
     if (streamed || !pred_var_dev) { if (int rc = t.get(&dcov.pred_var, (size_t)L * max_rows, false)) return rc; }
   }
   float* const d_pred_var = var ? dvar.pred_var : dcov.pred_var;
-  int* d_bad;
-  if (int rc = t.get(&d_bad, 1, false)) return rc;
+  int* d_bad;   // [0] the row checks of the kernels, [1] check_rowptr's flag
+  if (int rc = t.get(&d_bad, 2, false)) return rc;
   CK(cudaMemsetAsync(d_bad, 0, 4, st));
   if (int rc = ring.open()) return rc;
   float* d_table = nullptr;
@@ -817,6 +837,8 @@ static int score_keyed(int32_t device, void* stream, int32_t Dg, int32_t K, cons
     if (int rc = to_device(rt, (const float*)v[V], (size_t)nz, &vv, st)) return rc;
     if (int rc = to_device(rt, (const float*)v[O], (size_t)n, &o, st)) return rc;
     if (z0) rebase_rowptr(st, n, rp, z0, (long long*)rp);   // in place: a range after the first is in a ring slot
+    if (int rc = check_rowptr(st, n, rp, d_bad + 1, "keys " + std::to_string(ranges[c]) + ".." + std::to_string(ranges[c + 1] - 1) + ": "))
+      return rc;
     if (!d_table) {   // a resident call's table chunks fit the memory left after its upload
       if (!ring.staged()) { CK(cudaMemGetInfo(&free_b, &total_b)); kpc = chunk_keys(keyed_budget(free_b)); }
       if (int rc = t.get(&d_table, (size_t)kpc * key_bytes / sizeof(float), false)) return rc;

@@ -298,6 +298,9 @@ int KeyedFit::run() {
     if (int rc = gather_rowptr(rowptr, idx, key_nnz0)) return rc;
     if (key_nnz0.back() != 0) return fail(MLEASE_ERR_INVALID, "rowptr[0] must be 0");
     key_nnz0.pop_back();
+    // the ranges' entry counts come from these; every range's own rows are checked on the device before a kernel indexes by them
+    for (int k = 0; k < K; k++)
+      if (key_nnz0[k + 1] < key_nnz0[k]) return fail(MLEASE_ERR_INVALID, "rowptr must never decrease (key " + std::to_string(k) + ")");
     // any key may list fewer columns than the dictionary holds (the bound above only caps its width): every range builds its lists
     lists = ldh > 32 && !todo.empty();
   }
@@ -372,6 +375,7 @@ int KeyedFit::run() {
         CK(cudaMemcpyAsync(cr.v, vals, (size_t)nz * 4, cudaMemcpyDefault, st));
       }
       if (z0) rebase_rowptr(st, n, cr.rp, z0, (long long*)cr.rp);   // in place: a range after the first is in a ring slot
+      if (int rc = check_rowptr(st, n, cr.rp, dflag, "keys " + std::to_string(k0) + ".." + std::to_string(k1 - 1) + ": ")) return rc;
       CK(cudaMemsetAsync(dflag, 0, 8, st));
       check_csr(st, n, nz, cr.rp, cr.ci, cr.v, Dg, binary_feature, dflag);
       CK(cudaMemcpyAsync(hflag, dflag, 8, cudaMemcpyDeviceToHost, st));

@@ -198,6 +198,20 @@ int mlease_internal_consensus(mlease_session* s, int32_t stages, const double* a
                               double* diff, int32_t* ctrl, uint8_t* ctrl_raw, double* wz, double* l1thr, double* rho, double* res,
                               int32_t* info);
 
+/* Partition pid of the session as its upload left it, after the deferred CSR checks and lists are built (their refusal is returned).
+ * Neither hook touches the ADMM batch.
+ * mlease_internal_partition_info: out (PARTITION_INFO_LEN doubles, every value exact): [0] rows n, [1] stored entries (0 for a dense
+ * partition), [2] CSR, [3] ldx (floats per dense row), [4] wmax (largest weight), [5] vmax (largest |stored value|), [6] rowl1 (largest
+ * row sum of |stored value|), [7] gram_pairs (products of one sparse Gram build; 0 where no block-major list was built), [8] csr_unique,
+ * [9] block-major Gram list built, [10] column index of the sparse Gram built, [11] fused-K1 segment lists built, [12] sg_S (their
+ * segments, 0 without them).
+ * mlease_internal_partition_data: the session's device copies, each to the host if not NULL: y (n int8, +1 / -1), w and o (n floats),
+ * X_or_vals (a dense partition's X, n x ldx floats with the intercept column and the padding; a CSR partition's nnz stored values, as
+ * binary.feature left them). */
+#define PARTITION_INFO_LEN 13
+int mlease_internal_partition_info(mlease_session* s, int32_t pid, double* out);
+int mlease_internal_partition_data(mlease_session* s, int32_t pid, int8_t* y, float* w, float* o, float* X_or_vals);
+
 #ifdef __cplusplus
 }
 #endif

@@ -152,6 +152,15 @@ int mlease::scratch_for(mlease_session* s, int pid, Batch** B) {
   return 0;
 }
 
+int mlease::resident_part(mlease_session* s, int pid, const PartData** pd) {
+  CK(cudaSetDevice(s->cfg.device));
+  if (int rc = csr_flush_pending(s)) return rc;
+  const int pi = find_part(s, pid);
+  if (pi < 0) return fail(MLEASE_ERR_INVALID, "partition not resident in this session");
+  *pd = &s->parts[pi];
+  return 0;
+}
+
 // the Hv pass multiplies the fp32 copy of v (hv_vf) and scales its fixed-point sums by max |v| (Ctrl::hv_vinf)
 int mlease::load_hv(Batch& B, int b, const double* v, cudaStream_t st) {
   std::vector<float> vf(B.ldx, 0.f);

@@ -701,6 +701,33 @@ int mlease_internal_csr_gram(mlease_session* s, int32_t* batch_kind, int32_t* sc
   return 0;
 }
 
+int mlease_internal_partition_info(mlease_session* s, int32_t pid, double* out) {
+  if (!s || !out) return fail(MLEASE_ERR_INVALID, "null argument");
+  const PartData* pd;
+  if (int rc = resident_part(s, pid, &pd)) return rc;
+  const Problem& d = pd->data;
+  const double v[PARTITION_INFO_LEN] = {(double)d.n, pd->csr ? (double)d.nnz_hint : 0.0, pd->csr ? 1.0 : 0.0, (double)s->ldx, (double)d.wmax,
+                                        (double)d.vmax, (double)d.rowl1, d.gram_pairs, (double)d.csr_unique, d.bm_offs ? 1.0 : 0.0,
+                                        d.gc_offs ? 1.0 : 0.0, d.sg_perm ? 1.0 : 0.0, (double)d.sg_S};
+  std::copy(v, v + PARTITION_INFO_LEN, out);
+  return 0;
+}
+
+int mlease_internal_partition_data(mlease_session* s, int32_t pid, int8_t* y, float* w, float* o, float* X_or_vals) {
+  if (!s) return fail(MLEASE_ERR_INVALID, "null session");
+  const PartData* pd;
+  if (int rc = resident_part(s, pid, &pd)) return rc;
+  const Problem& d = pd->data;
+  CK(cudaStreamSynchronize(s->stream));
+  const size_t n = (size_t)d.n;
+  if (y) CK(cudaMemcpy(y, d.y, n, cudaMemcpyDeviceToHost));
+  if (w) CK(cudaMemcpy(w, d.w, n * sizeof(float), cudaMemcpyDeviceToHost));
+  if (o) CK(cudaMemcpy(o, d.o, n * sizeof(float), cudaMemcpyDeviceToHost));
+  if (X_or_vals && pd->csr && d.nnz_hint > 0) CK(cudaMemcpy(X_or_vals, d.vals, (size_t)d.nnz_hint * sizeof(float), cudaMemcpyDeviceToHost));
+  if (X_or_vals && !pd->csr) CK(cudaMemcpy(X_or_vals, d.X, n * s->ldx * sizeof(float), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
 int mlease_internal_dmma_shapes(const double* A, const double* B, int32_t n, int32_t K, double* D8, double* D16) {
   if (!A || !B || !D8 || !D16 || n <= 0 || K <= 0 || K % 4) return fail(MLEASE_ERR_INVALID, "bad argument");
   const size_t na = (size_t)n * 16 * K, nb = (size_t)n * 8 * K, nd = (size_t)n * 128;

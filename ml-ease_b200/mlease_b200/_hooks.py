@@ -30,6 +30,8 @@ SIG = {
     "mlease_internal_csr_gram": [_vp, _pi32, _pi32],
     "mlease_internal_dmma_shapes": [_vp, _vp, _i32, _i32, _vp, _vp],
     "mlease_internal_consensus": [_vp, _i32] + [_vp] * 13,
+    "mlease_internal_partition_info": [_vp, _i32, _vp],
+    "mlease_internal_partition_data": [_vp, _i32, _vp, _vp, _vp, _vp],
 }
 
 _bound = None
@@ -64,6 +66,34 @@ def keyed_last_call():
     bounds = np.zeros(max(n.value, 1), np.int64)
     check(fn(bounds.ctypes.data, n.value, C.byref(n), C.byref(s), C.byref(a), C.byref(b)))
     return bounds[:n.value], bool(s.value), a.value, b.value
+
+
+PARTITION_INFO = ("n", "nnz", "csr", "ldx", "wmax", "vmax", "rowl1", "gram_pairs", "csr_unique", "block_major", "gram_col_index",
+                  "k1_segments", "sg_S")
+
+
+def partition_info(session, pid):
+    """Partition pid as uploaded, after its deferred CSR checks and lists: dict of PARTITION_INFO (wmax, vmax, rowl1 float32, flags
+    bool, the rest int)."""
+    out = np.zeros(len(PARTITION_INFO), np.float64)
+    check(bound().mlease_internal_partition_info(session._h, int(pid), out.ctypes.data))
+    info = dict(zip(PARTITION_INFO, out))
+    for k in PARTITION_INFO:
+        info[k] = np.float32(info[k]) if k in ("wmax", "vmax", "rowl1") else \
+            bool(info[k]) if k in ("csr", "csr_unique", "block_major", "gram_col_index", "k1_segments") else int(info[k])
+    return info
+
+
+def partition_data(session, pid, info=None):
+    """The session's device copies of partition pid -> dict(y int8 [n], w, o float32 [n], X float32 [n, ldx] (dense) or vals float32
+    [nnz] (CSR, as binary.feature left them))."""
+    info = info or partition_info(session, pid)
+    n = info["n"]
+    y = np.zeros(n, np.int8)
+    w, o = np.zeros(n, np.float32), np.zeros(n, np.float32)
+    xv = np.zeros(info["nnz"] if info["csr"] else (n, info["ldx"]), np.float32)
+    check(bound().mlease_internal_partition_data(session._h, int(pid), y.ctypes.data, w.ctypes.data, o.ctypes.data, xv.ctypes.data))
+    return dict(y=y, w=w, o=o, **{"vals" if info["csr"] else "X": xv})
 
 
 K1_KINDS = {1: "dense", 2: "fx", 3: "fx_window", 4: "csr", 5: "fused"}

@@ -115,7 +115,7 @@ def reference(part: Part, beta) -> Ref:
     q = np.where(t >= 0, e / (1.0 + e), 1.0 / (1.0 + e))
     r = -w * y * q
     lr = w * (np.log1p(e) + np.maximum(-t, 0.0))
-    g = np.bincount(part.colidx, x * r[rows], part.Dt)
+    g = np.bincount(part.colidx, x * r[rows], part.Dt).astype(np.float64)   # (int64 when the partition stores no value)
     g[-1] = r.sum()
     absdot = np.bincount(rows, np.abs(xb), part.n) + abs(b[-1]) + np.abs(part.o.astype(np.float64))
     return Ref(s, t, p, q, r, g, float(lr.sum()), np.sqrt(w * p * q), lr, absdot, ref_nterms(part))
@@ -242,7 +242,7 @@ def grad_bound(part: Part, ref: Ref, plan: Plan, err: RowErr | None = None):
     x = np.abs(part.vals.astype(np.float64))
     xr = x * np.abs(ref.r[rows])
     absr = np.abs(ref.r)
-    prop = np.bincount(part.colidx, x * err.dr[rows], Dt)
+    prop = np.bincount(part.colidx, x * err.dr[rows], Dt).astype(np.float64)
     prop[-1] = err.dr.sum()
     ch = _chunk_of_rows(part, plan)
     nch = int(ch.max()) + 1 if part.n else 1
