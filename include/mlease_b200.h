@@ -434,6 +434,24 @@ int mlease_score_keyed_cov(int32_t device, void* stream, int32_t num_features, i
 int mlease_test_loglik_keyed(int32_t device, void* stream, int64_t nentries, const int32_t* entry_key, const int32_t* entry_group,
                              const int32_t* response, const float* weight, const float* pred, int32_t num_keys,
                              float* out_loglik, double* out_count);
+/* The weighted ROC AUC of held-out predictions: the exact Mann-Whitney statistic with weights, tied pairs counting 1/2.
+ * pred [num_sets][nrows] (a set is a lambda or a grid point: the pred of mlease_score_keyed[_var|_cov]); response [nrows] (1
+ * positive; 0 or -1 negative, ItemModelTestLoglik's labels) and weight [nrows] (NULL = 1) are shared by every set.  key_rowstart
+ * [num_keys + 1] (NULL with num_keys = 0: no per-key results): key k owns rows [key_rowstart[k], key_rowstart[k+1]).  Input
+ * pointers host-or-device.
+ * A segment is a set, or a (set, key) pair.  Over its runs r of equal pred in ascending order (-0.0 and +0.0 tie; +-inf are
+ * ordinary values), with P_r / N_r its positive / negative weight and Nb_r the negative weight of the runs below r, in fp64:
+ * U = sum_r P_r (Nb_r + N_r / 2), P = sum P_r, N = sum N_r, auc = U / (P N), NaN when P or N is 0.
+ * Outputs (host memory, each may be NULL, not both AUC outputs): out_auc [num_sets]; out_weight [2] = positive and negative weight
+ * of all rows; out_key_auc [num_sets][num_keys]; out_key_weight [num_keys][2].
+ * Every AUC is bitwise repeatable and depends only on its own segment's records in stable sorted order (ties in row order): a
+ * key's or a set's AUC is the same computed alone or among others.  The call streams over chunks of sets within free device
+ * memory; a set that does not fit is MLEASE_ERR_INVALID, with the bytes it needs.  MLEASE_ERR_INVALID, before any output is
+ * written: nrows outside [1, 2^31 - 1], num_sets < 1, a NaN pred, a response other than 1, 0, -1, a negative or NaN weight,
+ * key_rowstart not starting at 0, decreasing or not ending at nrows, both AUC outputs NULL. */
+int mlease_test_auc(int32_t device, void* stream, int64_t nrows, int32_t num_sets, const float* pred, const int32_t* response,
+                    const float* weight, int32_t num_keys, const int64_t* key_rowstart, double* out_auc, double* out_weight,
+                    double* out_key_auc, double* out_key_weight);
 
 /* Bench / profiling hooks (not part of the reference surface): time one fused K1 pass or one Gram build
  * on a resident partition with CUDA events on the session stream, `reps` launches, returns avg ms. */

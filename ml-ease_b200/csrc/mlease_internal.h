@@ -19,11 +19,12 @@ extern "C" {
 #endif
 
 /* mlease_internal_set_keyed_budget caps, process-wide, the device bytes the keyed calls (mlease_naive_train*,
- * mlease_item_model_train, mlease_score_keyed[_var]) plan with (0 = the free memory only), so that small inputs stream through many
- * chunks.  mlease_internal_keyed_last_call reports the most recent keyed call of the process: the key boundaries of its chunks
- * (*count of them, the first 0 and the last K; up to cap are written), whether it streamed, and for a streamed call the host
+ * mlease_item_model_train, mlease_score_keyed[_var]) and mlease_test_auc plan with (0 = the free memory only), so that small inputs
+ * stream through many chunks.  mlease_internal_keyed_last_call reports the most recent keyed call of the process: the key
+ * boundaries of its chunks (*count of them, the first 0 and the last K; for mlease_test_auc the set boundaries, the last num_sets;
+ * up to cap are written), whether it streamed (mlease_test_auc: ran more than one chunk), and for a streamed call the host
  * milliseconds its rows took to stage (all chunks: a fit's copy into the pinned ring and H2D, on a staging thread; scoring's
- * direct copies, queued from the calling thread) and the milliseconds a fit waited for its staging thread (0 for scoring). */
+ * direct copies, queued from the calling thread) and the milliseconds a fit waited for its staging thread (0 for scoring; both 0 for mlease_test_auc). */
 int mlease_internal_set_keyed_budget(int64_t bytes);
 int mlease_internal_keyed_last_call(int64_t* bounds, int32_t cap, int32_t* count, int32_t* streamed, double* stage_ms, double* wait_ms);
 

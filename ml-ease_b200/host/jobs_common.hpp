@@ -166,6 +166,9 @@ Value feature_value(const std::string& key, float v);
 std::map<std::string, std::unordered_map<std::string, double>> read_linear_models(const std::string& path, bool last_wins = false);
 // RegressionTest-style output schema: input fields with unions removed + pred:float (+ predVar:float)
 std::string test_output_schema(const SchemaP& in, const char* name = "AdmmTestOutput", const char* ns = nullptr, bool pred_var = false);
+// (response, pred, weight) of the scored records of one file (RegressionTest / ItemModelGridTest output), appended; weight 1 when
+// absent
+void read_scored(const std::string& f, std::vector<int32_t>& resp, std::vector<float>& pred, std::vector<float>& weight);
 // a record's bytes with the union branch indices dropped; throws NotPlain when the record is not plain
 struct NotPlain {};
 void transcode_plain(const Plan& pl, const uint8_t*& p, const uint8_t* e, std::string& o);

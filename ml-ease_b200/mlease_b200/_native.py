@@ -76,6 +76,7 @@ def lib():
             "mlease_score_keyed_var": [i32, vp, i32, i32, vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, i32, vp, vp],
             "mlease_score_keyed_cov": [i32, vp, i32, i32, vp, vp, vp, vp, vp, i32, vp, vp, vp, vp, vp, vp, vp, i32, vp, vp],
             "mlease_test_loglik_keyed": [i32, vp, i64, vp, vp, vp, vp, vp, i32, vp, vp],
+            "mlease_test_auc": [i32, vp, i64, i32, vp, vp, vp, i32, vp, vp, vp, vp, vp],
             "mlease_time_kernel": [vp, i32, i32, i32, i32, C.POINTER(f32)],
             "mlease_profile": [vp, i32, vp, vp, C.POINTER(f64), C.POINTER(f64), C.POINTER(f64)],
             "mlease_posterior_variance": [vp, i32, vp, vp, i32, vp, vp],
@@ -124,7 +125,7 @@ EXPORTED = ["mlease_last_error", "mlease_abi_version", "mlease_session_create", 
             "mlease_add_partition_dense", "mlease_add_partition_csr", "mlease_admm_begin", "mlease_admm_begin_initialized", "mlease_admm_local_step",
             "mlease_admm_consensus", "mlease_admm_run", "mlease_admm_iterate", "mlease_get_z", "mlease_get_final_model", "mlease_get_x", "mlease_get_u",
             "mlease_get_uplusx", "mlease_get_stats", "mlease_objective", "mlease_fit_partition", "mlease_hessian_vector", "mlease_naive_train_dense",
-            "mlease_score", "mlease_test_loglik", "mlease_score_keyed", "mlease_score_keyed_var", "mlease_score_keyed_cov", "mlease_test_loglik_keyed", "mlease_time_kernel", "mlease_profile",
+            "mlease_score", "mlease_test_loglik", "mlease_score_keyed", "mlease_score_keyed_var", "mlease_score_keyed_cov", "mlease_test_loglik_keyed", "mlease_test_auc", "mlease_time_kernel", "mlease_profile",
             "mlease_posterior_variance", "mlease_admm_posterior", "mlease_world_admm_posterior", "mlease_score_var", "mlease_naive_train", "mlease_item_model_train", "mlease_naive_train_sparse", "mlease_item_model_train_sparse", "mlease_item_model_train_cov", "mlease_comm_unique_id", "mlease_comm_create", "mlease_comm_destroy", "mlease_comm_info", "mlease_session_set_comm",
             "mlease_world_create", "mlease_world_destroy", "mlease_world_num_devices", "mlease_world_add_partition_dense",
             "mlease_world_add_partition_csr", "mlease_world_begin", "mlease_world_begin_initialized", "mlease_world_iterate",

@@ -516,6 +516,27 @@ def test_loglik_keyed(entry_key, entry_group, response, pred, num_keys, weight=N
 test_loglik_keyed.__test__ = False
 
 
+def test_auc(response, pred, weight=None, key_rowstart=None, device=0, stream=None):
+    """Weighted ROC AUC (Mann-Whitney U, ties 1/2) of pred [S, n] (1-D: S = 1) against response (1 positive; 0, -1 negative) ->
+    (auc [S], weight [2] = positive and negative weight of all rows, key_auc [S, K] or None, key_weight [K, 2] or None); keys own
+    rows [key_rowstart[k], key_rowstart[k+1]).  pred, response and weight may be CUDA tensors."""
+    p = _keep(pred, np.float32)
+    S = 1 if len(p.shape) == 1 else int(p.shape[0])
+    n = int(p.shape[-1])
+    r, w = _keep(response, np.int32), _keep(weight, np.float32)
+    krs = None if key_rowstart is None else np.ascontiguousarray(key_rowstart, np.int64)
+    K = 0 if krs is None else len(krs) - 1
+    auc = np.zeros(S, np.float64)
+    wt = np.zeros(2, np.float64)
+    kauc = np.zeros((S, K), np.float64) if krs is not None else None
+    kw = np.zeros((K, 2), np.float64) if krs is not None else None
+    check(lib().mlease_test_auc(device, stream, n, S, ptr(p), ptr(r), ptr(w), K, ptr(krs), ptr(auc), ptr(wt), ptr(kauc), ptr(kw)))
+    return auc, wt, kauc, kw
+
+
+test_auc.__test__ = False
+
+
 def naive_train_dense(X, key_rowstart, response, lam, weight=None, offset=None, lambda_map=None, prior_mean=0.0,
                       penalize_intercept=False, has_intercept=True, data_size_threshold=0, device=0, stream=None):
     """RegressionNaiveTrain reducer for K keys (jobs/RegressionNaiveTrain.java:302-415) -> (models [K,D+1], skipped[K])."""

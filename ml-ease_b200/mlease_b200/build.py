@@ -10,7 +10,7 @@ ROOT = os.path.dirname(PKG)            # ml-ease_b200/
 CSRC = os.path.join(ROOT, "csrc")
 LIBDIR = os.path.join(ROOT, "lib")
 SO = os.path.join(LIBDIR, "libmlease_b200.so")
-SOURCES = ["session.cu", "batch.cu", "ingest.cu", "keyed_fit.cu", "keyed_cols.cu", "key_ranges.cu", "test_hooks.cu", "k1_score_grad.cu", "k1_csr_fused.cu", "newton.cu", "k2_gram.cu", "k3_cholesky.cu", "k4_consensus.cu", "k5_score.cu", "k6_postvar.cu", "comm.cu"]
+SOURCES = ["session.cu", "batch.cu", "ingest.cu", "keyed_fit.cu", "keyed_cols.cu", "key_ranges.cu", "test_hooks.cu", "k1_score_grad.cu", "k1_csr_fused.cu", "newton.cu", "k2_gram.cu", "k3_cholesky.cu", "k4_consensus.cu", "k5_score.cu", "k6_postvar.cu", "k7_auc.cu", "comm.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-Xptxas", "-v"]
@@ -61,7 +61,7 @@ HOST_CLI = os.path.join(LIBDIR, "mlease_regression")
 def build_host(force: bool = False) -> str:
     """Host job layer (C++17, zlib): libmlease_host.so + the mlease_regression CLI, both linked to libmlease_b200.so."""
     srcs = [os.path.join(HOST, f) for f in ("avro_io.cpp", "regression_jobs.cpp", "item_model_jobs.cpp", "item_model_train_job.cpp",
-                                                 "item_model_grid_test_job.cpp", "regression_posterior_job.cpp")]
+                                                 "item_model_grid_test_job.cpp", "regression_posterior_job.cpp", "auc_jobs.cpp")]
     deps = srcs + [os.path.join(HOST, "avro_io.hpp"), os.path.join(HOST, "avro_walk.hpp"), os.path.join(HOST, "jobs_common.hpp"), os.path.join(os.path.dirname(ROOT), "include", "mlease_b200.h"),
                    os.path.join(os.path.dirname(ROOT), "include", "mlease_host.h"), SO]
     cxx = os.environ.get("CXX", "g++")
