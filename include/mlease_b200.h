@@ -340,6 +340,38 @@ int mlease_item_model_train_sparse(int32_t device, void* stream, int32_t num_key
                                    const float* default_lambdas, const float* lambda_map, int32_t binary_feature, int32_t compute_var,
                                    int64_t capacity, int64_t* out_key_ptr, int32_t* out_col, double* out_model, double* out_var);
 
+/* mlease_item_model_train_sparse under a prior of each key's own (llf/LibLinear.java:221-245 with per-fit priorMean / priorVar maps),
+ * such as an earlier run's posterior, so that a per-item model can be refreshed with new data instead of refitting its history.  The
+ * same inputs, checks, plan, streaming, budgets, outputs and several-device use (each device's key range with its own prior_ptr from
+ * 0), plus key k's prior list, entries [prior_ptr[k], prior_ptr[k+1]) of:
+ *   prior_col   int32, strictly ascending within a key, in [0, num_features] (num_features = the intercept);
+ *   prior_mean  double, finite;
+ *   prior_var   double, finite and >= 0; 0 = the column's usual variance (1/lambda_map[j], 1/default lambda, for the intercept
+ *               1/intercept lambda), so a mean-only prior (a model written without compute.var) is one with zeros.
+ * prior_ptr [num_keys+1] int64, prior_ptr[0] = 0, non-decreasing.  Host or device pointers, all four required (with empty lists too).
+ * Fit (a, b) of key k, column j (the rules of initSetup, :476-497, with the key's list as the prior maps):
+ *   j listed by the key's rows, with an entry: its mean, and its variance when > 0, replace lambda_map, the grid lambda and
+ *              intercept_prior_mean[k] (an intercept entry replaces the intercept lambda and mean);
+ *   j listed, no entry: the prior of mlease_item_model_train_sparse;
+ *   j with an entry but not listed by the rows (prior-only): not part of the fit.  The key's list reports it with coefficient =
+ *              the entry's mean and variance = its variance, or 1/q of the column's usual prior when that is 0 (:373-397), copied
+ *              from the inputs.
+ *   lists:     each fitted key's list is the union of the columns its rows list and its prior-only columns, ascending, then the
+ *              intercept; keys that are not fitted have empty lists.  capacity is checked before any row is read against the
+ *              bound sum over fitted keys of min(stored entries + non-intercept prior entries, num_features) + 1.
+ * Refused with MLEASE_ERR_INVALID before anything is written, the message naming the key: a bad prior_ptr, a column out of range or
+ * not ascending, a mean that is not finite, a variance that is negative or not finite.  The fits start from 0 (init = null); warm
+ * starts, mlease_item_model_train_cov and NaiveTrain have no per-key priors.  With every list empty the lists and values are those of
+ * mlease_item_model_train_sparse (bit for bit for one-row keys in their own column spaces). */
+int mlease_item_model_train_prior(int32_t device, void* stream, int32_t num_keys, int32_t num_features, const int64_t* key_rowstart,
+                                  const int64_t* rowptr, const int32_t* colidx, const float* vals, const int32_t* response,
+                                  const float* weight, const float* offset, const double* intercept_prior_mean,
+                                  int32_t num_intercept_lambdas, const float* intercept_lambdas, int32_t num_default_lambdas,
+                                  const float* default_lambdas, const float* lambda_map, int32_t binary_feature, int32_t compute_var,
+                                  int64_t capacity, int64_t* out_key_ptr, int32_t* out_col, double* out_model, double* out_var,
+                                  const int64_t* prior_ptr, const int32_t* prior_col, const double* prior_mean,
+                                  const double* prior_var);
+
 /* mlease_item_model_train_sparse with the full posterior of every fit (computeFullPostVar, llf/LibLinear.java:315-326): the same
  * inputs, plan, fits, lists and several-device use, the models bit for bit those of the sparse call for one-row keys in their own
  * column spaces (within its run-to-run spread otherwise).  At each fit, H = diag(q) + sum_i w_i p_i (1-p_i) x_i x_i^T is assembled

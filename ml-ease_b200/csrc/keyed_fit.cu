@@ -1,6 +1,7 @@
 // keyed_fit.cu -- K independent fits per prior over one upload of the rows: RegressionNaiveTrain (mlease_naive_train,
 // mlease_naive_train_dense) and ItemModelTrain (mlease_item_model_train), both with sparse outputs (mlease_*_train_sparse), and
-// ItemModelTrain with each key's full posterior covariance (mlease_item_model_train_cov).
+// ItemModelTrain with each key's full posterior covariance (mlease_item_model_train_cov) or under per-key prior lists
+// (mlease_item_model_train_prior).
 #include <cub/block/block_scan.cuh>
 
 #include <algorithm>
@@ -71,14 +72,31 @@ __global__ void span_present_kernel(const long long* rp, const int* ci, const lo
   if (threadIdx.x == 0) count[blockIdx.x] = total;
 }
 // Where problem b of a batch writes its list in a chunk's slab: entries dst .. of out.  dk >= 0: the list is cols[s0 .. s0 + dk)
-// (then the intercept); dk < 0: no list, the ones of mask row mrow in column order (the intercept's included)
-struct GatherJob { long long dst, s0; int dk, mrow; };
+// (then the intercept); dk < 0: no list, the ones of mask row mrow in column order (the intercept's included).  Per-key priors: the
+// key's prior list is entries p0 .. p0 + pn of its range's PriorDev (pn = 0 without one)
+struct GatherJob { long long dst, s0; int dk, mrow; long long p0; int pn; };
+// A key range's per-key prior lists on the device (mlease_item_model_train_prior), entries numbered from the range's first key's;
+// col NULL: the call has none
+struct PriorDev { const int* col; const double* mean; const double* var; };
 constexpr int GATHER_THREADS = 256;
+// the first index i of the ascending a[0 .. n) with a[i] >= x
+__device__ __forceinline__ int lower_index(const int* a, int n, int x) {
+  int lo = 0, hi = n;
+  while (lo < hi) { const int mid = (lo + hi) >> 1; if (a[mid] < x) lo = mid + 1; else hi = mid; }
+  return lo;
+}
+// the index of x in the ascending a[0 .. n), or -1
+__device__ __forceinline__ int find_index(const int* a, int n, int x) {
+  const int i = lower_index(a, n, x);
+  return i < n && a[i] == x ? i : -1;
+}
 // One problem per block: beta (hdiag: 1 / g_t, IEEE fp64 like the host's 1.0 / x) at the problem's listed columns into out, and the
 // global column ids into out_col (NULL: already written).  A local problem (local = 1) holds its list's columns at 0 .. dk - 1 and
-// the intercept at Dt - 1; a global-width one holds global column c at c.
+// the intercept at Dt - 1; a global-width one holds global column c at c.  Per-key priors (pr.col): the list is the union of the
+// listed columns and the key's prior-only columns (prior entries its rows do not list), ascending, then the intercept; a prior-only
+// column takes its entry's mean (hdiag: its variance, or 1 / q[c] where that is 0), never a value of the fit.
 __global__ void sparse_gather_kernel(const Problem* probs, const GatherJob* jobs, const int* cols, const unsigned char* mask, int local,
-                                     int Dg, int has_bias, int hdiag, double* out, int* out_col) {
+                                     int Dg, int has_bias, int hdiag, double* out, int* out_col, PriorDev pr, const double* q) {
   using Scan = cub::BlockScan<int, GATHER_THREADS>;
   __shared__ typename Scan::TempStorage scan;
   __shared__ int carry;
@@ -89,10 +107,50 @@ __global__ void sparse_gather_kernel(const Problem* probs, const GatherJob* jobs
     out[jb.dst + e] = hdiag ? __ddiv_rn(1.0, v[src]) : v[src];
     if (out_col) out_col[jb.dst + e] = col;
   };
+  const int pn = pr.col ? jb.pn : 0;
+  const int* pc = pn ? pr.col + jb.p0 : nullptr;
+  auto put_prior = [&](long long e, int i, int col) {   // prior entry i of the key, a prior-only column
+    const double pv = pr.var[jb.p0 + i];
+    out[jb.dst + e] = hdiag ? (pv > 0.0 ? pv : __ddiv_rn(1.0, q[col])) : pr.mean[jb.p0 + i];
+    if (out_col) out_col[jb.dst + e] = col;
+  };
   if (jb.dk >= 0) {
     const int* c = cols + jb.s0;
-    for (int i = threadIdx.x; i < jb.dk; i += blockDim.x) put(i, local ? i : c[i], c[i]);
-    if (threadIdx.x == 0 && has_bias) put(jb.dk, pb.Dt - 1, Dg);
+    if (!pn) {
+      for (int i = threadIdx.x; i < jb.dk; i += blockDim.x) put(i, local ? i : c[i], c[i]);
+      if (threadIdx.x == 0 && has_bias) put(jb.dk, pb.Dt - 1, Dg);
+      return;
+    }
+    // listed column i: after i listed columns and the prior-only entries below c[i] -- the prior entries below it (lb) less those
+    // that are listed (a scan over the listed columns that have an entry)
+    if (threadIdx.x == 0) carry = 0;
+    __syncthreads();
+    for (int t0 = 0; t0 < jb.dk; t0 += GATHER_THREADS) {
+      const int i = t0 + threadIdx.x;
+      int lb = 0, h = 0;
+      if (i < jb.dk) { lb = lower_index(pc, pn, c[i]); h = lb < pn && pc[lb] == c[i]; }
+      int pos, tile;
+      Scan(scan).ExclusiveSum(h, pos, tile);
+      if (i < jb.dk) put(i + lb - (carry + pos), local ? i : c[i], c[i]);
+      __syncthreads();
+      if (threadIdx.x == 0) carry += tile;
+      __syncthreads();
+    }
+    // prior-only entry: after the prior-only entries before it and the listed columns below it
+    if (threadIdx.x == 0) carry = 0;
+    __syncthreads();
+    for (int t0 = 0; t0 < pn; t0 += GATHER_THREADS) {
+      const int i = t0 + threadIdx.x;
+      int lb = 0, f = 0;
+      if (i < pn && pc[i] != Dg) { lb = lower_index(c, jb.dk, pc[i]); f = !(lb < jb.dk && c[lb] == pc[i]); }
+      int pos, tile;
+      Scan(scan).ExclusiveSum(f, pos, tile);
+      if (f) put_prior(carry + pos + lb, i, pc[i]);
+      __syncthreads();
+      if (threadIdx.x == 0) carry += tile;
+      __syncthreads();
+    }
+    if (threadIdx.x == 0 && has_bias) put(jb.dk + carry, pb.Dt - 1, Dg);
     return;
   }
   const unsigned char* mk = mask + (size_t)jb.mrow * pb.Dt;
@@ -100,14 +158,84 @@ __global__ void sparse_gather_kernel(const Problem* probs, const GatherJob* jobs
   __syncthreads();
   for (int t0 = 0; t0 < pb.Dt; t0 += GATHER_THREADS) {
     const int k = t0 + threadIdx.x;
-    const int f = k < pb.Dt ? mk[k] : 0;
+    int f = k < pb.Dt ? mk[k] : 0, e = -1;
+    if (!f && pn && k < Dg) { e = find_index(pc, pn, k); f = e >= 0; }
     int pos, tile;
     Scan(scan).ExclusiveSum(f, pos, tile);
-    if (f) put(carry + pos, k, k);
+    if (f) { if (e < 0) put(carry + pos, k, k); else put_prior(carry + pos, e, k); }
     __syncthreads();
     if (threadIdx.x == 0) carry += tile;
     __syncthreads();
   }
+}
+// naive_init_kernel (span NULL: global width, mask[b] the columns the rows list) and local_init_kernel (cols / span) under per-key
+// priors: each column as they set it, then a column the rows list (local: the list's columns and the intercept) that has an entry
+// in its key's prior list (a binary search of jobs[b]'s) takes the entry's mean, and the precision 1 / var when var > 0.  Prior-only
+// columns, unlisted columns and the padding keep their q and m.
+__global__ void prior_init_kernel(const Problem* probs, const double* m, const double* q, const double* intercept_mean, const int* cols,
+                                  const long long* span, const unsigned char* mask, int Dg, const GatherJob* jobs, PriorDev pr) {
+  const Problem& pb = probs[blockIdx.x];
+  const GatherJob jb = jobs[blockIdx.x];
+  const int* pc = pr.col + jb.p0;
+  const int* c = span ? cols + span[2 * blockIdx.x] : nullptr;
+  const int dk = span ? (int)(span[2 * blockIdx.x + 1] - span[2 * blockIdx.x]) : 0;
+  for (int k = threadIdx.x; k < pb.ldx; k += blockDim.x) {
+    pb.beta[k] = 0.0;
+    int g = -1;   // the global column of k where the rows list it
+    double qk, mk;
+    if (span) {
+      if (k < dk) { g = c[k]; qk = q[g]; mk = m[g]; }
+      else if (k == pb.Dt - 1) { g = Dg; qk = q[Dg]; mk = intercept_mean ? intercept_mean[blockIdx.x] : m[Dg]; }
+      else { qk = 1.0; mk = 0.0; }
+    } else {
+      qk = q[k]; mk = (intercept_mean && k == pb.Dt - 1) ? intercept_mean[blockIdx.x] : m[k];
+      if (k < pb.Dt && mask[(size_t)blockIdx.x * pb.Dt + k]) g = k;
+    }
+    if (g >= 0 && jb.pn) {
+      const int e = find_index(pc, jb.pn, g);
+      if (e >= 0) {
+        mk = pr.mean[jb.p0 + e];
+        const double v = pr.var[jb.p0 + e];
+        if (v > 0.0) qk = 1.0 / v;
+      }
+    }
+    pb.q[k] = qk; pb.m[k] = mk;
+  }
+}
+// count[b] = the prior-only columns of key b (jobs[b]): the entries of its prior list that its rows do not list -- not in its column
+// list (dk >= 0) or 0 in its row of mask; the intercept is always listed
+__global__ void prior_only_count_kernel(const GatherJob* jobs, const int* cols, const unsigned char* mask, int Dt, int Dg, PriorDev pr,
+                                        int* count) {
+  const GatherJob jb = jobs[blockIdx.x];
+  __shared__ int total;
+  if (threadIdx.x == 0) total = 0;
+  __syncthreads();
+  int n = 0;
+  for (int i = threadIdx.x; i < jb.pn; i += blockDim.x) {
+    const int g = pr.col[jb.p0 + i];
+    if (g == Dg) continue;
+    n += (jb.dk >= 0 ? find_index(cols + jb.s0, jb.dk, g) >= 0 : mask[(size_t)jb.mrow * Dt + g] != 0) ? 0 : 1;
+  }
+  atomicAdd(&total, n);
+  __syncthreads();
+  if (threadIdx.x == 0) count[blockIdx.x] = total;
+}
+// The checks of the prior lists of nk keys (offs[i] .. offs[i + 1] of col / mean / var: key kbase + i): a column outside [0, Dg],
+// columns not strictly ascending, a mean that is not finite, a variance that is negative or not finite.  bad = the smallest
+// (key << 3 | reason) found (reasons 1 .. 4 in that order), left as is when all pass; nonint[i] = key i's entries less its intercept's.
+__global__ void prior_check_kernel(const long long* offs, int kbase, const int* col, const double* mean, const double* var, int Dg,
+                                   unsigned long long* bad, int* nonint) {
+  const long long e0 = offs[blockIdx.x], e1 = offs[blockIdx.x + 1];
+  for (long long e = e0 + threadIdx.x; e < e1; e += blockDim.x) {
+    const int c = col[e];
+    int why = 0;
+    if (c < 0 || c > Dg) why = 1;
+    else if (e > e0 && col[e - 1] >= c) why = 2;
+    else if (!isfinite(mean[e])) why = 3;
+    else if (!(var[e] >= 0.0) || isinf(var[e])) why = 4;
+    if (why) atomicMin(bad, ((unsigned long long)(kbase + blockIdx.x) << 3) | (unsigned long long)why);
+  }
+  if (threadIdx.x == 0) nonint[blockIdx.x] = (int)(e1 - e0) - (e1 > e0 && col[e1 - 1] == Dg ? 1 : 0);
 }
 // Where problem b of a batch writes its posterior in a chunk's slab: its list of n entries starts at entry dst of the variances (and
 // of the column ids the model gather wrote), the packed lower triangle of its covariance at entry cdst of the covariance slab (cdst
@@ -148,6 +276,11 @@ struct SparseOut { int64_t cap; int64_t* key_ptr; int32_t* col; };
 // The covariance output of mlease_item_model_train_cov: key k's block is entries ptr[k] .. ptr[k + 1] of val, prior p's at
 // val[p * cap + e]; val NULL: variances only (ptr unused)
 struct CovOut { int64_t cap; int64_t* ptr; double* val; };
+// The per-key priors of mlease_item_model_train_prior, host-or-device as the caller passed them: key k's entries are ptr[k] ..
+// ptr[k + 1] of col (ascending, Dg = the intercept), mean and var (0: the column's usual variance)
+struct KeyPriorIn { const int64_t* ptr; const int32_t* col; const double* mean; const double* var; };
+// prior entries checked per pass of prior_check_kernel (a larger key is checked on its own), 20 B each on the device
+constexpr size_t PRIOR_CHECK_BYTES = size_t(20) << 24;
 // the widest system whose explicit inverse K3 forms (wider ones keep it factored, cholesky_factored_direction)
 constexpr int COV_MAX_WIDTH = 2048;
 // solve_batch of a covariance call whose batch would be matrix-free: solve_group splits it
@@ -187,6 +320,8 @@ struct ChunkRows {
   int csr_unique = 0;
   const KeyCols* kc = nullptr;   // the column spaces of keys kbase.. (CSR calls wider than 32 columns), else NULL
   int kbase = 0;
+  PriorDev pd{nullptr, nullptr, nullptr};   // the range's per-key prior lists, entries from prior_ptr[pbase_key] on
+  long long pbase = 0;                      // prior_ptr at the range's first key
 };
 
 // One keyed fit call, over the key ranges of the keyed pipeline (key_ranges.cu).  Resident (the whole upload and the first chunk's
@@ -211,7 +346,10 @@ struct KeyedFit {
   int32_t* skipped;
   const SparseOut* sp;                    // the output sink: NULL = dense out_model / out_var; else the lists (out_model / out_var their values)
   const CovOut* cv;                       // NULL, or the full posterior (out_var = diag(Sigma)) and its blocks
+  const KeyPriorIn* kp;                   // NULL, or per-key priors (sparse sink only): each range uploads its keys' lists
   bool csr = false;
+  std::vector<long long> pptr;            // per-key priors: host copy of prior_ptr
+  std::vector<int> pnon;                  // per-key priors: each key's entries other than the intercept's
   int L = 0, Dt = 0, ldx = 0, Dp = 0, ldh = 0;
   std::vector<long long> krs, key_nnz0;   // key_nnz0: CSR rowptr at the key boundaries
   std::vector<int> todo;                  // the keys that are fitted
@@ -229,8 +367,14 @@ struct KeyedFit {
     const size_t x = (size_t)round_up(w, 4), p = (size_t)round_up((int)x, 128), h = (size_t)round_up(w, 32);
     return (size_t)n * p * 2 + p * p * 4 + 3 * h * h * 8 + 2 * h * 32 * 8 + 64 * x + (out_var ? (size_t)n * 8 : 0);
   }
-  // entries of a fitted CSR key's list at most: its stored entries or the dictionary, whichever is smaller, and the intercept
-  long long list_bound(int k) const { return std::min<long long>(key_nnz0[k + 1] - key_nnz0[k], Dg) + (has_intercept ? 1 : 0); }
+  // entries of a fitted CSR key's list at most: its stored entries (and prior entries other than the intercept's) or the dictionary,
+  // whichever is smaller, and the intercept
+  long long list_bound(int k) const {
+    return std::min<long long>(key_nnz0[k + 1] - key_nnz0[k] + (kp ? pnon[k] : 0), Dg) + (has_intercept ? 1 : 0);
+  }
+  // device bytes of the prior lists of keys [k0, k1)
+  size_t prior_bytes(long long k0, long long k1) const { return kp ? (size_t)(pptr[k1] - pptr[k0]) * 20 : 0; }
+  int check_priors();
   // device bytes of a fitted key's entries in its chunk's slab (values of every prior, variances, column ids, covariance blocks); 0 for
   // the dense sink.  len: the key's list length when known, else (< 0) its bound
   size_t slab_bytes(int k, long long len = -1) const {
@@ -304,13 +448,14 @@ int KeyedFit::run() {
     // any key may list fewer columns than the dictionary holds (the bound above only caps its width): every range builds its lists
     lists = ldh > 32 && !todo.empty();
   }
+  if (kp) { if (int rc = check_priors()) return rc; }   // before anything is written or indexed by the lists
   if (sp) {   // the lists' room, checked before any row is read
     long long need = 0;
     for (int k : todo) need += list_bound(k);
     if (sp->cap < need)
       return fail(MLEASE_ERR_INVALID, "capacity " + std::to_string(sp->cap) + " is too small: the keys' lists need up to " +
-                                          std::to_string(need) + " entries (the sum over fitted keys of min(stored entries, num_features)" +
-                                          (has_intercept ? " + 1)" : ")"));
+                                          std::to_string(need) + " entries (the sum over fitted keys of min(stored entries" +
+                                          (kp ? " + non-intercept prior entries" : "") + ", num_features)" + (has_intercept ? " + 1)" : ")"));
   }
   // resident (one range) when the whole upload (rows, labels, key boundaries, the temporaries of host input, the column lists) and
   // the first chunk's state fit the budget
@@ -320,7 +465,7 @@ int KeyedFit::run() {
   const long long nnz = csr ? key_nnz0[K] : 0;
   const bool host_rows = !is_device_ptr(csr ? (const void*)colidx : (const void*)vals);
   size_t up = (size_t)ntot * 9 + (is_device_ptr(response) ? 0 : (size_t)ntot * 12);
-  if (csr) up += (size_t)nnz * 4 + (host_rows ? (size_t)nnz * 4 + (size_t)(ntot + 1) * 8 : 0) + (size_t)(K + 1) * 16 + list_bytes(0, K);
+  if (csr) up += (size_t)nnz * 4 + (host_rows ? (size_t)nnz * 4 + (size_t)(ntot + 1) * 8 : 0) + (size_t)(K + 1) * 16 + list_bytes(0, K) + prior_bytes(0, K);
   else up += (size_t)ntot * ldx * 4 + (host_rows ? (size_t)256 << 20 : 0);
   const size_t first = todo.empty() ? 0 : state_bytes(krs[todo[0] + 1] - krs[todo[0]], bound_dt(todo[0])) + slab_bytes(todo[0]);
   const bool streamed = up + first > budget;
@@ -331,7 +476,7 @@ int KeyedFit::run() {
     ranges = plan_ranges(K, budget / 4, 16384, [&](long long k) -> size_t {
       const size_t n = (size_t)(krs[k + 1] - krs[k]);
       size_t b = n * (12 + 9);
-      b += csr ? n * 16 + (size_t)(key_nnz0[k + 1] - key_nnz0[k]) * 8 + list_bytes(k, k + 1) : n * ((size_t)ldx_in + ldx) * 4;
+      b += csr ? n * 16 + (size_t)(key_nnz0[k + 1] - key_nnz0[k]) * 8 + list_bytes(k, k + 1) + prior_bytes(k, k + 1) : n * ((size_t)ldx_in + ldx) * 4;
       return b + (solves(k) ? state_bytes(n, bound_dt(k)) + slab_bytes((int)k) : 0);
     }, [&](long long k) { return solves(k); });
   }
@@ -388,6 +533,17 @@ int KeyedFit::run() {
         if (int rc = build_lists(k0, k1, cr.ci, st, rt, &kc)) return rc;
         cr.kc = &kc; cr.kbase = k0;
       }
+      if (kp) {   // the range's slice of the prior lists (check_priors passed them all)
+        const long long p0 = pptr[k0], pn = pptr[k1] - p0;
+        int* pc; double *pm, *pv;
+        if (int rc = rt.get(&pc, (size_t)pn, false)) return rc;
+        if (int rc = rt.get(&pm, (size_t)pn, false)) return rc;
+        if (int rc = rt.get(&pv, (size_t)pn, false)) return rc;
+        CK(cudaMemcpyAsync(pc, kp->col + p0, (size_t)pn * 4, cudaMemcpyDefault, st));
+        CK(cudaMemcpyAsync(pm, kp->mean + p0, (size_t)pn * 8, cudaMemcpyDefault, st));
+        CK(cudaMemcpyAsync(pv, kp->var + p0, (size_t)pn * 8, cudaMemcpyDefault, st));
+        cr.pd = PriorDev{pc, pm, pv}; cr.pbase = p0;
+      }
     } else {
       if (int rc = upload_dense_rows(dX, ldx, (const float*)v[V], ldx_in, n, Dg, has_intercept ? 1 : 0, st)) return rc;
     }
@@ -416,6 +572,53 @@ int KeyedFit::run() {
   if (sp) close_lists(K);
   keyed_record(bounds, ring.staged(), ring.stage_ms, ring.wait_ms);
   if (cnt.not_converged) return fail(MLEASE_ERR_NUMERIC, "Model fitting error! (" + std::to_string(cnt.not_converged) + " fits did not converge)");
+  return 0;
+}
+
+// The per-key priors' checks, before the call writes anything: prior_ptr on the host (one value per key), every entry on the device
+// in passes over contiguous key slices of at most PRIOR_CHECK_BYTES; each key's non-intercept entries into pnon for the list bound
+int KeyedFit::check_priors() {
+  pptr.resize((size_t)K + 1);
+  CK(cudaMemcpy(pptr.data(), kp->ptr, (size_t)(K + 1) * 8, cudaMemcpyDefault));
+  if (pptr[0] != 0) return fail(MLEASE_ERR_INVALID, "prior_ptr[0] must be 0 (key 0)");
+  for (int k = 0; k < K; k++)
+    if (pptr[k + 1] < pptr[k]) return fail(MLEASE_ERR_INVALID, "prior_ptr must never decrease (key " + std::to_string(k) + ")");
+  pnon.assign(K, 0);
+  if (pptr[K] == 0) return 0;
+  const std::vector<long long> sl = plan_ranges(K, PRIOR_CHECK_BYTES, 1 << 20, [&](long long k) { return (size_t)(pptr[k + 1] - pptr[k]) * 20; },
+                                                nullptr);
+  long long mx = 0, mk = 0;
+  for (size_t s = 1; s < sl.size(); s++) { mx = std::max(mx, pptr[sl[s]] - pptr[sl[s - 1]]); mk = std::max(mk, sl[s] - sl[s - 1]); }
+  DevMem t;
+  int *pc, *nonint; double *pm, *pv; long long* offs; unsigned long long* bad;
+  if (int rc = t.get(&pc, (size_t)mx, false)) return rc;
+  if (int rc = t.get(&pm, (size_t)mx, false)) return rc;
+  if (int rc = t.get(&pv, (size_t)mx, false)) return rc;
+  if (int rc = t.get(&offs, (size_t)mk + 1, false)) return rc;
+  if (int rc = t.get(&nonint, (size_t)mk, false)) return rc;
+  if (int rc = t.get(&bad, 1, false)) return rc;
+  std::vector<long long> o;
+  for (size_t s = 1; s < sl.size(); s++) {
+    const long long k0 = sl[s - 1], k1 = sl[s], p0 = pptr[k0], pn = pptr[k1] - p0;
+    o.resize((size_t)(k1 - k0 + 1));
+    for (long long k = k0; k <= k1; k++) o[k - k0] = pptr[k] - p0;
+    CK(cudaMemcpyAsync(offs, o.data(), o.size() * 8, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(pc, kp->col + p0, (size_t)pn * 4, cudaMemcpyDefault, st));
+    CK(cudaMemcpyAsync(pm, kp->mean + p0, (size_t)pn * 8, cudaMemcpyDefault, st));
+    CK(cudaMemcpyAsync(pv, kp->var + p0, (size_t)pn * 8, cudaMemcpyDefault, st));
+    CK(cudaMemsetAsync(bad, 0xff, 8, st));
+    prior_check_kernel<<<(unsigned)(k1 - k0), 128, 0, st>>>(offs, (int)k0, pc, pm, pv, Dg, bad, nonint);
+    CK(cudaGetLastError());
+    unsigned long long hbad = 0;
+    CK(cudaMemcpyAsync(&hbad, bad, 8, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(pnon.data() + k0, nonint, (size_t)(k1 - k0) * 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (hbad != ~0ull) {
+      static const char* why[] = {"", "a prior column outside [0, num_features]", "prior columns that are not strictly ascending",
+                                  "a prior mean that is not finite", "a prior variance that is negative or not finite"};
+      return fail(MLEASE_ERR_INVALID, "key " + std::to_string(hbad >> 3) + ": " + why[hbad & 7]);
+    }
+  }
   return 0;
 }
 
@@ -473,6 +676,7 @@ int KeyedFit::open_slab(const int* keys, int nprob, const ChunkRows& cr, DevMem&
     }
   }
   const int nu = (int)rows.size() / 2;
+  std::vector<int> count(nu), pcount(kp ? nprob : 0);
   if (nu) {
     long long* drows; int* dcount;
     if (int rc = mem.get(&sl->mask, (size_t)nu * Dt, false)) return rc;
@@ -482,11 +686,28 @@ int KeyedFit::open_slab(const int* keys, int nprob, const ChunkRows& cr, DevMem&
     CK(cudaMemcpyAsync(drows, rows.data(), rows.size() * 8, cudaMemcpyHostToDevice, st));
     span_present_kernel<<<nu, 256, 0, st>>>(cr.rp, cr.ci, drows, Dt, has_intercept ? 1 : 0, sl->mask, dcount);
     CK(cudaGetLastError());
-    std::vector<int> count(nu);
     CK(cudaMemcpyAsync(count.data(), dcount, (size_t)nu * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    for (int i = 0; i < nk; i++) if (sl->mrow[i] >= 0) sl->len[i] = count[sl->mrow[i]];
   }
+  std::vector<GatherJob> pj(pcount.size());   // per-key priors: each key's list, or mask row, and its prior entries
+  if (kp) {
+    for (int b = 0; b < nprob; b++) {
+      const int k = keys[b];
+      GatherJob& j = pj[b];
+      j.mrow = sl->mrow[k - k0]; j.dk = -1;
+      if (j.mrow < 0) { j.s0 = cr.kc->start[k - cr.kbase]; j.dk = (int)(cr.kc->start[k - cr.kbase + 1] - j.s0); }
+      j.p0 = pptr[k] - cr.pbase; j.pn = (int)(pptr[k + 1] - pptr[k]);
+    }
+    GatherJob* dpj; int* dpcount;
+    if (int rc = mem.get(&dpj, pj.size(), false)) return rc;
+    if (int rc = mem.get(&dpcount, pj.size(), false)) return rc;
+    CK(cudaMemcpyAsync(dpj, pj.data(), pj.size() * sizeof(GatherJob), cudaMemcpyHostToDevice, st));
+    prior_only_count_kernel<<<nprob, 128, 0, st>>>(dpj, cr.kc ? cr.kc->d_cols : nullptr, sl->mask, Dt, Dg, cr.pd, dpcount);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(pcount.data(), dpcount, pj.size() * 4, cudaMemcpyDeviceToHost, st));
+  }
+  if (nu || kp) CK(cudaStreamSynchronize(st));
+  for (int i = 0; i < nk; i++) if (sl->mrow[i] >= 0) sl->len[i] = count[sl->mrow[i]];
+  for (size_t b = 0; b < pcount.size(); b++) sl->len[keys[b] - k0] += pcount[b];   // the union with the prior-only columns
   for (int i = 0; i < nk; i++) { sl->off[i] = sl->n; sl->n += sl->len[i]; }
   if (cv && cv->val) {
     // the lengths are fixed: the chunk's blocks must fit the room left, checked before the chunk writes anything
@@ -574,6 +795,7 @@ int KeyedFit::solve_batch(const int* keys, int nprob, int w, const ChunkRows& cr
       GatherJob& j = jobs[b];
       j.dst = sl->off[k - sl->k0]; j.mrow = sl->mrow[k - sl->k0]; j.s0 = 0; j.dk = -1;
       if (j.mrow < 0) { j.s0 = cr.kc->start[k - cr.kbase]; j.dk = (int)(cr.kc->start[k - cr.kbase + 1] - j.s0); }
+      if (kp) { j.p0 = pptr[k] - cr.pbase; j.pn = (int)(pptr[k + 1] - pptr[k]); }
     }
     if (int rc = ct.get(&djobs, jobs.size(), false)) return rc;
     CK(cudaMemcpyAsync(djobs, jobs.data(), jobs.size() * sizeof(GatherJob), cudaMemcpyHostToDevice, st));
@@ -609,10 +831,10 @@ int KeyedFit::solve_batch(const int* keys, int nprob, int w, const ChunkRows& cr
   if (local) {
     if (int rc = ct.get(&dspan, span.size(), false)) return rc;
     CK(cudaMemcpyAsync(dspan, span.data(), span.size() * 8, cudaMemcpyHostToDevice, st));
-  } else if (csr && !sl) {
+  } else if (csr && (!sl || kp)) {
     // features absent from a key's rows are not part of its dataset, hence not of its model (llf/LibLinear.java:343-350; the only
     // prior mean a caller may set per key is the intercept's, which every dataset holds, so :374-383 adds nothing): mask them out
-    // (the sparse sink reports only the listed columns)
+    // (the sparse sink reports only the listed columns).  Per-key priors: the mask says which columns take a prior entry in the fit
     if (int rc = ct.get(&dmask, (size_t)B.nprob * Dt, false)) return rc;
     CK(cudaMemsetAsync(dmask, 0, (size_t)B.nprob * Dt, st));
     naive_present_kernel<<<B.nprob, 256, 0, st>>>(B.d, Dt, has_intercept ? 1 : 0, dmask);
@@ -629,14 +851,16 @@ int KeyedFit::solve_batch(const int* keys, int nprob, int w, const ChunkRows& cr
     CK(cudaMemcpyAsync(dm, priors[l].m.data(), ldx * 8, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(dq, priors[l].q.data(), ldx * 8, cudaMemcpyHostToDevice, st));
     CK(cudaStreamSynchronize(st));   // dq / dm are reused by the next prior
-    if (local) local_init_kernel<<<B.nprob, 128, 0, st>>>(B.d, dm, dq, dim, cr.kc->d_cols, dspan, Dg);
+    if (kp) prior_init_kernel<<<B.nprob, 128, 0, st>>>(B.d, dm, dq, dim, local ? cr.kc->d_cols : nullptr, local ? dspan : nullptr, dmask, Dg,
+                                                        djobs, cr.pd);
+    else if (local) local_init_kernel<<<B.nprob, 128, 0, st>>>(B.d, dm, dq, dim, cr.kc->d_cols, dspan, Dg);
     else naive_init_kernel<<<B.nprob, 128, 0, st>>>(B.d, dm, dq, dim);
     B.mirror.clear();                // the factors of the previous prior belong to another prior
     if (int rc = batch_xupdate(B, st, 2e-7, 100, 0, 1, hflag, dflag, cnt)) return rc;
     if (sl) {   // the listed values straight into the slab (column ids with the first prior); no read-back until the chunk is done
       const int* kcols = cr.kc ? cr.kc->d_cols : nullptr;
       sparse_gather_kernel<<<B.nprob, GATHER_THREADS, 0, st>>>(B.d, djobs, kcols, sl->mask, local ? 1 : 0, Dg, B.has_bias, 0,
-                                                               sl->model + l * sl->n, l == 0 ? sl->col : nullptr);
+                                                               sl->model + l * sl->n, l == 0 ? sl->col : nullptr, cr.pd, dq);
       CK(cudaGetLastError());
       if (cv) {
         if (int rc = posterior_cov(B, local, drs, row_start[B.nprob], dvec, dcjobs, sl, l, dfail, factor_ctl, reset_ctl)) return rc;
@@ -644,7 +868,7 @@ int KeyedFit::solve_batch(const int* keys, int nprob, int w, const ChunkRows& cr
         CK(postvar_rowweights(B.d, B.nprob, drs, row_start[B.nprob], B.has_bias, dvec, st, nullptr));
         CK(postvar_diag(B.d, B.nprob, drs, row_start[B.nprob], dvec, B.has_bias, st, nullptr));
         sparse_gather_kernel<<<B.nprob, GATHER_THREADS, 0, st>>>(B.d, djobs, kcols, sl->mask, local ? 1 : 0, Dg, B.has_bias, 1,
-                                                                 sl->var + l * sl->n, nullptr);
+                                                                 sl->var + l * sl->n, nullptr, cr.pd, dq);
         CK(cudaGetLastError());
       }
       continue;
@@ -705,9 +929,10 @@ int KeyedFit::posterior_cov(Batch& B, bool local, const long long* drs, long lon
 int keyed_fit(int num_sms, cudaStream_t st, int32_t K, int32_t Dg, const int64_t* key_rowstart, const int64_t* rowptr, const int32_t* colidx,
               const float* vals, int64_t ldx_in, const int32_t* response, const float* weight, const float* offset, bool has_intercept,
               int32_t data_size_threshold, int32_t binary_feature, const std::vector<KeyedPrior>& priors, const double* intercept_mean,
-              double* out_model, double* out_var, int32_t* skipped, const SparseOut* sp, const CovOut* cv = nullptr) {
+              double* out_model, double* out_var, int32_t* skipped, const SparseOut* sp, const CovOut* cv = nullptr,
+              const KeyPriorIn* kp = nullptr) {
   KeyedFit f{num_sms, st, K, Dg, key_rowstart, rowptr, colidx, vals, ldx_in, response, weight, offset, has_intercept, data_size_threshold,
-             binary_feature, priors, intercept_mean, out_model, out_var, skipped, sp, cv};
+             binary_feature, priors, intercept_mean, out_model, out_var, skipped, sp, cv, kp};
   return f.run();
 }
 // host copy of a host-or-device array (NULL -> empty)
@@ -755,13 +980,14 @@ int naive_train(int32_t device, void* stream, int32_t K, int32_t Dg, const int64
 // ------------------------------------------------------------------------------------------
 // ItemModelTrain (jobs/ItemModelTrain.java:226-276): per key, one fit per (intercept lambda, default lambda) in config order, the
 // intercept's prior mean the key's own; diagonal posterior variance on request.  Dense outputs, or (sp) the sparse lists, with (cv)
-// the full posterior
+// the full posterior or (kp) per-key prior lists
 // ------------------------------------------------------------------------------------------
 int item_model_train(int32_t device, void* stream, int32_t K, int32_t Dg, const int64_t* key_rowstart, const int64_t* rowptr,
                      const int32_t* colidx, const float* vals, const int32_t* response, const float* weight, const float* offset,
                      const double* intercept_prior_mean, int32_t IL, const float* intercept_lambdas, int32_t DL,
                      const float* default_lambdas, const float* lambda_map, int32_t binary_feature, int32_t compute_var,
-                     double* out_model, double* out_var, const SparseOut* sp, const CovOut* cv = nullptr) {
+                     double* out_model, double* out_var, const SparseOut* sp, const CovOut* cv = nullptr,
+                     const KeyPriorIn* kp = nullptr) {
   int num_sms = 0;
   if (int rc = keyed_fit_check(device, Dg, rowptr, colidx, 0, binary_feature, &num_sms)) return rc;
   std::vector<float> lm, il, dl;
@@ -786,7 +1012,7 @@ int item_model_train(int32_t device, void* stream, int32_t K, int32_t Dg, const 
       q[Dg] = 1.0 / (1.0 / (double)il[a]);
     }
   return keyed_fit(num_sms, (cudaStream_t)stream, K, Dg, key_rowstart, rowptr, colidx, vals, 0, response, weight, offset, true, 0, binary_feature,
-                   priors, im.data(), out_model, compute_var ? out_var : nullptr, nullptr, sp, cv);
+                   priors, im.data(), out_model, compute_var ? out_var : nullptr, nullptr, sp, cv, kp);
 }
 }  // namespace
 
@@ -854,6 +1080,22 @@ int mlease_item_model_train_cov(int32_t device, void* stream, int32_t K, int32_t
   const CovOut cv{cov_capacity, out_cov ? out_cov_ptr : nullptr, out_cov};
   return item_model_train(device, stream, K, Dg, key_rowstart, rowptr, colidx, vals, response, weight, offset, intercept_prior_mean, IL,
                           intercept_lambdas, DL, default_lambdas, lambda_map, binary_feature, 1, out_model, out_var, &sp, &cv);
+}
+
+int mlease_item_model_train_prior(int32_t device, void* stream, int32_t K, int32_t Dg, const int64_t* key_rowstart, const int64_t* rowptr,
+                                  const int32_t* colidx, const float* vals, const int32_t* response, const float* weight, const float* offset,
+                                  const double* intercept_prior_mean, int32_t IL, const float* intercept_lambdas, int32_t DL,
+                                  const float* default_lambdas, const float* lambda_map, int32_t binary_feature, int32_t compute_var,
+                                  int64_t capacity, int64_t* out_key_ptr, int32_t* out_col, double* out_model, double* out_var,
+                                  const int64_t* prior_ptr, const int32_t* prior_col, const double* prior_mean, const double* prior_var) {
+  if (K <= 0 || Dg <= 0 || IL <= 0 || DL <= 0 || !intercept_lambdas || !default_lambdas || !key_rowstart || !rowptr || !colidx || !vals ||
+      !response || !intercept_prior_mean || capacity < 0 || !out_key_ptr || !out_col || !out_model || (compute_var && !out_var) ||
+      !prior_ptr || !prior_col || !prior_mean || !prior_var)
+    return fail(MLEASE_ERR_INVALID, "bad argument");
+  const SparseOut sp{capacity, out_key_ptr, out_col};
+  const KeyPriorIn kp{prior_ptr, prior_col, prior_mean, prior_var};
+  return item_model_train(device, stream, K, Dg, key_rowstart, rowptr, colidx, vals, response, weight, offset, intercept_prior_mean, IL,
+                          intercept_lambdas, DL, default_lambdas, lambda_map, binary_feature, compute_var, out_model, out_var, &sp, nullptr, &kp);
 }
 
 int mlease_naive_train_dense(int32_t device, void* stream, int32_t K, int32_t Dg, const int64_t* key_rowstart, const float* X, int64_t ldx_in,

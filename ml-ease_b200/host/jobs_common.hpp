@@ -7,6 +7,7 @@
 #include <exception>
 #include <fstream>
 #include <map>
+#include <memory>
 #include <stdexcept>
 #include <string>
 #include <thread>
@@ -314,6 +315,33 @@ inline std::vector<float> lambda_list(const JobConfig& c, const std::string& key
   if (out.empty()) io_error(key + ": no lambda given");
   return out;
 }
+
+// ------------------------------------------------------------------------------------------ ItemModelTrain's fit
+// What ItemModelTrain fits and writes: the keys (byte order) and their CSR rows, the grid, the lambda map and the intercept prior
+// means; out, the models and variances [grid point][key][D + 1] at the columns the writer reads, each key's model columns (cols,
+// ascending) and the columns its posteriorVar lists after the intercept (var_cols)
+struct ItemModelFit {
+  int D = 0;
+  std::vector<float> il, dl, lambda_map;
+  bool binary = false, compute_var = false;
+  std::vector<int32_t> devs;
+  std::vector<std::string> knames;
+  std::vector<int64_t> krs{0}, rp{0};
+  std::vector<int32_t> ci, rr;
+  std::vector<float> vv, ww, oo;
+  std::vector<double> means;
+  std::vector<double> m, var;
+  std::vector<std::vector<int32_t>> cols, var_cols;
+};
+// ItemModelTrain with prior.model.path (item_model_prior.cpp), reached through register_item_model_prior so that
+// item_model_train_job.cpp links without the library call it makes.  read: the earlier run's models of one grid point by item, the
+// features they name added to dict; fit: the keys' fits under those priors into f.
+struct ItemPriors;
+struct ItemPriorHooks {
+  std::shared_ptr<ItemPriors> (*read)(const JobConfig& c, Dictionary& dict);
+  void (*fit)(const ItemPriors& p, ItemModelFit& f);
+};
+bool register_item_model_prior(const ItemPriorHooks& h);
 
 // job_class -> job for mlease_job_run; returns true (for use in a namespace-scope initializer)
 using JobFn = void (*)(const JobConfig&);

@@ -91,6 +91,8 @@ def lib():
                                                vp, vp],
             "mlease_item_model_train_cov": [i32, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp, i32, vp, vp, i32, i64, vp, vp, vp, vp,
                                             i64, vp, vp],
+            "mlease_item_model_train_prior": [i32, vp, i32, i32, vp, vp, vp, vp, vp, vp, vp, vp, i32, vp, i32, vp, vp, i32, i32, i64, vp, vp,
+                                              vp, vp, vp, vp, vp, vp],
             "mlease_comm_unique_id": [vp],
             "mlease_comm_create": [vp, i32, i32, i32, C.POINTER(vp)],
             "mlease_comm_destroy": [vp],
@@ -126,7 +128,7 @@ EXPORTED = ["mlease_last_error", "mlease_abi_version", "mlease_session_create", 
             "mlease_admm_consensus", "mlease_admm_run", "mlease_admm_iterate", "mlease_get_z", "mlease_get_final_model", "mlease_get_x", "mlease_get_u",
             "mlease_get_uplusx", "mlease_get_stats", "mlease_objective", "mlease_fit_partition", "mlease_hessian_vector", "mlease_naive_train_dense",
             "mlease_score", "mlease_test_loglik", "mlease_score_keyed", "mlease_score_keyed_var", "mlease_score_keyed_cov", "mlease_test_loglik_keyed", "mlease_test_auc", "mlease_time_kernel", "mlease_profile",
-            "mlease_posterior_variance", "mlease_admm_posterior", "mlease_world_admm_posterior", "mlease_score_var", "mlease_naive_train", "mlease_item_model_train", "mlease_naive_train_sparse", "mlease_item_model_train_sparse", "mlease_item_model_train_cov", "mlease_comm_unique_id", "mlease_comm_create", "mlease_comm_destroy", "mlease_comm_info", "mlease_session_set_comm",
+            "mlease_posterior_variance", "mlease_admm_posterior", "mlease_world_admm_posterior", "mlease_score_var", "mlease_naive_train", "mlease_item_model_train", "mlease_naive_train_sparse", "mlease_item_model_train_sparse", "mlease_item_model_train_cov", "mlease_item_model_train_prior", "mlease_comm_unique_id", "mlease_comm_create", "mlease_comm_destroy", "mlease_comm_info", "mlease_session_set_comm",
             "mlease_world_create", "mlease_world_destroy", "mlease_world_num_devices", "mlease_world_add_partition_dense",
             "mlease_world_add_partition_csr", "mlease_world_begin", "mlease_world_begin_initialized", "mlease_world_iterate",
             "mlease_world_run", "mlease_world_get_z", "mlease_world_get_final_model", "mlease_world_get_x", "mlease_world_get_u",

@@ -609,9 +609,9 @@ def _host(a, dtype):
     return np.ascontiguousarray(a, dtype=dtype)
 
 
-def _list_capacity(key_rowstart, rowptr, num_features, fitted, intercept):
+def _list_capacity(key_rowstart, rowptr, num_features, fitted, intercept, prior_ptr=None, prior_col=None):
     """entries the keys' lists may need: sum over fitted keys of min(stored entries, num_features) (+ 1 for the intercept), from
-    rowptr at the key boundaries alone"""
+    rowptr at the key boundaries alone; with per-key prior lists, each key's stored entries count its non-intercept prior entries too"""
     krs = _host(key_rowstart, np.int64)
     if hasattr(rowptr, "data_ptr"):
         import torch
@@ -619,6 +619,11 @@ def _list_capacity(key_rowstart, rowptr, num_features, fitted, intercept):
     else:
         at = np.asarray(rowptr, np.int64)[krs]
     nnz = np.diff(at)
+    if prior_ptr is not None:
+        pp, pc = _host(prior_ptr, np.int64), _host(prior_col, np.int64)
+        n = np.diff(pp)
+        last = pc[np.clip(pp[1:] - 1, 0, len(pc) - 1)] if len(pc) else np.zeros(len(n), np.int64)
+        nnz = nnz + n - ((n > 0) & (last == int(num_features)))
     return int((np.minimum(nnz, int(num_features))[fitted] + (1 if intercept else 0)).sum())
 
 
@@ -676,6 +681,57 @@ def item_model_train_sparse(vals, key_rowstart, response, intercept_lambdas, def
     shape = (len(il), len(dl), n)
     return (key_ptr, cols[:n].copy(), models[:, :n].reshape(shape).copy(),
             None if var is None else var[:, :n].reshape(shape).copy())
+
+
+def item_model_train_prior(vals, key_rowstart, response, intercept_lambdas, default_lambdas, *, rowptr, colidx, num_features, prior_ptr,
+                           prior_col, prior_mean, prior_var, intercept_prior_mean=None, weight=None, offset=None, lambda_map=None,
+                           binary_feature=False, compute_var=False, device=0, stream=None, capacity=None):
+    """item_model_train_sparse under each key's own prior (mlease_item_model_train_prior): key k's prior is entries
+    prior_ptr[k]:prior_ptr[k+1] of prior_col (strictly ascending, num_features = the intercept), prior_mean and prior_var (0: the
+    column's usual variance).  A column the key's rows list takes its entry in the fit; a prior-only column joins the key's list at
+    its prior mean and variance.  keyed_prior_from_fit turns an earlier result into these lists.
+    -> (key_ptr [K+1] int64, cols [n] int32, models [IL, DL, n] float64, var [IL, DL, n] float64 or None)."""
+    krs = np.ascontiguousarray(key_rowstart, np.int64)
+    K, D = len(krs) - 1, int(num_features)
+    il, dl = _f32(np.atleast_1d(intercept_lambdas)), _f32(np.atleast_1d(default_lambdas))
+    rp, ci, vals = _keep(rowptr, np.int64), _keep(colidx, np.int32), _keep(vals, np.float32)
+    r, w, o, lm = _keep(response, np.int32), _keep(weight, np.float32), _keep(offset, np.float32), _keep(lambda_map, np.float32)
+    pp, pc = _keep(prior_ptr, np.int64), _keep(prior_col, np.int32)
+    pm, pv = _keep(prior_mean, np.float64), _keep(prior_var, np.float64)
+    if len(pp) != K + 1:
+        raise ValueError("prior_ptr must hold one entry per key and one more")
+    # the library takes a pointer for every list, empty ones included
+    pc, pm, pv = (np.zeros(1, a.dtype) if len(a) == 0 and not hasattr(a, "data_ptr") else a for a in (pc, pm, pv))
+    im = np.zeros(K, np.float64) if intercept_prior_mean is None else np.ascontiguousarray(intercept_prior_mean, np.float64)
+    if len(im) != K:
+        raise ValueError("intercept_prior_mean must hold one entry per key")
+    cap = _list_capacity(krs, rp, D, np.diff(krs) > 0, True, pp, pc) if capacity is None else int(capacity)
+    G = len(il) * len(dl)
+    key_ptr = np.zeros(K + 1, np.int64)
+    cols = np.zeros(max(cap, 1), np.int32)
+    models = np.zeros((G, max(cap, 1)), np.float64)
+    var = np.zeros_like(models) if compute_var else None
+    check(lib().mlease_item_model_train_prior(device, stream, K, D, ptr(krs), ptr(rp), ptr(ci), ptr(vals), ptr(r), ptr(w), ptr(o), ptr(im),
+                                              len(il), ptr(il), len(dl), ptr(dl), ptr(lm), int(bool(binary_feature)), int(bool(compute_var)),
+                                              cap, ptr(key_ptr), ptr(cols), ptr(models), ptr(var), ptr(pp), ptr(pc), ptr(pm), ptr(pv)))
+    n = int(key_ptr[K])
+    shape = (len(il), len(dl), n)
+    return (key_ptr, cols[:n].copy(), models[:, :n].reshape(shape).copy(),
+            None if var is None else var[:, :n].reshape(shape).copy())
+
+
+def keyed_prior_from_fit(key_ptr, cols, models, var, grid_point):
+    """One grid point of a sparse keyed fit (item_model_train_sparse or item_model_train_prior) as the prior lists of the next
+    item_model_train_prior call on the same keys: each key's model as its prior means, its posterior variances (var None: 0, the
+    columns' usual variances) as its prior variances.  grid_point: (a, b) of models [IL, DL, n], or a flat index over IL * DL.
+    -> (prior_ptr [K+1] int64, prior_col int32, prior_mean float64, prior_var float64)."""
+    kp = np.ascontiguousarray(key_ptr, np.int64)
+    n = int(kp[-1])
+    models = np.asarray(models, np.float64)
+    g = np.ravel_multi_index(grid_point, models.shape[:-1]) if isinstance(grid_point, tuple) else int(grid_point)
+    mean = np.ascontiguousarray(models.reshape(-1, models.shape[-1])[g, :n])
+    pv = np.zeros(n) if var is None else np.ascontiguousarray(np.asarray(var, np.float64).reshape(-1, models.shape[-1])[g, :n])
+    return kp.copy(), np.ascontiguousarray(cols, np.int32)[:n].copy(), mean, pv
 
 
 def _list_lengths(key_rowstart, rowptr, colidx, num_features):

@@ -61,7 +61,7 @@ HOST_CLI = os.path.join(LIBDIR, "mlease_regression")
 def build_host(force: bool = False) -> str:
     """Host job layer (C++17, zlib): libmlease_host.so + the mlease_regression CLI, both linked to libmlease_b200.so."""
     srcs = [os.path.join(HOST, f) for f in ("avro_io.cpp", "regression_jobs.cpp", "item_model_jobs.cpp", "item_model_train_job.cpp",
-                                                 "item_model_grid_test_job.cpp", "regression_posterior_job.cpp", "auc_jobs.cpp")]
+                                                 "item_model_grid_test_job.cpp", "regression_posterior_job.cpp", "auc_jobs.cpp", "item_model_prior.cpp")]
     deps = srcs + [os.path.join(HOST, "avro_io.hpp"), os.path.join(HOST, "avro_walk.hpp"), os.path.join(HOST, "jobs_common.hpp"), os.path.join(os.path.dirname(ROOT), "include", "mlease_b200.h"),
                    os.path.join(os.path.dirname(ROOT), "include", "mlease_host.h"), SO]
     cxx = os.environ.get("CXX", "g++")
